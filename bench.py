@@ -24,7 +24,7 @@ own shard (items are independent: weak scaling, no data-path collective); the ti
                 65 536 x 768, forward and forward + backward, device-timed, with the train-forward algorithmic bytes of SURVEY 8(d)
 
 --impl reference times that CPU port as the reference arm (the reference is pure Python/PyTorch: there is nothing
-to compile into oracle/_ref, see DESIGN.md).
+to compile into oracle/_ref).
 """
 import argparse
 import json
@@ -59,7 +59,7 @@ def algorithmic_bytes(n_items):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -109,7 +109,7 @@ _BEST_THREADS = None
 
 def cpu_threads(x=None, cbt=None):
     """Thread count at which the reference's CPU path runs FASTEST on this host.  More threads is not always faster for
-    these memory-bound ops (128 threads measured 3x slower than 8-32 on the B200 host), and the fair baseline is the
+    these memory-bound ops (on many-core hosts more threads can be several times slower), and the fair baseline is the
     reference at its best, so a few counts are timed on a full-size pass and the best is kept."""
     global _BEST_THREADS
     import torch
@@ -323,7 +323,7 @@ def _event_ms(torch, fn, n=10, warm=3):
 
 
 def run_c2(x, cbs, torch, ops):
-    """BASELINE configs[1]: ~12K x 768 items on one B200, through the routing the module API uses."""
+    """BASELINE configs[1]: ~12K x 768 items on one GPU, through the routing the module API uses."""
     n = 12101
     xs = x[:n].contiguous()
     with torch.no_grad():
@@ -390,7 +390,7 @@ def run_c4(x, cbs, torch, ops):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))
 
     def rot_fwd():
         return ops.RqChainFunction.apply(xg, ops.MODE_ROTATION, beta, True, *cg)
@@ -435,6 +435,8 @@ def main():
     ap.add_argument("--impl", default="ours")
     ap.add_argument("--path", default="auto", choices=["auto", "tc", "simt"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed (the ids, as float64) to DIR/ids.npy; inputs are seeded")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -498,6 +500,10 @@ def main():
             ids = step()
             ev[i + 1].record()
         sync()
+        if args.dump_outputs:                           # the caller's view of the last timed step: ids [N_ITEMS, L]
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            name = "ids.npy" if world == 1 else f"ids_rank{rank}.npy"
+            np.save(os.path.join(args.dump_outputs, name), ids.cpu().numpy().astype(np.float64))
         launches_timed = ops.LAUNCHES - l0
         t_post = time.perf_counter()
         while time.perf_counter() - t_post < 0.5:       # continuation of the same load (untimed) so rows land after it too
@@ -559,7 +565,7 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak_gbs = float(peaks.get("hbm_gbs", 6650.0))
+        peak_gbs = float(peaks.get("hbm_gbs", 3350.0))
         kern_ms = float(np.mean(per_step))
         achieved = algorithmic_bytes(N_ITEMS) / (kern_ms * 1e-3) / 1e9
         out = {
@@ -567,13 +573,13 @@ def main():
             "warmup": max(args.warmup, 3), "ms_per_step": total_ms / args.steps, "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": {"workload": WORKLOAD, "per_gpu_items": N_ITEMS,
-                       "kernel": ("rq_tcx_kernel: tcgen05 fp16 filter (deterministic margin) + exact fp32 re-rank" if use_tc
+                       "kernel": ("rq_tcx_kernel: wgmma fp16 filter (deterministic margin) + exact fp32 re-rank" if use_tc
                                   else "fp32 CUDA-core fused chain"),
                        "api": "parallel.CorpusTokenizer -> ops.rq_tokenize_tc with a prepared state: the routing RqVae.tokenize / "
                               "SemanticIdTokenizer.precompute_corpus_ids use (ops.rq_tokenize_auto)",
                        "ms_per_step_per_rank": per_rank_ms,
                        "parallelism": f"items sharded over {world} GPU(s), no data-path collective",
-                       "l2": "input batch (201 MB) exceeds the 126 MB L2; no flush between steps"},
+                       "l2": "input batch (201 MB) exceeds the 50 MB L2; no flush between steps"},
             "clocks": dict(clocks.summary(), note=("sampled at 100 ms over pre-load + warm-up + timed region + 0.5 s "
                                                   "continuation of the same step loop (timed region itself: "
                                                   f"{total_ms:.1f} ms); rows before/after the timed region: {n_before}/{n_after - n_before}")),
@@ -585,10 +591,8 @@ def main():
             "prepare_ms": prepare_ms,
             "rerank": rerank,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak_gbs, "unit": "GB/s",
-                         "frac": achieved / peak_gbs, "traffic": tok.measured_traffic_bytes(),
-                         "traffic_source": "static: dram__bytes_read.sum + dram__bytes_write.sum of the committed ncu --set full "
-                                           "capture of this kernel at this shape (profiles/r2_tcx_ncu_summary.csv), not measured in this run",
-                         "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "6650 GB/s (of fallback)",
+                         "frac": achieved / peak_gbs,
+                         "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "3350 GB/s (H100 SXM data sheet, fallback)",
                          "kernel_ms": kern_ms, "algorithmic_bytes": algorithmic_bytes(N_ITEMS)},
         }
         if c3 is not None:

@@ -1,4 +1,4 @@
-/* librqb200 -- C ABI of the B200-native RQ-VAE residual-quantisation hot path.
+/* librqb200 -- C ABI of the H100-native RQ-VAE residual-quantisation hot path.
  *
  * The reference (EdoardoBotta/RQ-VAE-Recommender) has no FFI layer: its boundary is the Python module API
  * (modules/quantize.py, modules/rqvae.py, init/kmeans.py, distributions/gumbel.py, modules/encoder.py).
@@ -70,7 +70,7 @@ int rqb200_rq_backward(int mode, const float* x, int64_t ldx, const float* const
                        int64_t ge_sL, const float* g_res, int64_t gr_sB, int64_t gr_sD, int64_t gr_sL,
                        const float* g_loss, int64_t gl_sB, float* g_x, float* const* g_codebooks, void* stream);
 
-/* ---- tensor-core tokeniser (tcgen05 candidate filter + exact fp32 re-rank), see csrc/rq_tc.cu --------
+/* ---- tensor-core tokeniser (wgmma candidate filter + exact fp32 re-rank), see csrc/rq_tc.cu --------
  * Same result contract as rqb200_rq_forward(mode=EVAL, ids only).  `prepare` converts the codebooks once
  * (fp16 copies, norms, inter-level Gram tables) into `state`; `run` consumes x [B,D] fp32. */
 size_t rqb200_tokenize_tc_state_bytes(int D, int K, int L);

@@ -42,7 +42,7 @@ def mlp_forward(x: np.ndarray, weights: Sequence[np.ndarray], normalize: bool = 
     """modules/encoder.py:23-38: bias-free Linear (+ReLU between layers), optional final L2 norm.
 
     ``weights[i]`` has the nn.Linear layout [out, in].  ``act="silu"`` reproduces the
-    activation pickled inside the shipped Amazon checkpoints (SURVEY 5.4)."""
+    activation pickled inside the shipped Amazon checkpoints."""
     h = x
     n = len(weights)
     for i, w in enumerate(weights):
@@ -175,7 +175,7 @@ def rq_tokenize(res: np.ndarray, codebooks: Sequence[np.ndarray]) -> np.ndarray:
 
 def top2_gap(res64: np.ndarray, codebooks64: Sequence[np.ndarray], ids: Optional[np.ndarray] = None,
              return_abs: bool = False):
-    """float64 tie classifier (SURVEY 8c parity protocol).
+    """float64 tie classifier.
 
     Returns (ids64 [B,L], best2 [B,L], relgap [B,L]) where the chain follows ``ids`` if given
     (so level l is judged on the residual the implementation under test actually saw),
@@ -241,7 +241,7 @@ def rqvae_forward(x: np.ndarray, enc_w: Sequence[np.ndarray], codebooks: Sequenc
     res = mlp_forward(x, enc_w, normalize=codebook_normalize, act=act)
     q = rq_forward(res, codebooks, mode, training, temperature, beta, gumbel_uniform)
     x_hat = mlp_forward(q.embeddings.sum(axis=-1), dec_w, act=act)
-    if n_cat != 0:     # rqvae.py:147-150; with n_cat == 0 the [:-0] slice is empty -> no normalisation (SURVEY A.5)
+    if n_cat != 0:     # rqvae.py:147-150; with n_cat == 0 the [:-0] slice is empty -> no normalisation
         x_hat = np.concatenate([l2norm(x_hat[..., :-n_cat]), x_hat[..., -n_cat:]], axis=-1)
     rec = reconstruction_loss(x_hat, x, n_cat)
     loss = (rec + q.quantize_loss).mean()
@@ -250,7 +250,7 @@ def rqvae_forward(x: np.ndarray, enc_w: Sequence[np.ndarray], codebooks: Sequenc
                        np.asarray(p_unique_ids(q.sem_ids), dtype=x.dtype))
 
 
-# --------------------------------------------------------------------------- backward (SURVEY A.3)
+# --------------------------------------------------------------------------- backward
 def quantize_backward(mode: int, x: np.ndarray, codebook: np.ndarray, ids: np.ndarray,
                       g_out: np.ndarray, g_loss: np.ndarray, beta: float = 0.25,
                       temperature: float = 0.2, gumbel_uniform: Optional[np.ndarray] = None):
@@ -333,7 +333,7 @@ def kmeans_run(x: np.ndarray, k: int, init_idx: np.ndarray,
     return KmeansOut(c, assignment, i)
 
 
-# --------------------------------------------------------------------------- tokenizer helpers (SURVEY 8f-1)
+# --------------------------------------------------------------------------- tokenizer helpers
 def dedup_rank(sem_ids: np.ndarray) -> np.ndarray:
     """modules/tokenizer/semids.py:94-108: number of EARLIER corpus rows with the identical id tuple."""
     N = sem_ids.shape[0]

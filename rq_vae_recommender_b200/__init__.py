@@ -1,7 +1,7 @@
-"""B200-native RQ-VAE residual-quantisation hot path behind the reference's module API.
+"""H100-native RQ-VAE residual-quantisation hot path behind the reference's module API.
 
 Layout (only what the path needs):
-  csrc/            hand-written sm_100a CUDA kernels + the C ABI (include/rqb200.h) -> librqb200.so
+  csrc/            hand-written sm_90a CUDA kernels + the C ABI (include/rqb200.h) -> librqb200.so
   _lib.py          ctypes binding (fails loudly when the library is missing -- no fallback)
   ops.py           torch.Tensor <-> C ABI marshalling, autograd Functions
   modules/ init/ distributions/ data/   mirrors of the reference modules with identical public names

@@ -1,6 +1,6 @@
 """ctypes binding of librqb200.so (C ABI declared in include/rqb200.h).
 
-The shared library is built in-tree by ``build()`` (nvcc, sm_100a only) and loaded with ctypes -- no torch
+The shared library is built in-tree by ``build()`` (nvcc, sm_90a only) and loaded with ctypes -- no torch
 extension machinery, no torch types in any signature.  There is NO fallback: if the library is missing or a
 call fails, the product path raises.
 """
@@ -14,8 +14,8 @@ from typing import Optional
 PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "librqb200.so")
-SOURCES = ["api.cu", "rq_simt.cu", "dense.cu", "rq_tc.cu", "rq_tcx.cu", "rq_tcx96.cu", "gemm_tc.cu", "sid.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+SOURCES = ["api.cu", "rq_simt.cu", "dense.cu", "rq_tc.cu", "rq_tcx.cu", "gemm_tc.cu", "sid.cu"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-shared", "-Xcompiler", "-fPIC"]
 
 _lib: Optional[ctypes.CDLL] = None
@@ -84,7 +84,7 @@ class Rqb200Error(RuntimeError):
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/*.cu into librqb200.so for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile csrc/*.cu into librqb200.so for sm_90a (nvcc cross-compiles without a GPU)."""
     srcs = [os.path.join(CSRC, s) for s in SOURCES]
     deps = srcs + [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))]
     if not force and os.path.exists(LIB_PATH) and all(os.path.getmtime(LIB_PATH) >= os.path.getmtime(d) for d in deps):

@@ -1,4 +1,4 @@
-// Shared device/host helpers for librqb200 (sm_100a only).
+// Shared device/host helpers for librqb200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -103,7 +103,7 @@ __device__ __forceinline__ void mbar_wait_guarded(uint64_t* bar, uint32_t parity
     if (clock64() - t0 > 4000000000LL) __trap();
   }
 }
-// ---- cluster (CTA pair) variants: validated standalone by tools/pair_probe.cu
+// ---- cluster variants
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));

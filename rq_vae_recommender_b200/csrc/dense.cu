@@ -209,7 +209,7 @@ __global__ void gumbel_bwd_ge_kernel(const float* g_out, int64_t go_sB, int64_t 
 
 // gdist = -W * (gW - sum_k W gW) / T  (in place over gW);  rowsum[b] = sum_k gdist ; colsum[k] += gdist
 // Column sums: every CTA walks its rows (grid-stride) and keeps the K partial sums in shared memory, one global atomic per column
-// and CTA at the end (one atomic per ELEMENT into 256 addresses ran at 3 % of the SM throughput: profiles/r2_kernels_ncu_summary.csv)
+// and CTA at the end (one atomic per ELEMENT into 256 addresses ran at 3 % of the SM throughput)
 __global__ void gumbel_bwd_softmax_kernel(const float* w, float* gw, int B, int K, float temperature, float* rowsum,
                                           float* colsum) {
   extern __shared__ float s_col[];                            // [K] (K <= GUMBEL_SMEM_K), else straight to global
@@ -341,7 +341,7 @@ extern "C" int rqb200_gumbel_bwd_softmax(const float* weights, float* gw_inout, 
   RQB_CUDA(cudaMemsetAsync(colsum, 0, (size_t)K * sizeof(float), st));
   if (B == 0) return RQB_OK;
   int grid = (B + 7) / 8;
-  if (grid > 148 * 4) grid = 148 * 4;
+  if (grid > 132 * 4) grid = 132 * 4;
   gumbel_bwd_softmax_kernel<<<grid, 256, K <= 8192 ? (size_t)K * sizeof(float) : 0, st>>>(weights, gw_inout, B, K, temperature, rowsum, colsum);
   RQB_LAUNCH_CHECK();
   return RQB_OK;
@@ -407,7 +407,7 @@ extern "C" int rqb200_sid_histogram(const int64_t* ids, int B, int L, int K, int
   if (smem > 48 * 1024)
     RQB_CUDA(cudaFuncSetAttribute(sid_histogram_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int grid = (int)(((int64_t)B * L + 255) / 256);
-  if (grid > 148 * 4) grid = 148 * 4;
+  if (grid > 132 * 4) grid = 132 * 4;
   sid_histogram_kernel<<<grid, 256, smem, st>>>(ids, B, L, K, reinterpret_cast<unsigned long long*>(hist));
   RQB_LAUNCH_CHECK();
   return RQB_OK;

@@ -1,69 +1,27 @@
-// bf16 tcgen05 GEMM with fused ReLU for the encoder / decoder MLPs (modules/encoder.py:23-38), sm_100a.
+// bf16 wgmma GEMM with fused ReLU for the encoder / decoder MLPs (modules/encoder.py:23-38), sm_90a.
 //
-//   Y[M,N] = act( X[M,K] . W[N,K]^T ),   bf16 operands, fp32 accumulation in TMEM, act = ReLU or identity.
+//   Y[M,N] = act( X[M,K] . W[N,K]^T ),   bf16 operands, fp32 accumulation in registers, act = ReLU or identity.
 //
 // This is the reduced-precision (AMP-like) path: the reference runs these Linears in bf16 when
 // `train_rqvae.py:36,69` enables mixed precision.  The exact fp32 path (csrc/dense.cu sgemm) stays the default because
 // index parity at 1e-5 needs it; this kernel is opt-in and forward-only (tokenisation).
 //
 // Data layout ("image"): every operand is stored in HBM as the exact shared-memory image the tensor core reads --
-// [row-tile of 128][k-chunk of 64][128 rows x 128 B], K-major, 16-byte chunks XOR-swizzled with (row & 7) (UMMA
-// SWIZZLE_128B).  A stage is then ONE contiguous 16 KB TMA bulk copy, no tensor maps, and the epilogue of layer i
+// [row-tile of 128][k-chunk of 64][128 rows x 128 B], K-major, 16-byte chunks XOR-swizzled with (row & 7) (wgmma
+// SWIZZLE_128B).  A stage is then ONE contiguous 16 KB bulk copy, no tensor maps, and the epilogue of layer i
 // writes layer i+1's A operand directly in that layout, so activations never exist in row-major form.
 //
-// Kernel: persistent, one CTA per SM.  warp 0 = TMA producer (A + up to 2 W blocks per stage, 4-stage ring),
-// warp 1 = MMA issuer (tcgen05.mma M128 N128 K16, accumulators double-buffered in TMEM: 2 x 256 columns),
-// warps 4-11 = epilogue (2 per TMEM lane quarter, one per 128-column block): tcgen05.ld -> ReLU -> bf16 image or fp32 rows.
+// Kernel: persistent, one CTA per SM.  warps 0-7 = two consumer warpgroups (rows [0,64) and [64,128) of the tile, wgmma
+// m64n128k16 per 128-column W block, accumulators in registers), warp 8 = bulk-copy producer (A + up to 2 W blocks per stage,
+// 4-stage ring).  The epilogue (ReLU -> bf16 image or fp32 rows) runs from the accumulator registers.
 #include "common.cuh"
+#include "wgmma.cuh"
 #include <cuda_bf16.h>
 
 #define GT_KC 64
 #define GT_BLK_BYTES (128 * GT_KC * 2)   // 16 KB: 128 rows x 64 bf16
 #define GT_STAGES 4
-#define GT_THREADS 384                   // warps 0-3: producer, MMA, 2 idle | warps 4-11: epilogue
-
-// ------------------------------------------------------------------------------------------------ tcgen05 wrappers
-__device__ __forceinline__ void gt_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void gt_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void gt_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void gt_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void gt_mma(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void gt_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void gt_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// K-major SWIZZLE_128B smem descriptor / instruction descriptor: see rq_tc.cu (same encodings); A,B format 1 = BF16
-__device__ __forceinline__ uint64_t gt_smem_desc(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr >> 4) & 0x3FFF) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-__host__ __device__ constexpr uint32_t gt_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
+#define GT_THREADS 288                   // warps 0-7: two consumer warpgroups | warp 8: producer
 
 // ------------------------------------------------------------------------------------------------ image builders
 extern "C" size_t rqb200_bf16_image_bytes(int rows, int K) {
@@ -120,10 +78,34 @@ struct GtParams {
 
 struct GtSmemMisc {
   uint64_t full[GT_STAGES], empty[GT_STAGES];
-  uint64_t t_full[2][2], t_empty[2];
-  uint32_t tmem_base;
-  uint32_t pad;
 };
+
+// one 128-column block of the epilogue: columns col0 + 8 jb + 2 (lane % 4) + {0, 1} of rows ra and ra + 8 (acc[4 jb + 0..3])
+__device__ __forceinline__ void gt_store_block(const GtParams& p, const float (&acc)[64], int mt, int ra, int col0, int lane) {
+  const int q4 = lane & 3;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = ra + 8 * h, row = mt * 128 + r;
+#pragma unroll
+    for (int jb = 0; jb < 16; ++jb) {
+      const int col = col0 + 8 * jb + 2 * q4;
+      if (col >= p.N) continue;
+      float v0 = acc[4 * jb + 2 * h], v1 = acc[4 * jb + 2 * h + 1];
+      if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+      if (p.out_img) {
+        // next layer's A image (N % 64 == 0, so col + 1 < N): rows >= M hold act(0) = 0, harmless padding
+        unsigned char* dst = p.out_img + ((size_t)mt * (p.N / GT_KC) + (col >> 6)) * GT_BLK_BYTES + r * 128 +
+                             ((((col & 63) >> 3) ^ (r & 7)) << 4) + (col & 7) * 2;
+        *reinterpret_cast<__nv_bfloat162*>(dst) = __floats2bfloat162_rn(v0, v1);
+      }
+      if (p.out_f32 && row < p.M) {
+        float* o = p.out_f32 + (int64_t)row * p.ldo + col;
+        o[0] = v0;
+        if (col + 1 < p.N) o[1] = v1;
+      }
+    }
+  }
+}
 
 __global__ void __launch_bounds__(GT_THREADS, 1) gt_gemm_kernel(GtParams p) {
   extern __shared__ __align__(1024) unsigned char gsm[];
@@ -133,125 +115,72 @@ __global__ void __launch_bounds__(GT_THREADS, 1) gt_gemm_kernel(GtParams p) {
 
   if (tid == 0) {
     if ((smem_u32(gsm) & 1023u) != 0) __trap();
-    for (int i = 0; i < GT_STAGES; ++i) { mbar_init(&ms->full[i], 1); mbar_init(&ms->empty[i], 1); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&ms->t_full[i][0], 1); mbar_init(&ms->t_full[i][1], 1);
-      mbar_init(&ms->t_empty[i], 8 * 32);
-    }
+    for (int i = 0; i < GT_STAGES; ++i) { mbar_init(&ms->full[i], 1); mbar_init(&ms->empty[i], 8); }
     fence_mbar_init();
   }
-  if (warp == 1) gt_alloc(&ms->tmem_base, 512);
-  gt_fence_before();
   __syncthreads();
-  gt_fence_after();
-#define GT_TMEM() (*reinterpret_cast<volatile uint32_t*>(&ms->tmem_base))
 
   // work item = (row tile mt, group of up to two 128-column W blocks)
-  if (warp == 0 && lane == 0) {
-    // ============================================================== TMA producer
-    uint32_t s = 0;
-    for (int item = blockIdx.x; item < p.nitems; item += gridDim.x) {
-      const int mt = item / p.ngroups, g = item % p.ngroups;
-      const int nb = min(2, p.nblocks - 2 * g);
-      for (int kc = 0; kc < p.nkc; ++kc, ++s) {
-        const uint32_t st = s % GT_STAGES, u = s / GT_STAGES;
-        mbar_wait_guarded(&ms->empty[st], (u & 1) ^ 1, 1);
-        unsigned char* dst = gsm + st * 3 * GT_BLK_BYTES;
-        mbar_expect_tx(&ms->full[st], (1 + nb) * GT_BLK_BYTES);
-        bulk_g2s(dst, p.a_img + ((size_t)mt * p.nkc + kc) * GT_BLK_BYTES, GT_BLK_BYTES, &ms->full[st]);
-        for (int b = 0; b < nb; ++b)
-          bulk_g2s(dst + (1 + b) * GT_BLK_BYTES, p.w_img + ((size_t)(2 * g + b) * p.nkc + kc) * GT_BLK_BYTES, GT_BLK_BYTES,
-                   &ms->full[st]);
-      }
-    }
-  } else if (warp == 1 && lane == 0) {
-    // ============================================================== MMA issuer
-    const uint32_t idesc = gt_idesc_bf16(128, 128);
-    const uint32_t base = smem_u32(gsm);
-    uint32_t s = 0, it = 0;
-    for (int item = blockIdx.x; item < p.nitems; item += gridDim.x, ++it) {
-      const int g = item % p.ngroups;
-      const int nb = min(2, p.nblocks - 2 * g);
-      const uint32_t buf = it & 1, u = it >> 1;
-      mbar_wait_guarded(&ms->t_empty[buf], (u & 1) ^ 1, 2);
-      gt_fence_after();
-      for (int kc = 0; kc < p.nkc; ++kc, ++s) {
-        const uint32_t st = s % GT_STAGES;
-        mbar_wait_guarded(&ms->full[st], (s / GT_STAGES) & 1, 3);
-        gt_fence_after();
-        const uint32_t sa = base + st * 3 * GT_BLK_BYTES;
-        const uint64_t adesc = gt_smem_desc(sa);
-        for (int b = 0; b < nb; ++b) {
-          const uint64_t bdesc = gt_smem_desc(sa + (1 + b) * GT_BLK_BYTES);
-          const uint32_t d = GT_TMEM() + buf * 256 + b * 128;
-#pragma unroll
-          for (int j = 0; j < GT_KC / 16; ++j) gt_mma(d, adesc + 2 * j, bdesc + 2 * j, idesc, (kc | j) != 0);
-        }
-        gt_commit(&ms->empty[st]);
-      }
-      gt_commit(&ms->t_full[buf][0]);
-      gt_commit(&ms->t_full[buf][1]);
-    }
-  } else if (warp >= 4) {
-    // ============================================================== epilogue: TMEM -> act -> bf16 image / fp32 rows
-    const int quarter = warp & 3, blk = (warp - 4) >> 2;      // TMEM lane quarter, 128-column block inside the group
-    const int r = quarter * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(quarter * 32) << 16;
-    uint32_t it = 0;
-    for (int item = blockIdx.x; item < p.nitems; item += gridDim.x, ++it) {
-      const int mt = item / p.ngroups, g = item % p.ngroups;
-      const int nb = min(2, p.nblocks - 2 * g);
-      const uint32_t buf = it & 1, u = it >> 1;
-      mbar_wait_guarded(&ms->t_full[buf][blk], u & 1, 4);
-      gt_fence_after();
-      const int row = mt * 128 + r;
-      const int col0 = (2 * g + blk) * 128;                    // first output column of this block
-      if (blk < nb) {
-        const uint32_t tcol = GT_TMEM() + lane_addr + buf * 256 + blk * 128;
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-          const int col = col0 + c * 32;
-          if (col >= p.N) break;                               // warp-uniform
-          uint32_t sr[32];
-          gt_ld32(tcol + c * 32, sr);
-          float v[32];
-#pragma unroll
-          for (int e = 0; e < 32; ++e) {
-            v[e] = __uint_as_float(sr[e]);
-            if (p.relu) v[e] = fmaxf(v[e], 0.f);
-          }
-          if (p.out_img) {
-            // columns [col, col+32) = half of k-chunk (col / 64) of the next layer's A image: 4 x 16-byte swizzled chunks
-            unsigned char* dst = p.out_img + ((size_t)mt * (p.N / GT_KC) + (col >> 6)) * GT_BLK_BYTES + r * 128;
-            const int cbase = (col & 63) >> 3;
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              __nv_bfloat162 p0 = __floats2bfloat162_rn(v[q * 8 + 0], v[q * 8 + 1]), p1 = __floats2bfloat162_rn(v[q * 8 + 2], v[q * 8 + 3]);
-              __nv_bfloat162 p2 = __floats2bfloat162_rn(v[q * 8 + 4], v[q * 8 + 5]), p3 = __floats2bfloat162_rn(v[q * 8 + 6], v[q * 8 + 7]);
-              uint4 w;
-              w.x = *reinterpret_cast<uint32_t*>(&p0); w.y = *reinterpret_cast<uint32_t*>(&p1);
-              w.z = *reinterpret_cast<uint32_t*>(&p2); w.w = *reinterpret_cast<uint32_t*>(&p3);
-              *reinterpret_cast<uint4*>(dst + (((cbase + q) ^ (r & 7)) << 4)) = w;   // rows >= M hold act(0) = 0: harmless padding
-            }
-          }
-          if (p.out_f32 && row < p.M) {
-            float* o = p.out_f32 + (int64_t)row * p.ldo + col;
-#pragma unroll
-            for (int e = 0; e < 32; ++e)
-              if (col + e < p.N) o[e] = v[e];
-          }
+  if (warp == 8) {
+    // ============================================================== bulk-copy producer
+    if (lane == 0) {
+      uint32_t s = 0;
+      for (int item = blockIdx.x; item < p.nitems; item += gridDim.x) {
+        const int mt = item / p.ngroups, g = item % p.ngroups;
+        const int nb = min(2, p.nblocks - 2 * g);
+        for (int kc = 0; kc < p.nkc; ++kc, ++s) {
+          const uint32_t st = s % GT_STAGES, u = s / GT_STAGES;
+          mbar_wait_guarded(&ms->empty[st], (u & 1) ^ 1, 1);
+          unsigned char* dst = gsm + st * 3 * GT_BLK_BYTES;
+          mbar_expect_tx(&ms->full[st], (1 + nb) * GT_BLK_BYTES);
+          bulk_g2s(dst, p.a_img + ((size_t)mt * p.nkc + kc) * GT_BLK_BYTES, GT_BLK_BYTES, &ms->full[st]);
+          for (int b = 0; b < nb; ++b)
+            bulk_g2s(dst + (1 + b) * GT_BLK_BYTES, p.w_img + ((size_t)(2 * g + b) * p.nkc + kc) * GT_BLK_BYTES, GT_BLK_BYTES,
+                     &ms->full[st]);
         }
       }
-      gt_fence_before();
-      mbar_arrive(&ms->t_empty[buf]);
     }
+    return;
   }
-
-  gt_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    gt_fence_after();
-    gt_dealloc(GT_TMEM(), 512);
+  // ============================================================== consumers: warpgroup wg owns rows [64 wg, 64 wg + 64)
+  const int wg = warp >> 2;
+  const int ra = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const uint32_t base = smem_u32(gsm);
+  uint32_t s = 0;
+  for (int item = blockIdx.x; item < p.nitems; item += gridDim.x) {
+    const int mt = item / p.ngroups, g = item % p.ngroups;
+    const int nb = min(2, p.nblocks - 2 * g);
+    float acc0[64], acc1[64];
+    uint32_t prev = 0;
+    for (int kc = 0; kc < p.nkc; ++kc, ++s) {
+      const uint32_t st = s % GT_STAGES;
+      mbar_wait_guarded(&ms->full[st], (s / GT_STAGES) & 1, 3);
+      const uint32_t sa = base + st * 3 * GT_BLK_BYTES;
+      const uint64_t ad = wg_desc(sa + wg * (GT_BLK_BYTES / 2)), b0 = wg_desc(sa + GT_BLK_BYTES), b1 = wg_desc(sa + 2 * GT_BLK_BYTES);
+      wg_fence_acc(acc0); wg_fence_acc(acc1);
+      wg_fence();
+#pragma unroll
+      for (int j = 0; j < GT_KC / 16; ++j) {
+        // the second block is multiplied even when the group has one (its stale slot is never stored): a wgmma under a
+        // branch is serialised by the compiler
+        wg_m64n128_bf16(acc0, ad + 2 * j, b0 + 2 * j, (kc | j) != 0);
+        wg_m64n128_bf16(acc1, ad + 2 * j, b1 + 2 * j, (kc | j) != 0);
+      }
+      wg_commit();
+      wg_fence_acc(acc0); wg_fence_acc(acc1);
+      if (kc > 0) {
+        wg_wait<1>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&ms->empty[prev]);
+      }
+      prev = st;
+    }
+    wg_wait<0>();
+    wg_fence_acc(acc0); wg_fence_acc(acc1);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&ms->empty[prev]);
+    gt_store_block(p, acc0, mt, ra, 2 * g * 128, lane);
+    if (nb > 1) gt_store_block(p, acc1, mt, ra, (2 * g + 1) * 128, lane);
   }
 }
 
@@ -295,7 +224,7 @@ extern "C" int rqb200_gemm_bf16(const void* a_image, const void* w_image, int M,
 // Every operand row is scaled by a power of two so that its largest element lies in [2^14, 2^15) and stored as TWO fp16 images
 //   hi = fp16(v 2^e),  lo = fp16(v 2^e - hi)          (hi + lo carries 22 significant bits of v; lo may be subnormal: the error
 //                                                      is then 2^-25 absolute = 2^-39 of the row maximum)
-// and the product is three tcgen05.mma per k-step with fp32 accumulation in TMEM:  hi.hi + lo.hi + hi.lo  (lo.lo is 2^-22
+// and the product is three wgmma per k-step, hi.hi + lo.hi + hi.lo, each 64-wide k chunk promoted into an fp32 total (lo.lo is 2^-22
 // relative and dropped).  The epilogue multiplies by 2^-(e_row + e_col), both exact.  Measured against float64 the result is
 // as close as a plain fp32 FMA GEMM (tests/test_gpu_gemm_split.py states the bound that is asserted).
 //
@@ -303,15 +232,14 @@ extern "C" int rqb200_gemm_bf16(const void* a_image, const void* w_image, int M,
 // holds [hi image][lo image][row scales: 128 floats per row tile, value 2^-e].  K is padded with zeros to a multiple of 64, rows
 // to a multiple of 128.
 //
-// Kernel: persistent, one CTA per SM; work item = (row tile, group of up to 256 columns).  Stage = [A hi][A lo][B hi 0][B hi 1]
-// [B lo 0][B lo 1] = 96 KB, 2 stages; the two B blocks of a half are adjacent so that ONE tcgen05.mma covers N = 256.
-// warp 0 = bulk-copy producer, warp 1 = MMA issuer (two accumulators of 256 TMEM columns: hi.hi and the cross terms),
-// warps 4-11 = epilogue (sums the two, scales, activates).
+// Kernel: persistent, one CTA per SM; work item = (row tile, 128-column block, k slice).  Stage = [A hi][A lo][B hi][B lo]
+// = 64 KB, 3 stages.  warps 0-7 = two consumer warpgroups (64 rows each: an m64n128 register accumulator per k chunk, promoted
+// into an fp32 total; the epilogue scales and activates), warp 8 = bulk-copy producer.
 #include <cuda_fp16.h>
 
-#define GS_STAGES 2
+#define GS_STAGES 3
 #define GS_MAX_CHUNKS 12                   // 16-byte chunks per lane of the row splitter: K <= 32 * 8 * 12 = 3072
-#define GS_STAGE_BYTES (6 * GT_BLK_BYTES)
+#define GS_STAGE_BYTES (4 * GT_BLK_BYTES)
 
 extern "C" size_t rqb200_split_image_bytes(int rows, int K) {
   if (rows < 0 || K <= 0) return 0;
@@ -492,18 +420,14 @@ extern "C" int rqb200_f32_to_split_image(const float* x, int64_t ldx, int rows, 
 struct GsParams {
   const unsigned char *a_hi, *a_lo, *b_hi, *b_lo;   // [tiles][nkc][16 KB]
   const float *a_scale, *b_scale;                   // 2^-e per image row
-  int M, N, nkc, mtiles, nblocks, ngroups, nitems, relu;
-  int ksplit, kc_per;                               // split-K: item = (row tile, column group, k slice of kc_per chunks); slice ks
+  int M, N, nkc, mtiles, nblocks, nitems, relu;
+  int ksplit, kc_per;                               // split-K: item = (row tile, column block, k slice of kc_per chunks); slice ks
   int64_t part_stride;                              // writes its partial sums to out + ks * part_stride (ksplit == 1: 0)
   float* out;
   int64_t ldo;
   const float* mask;                                // optional [M, N] (ld = ldm): out = mask > 0 ? out : 0  (ReLU' of a backward GEMM)
   int64_t ldm;
 };
-
-__device__ __forceinline__ uint32_t gs_idesc_f16(int M, int N) {       // A, B = F16 (format 0), D = F32, K-major both
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
 
 __global__ void __launch_bounds__(GT_THREADS, 1) gs_gemm_kernel(GsParams p) {
   extern __shared__ __align__(1024) unsigned char gsm[];
@@ -512,141 +436,101 @@ __global__ void __launch_bounds__(GT_THREADS, 1) gs_gemm_kernel(GsParams p) {
 
   if (tid == 0) {
     if ((smem_u32(gsm) & 1023u) != 0) __trap();
-    for (int i = 0; i < GS_STAGES; ++i) { mbar_init(&ms->full[i], 1); mbar_init(&ms->empty[i], 1); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&ms->t_full[i][0], 1); mbar_init(&ms->t_full[i][1], 1);
-      mbar_init(&ms->t_empty[i], 8 * 32);
-    }
+    for (int i = 0; i < GS_STAGES; ++i) { mbar_init(&ms->full[i], 1); mbar_init(&ms->empty[i], 8); }
     fence_mbar_init();
   }
-  if (warp == 1) gt_alloc(&ms->tmem_base, 512);
-  gt_fence_before();
   __syncthreads();
-  gt_fence_after();
 
-  if (warp == 0 && lane == 0) {
-    // ============================================================== producer: 2 A blocks + 2 or 4 B blocks per stage
-    uint32_t s = 0;
-    for (int item = blockIdx.x; item < p.nitems; item += gridDim.x) {
-      const int ks = item % p.ksplit, tile = item / p.ksplit;
-      const int mt = tile / p.ngroups, g = tile % p.ngroups;
-      const int nb = min(2, p.nblocks - 2 * g);
-      const int kc_end = min(p.nkc, (ks + 1) * p.kc_per);
-      for (int kc = ks * p.kc_per; kc < kc_end; ++kc, ++s) {
-        const uint32_t st = s % GS_STAGES, u = s / GS_STAGES;
-        mbar_wait_guarded(&ms->empty[st], (u & 1) ^ 1, 1);
-        unsigned char* dst = gsm + st * GS_STAGE_BYTES;
-        mbar_expect_tx(&ms->full[st], (2 + 2 * nb) * GT_BLK_BYTES);
-        const size_t ao = ((size_t)mt * p.nkc + kc) * GT_BLK_BYTES;
-        bulk_g2s(dst, p.a_hi + ao, GT_BLK_BYTES, &ms->full[st]);
-        bulk_g2s(dst + GT_BLK_BYTES, p.a_lo + ao, GT_BLK_BYTES, &ms->full[st]);
-        for (int b = 0; b < nb; ++b) {
-          const size_t bo = ((size_t)(2 * g + b) * p.nkc + kc) * GT_BLK_BYTES;
-          bulk_g2s(dst + (2 + b) * GT_BLK_BYTES, p.b_hi + bo, GT_BLK_BYTES, &ms->full[st]);
-          bulk_g2s(dst + (4 + b) * GT_BLK_BYTES, p.b_lo + bo, GT_BLK_BYTES, &ms->full[st]);
+  if (warp == 8) {
+    // ============================================================== producer: A hi, A lo, B hi, B lo per stage
+    if (lane == 0) {
+      uint32_t s = 0;
+      for (int item = blockIdx.x; item < p.nitems; item += gridDim.x) {
+        const int ks = item % p.ksplit, tile = item / p.ksplit;
+        const int mt = tile / p.nblocks, nbk = tile % p.nblocks;
+        const int kc_end = min(p.nkc, (ks + 1) * p.kc_per);
+        for (int kc = ks * p.kc_per; kc < kc_end; ++kc, ++s) {
+          const uint32_t st = s % GS_STAGES, u = s / GS_STAGES;
+          mbar_wait_guarded(&ms->empty[st], (u & 1) ^ 1, 1);
+          unsigned char* dst = gsm + st * GS_STAGE_BYTES;
+          mbar_expect_tx(&ms->full[st], 4 * GT_BLK_BYTES);
+          const size_t ao = ((size_t)mt * p.nkc + kc) * GT_BLK_BYTES, bo = ((size_t)nbk * p.nkc + kc) * GT_BLK_BYTES;
+          bulk_g2s(dst, p.a_hi + ao, GT_BLK_BYTES, &ms->full[st]);
+          bulk_g2s(dst + GT_BLK_BYTES, p.a_lo + ao, GT_BLK_BYTES, &ms->full[st]);
+          bulk_g2s(dst + 2 * GT_BLK_BYTES, p.b_hi + bo, GT_BLK_BYTES, &ms->full[st]);
+          bulk_g2s(dst + 3 * GT_BLK_BYTES, p.b_lo + bo, GT_BLK_BYTES, &ms->full[st]);
         }
       }
     }
-  } else if (warp == 1 && lane == 0) {
-    // ============================================================== MMA issuer: hi.hi + lo.hi + hi.lo per k-step
-    const uint32_t base = smem_u32(gsm);
-    uint32_t s = 0, it = 0;
-    for (int item = blockIdx.x; item < p.nitems; item += gridDim.x, ++it) {
-      const int ks = item % p.ksplit, g = (item / p.ksplit) % p.ngroups;
-      const int nb = min(2, p.nblocks - 2 * g);
-      const uint32_t idesc = gs_idesc_f16(128, nb * 128);
-      const int kc_begin = ks * p.kc_per, kc_end = min(p.nkc, (ks + 1) * p.kc_per);
-      mbar_wait_guarded(&ms->t_empty[0], (it & 1) ^ 1, 2);
-      gt_fence_after();
-      // two accumulators: hi.hi in columns [0, 256), the cross terms in [256, 512).  The tensor core truncates the fp32
-      // accumulator after every MMA (measured: the error of one shared accumulator grows with the number of MMAs and matches a
-      // round-toward-zero model, 5.4e-7 of |a||b| at K = 768); apart, the large sum sees a third of the truncations and the
-      // small one truncates at 2^-11 of the magnitude: 1.8e-7, the level of a plain fp32 GEMM
-      const uint32_t d = GT_TMEM(), dx = GT_TMEM() + 256;
-      for (int kc = kc_begin; kc < kc_end; ++kc, ++s) {
-        const uint32_t st = s % GS_STAGES;
-        mbar_wait_guarded(&ms->full[st], (s / GS_STAGES) & 1, 3);
-        gt_fence_after();
-        const uint32_t sa = base + st * GS_STAGE_BYTES;
-        const uint64_t ahi = gt_smem_desc(sa), alo = gt_smem_desc(sa + GT_BLK_BYTES);
-        const uint64_t bhi = gt_smem_desc(sa + 2 * GT_BLK_BYTES), blo = gt_smem_desc(sa + 4 * GT_BLK_BYTES);
-#pragma unroll
-        for (int j = 0; j < GT_KC / 16; ++j) {
-          gt_mma(d, ahi + 2 * j, bhi + 2 * j, idesc, ((kc - kc_begin) | j) != 0);
-          gt_mma(dx, alo + 2 * j, bhi + 2 * j, idesc, ((kc - kc_begin) | j) != 0);
-          gt_mma(dx, ahi + 2 * j, blo + 2 * j, idesc, 1);
-        }
-        gt_commit(&ms->empty[st]);
-      }
-      gt_commit(&ms->t_full[0][0]);
-      gt_commit(&ms->t_full[0][1]);
-    }
-  } else if (warp >= 4) {
-    // ============================================================== epilogue: TMEM -> x 2^-(e_row + e_col) -> act -> fp32 rows
-    const int quarter = warp & 3, blk = (warp - 4) >> 2;
-    const int r = quarter * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(quarter * 32) << 16;
-    uint32_t it = 0;
-    for (int item = blockIdx.x; item < p.nitems; item += gridDim.x, ++it) {
-      const int ks = item % p.ksplit, tile = item / p.ksplit;
-      const int mt = tile / p.ngroups, g = tile % p.ngroups;
-      const int nb = min(2, p.nblocks - 2 * g);
-      mbar_wait_guarded(&ms->t_full[0][blk], it & 1, 4);
-      gt_fence_after();
-      const int row = mt * 128 + r;
-      const int col0 = (2 * g + blk) * 128;
-      if (blk < nb) {
-        const float rs = __ldg(p.a_scale + row);                 // scale vectors are padded to whole tiles
-        const uint32_t tcol = GT_TMEM() + lane_addr + blk * 128;
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-          const int col = col0 + c * 32;
-          if (col >= p.N) break;                                 // warp-uniform
-          uint32_t sr[32], sx[32];
-          gt_ld32(tcol + c * 32, sr);
-          gt_ld32(tcol + 256 + c * 32, sx);
-          // scale of column col + lane (vectors are padded to whole tiles).  2^-(e_row + e_col) is applied as two factors of half
-          // the exponent each (|e| <= 120 per operand): neither the factor nor the intermediate product leaves the fp32 range
-          // unless the result does
-          const int ea = (__float_as_int(rs) >> 23) & 0xff;                                    // this lane's ROW
-          const int ebl = (__float_as_int(__ldg(p.b_scale + col + lane)) >> 23) & 0xff;         // column col + lane
-          float v[32];
-#pragma unroll
-          for (int e = 0; e < 32; ++e) {
-            const int et = ea + __shfl_sync(0xffffffffu, ebl, e) - 254;                         // -(e_row + e_col)
-            const int e1 = et >> 1;
-            v[e] = ((__uint_as_float(sr[e]) + __uint_as_float(sx[e])) * __int_as_float((e1 + 127) << 23)) * __int_as_float((et - e1 + 127) << 23);   // exact
-            if (p.relu) v[e] = fmaxf(v[e], 0.f);
-          }
-          if (p.mask && row < p.M) {
-            const float* mk = p.mask + (int64_t)row * p.ldm + col;
-#pragma unroll
-            for (int e = 0; e < 32; ++e)
-              if (col + e < p.N && !(__ldg(mk + e) > 0.f)) v[e] = 0.f;
-          }
-          if (row < p.M) {
-            float* o = p.out + (int64_t)ks * p.part_stride + (int64_t)row * p.ldo + col;
-            if (col + 32 <= p.N && (p.ldo & 3) == 0 && (reinterpret_cast<uintptr_t>(p.out) & 15) == 0) {
-#pragma unroll
-              for (int e = 0; e < 32; e += 4) *reinterpret_cast<float4*>(o + e) = make_float4(v[e], v[e + 1], v[e + 2], v[e + 3]);
-            } else {
-#pragma unroll
-              for (int e = 0; e < 32; ++e)
-                if (col + e < p.N) o[e] = v[e];
-            }
-          }
-        }
-      }
-      gt_fence_before();
-      mbar_arrive(&ms->t_empty[0]);
-    }
+    return;
   }
-
-  gt_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    gt_fence_after();
-    gt_dealloc(GT_TMEM(), 512);
+  // ============================================================== consumers: hi.hi + lo.hi + hi.lo per k-step
+  const int wg = warp >> 2, q4 = lane & 3;
+  const int ra = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const uint32_t base = smem_u32(gsm);
+  uint32_t s = 0;
+  for (int item = blockIdx.x; item < p.nitems; item += gridDim.x) {
+    const int ks = item % p.ksplit, tile = item / p.ksplit;
+    const int mt = tile / p.nblocks, nbk = tile % p.nblocks;
+    const int kc_begin = ks * p.kc_per, kc_end = min(p.nkc, (ks + 1) * p.kc_per);
+    // the three products of a 64-wide k chunk accumulate in the tensor core, then the chunk is promoted into an fp32 register
+    // total with round-to-nearest adds.  The tensor core truncates its fp32 accumulator after every MMA: summed over the whole
+    // K in the tensor core the error grows with the number of MMAs (measured on H100 at K = 512-768: 2-4x that of a plain
+    // fp32 GEMM, enough to flip ReLU masks of the MLP backward); promoted every 64 k it stays at the level of a plain fp32 GEMM
+    float acc[64], tot[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) tot[i] = 0.f;
+    for (int kc = kc_begin; kc < kc_end; ++kc, ++s) {
+      const uint32_t st = s % GS_STAGES;
+      mbar_wait_guarded(&ms->full[st], (s / GS_STAGES) & 1, 3);
+      const uint32_t sa = base + st * GS_STAGE_BYTES + wg * (GT_BLK_BYTES / 2);
+      const uint64_t ahi = wg_desc(sa), alo = wg_desc(sa + GT_BLK_BYTES);
+      const uint32_t sb = base + st * GS_STAGE_BYTES + 2 * GT_BLK_BYTES;
+      const uint64_t bhi = wg_desc(sb), blo = wg_desc(sb + GT_BLK_BYTES);
+      wg_fence_acc(acc);
+      wg_fence();
+#pragma unroll
+      for (int j = 0; j < GT_KC / 16; ++j) {
+        wg_m64n128_f16(acc, ahi + 2 * j, bhi + 2 * j, j != 0);
+        wg_m64n128_f16(acc, alo + 2 * j, bhi + 2 * j, 1);
+        wg_m64n128_f16(acc, ahi + 2 * j, blo + 2 * j, 1);
+      }
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_acc(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&ms->empty[st]);
+#pragma unroll
+      for (int i = 0; i < 64; ++i) tot[i] += acc[i];
+    }
+    // ---- epilogue: x 2^-(e_row + e_col) -> act -> mask -> fp32 rows.  2^-(e_row + e_col) is applied as two factors of half
+    // the exponent each (|e| <= 120 per operand): neither the factor nor the intermediate product leaves the fp32 range
+    // unless the result does.  Scale vectors are padded to whole tiles.
+    const int col0 = nbk * 128;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = mt * 128 + ra + 8 * h;
+      const int ea = (__float_as_int(__ldg(p.a_scale + row)) >> 23) & 0xff;
+      float* orow = p.out + (int64_t)ks * p.part_stride + (int64_t)row * p.ldo;
+#pragma unroll
+      for (int jb = 0; jb < 16; ++jb) {
+        const int col = col0 + 8 * jb + 2 * q4;
+        if (row >= p.M || col >= p.N) continue;
+        const float2 bs = __ldg(reinterpret_cast<const float2*>(p.b_scale + col));
+        float v[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int et = ea + ((__float_as_int(e ? bs.y : bs.x) >> 23) & 0xff) - 254;     // -(e_row + e_col)
+          const int e1 = et >> 1;
+          v[e] = (tot[4 * jb + 2 * h + e] * __int_as_float((e1 + 127) << 23)) *
+                 __int_as_float((et - e1 + 127) << 23);   // exact
+          if (p.relu) v[e] = fmaxf(v[e], 0.f);
+          if (p.mask && col + e < p.N && !(__ldg(p.mask + (int64_t)row * p.ldm + col + e) > 0.f)) v[e] = 0.f;
+        }
+        orow[col] = v[0];
+        if (col + 1 < p.N) orow[col + 1] = v[1];
+      }
+    }
   }
 }
 
@@ -666,9 +550,8 @@ static int gs_run(const void* a_image, const void* b_image, int M, int N, int K,
   p.M = M; p.N = N; p.nkc = (K + GT_KC - 1) / GT_KC;
   p.mtiles = (M + 127) / 128;
   p.nblocks = (N + 127) / 128;
-  p.ngroups = (p.nblocks + 1) / 2;
   p.ksplit = ksplit; p.kc_per = kc_per; p.part_stride = part_stride;
-  p.nitems = p.mtiles * p.ngroups * ksplit;
+  p.nitems = p.mtiles * p.nblocks * ksplit;
   p.relu = relu;
   const size_t a_img = (size_t)p.mtiles * p.nkc * GT_BLK_BYTES, b_img = (size_t)p.nblocks * p.nkc * GT_BLK_BYTES;
   p.a_hi = reinterpret_cast<const unsigned char*>(a_image); p.a_lo = p.a_hi + a_img;
@@ -703,10 +586,10 @@ extern "C" int rqb200_gemm_split(const void* a_image, const void* b_image, int M
 // [slices][M][N], and a fixed-order reduction produces out.  gemm_split_k_slices picks the slice count that fills the SMs.
 extern "C" int rqb200_gemm_split_k_slices(int M, int N, int K) {
   if (M <= 0 || N <= 0 || K <= 0) return 1;
-  int dev = 0, sm_count = 148;
+  int dev = 0, sm_count = 132;
   if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev);
   const int nkc = (K + GT_KC - 1) / GT_KC;
-  const int tiles = ((M + 127) / 128) * (((N + 127) / 128 + 1) / 2);
+  const int tiles = ((M + 127) / 128) * ((N + 127) / 128);
   int want = (sm_count + tiles - 1) / tiles;                 // slices that give every SM an item
   if (want > nkc / 4) want = nkc / 4;                        // at least 4 chunks (256 k) per slice
   if (want < 1) want = 1;
@@ -729,7 +612,7 @@ extern "C" int rqb200_gemm_split_k(const void* a_image, const void* b_image, int
   if (rc) return rc;
   const int64_t n = (int64_t)M * N;
   int grid = (int)((n + 255) / 256);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > 132 * 8) grid = 132 * 8;
   gs_reduce_kernel<<<grid, 256, 0, st>>>(workspace, slices, M, N, out, ldo);
   RQB_LAUNCH_CHECK();
   return RQB_OK;

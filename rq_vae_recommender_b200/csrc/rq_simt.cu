@@ -1,4 +1,4 @@
-// Exact-fp32 fused L-level residual-quantisation kernels (CUDA cores, sm_100a).
+// Exact-fp32 fused L-level residual-quantisation kernels (CUDA cores, sm_90a).
 //
 // One launch runs all L Quantize levels of modules/rqvae.py:125-132 for a tile of rows:
 //   * the residual tile lives in shared memory for the whole kernel (never written to HBM unless the
@@ -610,13 +610,12 @@ static int pick_tm(int B, int tn, int Dp) {
     const int f = atoi(e);
     if ((f == 8 || f == 4 || f == 2 || f == 1) && fused_smem_bytes(f, tn, Dp) <= 200 * 1024) return f;
   }
-  // Measured on B200 (tools/rq_tm_sweep.py, K=256, L=3): with a short K loop (D <= 64: at most 4 chunks per level) the
-  // 8x8 register tile costs occupancy (168 regs -> one CTA per SM) without paying back in FMA efficiency; TM=4 is 15 %
-  // faster at D=32 and 8 % at D=64, equal at D=128, and TM=2/1 are slower everywhere.
+  // With a short K loop (D <= 64: at most 4 chunks per level) the 8x8 register tile costs occupancy (168 regs -> one CTA
+  // per SM) without paying back in FMA efficiency, so TM = 4 is used there.
   int tm = (Dp <= 64) ? 4 : 8;
   while (tm >= 1 && fused_smem_bytes(tm, tn, Dp) > 200 * 1024) tm >>= 1;
   if (tm < 1) return 0;
-  while (tm > 1 && (B + 8 * tm - 1) / (8 * tm) < 148) tm >>= 1;
+  while (tm > 1 && (B + 8 * tm - 1) / (8 * tm) < 132) tm >>= 1;
   return tm;
 }
 
@@ -732,7 +731,7 @@ extern "C" int rqb200_rq_forward_from_ids(int mode, const float* x, int64_t ldx,
   if (smem > 200 * 1024) { rqb_set_error("rq_forward_from_ids: D too large (%d)", D); return RQB_ERR_UNSUPPORTED; }
   RQB_CUDA(cudaFuncSetAttribute(rq_replay_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int grid = (B + wpb - 1) / wpb;
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > 132 * 8) grid = 132 * 8;
   rq_replay_kernel<<<grid, wpb * 32, smem, reinterpret_cast<cudaStream_t>(stream)>>>(p);
   RQB_LAUNCH_CHECK();
   return RQB_OK;
@@ -760,7 +759,7 @@ extern "C" int rqb200_rq_backward(int mode, const float* x, int64_t ldx, const f
   if (smem > 200 * 1024) { rqb_set_error("rq_backward: L*D too large (%d x %d)", L, D); return RQB_ERR_UNSUPPORTED; }
   RQB_CUDA(cudaFuncSetAttribute(rq_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int grid = (B + wpb - 1) / wpb;
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > 132 * 8) grid = 132 * 8;
   rq_bwd_kernel<<<grid, wpb * 32, smem, st>>>(p);
   RQB_LAUNCH_CHECK();
   return RQB_OK;

@@ -1,11 +1,11 @@
-// Tensor-core tokeniser for sm_100a: prepared codebook state + C-ABI entry points (the kernel is csrc/rq_tcx.cu).
+// Tensor-core tokeniser for sm_90a: prepared codebook state + C-ABI entry points (the kernel is csrc/rq_tcx.cu).
 //
 // Result contract: identical to rqb200_rq_forward(mode = EVAL, ids only) -- the hard-argmin chain of
 // modules/quantize.py:113-128,159-161 x L + modules/rqvae.py:125-132 (what semids.py:125 consumes).
 //
 // Why tensor cores: the distance term x.c^T is 2*D*K*L = 1.18 MFLOP per 3 KB item (381 FLOP/B, SURVEY 8d);
 // on CUDA cores the pass is ~30x compute bound.  Why it is still exact: the fp16 product only FILTERS.
-//   S_l[b,k]  = fp16(x_b) . fp16(c_{l,k})            (tcgen05.mma, fp32 accumulate in TMEM; exact power-of-two scales)
+//   S_l[b,k]  = fp16(x_b) . fp16(c_{l,k})            (wgmma, fp32 accumulate in registers; exact power-of-two scales)
 //   score_l   = cc_{l,k} - 2 (S_l - sum_{j<l} G_{jl}[id_j, k])     (G = fp32 Gram tables C_j C_l^T, so every level is
 //               scored from the ONE fp16 image of x: the residual never has to be re-quantised or re-staged)
 //   candidates = { k : score <= min + 4 eps_b }      eps_b bounds the fp16 rounding of the dot product (margin in the epilogue)
@@ -14,16 +14,8 @@
 //
 #include "tc_common.cuh"
 
-// csrc/rq_tcx.cu: the transposed CTA-pair kernel (codes on the TMEM lanes); shares the prepared state
-// csrc/rq_tcx.cu / rq_tcx96.cu: the same kernel at two tile shapes (64 / 96 rows per CTA)
-int tcx_run_r64(const float* x, int64_t ldx, int B, const void* state, int D, int L, int64_t* ids, int* stats, int sm_count,
-                bool trace, cudaStream_t st);
-int tcx_run_r96(const float* x, int64_t ldx, int B, const void* state, int D, int L, int64_t* ids, int* stats, int sm_count,
-                bool trace, cudaStream_t st);
-// TMA needs a 16-byte aligned base and row pitch; the kernel runs as CTA pairs
-static int tcx_can_run(const float* x, int64_t ldx, int sm_count) {
-  return ((ldx & 3) == 0) && ((reinterpret_cast<uintptr_t>(x) & 15) == 0) && sm_count >= 2;
-}
+int tcx_run(const float* x, int64_t ldx, int B, const void* state, int D, int L, int64_t* ids, int* stats, int sm_count,
+            cudaStream_t st);
 
 extern "C" int rqb200_tokenize_tc_supported(int D, int K, int L) {
   return (K == TC_K && D >= TC_KC && D <= TC_MAX_D && D % TC_KC == 0 && L >= 1 && L <= RQB_MAX_LEVELS) ? 1 : 0;
@@ -121,7 +113,8 @@ __global__ void tc_prep_consts_kernel(TcHeader* hdr, int L) {
 }
 
 // Bblob[(l*2+h)*nkc + kc] = 16 KB smem image of codes [128h, 128h+128) x k [64kc, 64kc+64):
-// K-major, 128 B per code row, 16-byte chunks XOR-swizzled with (row & 7)  (UMMA SWIZZLE_128B canonical layout)
+// K-major, 128 B per code row, 16-byte chunks XOR-swizzled with (row & 7)  (the wgmma SWIZZLE_128B canonical layout); the blocks
+// h = 0 and h = 1 of a (level, chunk) form one 256-code operand in shared memory
 __global__ void tc_prep_blob_kernel(const float* const* cbs, int D, const TcHeader* hdr, __half* blob) {
   const int nkc = D / TC_KC;
   const int blk = blockIdx.x;  // (l*2+h)*nkc + kc
@@ -225,16 +218,8 @@ extern "C" int rqb200_tokenize_tc_run(const float* x, int64_t ldx, int B, const 
   int dev = 0, sm_count = 0;
   RQB_CUDA(cudaGetDevice(&dev));
   RQB_CUDA(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev));     // per call: the state may live on any device
-  // x reaches the kernel through TMA (tensor map over [B][D] fp32): 16-byte aligned base and row pitch
-  RQB_CHECK_ARG(tcx_can_run(x, ldx, sm_count),
-                "tokenize_tc_run: x must be 16-byte aligned with a row stride that is a multiple of 4 floats (and the device needs >= 2 SMs)");
-  static const bool want_trace = []() { const char* e = getenv("RQB200_TC_TRACE"); return e && e[0] == '1'; }();
-  const bool trace = want_trace && stats;       // tracing: the caller passes >= 4096 ints (tools/tc_native_check.cu)
-  // Tile shape: 96-row CTAs move a third fewer codebook bytes and hand-offs per row and win once every CTA pair has several
-  // tiles (12 101 rows: 0.041 vs 0.052 ms; 84 000: 0.193 vs 0.204); 64-row CTAs have the shorter pipeline and win below that
-  // (5 000 x 256: 0.053 vs 0.072 ms).  Both return identical ids (profiles/r2_tcx_shapes.txt).
-  static const int force = []() { const char* e = getenv("RQB200_TC_ROWS"); return e ? atoi(e) : 0; }();
-  const bool big = force ? force == 96 : (int64_t)B > 128ll * (sm_count / 2);     // more than one 64-row tile per CTA
-  return big ? tcx_run_r96(x, ldx, B, state, D, L, ids, stats, sm_count, trace, st)
-             : tcx_run_r64(x, ldx, B, state, D, L, ids, stats, sm_count, trace, st);
+  // the converter reads x as float4: 16-byte aligned base and row pitch (ops.py copies other layouts)
+  RQB_CHECK_ARG(((ldx & 3) == 0) && ((reinterpret_cast<uintptr_t>(x) & 15) == 0),
+                "tokenize_tc_run: x must be 16-byte aligned with a row stride that is a multiple of 4 floats");
+  return tcx_run(x, ldx, B, state, D, L, ids, stats, sm_count, st);
 }

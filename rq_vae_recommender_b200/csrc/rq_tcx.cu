@@ -1,761 +1,382 @@
-// Tensor-core tokeniser for sm_100a, transposed: tcgen05 fp16 candidate filter with CODES on the TMEM lanes + exact fp32 re-rank.
+// Tensor-core tokeniser for sm_90a: wgmma fp16 candidate filter + exact fp32 re-rank.
 //
 // Result contract: identical to rqb200_rq_forward(mode = EVAL, ids only) -- the hard-argmin chain of
 // modules/quantize.py:113-128,159-161 x L + modules/rqvae.py:125-132 (what semids.py:125 consumes).
 //
-//   S_l[k,b]  = fp16(c_{l,k}) . fp16(x_b)            (tcgen05.mma cta_group::2, M = 256 codes, N = 192 rows, fp32 accumulate in TMEM)
-//   h_l[k,b]  = T_l[k,b] - S_l[k,b] / 2^s,  T = cc/2 + sum_{j<l} G_{jl}[id_j(b), k]   (G = float64 Gram tables rounded once: every
-//               level is scored from the ONE fp16 image of x, the MMA stream never waits for an argmin)
+//   S_l[b,k]  = fp16(x_b) . fp16(c_{l,k})            (wgmma m64n256k16, fp32 accumulate in registers)
+//   h_l[b,k]  = T_l[b,k] - S_l[b,k] / 2^s,  T = cc/2 + sum_{j<l} G_{jl}[id_j(b), k]   (G = float64 Gram tables rounded once: every
+//               level is scored from the ONE fp16 image of x, which stays in shared memory for all L levels)
 //   candidates(b) = { k : h <= min_k h + 2 eps_b }    eps_b = DETERMINISTIC bound on |h - exact half-distance| (tc_eps, tc_common.cuh)
 //   one candidate -> it is the exact argmin;  else the candidates are re-scored with the exact fp32 arithmetic of the
 //   CUDA-core kernel (sequential fp32 residual, (xx + cc) - 2 dot, first index wins ties).
 //
-// Why transposed (round 2; the round-1 kernel had rows on the lanes): with a row per lane every score costs ~10 instructions
-// of top-3 bookkeeping and the Gram rows are per-lane gathers (32 uncoalesced 32-byte requests per row and table; measured
-// 0.53 requests/clk/SM = the L1TEX floor of the level-1/2 scans, profiles/r2_first_call_variants.txt).  With a CODE per lane
-// a row is one warp-wide step: its Gram values are ONE coalesced 128-byte line per table, the minimum over the warp's 32 codes
-// comes from a transposed butterfly over 32 rows at once (31 SHFL + 31 FMNMX per 32 rows; one CREDUX.MIN.F32 per row was tried
-// first and measured ~16 cycles per instruction and SM), the candidate set is ONE ballot.  ~14 warp instructions per 32 scores
-// instead of ~320.  The price is a merge across the 8 warps (4 TMEM lane quarters x 2 CTAs) that hold a row's 256 codes:
-// 8 bytes per (row, warp) through shared memory / DSMEM, two mbarrier hand-offs per level.
-//
-// One CTA PAIR (cluster of 2) per 192-row tile, 96 rows per CTA, persistent over tiles:
-//   CTA c holds   the fp16 image of ITS 96 rows (12 k-chunks x 12 KB, resident for all L levels: x is read from HBM once),
-//                 streams ITS 128 codes of every codebook block (16 KB stages), accumulates codes [128c, 128c+128) x 192 rows;
-//   warp 0        codebook producer: tensor-map TMA, bytes of both CTAs counted on the leader's mbarrier
-//   warp 1        MMA issuer (leader CTA only): M256 N192 K16, accumulators double-buffered in TMEM (2 x 192 columns)
-//   warp 2        x producer: fp32 boxes of 96 rows x 32 floats -> 3-stage staging ring (TMA zero-fills rows past B)
-//   warps 4-7     converters: staging -> fp16 -> K-major SWIZZLE_128B image slot; measure ||fp16(x) - x||^2 and ||x||^2 per row
-//   warps 8-15    epilogue: warp (q, ch) scans codes 128c + 32q + lane for the 96 rows of CTA ch, delivers (min, candidate mask)
-//                 per row to CTA ch; then all 8 warps of a CTA finalise its own rows (merge, exact re-rank from a shared queue)
-//                 and publish the level's ids to both CTAs (the next level's Gram rows are addressed by them).
-// Measured limits, timeline and ncu: DESIGN.md 5.2 / 6.1, profiles/r2_tcx_*.
+// One CTA per SM, persistent over 64-row tiles:
+//   warps 0-3 (one warpgroup)  convert the tile's rows to the fp16 image (K-major SWIZZLE_128B, resident for all levels) and
+//                              measure ||fp16(x) - x||^2 and ||x||^2 per row; per level: 4 x wgmma per 64-wide k chunk into a
+//                              64 x 256 register accumulator, then score.  All 256 codes of a row sit in one thread quad, so the
+//                              row minimum and the candidate set are two quad shuffles; rows with more than one candidate go to
+//                              a shared queue that the four warps re-rank exactly.
+//   warp 4                     codebook producer: the prepared 16 KB blocks of codes [0,128) and [128,256) of (level, k chunk)
+//                              -> one 32 KB stage of a ring (bulk copies counted on an mbarrier); it runs ahead into the next
+//                              level and tile while the warpgroup scores and converts.
 #include "tc_common.cuh"
-#include <type_traits>
+#include "wgmma.cuh"
 
-// Tile shape.  Everything in flight is bounded by shared memory, and the codebook stream needs (bytes per MMA cycle) x (TMA
-// latency) in flight: a stage of 16 KB feeds 4 MMAs of TX_PR / 2 cycles each, i.e. 64 B/clk/SM at TX_R = 64 and 43 B/clk at 96,
-// against a measured ~1.5-2 K cycle bulk-copy latency under load.  With 96 rows per CTA the fp16 image (144 KB) leaves room for a
-// 2-stage ring (measured: 9-12 K cycles per level instead of 4.6 K); with 64 rows (96 KB) there is room for 6 stages, four TMEM
-// accumulator buffers (the MMA stream runs up to three levels ahead of the scans), and 7 x 74 pair tiles cover 65 536 rows.
-#ifndef TX_R
-#define TX_R 64                                   // rows per CTA per tile (multiple of 32): 64 here, 96 in rq_tcx96.cu (same source)
-#endif
-// The file is compiled twice (rq_tcx96.cu includes it with TX_R = 96): every symbol with linkage carries the tile shape.
-#define TX_CAT2(a, b) a##b
-#define TX_CAT(a, b) TX_CAT2(a, b)
-#define TX_SFX(name) TX_CAT(name, TX_CAT(_r, TX_R))
-#define rq_tcx_kernel TX_SFX(rq_tcx_kernel)
-#define tcx_run TX_SFX(tcx_run)
-#define TxSmem TX_SFX(TxSmem)
-#define TxParams TX_SFX(TxParams)
-#define TX_PR (2 * TX_R)                          // rows per pair tile = MMA N
-#define TX_NG (TX_R / 32)                         // 32-row scan groups per warp and level
-#define TX_SLOT_BYTES (TX_R * TC_KC * 2)          // one k-chunk of the fp16 image
-#if TX_R == 64
-// 64 rows: image 96 KB -> 4 codebook stages, 3 staging boxes of 16 KB, four TMEM buffers, everything double-buffered.  Best for
-// small and medium batches (short tiles, 7 x 74 pair tiles cover 65 536 rows).
-#define TX_NBX 2                                  // staging boxes per chunk pair: 32 rows x 128 floats = 16 KB
-#define TX_NB_MAX 4                               // codebook ring stages (16 KB)
-#define TX_NX 3                                   // x staging ring stages
-#define TX_NT 4                                   // TMEM accumulator buffers of TX_PR columns
-#define TX_XBUF 2                                 // exchange buffers: 2 = the level-0 scan of a tile overlaps the previous tile's last finalise
-#define TX_RIBUF 2                                // row-statistics buffers
-#else
-// 96 rows: image 144 KB.  Two thirds of the codebook bytes and of the per-level hand-offs per row, but shared memory is tight:
-// 2 codebook stages, 3 staging boxes of 12 KB, two TMEM buffers, single exchange buffer.  (A 3-stage codebook ring fits only
-// with 2 staging boxes and single-buffered row statistics; measured: 0.161 vs 0.155 ms at 65 536 rows -- the ring gains what
-// the stalled converter loses.)  Best for large batches (5 x 74 pair tiles cover 65 536 rows).
-#define TX_NBX 4                                  // 24 rows x 128 floats = 12 KB
-#define TX_NB_MAX 3                               // (tcx_run takes as many stages as fit: 2 at D = 768)
-#define TX_NX 3
-#define TX_NT 2
-#define TX_XBUF 1
-#define TX_RIBUF 2
-#endif
-#define TX_XBOX_ROWS (TX_R / TX_NBX)              // fp32 staging box rows.  512-byte box rows on purpose: with 128-byte rows the TMA
-#define TX_XBOX_COLS 128                          // engine delivered 13 B/clk/SM (profiles/r2_tcx_bringup.txt)
-#define TX_XBOX_BYTES (TX_XBOX_ROWS * TX_XBOX_COLS * 4)
-#define TX_RPW (TX_XBOX_ROWS / TC_NCONV_WARPS)    // box rows per converter warp
-#define TX_ROWS_PER_FIN (TX_R / TC_NEPI_WARPS)    // rows a warp finalises per level
+#define TX_R 64                                   // rows per tile = wgmma M
+#define TX_NB_MAX 4                               // codebook ring stages
+#define TX_STAGE_BYTES (2 * TC_BSTAGE_BYTES)      // 256 codes x 64 k fp16 = 32 KB
+#define TX_SLOT_BYTES (TX_R * TC_KC * 2)          // one k chunk of the x image: 8 KB
+#define TX_THREADS 160
+#define TX_SMEM_LIMIT 232448                      // 227 KB of opt-in shared memory per block
 
 struct TxSmem {
-  uint64_t a_full[TC_MAX_KC], a_empty[TC_MAX_KC];
-  uint64_t b_full[TX_NB_MAX], b_empty[TX_NB_MAX];
-  uint64_t xs_full[TX_NX], xs_empty[TX_NX];
-  uint64_t t_full[TX_NT], t_empty[TX_NT];
-  uint64_t x_full[TX_XBUF];               // [step parity] (min, mask) of every (row of this CTA, warp slot) delivered: 4 local + 4 remote warps.
-                                    // Per parity, like exch[]: the level-0 scan of a tile does not wait for the previous tile's last finalise
-  uint64_t ids_ready;               // the level's ids of all 2 TX_R rows are in ids8[]: 8 local warps + TX_R bytes bulk-copied by the peer
-  uint64_t ri_full[2];              // rowinfo[parity] of a tile: 4 local converter warps (+ 4 TX_R bytes by st.async from the peer).
-                                    // One barrier per parity: the converters may finish tile it + 1 before the epilogue waits for tile it
-  uint32_t tmem_base;
-  uint32_t fl_count, fl_next;       // queue of rows that need the exact re-rank
-  uint32_t tiles_done;              // += 1 per epilogue warp of EITHER CTA per finished tile (monotonic: guards rowinfo[] reuse)
-  uint32_t rowinfo[TX_RIBUF][TX_PR];  // [tile % TX_RIBUF][pair row]: bf16_up(||fp16(x)-x||^2) << 16 | bf16_up(||x||^2)
+  uint64_t full[TX_NB_MAX], empty[TX_NB_MAX];
+  uint32_t fl_count, fl_next;                     // queue of rows that need the exact re-rank
+  uint32_t rowinfo[TX_R];                         // bf16_up(||fp16(x)-x||^2) << 16 | bf16_up(||x||^2)
+  uint32_t cmask[TX_R][8];                        // candidate bits of the queued rows (code 32 w + b -> word w, bit b)
   unsigned char flist[TX_R];
-  alignas(16) uint2 exch[TX_XBUF][8][TX_R];           // [step parity][warp slot = 4 * source CTA + lane quarter][row of this CTA] = (min as float bits, candidate mask)
-  alignas(16) uint2 xstage[TX_XBUF][4][TX_R];         // [step parity] what this CTA's warps found for the PEER's rows: one 768-byte DSMEM bulk copy per warp and level
 };
 
-// ---- cluster hand-offs WITHOUT cluster-scope fences.  `mbarrier.arrive.release.cluster` / `try_wait.acquire.cluster` compile to
-// MEMBAR.ALL.GPU + ERRBAR / CCTL.IVALL (seen in SASS; ~2 K cycles per converter half-box in the first run of this kernel).
-// Remote DATA therefore travels by st.async, which completes transaction bytes on the destination CTA's mbarrier: the
-// consumer's ordinary wait covers it, and remote ARRIVES only signal control (default .release.cta is enough).
-__device__ __forceinline__ void tx_arrive_remote(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void tx_arrive_expect_tx_remote(uint32_t cluster_addr, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cluster.b64 _, [%0], %1;" ::"r"(cluster_addr), "r"(bytes) : "memory");
-}
-// 8 bytes into the shared memory of any CTA of the cluster, counted (8) on the mbarrier `mbar` of that same CTA
-__device__ __forceinline__ void tx_st_async_b64(uint32_t addr, uint32_t lo, uint32_t hi, uint32_t mbar) {
-  asm volatile("{\n\t.reg .b64 v;\n\tmov.b64 v, {%1, %2};\n\t"
-               "st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.b64 [%0], v, [%3];\n\t}"
-               ::"r"(addr), "r"(lo), "r"(hi), "r"(mbar) : "memory");
-}
-// `bytes` (multiple of 16) of this CTA's shared memory -> the peer's, counted on the peer's mbarrier (cp.async.bulk through DSMEM)
-__device__ __forceinline__ void tx_bulk_s2peer(uint32_t dst_cluster, const void* src, uint32_t bytes, uint32_t mbar_cluster) {
-  asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(dst_cluster), "r"(smem_u32(src)), "r"(bytes), "r"(mbar_cluster) : "memory");
-}
-__device__ __forceinline__ void tx_st_async_b32(uint32_t addr, uint32_t v, uint32_t mbar) {
-  asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(addr), "r"(v), "r"(mbar) : "memory");
-}
-__device__ __forceinline__ void tx_red_add_cluster(uint32_t addr, uint32_t v) {
-  asm volatile("red.relaxed.cluster.shared::cluster.add.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
-}
+struct TxParams {
+  const float* x;
+  int64_t ldx;
+  int B, D, L, nkc, ntiles, nb;
+  const TcHeader* hdr;
+  const float* cc;               // [L][256]  fp32 cc of the exact kernels
+  const float* hcc;              // [L][256]  cc / 2 from float64
+  const float* gram;             // [L(L-1)/2][256][256]
+  const float* cbf;              // [L][256][D] fp32 codebook copy (exact re-rank)
+  const unsigned char* blob;     // [L][2][nkc][16 KB] fp16 codebook images
+  int64_t* ids;                  // [B][L]
+  int* stats;                    // optional: [0] rows re-ranked, [1] candidates re-scored, [2] rows with >= 3 candidates
+};
+
 // candidate margin of a row at a level: 2 eps (1 + 2^-16) from the published statistics
 __device__ __forceinline__ float tx_margin(const TcLevelConst& lc, uint32_t ri) {
   return 2.f * tc_eps(lc, __uint_as_float(ri & 0xffff0000u), __uint_as_float(ri << 16)) * 1.0000153f;
 }
-// minimum over the 32 lanes of each of 32 per-lane values; lane r returns the minimum of v[r].  Butterfly with halving: at offset
-// o a lane keeps the rows whose bit o equals its own lane bit o and sends the others: 16 + 8 + 4 + 2 + 1 shuffles.
-__device__ __forceinline__ float tx_transpose_min(const float (&v)[32], int lane) {
-  float a[16], b[8], c[4], d[2];
-  const bool u4 = lane & 16, u3 = lane & 8, u2 = lane & 4, u1 = lane & 2, u0 = lane & 1;
-#pragma unroll
-  for (int i = 0; i < 16; ++i) a[i] = fminf(u4 ? v[i + 16] : v[i], __shfl_xor_sync(0xffffffffu, u4 ? v[i] : v[i + 16], 16));
-#pragma unroll
-  for (int i = 0; i < 8; ++i) b[i] = fminf(u3 ? a[i + 8] : a[i], __shfl_xor_sync(0xffffffffu, u3 ? a[i] : a[i + 8], 8));
-#pragma unroll
-  for (int i = 0; i < 4; ++i) c[i] = fminf(u2 ? b[i + 4] : b[i], __shfl_xor_sync(0xffffffffu, u2 ? b[i] : b[i + 4], 4));
-#pragma unroll
-  for (int i = 0; i < 2; ++i) d[i] = fminf(u1 ? c[i + 2] : c[i], __shfl_xor_sync(0xffffffffu, u1 ? c[i] : c[i + 2], 2));
-  return fminf(u0 ? d[1] : d[0], __shfl_xor_sync(0xffffffffu, u0 ? d[0] : d[1], 1));
-}
-__device__ __forceinline__ float tx_transpose_sum(const float (&v)[32], int lane) {      // same butterfly, sums: lane r returns sum_lanes v[r]
-  float a[16], b[8], c[4], d[2];
-  const bool u4 = lane & 16, u3 = lane & 8, u2 = lane & 4, u1 = lane & 2, u0 = lane & 1;
-#pragma unroll
-  for (int i = 0; i < 16; ++i) a[i] = (u4 ? v[i + 16] : v[i]) + __shfl_xor_sync(0xffffffffu, u4 ? v[i] : v[i + 16], 16);
-#pragma unroll
-  for (int i = 0; i < 8; ++i) b[i] = (u3 ? a[i + 8] : a[i]) + __shfl_xor_sync(0xffffffffu, u3 ? a[i] : a[i + 8], 8);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) c[i] = (u2 ? b[i + 4] : b[i]) + __shfl_xor_sync(0xffffffffu, u2 ? b[i] : b[i + 4], 4);
-#pragma unroll
-  for (int i = 0; i < 2; ++i) d[i] = (u1 ? c[i + 2] : c[i]) + __shfl_xor_sync(0xffffffffu, u1 ? c[i] : c[i + 2], 2);
-  return (u0 ? d[1] : d[0]) + __shfl_xor_sync(0xffffffffu, u0 ? d[0] : d[1], 1);
-}
-// Barrier wait that does not spin: try_wait with a suspend-time hint parks the warp until the phase completes (or ~20 us pass).
-// The first run of this kernel spent 40 % of its executed instructions in try_wait / clock64 polling loops (ncu capture of
-// that build, summarised in DESIGN.md 5.2): warps that wait must not take issue slots from the four converter / eight epilogue warps that work.
-__device__ __forceinline__ bool tx_try_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-      "selp.b32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity), "r"(20000u) : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ void tx_wait(uint64_t* bar, uint32_t parity) {
-  if (tx_try_wait(bar, parity)) return;
-  uint32_t n = 0;
-  while (!tx_try_wait(bar, parity)) {
-    if (++n > 200000u) __trap();          // ~4 s: a protocol bug, never legitimate
-  }
-}
-__device__ __forceinline__ void tx_epi_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }   // the 8 epilogue warps of this CTA
+__device__ __forceinline__ void tx_wg_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }   // the 4 warps of the warpgroup
 
-struct TxParams {
-  CUtensorMap tmapB;    // fp16 codebook blob viewed as [blocks * 16][256 x 32 bit] (1 KB rows), box = 16 rows = one 16 KB block
-  CUtensorMap tmapX;    // x as a [B][D] fp32 tensor, box = 24 rows x 128 floats
-  const float* x;
-  int64_t ldx;
-  int B, D, L, nkc, ntiles;     // ntiles = pair tiles of 192 rows
-  const TcHeader* hdr;
-  const float* cc;      // [L][256]  fp32 cc of the exact kernels
-  const float* hcc;     // [L][256]  cc / 2 from float64
-  const float* gram;    // [L(L-1)/2][256][256]
-  const float* cbf;     // [L][256][D] fp32 codebook copy (exact re-rank)
-  int64_t* ids;         // [B][L]
-  int* stats;           // optional: [0] rows re-ranked, [1] candidates re-scored, [2] rows with >= 3 candidates
-  int prefetch;         // 1: the x producer pulls the next tile's rows into L2 while this tile is staged
-  int nb;               // codebook ring stages in use (<= TX_NB_MAX)
-};
-
-template <bool kTrace>
-__global__ void __launch_bounds__(TC_THREADS, 1) rq_tcx_kernel(const __grid_constant__ TxParams p) {
+__global__ void __launch_bounds__(TX_THREADS, 1) rq_tcx_kernel(const __grid_constant__ TxParams p) {
   extern __shared__ __align__(1024) unsigned char tsm[];
-  unsigned char* sX = tsm;                                          // [TC_MAX_KC][12 KB] fp16 image of this CTA's rows
-  unsigned char* sC = sX + TC_MAX_KC * TX_SLOT_BYTES;               // [TX_NB][16 KB] codebook ring
-  unsigned char* sS = sC + p.nb * TC_BSTAGE_BYTES;                  // [TX_NX] fp32 staging ring
-  TxSmem* ms = reinterpret_cast<TxSmem*>(sS + TX_NX * TX_XBOX_BYTES);
-  // ids of the current tile, level-major bytes [L][TX_PR] behind the fixed part (sized by L at launch: at TX_R = 96 the third
-  // codebook stage only fits with <= 4 levels of them)
-  unsigned char* const ids8 = reinterpret_cast<unsigned char*>(ms + 1);
-  const uint32_t nb = (uint32_t)p.nb;                                 // codebook ring depth (run time: see tcx_run)
-
+  const int nkc = p.nkc, L = p.L, D = p.D;
+  const uint32_t nb = (uint32_t)p.nb;
+  unsigned char* sX = tsm;                                   // [nkc][8 KB] fp16 image of the tile's rows
+  unsigned char* sC = sX + nkc * TX_SLOT_BYTES;              // [nb][32 KB] codebook ring
+  TxSmem* ms = reinterpret_cast<TxSmem*>(sC + nb * TX_STAGE_BYTES);
+  unsigned char* const ids8 = reinterpret_cast<unsigned char*>(ms + 1);   // [L][TX_R] ids of the tile
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int nkc = p.nkc, L = p.L;
-  const bool trace = kTrace && p.stats != nullptr;
-  const uint32_t crank = cluster_ctarank();                          // 0 = leader
-  const int u_first = (int)(blockIdx.x >> 1), u_step = (int)(gridDim.x >> 1), u_count = p.ntiles;
 
   if (tid == 0) {
-    if ((smem_u32(tsm) & 1023u) != 0) __trap();                      // the swizzle pattern needs a 1024-byte aligned base
-    for (int i = 0; i < TC_MAX_KC; ++i) { mbar_init(&ms->a_full[i], 2 * TX_NBX * TC_NCONV_WARPS); mbar_init(&ms->a_empty[i], 1); }
-    for (int i = 0; i < TX_NB_MAX; ++i) { mbar_init(&ms->b_full[i], 1); mbar_init(&ms->b_empty[i], 1); }
-    for (int i = 0; i < TX_NX; ++i) { mbar_init(&ms->xs_full[i], 1); mbar_init(&ms->xs_empty[i], TC_NCONV_WARPS); }
-    for (int i = 0; i < TX_NT; ++i) { mbar_init(&ms->t_full[i], 1); mbar_init(&ms->t_empty[i], 2 * TC_NEPI_WARPS); }
-    for (int i = 0; i < TX_XBUF; ++i) mbar_init(&ms->x_full[i], TC_NEPI_WARPS);
-    mbar_init(&ms->ids_ready, TC_NEPI_WARPS);
-    mbar_init(&ms->ri_full[0], TC_NCONV_WARPS); mbar_init(&ms->ri_full[1], TC_NCONV_WARPS);
-    ms->fl_count = 0; ms->fl_next = 0; ms->tiles_done = 0;
+    if ((smem_u32(tsm) & 1023u) != 0) __trap();              // the swizzle pattern needs a 1024-byte aligned base
+    for (int i = 0; i < TX_NB_MAX; ++i) { mbar_init(&ms->full[i], 1); mbar_init(&ms->empty[i], 4); }
+    ms->fl_count = 0; ms->fl_next = 0;
     fence_mbar_init();
   }
-  if (warp == 1) tc_alloc2(&ms->tmem_base, 512);                   // TX_NT x TX_PR <= 512 columns
-  tc_fence_before();
   __syncthreads();
-  cluster_sync_all();                                                // the peer's barriers exist before anything remote touches them
-  tc_fence_after();
-  #define TX_TMEM_BASE() (*reinterpret_cast<volatile uint32_t*>(&ms->tmem_base))
 
-  if (warp < 4) {
-    // register budget of the CTA (512 threads x 128 at launch = 65536): 128 x 40 + 128 x 104 + 256 x 184
-    tc_setmaxnreg_dec<40>();
-    if (warp == 0) {
-      // ============================================================== codebook producer: this CTA's 128 codes of (level, chunk)
+  if (warp == 4) {
+    // ============================================================== codebook producer
+    if (lane == 0) {
       uint32_t s = 0;
-      for (int unit = u_first; unit < u_count; unit += u_step)
+      for (int unit = blockIdx.x; unit < p.ntiles; unit += gridDim.x)
         for (int l = 0; l < L; ++l)
           for (int kc = 0; kc < nkc; ++kc, ++s) {
             const uint32_t st = s % nb, u = s / nb;
-            tx_wait(&ms->b_empty[st], (u & 1) ^ 1);     // local: the leader's commits are multicast
-            if (tc_elect_one()) {
-              if (crank == 0) mbar_expect_tx(&ms->b_full[st], 2 * TC_BSTAGE_BYTES);
-              tc_tma2d_pair(sC + st * TC_BSTAGE_BYTES, &p.tmapB, 0, ((l * 2 + (int)crank) * nkc + kc) * 16,
-                            cluster_map(smem_u32(&ms->b_full[st]), 0));
-            }
-            __syncwarp();
+            mbar_wait_guarded(&ms->empty[st], (u & 1) ^ 1, 1);
+            mbar_expect_tx(&ms->full[st], TX_STAGE_BYTES);
+            unsigned char* dst = sC + st * TX_STAGE_BYTES;
+            bulk_g2s(dst, p.blob + ((size_t)(l * 2) * nkc + kc) * TC_BSTAGE_BYTES, TC_BSTAGE_BYTES, &ms->full[st]);
+            bulk_g2s(dst + TC_BSTAGE_BYTES, p.blob + ((size_t)(l * 2 + 1) * nkc + kc) * TC_BSTAGE_BYTES, TC_BSTAGE_BYTES,
+                     &ms->full[st]);
           }
-    } else if (warp == 1 && crank == 0) {
-      // ============================================================== MMA issuer: D[codes, rows] += C_block . X_chunk^T
-      const uint32_t idesc = tc_idesc(256, TX_PR);
-      const uint32_t x_base = smem_u32(sX), c_base = smem_u32(sC);
-      uint32_t s = 0, g = 0, it = 0;
-      TC_EV_DECL();
-      for (int unit = u_first; unit < u_count; unit += u_step, ++it)
-        for (int l = 0; l < L; ++l, ++g) {
-          const uint32_t buf = g % TX_NT, u = g / TX_NT;
-          tx_wait(&ms->t_empty[buf], (u & 1) ^ 1);
-          TC_EV(0, 1, it * 16 + l);
-          tc_fence_after();
-          const uint32_t d_base = TX_TMEM_BASE() + buf * TX_PR;
-          for (int kc = 0; kc < nkc; ++kc, ++s) {
-            if (l == 0) {
-              tx_wait(&ms->a_full[kc], it & 1);
-              TC_EV(0, 2, it * 16 + kc);
-            }
-            const uint32_t st = s % nb;
-            tx_wait(&ms->b_full[st], (s / nb) & 1);
-            tc_fence_after();
-            const uint64_t adesc = tc_smem_desc(c_base + st * TC_BSTAGE_BYTES);      // M side: codes
-            const uint64_t bdesc = tc_smem_desc(x_base + kc * TX_SLOT_BYTES);        // N side: rows
-            if (tc_elect_one()) {
-#pragma unroll
-              for (int j = 0; j < TC_KC / 16; ++j)      // K = 16 per instruction: +32 B inside the 128 B swizzle row
-                tc_mma_f16_2(d_base, adesc + 2 * j, bdesc + 2 * j, idesc, (kc | j) != 0);
-              tc_commit2(&ms->b_empty[st]);
-              if (l == L - 1) tc_commit2(&ms->a_empty[kc]);
-              if (kc == nkc - 1) tc_commit2(&ms->t_full[buf]);
-            }
-            __syncwarp();
-          }
-          TC_EV(0, 3, it * 16 + l);
-        }
-    } else if (warp == 2) {
-      // ============================================================== x producer: fp32 boxes of 24 rows x 2 k-chunks -> staging ring
-      uint32_t ls = 0;
-      const int npair = (nkc + 1) >> 1;
-      for (int unit = u_first; unit < u_count; unit += u_step) {
-        const int row0 = (unit * 2 + (int)crank) * TX_R;             // rows past B / columns past D read as zero (tensor-map bounds)
-        if (p.prefetch && unit + u_step < u_count) {
-          // pull the NEXT tile's rows into L2 now: the staging ring (36 KB in flight) then runs at L2 latency, not HBM's
-          const int nrow0 = ((unit + u_step) * 2 + (int)crank) * TX_R;
-          for (int r = lane; r < TX_R; r += 32)
-            if (nrow0 + r < p.B) bulk_prefetch_l2(p.x + (int64_t)(nrow0 + r) * p.ldx, (uint32_t)p.D * 4u);
-        }
-        for (int pr = 0; pr < npair; ++pr)
-          for (int bx = 0; bx < TX_NBX; ++bx, ++ls) {
-            const uint32_t st = ls % TX_NX;
-            tx_wait(&ms->xs_empty[st], ((ls / TX_NX) & 1) ^ 1);
-            if (tc_elect_one()) {
-              mbar_expect_tx(&ms->xs_full[st], TX_XBOX_BYTES);
-              tc_tma2d(sS + st * TX_XBOX_BYTES, &p.tmapX, pr * TX_XBOX_COLS, row0 + bx * TX_XBOX_ROWS, &ms->xs_full[st]);
-            }
-            __syncwarp();
-          }
-      }
     }
-  } else if (warp < 4 + TC_NCONV_WARPS) {
-    // ============================================================== converters: staging box -> fp16 image slots + row statistics
-    // A box is 24 rows x 128 floats (k-chunks 2 pr and 2 pr + 1).  Warp cw owns box rows [6cw, 6cw + 6); lane = float4 column:
-    // one LDS.128 of a warp is one whole 512-byte staging row (conflict-free), one STS.64 writes that row's 128 bytes in each of
-    // the two chunk slots.
-    tc_setmaxnreg_dec<104>();
-    const int cw = warp - 4;
-    const int sub = lane >> 4;                                       // which of the two chunks this lane's columns belong to
-    const uint32_t u16 = (uint32_t)(lane & 15) >> 1, hoff = (uint32_t)(lane & 1) * 8u;
-    const int npair = (nkc + 1) >> 1;
-    uint32_t it = 0, ls = 0;
-    TC_EV_DECL();
-    const uint32_t peer_ri = cluster_map(smem_u32(&ms->rowinfo[0][0]), crank ^ 1u);
-    const uint32_t peer_rifull0 = cluster_map(smem_u32(&ms->ri_full[0]), crank ^ 1u);
-    const uint32_t afull_leader = cluster_map(smem_u32(&ms->a_full[0]), 0);
+    return;
+  }
+
+  // ============================================================== warpgroup
+  const int q4 = lane & 3;
+  const int r0 = warp * 16 + (lane >> 2), r1 = r0 + 8;      // accumulator rows of this thread
+  const int lane4 = lane * 4;
+  const uint32_t x_base = smem_u32(sX), c_base = smem_u32(sC);
+  uint32_t s = 0;
 #pragma unroll 1
-    for (int unit = u_first; unit < u_count; unit += u_step, ++it) {
-      float s2[TX_NBX][TX_RPW], e2[TX_NBX][TX_RPW];                                      // per (box of the pair step, row): partial sums of this lane's columns
+  for (int unit = blockIdx.x; unit < p.ntiles; unit += gridDim.x) {
+    const int row0 = unit * TX_R;
+    // ---- fp16 image + row statistics: warp w converts rows [16w, 16w + 16); lane = float4 column of every 512-byte stretch
+#pragma unroll 2
+    for (int i = 0; i < 16; ++i) {
+      const int R = warp * 16 + i, grow = row0 + R;
+      const float* xr = p.x + (int64_t)grow * p.ldx;
+      float4 v[6];
 #pragma unroll
-      for (int bx = 0; bx < TX_NBX; ++bx)
+      for (int c4 = 0; c4 < 6; ++c4) {
+        const int c = c4 * 128 + lane4;
+        v[c4] = (grow < p.B && c < D) ? __ldg(reinterpret_cast<const float4*>(xr + c)) : make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+      float s2 = 0.f, e2 = 0.f;
 #pragma unroll
-        for (int i = 0; i < TX_RPW; ++i) { s2[bx][i] = 0.f; e2[bx][i] = 0.f; }
+      for (int c4 = 0; c4 < 6; ++c4) {
+        const int c = c4 * 128 + lane4;
+        if (c < D) {
+          const float4 a = v[c4];
+          const __half2 h0 = __floats2half2_rn(a.x, a.y), h1 = __floats2half2_rn(a.z, a.w);
+          // the MEASURED rounding error of this row: fp16(x) - x is exact in fp32 (nearby values, or a flush to zero / inf)
+          const float2 b0 = __half22float2(h0), b1 = __half22float2(h1);
+          const float d0 = b0.x - a.x, d1 = b0.y - a.y, d2 = b1.x - a.z, d3 = b1.y - a.w;
+          s2 = fmaf(a.x, a.x, fmaf(a.y, a.y, fmaf(a.z, a.z, fmaf(a.w, a.w, s2))));
+          e2 = fmaf(d0, d0, fmaf(d1, d1, fmaf(d2, d2, fmaf(d3, d3, e2))));
+          const uint32_t addr = x_base + (uint32_t)(c >> 6) * TX_SLOT_BYTES + (uint32_t)R * 128u +
+                                ((((uint32_t)(c & 63) >> 3) ^ ((uint32_t)R & 7u)) << 4) + (uint32_t)(c & 7) * 2u;
+          asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(*reinterpret_cast<const uint32_t*>(&h0)),
+                       "r"(*reinterpret_cast<const uint32_t*>(&h1)) : "memory");
+        }
+      }
+      s2 = warp_sum(s2); e2 = warp_sum(e2);
+      if (lane == 0) ms->rowinfo[R] = (tc_bf16_up(e2) << 16) | tc_bf16_up(s2);
+    }
+    fence_proxy_async();                 // generic-proxy smem writes -> visible to the tensor core (async proxy)
+    tx_wg_sync();
+
 #pragma unroll 1
-      for (int pr = 0; pr < npair; ++pr) {
-        const int kc0 = 2 * pr;
-        const bool has1 = kc0 + 1 < nkc;
-        const bool mine = (sub == 0) || has1;                        // D = 64 (2 pr + 1 == nkc): the upper 64 columns are TMA zero fill
-        tx_wait(&ms->a_empty[kc0], (it & 1) ^ 1);       // the previous tile's last level released these slots
-        if (has1) tx_wait(&ms->a_empty[kc0 + 1], (it & 1) ^ 1);
-        const uint32_t slot = smem_u32(sX) + (uint32_t)(kc0 + sub) * TX_SLOT_BYTES + hoff;
+    for (int l = 0; l < L; ++l) {
+      // ---- S = X . C_l^T over the k chunks; a stage is released as soon as the MMAs that read it have completed
+      float acc[128];
+      uint32_t prev = 0;
+#pragma unroll 1
+      for (int kc = 0; kc < nkc; ++kc, ++s) {
+        const uint32_t st = s % nb;
+        mbar_wait_guarded(&ms->full[st], (s / nb) & 1, 2);
+        const uint64_t ad = wg_desc(x_base + kc * TX_SLOT_BYTES), bd = wg_desc(c_base + st * TX_STAGE_BYTES);
+        wg_fence_acc(acc);
+        wg_fence();
 #pragma unroll
-        for (int bx = 0; bx < TX_NBX; ++bx, ++ls) {
-          const uint32_t st = ls % TX_NX;
-          tx_wait(&ms->xs_full[st], (ls / TX_NX) & 1);
-          if (cw == 0) TC_EV(1, 1, it * 16 + kc0);
-          const unsigned char* sp = sS + st * TX_XBOX_BYTES + (cw * TX_RPW) * (TX_XBOX_COLS * 4) + lane * 16;
-          float4 v[TX_RPW];
-#pragma unroll
-          for (int i = 0; i < TX_RPW; ++i) v[i] = *reinterpret_cast<const float4*>(sp + i * (TX_XBOX_COLS * 4));
-#pragma unroll
-          for (int i = 0; i < TX_RPW; ++i) {
-            const float4 a = v[i];
-            const __half2 h0 = __floats2half2_rn(a.x, a.y), h1 = __floats2half2_rn(a.z, a.w);
-            // the MEASURED rounding error of this row: fp16(x) - x is exact in fp32 (nearby values, or a flush to zero / inf)
-            const float2 b0 = __half22float2(h0), b1 = __half22float2(h1);
-            const float d0 = b0.x - a.x, d1 = b0.y - a.y, d2 = b1.x - a.z, d3 = b1.y - a.w;
-            s2[bx][i] = fmaf(a.x, a.x, fmaf(a.y, a.y, fmaf(a.z, a.z, fmaf(a.w, a.w, s2[bx][i]))));
-            e2[bx][i] = fmaf(d0, d0, fmaf(d1, d1, fmaf(d2, d2, fmaf(d3, d3, e2[bx][i]))));
-            const uint32_t R = (uint32_t)(bx * TX_XBOX_ROWS + cw * TX_RPW + i);      // image row; 16-byte units XOR-swizzled with R & 7
-            const uint32_t addr = slot + R * 128u + ((u16 ^ (R & 7u)) << 4);
-            if (mine)
-              asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(*reinterpret_cast<const uint32_t*>(&h0)),
-                           "r"(*reinterpret_cast<const uint32_t*>(&h1)) : "memory");
-          }
-          if (pr == npair - 1 && bx == TX_NBX - 1) {
-            // row statistics of the tile -> both CTAs (the scan of either CTA needs the margin of all 192 rows).  The buffer of
-            // this index was last read by the epilogue of tile it - TX_RIBUF (both CTAs): wait until all 16 warps have left that tile.
-            if (it >= TX_RIBUF) {
-              const long long t0 = clock64();
-              while (*reinterpret_cast<volatile uint32_t*>(&ms->tiles_done) < 2u * TC_NEPI_WARPS * (it - TX_RIBUF + 1)) {
-                __nanosleep(200);
-                if (clock64() - t0 > 4000000000LL) __trap();
-              }
-            }
-            {
-              // TX_NBX * TX_RPW rows x 2 statistics, each spread over the 32 lanes: two transposed butterfly sums (lane r gets row r's totals)
-              float vs[32], ve[32];
-#pragma unroll
-              for (int b2 = 0; b2 < TX_NBX; ++b2)
-#pragma unroll
-                for (int i = 0; i < TX_RPW; ++i) { vs[b2 * TX_RPW + i] = s2[b2][i]; ve[b2 * TX_RPW + i] = e2[b2][i]; }
-#pragma unroll
-              for (int r = TX_NBX * TX_RPW; r < 32; ++r) { vs[r] = 0.f; ve[r] = 0.f; }
-              const float ss = tx_transpose_sum(vs, lane), ee = tx_transpose_sum(ve, lane);
-              if (lane < TX_NBX * TX_RPW) {
-                const uint32_t ri = (tc_bf16_up(ee) << 16) | tc_bf16_up(ss);
-                const uint32_t idx = (it % TX_RIBUF) * TX_PR + crank * TX_R + (uint32_t)((lane / TX_RPW) * TX_XBOX_ROWS + cw * TX_RPW + lane % TX_RPW);
-                (&ms->rowinfo[0][0])[idx] = ri;
-                tx_st_async_b32(peer_ri + idx * 4u, ri, peer_rifull0 + (it & 1) * 8u);
-              }
-            }
-            __syncwarp();
-            if (lane == 0) { if (cw == 0) mbar_expect_tx(&ms->ri_full[it & 1], TX_R * 4u); else mbar_arrive(&ms->ri_full[it & 1]); }
-          }
-          fence_proxy_async();                 // generic-proxy smem writes -> visible to the tensor-core (async) proxy
+        for (int j = 0; j < TC_KC / 16; ++j) wg_m64n256_f16(acc, ad + 2 * j, bd + 2 * j, (kc | j) != 0);
+        wg_commit();
+        wg_fence_acc(acc);
+        if (kc > 0) {
+          wg_wait<1>();
           __syncwarp();
-          if (lane == 0) {
-            mbar_arrive(&ms->xs_empty[st]);    // the STS above consumed every loaded value: the staging box is free
-            tx_arrive_remote(afull_leader + kc0 * 8u);
-            if (has1) tx_arrive_remote(afull_leader + (kc0 + 1) * 8u);
+          if (lane == 0) mbar_arrive(&ms->empty[prev]);
+        }
+        prev = st;
+      }
+      wg_wait<0>();
+      wg_fence_acc(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&ms->empty[prev]);
+
+      // ---- score: h = T - S / 2^s in place; columns 8 jb + 2 q4 + {0, 1} of rows r0 (acc[4 jb + 0..1]) and r1 (acc[4 jb + 2..3])
+      const TcLevelConst lc = p.hdr->lv[l];
+      const float ninv = -1.f / lc.sc;
+      if (l == 0) {
+#pragma unroll
+        for (int jb = 0; jb < 32; ++jb) {
+          const float2 t = __ldg(reinterpret_cast<const float2*>(p.hcc + 8 * jb + 2 * q4));
+          acc[4 * jb + 0] = fmaf(acc[4 * jb + 0], ninv, t.x); acc[4 * jb + 1] = fmaf(acc[4 * jb + 1], ninv, t.y);
+          acc[4 * jb + 2] = fmaf(acc[4 * jb + 2], ninv, t.x); acc[4 * jb + 3] = fmaf(acc[4 * jb + 3], ninv, t.y);
+        }
+      } else {
+        // Gram rows of the previous levels' ids, table (j, l) at gram + (l (l - 1) / 2 + j) 256^2, summed in level order
+        const float* g0 = p.gram + (size_t)(l * (l - 1) / 2) * TC_K * TC_K + 2 * q4;
+        const float* a0 = g0 + (uint32_t)ids8[r0] * TC_K;
+        const float* a1 = g0 + (uint32_t)ids8[r1] * TC_K;
+#pragma unroll
+        for (int jb = 0; jb < 32; ++jb) {
+          float2 t0 = __ldg(reinterpret_cast<const float2*>(a0 + 8 * jb));
+          float2 t1 = __ldg(reinterpret_cast<const float2*>(a1 + 8 * jb));
+#pragma unroll 1
+          for (int j = 1; j < l; ++j) {
+            const float* gj = g0 + (size_t)j * TC_K * TC_K + 8 * jb;
+            const float2 u0 = __ldg(reinterpret_cast<const float2*>(gj + (uint32_t)ids8[j * TX_R + r0] * TC_K));
+            const float2 u1 = __ldg(reinterpret_cast<const float2*>(gj + (uint32_t)ids8[j * TX_R + r1] * TC_K));
+            t0.x += u0.x; t0.y += u0.y; t1.x += u1.x; t1.y += u1.y;
           }
-          if (cw == 0) TC_EV(1, 2, it * 16 + kc0);
+          acc[4 * jb + 0] = fmaf(acc[4 * jb + 0], ninv, t0.x); acc[4 * jb + 1] = fmaf(acc[4 * jb + 1], ninv, t0.y);
+          acc[4 * jb + 2] = fmaf(acc[4 * jb + 2], ninv, t1.x); acc[4 * jb + 3] = fmaf(acc[4 * jb + 3], ninv, t1.y);
         }
       }
-    }
-  } else {
-    // ============================================================== epilogue: scan -> deliver -> finalise (merge, exact re-rank) -> ids
-    tc_setmaxnreg_inc<184>();
-    const int e = warp - (4 + TC_NCONV_WARPS);           // 0..7
-    const int q = warp & 3;                              // TMEM lane quarter this warp may read
-    const int ch = e >> 2;                               // the CTA whose rows this warp scans
-    const int kq = (int)crank * 128 + q * 32 + lane;     // this lane's code
-    const uint32_t slot = crank * 4u + (uint32_t)q;
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    const int D = p.D;
-    const int lane4 = lane * 4;
-    const bool own = (ch == (int)crank);                 // this warp scans its own CTA's rows: results stay local
-    uint2* const xout0 = own ? &ms->exch[0][slot][0] : &ms->xstage[0][q][0];      // + (g & 1) * (exch or xstage parity stride)
-    const uint32_t xout_pstride = own ? 8u * TX_R : 4u * TX_R;
-    const uint32_t exch_peer0 = cluster_map(smem_u32(&ms->exch[0][slot][0]), crank ^ 1u);
-    const uint32_t xfull_dst0 = cluster_map(smem_u32(&ms->x_full[0]), (uint32_t)ch);
-    const uint32_t ids_peer = cluster_map(smem_u32(ids8), crank ^ 1u);
-    const uint32_t idsrdy_peer = cluster_map(smem_u32(&ms->ids_ready), crank ^ 1u);
-    const uint32_t tempty_leader = cluster_map(smem_u32(&ms->t_empty[0]), 0);
-    const bool designated = (e == 4 * (int)crank);       // scans this CTA's own rows (ch == crank): see the queue reset below
-    uint32_t g = 0, it = 0;
-    TC_EV_DECL();
-    // per-warp phase clocks of CTA 0 (trace instantiation): [step < 24][warp e][5] at stats + 2176 (64-bit)
-    #define TX_PH(k) do { if (ev_on && lane == 0 && g < 24) reinterpret_cast<long long*>(p.stats + 2176)[(g * 8 + e) * 5 + (k)] = clock64(); } while (0)
-    const int ev_role = 2 + ch;                          // lane quarter 0 only
-#pragma unroll 1
-    for (int unit = u_first; unit < u_count; unit += u_step, ++it) {
-      uint32_t ri0 = 0u, ri1 = 0u, ri2 = 0u;             // (ri2 unused when TX_NG == 2)             // row statistics of the rows this lane is "home" of during the scan
-#pragma unroll 1
-      for (int l = 0; l < L; ++l, ++g) {
-        const uint32_t buf = g % TX_NT, u = g / TX_NT;
-        const TcLevelConst lc = p.hdr->lv[l];
-        const float ninv = -1.f / lc.sc;
-        // Gram tables (j, l), j < l, offset to this lane's code; level 0 scores against cc/2
-        const float* g0 = p.gram + (size_t)(l * (l - 1) / 2) * TC_K * TC_K + kq;
-        const float t0 = (l == 0) ? __ldg(p.hcc + kq) : 0.f;
-        // ids of the previous level (Gram row addresses).  Level 0 needs none: its scan overlaps the previous tile's last
-        // finalise / re-rank (exch[], xstage[], x_full[] alternate with the step parity; the phase of ids_ready it skips is
-        // complete before the next one can be: the next arrivals come after this step's finalise)
-        if ((l > 0 || TX_XBUF == 1) && g > 0) tx_wait(&ms->ids_ready, (g - 1) & 1);
-        const uint32_t xb = g % TX_XBUF, xph = (g / TX_XBUF) & 1;      // exchange buffer of this step and its barrier phase
-        uint2* const xout = xout0 + xb * xout_pstride;
-        const uint32_t xfull_dst = xfull_dst0 + xb * 8u;
-        if (l == 0) {
-          tx_wait(&ms->ri_full[it & 1], (it >> 1) & 1);                       // row statistics of this tile (both CTAs' rows)
-          ri0 = ms->rowinfo[it % TX_RIBUF][ch * TX_R + lane];
-          ri1 = ms->rowinfo[it % TX_RIBUF][ch * TX_R + 32 + lane];
-          if (TX_NG > 2) ri2 = ms->rowinfo[it % TX_RIBUF][ch * TX_R + 64 + lane];
-        }
-        const float mg0 = tx_margin(lc, ri0), mg1 = tx_margin(lc, ri1), mg2 = tx_margin(lc, ri2);
-        tx_wait(&ms->t_full[buf], u & 1);
-        if (q == 0) TC_EV(ev_role, 1, it * 16 + l);
-        tc_fence_after();
-        const uint32_t tcol = TX_TMEM_BASE() + lane_addr + buf * TX_PR + ch * TX_R;
-        // ---- scan: 3 groups of 32 rows; NT = number of Gram tables (compile-time: the inner loops carry no branches).
-        // Per group: 32 scores per lane -> transposed butterfly minimum (lane r ends up with the minimum of row r over the warp's
-        // 32 codes: 31 SHFL + 31 FMNMX for 32 rows; CREDUX.MIN.F32 measured ~16 cycles per instruction and SM) -> threshold in
-        // the row's home lane -> one broadcast + ballot per row.
-        auto scan = [&](auto nt_tag) {
-          constexpr int NT = decltype(nt_tag)::value;
-          uint32_t sa[32];
-          tc_ld32_issue(tcol, sa);
-#pragma unroll 1
-          for (int g3 = 0; g3 < TX_NG; ++g3) {
-            const float mgg = g3 == 0 ? mg0 : (g3 == 1 ? mg1 : mg2);         // margin of row 32 g3 + lane
-            const unsigned char* idrow = ids8 + ch * TX_R + g3 * 32;
-            float h[32];
-            if constexpr (NT == 0) {
-              tc_ld_wait();
+      // ---- row minimum over the quad's 256 codes, then the candidate bits (NaN keeps the code)
+      float m0 = INFINITY, m1 = INFINITY;
 #pragma unroll
-              for (int r = 0; r < 32; ++r) h[r] = fmaf(__uint_as_float(sa[r]), ninv, t0);
-            } else {
+      for (int jb = 0; jb < 32; ++jb) {
+        m0 = fminf(m0, fminf(acc[4 * jb + 0], acc[4 * jb + 1]));
+        m1 = fminf(m1, fminf(acc[4 * jb + 2], acc[4 * jb + 3]));
+      }
 #pragma unroll
-              for (int r = 0; r < 32; ++r) {                                 // all gathers of the group in flight together
-                // uniform byte loads (every lane reads the same address), then ONE coalesced 128-byte line per table and row
-                h[r] = __ldg(g0 + (uint32_t)idrow[r] * (uint32_t)TC_K);
-                if constexpr (NT >= 2) h[r] += __ldg(g0 + TC_K * TC_K + (uint32_t)idrow[TX_PR + r] * (uint32_t)TC_K);
-                if constexpr (NT >= 3) {
-#pragma unroll 1
-                  for (int j = 2; j < l; ++j) h[r] += __ldg(g0 + (size_t)j * TC_K * TC_K + (uint32_t)idrow[j * TX_PR + r] * (uint32_t)TC_K);
-                }
-              }
-              tc_ld_wait();
+      for (int o = 1; o < 4; o <<= 1) {
+        m0 = fminf(m0, __shfl_xor_sync(0xffffffffu, m0, o));
+        m1 = fminf(m1, __shfl_xor_sync(0xffffffffu, m1, o));
+      }
+      const float thr0 = m0 + tx_margin(lc, ms->rowinfo[r0]), thr1 = m1 + tx_margin(lc, ms->rowinfo[r1]);
+      uint32_t w0[8], w1[8];
+      int cnt0 = 0, cnt1 = 0, first0 = 256, first1 = 256;
 #pragma unroll
-              for (int r = 0; r < 32; ++r) h[r] = fmaf(__uint_as_float(sa[r]), ninv, h[r]);
-            }
-            if (g3 < TX_NG - 1) tc_ld32_issue(tcol + (g3 + 1) * 32, sa);             // next group's scores in flight
-            const float km = tx_transpose_min(h, lane);
-            const float thr = km + mgg;
-            uint2* const xo = xout + g3 * 32;
-            xo[lane].x = __float_as_uint(km);
+      for (int w = 7; w >= 0; --w) {
+        uint32_t b0 = 0u, b1 = 0u;
 #pragma unroll
-            for (int r = 0; r < 32; ++r) {
-              const uint32_t mask = __ballot_sync(0xffffffffu, !(h[r] > __shfl_sync(0xffffffffu, thr, r)));   // NaN keeps the code
-              if (lane == 0) xo[r].y = mask;
-            }
+        for (int t = 0; t < 4; ++t)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const uint32_t bit = 1u << (8 * t + 2 * q4 + e);
+            b0 |= !(acc[4 * (4 * w + t) + e] > thr0) ? bit : 0u;
+            b1 |= !(acc[4 * (4 * w + t) + 2 + e] > thr1) ? bit : 0u;
           }
+        b0 |= __shfl_xor_sync(0xffffffffu, b0, 1); b0 |= __shfl_xor_sync(0xffffffffu, b0, 2);
+        b1 |= __shfl_xor_sync(0xffffffffu, b1, 1); b1 |= __shfl_xor_sync(0xffffffffu, b1, 2);
+        w0[w] = b0; w1[w] = b1;
+        cnt0 += __popc(b0); cnt1 += __popc(b1);
+        first0 = b0 ? w * 32 + __ffs(b0) - 1 : first0;
+        first1 = b1 ? w * 32 + __ffs(b1) - 1 : first1;
+      }
+      if (q4 < 2) {                                         // lane 4i + 0 finalises row r0, lane 4i + 1 row r1
+        const int r = q4 ? r1 : r0, cnt = q4 ? cnt1 : cnt0, first = q4 ? first1 : first0;
+        const int grow = row0 + r;
+        if (cnt != 1 && grow < p.B) {
+          const uint32_t qi = atomicAdd(&ms->fl_count, 1u);
+          ms->flist[qi] = (unsigned char)r;
+#pragma unroll
+          for (int w = 0; w < 8; ++w) ms->cmask[r][w] = q4 ? w1[w] : w0[w];
+        } else {
+          const int my_id = first > 255 ? 0 : first;
+          ids8[l * TX_R + r] = (unsigned char)my_id;
+          if (grow < p.B) p.ids[(int64_t)grow * L + l] = my_id;
+        }
+      }
+      tx_wg_sync();                                         // the re-rank queue of the tile is complete
+
+      // ---- exact re-rank of the queued rows, any warp takes the next one (same arithmetic as rq_simt.cu: sequential fp32
+      // residual, (xx + cc) - 2 dot, candidates in ascending index order with a strict '<': first index wins ties).
+      // Lane covers elements 128 i + 4 lane .. +3 of a row (6 x LDG.128 per row).
+      {
+        const float* ccl = p.cc + l * TC_K;
+        const float* cl = p.cbf + (size_t)l * TC_K * D;
+        const uint32_t nfl = *reinterpret_cast<volatile uint32_t*>(&ms->fl_count);
+        int n_rows = 0, n_cand = 0, n_many = 0;
+        auto ld_row = [&](const float* base, float4 (&v)[6]) {
+#pragma unroll
+          for (int i = 0; i < 6; ++i)
+            v[i] = (i * 128 + lane4 < D) ? __ldg(reinterpret_cast<const float4*>(base + i * 128 + lane4)) : make_float4(0.f, 0.f, 0.f, 0.f);
         };
-        if (l == 0) scan(std::integral_constant<int, 0>{});
-        else if (l == 1) scan(std::integral_constant<int, 1>{});
-        else if (l == 2) scan(std::integral_constant<int, 2>{});
-        else scan(std::integral_constant<int, 3>{});
-        if (q == 0) TC_EV(ev_role, 2, it * 16 + l);
-        // accumulator buffer free: one arrive per warp on the leader's barrier
-        // and the (min, mask) rows delivered: locally by the plain stores above, to the peer by ONE bulk copy through DSMEM
-        // (per-row st.async packets ran at ~16 cycles each per SM: 12 K cycles per level, profiles/r2_tcx_bringup.txt)
-        tc_fence_before();
-        if (!own) fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) {
-          tx_arrive_remote(tempty_leader + buf * 8u);
-          if (own) mbar_arrive(&ms->x_full[xb]);
-          else {
-            tx_arrive_expect_tx_remote(xfull_dst, TX_R * 8u);
-            tx_bulk_s2peer(exch_peer0 + xb * (8u * TX_R * 8u), &ms->xstage[xb][q][0], TX_R * 8u, xfull_dst);
-          }
-        }
-        // ---- finalise this CTA's rows: warp e owns rows [12e, 12e + 12), one per lane
-        TX_PH(0);
-        tx_wait(&ms->x_full[xb], xph);
-        TX_PH(1);
-        if (q == 0) TC_EV(ev_role, 3, it * 16 + l);
-        {
-          const int frow = e * TX_ROWS_PER_FIN + lane;                  // row of this CTA (lanes >= 12 idle here)
-          const int prow = (int)crank * TX_R + frow;
-          const int grow = (unit * 2 + (int)crank) * TX_R + frow;      // global row
-          if (lane < TX_ROWS_PER_FIN) {
-            const float mgf = tx_margin(lc, ms->rowinfo[it % TX_RIBUF][prow]);
-            uint32_t mw[8], kw[8];
-#pragma unroll
-            for (int w = 0; w < 8; ++w) {
-              const uint2 a = ms->exch[xb][w][frow];
-              mw[w] = a.x; kw[w] = a.y;
+#pragma unroll 1
+        while (true) {
+          uint32_t qi = 0;
+          if (lane == 0) qi = atomicAdd(&ms->fl_next, 1u);
+          qi = __shfl_sync(0xffffffffu, qi, 0);
+          if (qi >= nfl) break;
+          const int rrow = ms->flist[qi];
+          const int rgrow = row0 + rrow;
+          const uint32_t word = ms->cmask[rrow][lane & 7];     // lane w < 8 holds candidate word w
+          // first two candidates (ascending code order): their rows, the x row and the first prior code are ALL requested
+          // before anything is consumed -- one or two L2 round trips instead of four dependent ones
+          uint32_t wcur = 0, mwd = 0;
+          int w = 0;
+          auto next_cand = [&]() -> int {                     // -1 when the candidate words are exhausted
+            while (mwd == 0u) {
+              if (w >= 8) return -1;
+              mwd = __shfl_sync(0xffffffffu, word, w);
+              wcur = (uint32_t)w * 32u;
+              ++w;
             }
-            float M = __uint_as_float(mw[0]);
-#pragma unroll
-            for (int w = 1; w < 8; ++w) M = fminf(M, __uint_as_float(mw[w]));
-            const float thr = M + mgf;
-            int cnt = 0, first = -1;
-#pragma unroll
-            for (int w = 7; w >= 0; --w) {                              // branch-free: 8 lanes walk this in lock step
-              const uint32_t k = (!(__uint_as_float(mw[w]) > thr)) ? kw[w] : 0u;    // a warp whose minimum is outside the margin holds no candidate
-              cnt += __popc(k);
-              first = k ? w * 32 + __ffs(k) - 1 : first;
-            }
-            const int my_id = first < 0 ? 0 : first;
-            if ((cnt != 1) && grow < p.B) ms->flist[atomicAdd(&ms->fl_count, 1u)] = (unsigned char)frow;
-            else {
-              ids8[l * TX_PR + prow] = (unsigned char)my_id;
-              if (grow < p.B) p.ids[(int64_t)grow * L + l] = my_id;
-            }
-          }
-        }
-        tx_epi_sync();                                                  // the re-rank queue of this CTA is complete
-        TX_PH(2);
-        // ---- exact re-rank of the queued rows, any warp takes the next one (same arithmetic as rq_simt.cu: sequential fp32
-        // residual, (xx + cc) - 2 dot, candidates in ascending index order with a strict '<': first index wins ties).
-        // Lane covers elements 128 i + 4 lane .. +3 of a row (6 x LDG.128 per row).
-        {
-          const float* ccl = p.cc + l * TC_K;
-          const float* cl = p.cbf + (size_t)l * TC_K * D;
-          const uint32_t nfl = *reinterpret_cast<volatile uint32_t*>(&ms->fl_count);
-          int n_rows = 0, n_cand = 0, n_many = 0;
-          auto ld_row = [&](const float* base, float4 (&v)[6]) {
-#pragma unroll
-            for (int i = 0; i < 6; ++i)
-              v[i] = (i * 128 + lane4 < D) ? __ldg(reinterpret_cast<const float4*>(base + i * 128 + lane4)) : make_float4(0.f, 0.f, 0.f, 0.f);
+            const int k = (int)wcur + __ffs(mwd) - 1;
+            mwd &= mwd - 1;
+            return k;
           };
+          int ka = next_cand(), kb = next_cand();
+          float4 res[6], va[6], vb[6];
+          ld_row(p.x + (int64_t)rgrow * p.ldx, res);
+          if (l > 0) ld_row(p.cbf + (size_t)ids8[rrow] * D, vb);          // first prior code travels in vb
+          if (ka >= 0) ld_row(cl + (size_t)ka * D, va);
 #pragma unroll 1
-          while (true) {
-            uint32_t qi = 0;
-            if (lane == 0) qi = atomicAdd(&ms->fl_next, 1u);
-            qi = __shfl_sync(0xffffffffu, qi, 0);
-            if (qi >= nfl) break;
-            const int rrow = ms->flist[qi];                             // row of this CTA
-            const int rprow = (int)crank * TX_R + rrow;
-            const int rgrow = (unit * 2 + (int)crank) * TX_R + rrow;
-            // candidate words of the row (lane w < 8 holds word w); a warp whose minimum is outside the margin contributes nothing
-            const float mgf = tx_margin(lc, ms->rowinfo[it % TX_RIBUF][rprow]);
-            const uint2 ex = ms->exch[xb][lane & 7][rrow];
-            float M = __uint_as_float(ex.x);
+          for (int j = 0; j < l; ++j) {
 #pragma unroll
-            for (int o = 4; o > 0; o >>= 1) M = fminf(M, __shfl_xor_sync(0xffffffffu, M, o));
-            const uint32_t word = (!(__uint_as_float(ex.x) > M + mgf)) ? ex.y : 0u;
-            // first two candidates (ascending code order): their rows, the x row and the first prior code are ALL requested
-            // before anything is consumed -- one or two L2 round trips instead of four dependent ones (the re-rank sits on the level's
-            // critical path: every warp of both CTAs waits for the slowest queue entry)
-            uint32_t wcur = 0, mwd = 0;
-            int w = 0;
-            auto next_cand = [&]() -> int {                              // -1 when the candidate words are exhausted
-              while (mwd == 0u) {
-                if (w >= 8) return -1;
-                mwd = __shfl_sync(0xffffffffu, word, w);
-                wcur = (uint32_t)w * 32u;
-                ++w;
-              }
-              const int k = (int)wcur + __ffs(mwd) - 1;
-              mwd &= mwd - 1;
-              return k;
-            };
-            int ka = next_cand(), kb = next_cand();
-            float4 res[6], va[6], vb[6];                                 // three row buffers: a fourth one spills (no L1: a spill is an L2 trip)
-            ld_row(p.x + (int64_t)rgrow * p.ldx, res);
-            if (l > 0) ld_row(p.cbf + ((size_t)0 * TC_K + (size_t)ids8[rprow]) * D, vb);     // first prior code travels in vb
-            if (ka >= 0) ld_row(cl + (size_t)ka * D, va);
+            for (int i = 0; i < 6; ++i) { res[i].x -= vb[i].x; res[i].y -= vb[i].y; res[i].z -= vb[i].z; res[i].w -= vb[i].w; }   // rqvae.py:130, level order
+            if (j + 1 < l) ld_row(p.cbf + ((size_t)(j + 1) * TC_K + (size_t)ids8[(j + 1) * TX_R + rrow]) * D, vb);
+          }
+          if (kb >= 0) ld_row(cl + (size_t)kb * D, vb);
+          float cca = (ka >= 0) ? __ldg(ccl + ka) : 0.f, ccb = (kb >= 0) ? __ldg(ccl + kb) : 0.f;
+          float best = INFINITY;
+          int besti = 0x7fffffff, nc = 0;
+          const int firsti = ka;
+          float xx = 0.f;
+          bool have_xx = false;
 #pragma unroll 1
-            for (int j = 0; j < l; ++j) {
+          while (ka >= 0) {
+            // per-lane partial sums in the exact kernel's order, then ONE butterfly for all of them
+            float da = 0.f, db = 0.f, xp = 0.f;
 #pragma unroll
-              for (int i = 0; i < 6; ++i) { res[i].x -= vb[i].x; res[i].y -= vb[i].y; res[i].z -= vb[i].z; res[i].w -= vb[i].w; }   // rqvae.py:130, level order
-              if (j + 1 < l) ld_row(p.cbf + ((size_t)(j + 1) * TC_K + (size_t)ids8[(j + 1) * TX_PR + rprow]) * D, vb);
+            for (int i = 0; i < 6; ++i) da = tc_dot4(res[i], va[i], da);
+            if (kb >= 0) {
+#pragma unroll
+              for (int i = 0; i < 6; ++i) db = tc_dot4(res[i], vb[i], db);
             }
-            if (kb >= 0) ld_row(cl + (size_t)kb * D, vb);                // level 0: requested together with x and the first candidate
-            float cca = (ka >= 0) ? __ldg(ccl + ka) : 0.f, ccb = (kb >= 0) ? __ldg(ccl + kb) : 0.f;   // in flight with the rows
-            float best = INFINITY;
-            int besti = 0x7fffffff, nc = 0;
-            const int firsti = ka;
-            float xx = 0.f;
-            bool have_xx = false;
-#pragma unroll 1
-            while (ka >= 0) {
-              // per-lane partial sums in the exact kernel's order, then ONE butterfly for all of them (three dependent
-              // warp reductions in a row cost ~450 cycles of shuffle latency)
-              float da = 0.f, db = 0.f, xp = 0.f;
+            if (!have_xx) {
 #pragma unroll
-              for (int i = 0; i < 6; ++i) da = tc_dot4(res[i], va[i], da);
-              if (kb >= 0) {
+              for (int i = 0; i < 6; ++i) xp = tc_dot4(res[i], res[i], xp);
+            }
 #pragma unroll
-                for (int i = 0; i < 6; ++i) db = tc_dot4(res[i], vb[i], db);
-              }
-              if (!have_xx) {
-#pragma unroll
-                for (int i = 0; i < 6; ++i) xp = tc_dot4(res[i], res[i], xp);
-              }
-#pragma unroll
-              for (int o = 16; o > 0; o >>= 1) {
-                da += __shfl_xor_sync(0xffffffffu, da, o);
-                db += __shfl_xor_sync(0xffffffffu, db, o);
-                xp += __shfl_xor_sync(0xffffffffu, xp, o);
-              }
-              if (!have_xx) { xx = xp; have_xx = true; }
-              const float dist_a = (xx + cca) - 2.f * da;                 // quantize.py:113-117
-              if (dist_a < best) { best = dist_a; besti = ka; }
+            for (int o = 16; o > 0; o >>= 1) {
+              da += __shfl_xor_sync(0xffffffffu, da, o);
+              db += __shfl_xor_sync(0xffffffffu, db, o);
+              xp += __shfl_xor_sync(0xffffffffu, xp, o);
+            }
+            if (!have_xx) { xx = xp; have_xx = true; }
+            const float dist_a = (xx + cca) - 2.f * da;       // quantize.py:113-117
+            if (dist_a < best) { best = dist_a; besti = ka; }
+            ++nc;
+            if (kb >= 0) {
+              const float dist_b = (xx + ccb) - 2.f * db;
+              if (dist_b < best) { best = dist_b; besti = kb; }
               ++nc;
-              if (kb >= 0) {
-                const float dist_b = (xx + ccb) - 2.f * db;
-                if (dist_b < best) { best = dist_b; besti = kb; }
-                ++nc;
-              }
-              ka = (kb >= 0) ? next_cand() : -1;
-              kb = (ka >= 0) ? next_cand() : -1;
-              if (ka >= 0) { ld_row(cl + (size_t)ka * D, va); cca = __ldg(ccl + ka); }
-              if (kb >= 0) { ld_row(cl + (size_t)kb * D, vb); ccb = __ldg(ccl + kb); }
             }
-            if (besti > 255) besti = firsti < 0 ? 0 : firsti;          // all-NaN distances: keep a valid code
-            if (lane == 0) {
-              ids8[l * TX_PR + rprow] = (unsigned char)besti;
-              p.ids[(int64_t)rgrow * L + l] = besti;
-            }
-            ++n_rows; n_cand += nc; n_many += (nc >= 3);
+            ka = (kb >= 0) ? next_cand() : -1;
+            kb = (ka >= 0) ? next_cand() : -1;
+            if (ka >= 0) { ld_row(cl + (size_t)ka * D, va); cca = __ldg(ccl + ka); }
+            if (kb >= 0) { ld_row(cl + (size_t)kb * D, vb); ccb = __ldg(ccl + kb); }
           }
-          if (p.stats && lane == 0 && n_rows) {
-            atomicAdd(p.stats + 0, n_rows);
-            atomicAdd(p.stats + 1, n_cand);
-            atomicAdd(p.stats + 2, n_many);
-          }
-        }
-        if (q == 0) TC_EV(ev_role, 4, it * 16 + l);
-        TX_PH(3);
-        // ---- the level's ids of this CTA's rows are final in ids8[l][own rows] once all 8 warps are here: one warp ships the
-        // TX_R bytes to the peer (bulk copy through DSMEM, counted on the peer's ids_ready) and announces the TX_R bytes the
-        // peer ships to us; every warp arrives locally.
-        fence_proxy_async();                  // the byte stores above -> visible to the bulk copy (async proxy)
-        __syncwarp();
-        if (lane == 0 && !designated) mbar_arrive(&ms->ids_ready);
-        tx_epi_sync();                        // every local warp has left the re-rank loop and stored its ids
-        TX_PH(4);
-        if (designated && lane == 0) {
-          // the queue is idle until x_full of the NEXT step completes, which needs this warp's own delivery (it scans this
-          // CTA's rows: ch == crank) -- after this reset in program order
-          ms->fl_count = 0; ms->fl_next = 0;
-          fence_proxy_async();
-          tx_bulk_s2peer(ids_peer + (uint32_t)(l * TX_PR) + crank * TX_R, ids8 + l * TX_PR + crank * TX_R, TX_R, idsrdy_peer);
-          mbar_expect_tx(&ms->ids_ready, TX_R);
-        }
-        if (l == L - 1) {
-          // every rowinfo[] read of this warp for the tile is done (both CTAs count: the peer's converter writes into ours)
-          __threadfence_block();
-          __syncwarp();
+          if (besti > 255) besti = firsti < 0 ? 0 : firsti;   // all-NaN distances: keep a valid code
           if (lane == 0) {
-            tx_red_add_cluster(cluster_map(smem_u32(&ms->tiles_done), 0), 1u);
-            tx_red_add_cluster(cluster_map(smem_u32(&ms->tiles_done), 1), 1u);
+            ids8[l * TX_R + rrow] = (unsigned char)besti;
+            p.ids[(int64_t)rgrow * L + l] = besti;
           }
+          ++n_rows; n_cand += nc; n_many += (nc >= 3);
+        }
+        if (p.stats && lane == 0 && n_rows) {
+          atomicAdd(p.stats + 0, n_rows);
+          atomicAdd(p.stats + 1, n_cand);
+          atomicAdd(p.stats + 2, n_many);
         }
       }
+      tx_wg_sync();                                         // every id of the level is in ids8[]; the queue is drained
+      if (tid == 0) { ms->fl_count = 0; ms->fl_next = 0; }
+      tx_wg_sync();
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                // neither CTA may exit (or free TMEM) while the other can still reach into it
-  if (warp == 1) {
-    tc_fence_after();
-    tc_dealloc2(TX_TMEM_BASE(), 512);
-  }
-}
-
-template <bool kTrace>
-static int tx_launch(const TxParams& p, int grid, size_t smem, cudaStream_t st) {
-  auto kern = rq_tcx_kernel<kTrace>;
-  RQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)grid);
-  cfg.blockDim = dim3(TC_THREADS);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 1;
-  RQB_CUDA(cudaLaunchKernelEx(&cfg, kern, p));
-  RQB_LAUNCH_CHECK();
-  return RQB_OK;
 }
 
 int tcx_run(const float* x, int64_t ldx, int B, const void* state, int D, int L, int64_t* ids, int* stats, int sm_count,
-            bool trace, cudaStream_t st) {
+            cudaStream_t st) {
   const char* base = reinterpret_cast<const char*>(state);
   TxParams p{};
   p.x = x; p.ldx = ldx; p.B = B; p.D = D; p.L = L; p.nkc = D / TC_KC;
-  p.ntiles = (B + TX_PR - 1) / TX_PR;
+  p.ntiles = (B + TX_R - 1) / TX_R;
   p.hdr = reinterpret_cast<const TcHeader*>(base);
   p.cc = reinterpret_cast<const float*>(base + tc_off_cc(L));
   p.hcc = reinterpret_cast<const float*>(base + tc_off_hcc(L));
   p.gram = reinterpret_cast<const float*>(base + tc_off_gram(L));
   p.cbf = reinterpret_cast<const float*>(base + tc_off_cbf(L));
+  p.blob = reinterpret_cast<const unsigned char*>(base + tc_off_blob(D, L));
   p.ids = ids; p.stats = stats;
-  static const int opt_pf = []() { const char* e = getenv("RQB200_TC_PREFETCH"); return (e && e[0] == '1') ? 1 : 0; }();
-  p.prefetch = opt_pf;     // measured slower on B200 with the staging ring (0.178 vs 0.166 ms): opt-in
-  // the blob is a sequence of 16 KB shared-memory images: 16 box rows of 1 KB each (128 rows of 128 bytes cost the TMA engine
-  // ~1 K cycles per block: it is paced per row)
-  int rc = tc_encode_2d(&p.tmapB, CU_TENSOR_MAP_DATA_TYPE_UINT32, base + tc_off_blob(D, L), 256, (uint64_t)L * 2 * p.nkc * 16, 1024, 256, 16);
-  if (rc) return rc;
-  rc = tc_encode_2d(&p.tmapX, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, x, (uint64_t)D, (uint64_t)B, (uint64_t)ldx * 4, TX_XBOX_COLS, TX_XBOX_ROWS);
-  if (rc) return rc;
-  const int nclusters = p.ntiles < sm_count / 2 ? p.ntiles : sm_count / 2;
-  // shared memory: image + codebook ring + staging ring + fixed part + id bytes of L levels; the ring gets as many 16 KB stages
-  // (<= TX_NB_MAX) as fit under the 227 KB limit
-  const size_t fixed = (size_t)TC_MAX_KC * TX_SLOT_BYTES + TX_NX * TX_XBOX_BYTES + sizeof(TxSmem) + (size_t)rqb_round_up((int64_t)L * TX_PR, 16);
+  // shared memory: x image + codebook ring + fixed part + id bytes of L levels; the ring gets as many 32 KB stages
+  // (<= TX_NB_MAX) as fit under the 227 KB limit (2 at D = 768 with 8 levels, 4 with 3 levels)
+  const size_t fixed = (size_t)p.nkc * TX_SLOT_BYTES + sizeof(TxSmem) + (size_t)L * TX_R;
   int nbs = TX_NB_MAX;
-  while (nbs > 2 && fixed + (size_t)nbs * TC_BSTAGE_BYTES > 232448) --nbs;
+  while (nbs > 2 && fixed + (size_t)nbs * TX_STAGE_BYTES > TX_SMEM_LIMIT) --nbs;
   p.nb = nbs;
-  const size_t smem = fixed + (size_t)nbs * TC_BSTAGE_BYTES;
-  return trace ? tx_launch<true>(p, 2 * nclusters, smem, st) : tx_launch<false>(p, 2 * nclusters, smem, st);
+  const size_t smem = fixed + (size_t)nbs * TX_STAGE_BYTES;
+  RQB_CUDA(cudaFuncSetAttribute(rq_tcx_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int grid = p.ntiles < sm_count ? p.ntiles : sm_count;
+  rq_tcx_kernel<<<grid, TX_THREADS, smem, st>>>(p);
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
 }

@@ -107,7 +107,7 @@ extern "C" int rqb200_sid_dedup_rank(const int64_t* ids, int N, int L, int K, in
   int* next = head + keys;
   RQB_CUDA(cudaMemsetAsync(head, 0xFF, (size_t)keys * sizeof(int), st));     // -1 = empty list
   int grid = (N + 255) / 256;
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > 132 * 8) grid = 132 * 8;
   sid_link_kernel<<<grid, 256, 0, st>>>(ids, N, L, K, head, next);
   RQB_LAUNCH_CHECK();
   sid_rank_kernel<<<grid, 256, 0, st>>>(ids, N, L, K, head, next, rank, stats, entropy);
@@ -142,7 +142,7 @@ extern "C" int rqb200_sid_gather(const int64_t* cached_ids, int64_t n_corpus, in
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int64_t total = (int64_t)B * S * C;
   int grid = (int)((total + 255) / 256);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > 132 * 8) grid = 132 * 8;
   sid_gather_kernel<<<grid, 256, 0, st>>>(cached_ids, C, item_ids, item_stride, seq_mask, mask_stride, B, S, out, token_type);
   RQB_LAUNCH_CHECK();
   return RQB_OK;
@@ -240,7 +240,7 @@ extern "C" int rqb200_sid_prefix_build(const int64_t* cached_ids, int64_t N, int
   SidPrefixOffsets o{};
   sid_prefix_offsets(C, K, o);
   int grid = (int)((N + 255) / 256);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > 132 * 8) grid = 132 * 8;
   sid_prefix_build_kernel<<<grid, 256, 0, st>>>(cached_ids, N, C, K, reinterpret_cast<unsigned int*>(workspace), o);
   RQB_LAUNCH_CHECK();
   return RQB_OK;
@@ -257,7 +257,7 @@ extern "C" int rqb200_sid_prefix_check(const int64_t* prefix, int64_t row_stride
     return RQB_ERR_UNSUPPORTED;
   }
   int grid = (int)((P + 255) / 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > 132 * 16) grid = 132 * 16;
   sid_prefix_check_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       prefix, row_stride, P, l, K, reinterpret_cast<const unsigned int*>(reinterpret_cast<const char*>(workspace) + o.off[l]), valid);
   RQB_LAUNCH_CHECK();

@@ -1,9 +1,8 @@
-// Shared definitions of the tensor-core tokeniser kernels (csrc/rq_tc.cu, csrc/rq_tcx.cu): prepared-state layout, kernel
-// parameters, tcgen05 / TMA PTX wrappers.
+// Shared definitions of the tensor-core tokeniser (csrc/rq_tc.cu, csrc/rq_tcx.cu): prepared-state layout, filter bound,
+// small device helpers.
 // Everything here is static / inline; the result contract is stated at the top of rq_tc.cu.
 #pragma once
 #include "common.cuh"
-#include <cuda.h>        // CUtensorMap (the CTA-pair variants load codebook blocks / x tiles with tensor-map TMA)
 #include <cuda_fp16.h>
 #include <cmath>
 #include <cstdlib>
@@ -13,10 +12,7 @@
 #define TC_MAX_D 768
 #define TC_MAX_KC (TC_MAX_D / TC_KC)
 #define TC_BSTAGE_BYTES (128 * TC_KC * 2)   // 128 codes x 64 k x fp16 = 16 KB
-#define TC_NCONV_WARPS 4
-#define TC_NEPI_WARPS 8
-#define TC_THREADS ((4 + TC_NCONV_WARPS + TC_NEPI_WARPS) * 32)   // warpgroups: {producer, MMA, 2 idle} | 4 converters | 8 epilogue (2 per TMEM lane quarter) = 512 threads
-// Filter error bound (DESIGN.md 5.2 "filter error bound", tests/tc_filter_model.py): DETERMINISTIC.  With x~ = fp16(x) and
+// Filter error bound: DETERMINISTIC.  With x~ = fp16(x) and
 // c~ = fp16(c 2^s) / 2^s,   x~.c~ - x.c = (x~ - x).c~ + x.(c~ - c)   exactly, hence by Cauchy-Schwarz
 //   |x~.c~_k - x.c_k| <= ||x~ - x|| ||c~_k|| + ||x|| ||c~_k - c_k||  <=  ex_b chat_l + xn_b ec_l
 // ex_b is MEASURED per row by the converter (subnormal flushes and overflow are inside it: an overflowing row gets
@@ -61,167 +57,12 @@ static size_t tc_off_cbptr(int L) { return tc_off_gram(L) + (size_t)(L * (L - 1)
 static size_t tc_off_cbf(int L) { return rqb_round_up(tc_off_cbptr(L) + RQB_MAX_LEVELS * 8, 256); }   // fp32 copy [L][256][D]
 static size_t tc_off_blob(int D, int L) { return rqb_round_up(tc_off_cbf(L) + (size_t)L * TC_K * D * 4, 1024); }
 
-// ------------------------------------------------------------------------------------------------ tcgen05 wrappers
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void tc_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tc_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, fp16 inputs, fp32 accumulate; issued by ONE thread
-__device__ __forceinline__ void tc_mma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// ---- CTA-pair (cta_group::2) forms, validated standalone by tools/pair_probe.cu.  Issued by the leader CTA (rank 0) only,
-// except alloc / dealloc which warp 1 of BOTH CTAs executes.
-__device__ __forceinline__ void tc_alloc2(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tc_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A * B^T with M = 256 (128 rows from each CTA's smem) and N = 256 (128 B rows from each CTA's smem)
-__device__ __forceinline__ void tc_mma_f16_2(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// completion of all prior tcgen05 ops of this thread -> the mbarrier at this offset in BOTH CTAs of the pair
-__device__ __forceinline__ void tc_commit2(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-// one box of a 2-D tensor map -> this CTA's shared memory, the bytes counted on an mbarrier that may live in the peer CTA
-__device__ __forceinline__ void tc_tma2d_pair(void* smem_dst, const CUtensorMap* tmap, int c0, int c1, uint32_t mbar_cluster_addr) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(mbar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-
-// one box of a 2-D tensor map -> this CTA's shared memory, bytes counted on a local mbarrier
-__device__ __forceinline__ void tc_tma2d(void* smem_dst, const CUtensorMap* tmap, int c0, int c1, uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-      : "memory");
-}
-// mbarrier arrives when all tcgen05 ops issued so far by this thread have completed
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// 32 consecutive fp32 columns of this thread's TMEM lane (row); asynchronous until tc_ld_wait()
-__device__ __forceinline__ void tc_ld32_issue(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tc_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, mma_sm100_desc.hpp):
-// start>>4 [0,14) | LBO>>4 [16,30) (=1, unused for swizzled K-major) | SBO>>4 [32,46) (=1024 B: 8 rows x 128 B)
-// | version=1 [46,48) | layout SWIZZLE_128B=2 [61,64)
-__device__ __forceinline__ uint64_t tc_smem_desc(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr >> 4) & 0x3FFF) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-// instruction descriptor (cute::UMMA::InstrDescriptor): D=f32 [4,6)=1, A=B=f16 (0), both K-major, N>>3 [17,23), M>>4 [24,29)
-__host__ __device__ constexpr uint32_t tc_idesc(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// event timeline of CTA 0 (RQB200_TC_TRACE=1 and stats[4] != 0; the caller passes >= 4096 ints): role r appends
-// (tag << 56 | payload << 48 | clock) records at ((long long*)(stats + 128))[r * 256 ...]; tools/tc_native_check.cu prints them
-#define TC_EV_DECL() int ev_n = 0; const bool ev_on = trace && blockIdx.x == 0 && p.stats[4] != 0
-#define TC_EV(role, tag, payload) do { if (ev_on && (threadIdx.x & 31) == 0 && ev_n < 256) { \
-    reinterpret_cast<long long*>(p.stats + 128)[(role) * 256 + ev_n++] = \
-        ((long long)(tag) << 56) | ((long long)((payload) & 0xff) << 48) | (clock64() & 0xffffffffffffLL); } } while (0)
-template <int N> __device__ __forceinline__ void tc_setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
-template <int N> __device__ __forceinline__ void tc_setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 __device__ __forceinline__ uint32_t tc_bf16_up(float v) {   // bf16 bits of the smallest bf16 >= v (v >= 0, inf/nan kept)
   uint32_t b = __float_as_uint(v);
   if ((b & 0x7f800000u) != 0x7f800000u && (b & 0xffffu)) b += 0x10000u;
   return b >> 16;
 }
 
-// 16 consecutive fp32 columns of this thread's TMEM lane (row); asynchronous until tc_ld_wait()
-__device__ __forceinline__ void tc_ld16_issue(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-
-// one lane of a fully active warp (CUTLASS elect_one_sync idiom).  The producer and MMA warps run their schedules with ALL
-// lanes (warp-uniform control flow) and only issue under this predicate: ptxas then keeps descriptors, addresses and loop
-// state in uniform registers.  Issuing from `if (lane == 0)` divergent code instead cost ~25 instructions (ELECT / PLOP3 /
-// R2UR chains) and ~140 cycles per tcgen05.mma -- more than twice the 64 cycles the tensor core needs to execute it.
-__device__ __forceinline__ bool tc_elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
-
 __device__ __forceinline__ float tc_dot4(const float4& a, const float4& b, float acc) {
   return fmaf(a.x, b.x, fmaf(a.y, b.y, fmaf(a.z, b.z, fmaf(a.w, b.w, acc))));
-}
-
-// cuTensorMapEncodeTiled through the runtime (no link-time dependency on libcuda): a row-major 2-D tensor, no swizzle,
-// out-of-bounds elements read as zero
-typedef CUresult (*TcEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static inline int tc_encode_2d(CUtensorMap* tm, CUtensorMapDataType dt, const void* base, uint64_t dim0, uint64_t dim1,
-                               uint64_t stride1_bytes, uint32_t box0, uint32_t box1) {
-  static TcEncodeFn fn = nullptr;
-  if (!fn) {
-    void* f = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    RQB_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q));
-    if (!f || q != cudaDriverEntryPointSuccess) {
-      rqb_set_error("tokenize_tc: cuTensorMapEncodeTiled is not available from this driver");
-      return RQB_ERR_UNSUPPORTED;
-    }
-    fn = reinterpret_cast<TcEncodeFn>(f);
-  }
-  const cuuint64_t gdim[2] = {dim0, dim1};
-  const cuuint64_t gstr[1] = {stride1_bytes};
-  const cuuint32_t box[2] = {box0, box1};
-  const cuuint32_t estr[2] = {1, 1};
-  const CUresult r = fn(tm, dt, 2, const_cast<void*>(base), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    rqb_set_error("tokenize_tc: cuTensorMapEncodeTiled failed (%d)", (int)r);
-    return RQB_ERR_CUDA;
-  }
-  return RQB_OK;
 }

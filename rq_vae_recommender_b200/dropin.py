@@ -1,4 +1,4 @@
-"""Make the UNMODIFIED reference scripts run on the B200 modules.
+"""Make the UNMODIFIED reference scripts run on the H100 modules.
 
     import rq_vae_recommender_b200.dropin as dropin
     dropin.install(reference_root="/path/to/RQ-VAE-Recommender")   # before `import train_rqvae`
@@ -7,7 +7,7 @@
 ``install`` pre-seeds ``sys.modules`` so that every ``from modules.quantize import ...`` / ``from init.kmeans import
 ...`` inside the reference (train_rqvae.py:13-15, modules/tokenizer/semids.py:10, train_decoder.py:13-20) resolves to
 the replacement modules of this package; everything else (data/, modules/model.py, evaluate/, the scripts) is imported
-from the reference tree untouched.  Checkpoints pickle ``modules.quantize.Quantize`` etc. by module path (SURVEY 5.4),
+from the reference tree untouched.  Checkpoints pickle ``modules.quantize.Quantize`` etc. by module path,
 so ``torch.load(..., weights_only=False)`` of the shipped files also lands on the replacement classes.
 gin-config is not in this image: a small compatible shim is registered as ``gin`` when the real one is missing.
 """

@@ -6,7 +6,7 @@ a second one writes the means.  RNG draws stay on the host in the reference's or
 (kmeans.py:35), ``torch.randint`` once per empty cluster in cluster order (kmeans.py:53).
 
 ``group``: when a torch.distributed process group is given, ``x`` is this rank's shard of the rows and the
-sums/counts are all-reduced every iteration (SURVEY 8e); see parallel.py for the driver."""
+sums/counts are all-reduced every iteration; see parallel.py for the driver."""
 from typing import NamedTuple, Optional
 
 import numpy as np

@@ -34,9 +34,9 @@ class MLP(nn.Module):
         self.mlp.append(L2NormalizationLayer() if normalize else nn.Identity())
 
     # ---- default precision: fp32-accurate.  From ops.SPLIT_MIN_ROWS rows on every Linear (forward and dgrad) runs on the fp16
-    # tensor cores as a split-precision GEMM (three tcgen05 products per k-step, as close to float64 as a plain fp32 GEMM:
+    # tensor cores as a split-precision GEMM (three wgmma products per k-step, as close to float64 as a plain fp32 GEMM:
     # csrc/gemm_tc.cu gs_gemm_kernel, tests/test_gpu_gemm_split.py); smaller batches use the CUDA-core SGEMM.
-    # ---- reduced-precision path: bf16 tcgen05 GEMMs (gt_gemm_kernel).  Opt-in and forward-only: chosen when no
+    # ---- reduced-precision path: bf16 wgmma GEMMs (gt_gemm_kernel).  Opt-in and forward-only: chosen when no
     # gradient is needed AND (self.precision == "bf16" OR a bf16 torch.autocast region is active -- the reference runs
     # these Linears in bf16 under accelerator.autocast(), train_rqvae.py:36,69).
     precision = "fp32"

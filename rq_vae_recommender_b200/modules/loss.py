@@ -1,5 +1,5 @@
 """Loss modules of the reference (modules/loss.py) kept importable under the same names: shipped checkpoints
-pickle them (SURVEY 5.4).  The fused RQ kernels compute QuantizeLoss in their epilogue; these classes are the
+pickle them.  The fused RQ kernels compute QuantizeLoss in their epilogue; these classes are the
 stand-alone API (thin tensor expressions, same arithmetic as loss.py:9-10,19-30,38-41)."""
 from torch import nn
 from torch import Tensor

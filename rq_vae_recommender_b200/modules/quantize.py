@@ -1,4 +1,4 @@
-"""modules/quantize.py of the reference (:16-163) on the fused sm_100a kernels.
+"""modules/quantize.py of the reference (:16-163) on the fused sm_90a kernels.
 
 Same public names, constructor signature, state-dict keys (``embedding.weight``, ``out_proj.0.weight``) and
 forward contract ``Quantize.forward(x, temperature) -> QuantizeOutput(embeddings, ids, loss)``.
@@ -164,7 +164,7 @@ class Quantize(nn.Module):
         if self.distance_mode != QuantizeDistance.L2:
             if self.distance_mode == QuantizeDistance.COSINE:
                 raise NotImplementedError("QuantizeDistance.COSINE is never selected by a reference caller "
-                                          "(SURVEY 2 #1) and is not built")
+                                          " and is not built")
             raise Exception("Unsupported Quantize distance mode.")
 
         codebook = self.codebook()

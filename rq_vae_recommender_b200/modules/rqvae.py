@@ -1,4 +1,4 @@
-"""modules/rqvae.py of the reference (:37-175) on the fused sm_100a kernels.
+"""modules/rqvae.py of the reference (:37-175) on the fused sm_90a kernels.
 
 Same class / NamedTuple names, constructor signature, state-dict keys and HF-hub mixin, so the reference's
 train_rqvae.py, train_decoder.py and SemanticIdTokenizer use it unchanged.  What differs is underneath:
@@ -209,7 +209,7 @@ class RqVae(nn.Module, PyTorchModelHubMixin):
         """sem_ids [B,L] only: what SemanticIdTokenizer consumes (semids.py:125).  Large batches go through the tcgen05
         candidate filter + exact re-rank (prepared codebook state cached on the codebooks' identity and version; the shipped
         D = 32 quantiser is zero-padded to 64), small ones through the exact CUDA-core kernel: ops.rq_tokenize_auto.
-        ``mlp_precision="bf16"`` runs the encoder on the bf16 tcgen05 GEMMs (faster, NOT index-exact vs fp32)."""
+        ``mlp_precision="bf16"`` runs the encoder on the bf16 wgmma GEMMs (faster, NOT index-exact vs fp32)."""
         x = x.to(next(self.encoder.parameters()).dtype)
         if mlp_precision is not None:
             old, self.encoder.precision = self.encoder.precision, mlp_precision
@@ -227,7 +227,7 @@ class RqVae(nn.Module, PyTorchModelHubMixin):
         res = self.encode(xin)
         emb_sum, embs_norm, sem_ids, rqvae_loss = self._chain(res, gumbel_t, lean=True)
         x_hat = self.decode(emb_sum)
-        if self.n_cat_feats != 0:   # with n_cat_feats == 0 the reference's [:-0] slice is empty: no-op (SURVEY A.5)
+        if self.n_cat_feats != 0:   # with n_cat_feats == 0 the reference's [:-0] slice is empty: no-op
             x_hat = torch.cat(
                 [l2norm(x_hat[..., : -self.n_cat_feats]), x_hat[..., -self.n_cat_feats:]],
                 axis=-1,

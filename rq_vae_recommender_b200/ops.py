@@ -652,7 +652,7 @@ def tc_supported(D: int, K: int, L: int) -> bool:
     return bool(_lib.load().rqb200_tokenize_tc_supported(D, K, L))
 
 
-TC_PAD = 64   # the tcgen05 tokeniser wants D % 64 == 0: narrower / odd widths are zero-padded (exact for every dot product)
+TC_PAD = 64   # the wgmma tokeniser wants D % 64 == 0: narrower / odd widths are zero-padded (exact for every dot product)
 
 
 def tc_padded_dim(D: int, K: int, L: int) -> int:
@@ -663,7 +663,7 @@ def tc_padded_dim(D: int, K: int, L: int) -> int:
 
 
 class TcState:
-    """Device-side prepared codebooks for the tcgen05 tokeniser (fp16 images, measured rounding norms, float64 Gram
+    """Device-side prepared codebooks for the wgmma tokeniser (fp16 images, measured rounding norms, float64 Gram
     tables, an fp32 copy for the exact re-rank).  Owns everything it needs: the caller's tensors are not referenced after
     construction.  Codebooks narrower than a multiple of 64 are zero-padded (``self.D`` is the padded width,
     ``self.D_in`` the caller's)."""
@@ -676,7 +676,7 @@ class TcState:
         self.L = len(cbs)
         self.D = tc_padded_dim(self.D_in, self.K, self.L)
         if not self.D:
-            raise _lib.Rqb200Error(f"tcgen05 tokeniser does not support D={self.D_in} K={self.K} L={self.L}")
+            raise _lib.Rqb200Error(f"wgmma tokeniser does not support D={self.D_in} K={self.K} L={self.L}")
         if self.D != self.D_in:
             cbs = [torch.nn.functional.pad(c, (0, self.D - self.D_in)) for c in cbs]
         self.device = cbs[0].device
@@ -692,8 +692,8 @@ class TcState:
 
 
 def rq_tokenize_tc(x: torch.Tensor, codebooks=None, state: Optional[TcState] = None, stats=None) -> torch.Tensor:
-    """sem_ids [B,L] int64 via the tcgen05 candidate filter + exact fp32 re-rank (csrc/rq_tcx.cu).  Same result contract as
-    ``rq_tokenize``: the filter's margin is a deterministic bound on the fp16 rounding (DESIGN.md 5.2), every row with more
+    """sem_ids [B,L] int64 via the wgmma candidate filter + exact fp32 re-rank (csrc/rq_tcx.cu).  Same result contract as
+    ``rq_tokenize``: the filter's margin is a deterministic bound on the fp16 rounding, every row with more
     than one candidate inside it is re-scored with the exact kernel's fp32 arithmetic."""
     _need_cuda(x)
     lib = _lib.load()
@@ -725,7 +725,7 @@ def rq_tokenize_tc(x: torch.Tensor, codebooks=None, state: Optional[TcState] = N
 _TC_CACHE: "dict[tuple, tuple]" = {}
 _TC_CACHE_MAX = 4
 #: rows below which the exact CUDA-core kernel is used even when the tensor-core path is available (one 128-row tile keeps
-#: 2 of 148 SMs busy; the prepare step costs ~0.4 ms when the cache misses)
+#: 2 of 132 SMs busy; the prepare step runs again whenever the cache misses)
 TC_MIN_ROWS = 1024
 
 
@@ -784,7 +784,7 @@ def to_bf16_image(x: torch.Tensor) -> torch.Tensor:
 @torch.no_grad()
 def mlp_forward_bf16(x: torch.Tensor, weights: Sequence[torch.Tensor], normalize: bool = False,
                      weight_images: Optional[Sequence[torch.Tensor]] = None) -> torch.Tensor:
-    """modules/encoder.py:23-38 with bf16 tcgen05 GEMMs (fp32 accumulate, ReLU fused; activations stay in the bf16
+    """modules/encoder.py:23-38 with bf16 wgmma GEMMs (fp32 accumulate, ReLU fused; activations stay in the bf16
     operand-image layout between layers).  Forward only, reduced precision: NOT index-exact vs the fp32 reference."""
     _need_cuda(x, *weights)
     lib = _lib.load()

@@ -1,4 +1,4 @@
-"""Multi-GPU and host-facing drivers of the hot path (SURVEY 8e).
+"""Multi-GPU and host-facing drivers of the hot path.
 
 * ``CorpusTokenizer``: items -> semantic ids.  Rows are independent, so a corpus is cut into contiguous shards,
   one per rank, tokenised with no data-path collective, and only the [N/G, L] id blocks are all-gathered.
@@ -27,7 +27,7 @@ def shard_bounds(n: int, world: int, rank: int):
 
 
 class CorpusTokenizer:
-    """Frozen codebooks -> ids.  ``use_tc`` selects the tcgen05 filter + exact re-rank kernel (state prepared once; its margin is
+    """Frozen codebooks -> ids.  ``use_tc`` selects the wgmma filter + exact re-rank kernel (state prepared once; its margin is
     a deterministic bound, so the result contract is the exact kernel's).  Default: on whenever the shape allows it (K = 256,
     D <= 768; widths that are not a multiple of 64 are zero-padded)."""
 
@@ -118,28 +118,6 @@ class CorpusTokenizer:
         if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
             return ids_local
         return all_gather_rows(ids_local.to(torch.int32), n_total, group).to(torch.int64)
-
-    def measured_traffic_bytes(self):
-        """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel at the 65 536 x 768 bench shape,
-        from the committed `ncu --set full` capture of the shipped kernel (profiles/r2_tcx_ncu_summary.csv); None when no
-        capture covers the active kernel."""
-        import csv
-        import os
-        if not self.use_tc:
-            return None
-        path = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "profiles",
-                            "r2_tcx_ncu_summary.csv")
-        try:
-            rows = list(csv.reader(open(path)))
-            hdr, units, vals = rows[0], rows[1], rows[2]
-            scale = {"byte": 1, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-            tot = 0.0
-            for name in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-                i = hdr.index(name)
-                tot += float(vals[i]) * scale[units[i]]
-            return int(tot)
-        except Exception:
-            return None
 
 
 def all_gather_rows(block: torch.Tensor, n_total: int, group=None) -> torch.Tensor:

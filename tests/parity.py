@@ -1,4 +1,4 @@
-"""Parity protocol helpers shared by the CPU and GPU tests (SURVEY 8c)."""
+"""Parity protocol helpers shared by the CPU and GPU tests."""
 import os
 
 import numpy as np

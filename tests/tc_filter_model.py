@@ -2,11 +2,11 @@
 
 The kernel's exactness argument has two halves: the exact fp32 re-rank (same arithmetic as the CUDA-core kernel, tested
 against the oracle on the GPU) and the claim that the fp16 tensor-core scores never drop the true argmin from the candidate
-set {k : h[k] <= min h + 2 eps_b}.  The second half is a DETERMINISTIC bound (DESIGN.md 5.2 "filter error bound") and this
+set {k : h[k] <= min h + 2 eps_b}.  The second half is a DETERMINISTIC bound and this
 model restates it on the CPU with the kernel's own formulas, so the margin can be checked -- and changed -- without a GPU:
 
   x~ = fp16(x), c~ = fp16(c * 2^s) / 2^s        (tc_prep_blob_kernel, converter; the power-of-two scale is exact)
-  S  = x~ . c~                                  (tcgen05.mma, fp32 accumulation)
+  S  = x~ . c~                                  (wgmma, fp32 accumulation)
   h  = T[k] - S,  T = cc/2 + sum_j G_jl[id_j]   (Gram tables from float64, rounded once; epilogue)
   x~.c~ - x.c = (x~ - x).c~ + x.(c~ - c)   exactly, so by Cauchy-Schwarz
   |x~.c~ - x.c| <= ||x~ - x|| ||c~_k|| + ||x|| ||c~_k - c_k||  <=  ex_b chat_l + xn_b ec_l

@@ -1,8 +1,8 @@
 """CPU model of the split-precision tensor-core GEMM (csrc/gemm_tc.cu: gs_split_* / gs_gemm_kernel): the operand representation
 and the accumulation scheme restated in numpy, checked against float64.  It pins the two design claims of DESIGN.md 5.3 without a
 GPU: (1) hi + lo fp16 images of a power-of-two scaled row carry the operand to ~2^-22, so three products reproduce the fp32
-product; (2) with an fp32 accumulator that truncates after every MMA (the behaviour the B200 measurement matched), ONE accumulator
-loses ~3x more than hi.hi and the cross terms kept apart -- the reason the kernel spends 512 TMEM columns on two accumulators."""
+product; (2) with an fp32 accumulator that truncates after every MMA (the behaviour tensor-core measurements match), ONE accumulator
+loses ~3x more than hi.hi and the cross terms kept apart -- the reason the products are kept in short tensor-core sums (the kernel promotes every 64 k into an fp32 total)."""
 import numpy as np
 import pytest
 
@@ -28,7 +28,7 @@ def model_gemm(a, b, separate):
     bh, bl, sb = split_rows(b)
     main = np.zeros((a.shape[0], b.shape[0]))
     cross = np.zeros_like(main)
-    for k0 in range(0, a.shape[1], 16):                       # one tcgen05.mma = 16 k: products exact, accumulator truncated
+    for k0 in range(0, a.shape[1], 16):                       # one MMA = 16 k: products exact, accumulator truncated
         sl = slice(k0, k0 + 16)
         if separate:
             main = trunc24(main + ah[:, sl] @ bh[:, sl].T)
@@ -70,7 +70,7 @@ def test_three_products_match_float64_and_two_accumulators_pay(K):
     e_two = (np.abs(model_gemm(a, b, separate=True) - ref) / scale).max()
     e_one = (np.abs(model_gemm(a, b, separate=False) - ref) / scale).max()
     e_f32 = (np.abs((a @ b.T).astype(np.float64) - ref) / scale).max()
-    assert e_two <= 3e-7, e_two                               # the level of a plain fp32 GEMM (B200 measured 2.2e-7 at K = 768)
+    assert e_two <= 3e-7, e_two                               # the level of a plain fp32 GEMM
     assert e_two <= max(3.0 * e_f32, 2.5e-7)
     if K >= 256:
-        assert e_one >= 1.8 * e_two, (e_one, e_two)           # one shared accumulator: B200 measured 5.4e-7 at K = 768
+        assert e_one >= 1.8 * e_two, (e_one, e_two)           # one shared accumulator

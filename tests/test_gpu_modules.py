@@ -202,7 +202,7 @@ def test_tokenizer_corpus_pass_vs_reference():
 
 @pytest.mark.parametrize("D,hidden", [(768, ()), (64, (128,)), (32, (512, 256, 128))])
 def test_module_api_routes_to_the_tensor_core_tokeniser(D, hidden):
-    """VERDICT r1 item 3: SemanticIdTokenizer.precompute_corpus_ids -> RqVae.tokenize must run the tcgen05 tokeniser (prepared
+    """VERDICT r1 item 3: SemanticIdTokenizer.precompute_corpus_ids -> RqVae.tokenize must run the wgmma tokeniser (prepared
     state cached across batches) for K = 256 models -- D = 768, D = 64 and the shipped D = 32 (zero-padded to 64) -- and return
     the exact kernel's ids (modules/tokenizer/semids.py:76-125)."""
     from rq_vae_recommender_b200 import ops
@@ -292,7 +292,7 @@ def test_training_loop_like_train_rqvae():
 
 
 def test_mlp_bf16_path_is_opt_in_and_forward_only():
-    """precision="bf16" / bf16 autocast selects the tcgen05 GEMMs only when no gradient is needed; default stays exact."""
+    """precision="bf16" / bf16 autocast selects the wgmma GEMMs only when no gradient is needed; default stays exact."""
     from rq_vae_recommender_b200.modules.encoder import MLP
     torch.manual_seed(0)
     mlp = MLP(input_dim=768, hidden_dims=[512, 256, 128], out_dim=32).cuda()

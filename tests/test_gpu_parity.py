@@ -1,5 +1,5 @@
 """GPU parity tests proper: the CUDA path (through the C ABI) against the oracle on seeded inputs and against
-the committed reference-generated fixtures.  Run with `pytest -m gpu` on a B200."""
+the committed reference-generated fixtures.  Run with `pytest -m gpu` on an H100."""
 import numpy as np
 import pytest
 import torch
@@ -242,7 +242,9 @@ def test_mlp_vs_reference(ops):
         y = ops.MLPFunction.apply(xt, norm, *wts)
         (y * dev(gy)).sum().backward()
         assert rel_err(host(y), g[f"y_norm{int(norm)}"]) < TOL
-        assert rel_err(host(xt.grad), g[f"gx_norm{int(norm)}"]) < 2e-5
+        gx = host(xt.grad)                                   # the fixture stores the first rows and every row sum
+        assert rel_err(gx[:len(g[f"gx_norm{int(norm)}"])], g[f"gx_norm{int(norm)}"]) < 2e-5
+        assert rel_err(gx.astype(np.float64).sum(1), g[f"gx_rowsum_norm{int(norm)}"]) < 2e-5
         assert rel_err(host(wts[3].grad), g[f"gw3_norm{int(norm)}"]) < 2e-5
         assert rel_err(host(wts[0].grad).astype(np.float64).sum(1), g[f"gw0_rowsum_norm{int(norm)}"]) < 2e-5
     assert rel_err(host(ops.l2norm_rows(dev(I.randn(503, 256, 40)))), g["l2norm"]) < TOL
@@ -279,7 +281,7 @@ def test_sid_histogram(ops):
 @pytest.mark.parametrize("M,dims", [(1, [64, 64]), (130, [128, 64, 32]), (1000, [768, 512, 256, 128, 32]),
                                      (257, [192, 320, 70])])
 def test_gemm_bf16_mlp_vs_bf16_oracle(ops, M, dims):
-    """tcgen05 bf16 GEMM chain vs the oracle's bf16-rounding emulation of the reference under autocast."""
+    """wgmma bf16 GEMM chain vs the oracle's bf16-rounding emulation of the reference under autocast."""
     x = I.randn(40, M, dims[0]) * 0.3
     ws = I.mlp_weights(41, dims)
     dws = [dev(w) for w in ws]
@@ -296,7 +298,7 @@ def test_gemm_bf16_mlp_vs_bf16_oracle(ops, M, dims):
         assert rel_err(yk, expect) < 1e-5, (k, rel_err(yk, expect))
         prev = yk
     # (2) END TO END against the pure oracle chain.  Here a few intermediate activations legitimately round the other
-    #     way (fp32-in-TMEM vs float64 accumulation on opposite sides of a bf16 boundary, 1 ulp = 0.4 %); measured on
+    #     way (fp32 tensor-core accumulation vs float64 accumulation on opposite sides of a bf16 boundary, 1 ulp = 0.4 %); measured on
     #     the 4-layer shipped architecture: most outputs bit-identical, ~1/4 of rows touched at a few 1e-4, max 2.6e-3.
     #     (1) above is the correctness proof; this bounds the bulk tightly and the tail by a few bf16 ulps.
     for norm in (False, True):

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 tokeniser (fp16 candidate filter + exact fp32 re-rank) against the oracle, the
+"""GPU parity of the wgmma tokeniser (fp16 candidate filter + exact fp32 re-rank) against the oracle, the
 reference-generated fixtures and the exact CUDA-core kernel.  `pytest -m gpu`."""
 import numpy as np
 import pytest

@@ -123,7 +123,7 @@ def test_beauty_checkpoint_codebooks():
     assert n_tie <= 4
     assert rel_err(so.quantize_loss[same], g["qloss"][same]) < TOL
     assert rel_err(np.sqrt((so.embeddings ** 2).sum(1))[same], g["embs_norm"][same]) < TOL
-    # a non-degenerate argmin workload (SURVEY 8c): most codes of every level are live
+    # a non-degenerate argmin workload: most codes of every level are live
     assert all(len(np.unique(g["sem_ids"][:, l])) > 150 for l in range(3))
 
 
