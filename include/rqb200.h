@@ -72,7 +72,9 @@ int rqb200_rq_backward(int mode, const float* x, int64_t ldx, const float* const
 
 /* ---- tensor-core tokeniser (wgmma candidate filter + exact fp32 re-rank), see csrc/rq_tc.cu --------
  * Same result contract as rqb200_rq_forward(mode=EVAL, ids only).  `prepare` converts the codebooks once
- * (fp16 copies, norms, inter-level Gram tables) into `state`; `run` consumes x [B,D] fp32. */
+ * (fp16 copies, norms, inter-level Gram tables) into `state`; `run` consumes x [B,D] fp32.
+ * Supported: K = 256 m with 1 <= m <= 8 (256 ... 2048 codes), D a multiple of 64 in 64..768, 1 <= L <= 8.
+ * state_bytes grows as K^2 L(L-1)/2 (the Gram tables): ~80 MB at K = 2048, L = 3, D = 768; ~0.55 GB at L = 8. */
 size_t rqb200_tokenize_tc_state_bytes(int D, int K, int L);
 int rqb200_tokenize_tc_supported(int D, int K, int L);
 int rqb200_tokenize_tc_prepare(const float* const* codebooks, int D, int K, int L, void* state, size_t state_bytes,

@@ -12,26 +12,32 @@
 //   |candidates| == 1  -> that code is the exact argmin;  else the candidates are re-scored with the exact fp32
 //   arithmetic of the CUDA-core kernel (sequential fp32 residual, (xx + cc) - 2 dot, first index wins ties).
 //
+// K = 256 m codes per level, m = 1..8.  The Gram tables cost K^2 L(L-1)/2 x 4 bytes of state (50 MB at K = 2048, L = 3;
+// 470 MB at L = 8) and l K 4 bytes of reads per row at level l; prepare computes them in float64, (K / 16)^2 blocks per table.
+//
 #include "tc_common.cuh"
 
 int tcx_run(const float* x, int64_t ldx, int B, const void* state, int D, int L, int64_t* ids, int* stats, int sm_count,
             cudaStream_t st);
+int tcx_blocked_run(const float* x, int64_t ldx, int B, const void* state, int D, int K, int L, int64_t* ids, int* stats,
+                    int sm_count, cudaStream_t st);
 
 extern "C" int rqb200_tokenize_tc_supported(int D, int K, int L) {
-  return (K == TC_K && D >= TC_KC && D <= TC_MAX_D && D % TC_KC == 0 && L >= 1 && L <= RQB_MAX_LEVELS) ? 1 : 0;
+  return (K >= TC_K && K <= TC_MAX_K && K % TC_K == 0 && D >= TC_KC && D <= TC_MAX_D && D % TC_KC == 0 && L >= 1 &&
+          L <= RQB_MAX_LEVELS) ? 1 : 0;
 }
 
 extern "C" size_t rqb200_tokenize_tc_state_bytes(int D, int K, int L) {
   if (!rqb200_tokenize_tc_supported(D, K, L)) return 0;
-  return tc_off_blob(D, L) + (size_t)L * 2 * (D / TC_KC) * TC_BSTAGE_BYTES;
+  return tc_state_size(D, K, L);
 }
 
 // ------------------------------------------------------------------------------------------------ prepare
 // hcc[l][k] = cc/2 from a float64 sum (the filter's table); amax and c2max of the level
-__global__ void tc_prep_stats_kernel(const float* const* cbs, int D, TcHeader* hdr, float* hcc) {
+__global__ void tc_prep_stats_kernel(const float* const* cbs, int D, int K, TcHeader* hdr, float* hcc) {
   const int l = blockIdx.y;
   const int k = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (k >= TC_K) return;
+  if (k >= K) return;
   const float* c = cbs[l] + (int64_t)k * D;
   double s2 = 0.0;
   float mx = 0.f;
@@ -44,7 +50,7 @@ __global__ void tc_prep_stats_kernel(const float* const* cbs, int D, TcHeader* h
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
   if (lane == 0) {
-    hcc[l * TC_K + k] = (float)(0.5 * s2);
+    hcc[l * K + k] = (float)(0.5 * s2);
     atomicMax(&hdr->amax_bits[l], __float_as_uint(mx));
     atomicMax(&hdr->c2_bits[l], __float_as_uint(__double2float_ru(sqrt(s2))));
   }
@@ -52,15 +58,15 @@ __global__ void tc_prep_stats_kernel(const float* const* cbs, int D, TcHeader* h
 
 // cc[l][k] = sum_d c^2 in fp32, lane-strided fma + shuffle tree: bit-identical to rq_prep_norm_kernel (csrc/rq_simt.cu), it is
 // the value the exact re-rank adds in (xx + cc) - 2 dot
-__global__ void tc_prep_cc_kernel(const float* const* cbs, int D, float* cc) {
+__global__ void tc_prep_cc_kernel(const float* const* cbs, int D, int K, float* cc) {
   const int l = blockIdx.y;
   const int k = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (k >= TC_K) return;
+  if (k >= K) return;
   const float* c = cbs[l] + (int64_t)k * D;
   float s2 = 0.f;
   for (int d = lane; d < D; d += 32) s2 = fmaf(c[d], c[d], s2);
   s2 = warp_sum(s2);
-  if (lane == 0) cc[l * TC_K + k] = s2;
+  if (lane == 0) cc[l * K + k] = s2;
 }
 
 __global__ void tc_prep_scale_kernel(TcHeader* hdr, int L) {
@@ -78,10 +84,10 @@ __global__ void tc_prep_scale_kernel(TcHeader* hdr, int L) {
 }
 
 // measured fp16 rounding of every code: chat = max_k ||c~_k||, ec = max_k ||c~_k - c_k||  (c~ = fp16(c sc) / sc), float64 sums
-__global__ void tc_prep_err_kernel(const float* const* cbs, int D, TcHeader* hdr) {
+__global__ void tc_prep_err_kernel(const float* const* cbs, int D, int K, TcHeader* hdr) {
   const int l = blockIdx.y;
   const int k = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (k >= TC_K) return;
+  if (k >= K) return;
   const float sc = hdr->lv[l].sc;
   const double inv = 1.0 / (double)sc;
   const float* c = cbs[l] + (int64_t)k * D;
@@ -112,13 +118,13 @@ __global__ void tc_prep_consts_kernel(TcHeader* hdr, int L) {
   c.gerr = 2.38418579e-7f * (c.c2max * g + 0.5f * c.c2max * c.c2max);   // 2^-22: tables from float64 rounded once, <= 4 fp32 roundings after
 }
 
-// Bblob[(l*2+h)*nkc + kc] = 16 KB smem image of codes [128h, 128h+128) x k [64kc, 64kc+64):
+// Bblob[(l*(K/128)+h)*nkc + kc] = 16 KB smem image of codes [128h, 128h+128) x k [64kc, 64kc+64):
 // K-major, 128 B per code row, 16-byte chunks XOR-swizzled with (row & 7)  (the wgmma SWIZZLE_128B canonical layout); the blocks
-// h = 0 and h = 1 of a (level, chunk) form one 256-code operand in shared memory
-__global__ void tc_prep_blob_kernel(const float* const* cbs, int D, const TcHeader* hdr, __half* blob) {
-  const int nkc = D / TC_KC;
-  const int blk = blockIdx.x;  // (l*2+h)*nkc + kc
-  const int kc = blk % nkc, h = (blk / nkc) & 1, l = blk / (2 * nkc);
+// h = 2nb and h = 2nb + 1 of a (level, chunk) form the 256-code operand of code block nb in shared memory
+__global__ void tc_prep_blob_kernel(const float* const* cbs, int D, int K, const TcHeader* hdr, __half* blob) {
+  const int nkc = D / TC_KC, nh = K / 128;
+  const int blk = blockIdx.x;  // (l*nh+h)*nkc + kc
+  const int kc = blk % nkc, h = (blk / nkc) % nh, l = blk / (nh * nkc);
   const float sc = hdr->lv[l].sc;
   const float* c = cbs[l];
   __half* out = blob + (size_t)blk * (TC_BSTAGE_BYTES / 2);
@@ -134,7 +140,7 @@ __global__ void tc_prep_blob_kernel(const float* const* cbs, int D, const TcHead
 // folded in before the rounding, so the epilogue scores with one table sum:  h[k] = T[k] - S[k] / sc,
 // T = cc/2 + sum_j G_{j,l}[id_j]  (argmin-equivalent to quantize.py:113-117).  16 x 16 outputs per block, k tiles of 16 through smem.
 __global__ void __launch_bounds__(256) tc_prep_gram_kernel(const float* __restrict__ cj, const float* __restrict__ cl, int D,
-                                                           float* __restrict__ g, int fold_cc) {
+                                                           int K, float* __restrict__ g, int fold_cc) {
   __shared__ float sa[16][17], sb[16][17];
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
   const int i = blockIdx.y * 16 + ty, k = blockIdx.x * 16 + tx;
@@ -151,13 +157,13 @@ __global__ void __launch_bounds__(256) tc_prep_gram_kernel(const float* __restri
     }
     __syncthreads();
   }
-  g[(size_t)i * TC_K + k] = (float)(fold_cc ? acc + 0.5 * cck : acc);
+  g[(size_t)i * K + k] = (float)(fold_cc ? acc + 0.5 * cck : acc);
 }
 
 extern "C" int rqb200_tokenize_tc_prepare(const float* const* codebooks, int D, int K, int L, void* state,
                                           size_t state_bytes, void* stream) {
   if (!rqb200_tokenize_tc_supported(D, K, L)) {
-    rqb_set_error("tokenize_tc: shape D=%d K=%d L=%d not supported (need K=256, D %% 64 == 0, 64 <= D <= 768)", D, K, L);
+    rqb_set_error("tokenize_tc: shape D=%d K=%d L=%d not supported (need K = 256 m with 1 <= m <= 8, D %% 64 == 0, 64 <= D <= 768)", D, K, L);
     return RQB_ERR_UNSUPPORTED;
   }
   RQB_CHECK_ARG(codebooks && state, "tokenize_tc_prepare: null pointer");
@@ -168,37 +174,37 @@ extern "C" int rqb200_tokenize_tc_prepare(const float* const* codebooks, int D, 
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   char* base = reinterpret_cast<char*>(state);
   TcHeader* hdr = reinterpret_cast<TcHeader*>(base);
-  float* cc = reinterpret_cast<float*>(base + tc_off_cc(L));
-  float* hcc = reinterpret_cast<float*>(base + tc_off_hcc(L));
-  float* gram = reinterpret_cast<float*>(base + tc_off_gram(L));
-  const float** cbptr = reinterpret_cast<const float**>(base + tc_off_cbptr(L));
-  __half* blob = reinterpret_cast<__half*>(base + tc_off_blob(D, L));
-  float* cbf = reinterpret_cast<float*>(base + tc_off_cbf(L));
+  float* cc = reinterpret_cast<float*>(base + tc_off_cc(K, L));
+  float* hcc = reinterpret_cast<float*>(base + tc_off_hcc(K, L));
+  float* gram = reinterpret_cast<float*>(base + tc_off_gram(K, L));
+  const float** cbptr = reinterpret_cast<const float**>(base + tc_off_cbptr(K, L));
+  __half* blob = reinterpret_cast<__half*>(base + tc_off_blob(D, K, L));
+  float* cbf = reinterpret_cast<float*>(base + tc_off_cbf(K, L));
   RQB_CUDA(cudaMemsetAsync(hdr, 0, sizeof(TcHeader), st));
   // fp32 copy for the exact re-rank: 256-byte aligned rows whatever the caller's tensors look like, and the prepared state
   // no longer references caller memory after this call returns (stream order); every prepare kernel reads the copy
   const float* cbfp[RQB_MAX_LEVELS] = {};
   for (int l = 0; l < L; ++l) {
-    RQB_CUDA(cudaMemcpyAsync(cbf + (size_t)l * TC_K * D, codebooks[l], sizeof(float) * TC_K * D, cudaMemcpyDeviceToDevice, st));
-    cbfp[l] = cbf + (size_t)l * TC_K * D;
+    RQB_CUDA(cudaMemcpyAsync(cbf + (size_t)l * K * D, codebooks[l], sizeof(float) * K * D, cudaMemcpyDeviceToDevice, st));
+    cbfp[l] = cbf + (size_t)l * K * D;
   }
   RQB_CUDA(cudaMemcpyAsync(cbptr, cbfp, sizeof(float*) * L, cudaMemcpyHostToDevice, st));   // pageable source: staged before the call returns
-  tc_prep_stats_kernel<<<dim3(TC_K / 8, L), 256, 0, st>>>(cbptr, D, hdr, hcc);
+  tc_prep_stats_kernel<<<dim3(K / 8, L), 256, 0, st>>>(cbptr, D, K, hdr, hcc);
   RQB_LAUNCH_CHECK();
-  tc_prep_cc_kernel<<<dim3(TC_K / 8, L), 256, 0, st>>>(cbptr, D, cc);
+  tc_prep_cc_kernel<<<dim3(K / 8, L), 256, 0, st>>>(cbptr, D, K, cc);
   RQB_LAUNCH_CHECK();
   tc_prep_scale_kernel<<<1, 32, 0, st>>>(hdr, L);
   RQB_LAUNCH_CHECK();
-  tc_prep_err_kernel<<<dim3(TC_K / 8, L), 256, 0, st>>>(cbptr, D, hdr);
+  tc_prep_err_kernel<<<dim3(K / 8, L), 256, 0, st>>>(cbptr, D, K, hdr);
   RQB_LAUNCH_CHECK();
   tc_prep_consts_kernel<<<1, 32, 0, st>>>(hdr, L);
   RQB_LAUNCH_CHECK();
-  tc_prep_blob_kernel<<<L * 2 * (D / TC_KC), 256, 0, st>>>(cbptr, D, hdr, blob);
+  tc_prep_blob_kernel<<<L * (K / 128) * (D / TC_KC), 256, 0, st>>>(cbptr, D, K, hdr, blob);
   RQB_LAUNCH_CHECK();
   for (int l = 1; l < L; ++l)
     for (int j = 0; j < l; ++j) {
-      float* g = gram + (size_t)(l * (l - 1) / 2 + j) * TC_K * TC_K;
-      tc_prep_gram_kernel<<<dim3(TC_K / 16, TC_K / 16), 256, 0, st>>>(cbf + (size_t)j * TC_K * D, cbf + (size_t)l * TC_K * D, D, g, j == 0);
+      float* g = gram + (size_t)(l * (l - 1) / 2 + j) * K * K;
+      tc_prep_gram_kernel<<<dim3(K / 16, K / 16), 256, 0, st>>>(cbf + (size_t)j * K * D, cbf + (size_t)l * K * D, D, K, g, j == 0);
       RQB_LAUNCH_CHECK();
     }
   return RQB_OK;
@@ -221,5 +227,7 @@ extern "C" int rqb200_tokenize_tc_run(const float* x, int64_t ldx, int B, const 
   // the converter reads x as float4: 16-byte aligned base and row pitch (ops.py copies other layouts)
   RQB_CHECK_ARG(((ldx & 3) == 0) && ((reinterpret_cast<uintptr_t>(x) & 15) == 0),
                 "tokenize_tc_run: x must be 16-byte aligned with a row stride that is a multiple of 4 floats");
-  return tcx_run(x, ldx, B, state, D, L, ids, stats, sm_count, st);
+  // K = 256: one accumulator holds a level (csrc/rq_tcx.cu); larger K is scored in 256-code blocks (csrc/rq_tcx_blocked.cu)
+  if (K == TC_K) return tcx_run(x, ldx, B, state, D, L, ids, stats, sm_count, st);
+  return tcx_blocked_run(x, ldx, B, state, D, K, L, ids, stats, sm_count, st);
 }

@@ -1,4 +1,5 @@
-// Tensor-core tokeniser for sm_90a: wgmma fp16 candidate filter + exact fp32 re-rank.
+// Tensor-core tokeniser for sm_90a: wgmma fp16 candidate filter + exact fp32 re-rank, K = 256 codes per level (one 256-code
+// accumulator holds all of a level's codes).  K = 512 .. 2048 is csrc/rq_tcx_blocked.cu.
 //
 // Result contract: identical to rqb200_rq_forward(mode = EVAL, ids only) -- the hard-argmin chain of
 // modules/quantize.py:113-128,159-161 x L + modules/rqvae.py:125-132 (what semids.py:125 consumes).
@@ -361,11 +362,11 @@ int tcx_run(const float* x, int64_t ldx, int B, const void* state, int D, int L,
   p.x = x; p.ldx = ldx; p.B = B; p.D = D; p.L = L; p.nkc = D / TC_KC;
   p.ntiles = (B + TX_R - 1) / TX_R;
   p.hdr = reinterpret_cast<const TcHeader*>(base);
-  p.cc = reinterpret_cast<const float*>(base + tc_off_cc(L));
-  p.hcc = reinterpret_cast<const float*>(base + tc_off_hcc(L));
-  p.gram = reinterpret_cast<const float*>(base + tc_off_gram(L));
-  p.cbf = reinterpret_cast<const float*>(base + tc_off_cbf(L));
-  p.blob = reinterpret_cast<const unsigned char*>(base + tc_off_blob(D, L));
+  p.cc = reinterpret_cast<const float*>(base + tc_off_cc(TC_K, L));
+  p.hcc = reinterpret_cast<const float*>(base + tc_off_hcc(TC_K, L));
+  p.gram = reinterpret_cast<const float*>(base + tc_off_gram(TC_K, L));
+  p.cbf = reinterpret_cast<const float*>(base + tc_off_cbf(TC_K, L));
+  p.blob = reinterpret_cast<const unsigned char*>(base + tc_off_blob(D, TC_K, L));
   p.ids = ids; p.stats = stats;
   // shared memory: x image + codebook ring + fixed part + id bytes of L levels; the ring gets as many 32 KB stages
   // (<= TX_NB_MAX) as fit under the 227 KB limit (2 at D = 768 with 8 levels, 4 with 3 levels)

@@ -7,7 +7,8 @@
 #include <cmath>
 #include <cstdlib>
 
-#define TC_K 256          // codes per level (fixed)
+#define TC_K 256          // codes per block: one wgmma m64n256 accumulator; a level has K = 256 m codes, m = 1..8
+#define TC_MAX_K 2048
 #define TC_KC 64          // fp16 elements per 128-byte swizzle row
 #define TC_MAX_D 768
 #define TC_MAX_KC (TC_MAX_D / TC_KC)
@@ -50,12 +51,16 @@ __host__ __device__ __forceinline__ float tc_eps(const TcLevelConst& lc, float e
   return TC_INFL * (ex * lc.chat + xn * lc.ec) + acc + lc.gerr + ref;
 }
 
-static size_t tc_off_cc(int L) { return rqb_round_up(sizeof(TcHeader), 256); }
-static size_t tc_off_hcc(int L) { return tc_off_cc(L) + rqb_round_up((size_t)L * TC_K * 4, 256); }
-static size_t tc_off_gram(int L) { return tc_off_hcc(L) + rqb_round_up((size_t)L * TC_K * 4, 256); }
-static size_t tc_off_cbptr(int L) { return tc_off_gram(L) + (size_t)(L * (L - 1) / 2) * TC_K * TC_K * 4; }
-static size_t tc_off_cbf(int L) { return rqb_round_up(tc_off_cbptr(L) + RQB_MAX_LEVELS * 8, 256); }   // fp32 copy [L][256][D]
-static size_t tc_off_blob(int D, int L) { return rqb_round_up(tc_off_cbf(L) + (size_t)L * TC_K * D * 4, 1024); }
+// Prepared state, in order: header | cc [L][K] | hcc [L][K] | Gram tables [L(L-1)/2][K][K] | codebook pointers |
+// fp32 codebooks [L][K][D] | fp16 blob [L][K/128][D/64][16 KB].  The Gram tables dominate at large K (K^2 L(L-1)/2 x 4 bytes:
+// 50 MB of the ~80 MB at K = 2048, L = 3, D = 768; 470 MB of the ~0.55 GB at L = 8).
+static size_t tc_off_cc(int K, int L) { return rqb_round_up(sizeof(TcHeader), 256); }
+static size_t tc_off_hcc(int K, int L) { return tc_off_cc(K, L) + rqb_round_up((size_t)L * K * 4, 256); }
+static size_t tc_off_gram(int K, int L) { return tc_off_hcc(K, L) + rqb_round_up((size_t)L * K * 4, 256); }
+static size_t tc_off_cbptr(int K, int L) { return tc_off_gram(K, L) + (size_t)(L * (L - 1) / 2) * K * K * 4; }
+static size_t tc_off_cbf(int K, int L) { return rqb_round_up(tc_off_cbptr(K, L) + RQB_MAX_LEVELS * 8, 256); }   // fp32 copy [L][K][D]
+static size_t tc_off_blob(int D, int K, int L) { return rqb_round_up(tc_off_cbf(K, L) + (size_t)L * K * D * 4, 1024); }
+static size_t tc_state_size(int D, int K, int L) { return tc_off_blob(D, K, L) + (size_t)L * (K / 128) * (D / TC_KC) * TC_BSTAGE_BYTES; }
 
 __device__ __forceinline__ uint32_t tc_bf16_up(float v) {   // bf16 bits of the smallest bf16 >= v (v >= 0, inf/nan kept)
   uint32_t b = __float_as_uint(v);

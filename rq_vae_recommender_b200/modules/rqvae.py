@@ -206,9 +206,10 @@ class RqVae(nn.Module, PyTorchModelHubMixin):
     @torch.compiler.disable
     @torch.no_grad()
     def tokenize(self, x: Tensor, mlp_precision: str = None) -> Tensor:
-        """sem_ids [B,L] only: what SemanticIdTokenizer consumes (semids.py:125).  Large batches go through the tcgen05
-        candidate filter + exact re-rank (prepared codebook state cached on the codebooks' identity and version; the shipped
-        D = 32 quantiser is zero-padded to 64), small ones through the exact CUDA-core kernel: ops.rq_tokenize_auto.
+        """sem_ids [B,L] only: what SemanticIdTokenizer consumes (semids.py:125).  Large batches of a model whose codebook
+        size is 256 m (m = 1..8) go through the wgmma candidate filter + exact re-rank (prepared codebook state cached on the
+        codebooks' identity and version; the shipped D = 32 quantiser is zero-padded to 64), everything else through the exact
+        CUDA-core kernel: ops.rq_tokenize_auto.
         ``mlp_precision="bf16"`` runs the encoder on the bf16 wgmma GEMMs (faster, NOT index-exact vs fp32)."""
         x = x.to(next(self.encoder.parameters()).dtype)
         if mlp_precision is not None:

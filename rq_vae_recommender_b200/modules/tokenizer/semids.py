@@ -1,9 +1,10 @@
 """modules/tokenizer/semids.py of the reference (:22-146) on the fused tokeniser kernels.
 
 Same class name, constructor and methods.  ``precompute_corpus_ids`` differs underneath:
-  * the corpus goes through ``RqVae.tokenize`` in 65 536-row batches -> ``ops.rq_tokenize_auto``: the tcgen05 candidate
-    filter + exact re-rank (prepared state cached on the codebooks; D = 32 / 64 quantisers zero-padded to 64) when K = 256
-    and the batch has >= 1 024 rows, else the exact CUDA-core kernel -- instead of 512-row batches of full RqVae forwards;
+  * the corpus goes through ``RqVae.tokenize`` in 65 536-row batches -> ``ops.rq_tokenize_auto``: the wgmma candidate
+    filter + exact re-rank (prepared state cached on the codebooks; D = 32 / 64 quantisers zero-padded to 64) when K is
+    256, 512, ..., 2048 and the batch has >= 1 024 rows, else the exact CUDA-core kernel -- instead of 512-row batches of
+    full RqVae forwards;
   * the dedup column -- the number of EARLIER corpus rows with the same id tuple, which the reference finds with an
     O(N^2) compare against everything seen so far (semids.py:94-108, 90-97 % of its wall time, SURVEY 8f-1) -- is the
     rank inside a stable sort of packed tuples: identical values, O(N log N).

@@ -657,7 +657,7 @@ TC_PAD = 64   # the wgmma tokeniser wants D % 64 == 0: narrower / odd widths are
 
 def tc_padded_dim(D: int, K: int, L: int) -> int:
     """Width the tensor-core tokeniser runs a D-wide quantiser at (D itself, or D zero-padded to the next multiple of 64);
-    0 when the shape cannot use it at all (K != 256, D > 768, L > 8)."""
+    0 when the shape cannot use it at all (K not one of 256, 512, ..., 2048; D > 768; L > 8)."""
     Dp = (D + TC_PAD - 1) // TC_PAD * TC_PAD
     return Dp if tc_supported(Dp, K, L) else 0
 
@@ -751,8 +751,9 @@ def tc_state_for(codebooks: Sequence[torch.Tensor]) -> TcState:
 
 def rq_tokenize_auto(x: torch.Tensor, codebooks: Sequence[torch.Tensor], stats=None) -> torch.Tensor:
     """What the module API calls (RqVae.tokenize, SemanticIdTokenizer.precompute_corpus_ids, modules/rqvae.py:118-139 ids
-    only): the tensor-core tokeniser with a cached prepared state whenever the shape allows (K = 256, D <= 768 after
-    zero-padding to a multiple of 64) and the batch is large enough to fill the GPU, else the exact CUDA-core kernel."""
+    only): the tensor-core tokeniser with a cached prepared state whenever the shape allows (K = 256 m with m = 1..8,
+    D <= 768 after zero-padding to a multiple of 64) and the batch is large enough to fill the GPU, else the exact CUDA-core
+    kernel."""
     K, D = codebooks[0].shape
     if x.shape[0] >= TC_MIN_ROWS and not torch.is_grad_enabled() and tc_padded_dim(D, K, len(codebooks)):
         return rq_tokenize_tc(x, state=tc_state_for(codebooks), stats=stats)

@@ -28,8 +28,8 @@ def shard_bounds(n: int, world: int, rank: int):
 
 class CorpusTokenizer:
     """Frozen codebooks -> ids.  ``use_tc`` selects the wgmma filter + exact re-rank kernel (state prepared once; its margin is
-    a deterministic bound, so the result contract is the exact kernel's).  Default: on whenever the shape allows it (K = 256,
-    D <= 768; widths that are not a multiple of 64 are zero-padded)."""
+    a deterministic bound, so the result contract is the exact kernel's).  Default: on whenever the shape allows it (K = 256 m
+    with m = 1..8, D <= 768; widths that are not a multiple of 64 are zero-padded)."""
 
     def __init__(self, codebooks: Sequence[torch.Tensor], use_tc: Optional[bool] = None,
                  encoder: Optional[Callable[[torch.Tensor], torch.Tensor]] = None, chunk_rows: int = 16384):
