@@ -14,7 +14,7 @@ from typing import Optional
 PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "librqb200.so")
-SOURCES = ["api.cu", "rq_simt.cu", "dense.cu", "rq_tc.cu", "rq_tcx.cu", "rq_tcx_blocked.cu", "gemm_tc.cu", "sid.cu"]
+SOURCES = ["api.cu", "rq_simt.cu", "dense.cu", "rq_tc.cu", "rq_tcx.cu", "gemm_tc.cu", "sid.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-shared", "-Xcompiler", "-fPIC"]
 

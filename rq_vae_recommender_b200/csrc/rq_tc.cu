@@ -1,4 +1,4 @@
-// Tensor-core tokeniser for sm_90a: prepared codebook state + C-ABI entry points (the kernel is csrc/rq_tcx.cu).
+// Tensor-core tokeniser for sm_90a: prepared codebook state + C-ABI entry points (the kernels are in csrc/rq_tcx.cu).
 //
 // Result contract: identical to rqb200_rq_forward(mode = EVAL, ids only) -- the hard-argmin chain of
 // modules/quantize.py:113-128,159-161 x L + modules/rqvae.py:125-132 (what semids.py:125 consumes).
@@ -17,10 +17,8 @@
 //
 #include "tc_common.cuh"
 
-int tcx_run(const float* x, int64_t ldx, int B, const void* state, int D, int L, int64_t* ids, int* stats, int sm_count,
+int tcx_run(const float* x, int64_t ldx, int B, const void* state, int D, int K, int L, int64_t* ids, int* stats, int sm_count,
             cudaStream_t st);
-int tcx_blocked_run(const float* x, int64_t ldx, int B, const void* state, int D, int K, int L, int64_t* ids, int* stats,
-                    int sm_count, cudaStream_t st);
 
 extern "C" int rqb200_tokenize_tc_supported(int D, int K, int L) {
   return (K >= TC_K && K <= TC_MAX_K && K % TC_K == 0 && D >= TC_KC && D <= TC_MAX_D && D % TC_KC == 0 && L >= 1 &&
@@ -227,7 +225,5 @@ extern "C" int rqb200_tokenize_tc_run(const float* x, int64_t ldx, int B, const 
   // the converter reads x as float4: 16-byte aligned base and row pitch (ops.py copies other layouts)
   RQB_CHECK_ARG(((ldx & 3) == 0) && ((reinterpret_cast<uintptr_t>(x) & 15) == 0),
                 "tokenize_tc_run: x must be 16-byte aligned with a row stride that is a multiple of 4 floats");
-  // K = 256: one accumulator holds a level (csrc/rq_tcx.cu); larger K is scored in 256-code blocks (csrc/rq_tcx_blocked.cu)
-  if (K == TC_K) return tcx_run(x, ldx, B, state, D, L, ids, stats, sm_count, st);
-  return tcx_blocked_run(x, ldx, B, state, D, K, L, ids, stats, sm_count, st);
+  return tcx_run(x, ldx, B, state, D, K, L, ids, stats, sm_count, st);
 }

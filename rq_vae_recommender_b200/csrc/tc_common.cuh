@@ -1,5 +1,5 @@
-// Shared definitions of the tensor-core tokeniser (csrc/rq_tc.cu, csrc/rq_tcx.cu): prepared-state layout, filter bound,
-// small device helpers.
+// Shared definitions of the tensor-core tokeniser (csrc/rq_tc.cu: prepare and C ABI; csrc/rq_tcx.cu: the K = 256 and blocked
+// kernels): prepared-state layout, filter bound, small device helpers.
 // Everything here is static / inline; the result contract is stated at the top of rq_tc.cu.
 #pragma once
 #include "common.cuh"

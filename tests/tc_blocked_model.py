@@ -1,5 +1,5 @@
 """numpy model of the blocked candidate selection of the tensor-core tokeniser for K = 512 .. 2048 codes
-(csrc/rq_tcx_blocked.cu) -- test infrastructure, built on the unblocked filter model of tests/tc_filter_model.py.
+(rq_tcx_blocked_kernel in csrc/rq_tcx.cu) -- test infrastructure, built on the unblocked filter model of tests/tc_filter_model.py.
 
 The codes of a level are scored one 256-code block at a time.  Block b keeps {k in b : h[k] <= M_b + margin}, with M_b the
 running row minimum over blocks 0..b and margin = 2 eps (1 + 2^-16).  At the end of the level every block whose minimum is

@@ -1,5 +1,5 @@
 """CPU model of the tensor-core tokeniser's blocked candidate selection for K = 512 .. 2048 codes
-(tests/tc_blocked_model.py restates csrc/rq_tcx_blocked.cu): the kept set always contains the unblocked filter's set,
+(tests/tc_blocked_model.py restates rq_tcx_blocked_kernel in csrc/rq_tcx.cu): the kept set always contains the unblocked filter's set,
 which contains the float64 argmin, and blocking adds (almost) no rows to the exact re-rank."""
 import numpy as np
 import pytest
