@@ -1,0 +1,170 @@
+#!/usr/bin/env python
+"""bench_generate.py -- the sampled, prefix-constrained beam search of the generative-retrieval model.
+
+    python bench_generate.py [--min-window-s 1.0]
+
+At the shipped evaluation settings (configs/decoder_amazon.gin: batch 640, top_k_for_generation 10, 64 sampled candidates per
+beam, K = 256 codes, 3 hierarchy levels), on a 12 101-row corpus (Amazon Beauty's size) and a 1 M-row synthetic one:
+  * ms per level h = 0, 1, 2 for three arms that all start from the level's probabilities:
+      reference   torch.multinomial, log/gather, the reference's prefix check (every prefix against every corpus row, in
+                  100 000-prefix chunks), masked_fill, sort and gathers (modules/model.py's expression);
+      composed    torch.multinomial, log/gather, then SidPrefixIndex.beam_select (one kernel);
+      fused       draw_exponential, then SidPrefixIndex.sample_select (one kernel);
+    the reference arm is not run on the 1 M-row corpus: one chunk would need 100 000 x 1 M x l bytes of bool temporaries;
+  * whole-generate ms of the drop-in EncoderDecoderRetrievalModel at the decoder_amazon.gin T5 shape (d_model 384, 6 heads,
+    d_ff 1024, 4 layers, randomly initialised) on 20-item histories, and of the same model with the composed arm in place of
+    sample_select, under the same seed (their beams are compared); three alternating windows each.
+Every shape is warmed up, every timed window lasts at least --min-window-s seconds (CUDA events).  Prints the card's name,
+power limit and max SM clock, and one JSON line; writes nothing.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, ROOT)
+
+B, TOP_K, NC, K, H, ITEMS = 640, 10, 64, 256, 3, 20
+
+
+def _card():
+    """Name, power limit and max SM clock of GPU 0 (read-only query); the numbers are only meaningful beside them."""
+    try:
+        q = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30)
+        return q.stdout.strip() or None
+    except Exception:
+        return None
+
+
+def timed_ms(torch, fn, min_window_s):
+    """ms per call over a window of at least min_window_s seconds, after warm-up calls."""
+    for _ in range(3):
+        fn()
+    torch.cuda.synchronize()
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    n = 1
+    while True:
+        a.record()
+        for _ in range(n):
+            fn()
+        b.record()
+        torch.cuda.synchronize()
+        ms = a.elapsed_time(b)
+        if ms >= min_window_s * 1e3:
+            return ms / n
+        n = max(n * 2, int(n * min_window_s * 1e3 / max(ms, 1e-3) * 1.2) + 1)
+
+
+def reference_level(torch, corpus, probas, generated, log_probas, k, nc):
+    """modules/model.py's sampling and selection step, as the reference computes it."""
+    samples = torch.multinomial(probas, num_samples=nc)
+    samp_log_p = torch.log(torch.gather(probas, 1, samples))
+    if generated is None:
+        prefix = samples.reshape(-1, 1)
+    else:
+        h = generated.shape[2]
+        prefix = torch.cat([generated.reshape(-1, h).repeat_interleave(nc, dim=0), samples.reshape(-1, 1)], dim=1)
+    trimmed = corpus[:, : prefix.shape[1]]
+    valid = torch.cat([(trimmed.unsqueeze(1) == prefix[i:i + 100000].unsqueeze(0)).all(dim=2).any(dim=0)
+                       for i in range(0, prefix.shape[0], 100000)])
+    Bn = probas.shape[0] if generated is None else generated.shape[0]
+    if generated is None:
+        scores, idx = samp_log_p.masked_fill(~valid.reshape(Bn, nc), float("-inf")).sort(-1, descending=True)
+        return torch.gather(samples, 1, idx[:, :k]).unsqueeze(-1), scores[:, :k], None
+    kp, h = generated.shape[1], generated.shape[2]
+    total = samp_log_p.reshape(Bn, kp * nc) + log_probas.repeat_interleave(nc, dim=1)
+    scores, idx = total.masked_fill(~valid.reshape(Bn, kp * nc), float("-inf")).sort(-1, descending=True)
+    top = idx[:, :k]
+    parent = top // nc
+    parent_global = (parent + torch.arange(Bn, device=parent.device).unsqueeze(1) * kp).flatten()
+    parent_ids = torch.gather(generated, 1, parent.unsqueeze(-1).expand(-1, -1, h))
+    new_ids = torch.gather(samples.reshape(Bn, kp * nc), 1, top).unsqueeze(-1)
+    return torch.cat([parent_ids, new_ids], dim=-1), scores[:, :k], parent_global
+
+
+def composed_level(torch, index, probas, generated, log_probas, k, nc):
+    samples = torch.multinomial(probas, num_samples=nc)
+    samp_log_p = torch.log(torch.gather(probas, 1, samples))
+    return index.beam_select(samples, samp_log_p, generated, log_probas, k)
+
+
+def corpus_of(np, rows, seed):
+    rs = np.random.RandomState(seed)
+    return rs.randint(0, K, size=(rows, H)).astype(np.int64)
+
+
+def level_inputs(torch, F, index, seed):
+    """Per level: probabilities (softmax of random logits) and the beams entering it (from the fused chain)."""
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    out, generated, log_probas = [], None, None
+    from rq_vae_recommender_b200.modules.model import draw_exponential
+    for h in range(H):
+        rows = B if h == 0 else B * TOP_K
+        probas = F.softmax(torch.randn(rows, K, device="cuda", generator=g) * 3, dim=-1)
+        out.append((probas, generated, log_probas))
+        generated, log_probas, _ = index.sample_select(probas, draw_exponential(probas), generated, log_probas, TOP_K, NC)
+    return out
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--min-window-s", type=float, default=1.0)
+    args = ap.parse_args()
+    import numpy as np
+    import torch
+    import torch.nn.functional as F
+    from rq_vae_recommender_b200 import ops
+    from rq_vae_recommender_b200.modules import model as M
+    assert torch.cuda.is_available(), "bench_generate.py measures on a CUDA device"
+    w = args.min_window_s
+    out = {"card": _card(), "batch": B, "top_k": TOP_K, "candidates": NC, "codes": K, "levels": H}
+    for name, rows in (("corpus_12101", 12101), ("corpus_1M", 1 << 20)):
+        corpus = torch.from_numpy(corpus_of(np, rows, rows)).cuda()
+        index = ops.SidPrefixIndex(corpus, K)
+        res = {}
+        for h, (probas, generated, log_probas) in enumerate(level_inputs(torch, F, index, 7)):
+            arms = {"composed_ms": lambda: composed_level(torch, index, probas, generated, log_probas, TOP_K, NC),
+                    "fused_ms": lambda: index.sample_select(probas, M.draw_exponential(probas), generated, log_probas, TOP_K, NC)}
+            if rows < 100000:
+                arms["reference_ms"] = lambda: reference_level(torch, corpus, probas, generated, log_probas, TOP_K, NC)
+            res[f"level{h}"] = {arm: timed_ms(torch, fn, w) for arm, fn in arms.items()}
+        out[name] = res
+        del index, corpus
+        torch.cuda.empty_cache()
+
+    class Composed(M.EncoderDecoderRetrievalModel):
+        def _sample_and_select(self, index, probas, generated, log_probas, k, n_cands, reject):
+            return composed_level(torch, index, probas, generated, log_probas, k, n_cands)
+
+    corpus = torch.from_numpy(corpus_of(np, 12101, 12101))
+    shape = dict(num_hierarchies=H, num_embeddings_per_hierarchy=K, t5_d_model=384, t5_num_heads=6, t5_d_ff=1024,
+                 t5_num_layers=4, top_k_for_generation=TOP_K, should_add_sep_token=True)
+    torch.manual_seed(0)
+    fused = M.EncoderDecoderRetrievalModel(codebooks=corpus.clone(), **shape).cuda().eval()
+    composed = Composed(codebooks=corpus.clone(), **shape).cuda().eval()
+    composed.load_state_dict(fused.state_dict())
+    rs = np.random.RandomState(1)
+    ids = torch.from_numpy(rs.randint(0, K, size=(B, ITEMS * H))).cuda()
+    mask = torch.ones_like(ids)
+    torch.manual_seed(3)
+    g_f, p_f = fused.generate(mask, ids)
+    torch.manual_seed(3)
+    g_c, p_c = composed.generate(mask, ids)
+    fused_ms, composed_ms = [], []
+    for _ in range(3):                                        # alternate the two models: clock drift hits both alike
+        fused_ms.append(timed_ms(torch, lambda: fused.generate(mask, ids), w))
+        composed_ms.append(timed_ms(torch, lambda: composed.generate(mask, ids), w))
+    out["generate"] = {
+        "fused_ms": fused_ms, "composed_ms": composed_ms,
+        "beams_equal": bool(torch.equal(g_f, g_c)), "log_probas_equal": bool(torch.equal(p_f, p_c)),
+        "history_items": ITEMS, "t5": "d_model 384, 6 heads, d_ff 1024, 4 layers, random init, TF32 matmuls"}
+    out["timed"] = "CUDA events, windows >= %.1f s after warm-up; per-level arms start from the level's probabilities" % w
+    print(out["card"])
+    print(json.dumps(out))
+
+
+if __name__ == "__main__":
+    main()

@@ -192,6 +192,29 @@ int rqb200_sid_beam_select(const int64_t* samples, const float* samp_log_p, cons
                            int B, int kp, int nc, int h, int k, int C, int K, const void* prefix_workspace,
                            int64_t* out_generated, float* out_log_probas, int64_t* out_parent, void* stream);
 
+/* sid_sample_select : the sampling step of the same beam search fused with sid_beam_select, one launch per level h
+ *                     (modules/model.py:345-388 after the softmax).  torch.multinomial(p, nc) without replacement is
+ *                     topk(p / q, nc) with q = empty_like(p).exponential_(1) from the same generator; given that q in `noise`,
+ *                     this call reproduces its samples bit for bit and then selects exactly as sid_beam_select does:
+ *   probas, noise    [B*kp, K] fp32, row strides in elements (kp = 1 at h = 0, where generated and log_probas are null)
+ *   generated        [B, kp, h] int64, log_probas [B, kp] fp32: the beams entering the level
+ *   per row          ratio = probas / noise (IEEE fp32 division), the nc largest ratios in torch.topk's order (descending, NaN
+ *                    largest, equal ratios by ascending index) are the samples, samp_log_p = logf(probas[sample])
+ *   selection        score = samp_log_p + the parent's log-probability, -inf when the extended prefix is not in the corpus; the
+ *                    k best in descending order (ties: lowest candidate index; NaN last) -> out_generated [B, k, h + 1],
+ *                    out_log_probas [B, k], out_parent [B*k] = b * kp + beam
+ *   samples, samp_log_p  [B*kp, nc], optional (null: not written)
+ *   reject           optional int[2], ADDED to (never cleared): [0] rows holding a NaN, +-inf or negative probability, [1] other
+ *                    rows whose probabilities are all zero -- the rows torch.multinomial would reject with "probability
+ *                    tensor contains either `inf`, `nan` or element < 0" / "invalid multinomial distribution (sum of
+ *                    probabilities <= 0)".  Such rows still complete, with unspecified samples in [0, K).
+ *   limits           1 <= nc <= K <= 2048, kp * nc <= 1024, k <= 32, h < C <= 8, K^C within the prefix bitmap limit;
+ *                    RQB_ERR_UNSUPPORTED otherwise.  Deterministic: no result depends on the order of atomics. */
+int rqb200_sid_sample_select(const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride,
+                             const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k, int C, int K,
+                             const void* prefix_workspace, int64_t* out_generated, float* out_log_probas, int64_t* out_parent,
+                             int64_t* samples, float* samp_log_p, int* reject, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

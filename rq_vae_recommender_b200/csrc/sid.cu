@@ -274,36 +274,28 @@ extern "C" int rqb200_sid_prefix_check(const int64_t* prefix, int64_t row_stride
 // One warp per batch row; kp * nc <= 1024, k <= 32.
 #define SID_BEAM_MAX_E 1024
 
-__global__ void __launch_bounds__(128) sid_beam_select_kernel(
-    const int64_t* __restrict__ samples, const float* __restrict__ samp_log_p, const int64_t* __restrict__ generated,
-    const float* __restrict__ log_probas, int B, int kp, int nc, int h, int k, int K, const unsigned int* __restrict__ bitmap,
-    int64_t* __restrict__ out_generated, float* __restrict__ out_log_probas, int64_t* __restrict__ out_parent) {
-  __shared__ float s_score[4][SID_BEAM_MAX_E];
-  __shared__ unsigned char s_taken[4][SID_BEAM_MAX_E];
-  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int b = blockIdx.x * 4 + w;
-  if (b >= B) return;
-  const int E = kp * nc;
-  float* sc = s_score[w];
-  unsigned char* tk = s_taken[w];
-  for (int e = lane; e < E; e += 32) {
-    const int beam = e / nc;
-    const int64_t tok = samples[((int64_t)b * kp + beam) * nc + (e - beam * nc)];
-    unsigned long long key = 0;
-    bool ok = tok >= 0 && tok < K;
-    for (int j = 0; j < h; ++j) {
-      const int64_t v = generated[((int64_t)b * kp + beam) * h + j];
-      ok = ok && v >= 0 && v < K;
-      key = key * (unsigned long long)K + (unsigned long long)(ok ? v : 0);
-    }
-    key = key * (unsigned long long)K + (unsigned long long)(ok ? tok : 0);
-    ok = ok && ((__ldg(bitmap + (key >> 5)) >> (key & 31)) & 1u);
-    float s = samp_log_p[((int64_t)b * kp + beam) * nc + (e - beam * nc)] + (log_probas ? log_probas[(int64_t)b * kp + beam] : 0.f);
-    if (!ok || s != s) s = -INFINITY;                       // invalid prefix (model.py:356,366); NaN ranks last here
-    sc[e] = s;
-    tk[e] = 0;
+// Score of one candidate extension: lp (token log-probability + parent beam log-probability), or -inf when the prefix
+// parent_ids[0..h) + tok is not in the corpus (model.py:356,366) or lp is NaN (NaN ranks last here).
+__device__ __forceinline__ float sid_extension_score(int64_t tok, const int64_t* parent_ids, int h, int K,
+                                                     const unsigned int* __restrict__ bitmap, float lp) {
+  unsigned long long key = 0;
+  bool ok = tok >= 0 && tok < K;
+  for (int j = 0; j < h; ++j) {
+    const int64_t v = parent_ids[j];
+    ok = ok && v >= 0 && v < K;
+    key = key * (unsigned long long)K + (unsigned long long)(ok ? v : 0);
   }
-  __syncwarp();
+  key = key * (unsigned long long)K + (unsigned long long)(ok ? tok : 0);
+  ok = ok && ((__ldg(bitmap + (key >> 5)) >> (key & 31)) & 1u);
+  return (!ok || lp != lp) ? -INFINITY : lp;
+}
+
+// One warp keeps the k best of batch row b's E = kp * nc candidate scores sc[] in descending order: k rounds of a warp
+// arg-max over the candidates not yet taken (tk[], cleared by the caller).  tok[e] is candidate e's token (e = beam * nc + j).
+// Writes the new beams, their scores and the parent beam's global index b * kp + beam.
+__device__ __forceinline__ void sid_keep_best(const float* sc, unsigned char* tk, const int64_t* tok, int E, int nc, int b, int kp,
+                                              int h, int k, const int64_t* __restrict__ generated, int64_t* __restrict__ out_generated,
+                                              float* __restrict__ out_log_probas, int64_t* __restrict__ out_parent, int lane) {
   for (int r = 0; r < k; ++r) {
     float best = -INFINITY;
     int bi = 0x7fffffff;
@@ -324,12 +316,35 @@ __global__ void __launch_bounds__(128) sid_beam_select_kernel(
       tk[bi] = 1;
       out_log_probas[(int64_t)b * k + r] = best;
       out_parent[(int64_t)b * k + r] = (int64_t)b * kp + beam;
-      out_generated[((int64_t)b * k + r) * (h + 1) + h] = samples[((int64_t)b * kp + beam) * nc + (bi - beam * nc)];
+      out_generated[((int64_t)b * k + r) * (h + 1) + h] = tok[bi];
     }
     for (int j = lane; j < h; j += 32)
       out_generated[((int64_t)b * k + r) * (h + 1) + j] = generated[((int64_t)b * kp + beam) * h + j];
     __syncwarp();
   }
+}
+
+__global__ void __launch_bounds__(128) sid_beam_select_kernel(
+    const int64_t* __restrict__ samples, const float* __restrict__ samp_log_p, const int64_t* __restrict__ generated,
+    const float* __restrict__ log_probas, int B, int kp, int nc, int h, int k, int K, const unsigned int* __restrict__ bitmap,
+    int64_t* __restrict__ out_generated, float* __restrict__ out_log_probas, int64_t* __restrict__ out_parent) {
+  __shared__ float s_score[4][SID_BEAM_MAX_E];
+  __shared__ unsigned char s_taken[4][SID_BEAM_MAX_E];
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int b = blockIdx.x * 4 + w;
+  if (b >= B) return;
+  const int E = kp * nc;
+  float* sc = s_score[w];
+  unsigned char* tk = s_taken[w];
+  for (int e = lane; e < E; e += 32) {
+    const int beam = e / nc;
+    const int64_t row = (int64_t)b * kp + beam;
+    const float s = samp_log_p[row * nc + (e - beam * nc)] + (log_probas ? log_probas[row] : 0.f);
+    sc[e] = sid_extension_score(samples[row * nc + (e - beam * nc)], generated + row * h, h, K, bitmap, s);
+    tk[e] = 0;
+  }
+  __syncwarp();
+  sid_keep_best(sc, tk, samples + (int64_t)b * kp * nc, E, nc, b, kp, h, k, generated, out_generated, out_log_probas, out_parent, lane);
 }
 
 extern "C" int rqb200_sid_beam_select(const int64_t* samples, const float* samp_log_p, const int64_t* generated,
@@ -353,6 +368,178 @@ extern "C" int rqb200_sid_beam_select(const int64_t* samples, const float* samp_
       samples, samp_log_p, generated, log_probas, B, kp, nc, h, k, K,
       reinterpret_cast<const unsigned int*>(reinterpret_cast<const char*>(prefix_workspace) + o.off[h + 1]), out_generated,
       out_log_probas, out_parent);
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// The sampling step of the beam search fused with the selection step above (modules/model.py:344-388 after the softmax).
+// torch.multinomial(p, n) without replacement is topk(p / q, n) with q = empty_like(p).exponential_(1) drawn from the same
+// generator; given that q, this kernel reproduces its samples bit for bit: ratio = p / q as an IEEE fp32 division (at::div),
+// the n largest ratios in torch.topk's order (descending; NaN above +inf and -0 below +0, as its radix selection ranks them;
+// equal ratios by ascending index, as its gather and stable sort leave them), samp_log_p = logf(p[sample]).  The candidates
+// then go through sid_extension_score / sid_keep_best exactly as in rqb200_sid_beam_select.
+// One CTA per batch row; warp w samples beams w, w + W, ... (W = min(kp, 16)) from its own shared-memory copy of the row's
+// ratio keys; warp 0 then selects from the kp * nc candidates.  Nothing is ordered by atomics: the results are deterministic.
+#define SID_SAMPLE_MAX_WARPS 16
+#define SID_SAMPLE_MAX_K 2048
+
+// Order-preserving image of an fp32 value in the order torch.topk's radix selection uses: NaN largest, -0 below +0.
+__device__ __forceinline__ unsigned int sid_topk_key(float v) {
+  const unsigned int x = __float_as_uint(v);
+  return v == v ? x ^ ((x & 0x80000000u) ? 0xffffffffu : 0x80000000u) : 0xffffffffu;
+}
+
+// One warp: the indices of the n largest of key[0..K) into out[0..n), descending, equal keys by ascending index.  Radix
+// selection of the n-th largest key T (four 8-bit digits, shared histogram hist[256]), compaction of every key above T and of
+// the lowest-index keys equal to T (index order, sel_key / sel_idx [n]), then each kept key's rank among the kept ones.
+__device__ void sid_warp_top_n(const unsigned int* key, int K, int n, int* hist, unsigned int* sel_key, int* sel_idx, int64_t* out,
+                               int lane) {
+  const unsigned int lt = (1u << lane) - 1u;
+  unsigned int prefix = 0, pmask = 0;
+  int want = n;                                             // entries still needed among those matching the decided digits
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    for (int i = lane; i < 256; i += 32) hist[i] = 0;
+    __syncwarp();
+    for (int base = 0; base < K; base += 32) {
+      const int i = base + lane;
+      const unsigned int v = i < K ? key[i] : 0u;
+      const int d = (i < K && (v & pmask) == prefix) ? (int)((v >> shift) & 255u) : 256;
+      const unsigned int same = __match_any_sync(0xffffffffu, d);
+      if (d < 256 && (same & lt) == 0) atomicAdd(&hist[d], __popc(same));   // one add per distinct digit of the 32 keys
+    }
+    __syncwarp();
+    int c[8], s = 0;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { c[j] = hist[lane * 8 + j]; s += c[j]; }
+    int suf = s;                                            // entries in bins >= lane * 8
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int t = __shfl_down_sync(0xffffffffu, suf, o);
+      if (lane + o < 32) suf += t;
+    }
+    const int owner = 31 - __clz(__ballot_sync(0xffffffffu, suf >= want));   // the lane holding the n-th largest digit
+    int digit = 0, above = 0;
+    if (lane == owner) {
+      int acc = suf - s;
+      for (int j = 7; j >= 0; --j) {
+        if (acc + c[j] >= want) { digit = lane * 8 + j; above = acc; break; }
+        acc += c[j];
+      }
+    }
+    digit = __shfl_sync(0xffffffffu, digit, owner);
+    above = __shfl_sync(0xffffffffu, above, owner);
+    want -= above;
+    prefix |= (unsigned int)digit << shift;
+    pmask |= 255u << shift;
+    __syncwarp();
+  }
+  int kept = 0, eq_seen = 0;                                // keys above T: n - want of them; keys equal to T: the first `want`
+  for (int base = 0; base < K; base += 32) {
+    const int i = base + lane;
+    const unsigned int v = i < K ? key[i] : 0u;
+    const bool eq = i < K && v == prefix;
+    const unsigned int beq = __ballot_sync(0xffffffffu, eq);
+    const bool take = (i < K && v > prefix) || (eq && eq_seen + __popc(beq & lt) < want);
+    const unsigned int bt = __ballot_sync(0xffffffffu, take);
+    if (take) {
+      sel_key[kept + __popc(bt & lt)] = v;
+      sel_idx[kept + __popc(bt & lt)] = i;
+    }
+    kept += __popc(bt);
+    eq_seen += __popc(beq);
+  }
+  __syncwarp();
+  for (int p = lane; p < n; p += 32) {
+    const unsigned int v = sel_key[p];
+    int r = 0;
+    for (int q = 0; q < n; ++q) {
+      const unsigned int u = sel_key[q];
+      r += (u > v) || (u == v && q < p);
+    }
+    out[r] = sel_idx[p];
+  }
+  __syncwarp();
+}
+
+static size_t sid_sample_smem(int kp, int nc, int K) {
+  const int W = kp < SID_SAMPLE_MAX_WARPS ? kp : SID_SAMPLE_MAX_WARPS;
+  const size_t E = (size_t)kp * nc;
+  return E * (sizeof(int64_t) + sizeof(float) + 1) + (size_t)W * (K + 256 + 2 * nc) * 4;
+}
+
+__global__ void __launch_bounds__(SID_SAMPLE_MAX_WARPS * 32) sid_sample_select_kernel(
+    const float* __restrict__ probas, int64_t p_stride, const float* __restrict__ noise, int64_t n_stride,
+    const int64_t* __restrict__ generated, const float* __restrict__ log_probas, int kp, int nc, int h, int k, int K,
+    const unsigned int* __restrict__ bitmap, int64_t* __restrict__ out_generated, float* __restrict__ out_log_probas,
+    int64_t* __restrict__ out_parent, int64_t* __restrict__ samples, float* __restrict__ samp_log_p, int* __restrict__ reject) {
+  extern __shared__ __align__(16) unsigned char sid_smem[];
+  const int W = blockDim.x >> 5, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int b = blockIdx.x, E = kp * nc;
+  int64_t* s_tok = reinterpret_cast<int64_t*>(sid_smem);                          // [E] candidate tokens
+  float* s_score = reinterpret_cast<float*>(s_tok + E);                          // [E] candidate scores
+  unsigned int* s_key = reinterpret_cast<unsigned int*>(s_score + E) + (size_t)w * K;                      // [W][K]
+  int* s_hist = reinterpret_cast<int*>(reinterpret_cast<unsigned int*>(s_score + E) + (size_t)W * K) + w * 256;   // [W][256]
+  unsigned int* s_sk = reinterpret_cast<unsigned int*>(s_hist - w * 256 + W * 256) + w * nc;               // [W][nc]
+  int* s_si = reinterpret_cast<int*>(s_sk - w * nc + W * nc) + w * nc;                                     // [W][nc]
+  unsigned char* s_taken = reinterpret_cast<unsigned char*>(s_si - w * nc + W * nc);                      // [E]
+  for (int beam = w; beam < kp; beam += W) {
+    const int64_t row = (int64_t)b * kp + beam;
+    const float* p = probas + row * p_stride;
+    const float* q = noise + row * n_stride;
+    bool bad = false, nonzero = false;
+    for (int i = lane; i < K; i += 32) {
+      const float pv = p[i];
+      bad |= !(pv >= 0.f) || pv == INFINITY;               // what torch.multinomial rejects: NaN, +-inf, negative ...
+      nonzero |= pv != 0.f;                                 // ... or a zero sum
+      s_key[i] = sid_topk_key(__fdiv_rn(pv, q[i]));
+    }
+    bad = __any_sync(0xffffffffu, bad);
+    nonzero = __any_sync(0xffffffffu, nonzero);
+    if (reject && lane == 0 && (bad || !nonzero)) atomicAdd(&reject[bad ? 0 : 1], 1);
+    __syncwarp();
+    sid_warp_top_n(s_key, K, nc, s_hist, s_sk, s_si, s_tok + beam * nc, lane);
+    const float plp = log_probas ? log_probas[row] : 0.f;
+    for (int r = lane; r < nc; r += 32) {
+      const int64_t tok = s_tok[beam * nc + r];
+      const float lp = logf(p[tok]);
+      if (samples) samples[row * nc + r] = tok;
+      if (samp_log_p) samp_log_p[row * nc + r] = lp;
+      s_score[beam * nc + r] = sid_extension_score(tok, generated + row * h, h, K, bitmap, lp + plp);
+      s_taken[beam * nc + r] = 0;
+    }
+  }
+  __syncthreads();
+  if (w == 0)
+    sid_keep_best(s_score, s_taken, s_tok, E, nc, b, kp, h, k, generated, out_generated, out_log_probas, out_parent, lane);
+}
+
+extern "C" int rqb200_sid_sample_select(const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride,
+                                        const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k,
+                                        int C, int K, const void* prefix_workspace, int64_t* out_generated, float* out_log_probas,
+                                        int64_t* out_parent, int64_t* samples, float* samp_log_p, int* reject, void* stream) {
+  RQB_CHECK_ARG(B >= 0 && kp > 0 && nc > 0 && h >= 0 && h < C && C <= 8 && k > 0 && K > 0 && probas_stride >= K &&
+                    noise_stride >= K, "sid_sample_select: bad argument (B=%d kp=%d nc=%d h=%d k=%d C=%d K=%d)", B, kp, nc, h, k, C, K);
+  if (nc > K || K > SID_SAMPLE_MAX_K || kp * nc > SID_BEAM_MAX_E || k > 32) {
+    rqb_set_error("sid_sample_select: need nc <= K <= %d, kp * nc <= %d, k <= 32 (nc = %d, K = %d, kp * nc = %d, k = %d)",
+                  SID_SAMPLE_MAX_K, SID_BEAM_MAX_E, nc, K, kp * nc, k);
+    return RQB_ERR_UNSUPPORTED;
+  }
+  if (B == 0) return RQB_OK;
+  RQB_CHECK_ARG(probas && noise && prefix_workspace && out_generated && out_log_probas && out_parent && (h == 0 || generated) &&
+                    (h == 0 || log_probas), "sid_sample_select: null pointer");
+  SidPrefixOffsets o{};
+  if (sid_prefix_offsets(C, K, o)) {
+    rqb_set_error("sid_sample_select: key space %d^%d exceeds the bitmap limit (2^33 bits)", K, C);
+    return RQB_ERR_UNSUPPORTED;
+  }
+  const int W = kp < SID_SAMPLE_MAX_WARPS ? kp : SID_SAMPLE_MAX_WARPS;
+  const size_t smem = sid_sample_smem(kp, nc, K);
+  RQB_CUDA(cudaFuncSetAttribute(sid_sample_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  sid_sample_select_kernel<<<B, W * 32, smem, reinterpret_cast<cudaStream_t>(stream)>>>(
+      probas, probas_stride, noise, noise_stride, generated, log_probas, kp, nc, h, k, K,
+      reinterpret_cast<const unsigned int*>(reinterpret_cast<const char*>(prefix_workspace) + o.off[h + 1]), out_generated,
+      out_log_probas, out_parent, samples, samp_log_p, reject);
   RQB_LAUNCH_CHECK();
   return RQB_OK;
 }

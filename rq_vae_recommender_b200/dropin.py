@@ -6,8 +6,9 @@
 
 ``install`` pre-seeds ``sys.modules`` so that every ``from modules.quantize import ...`` / ``from init.kmeans import
 ...`` inside the reference (train_rqvae.py:13-15, modules/tokenizer/semids.py:10, train_decoder.py:13-20) resolves to
-the replacement modules of this package; everything else (data/, modules/model.py, evaluate/, the scripts) is imported
-from the reference tree untouched.  Checkpoints pickle ``modules.quantize.Quantize`` etc. by module path,
+the replacement modules of this package; everything else (data/, evaluate/, the scripts) is imported from the reference
+tree untouched.  ``replace_model=True`` also aliases ``modules.model`` (train_decoder.py:14), whose
+``EncoderDecoderRetrievalModel.generate`` then runs its beam search on the fused sampling and selection kernel.  Checkpoints pickle ``modules.quantize.Quantize`` etc. by module path,
 so ``torch.load(..., weights_only=False)`` of the shipped files also lands on the replacement classes.
 gin-config is not in this image: a small compatible shim is registered as ``gin`` when the real one is missing.
 """
@@ -25,9 +26,10 @@ _ALIASES = {
     "distributions.gumbel": "rq_vae_recommender_b200.distributions.gumbel",
 }
 _TOKENIZER = ("modules.tokenizer.semids", "rq_vae_recommender_b200.modules.tokenizer.semids")
+_MODEL = ("modules.model", "rq_vae_recommender_b200.modules.model")
 
 
-def install(reference_root=None, replace_tokenizer=True, gin_shim=True):
+def install(reference_root=None, replace_tokenizer=True, gin_shim=True, replace_model=False):
     if gin_shim and "gin" not in sys.modules:
         try:
             import gin  # noqa: F401
@@ -44,11 +46,13 @@ def install(reference_root=None, replace_tokenizer=True, gin_shim=True):
         sys.modules[alias] = importlib.import_module(real)
     if replace_tokenizer:
         sys.modules[_TOKENIZER[0]] = importlib.import_module(_TOKENIZER[1])
-    return sorted(list(_ALIASES) + ([_TOKENIZER[0]] if replace_tokenizer else []))
+    if replace_model:
+        sys.modules[_MODEL[0]] = importlib.import_module(_MODEL[1])
+    return sorted(list(_ALIASES) + ([_TOKENIZER[0]] if replace_tokenizer else []) + ([_MODEL[0]] if replace_model else []))
 
 
 def uninstall():
-    for alias in list(_ALIASES) + [_TOKENIZER[0]]:
+    for alias in list(_ALIASES) + [_TOKENIZER[0], _MODEL[0]]:
         mod = sys.modules.get(alias)
         if mod is not None and mod.__name__.startswith("rq_vae_recommender_b200"):
             del sys.modules[alias]

@@ -1,0 +1,234 @@
+"""modules/model.py of the reference: the T5 encoder-decoder generative-retrieval model, with its constrained beam search on
+the semantic-id kernels.
+
+Same names (``EncoderDecoderRetrievalModel``, ``ModelOutput``, ``GenerationOutput``, ``_strip_dedup_col``), constructor
+signature and ``state_dict`` keys, so decoder checkpoints load with ``strict=True``.  ``forward`` and the encoder / decoder
+passes are plain torch on HF T5, as in the reference.  What differs is the search in ``generate``:
+  * ``_check_valid_prefix`` is one bit test per prefix in a bitmap index of the corpus id table (``ops.SidPrefixIndex``),
+    instead of a compare of every prefix with every corpus row.  The index is built on first use and rebuilt when the
+    ``codebooks`` buffer is replaced, written to (``load_state_dict``) or moved;
+  * each hierarchy level runs the head, the softmax, ``draw_exponential`` and ONE kernel (``SidPrefixIndex.sample_select``)
+    that samples, checks the prefixes, scores and keeps the k best.  ``torch.multinomial(p, n)`` without replacement is
+    ``topk(p / q, n)`` with ``q = draw_exponential(p)`` from the same generator, so under the same seed the samples, beams and
+    log-probabilities are the reference's.  Nothing in the level loop waits for the device: rows ``torch.multinomial`` would
+    reject are counted on the device and raise its error after the last level.
+Shapes outside the kernel's limits (codebooks above 2048 codes, top_k * 64 candidates above 1024, top_k above 32) raise
+``Rqb200Error``; there is no fallback to the reference's search.
+"""
+from typing import NamedTuple
+from typing import Optional
+
+import torch
+import torch.nn.functional as F
+from torch import nn
+from torch import Tensor
+from transformers import T5EncoderModel
+from transformers.cache_utils import DynamicCache
+from transformers.cache_utils import EncoderDecoderCache
+from transformers.models.t5.modeling_t5 import T5Config
+from transformers.models.t5.modeling_t5 import T5Stack
+
+from .. import ops
+from .._lib import Rqb200Error
+from ..data.schemas import TokenizedSeqBatch
+
+# The reference module sets this on import; the T5 passes of a script that imports this module instead run with TF32 as before.
+torch.set_float32_matmul_precision("high")
+
+MAX_CANDIDATES = 64
+_MULTINOMIAL_ERRORS = ("probability tensor contains either `inf`, `nan` or element < 0",
+                       "invalid multinomial distribution (sum of probabilities <= 0)")
+
+
+class ModelOutput(NamedTuple):
+    loss: Tensor
+    logits: Tensor
+    loss_d: Tensor
+
+
+class GenerationOutput(NamedTuple):
+    sem_ids: Tensor
+    log_probas: Tensor
+
+
+def draw_exponential(probas: Tensor) -> Tensor:
+    """The Exp(1) draw ``torch.multinomial(probas, n)`` (without replacement) makes from the default generator: sampling is
+    then ``topk(probas / draw, n)``.  Patch this function to inject noise."""
+    return torch.empty_like(probas).exponential_(1)
+
+
+def _strip_dedup_col(tensor: Tensor, sem_ids_dim: int, n_layers: int) -> Tensor:
+    """[B, N * sem_ids_dim] token rows (each item: n_layers ids + the tokenizer's dedup column) -> [B, N * n_layers]."""
+    B, width = tensor.shape
+    items = width // sem_ids_dim
+    return tensor.view(B, items, sem_ids_dim)[:, :, :n_layers].contiguous().view(B, items * n_layers)
+
+
+class EncoderDecoderRetrievalModel(nn.Module):
+    """T5 encoder over the history's semantic ids, T5 decoder stack plus one Linear head per hierarchy level for the next
+    item's ids; ``generate`` is a sampled beam search restricted to id prefixes that occur in the corpus (``codebooks``)."""
+
+    def __init__(self, codebooks: Tensor, num_hierarchies: int, num_embeddings_per_hierarchy: int, t5_d_model: int = 128,
+                 t5_num_heads: int = 6, t5_d_ff: int = 1024, t5_num_layers: int = 4, top_k_for_generation: int = 10,
+                 should_add_sep_token: bool = True, num_user_bins: Optional[int] = None):
+        super().__init__()
+        self.num_hierarchies = num_hierarchies
+        self.num_embeddings_per_hierarchy = num_embeddings_per_hierarchy
+        self.top_k_for_generation = top_k_for_generation
+        self.register_buffer("codebooks", codebooks)
+        vocab = num_embeddings_per_hierarchy * num_hierarchies
+        shape = dict(vocab_size=vocab, d_model=t5_d_model, num_heads=t5_num_heads, d_ff=t5_d_ff, num_layers=t5_num_layers)
+        self.encoder = T5EncoderModel(T5Config(**shape, is_decoder=False))
+        self.t5_decoder = T5Stack(T5Config(**shape, is_decoder=True, is_encoder_decoder=False))
+        self.bos_token = nn.Parameter(torch.randn(1, t5_d_model), requires_grad=True)
+        self.decoder_mlp = nn.ModuleList(
+            [nn.Linear(t5_d_model, num_embeddings_per_hierarchy, bias=False) for _ in range(num_hierarchies)])
+        # one table for all levels: token t of level h is row h * num_embeddings_per_hierarchy + t
+        self.item_sid_embedding_table = nn.Embedding(vocab, t5_d_model)
+        self.user_embedding = nn.Embedding(num_user_bins, t5_d_model) if num_user_bins else None
+        self.sep_token = nn.Parameter(torch.randn(1, t5_d_model), requires_grad=True) if should_add_sep_token else None
+        self._prefix_index_cache = None
+
+    @property
+    def device(self) -> torch.device:
+        return next(self.parameters()).device
+
+    # ------------------------------------------------------------------------------------------------ transformer passes
+    def _level_offsets(self, ids: Tensor, mask: Optional[Tensor] = None) -> Tensor:
+        """Column c of a [B, n] id row belongs to level c % num_hierarchies: shift it into that level's rows of the table;
+        padded positions (mask 0) become 0."""
+        if ids.ndim != 2:
+            raise ValueError("Input tensor must be 2-dimensional.")
+        level = torch.arange(ids.shape[1], device=ids.device) % self.num_hierarchies
+        out = ids + level * self.num_embeddings_per_hierarchy
+        return out if mask is None else out * mask
+
+    def _append_sep_tokens(self, emb: Tensor, mask: Tensor):
+        """Insert sep_token after every item's num_hierarchies embeddings; the separator inherits the mask of the item's last id."""
+        B, n, d = emb.shape
+        H = self.num_hierarchies
+        items = n // H
+        sep = self.sep_token.view(1, 1, 1, d).expand(B, items, 1, d)
+        emb = torch.cat([emb.view(B, items, H, d), sep], dim=2).reshape(B, items * (H + 1), d)
+        mask = mask.view(B, items, H)
+        mask = torch.cat([mask, mask[:, :, -1:]], dim=2).reshape(B, items * (H + 1))
+        return emb, mask
+
+    def encoder_forward_pass(self, attention_mask, input_ids, user_id=None):
+        inputs_embeds = self.item_sid_embedding_table(self._level_offsets(input_ids, attention_mask))
+        if self.sep_token is not None:
+            inputs_embeds, attention_mask = self._append_sep_tokens(inputs_embeds, attention_mask)
+        if user_id is not None and self.user_embedding is not None:
+            user = self.user_embedding(torch.remainder(user_id[:, 0], self.user_embedding.num_embeddings))
+            inputs_embeds = torch.cat([user.unsqueeze(1), inputs_embeds], dim=1)
+            attention_mask = torch.cat([torch.ones(attention_mask.shape[0], 1, device=attention_mask.device), attention_mask],
+                                       dim=1)
+        out = self.encoder(inputs_embeds=inputs_embeds, attention_mask=attention_mask).last_hidden_state
+        return out, attention_mask
+
+    @staticmethod
+    def _cache_holds_steps(past_key_values) -> bool:
+        if isinstance(past_key_values, (EncoderDecoderCache, DynamicCache)):
+            return len(past_key_values) > 0
+        return isinstance(past_key_values, tuple)
+
+    def decoder_forward_pass(self, attention_mask=None, future_ids=None, encoder_output=None, attention_mask_for_encoder=None,
+                             use_cache=False, past_key_values=None):
+        if future_ids is None:
+            inputs_embeds = self.bos_token.unsqueeze(0).expand(encoder_output.shape[0], 1, -1)
+        else:
+            mask = torch.ones_like(future_ids) if attention_mask is None else attention_mask
+            inputs_embeds = self.item_sid_embedding_table(self._level_offsets(future_ids, mask))
+            if self._cache_holds_steps(past_key_values):
+                inputs_embeds = inputs_embeds[:, -1:, :]          # the cache holds every earlier step
+            else:
+                B = future_ids.shape[0]
+                inputs_embeds = torch.cat([self.bos_token.unsqueeze(0).expand(B, 1, -1), inputs_embeds], dim=1)
+                if attention_mask is not None:
+                    attention_mask = torch.cat([torch.ones(B, 1, device=future_ids.device), attention_mask], dim=1)
+        out = self.t5_decoder(inputs_embeds=inputs_embeds, attention_mask=attention_mask, encoder_hidden_states=encoder_output,
+                              encoder_attention_mask=attention_mask_for_encoder, use_cache=use_cache,
+                              past_key_values=past_key_values)
+        if use_cache:
+            return out.last_hidden_state, out.past_key_values
+        return out.last_hidden_state
+
+    def forward(self, batch: TokenizedSeqBatch) -> ModelOutput:
+        H = self.num_hierarchies
+        input_ids = _strip_dedup_col(batch.sem_ids, H + 1, H)
+        attention_mask = _strip_dedup_col(batch.seq_mask.long(), H + 1, H)
+        fut_ids = batch.sem_ids_fut[:, :H]
+        enc, enc_mask = self.encoder_forward_pass(attention_mask=attention_mask, input_ids=input_ids, user_id=batch.user_ids)
+        dec = self.decoder_forward_pass(future_ids=fut_ids, encoder_output=enc, attention_mask_for_encoder=enc_mask,
+                                        use_cache=False)[:, :-1]
+        loss = torch.tensor(0.0, device=dec.device)
+        per_level = []
+        for h in range(H):
+            level_loss = F.cross_entropy(self.decoder_mlp[h](dec[:, h]), fut_ids[:, h].long())
+            loss = loss + level_loss
+            per_level.append(level_loss.detach())
+        return ModelOutput(loss=loss, logits=None, loss_d=torch.stack(per_level))
+
+    # ------------------------------------------------------------------------------------------------ constrained search
+    def _prefix_index(self, device: torch.device) -> ops.SidPrefixIndex:
+        """The corpus prefix index, built on first use and again whenever the codebooks buffer is another tensor, has been
+        written to (load_state_dict copies into it) or the search runs on another device."""
+        cb = self.codebooks
+        key = (id(cb), cb._version, cb.device, torch.device(device))
+        if self._prefix_index_cache is None or self._prefix_index_cache[0] != key:
+            index = ops.SidPrefixIndex(cb.to(device), self.num_embeddings_per_hierarchy)
+            self._prefix_index_cache = (key, index)
+        return self._prefix_index_cache[1]
+
+    def _check_valid_prefix(self, prefix: Tensor, batch_size: int = 100000) -> Tensor:
+        """bool [P]: some corpus row starts with prefix[p] (batch_size is accepted for the reference's signature)."""
+        return self._prefix_index(prefix.device).check(prefix)
+
+    def _sample_and_select(self, index: ops.SidPrefixIndex, probas: Tensor, generated: Optional[Tensor],
+                           log_probas: Optional[Tensor], k: int, n_cands: int, reject: Tensor):
+        """One level of the search after the softmax: n_cands samples per beam, prefix check, scores, the k best beams."""
+        return index.sample_select(probas, draw_exponential(probas), generated, log_probas, k, n_cands, reject=reject)
+
+    @torch.no_grad()
+    def generate(self, attention_mask, input_ids, user_id=None):
+        """Top-k semantic ids by sampled beam search: per level, n_cands = min(64, K) tokens sampled without replacement per
+        beam, scored by cumulative log-probability, prefixes absent from the corpus scored -inf, the k best kept.
+        Returns generated [B, top_k, num_hierarchies] and log_probas [B, top_k]."""
+        B = input_ids.shape[0]
+        k = self.top_k_for_generation
+        n_cands = min(MAX_CANDIDATES, self.num_embeddings_per_hierarchy)
+        if k > 32 or k * n_cands > 1024 or self.num_embeddings_per_hierarchy > 2048:
+            raise Rqb200Error(f"generate: top_k_for_generation = {k} (at most 32, and top_k * {n_cands} candidates at most 1024) "
+                              f"with {self.num_embeddings_per_hierarchy} codes per level (at most 2048) is outside the "
+                              "sampling kernel's limits")
+        enc_out, enc_mask = self.encoder_forward_pass(attention_mask=attention_mask, input_ids=input_ids, user_id=user_id)
+        index = self._prefix_index(enc_out.device)
+        rep_enc, rep_mask = enc_out.repeat_interleave(k, dim=0), enc_mask.repeat_interleave(k, dim=0)
+        reject = torch.zeros(2, dtype=torch.int32, device=enc_out.device)
+        generated, log_probas = None, None
+        past_kv = EncoderDecoderCache(DynamicCache(), DynamicCache())
+        for h in range(self.num_hierarchies):
+            first = generated is None
+            dec_out, past_kv = self.decoder_forward_pass(
+                future_ids=None if first else generated.reshape(-1, h), encoder_output=enc_out if first else rep_enc,
+                attention_mask_for_encoder=enc_mask if first else rep_mask, use_cache=True, past_key_values=past_kv)
+            probas = F.softmax(self.decoder_mlp[h](dec_out[:, -1, :]), dim=-1)
+            generated, log_probas, parent_global = self._sample_and_select(index, probas, generated, log_probas, k, n_cands,
+                                                                           reject)
+            if first:
+                past_kv = EncoderDecoderCache(DynamicCache(), DynamicCache())   # level 1 re-runs the decoder on B * k rows
+            else:
+                past_kv.reorder_cache(parent_global)
+        bad, zero_sum = reject.tolist()
+        if bad:
+            raise RuntimeError(_MULTINOMIAL_ERRORS[0])
+        if zero_sum:
+            raise RuntimeError(_MULTINOMIAL_ERRORS[1])
+        return generated, log_probas
+
+    @torch.no_grad()
+    def generate_next_sem_id(self, batch: TokenizedSeqBatch, top_k: bool = True, temperature: int = 1) -> GenerationOutput:
+        H = self.num_hierarchies
+        generated, log_probas = self.generate(attention_mask=_strip_dedup_col(batch.seq_mask.long(), H + 1, H),
+                                              input_ids=_strip_dedup_col(batch.sem_ids, H + 1, H), user_id=batch.user_ids)
+        return GenerationOutput(sem_ids=generated, log_probas=log_probas)

@@ -621,6 +621,48 @@ class SidPrefixIndex:
         _count(1)
         return out_g, out_p, out_parent
 
+    def sample_select(self, probas: torch.Tensor, noise: torch.Tensor, generated: Optional[torch.Tensor],
+                      log_probas: Optional[torch.Tensor], k: int, nc: int, want_samples: bool = False,
+                      reject: Optional[torch.Tensor] = None):
+        """The sampling step fused with ``beam_select`` (rqb200_sid_sample_select), one launch.  probas / noise [B * kp, K]
+        (kp = 1 on the first level; noise = the Exp(1) draw torch.multinomial makes, ``torch.empty_like(probas).exponential_(1)``),
+        generated [B, kp, h] or None, log_probas [B, kp] or None -> (generated [B, k, h + 1], log_probas [B, k],
+        parent_global [B * k]), plus (samples [B * kp, nc], samp_log_p [B * kp, nc]) when ``want_samples``: the samples are
+        ``torch.multinomial(probas, nc)``'s under the same generator state.  ``reject``, an int32 [2] device tensor, is ADDED the
+        number of rows torch.multinomial would reject: [0] with a NaN, +-inf or negative entry, [1] otherwise all zero."""
+        _need_cuda(probas, noise, reject)
+        lib = _lib.load()
+        if generated is None:
+            B, kp, h = probas.shape[0], 1, 0
+        else:
+            B, kp, h = generated.shape
+            generated = generated.to(torch.int64).contiguous()
+            if log_probas is None:
+                raise ValueError("log_probas is required with generated")
+            log_probas = log_probas.to(torch.float32).reshape(B, kp).contiguous()
+        probas, noise = _rows(probas), _rows(noise)
+        if probas.shape != noise.shape or probas.shape[0] != B * kp:
+            raise ValueError(f"probas {tuple(probas.shape)} / noise {tuple(noise.shape)} must both be [B * kp = {B * kp}, K]")
+        if probas.shape[1] != self.K:
+            raise ValueError(f"probas has {probas.shape[1]} codes, the prefix index {self.K}")
+        if reject is not None and (reject.dtype != torch.int32 or reject.numel() < 2 or not reject.is_contiguous()):
+            raise ValueError("reject must be a contiguous int32 tensor of 2 elements")
+        dev = probas.device
+        out_g = torch.empty((B, k, h + 1), dtype=torch.int64, device=dev)
+        out_p = torch.empty((B, k), dtype=torch.float32, device=dev)
+        out_parent = torch.empty((B * k,), dtype=torch.int64, device=dev)
+        samples = torch.empty((B * kp, nc), dtype=torch.int64, device=dev) if want_samples else None
+        samp_log_p = torch.empty((B * kp, nc), dtype=torch.float32, device=dev) if want_samples else None
+        with torch.cuda.device(dev):
+            _lib.check(lib.rqb200_sid_sample_select(_p(probas), probas.stride(0), _p(noise), noise.stride(0), _p(generated),
+                                                    _p(log_probas), B, kp, nc, h, k, self.C, self.K, _p(self.ws), _p(out_g),
+                                                    _p(out_p), _p(out_parent), _p(samples), _p(samp_log_p), _p(reject),
+                                                    _stream()), "sid_sample_select")
+        _count(1)
+        if want_samples:
+            return out_g, out_p, out_parent, samples, samp_log_p
+        return out_g, out_p, out_parent
+
 
 def sid_gather(cached_ids: torch.Tensor, item_ids: torch.Tensor, seq_mask: Optional[torch.Tensor] = None,
                want_token_type: bool = True):
