@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench_generate.py -- the sampled, prefix-constrained beam search of the generative-retrieval model.
+"""bench_generate.py -- the prefix-constrained beam searches of the generative-retrieval model, sampled and exhaustive.
 
     python bench_generate.py [--min-window-s 1.0]
 
@@ -11,9 +11,16 @@ beam, K = 256 codes, 3 hierarchy levels), on a 12 101-row corpus (Amazon Beauty'
       composed    torch.multinomial, log/gather, then SidPrefixIndex.beam_select (one kernel);
       fused       draw_exponential, then SidPrefixIndex.sample_select (one kernel);
     the reference arm is not run on the 1 M-row corpus: one chunk would need 100 000 x 1 M x l bytes of bool temporaries;
+    and two arms of the exhaustive search (generate(search="beam")) that start from the level's logits:
+      beam            SidPrefixIndex.beam_topk (one kernel);
+      beam_composed   torch: log_softmax, SidPrefixIndex.check of every extension, masked_fill, a stable descending sort,
+                      gathers;
+  * the two exhaustive arms again at top-k 32 and K = 2048 (65 536 candidates per history) on a 12 101-row corpus;
   * whole-generate ms of the drop-in EncoderDecoderRetrievalModel at the decoder_amazon.gin T5 shape (d_model 384, 6 heads,
-    d_ff 1024, 4 layers, randomly initialised) on 20-item histories, and of the same model with the composed arm in place of
-    sample_select, under the same seed (their beams are compared); three alternating windows each.
+    d_ff 1024, 4 layers, randomly initialised) on 20-item histories, of the same model with the composed arm in place of
+    sample_select, under the same seed (their beams are compared), and of generate(search="beam"); three alternating windows
+    each.  Also the fraction of returned beams with a finite log-probability under each search (of this randomly
+    initialised model: it says how often a search runs out of valid prefixes, not how good its beams are).
 Every shape is warmed up, every timed window lasts at least --min-window-s seconds (CUDA events).  Prints the card's name,
 power limit and max SM clock, and one JSON line; writes nothing.
 """
@@ -91,21 +98,53 @@ def composed_level(torch, index, probas, generated, log_probas, k, nc):
     return index.beam_select(samples, samp_log_p, generated, log_probas, k)
 
 
-def corpus_of(np, rows, seed):
+def beam_composed_level(torch, F, index, logits, generated, log_probas, k):
+    """One level of the exhaustive search in torch: log_softmax, the prefix check of every extension, masked_fill, a stable
+    descending sort and gathers."""
+    Kc = logits.shape[1]
+    Bn, kp, h = (logits.shape[0], 1, 0) if generated is None else generated.shape
+    codes = torch.arange(Kc, device=logits.device).repeat(Bn * kp).unsqueeze(1)
+    prefix = codes if h == 0 else torch.cat([generated.reshape(-1, h).repeat_interleave(Kc, dim=0), codes], dim=1)
+    scores = F.log_softmax(logits, dim=-1).reshape(Bn, kp * Kc)
+    if h:
+        scores = scores + log_probas.repeat_interleave(Kc, dim=1)
+    scores = scores.masked_fill(~index.check(prefix).reshape(Bn, kp * Kc), float("-inf"))
+    scores, idx = scores.sort(dim=-1, descending=True, stable=True)
+    top = idx[:, :k]
+    parent = top // Kc
+    new_ids = (top % Kc).unsqueeze(-1)
+    if h:
+        new_ids = torch.cat([torch.gather(generated, 1, parent.unsqueeze(-1).expand(-1, -1, h)), new_ids], dim=-1)
+    return new_ids, scores[:, :k], (parent + torch.arange(Bn, device=logits.device).unsqueeze(1) * kp).flatten()
+
+
+def corpus_of(np, rows, seed, codes=K):
     rs = np.random.RandomState(seed)
-    return rs.randint(0, K, size=(rows, H)).astype(np.int64)
+    return rs.randint(0, codes, size=(rows, H)).astype(np.int64)
 
 
 def level_inputs(torch, F, index, seed):
-    """Per level: probabilities (softmax of random logits) and the beams entering it (from the fused chain)."""
+    """Per level: probabilities (softmax of random logits), the logits, and the beams entering it (from the fused chain)."""
     g = torch.Generator(device="cuda").manual_seed(seed)
     out, generated, log_probas = [], None, None
     from rq_vae_recommender_b200.modules.model import draw_exponential
     for h in range(H):
         rows = B if h == 0 else B * TOP_K
-        probas = F.softmax(torch.randn(rows, K, device="cuda", generator=g) * 3, dim=-1)
-        out.append((probas, generated, log_probas))
+        logits = torch.randn(rows, K, device="cuda", generator=g) * 3
+        probas = F.softmax(logits, dim=-1)
+        out.append((probas, logits, generated, log_probas))
         generated, log_probas, _ = index.sample_select(probas, draw_exponential(probas), generated, log_probas, TOP_K, NC)
+    return out
+
+
+def beam_level_inputs(torch, index, k, codes, seed):
+    """Per level: random logits and the beams entering it (from the exhaustive chain)."""
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    out, generated, log_probas = [], None, None
+    for h in range(H):
+        logits = torch.randn(B if h == 0 else B * k, codes, device="cuda", generator=g) * 3
+        out.append((logits, generated, log_probas))
+        generated, log_probas, _ = index.beam_topk(logits, generated, log_probas, k)
     return out
 
 
@@ -125,15 +164,32 @@ def main():
         corpus = torch.from_numpy(corpus_of(np, rows, rows)).cuda()
         index = ops.SidPrefixIndex(corpus, K)
         res = {}
-        for h, (probas, generated, log_probas) in enumerate(level_inputs(torch, F, index, 7)):
+        for h, (probas, logits, generated, log_probas) in enumerate(level_inputs(torch, F, index, 7)):
             arms = {"composed_ms": lambda: composed_level(torch, index, probas, generated, log_probas, TOP_K, NC),
-                    "fused_ms": lambda: index.sample_select(probas, M.draw_exponential(probas), generated, log_probas, TOP_K, NC)}
+                    "fused_ms": lambda: index.sample_select(probas, M.draw_exponential(probas), generated, log_probas, TOP_K, NC),
+                    "beam_ms": lambda: index.beam_topk(logits, generated, log_probas, TOP_K),
+                    "beam_composed_ms": lambda: beam_composed_level(torch, F, index, logits, generated, log_probas, TOP_K)}
             if rows < 100000:
                 arms["reference_ms"] = lambda: reference_level(torch, corpus, probas, generated, log_probas, TOP_K, NC)
             res[f"level{h}"] = {arm: timed_ms(torch, fn, w) for arm, fn in arms.items()}
         out[name] = res
         del index, corpus
         torch.cuda.empty_cache()
+    big_k, big_codes = 32, 2048                               # 65 536 candidates per history
+    corpus = torch.from_numpy(corpus_of(np, 12101, 12101, big_codes)).cuda()
+    index = ops.SidPrefixIndex(corpus, big_codes)
+    res = {}
+    for h, (logits, generated, log_probas) in enumerate(beam_level_inputs(torch, index, big_k, big_codes, 8)):
+        want = index.beam_topk(logits, generated, log_probas, big_k)
+        got = beam_composed_level(torch, F, index, logits, generated, log_probas, big_k)
+        res[f"level{h}"] = {
+            "beam_ms": timed_ms(torch, lambda: index.beam_topk(logits, generated, log_probas, big_k), w),
+            "beam_composed_ms": timed_ms(torch, lambda: beam_composed_level(torch, F, index, logits, generated, log_probas, big_k), w),
+            "rows_with_equal_beams": float((want[0] == got[0]).reshape(B, -1).all(1).float().mean()),
+            "log_probas_max_abs_diff": float((want[1] - got[1]).nan_to_num(posinf=0, neginf=0).abs().max())}
+    out["beam_top_k32_codes2048_corpus_12101"] = res
+    del index, corpus
+    torch.cuda.empty_cache()
 
     class Composed(M.EncoderDecoderRetrievalModel):
         def _sample_and_select(self, index, probas, generated, log_probas, k, n_cands, reject):
@@ -153,15 +209,20 @@ def main():
     g_f, p_f = fused.generate(mask, ids)
     torch.manual_seed(3)
     g_c, p_c = composed.generate(mask, ids)
-    fused_ms, composed_ms = [], []
-    for _ in range(3):                                        # alternate the two models: clock drift hits both alike
+    g_b, p_b = fused.generate(mask, ids, search="beam")
+    fused_ms, composed_ms, beam_ms = [], [], []
+    for _ in range(3):                                        # alternate the models: clock drift hits all alike
         fused_ms.append(timed_ms(torch, lambda: fused.generate(mask, ids), w))
         composed_ms.append(timed_ms(torch, lambda: composed.generate(mask, ids), w))
+        beam_ms.append(timed_ms(torch, lambda: fused.generate(mask, ids, search="beam"), w))
     out["generate"] = {
-        "fused_ms": fused_ms, "composed_ms": composed_ms,
+        "fused_ms": fused_ms, "composed_ms": composed_ms, "beam_ms": beam_ms,
         "beams_equal": bool(torch.equal(g_f, g_c)), "log_probas_equal": bool(torch.equal(p_f, p_c)),
+        "finite_beam_fraction_random_init_model": {"sample": float(torch.isfinite(p_f).float().mean()),
+                                                   "beam": float(torch.isfinite(p_b).float().mean())},
         "history_items": ITEMS, "t5": "d_model 384, 6 heads, d_ff 1024, 4 layers, random init, TF32 matmuls"}
-    out["timed"] = "CUDA events, windows >= %.1f s after warm-up; per-level arms start from the level's probabilities" % w
+    out["timed"] = ("CUDA events, windows >= %.1f s after warm-up; per-level arms start from the level's probabilities (beam arms: "
+                    "its logits)" % w)
     print(out["card"])
     print(json.dumps(out))
 

@@ -215,6 +215,21 @@ int rqb200_sid_sample_select(const float* probas, int64_t probas_stride, const f
                              const void* prefix_workspace, int64_t* out_generated, float* out_log_probas, int64_t* out_parent,
                              int64_t* samples, float* samp_log_p, int* reject, void* stream);
 
+/* sid_beam_topk     : one level h of the exhaustive (deterministic) constrained beam search, from the head's logits, one launch:
+ *   logits           [B*kp, K] fp32, row stride in elements (kp = 1 at h = 0, where generated and log_probas may be null)
+ *   generated        [B, kp, h] int64, log_probas [B, kp] fp32: the beams entering the level
+ *   per row          lse = m + logf(sum expf(x - m)) in fp32 (m the row maximum, fixed reduction order)
+ *   selection        candidate e = beam * K + c of every beam and code scores (x[c] - lse) + log_probas[beam], -inf when
+ *                    generated[beam] ++ c is not a corpus prefix or the score is NaN; the k best in descending order (ties:
+ *                    lowest e) -> out_generated [B, k, h + 1], out_log_probas [B, k], out_parent [B*k] = b * kp + beam
+ *   bad              optional int[1], ADDED to (never cleared): beam rows holding a NaN or +inf logit, or whose logits are all
+ *                    -inf.  Such rows still complete; all their candidates score -inf.
+ *   limits           K <= 2048, k <= 32, k <= K, kp <= 32, h < C <= 8, K^C within the prefix bitmap limit; RQB_ERR_UNSUPPORTED
+ *                    otherwise.  B = 0 is a no-op.  Deterministic: no result depends on the order of atomics. */
+int rqb200_sid_beam_topk(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas, int B,
+                         int kp, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
+                         float* out_log_probas, int64_t* out_parent, int* bad, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

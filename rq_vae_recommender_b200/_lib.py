@@ -70,6 +70,8 @@ _SIGNATURES = {
                                        c_vp, c_vp, c_vp]),
     "rqb200_sid_sample_select": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
                                          c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "rqb200_sid_beam_topk": (c_int, [c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp,
+                                     c_vp, c_vp]),
     "rqb200_bf16_image_bytes": (c_size, [c_int, c_int]),
     "rqb200_f32_to_bf16_image": (c_int, [c_vp, c_i64, c_int, c_int, c_vp, c_vp]),
     "rqb200_gemm_bf16": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_i64, c_vp]),

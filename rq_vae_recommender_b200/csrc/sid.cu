@@ -543,3 +543,190 @@ extern "C" int rqb200_sid_sample_select(const float* probas, int64_t probas_stri
   RQB_LAUNCH_CHECK();
   return RQB_OK;
 }
+
+// ---------------------------------------------------------------------------------------------------------------------
+// One level of the exhaustive constrained beam search, from the head's logits, in one launch: every code of every beam is a
+// candidate.  Per beam row lse = m + logf(sum expf(x - m)) in a fixed reduction order; candidate e = beam * K + c scores
+// (x[c] - lse) + log_probas[beam], -inf when the extended prefix is not in the corpus or the score is NaN
+// (sid_extension_score); the k largest are kept in descending order, equal scores by ascending e (sid_keep_best's rule).
+// One CTA per batch row.  A candidate's order key is the sid_topk_key image of its score (-0 folded into +0) above the 16 bits
+// 0xffff - e, so the E = kp * K <= 65 536 keys of a row are distinct and "the k largest keys" is exactly that order.  A
+// block-wide radix selection (8-bit digits; it stops once the bin of the chosen digit holds exactly the entries still wanted)
+// finds the smallest kept key, the k keys at or above it are collected and each is ranked among them.  The histograms are
+// integer counts and the ranks compare distinct keys: no result depends on the order of atomics.  The 32-bit score keys stay
+// in shared memory when E <= SID_TOPK_SMEM_KEYS; above that every pass recomputes them from the logits.  The score is written
+// with explicit roundings (no contraction), so a recomputed key has the same bits as the first.
+#define SID_TOPK_MAX_K 2048
+#define SID_TOPK_MAX_BEAMS 32
+#define SID_TOPK_MAX_THREADS 512
+#define SID_TOPK_SMEM_KEYS (48 * 1024)
+
+struct SidTopkShared {
+  int hist[256];
+  int ctl[3];                                               // chosen digit, entries above its bin, entries in its bin
+  int nsel;
+  float lse[SID_TOPK_MAX_BEAMS];
+  float plp[SID_TOPK_MAX_BEAMS];
+  int64_t gen[SID_TOPK_MAX_BEAMS * 7];                      // the beams' ids, [kp][h], h < C <= 8
+  unsigned long long sel[32];
+};
+
+// candidate e's 32-bit score key
+__device__ __forceinline__ unsigned int sid_topk_candidate(const float* __restrict__ logits, int64_t ld, int64_t row0, int K, int h,
+                                                           int e, const SidTopkShared& s, const unsigned int* __restrict__ bitmap) {
+  const int beam = e / K, c = e - beam * K;
+  const float lp = __fadd_rn(__fsub_rn(logits[(row0 + beam) * ld + c], s.lse[beam]), s.plp[beam]);
+  const float sc = sid_extension_score(c, s.gen + beam * h, h, K, bitmap, lp);
+  return sid_topk_key(sc == 0.f ? 0.f : sc);
+}
+
+template <bool KEYS_IN_SMEM>
+__global__ void __launch_bounds__(SID_TOPK_MAX_THREADS) sid_beam_topk_kernel(
+    const float* __restrict__ logits, int64_t ld, const int64_t* __restrict__ generated, const float* __restrict__ log_probas,
+    int kp, int h, int k, int K, const unsigned int* __restrict__ bitmap, int64_t* __restrict__ out_generated,
+    float* __restrict__ out_log_probas, int64_t* __restrict__ out_parent, int* __restrict__ bad) {
+  extern __shared__ __align__(16) unsigned char sid_smem[];
+  __shared__ SidTopkShared s;
+  unsigned int* s_key = reinterpret_cast<unsigned int*>(sid_smem);                // [E] when KEYS_IN_SMEM
+  const int nt = blockDim.x, W = nt >> 5, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const unsigned int lt = (1u << lane) - 1u;
+  const int b = blockIdx.x, E = kp * K;
+  const int64_t row0 = (int64_t)b * kp;
+  for (int i = threadIdx.x; i < 256; i += nt) s.hist[i] = 0;
+  for (int i = threadIdx.x; i < kp * h; i += nt) s.gen[i] = generated[row0 * h + i];
+  if (threadIdx.x == 0) s.nsel = 0;
+  for (int beam = w; beam < kp; beam += W) {                // warp per beam: row maximum, then log-sum-exp
+    const float* x = logits + (row0 + beam) * ld;
+    float m = -INFINITY;
+    bool odd = false;
+    for (int c = lane; c < K; c += 32) {
+      const float v = x[c];
+      m = fmaxf(m, v);
+      odd |= v != v || v == INFINITY;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    odd = __any_sync(0xffffffffu, odd);
+    float sum = 0.f;
+    for (int c = lane; c < K; c += 32) sum += expf(x[c] - m);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);   // every lane ends with the same bits
+    if (lane == 0) {
+      s.lse[beam] = m + logf(sum);                          // NaN for a row with NaN or +inf, or all -inf: its scores are -inf
+      s.plp[beam] = log_probas ? log_probas[row0 + beam] : 0.f;
+      if (bad && (odd || m == -INFINITY)) atomicAdd(bad, 1);
+    }
+  }
+  __syncthreads();
+  unsigned long long prefix = 0, pmask = 0;
+  int want = k;                                             // entries still needed among those matching the decided digits
+  for (int shift = 40; shift >= 0; shift -= 8) {
+    for (int base = 0; base < E; base += nt) {
+      const int e = base + threadIdx.x;
+      int d = 256;
+      if (e < E) {
+        unsigned int key;
+        if (KEYS_IN_SMEM) {
+          if (shift == 40) s_key[e] = key = sid_topk_candidate(logits, ld, row0, K, h, e, s, bitmap);
+          else key = s_key[e];
+        } else {
+          key = sid_topk_candidate(logits, ld, row0, K, h, e, s, bitmap);
+        }
+        const unsigned long long v = ((unsigned long long)key << 16) | (unsigned int)(0xffff - e);
+        if ((v & pmask) == prefix) d = (int)((v >> shift) & 255u);
+      }
+      const unsigned int same = __match_any_sync(0xffffffffu, d);
+      if (d < 256 && (same & lt) == 0) atomicAdd(&s.hist[d], __popc(same));   // one add per distinct digit of the warp
+    }
+    __syncthreads();
+    if (w == 0) {
+      int c[8], sum = 0;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        c[j] = s.hist[lane * 8 + j];
+        s.hist[lane * 8 + j] = 0;                           // cleared for the next pass
+        sum += c[j];
+      }
+      int suf = sum;                                        // entries in bins >= lane * 8
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_down_sync(0xffffffffu, suf, o);
+        if (lane + o < 32) suf += t;
+      }
+      const int owner = 31 - __clz(__ballot_sync(0xffffffffu, suf >= want));
+      if (lane == owner) {
+        int acc = suf - sum;
+        for (int j = 7; j >= 0; --j) {
+          if (acc + c[j] >= want) {
+            s.ctl[0] = lane * 8 + j;
+            s.ctl[1] = acc;
+            s.ctl[2] = c[j];
+            break;
+          }
+          acc += c[j];
+        }
+      }
+    }
+    __syncthreads();
+    want -= s.ctl[1];
+    prefix |= (unsigned long long)s.ctl[0] << shift;
+    pmask |= 255ull << shift;
+    if (s.ctl[2] == want) break;                            // the whole bin is kept: the threshold is decided
+  }
+  // the kept set: keys whose decided digits are above the prefix (k - want of them) or equal to it (want of them)
+  for (int e = threadIdx.x; e < E; e += nt) {
+    const unsigned int key = KEYS_IN_SMEM ? s_key[e] : sid_topk_candidate(logits, ld, row0, K, h, e, s, bitmap);
+    const unsigned long long v = ((unsigned long long)key << 16) | (unsigned int)(0xffff - e);
+    if ((v & pmask) >= prefix) s.sel[atomicAdd(&s.nsel, 1)] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x < k) {
+    const unsigned long long v = s.sel[threadIdx.x];
+    int r = 0;
+    for (int q = 0; q < k; ++q) r += s.sel[q] > v;
+    const unsigned int key = (unsigned int)(v >> 16);
+    const int e = 0xffff - (int)(v & 0xffffu);
+    const int beam = e / K;
+    const int64_t o = (int64_t)b * k + r;
+    out_log_probas[o] = __uint_as_float((key & 0x80000000u) ? key ^ 0x80000000u : ~key);   // sid_topk_key inverted
+    out_parent[o] = row0 + beam;
+    int64_t* g = out_generated + o * (h + 1);
+    for (int j = 0; j < h; ++j) g[j] = s.gen[beam * h + j];
+    g[h] = e - beam * K;
+  }
+}
+
+extern "C" int rqb200_sid_beam_topk(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas,
+                                    int B, int kp, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
+                                    float* out_log_probas, int64_t* out_parent, int* bad, void* stream) {
+  RQB_CHECK_ARG(B >= 0 && kp > 0 && h >= 0 && h < C && C <= 8 && k > 0 && K > 0 && logits_stride >= K,
+                "sid_beam_topk: bad argument (B=%d kp=%d h=%d k=%d C=%d K=%d)", B, kp, h, k, C, K);
+  if (K > SID_TOPK_MAX_K || k > 32 || k > K || kp > SID_TOPK_MAX_BEAMS) {
+    rqb_set_error("sid_beam_topk: need K <= %d, k <= 32, k <= K, kp <= %d (K = %d, k = %d, kp = %d)", SID_TOPK_MAX_K,
+                  SID_TOPK_MAX_BEAMS, K, k, kp);
+    return RQB_ERR_UNSUPPORTED;
+  }
+  if (B == 0) return RQB_OK;
+  RQB_CHECK_ARG(logits && prefix_workspace && out_generated && out_log_probas && out_parent && (h == 0 || generated) &&
+                    (h == 0 || log_probas), "sid_beam_topk: null pointer");
+  SidPrefixOffsets o{};
+  if (sid_prefix_offsets(C, K, o)) {
+    rqb_set_error("sid_beam_topk: key space %d^%d exceeds the bitmap limit (2^33 bits)", K, C);
+    return RQB_ERR_UNSUPPORTED;
+  }
+  const int E = kp * K;
+  const int nt = E >= 4096 ? SID_TOPK_MAX_THREADS : E >= 1024 ? 256 : 128;
+  const unsigned int* bitmap = reinterpret_cast<const unsigned int*>(reinterpret_cast<const char*>(prefix_workspace) + o.off[h + 1]);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (E <= SID_TOPK_SMEM_KEYS) {
+    const size_t smem = (size_t)E * sizeof(unsigned int);
+    RQB_CUDA(cudaFuncSetAttribute(sid_beam_topk_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    sid_beam_topk_kernel<true><<<B, nt, smem, st>>>(logits, logits_stride, generated, log_probas, kp, h, k, K, bitmap,
+                                                    out_generated, out_log_probas, out_parent, bad);
+  } else {
+    sid_beam_topk_kernel<false><<<B, nt, 0, st>>>(logits, logits_stride, generated, log_probas, kp, h, k, K, bitmap,
+                                                  out_generated, out_log_probas, out_parent, bad);
+  }
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
+}

@@ -8,7 +8,9 @@
 ...`` inside the reference (train_rqvae.py:13-15, modules/tokenizer/semids.py:10, train_decoder.py:13-20) resolves to
 the replacement modules of this package; everything else (data/, evaluate/, the scripts) is imported from the reference
 tree untouched.  ``replace_model=True`` also aliases ``modules.model`` (train_decoder.py:14), whose
-``EncoderDecoderRetrievalModel.generate`` then runs its beam search on the fused sampling and selection kernel.  Checkpoints pickle ``modules.quantize.Quantize`` etc. by module path,
+``EncoderDecoderRetrievalModel.generate`` then runs its beam search on the fused sampling and selection kernel;
+``search="beam"`` (with ``replace_model=True``) makes the exhaustive, deterministic beam search over every code its default, so
+an unmodified ``train_decoder.py`` evaluates with it.  Checkpoints pickle ``modules.quantize.Quantize`` etc. by module path,
 so ``torch.load(..., weights_only=False)`` of the shipped files also lands on the replacement classes.
 gin-config is not in this image: a small compatible shim is registered as ``gin`` when the real one is missing.
 """
@@ -29,7 +31,11 @@ _TOKENIZER = ("modules.tokenizer.semids", "rq_vae_recommender_b200.modules.token
 _MODEL = ("modules.model", "rq_vae_recommender_b200.modules.model")
 
 
-def install(reference_root=None, replace_tokenizer=True, gin_shim=True, replace_model=False):
+def install(reference_root=None, replace_tokenizer=True, gin_shim=True, replace_model=False, search="sample"):
+    if search not in ("sample", "beam"):
+        raise ValueError(f"search must be 'sample' or 'beam', got {search!r}")
+    if search != "sample" and not replace_model:
+        raise ValueError(f"search={search!r} selects the replacement model's search: it needs replace_model=True")
     if gin_shim and "gin" not in sys.modules:
         try:
             import gin  # noqa: F401
@@ -48,6 +54,7 @@ def install(reference_root=None, replace_tokenizer=True, gin_shim=True, replace_
         sys.modules[_TOKENIZER[0]] = importlib.import_module(_TOKENIZER[1])
     if replace_model:
         sys.modules[_MODEL[0]] = importlib.import_module(_MODEL[1])
+        sys.modules[_MODEL[0]].DEFAULT_SEARCH = search
     return sorted(list(_ALIASES) + ([_TOKENIZER[0]] if replace_tokenizer else []) + ([_MODEL[0]] if replace_model else []))
 
 
@@ -56,3 +63,6 @@ def uninstall():
         mod = sys.modules.get(alias)
         if mod is not None and mod.__name__.startswith("rq_vae_recommender_b200"):
             del sys.modules[alias]
+    model = sys.modules.get(_MODEL[1])
+    if model is not None:
+        model.DEFAULT_SEARCH = "sample"

@@ -14,6 +14,11 @@ passes are plain torch on HF T5, as in the reference.  What differs is the searc
     reject are counted on the device and raise its error after the last level.
 Shapes outside the kernel's limits (codebooks above 2048 codes, top_k * 64 candidates above 1024, top_k above 32) raise
 ``Rqb200Error``; there is no fallback to the reference's search.
+
+``generate(..., search="beam")`` runs a different search instead: an exhaustive, deterministic beam search over every code
+(``SidPrefixIndex.beam_topk``: per level the head and ONE kernel that scores all top_k x K extensions by log_softmax plus the
+parent's log-probability and keeps the k best valid ones; no sampling, no draw from any generator).  ``DEFAULT_SEARCH`` picks the
+search when ``generate`` / ``generate_next_sem_id`` are not given one (``dropin.install(search=...)`` sets it).
 """
 from typing import NamedTuple
 from typing import Optional
@@ -36,6 +41,9 @@ from ..data.schemas import TokenizedSeqBatch
 torch.set_float32_matmul_precision("high")
 
 MAX_CANDIDATES = 64
+#: the search generate() runs when it is not given one: "sample" (the reference's sampled beam search) or "beam" (exhaustive)
+DEFAULT_SEARCH = "sample"
+SEARCHES = ("sample", "beam")
 _MULTINOMIAL_ERRORS = ("probability tensor contains either `inf`, `nan` or element < 0",
                        "invalid multinomial distribution (sum of probabilities <= 0)")
 
@@ -189,22 +197,37 @@ class EncoderDecoderRetrievalModel(nn.Module):
         """One level of the search after the softmax: n_cands samples per beam, prefix check, scores, the k best beams."""
         return index.sample_select(probas, draw_exponential(probas), generated, log_probas, k, n_cands, reject=reject)
 
+    def _check_search_limits(self, search: str, k: int, n_cands: int) -> None:
+        K = self.num_embeddings_per_hierarchy
+        if search == "sample":
+            if k > 32 or k * n_cands > 1024 or K > 2048:
+                raise Rqb200Error(f"generate: top_k_for_generation = {k} (at most 32, and top_k * {n_cands} candidates at most "
+                                  f"1024) with {K} codes per level (at most 2048) is outside the sampling kernel's limits")
+        elif search == "beam":
+            if k > 32 or k > K or K > 2048:
+                raise Rqb200Error(f"generate: top_k_for_generation = {k} (at most 32 and at most the number of codes) with {K} "
+                                  "codes per level (at most 2048) is outside the beam search kernel's limits")
+        else:
+            raise ValueError(f"generate: search must be one of {SEARCHES}, got {search!r}")
+
     @torch.no_grad()
-    def generate(self, attention_mask, input_ids, user_id=None):
-        """Top-k semantic ids by sampled beam search: per level, n_cands = min(64, K) tokens sampled without replacement per
-        beam, scored by cumulative log-probability, prefixes absent from the corpus scored -inf, the k best kept.
+    def generate(self, attention_mask, input_ids, user_id=None, search: Optional[str] = None):
+        """Top-k semantic ids by beam search restricted to id prefixes of the corpus.  ``search`` (default: the module's
+        ``DEFAULT_SEARCH``, read at call time):
+          "sample"  per level, n_cands = min(64, K) tokens sampled without replacement per beam, scored by cumulative
+                    log-probability, prefixes absent from the corpus scored -inf, the k best kept (the reference's search);
+          "beam"    per level, every code of every beam scored by cumulative log-probability, the k best valid extensions kept
+                    (equal scores: lowest beam * K + code first); deterministic, draws no random numbers.
         Returns generated [B, top_k, num_hierarchies] and log_probas [B, top_k]."""
-        B = input_ids.shape[0]
+        search = DEFAULT_SEARCH if search is None else search
         k = self.top_k_for_generation
         n_cands = min(MAX_CANDIDATES, self.num_embeddings_per_hierarchy)
-        if k > 32 or k * n_cands > 1024 or self.num_embeddings_per_hierarchy > 2048:
-            raise Rqb200Error(f"generate: top_k_for_generation = {k} (at most 32, and top_k * {n_cands} candidates at most 1024) "
-                              f"with {self.num_embeddings_per_hierarchy} codes per level (at most 2048) is outside the "
-                              "sampling kernel's limits")
+        self._check_search_limits(search, k, n_cands)
+        beam = search == "beam"
         enc_out, enc_mask = self.encoder_forward_pass(attention_mask=attention_mask, input_ids=input_ids, user_id=user_id)
         index = self._prefix_index(enc_out.device)
         rep_enc, rep_mask = enc_out.repeat_interleave(k, dim=0), enc_mask.repeat_interleave(k, dim=0)
-        reject = torch.zeros(2, dtype=torch.int32, device=enc_out.device)
+        reject = torch.zeros(1 if beam else 2, dtype=torch.int32, device=enc_out.device)
         generated, log_probas = None, None
         past_kv = EncoderDecoderCache(DynamicCache(), DynamicCache())
         for h in range(self.num_hierarchies):
@@ -212,13 +235,22 @@ class EncoderDecoderRetrievalModel(nn.Module):
             dec_out, past_kv = self.decoder_forward_pass(
                 future_ids=None if first else generated.reshape(-1, h), encoder_output=enc_out if first else rep_enc,
                 attention_mask_for_encoder=enc_mask if first else rep_mask, use_cache=True, past_key_values=past_kv)
-            probas = F.softmax(self.decoder_mlp[h](dec_out[:, -1, :]), dim=-1)
-            generated, log_probas, parent_global = self._sample_and_select(index, probas, generated, log_probas, k, n_cands,
-                                                                           reject)
+            logits = self.decoder_mlp[h](dec_out[:, -1, :])
+            if beam:
+                generated, log_probas, parent_global = index.beam_topk(logits, generated, log_probas, k, bad=reject)
+            else:
+                generated, log_probas, parent_global = self._sample_and_select(index, F.softmax(logits, dim=-1), generated,
+                                                                               log_probas, k, n_cands, reject)
             if first:
                 past_kv = EncoderDecoderCache(DynamicCache(), DynamicCache())   # level 1 re-runs the decoder on B * k rows
             else:
                 past_kv.reorder_cache(parent_global)
+        if beam:
+            n_bad = int(reject[0])
+            if n_bad:
+                raise RuntimeError(f"generate: {n_bad} beam row(s) of the decoder head's logits hold a NaN or +inf or are all "
+                                   "-inf; the beam search cannot rank them")
+            return generated, log_probas
         bad, zero_sum = reject.tolist()
         if bad:
             raise RuntimeError(_MULTINOMIAL_ERRORS[0])
@@ -227,8 +259,10 @@ class EncoderDecoderRetrievalModel(nn.Module):
         return generated, log_probas
 
     @torch.no_grad()
-    def generate_next_sem_id(self, batch: TokenizedSeqBatch, top_k: bool = True, temperature: int = 1) -> GenerationOutput:
+    def generate_next_sem_id(self, batch: TokenizedSeqBatch, top_k: bool = True, temperature: int = 1,
+                             search: Optional[str] = None) -> GenerationOutput:
         H = self.num_hierarchies
         generated, log_probas = self.generate(attention_mask=_strip_dedup_col(batch.seq_mask.long(), H + 1, H),
-                                              input_ids=_strip_dedup_col(batch.sem_ids, H + 1, H), user_id=batch.user_ids)
+                                              input_ids=_strip_dedup_col(batch.sem_ids, H + 1, H), user_id=batch.user_ids,
+                                              search=search)
         return GenerationOutput(sem_ids=generated, log_probas=log_probas)

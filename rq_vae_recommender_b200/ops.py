@@ -663,6 +663,42 @@ class SidPrefixIndex:
             return out_g, out_p, out_parent, samples, samp_log_p
         return out_g, out_p, out_parent
 
+    def beam_topk(self, logits: torch.Tensor, generated: Optional[torch.Tensor], log_probas: Optional[torch.Tensor], k: int,
+                  bad: Optional[torch.Tensor] = None):
+        """One level of the exhaustive constrained beam search from the head's logits (rqb200_sid_beam_topk), one launch.
+        logits [B * kp, K] (kp = 1 on the first level), generated [B, kp, h] or None, log_probas [B, kp] or None ->
+        (generated [B, k, h + 1], log_probas [B, k], parent_global [B * k]): of all kp * K extensions of each history, scored
+        log_softmax(logits)[code] + the parent's log-probability (-inf when the extended prefix is not in the corpus), the k
+        best in descending order, equal scores by ascending beam * K + code.  Deterministic.  ``bad``, an int32 device tensor,
+        is ADDED the number of beam rows whose logits hold a NaN or +inf or are all -inf."""
+        _need_cuda(logits, bad)
+        lib = _lib.load()
+        if generated is None:
+            B, kp, h = logits.shape[0], 1, 0
+        else:
+            B, kp, h = generated.shape
+            generated = generated.to(torch.int64).contiguous()
+            if log_probas is None:
+                raise ValueError("log_probas is required with generated")
+            log_probas = log_probas.to(torch.float32).reshape(B, kp).contiguous()
+        logits = _rows(logits)
+        if logits.shape[0] != B * kp:
+            raise ValueError(f"logits {tuple(logits.shape)} must be [B * kp = {B * kp}, K]")
+        if logits.shape[1] != self.K:
+            raise ValueError(f"logits has {logits.shape[1]} codes, the prefix index {self.K}")
+        if bad is not None and (bad.dtype != torch.int32 or bad.numel() < 1 or not bad.is_contiguous()):
+            raise ValueError("bad must be a contiguous int32 tensor")
+        dev = logits.device
+        out_g = torch.empty((B, k, h + 1), dtype=torch.int64, device=dev)
+        out_p = torch.empty((B, k), dtype=torch.float32, device=dev)
+        out_parent = torch.empty((B * k,), dtype=torch.int64, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(lib.rqb200_sid_beam_topk(_p(logits), logits.stride(0), _p(generated), _p(log_probas), B, kp, h, k, self.C,
+                                                self.K, _p(self.ws), _p(out_g), _p(out_p), _p(out_parent), _p(bad), _stream()),
+                       "sid_beam_topk")
+        _count(1)
+        return out_g, out_p, out_parent
+
 
 def sid_gather(cached_ids: torch.Tensor, item_ids: torch.Tensor, seq_mask: Optional[torch.Tensor] = None,
                want_token_type: bool = True):
