@@ -16,10 +16,17 @@ beam, K = 256 codes, 3 hierarchy levels), on a 12 101-row corpus (Amazon Beauty'
       beam_composed   torch: log_softmax, SidPrefixIndex.check of every extension, masked_fill, a stable descending sort,
                       gathers;
   * the two exhaustive arms again at top-k 32 and K = 2048 (65 536 candidates per history) on a 12 101-row corpus;
+  * the corpus prefix index: build ms and device bytes of the bitmap and of the trie (ops.SidPrefixIndex(kind=...)) on a
+    12 101-row corpus at K = 256, C = 3 (the shipped shape), K = 2048, C = 3 (1 GiB of bitmap) and K = 256, C = 4 (512 MiB);
+    and the fused and beam arms above again on the trie of the same corpora (fused_trie_ms, beam_trie_ms);
+  * per-level ms of sample_select (top-k 10, 64 candidates) and beam_topk (top-k 10) on the trie alone, where no bitmap fits:
+    K = 256 with C = 5 and 8, K = 1024 and 2048 with C = 4, and beam_topk at top-k 32 with K = 2048, C = 4 (65 536
+    candidates per history), each on a 12 101-row corpus;
   * whole-generate ms of the drop-in EncoderDecoderRetrievalModel at the decoder_amazon.gin T5 shape (d_model 384, 6 heads,
     d_ff 1024, 4 layers, randomly initialised) on 20-item histories, of the same model with the composed arm in place of
     sample_select, under the same seed (their beams are compared), and of generate(search="beam"); three alternating windows
-    each.  Also the fraction of returned beams with a finite log-probability under each search (of this randomly
+    each; and generate(search="sample") and generate(search="beam") of the same T5 shape with 5 hierarchy levels at K = 256 (on
+    the trie).  Also the fraction of returned beams with a finite log-probability under each search (of this randomly
     initialised model: it says how often a search runs out of valid prefixes, not how good its beams are).
 Every shape is warmed up, every timed window lasts at least --min-window-s seconds (CUDA events).  Prints the card's name,
 power limit and max SM clock, and one JSON line; writes nothing.
@@ -118,34 +125,50 @@ def beam_composed_level(torch, F, index, logits, generated, log_probas, k):
     return new_ids, scores[:, :k], (parent + torch.arange(Bn, device=logits.device).unsqueeze(1) * kp).flatten()
 
 
-def corpus_of(np, rows, seed, codes=K):
+def corpus_of(np, rows, seed, codes=K, levels=H):
     rs = np.random.RandomState(seed)
-    return rs.randint(0, codes, size=(rows, H)).astype(np.int64)
+    return rs.randint(0, codes, size=(rows, levels)).astype(np.int64)
 
 
-def level_inputs(torch, F, index, seed):
+def level_inputs(torch, F, index, seed, codes=K, levels=H):
     """Per level: probabilities (softmax of random logits), the logits, and the beams entering it (from the fused chain)."""
     g = torch.Generator(device="cuda").manual_seed(seed)
     out, generated, log_probas = [], None, None
     from rq_vae_recommender_b200.modules.model import draw_exponential
-    for h in range(H):
+    for h in range(levels):
         rows = B if h == 0 else B * TOP_K
-        logits = torch.randn(rows, K, device="cuda", generator=g) * 3
+        logits = torch.randn(rows, codes, device="cuda", generator=g) * 3
         probas = F.softmax(logits, dim=-1)
         out.append((probas, logits, generated, log_probas))
         generated, log_probas, _ = index.sample_select(probas, draw_exponential(probas), generated, log_probas, TOP_K, NC)
     return out
 
 
-def beam_level_inputs(torch, index, k, codes, seed):
+def beam_level_inputs(torch, index, k, codes, seed, levels=H):
     """Per level: random logits and the beams entering it (from the exhaustive chain)."""
     g = torch.Generator(device="cuda").manual_seed(seed)
     out, generated, log_probas = [], None, None
-    for h in range(H):
+    for h in range(levels):
         logits = torch.randn(B if h == 0 else B * k, codes, device="cuda", generator=g) * 3
         out.append((logits, generated, log_probas))
         generated, log_probas, _ = index.beam_topk(logits, generated, log_probas, k)
     return out
+
+
+def build_ms(torch, ops, corpus, codes, kind, reps=5):
+    """Median ms of building the prefix index (host clock around the build and a device synchronise), and its bytes."""
+    import time
+    times = []
+    for _ in range(reps + 1):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        index = ops.SidPrefixIndex(corpus, codes, kind=kind)
+        torch.cuda.synchronize()
+        times.append((time.perf_counter() - t0) * 1e3)
+        nbytes = index.nbytes
+        del index
+    times = sorted(times[1:])                                  # the first build loads the module
+    return {"build_ms": times[len(times) // 2], "bytes": nbytes}
 
 
 def main():
@@ -163,17 +186,20 @@ def main():
     for name, rows in (("corpus_12101", 12101), ("corpus_1M", 1 << 20)):
         corpus = torch.from_numpy(corpus_of(np, rows, rows)).cuda()
         index = ops.SidPrefixIndex(corpus, K)
+        trie = ops.SidPrefixIndex(corpus, K, kind="trie")
         res = {}
         for h, (probas, logits, generated, log_probas) in enumerate(level_inputs(torch, F, index, 7)):
             arms = {"composed_ms": lambda: composed_level(torch, index, probas, generated, log_probas, TOP_K, NC),
                     "fused_ms": lambda: index.sample_select(probas, M.draw_exponential(probas), generated, log_probas, TOP_K, NC),
+                    "fused_trie_ms": lambda: trie.sample_select(probas, M.draw_exponential(probas), generated, log_probas, TOP_K, NC),
                     "beam_ms": lambda: index.beam_topk(logits, generated, log_probas, TOP_K),
+                    "beam_trie_ms": lambda: trie.beam_topk(logits, generated, log_probas, TOP_K),
                     "beam_composed_ms": lambda: beam_composed_level(torch, F, index, logits, generated, log_probas, TOP_K)}
             if rows < 100000:
                 arms["reference_ms"] = lambda: reference_level(torch, corpus, probas, generated, log_probas, TOP_K, NC)
             res[f"level{h}"] = {arm: timed_ms(torch, fn, w) for arm, fn in arms.items()}
         out[name] = res
-        del index, corpus
+        del index, trie, corpus
         torch.cuda.empty_cache()
     big_k, big_codes = 32, 2048                               # 65 536 candidates per history
     corpus = torch.from_numpy(corpus_of(np, 12101, 12101, big_codes)).cuda()
@@ -190,6 +216,30 @@ def main():
     out["beam_top_k32_codes2048_corpus_12101"] = res
     del index, corpus
     torch.cuda.empty_cache()
+    builds = {}
+    for codes, levels in ((K, 3), (2048, 3), (K, 4)):
+        corpus = torch.from_numpy(corpus_of(np, 12101, 12101, codes, levels)).cuda()
+        builds[f"codes{codes}_levels{levels}"] = {kind: build_ms(torch, ops, corpus, codes, kind) for kind in ("bitmap", "trie")}
+        torch.cuda.empty_cache()
+    out["index_build_corpus_12101"] = builds
+    deep = {}
+    for codes, levels in ((K, 5), (K, 8), (1024, 4), (2048, 4)):
+        corpus = torch.from_numpy(corpus_of(np, 12101, 12101, codes, levels)).cuda()
+        trie = ops.SidPrefixIndex(corpus, codes)
+        assert trie.kind == "trie"
+        res = {}
+        for h, (probas, logits, generated, log_probas) in enumerate(level_inputs(torch, F, trie, 9, codes, levels)):
+            res[f"level{h}"] = {
+                "fused_ms": timed_ms(torch, lambda: trie.sample_select(probas, M.draw_exponential(probas), generated, log_probas,
+                                                                       TOP_K, NC), w),
+                "beam_ms": timed_ms(torch, lambda: trie.beam_topk(logits, generated, log_probas, TOP_K), w)}
+        if codes == 2048:
+            for h, (logits, generated, log_probas) in enumerate(beam_level_inputs(torch, trie, big_k, codes, 10, levels)):
+                res[f"level{h}"]["beam_top_k32_ms"] = timed_ms(torch, lambda: trie.beam_topk(logits, generated, log_probas, big_k), w)
+        deep[f"codes{codes}_levels{levels}"] = res
+        del trie, corpus
+        torch.cuda.empty_cache()
+    out["trie_corpus_12101"] = deep
 
     class Composed(M.EncoderDecoderRetrievalModel):
         def _sample_and_select(self, index, probas, generated, log_probas, k, n_cands, reject):
@@ -221,6 +271,23 @@ def main():
         "finite_beam_fraction_random_init_model": {"sample": float(torch.isfinite(p_f).float().mean()),
                                                    "beam": float(torch.isfinite(p_b).float().mean())},
         "history_items": ITEMS, "t5": "d_model 384, 6 heads, d_ff 1024, 4 layers, random init, TF32 matmuls"}
+    del fused, composed
+    deep_h = 5                                                # no bitmap fits K^5: the model builds the trie
+    corpus5 = torch.from_numpy(corpus_of(np, 12101, 12101, K, deep_h))
+    torch.manual_seed(0)
+    model5 = M.EncoderDecoderRetrievalModel(codebooks=corpus5, **dict(shape, num_hierarchies=deep_h)).cuda().eval()
+    ids5 = torch.from_numpy(rs.randint(0, K, size=(B, ITEMS * deep_h))).cuda()
+    mask5 = torch.ones_like(ids5)
+    g_s5, p_s5 = model5.generate(mask5, ids5)
+    g_b5, p_b5 = model5.generate(mask5, ids5, search="beam")
+    sample5, beam5 = [], []
+    for _ in range(3):
+        sample5.append(timed_ms(torch, lambda: model5.generate(mask5, ids5), w))
+        beam5.append(timed_ms(torch, lambda: model5.generate(mask5, ids5, search="beam"), w))
+    out["generate_levels5"] = {
+        "index": model5._prefix_index(torch.device("cuda")).kind, "sample_ms": sample5, "beam_ms": beam5,
+        "finite_beam_fraction_random_init_model": {"sample": float(torch.isfinite(p_s5).float().mean()),
+                                                   "beam": float(torch.isfinite(p_b5).float().mean())}}
     out["timed"] = ("CUDA events, windows >= %.1f s after warm-up; per-level arms start from the level's probabilities (beam arms: "
                     "its logits)" % w)
     print(out["card"])

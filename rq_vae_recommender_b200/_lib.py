@@ -72,6 +72,15 @@ _SIGNATURES = {
                                          c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "rqb200_sid_beam_topk": (c_int, [c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp,
                                      c_vp, c_vp]),
+    "rqb200_sid_trie_workspace_bytes": (c_size, [c_i64, c_int, c_int]),
+    "rqb200_sid_trie_build": (c_int, [c_vp, c_i64, c_int, c_int, c_vp, c_size, c_vp]),
+    "rqb200_sid_trie_check": (c_int, [c_vp, c_i64, c_i64, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
+    "rqb200_sid_trie_beam_select": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp,
+                                            c_vp, c_vp, c_vp]),
+    "rqb200_sid_trie_sample_select": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int,
+                                              c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "rqb200_sid_trie_beam_topk": (c_int, [c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp,
+                                          c_vp, c_vp, c_vp]),
     "rqb200_bf16_image_bytes": (c_size, [c_int, c_int]),
     "rqb200_f32_to_bf16_image": (c_int, [c_vp, c_i64, c_int, c_int, c_vp, c_vp]),
     "rqb200_gemm_bf16": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_i64, c_vp]),

@@ -556,30 +556,54 @@ def sid_dedup_rank(ids: torch.Tensor, K: int):
 
 
 class SidPrefixIndex:
-    """Valid-prefix index of a corpus id table [N, C] (modules/model.py:169-182): one bitmap per prefix length, built once per
-    corpus by rqb200_sid_prefix_build.  ``check`` is the reference's `_check_valid_prefix`; ``beam_select`` one selection step of
-    its constrained beam search (model.py:340-376)."""
+    """Valid-prefix index of a corpus id table [N, C] (modules/model.py:169-182), built once per corpus: one bitmap per prefix
+    length (``kind == "bitmap"``, rqb200_sid_prefix_build) where K^C fits its 2^33-bit limit, else a trie of the corpus's
+    distinct prefixes (``kind == "trie"``, rqb200_sid_trie_build, O(N C) bytes).  ``check`` is the reference's
+    `_check_valid_prefix`; ``beam_select`` one selection step of its constrained beam search (model.py:340-376).  Every method
+    gives the same results on either index.  ``kind`` forces one (both indexes of one corpus are compared that way)."""
 
-    def __init__(self, cached_ids: torch.Tensor, codebook_size: int):
+    KINDS = ("bitmap", "trie")
+    _ENTRY = {"bitmap": ("rqb200_sid_prefix_build", "rqb200_sid_prefix_check", "rqb200_sid_beam_select",
+                         "rqb200_sid_sample_select", "rqb200_sid_beam_topk"),
+              "trie": ("rqb200_sid_trie_build", "rqb200_sid_trie_check", "rqb200_sid_trie_beam_select",
+                       "rqb200_sid_trie_sample_select", "rqb200_sid_trie_beam_topk")}
+
+    @staticmethod
+    def kind_for(num_levels: int, codebook_size: int) -> str:
+        """The index a corpus of num_levels ids per row over codebook_size codes gets: the bitmap wherever it fits."""
+        return "bitmap" if _lib.load().rqb200_sid_prefix_workspace_bytes(int(num_levels), int(codebook_size)) else "trie"
+
+    def __init__(self, cached_ids: torch.Tensor, codebook_size: int, kind: Optional[str] = None):
         _need_cuda(cached_ids)
         lib = _lib.load()
         ids = cached_ids.to(torch.int64).contiguous()
         self.N, self.C = ids.shape
         self.K = int(codebook_size)
         self.device = ids.device
-        nbytes = lib.rqb200_sid_prefix_workspace_bytes(self.C, self.K)
-        if nbytes == 0:
-            raise _lib.Rqb200Error(f"prefix index: key space {self.K}^{self.C} exceeds the bitmap limit (2^33 bits)")
-        self.ws = torch.empty(nbytes, dtype=torch.uint8, device=ids.device)
+        self.kind = self.kind_for(self.C, self.K) if kind is None else kind
+        if self.kind not in self.KINDS:
+            raise ValueError(f"prefix index: kind must be one of {self.KINDS}, got {kind!r}")
+        build, check, beam_select, sample_select, beam_topk = (getattr(lib, n) for n in self._ENTRY[self.kind])
+        self._check, self._beam_select, self._sample_select, self._beam_topk = check, beam_select, sample_select, beam_topk
         with torch.cuda.device(ids.device):
-            _lib.check(lib.rqb200_sid_prefix_build(_p(ids), self.N, self.C, self.K, _p(self.ws), nbytes, _stream()),
-                       "sid_prefix_build")
-        _count(1)
+            if self.kind == "bitmap":
+                nbytes = lib.rqb200_sid_prefix_workspace_bytes(self.C, self.K)
+                if nbytes == 0:
+                    raise _lib.Rqb200Error(f"prefix index: key space {self.K}^{self.C} exceeds the bitmap limit (2^33 bits)")
+            else:
+                nbytes = lib.rqb200_sid_trie_workspace_bytes(self.N, self.C, self.K)
+                if nbytes == 0:
+                    raise _lib.Rqb200Error(f"prefix index: a trie of {self.N} rows of {self.C} ids over {self.K} codes is "
+                                           "outside its limits (N < 2^31 - 1, C <= 8, K <= 65536)")
+            #: device bytes the index holds (the trie's include its build scratch)
+            self.nbytes = int(nbytes)
+            self.ws = torch.empty(nbytes, dtype=torch.uint8, device=ids.device)
+            _lib.check(build(_p(ids), self.N, self.C, self.K, _p(self.ws), nbytes, _stream()), self._ENTRY[self.kind][0][7:])
+        _count(1)                                             # one build call (the trie's sort and scans are several kernels)
 
     def check(self, prefix: torch.Tensor) -> torch.Tensor:
         """bool [P]: does some corpus row start with prefix[p] ([P, l], l <= C)."""
         _need_cuda(prefix)
-        lib = _lib.load()
         if prefix.dtype != torch.int64:
             prefix = prefix.to(torch.int64)
         if prefix.stride(-1) != 1:
@@ -589,7 +613,7 @@ class SidPrefixIndex:
             raise ValueError(f"prefix length {l} exceeds the id tuple length {self.C}")
         valid = torch.empty(P, dtype=torch.bool, device=prefix.device)
         with torch.cuda.device(prefix.device):
-            _lib.check(lib.rqb200_sid_prefix_check(_p(prefix), prefix.stride(0), P, l, self.C, self.K, _p(self.ws), _p(valid),
+            _lib.check(self._check(_p(prefix), prefix.stride(0), P, l, self.C, self.K, _p(self.ws), _p(valid),
                                                    _stream()), "sid_prefix_check")
         _count(1)
         return valid
@@ -599,7 +623,6 @@ class SidPrefixIndex:
         """samples / samp_log_p [B * kp, nc] (kp = 1 on the first level), generated [B, kp, h] or None, log_probas [B, kp] or None
         -> (generated [B, k, h + 1], log_probas [B, k], parent_global [B * k]) exactly as model.py:353-388 computes them."""
         _need_cuda(samples, samp_log_p)
-        lib = _lib.load()
         if generated is None:
             B, kp, h = samples.shape[0], 1, 0
         else:
@@ -615,7 +638,7 @@ class SidPrefixIndex:
         out_p = torch.empty((B, k), dtype=torch.float32, device=dev)
         out_parent = torch.empty((B * k,), dtype=torch.int64, device=dev)
         with torch.cuda.device(dev):
-            _lib.check(lib.rqb200_sid_beam_select(_p(samples), _p(samp_log_p), _p(generated), _p(log_probas), B, kp, nc, h, k,
+            _lib.check(self._beam_select(_p(samples), _p(samp_log_p), _p(generated), _p(log_probas), B, kp, nc, h, k,
                                                   self.C, self.K, _p(self.ws), _p(out_g), _p(out_p), _p(out_parent), _stream()),
                        "sid_beam_select")
         _count(1)
@@ -631,7 +654,6 @@ class SidPrefixIndex:
         ``torch.multinomial(probas, nc)``'s under the same generator state.  ``reject``, an int32 [2] device tensor, is ADDED the
         number of rows torch.multinomial would reject: [0] with a NaN, +-inf or negative entry, [1] otherwise all zero."""
         _need_cuda(probas, noise, reject)
-        lib = _lib.load()
         if generated is None:
             B, kp, h = probas.shape[0], 1, 0
         else:
@@ -654,7 +676,7 @@ class SidPrefixIndex:
         samples = torch.empty((B * kp, nc), dtype=torch.int64, device=dev) if want_samples else None
         samp_log_p = torch.empty((B * kp, nc), dtype=torch.float32, device=dev) if want_samples else None
         with torch.cuda.device(dev):
-            _lib.check(lib.rqb200_sid_sample_select(_p(probas), probas.stride(0), _p(noise), noise.stride(0), _p(generated),
+            _lib.check(self._sample_select(_p(probas), probas.stride(0), _p(noise), noise.stride(0), _p(generated),
                                                     _p(log_probas), B, kp, nc, h, k, self.C, self.K, _p(self.ws), _p(out_g),
                                                     _p(out_p), _p(out_parent), _p(samples), _p(samp_log_p), _p(reject),
                                                     _stream()), "sid_sample_select")
@@ -672,7 +694,6 @@ class SidPrefixIndex:
         best in descending order, equal scores by ascending beam * K + code.  Deterministic.  ``bad``, an int32 device tensor,
         is ADDED the number of beam rows whose logits hold a NaN or +inf or are all -inf."""
         _need_cuda(logits, bad)
-        lib = _lib.load()
         if generated is None:
             B, kp, h = logits.shape[0], 1, 0
         else:
@@ -693,7 +714,7 @@ class SidPrefixIndex:
         out_p = torch.empty((B, k), dtype=torch.float32, device=dev)
         out_parent = torch.empty((B * k,), dtype=torch.int64, device=dev)
         with torch.cuda.device(dev):
-            _lib.check(lib.rqb200_sid_beam_topk(_p(logits), logits.stride(0), _p(generated), _p(log_probas), B, kp, h, k, self.C,
+            _lib.check(self._beam_topk(_p(logits), logits.stride(0), _p(generated), _p(log_probas), B, kp, h, k, self.C,
                                                 self.K, _p(self.ws), _p(out_g), _p(out_p), _p(out_parent), _p(bad), _stream()),
                        "sid_beam_topk")
         _count(1)
