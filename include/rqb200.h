@@ -85,7 +85,8 @@ int rqb200_tokenize_tc_run(const float* x, int64_t ldx, int B, const void* state
 /* ---- k-means codebook initialisation (init/kmeans.py) ------------------------------------------------
  * assign_accumulate = one Lloyd assignment pass with the direct (x-c)^2 distance of kmeans.py:40-43 plus the
  * per-cluster sums (fp64) and counts that kmeans.py:48-58 derives with a Python loop; in the sharded setting
- * the caller all-reduces sums/counts between the two calls.  finalize writes the new centroids in place
+ * the caller all-reduces sums/counts between the two calls; an empty shard (B = 0, x and assignment may be
+ * NULL) contributes zero sums and counts.  finalize writes the new centroids in place
  * (mean, or x[reseed_rows[k]] for an empty cluster, kmeans.py:50-54; reseed_rows may be NULL) and the
  * max centroid shift of kmeans.py:68 into *max_shift (device float). */
 int rqb200_kmeans_assign_accumulate(const float* x, int64_t ldx, const float* centroids, int B, int D, int K,

@@ -770,11 +770,12 @@ extern "C" int rqb200_kmeans_assign_accumulate(const float* x, int64_t ldx, cons
                                                int64_t* assignment, double* sums, int* counts, void* workspace,
                                                size_t ws_bytes, void* stream) {
   RQB_CHECK_ARG(B >= 0 && D > 0 && K > 0, "kmeans: bad shape");
-  RQB_CHECK_ARG(x && centroids && assignment && sums && counts && workspace, "kmeans: null pointer");
+  RQB_CHECK_ARG(centroids && sums && counts, "kmeans: null pointer");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   RQB_CUDA(cudaMemsetAsync(sums, 0, (size_t)K * D * sizeof(double), st));
   RQB_CUDA(cudaMemsetAsync(counts, 0, (size_t)K * sizeof(int), st));
-  if (B == 0) return RQB_OK;
+  if (B == 0) return RQB_OK;  // an empty shard (x and assignment may be null): zero sums and counts
+  RQB_CHECK_ARG(x && assignment && workspace, "kmeans: null pointer");
   RqParams p{};
   const float* cbs[1] = {centroids};
   int rc = run_prep(cbs, D, K, 1, workspace, ws_bytes, st, &p.ct, &p.cc, &p.Dp, &p.Kp);

@@ -5,6 +5,7 @@ import pytest
 import torch
 
 import inputs as I
+import train_chain_ref as R
 from oracle import rq_oracle as O
 from parity import assert_ids_match, load_golden, rel_err
 
@@ -164,37 +165,12 @@ def test_chain_backward_vs_torch_autograd_of_oracle_formulas(ops, mname, lean):
     if not lean:
         obj = obj + (b * gb).sum()
     obj.backward()
-    # float64 reference on the SAME ids
-    ids_h = ids.cpu()
-    x64 = torch.from_numpy(x).double().requires_grad_(True)
-    c64 = [torch.from_numpy(c).double().requires_grad_(True) for c in cbs]
-    res = x64
-    embs, ress, tot = [], [], 0
-    for l in range(L):
-        ress.append(res)
-        e = c64[l][ids_h[:, l]]
-        if mname == "eval":
-            eo = e
-        elif mname == "ste":
-            eo = res + (e - res).detach()
-        else:
-            u = res / (res.norm(dim=-1, keepdim=True) + 1e-8)
-            q = e / (e.norm(dim=-1, keepdim=True) + 1e-8)
-            w = torch.nn.functional.normalize(u + q, p=2, dim=1, eps=1e-6).detach()
-            rot = res - 2 * (res * w).sum(1, keepdim=True) * w + 2 * (res * u.detach()).sum(1, keepdim=True) * q.detach()
-            eo = rot * (e.norm(dim=1, keepdim=True) / (res.norm(dim=1, keepdim=True) + 1e-6)).detach()
-        tot = tot + ((res.detach() - e) ** 2).sum(-1) + BETA * ((res - e.detach()) ** 2).sum(-1)
-        res = res - eo
-        embs.append(eo)
-    E = torch.stack(embs, 0)
-    if lean:
-        obj64 = (E.sum(0) * ga.cpu().double()).sum() + (tot * gl.cpu().double()).sum()
-    else:
-        obj64 = (E * ga.cpu().double()).sum() + (torch.stack(ress, 0) * gb.cpu().double()).sum() + (tot * gl.cpu().double()).sum()
-    obj64.backward()
-    assert rel_err(host(xt.grad), x64.grad.numpy()) < 2e-5
-    for ct, c in zip(cts, c64):
-        assert rel_err(host(ct.grad), c.grad.numpy()) < 2e-5
+    # float64 autograd of the reference expressions on the SAME ids
+    up = {"emb_sum": ga, "loss": gl} if lean else {"embeddings": ga.permute(1, 0, 2), "residuals": gb.permute(1, 0, 2), "loss": gl}
+    _, gx64, gc64 = R.evaluate(R.chain(KMODE[mname], BETA), xt.detach(), [c.detach() for c in cts], (ids,), upstream=up)
+    assert rel_err(host(xt.grad), host(gx64)) < 2e-5
+    for ct, g in zip(cts, gc64):
+        assert rel_err(host(ct.grad), host(g)) < 2e-5
 
 
 # ------------------------------------------------------------------ Gumbel level
