@@ -257,6 +257,43 @@ int rqb200_sid_trie_beam_topk(const float* logits, int64_t logits_stride, const 
                               int kp, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
                               float* out_log_probas, int64_t* out_parent, int* bad, void* stream);
 
+/* ---- from generated id tuples to corpus items ----
+ * Row n of the corpus id table [N, C] is item n; rows with equal tuples are told apart by their dedup rank (the tokeniser's last
+ * column: how many earlier rows carry the same tuple).  The item table maps a tuple back to its rows.  A row is retrievable
+ * only if all C of its ids are in [0, K); duplicated rows and N = 0 are legal.  Limits: C <= 8, K <= 65536, N < 2^31 - 1.
+ * sid_items_build     : stable radix sort of the rows on their packed tuple (the trie build's sort), then one scan over the
+ *                       first row of each distinct tuple.  The workspace (sid_items_workspace_bytes: O(N C) bytes, 0 outside the
+ *                       limits or when the current device cannot be queried) starts with a header that locates row [N] (row
+ *                       ids in sorted order; equal tuples in ascending row order, i.e. dedup rank 0, 1, 2, ...), the U distinct
+ *                       tuples' keys and start [U + 1] (tuple u's rows are row[start[u] .. start[u + 1])).  Runs on the stream
+ *                       without synchronising the host.
+ * sid_items_lookup    : out_item[p] for the tuple ids[p, 0:C] (row stride ids_stride, in elements): its first item, or with
+ *                       with_dedup the item of dedup rank d = ids[p, C]; -1 when the tuple holds an id outside [0, K), is not
+ *                       in the corpus, or d is outside [0, count).
+ * sid_items_retrieve  : generated [B, k, C] int64 (contiguous), log_probas [B, k] fp32 or null -> per history b, in beam order
+ *                       (generate returns beams by descending score), the items of every beam whose log-probability is above
+ *                       -inf (or log_probas is null) and whose tuple is in the corpus, each beam's in ascending row order
+ *                       (dedup rank 0, 1, ...), an item already written for b not repeated (two beams with one tuple), cut off
+ *                       at n: out_items [B, n] int64 (-1 pad), out_beam [B, n] int32 (the source beam, -1 pad), out_count [B]
+ *                       int32.  C must be the table's C (else no beam resolves).  One CTA per history; deterministic.
+ *                       Limits: k <= 1024, n <= 4096, RQB_ERR_UNSUPPORTED otherwise.  B = 0 is a no-op. */
+size_t rqb200_sid_items_workspace_bytes(int64_t N, int C, int K);
+int rqb200_sid_items_build(const int64_t* cached_ids, int64_t N, int C, int K, void* workspace, size_t ws_bytes, void* stream);
+int rqb200_sid_items_lookup(const void* workspace, const int64_t* ids, int64_t ids_stride, int64_t P, int with_dedup,
+                            int64_t* out_item /* [P] */, void* stream);
+int rqb200_sid_items_retrieve(const void* workspace, const int64_t* generated, const float* log_probas, int B, int k, int C, int n,
+                              int64_t* out_items, int* out_beam, int* out_count, void* stream);
+
+/* sid_topk_rank_hist  : evaluate/metrics.py's TopKAccumulator rule, accumulated on the device.  Row b's rank is its first
+ *                       candidate cand[b, j, 0:D] equal to actual[b, 0:D] in all D columns (`.all(-1).max(-1)`); hist[rank] += 1,
+ *                       or hist[k] += 1 when none matches.  hist is int64 [k + 1], ADDED to (never cleared), so batches
+ *                       accumulate exactly; NDCG = sum_r hist[r] / log2(r + 2) and h@j = sum_{r<j} hist[r] follow from it.
+ *                       item_mode: a value -1 (padding, an unresolvable item) never matches; otherwise every input keeps the
+ *                       reference's rule.  actual row stride a_stride >= D, cand [B, k, D] with history stride c_stride >= k D
+ *                       (elements).  B = 0 is a no-op. */
+int rqb200_sid_topk_rank_hist(const int64_t* actual, int64_t a_stride, const int64_t* cand, int64_t c_stride, int B, int k, int D,
+                              int item_mode, int64_t* hist, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -14,6 +14,7 @@
 #include <utility>
 
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/block/block_scan.cuh>
 #include <cub/device/device_scan.cuh>
 
 #include "common.cuh"
@@ -269,6 +270,23 @@ struct SidTrieLayout {
 
 static size_t sid_align256(size_t b) { return (b + 255) / 256 * 256; }
 
+// The row sort shared by the trie and the item table: bits per packed id (K itself, the "no id" mark, fits), ids per 64-bit
+// sort key, and the CUB scratch bytes of a sort or a scan of N entries.  Nonzero when the sort's workspace query fails.
+static int sid_sort_plan(int64_t N, int K, int& width, int& cols, size_t& temp_bytes) {
+  width = 32 - __builtin_clz((unsigned)K);
+  cols = 64 / width;
+  size_t sort_bytes = 0, scan_bytes = 0;
+  const int n = (int)N > 0 ? (int)N : 1;
+  if (cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                      (const int*)nullptr, (int*)nullptr, n, 0, 64) != cudaSuccess ||
+      cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, (const int*)nullptr, (int*)nullptr, n) != cudaSuccess) {
+    cudaGetLastError();
+    return 1;
+  }
+  temp_bytes = sort_bytes > scan_bytes ? sort_bytes : scan_bytes;
+  return 0;
+}
+
 static int sid_trie_layout(int64_t N, int C, int K, SidTrieLayout& t) {
   if (N < 0 || N >= 0x7fffffffll || C <= 0 || C > 8 || K <= 0 || K > 65536) return 1;
   t = SidTrieLayout{};
@@ -297,18 +315,8 @@ static int sid_trie_layout(int64_t N, int C, int K, SidTrieLayout& t) {
   at += sid_align256((size_t)C * N * sizeof(int));
   t.scan = at;
   at += sid_align256((size_t)C * N * sizeof(int));
-  t.width = 32 - __builtin_clz((unsigned)K);                // K itself (the "no id" mark) fits
-  t.cols = 64 / t.width;
-  size_t sort_bytes = 0, scan_bytes = 0;
-  const int n = (int)N > 0 ? (int)N : 1;
-  if (cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
-                                      (const int*)nullptr, (int*)nullptr, n, 0, 64) != cudaSuccess ||
-      cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, (const int*)nullptr, (int*)nullptr, n) != cudaSuccess) {
-    cudaGetLastError();
-    return 2;
-  }
+  if (sid_sort_plan(N, K, t.width, t.cols, t.temp_bytes)) return 2;
   t.temp = at;
-  t.temp_bytes = sort_bytes > scan_bytes ? sort_bytes : scan_bytes;
   t.total = at + sid_align256(t.temp_bytes);
   return 0;
 }
@@ -336,17 +344,48 @@ __global__ void sid_trie_iota_kernel(int* perm, int N) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < N; i += gridDim.x * blockDim.x) perm[i] = i;
 }
 
-// keys[i] = ids c0 .. c1 - 1 of row perm[i], `width` bits each, the first id most significant; ids at or after the row's first
-// id outside [0, K) are K
+// ids c0 .. c1 - 1 of a row, `width` bits each, the first id most significant; ids at or after position d are K
+__device__ __forceinline__ unsigned long long sid_pack_cols(const int64_t* row, int d, int c0, int c1, int width, int K) {
+  unsigned long long key = 0;
+  for (int c = c0; c < c1; ++c) key = (key << width) | (unsigned long long)(c < d ? row[c] : K);
+  return key;
+}
+
+// keys[i] = ids c0 .. c1 - 1 of row perm[i] packed, ids at or after the row's first id outside [0, K) K
 __global__ void sid_trie_key_kernel(const int64_t* __restrict__ ids, int N, int C, int K, const int* __restrict__ perm, int c0, int c1,
                                     int width, unsigned long long* __restrict__ keys) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < N; i += gridDim.x * blockDim.x) {
     const int64_t* row = ids + (int64_t)perm[i] * C;
-    const int d = sid_row_depth(row, C, K);
-    unsigned long long key = 0;
-    for (int c = c0; c < c1; ++c) key = (key << width) | (unsigned long long)(c < d ? row[c] : K);
-    keys[i] = key;
+    keys[i] = sid_pack_cols(row, sid_row_depth(row, C, K), c0, c1, width, K);
   }
+}
+
+// the item table's sort key: as sid_trie_key_kernel, but a row holding any id outside [0, K) is all K (it sorts last)
+__global__ void sid_items_key_kernel(const int64_t* __restrict__ ids, int N, int C, int K, const int* __restrict__ perm, int c0, int c1,
+                                     int width, unsigned long long* __restrict__ keys) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < N; i += gridDim.x * blockDim.x) {
+    const int64_t* row = ids + (int64_t)perm[i] * C;
+    keys[i] = sid_pack_cols(row, sid_row_depth(row, C, K) == C ? C : 0, c0, c1, width, K);
+  }
+}
+
+// Stable LSD radix sort of the N rows on their packed tuple, least significant column group first (CUB, on the stream).
+// perm[0] ends holding the sorted row ids; with `whole` rows that hold an id outside [0, K) sort last, else the trie's order.
+static int sid_sort_rows(const int64_t* ids, int n, int C, int K, int width, int cols, bool whole, unsigned long long* keys[2],
+                         int* perm[2], void* temp, size_t temp_bytes, int grid, cudaStream_t st) {
+  sid_trie_iota_kernel<<<grid, 256, 0, st>>>(perm[0], n);
+  RQB_LAUNCH_CHECK();
+  const int groups = (C + cols - 1) / cols;
+  for (int g = groups - 1; g >= 0; --g) {                   // least significant column group first; each sort is stable
+    const int c0 = g * cols, c1 = min(C, c0 + cols);
+    if (whole) sid_items_key_kernel<<<grid, 256, 0, st>>>(ids, n, C, K, perm[0], c0, c1, width, keys[0]);
+    else sid_trie_key_kernel<<<grid, 256, 0, st>>>(ids, n, C, K, perm[0], c0, c1, width, keys[0]);
+    RQB_LAUNCH_CHECK();
+    size_t tb = temp_bytes;
+    RQB_CUDA(cub::DeviceRadixSort::SortPairs(temp, tb, keys[0], keys[1], perm[0], perm[1], n, 0, width * (c1 - c0), st));
+    std::swap(perm[0], perm[1]);
+  }
+  return RQB_OK;
 }
 
 // flag[l - 1][r] = sorted row r starts a node of level l: l is within its valid length and beyond its common prefix with row r - 1
@@ -424,18 +463,8 @@ extern "C" int rqb200_sid_trie_build(const int64_t* cached_ids, int64_t N, int C
   int* perm[2] = {reinterpret_cast<int*>(ws + t.perm[0]), reinterpret_cast<int*>(ws + t.perm[1])};
   int* flag = reinterpret_cast<int*>(ws + t.flag);
   int* scan = reinterpret_cast<int*>(ws + t.scan);
-  sid_trie_iota_kernel<<<grid, 256, 0, st>>>(perm[0], n);
-  RQB_LAUNCH_CHECK();
-  const int groups = (C + t.cols - 1) / t.cols;
-  for (int g = groups - 1; g >= 0; --g) {                   // least significant column group first; each sort is stable
-    const int c0 = g * t.cols, c1 = min(C, c0 + t.cols);
-    sid_trie_key_kernel<<<grid, 256, 0, st>>>(cached_ids, n, C, K, perm[0], c0, c1, t.width, keys[0]);
-    RQB_LAUNCH_CHECK();
-    size_t temp_bytes = t.temp_bytes;
-    RQB_CUDA(cub::DeviceRadixSort::SortPairs(ws + t.temp, temp_bytes, keys[0], keys[1], perm[0], perm[1], n, 0,
-                                             t.width * (c1 - c0), st));
-    std::swap(perm[0], perm[1]);
-  }
+  const int sorted = sid_sort_rows(cached_ids, n, C, K, t.width, t.cols, false, keys, perm, ws + t.temp, t.temp_bytes, grid, st);
+  if (sorted != RQB_OK) return sorted;
   sid_trie_flag_kernel<<<grid, 256, 0, st>>>(cached_ids, n, C, K, perm[0], flag);
   RQB_LAUNCH_CHECK();
   for (int l = 0; l < C; ++l) {
@@ -1155,4 +1184,335 @@ extern "C" int rqb200_sid_trie_beam_topk(const float* logits, int64_t logits_str
   return sid_beam_topk_run(logits, logits_stride, generated, log_probas, B, kp, h, k, K,
                            SidTrie{reinterpret_cast<const unsigned char*>(prefix_workspace), h + 1}, out_generated, out_log_probas,
                            out_parent, bad, stream);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Corpus item table: from a generated id tuple back to the corpus items (rows) that carry it.  Row n of the corpus table
+// [N, C] is item n; rows with equal tuples are told apart by their dedup rank (the tokeniser's last column: the number of
+// earlier rows with the same tuple).  The build sorts the rows on their packed tuple with the trie's stable LSD radix sort
+// (sid_sort_rows; a row holding an id outside [0, K) sorts last and is never retrievable), flags the first row of each distinct
+// tuple, numbers the tuples with one scan and keeps
+//   row[N]        the row ids in sorted order: equal tuples in ascending row order, i.e. dedup rank 0, 1, 2, ...;
+//   key[U][G]     the U distinct retrievable tuples, packed as the sort packs them (G 64-bit words of `cols` ids each), ascending;
+//   start[U + 1]  tuple u's rows are row[start[u] .. start[u + 1]).
+// A lookup packs its tuple and binary-searches the keys.  A header at the start of the workspace locates the arrays.
+//   workspace layout: header | row (int [N]) | key (u64 [N * G]) | start (int [N + 1]) | build scratch, 256-byte aligned regions.
+struct SidItemsHeader {
+  int C, K;
+  long long N;
+  int U;                                                    // distinct retrievable tuples (written by the build)
+  int G, width, cols;                                       // words per packed tuple, bits per id, ids per word
+  unsigned long long row, key, start;                       // byte offsets
+};
+
+struct SidItemsLayout {
+  SidItemsHeader h;
+  size_t keys[2], perm[2], flag, scan, temp, temp_bytes, total;
+};
+
+#define SID_ITEMS_MAX_G 3                                   // C <= 8 ids of at most 17 bits: 3 ids per word
+#define SID_ITEMS_MAX_K 1024
+#define SID_ITEMS_MAX_N 4096
+
+static int sid_items_layout(int64_t N, int C, int K, SidItemsLayout& t) {
+  if (N < 0 || N >= 0x7fffffffll || C <= 0 || C > 8 || K <= 0 || K > 65536) return 1;
+  t = SidItemsLayout{};
+  if (sid_sort_plan(N, K, t.h.width, t.h.cols, t.temp_bytes)) return 2;
+  t.h.C = C;
+  t.h.K = K;
+  t.h.N = N;
+  t.h.G = (C + t.h.cols - 1) / t.h.cols;
+  size_t at = sid_align256(sizeof(SidItemsHeader));
+  t.h.row = at;
+  at += sid_align256((size_t)N * sizeof(int));
+  t.h.key = at;
+  at += sid_align256((size_t)N * t.h.G * sizeof(unsigned long long));
+  t.h.start = at;
+  at += sid_align256(((size_t)N + 1) * sizeof(int));
+  for (int i = 0; i < 2; ++i) {
+    t.keys[i] = at;
+    at += sid_align256((size_t)N * sizeof(unsigned long long));
+  }
+  for (int i = 0; i < 2; ++i) {
+    t.perm[i] = at;
+    at += sid_align256((size_t)N * sizeof(int));
+  }
+  t.flag = at;
+  at += sid_align256((size_t)N * sizeof(int));
+  t.scan = at;
+  at += sid_align256((size_t)N * sizeof(int));
+  t.temp = at;
+  t.total = at + sid_align256(t.temp_bytes);
+  return 0;
+}
+
+extern "C" size_t rqb200_sid_items_workspace_bytes(int64_t N, int C, int K) {
+  SidItemsLayout t;
+  return sid_items_layout(N, C, K, t) ? 0 : t.total;
+}
+
+__global__ void sid_items_header_kernel(SidItemsHeader h, unsigned char* ws) {
+  *reinterpret_cast<SidItemsHeader*>(ws) = h;               // U = 0 and start[0] = 0: the fill pass overwrites both when a row is valid
+  reinterpret_cast<int*>(ws + h.start)[0] = 0;
+}
+
+// flag[r] = sorted row r is retrievable and its tuple differs from sorted row r - 1's (the unretrievable rows sort last)
+__global__ void sid_items_flag_kernel(const int64_t* __restrict__ ids, int N, int C, int K, const int* __restrict__ perm,
+                                      int* __restrict__ flag) {
+  for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < N; r += gridDim.x * blockDim.x) {
+    const int64_t* row = ids + (int64_t)perm[r] * C;
+    bool f = sid_row_depth(row, C, K) == C;
+    if (f && r > 0) {
+      const int64_t* prev = ids + (int64_t)perm[r - 1] * C;
+      bool same = true;
+      for (int c = 0; c < C; ++c) same = same && prev[c] == row[c];
+      f = !same;
+    }
+    flag[r] = f ? 1 : 0;
+  }
+}
+
+// row[r] = perm[r]; the row starting tuple u = scan[r] - 1 writes key[u] and start[u]; the last retrievable row closes start[U]
+// and stores U
+__global__ void sid_items_fill_kernel(const int64_t* __restrict__ ids, int N, const int* __restrict__ perm, const int* __restrict__ flag,
+                                      const int* __restrict__ scan, unsigned char* ws) {
+  SidItemsHeader* hdr = reinterpret_cast<SidItemsHeader*>(ws);
+  const int C = hdr->C, K = hdr->K, G = hdr->G, width = hdr->width, cols = hdr->cols;
+  int* row_out = reinterpret_cast<int*>(ws + hdr->row);
+  unsigned long long* key = reinterpret_cast<unsigned long long*>(ws + hdr->key);
+  int* start = reinterpret_cast<int*>(ws + hdr->start);
+  for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < N; r += gridDim.x * blockDim.x) {
+    const int64_t* row = ids + (int64_t)perm[r] * C;
+    row_out[r] = perm[r];
+    if (sid_row_depth(row, C, K) < C) continue;
+    const int s = scan[r];
+    if (flag[r]) {
+      for (int g = 0; g < G; ++g) key[(int64_t)(s - 1) * G + g] = sid_pack_cols(row, C, g * cols, min(C, (g + 1) * cols), width, K);
+      start[s - 1] = r;
+    }
+    if (r == N - 1 || sid_row_depth(ids + (int64_t)perm[r + 1] * C, C, K) < C) {
+      start[s] = r + 1;
+      hdr->U = s;
+    }
+  }
+}
+
+extern "C" int rqb200_sid_items_build(const int64_t* cached_ids, int64_t N, int C, int K, void* workspace, size_t ws_bytes, void* stream) {
+  RQB_CHECK_ARG(N >= 0 && C > 0 && K > 0 && workspace, "sid_items_build: bad argument");
+  SidItemsLayout t;
+  const int rc = sid_items_layout(N, C, K, t);
+  if (rc == 1) {
+    rqb_set_error("sid_items_build: need C <= 8, K <= 65536 and N < 2^31 - 1 (N = %lld, C = %d, K = %d)", (long long)N, C, K);
+    return RQB_ERR_UNSUPPORTED;
+  }
+  if (rc == 2) {
+    rqb_set_error("sid_items_build: the sort's workspace query failed (no CUDA device?)");
+    return RQB_ERR_CUDA;
+  }
+  if (ws_bytes < t.total) {
+    rqb_set_error("sid_items_build: workspace too small");
+    return RQB_ERR_WORKSPACE;
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
+  sid_items_header_kernel<<<1, 1, 0, st>>>(t.h, ws);
+  RQB_LAUNCH_CHECK();
+  if (N == 0) return RQB_OK;
+  RQB_CHECK_ARG(cached_ids, "sid_items_build: null pointer");
+  const int n = (int)N;
+  int grid = (n + 255) / 256;
+  if (grid > 132 * 8) grid = 132 * 8;
+  unsigned long long* keys[2] = {reinterpret_cast<unsigned long long*>(ws + t.keys[0]),
+                                 reinterpret_cast<unsigned long long*>(ws + t.keys[1])};
+  int* perm[2] = {reinterpret_cast<int*>(ws + t.perm[0]), reinterpret_cast<int*>(ws + t.perm[1])};
+  int* flag = reinterpret_cast<int*>(ws + t.flag);
+  int* scan = reinterpret_cast<int*>(ws + t.scan);
+  const int sorted = sid_sort_rows(cached_ids, n, C, K, t.h.width, t.h.cols, true, keys, perm, ws + t.temp, t.temp_bytes, grid, st);
+  if (sorted != RQB_OK) return sorted;
+  sid_items_flag_kernel<<<grid, 256, 0, st>>>(cached_ids, n, C, K, perm[0], flag);
+  RQB_LAUNCH_CHECK();
+  size_t temp_bytes = t.temp_bytes;
+  RQB_CUDA(cub::DeviceScan::InclusiveSum(ws + t.temp, temp_bytes, flag, scan, n, st));
+  sid_items_fill_kernel<<<grid, 256, 0, st>>>(cached_ids, n, perm[0], flag, scan, ws);
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
+}
+
+// lexicographic order of the G-word packed tuples m and q: -1, 0 or 1
+__device__ __forceinline__ int sid_items_cmp(const unsigned long long* m, const unsigned long long (&q)[SID_ITEMS_MAX_G], int G) {
+  int cmp = 0;
+#pragma unroll
+  for (int g = 0; g < SID_ITEMS_MAX_G; ++g) {
+    if (cmp == 0 && g < G) {
+      const unsigned long long v = __ldg(m + g);
+      cmp = v < q[g] ? -1 : v > q[g] ? 1 : 0;
+    }
+  }
+  return cmp;
+}
+
+// tuple u of the table whose C ids equal t[0, C) (C = the table's), or -1 (an id outside [0, K), or not in the corpus)
+__device__ __forceinline__ int sid_items_find(const unsigned char* ws, const SidItemsHeader& h, const int64_t* t) {
+  unsigned long long q[SID_ITEMS_MAX_G];
+  for (int c = 0; c < h.C; ++c)
+    if (t[c] < 0 || t[c] >= h.K) return -1;
+#pragma unroll
+  for (int g = 0; g < SID_ITEMS_MAX_G; ++g)
+    q[g] = g < h.G ? sid_pack_cols(t, h.C, g * h.cols, min(h.C, (g + 1) * h.cols), h.width, h.K) : 0ull;
+  const unsigned long long* key = reinterpret_cast<const unsigned long long*>(ws + h.key);
+  int a = 0, b = h.U;                                       // first key >= q
+  while (a < b) {
+    const int mid = (a + b) >> 1;
+    if (sid_items_cmp(key + (int64_t)mid * h.G, q, h.G) < 0) a = mid + 1;
+    else b = mid;
+  }
+  return (a < h.U && sid_items_cmp(key + (int64_t)a * h.G, q, h.G) == 0) ? a : -1;
+}
+
+__global__ void sid_items_lookup_kernel(const unsigned char* __restrict__ ws, const int64_t* __restrict__ ids, int64_t stride, int64_t P,
+                                        int with_dedup, int64_t* __restrict__ out) {
+  const SidItemsHeader h = *reinterpret_cast<const SidItemsHeader*>(ws);
+  const int* row = reinterpret_cast<const int*>(ws + h.row);
+  const int* start = reinterpret_cast<const int*>(ws + h.start);
+  for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < P; p += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t* t = ids + p * stride;
+    const int u = sid_items_find(ws, h, t);
+    int64_t item = -1;
+    if (u >= 0) {
+      const int64_t d = with_dedup ? t[h.C] : 0;
+      const int s = __ldg(start + u), count = __ldg(start + u + 1) - s;
+      if (d >= 0 && d < count) item = __ldg(row + s + d);
+    }
+    out[p] = item;
+  }
+}
+
+extern "C" int rqb200_sid_items_lookup(const void* workspace, const int64_t* ids, int64_t ids_stride, int64_t P, int with_dedup,
+                                       int64_t* out_item, void* stream) {
+  RQB_CHECK_ARG(P >= 0 && ids_stride > 0, "sid_items_lookup: bad argument (P = %lld, stride = %lld)", (long long)P,
+                (long long)ids_stride);
+  if (P == 0) return RQB_OK;
+  RQB_CHECK_ARG(workspace && ids && out_item, "sid_items_lookup: null pointer");
+  int grid = (int)((P + 255) / 256);
+  if (grid > 132 * 16) grid = 132 * 16;
+  sid_items_lookup_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<const unsigned char*>(workspace), ids, ids_stride, P, with_dedup, out_item);
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
+}
+
+// One CTA per history b: each beam that is finite (log_probas null, or above -inf) and whose tuple is in the corpus resolves to
+// tuple u; a beam whose tuple an earlier beam carries counts 0 items, every other resolved beam its tuple's row count; an
+// exclusive block scan of the k counts places each beam's rows, in beam order, and output slot o takes the row of the beam
+// whose range holds it (a binary search in the scanned offsets).  No result depends on the order of atomics.
+#define SID_ITEMS_THREADS 256
+#define SID_ITEMS_PER_THREAD (SID_ITEMS_MAX_K / SID_ITEMS_THREADS)
+
+__global__ void __launch_bounds__(SID_ITEMS_THREADS) sid_items_retrieve_kernel(
+    const unsigned char* __restrict__ ws, const int64_t* __restrict__ generated, const float* __restrict__ log_probas, int k, int C,
+    int n, int64_t* __restrict__ out_items, int* __restrict__ out_beam, int* __restrict__ out_count) {
+  using Scan = cub::BlockScan<int, SID_ITEMS_THREADS>;
+  __shared__ typename Scan::TempStorage scan_tmp;
+  __shared__ int s_u[SID_ITEMS_MAX_K];
+  __shared__ int s_off[SID_ITEMS_MAX_K + 1];
+  const SidItemsHeader h = *reinterpret_cast<const SidItemsHeader*>(ws);
+  const int* row = reinterpret_cast<const int*>(ws + h.row);
+  const int* start = reinterpret_cast<const int*>(ws + h.start);
+  const int b = blockIdx.x;
+  for (int j = threadIdx.x; j < k; j += SID_ITEMS_THREADS) {
+    const int64_t bj = (int64_t)b * k + j;
+    const bool live = log_probas == nullptr || log_probas[bj] > -INFINITY;   // NaN is not above -inf either
+    s_u[j] = (live && C == h.C) ? sid_items_find(ws, h, generated + bj * C) : -1;
+  }
+  __syncthreads();
+  int cnt[SID_ITEMS_PER_THREAD];
+#pragma unroll
+  for (int i = 0; i < SID_ITEMS_PER_THREAD; ++i) {
+    const int j = threadIdx.x * SID_ITEMS_PER_THREAD + i;
+    cnt[i] = 0;
+    if (j < k && s_u[j] >= 0) {
+      const int u = s_u[j];
+      bool seen = false;
+      for (int q = 0; q < j && !seen; ++q) seen = s_u[q] == u;
+      if (!seen) cnt[i] = __ldg(start + u + 1) - __ldg(start + u);
+    }
+  }
+  int off[SID_ITEMS_PER_THREAD], total;
+  Scan(scan_tmp).ExclusiveSum(cnt, off, total);
+#pragma unroll
+  for (int i = 0; i < SID_ITEMS_PER_THREAD; ++i) {
+    const int j = threadIdx.x * SID_ITEMS_PER_THREAD + i;
+    if (j < k) s_off[j] = off[i];
+  }
+  if (threadIdx.x == 0) s_off[k] = total;
+  __syncthreads();
+  const int m = min(total, n);
+  for (int o = threadIdx.x; o < n; o += SID_ITEMS_THREADS) {
+    int64_t item = -1;
+    int beam = -1;
+    if (o < m) {                                            // s_off[lo] <= o < s_off[hi]: beam lo holds slot o
+      int lo = 0, hi = k;
+      while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (s_off[mid] <= o) lo = mid;
+        else hi = mid;
+      }
+      beam = lo;
+      item = __ldg(row + __ldg(start + s_u[lo]) + (o - s_off[lo]));
+    }
+    out_items[(int64_t)b * n + o] = item;
+    out_beam[(int64_t)b * n + o] = beam;
+  }
+  if (threadIdx.x == 0) out_count[b] = m;
+}
+
+extern "C" int rqb200_sid_items_retrieve(const void* workspace, const int64_t* generated, const float* log_probas, int B, int k, int C,
+                                         int n, int64_t* out_items, int* out_beam, int* out_count, void* stream) {
+  RQB_CHECK_ARG(B >= 0 && k > 0 && C > 0 && n > 0, "sid_items_retrieve: bad argument (B = %d, k = %d, C = %d, n = %d)", B, k, C, n);
+  if (k > SID_ITEMS_MAX_K || n > SID_ITEMS_MAX_N) {
+    rqb_set_error("sid_items_retrieve: need k <= %d and n <= %d (k = %d, n = %d)", SID_ITEMS_MAX_K, SID_ITEMS_MAX_N, k, n);
+    return RQB_ERR_UNSUPPORTED;
+  }
+  if (B == 0) return RQB_OK;
+  RQB_CHECK_ARG(workspace && generated && out_items && out_beam && out_count, "sid_items_retrieve: null pointer");
+  sid_items_retrieve_kernel<<<B, SID_ITEMS_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<const unsigned char*>(workspace), generated, log_probas, k, C, n, out_items, out_beam, out_count);
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Rank histogram of evaluate/metrics.py's TopKAccumulator: row b's rank is its first candidate whose D columns all equal
+// actual[b] (`.all(-1).max(-1)`), k when none does; hist[rank] += 1.  Integer atomics: the sums do not depend on their order.
+// item_mode: a value -1 (a padded or unresolvable item) never matches.
+__global__ void sid_topk_rank_hist_kernel(const int64_t* __restrict__ actual, int64_t a_stride, const int64_t* __restrict__ cand,
+                                          int64_t c_stride, int B, int k, int D, int item_mode, unsigned long long* __restrict__ hist) {
+  for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < B; b += gridDim.x * blockDim.x) {
+    const int64_t* a = actual + (int64_t)b * a_stride;
+    const int64_t* c = cand + (int64_t)b * c_stride;
+    int rank = k;
+    for (int j = 0; j < k && rank == k; ++j) {
+      bool match = true;
+      for (int d = 0; d < D && match; ++d) {
+        const int64_t v = a[d];
+        match = c[(int64_t)j * D + d] == v && !(item_mode && v == -1);
+      }
+      if (match) rank = j;
+    }
+    atomicAdd(hist + rank, 1ull);
+  }
+}
+
+extern "C" int rqb200_sid_topk_rank_hist(const int64_t* actual, int64_t a_stride, const int64_t* cand, int64_t c_stride, int B, int k,
+                                         int D, int item_mode, int64_t* hist, void* stream) {
+  RQB_CHECK_ARG(B >= 0 && k > 0 && D > 0 && a_stride >= D && c_stride >= (int64_t)k * D,
+                "sid_topk_rank_hist: bad argument (B = %d, k = %d, D = %d)", B, k, D);
+  if (B == 0) return RQB_OK;
+  RQB_CHECK_ARG(actual && cand && hist, "sid_topk_rank_hist: null pointer");
+  int grid = (B + 255) / 256;
+  if (grid > 132 * 8) grid = 132 * 8;
+  sid_topk_rank_hist_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      actual, a_stride, cand, c_stride, B, k, D, item_mode, reinterpret_cast<unsigned long long*>(hist));
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
 }

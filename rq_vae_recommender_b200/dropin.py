@@ -10,7 +10,8 @@ the replacement modules of this package; everything else (data/, evaluate/, the 
 tree untouched.  ``replace_model=True`` also aliases ``modules.model`` (train_decoder.py:14), whose
 ``EncoderDecoderRetrievalModel.generate`` then runs its beam search on the fused sampling and selection kernel;
 ``search="beam"`` (with ``replace_model=True``) makes the exhaustive, deterministic beam search over every code its default, so
-an unmodified ``train_decoder.py`` evaluates with it.  Checkpoints pickle ``modules.quantize.Quantize`` etc. by module path,
+an unmodified ``train_decoder.py`` evaluates with it.  ``replace_metrics=True`` also aliases ``evaluate.metrics``
+(train_decoder.py:13), whose ``TopKAccumulator`` accumulates on the device without waiting on the host.  Checkpoints pickle ``modules.quantize.Quantize`` etc. by module path,
 so ``torch.load(..., weights_only=False)`` of the shipped files also lands on the replacement classes.
 gin-config is not in this image: a small compatible shim is registered as ``gin`` when the real one is missing.
 """
@@ -29,9 +30,11 @@ _ALIASES = {
 }
 _TOKENIZER = ("modules.tokenizer.semids", "rq_vae_recommender_b200.modules.tokenizer.semids")
 _MODEL = ("modules.model", "rq_vae_recommender_b200.modules.model")
+_METRICS = ("evaluate.metrics", "rq_vae_recommender_b200.evaluate.metrics")
 
 
-def install(reference_root=None, replace_tokenizer=True, gin_shim=True, replace_model=False, search="sample"):
+def install(reference_root=None, replace_tokenizer=True, gin_shim=True, replace_model=False, search="sample",
+            replace_metrics=False):
     if search not in ("sample", "beam"):
         raise ValueError(f"search must be 'sample' or 'beam', got {search!r}")
     if search != "sample" and not replace_model:
@@ -44,7 +47,8 @@ def install(reference_root=None, replace_tokenizer=True, gin_shim=True, replace_
             sys.modules["gin"] = gin_compat
     if reference_root is not None and reference_root not in sys.path:
         sys.path.insert(0, reference_root)
-    for parent in ("init", "distributions"):          # namespace packages in the reference (no __init__.py)
+    parents = ("init", "distributions") + (("evaluate",) if replace_metrics else ())
+    for parent in parents:                             # namespace packages in the reference (no __init__.py)
         if parent not in sys.modules and reference_root is None:
             sys.modules[parent] = types.ModuleType(parent)
             sys.modules[parent].__path__ = []
@@ -55,11 +59,14 @@ def install(reference_root=None, replace_tokenizer=True, gin_shim=True, replace_
     if replace_model:
         sys.modules[_MODEL[0]] = importlib.import_module(_MODEL[1])
         sys.modules[_MODEL[0]].DEFAULT_SEARCH = search
-    return sorted(list(_ALIASES) + ([_TOKENIZER[0]] if replace_tokenizer else []) + ([_MODEL[0]] if replace_model else []))
+    if replace_metrics:
+        sys.modules[_METRICS[0]] = importlib.import_module(_METRICS[1])
+    return sorted(list(_ALIASES) + ([_TOKENIZER[0]] if replace_tokenizer else []) + ([_MODEL[0]] if replace_model else [])
+                  + ([_METRICS[0]] if replace_metrics else []))
 
 
 def uninstall():
-    for alias in list(_ALIASES) + [_TOKENIZER[0], _MODEL[0]]:
+    for alias in list(_ALIASES) + [_TOKENIZER[0], _MODEL[0], _METRICS[0]]:
         mod = sys.modules.get(alias)
         if mod is not None and mod.__name__.startswith("rq_vae_recommender_b200"):
             del sys.modules[alias]

@@ -16,6 +16,10 @@ passes are plain torch on HF T5, as in the reference.  What differs is the searc
 Shapes outside the kernel's limits (codebooks above 2048 codes, top_k * 64 candidates above 1024, top_k above 32) raise
 ``Rqb200Error``; there is no fallback to the reference's search.
 
+``generate_items`` turns the beams into corpus items: one more launch (``ops.SidItemTable.retrieve``) after ``generate``, through
+an item table of ``codebooks`` that is cached like the prefix index.  ``item_of`` resolves ``sem_ids_fut`` (ids plus the dedup
+column) to the true next item.
+
 ``generate(..., search="beam")`` runs a different search instead: an exhaustive, deterministic beam search over every code
 (``SidPrefixIndex.beam_topk``: per level the head and ONE kernel that scores all top_k x K extensions by log_softmax plus the
 parent's log-probability and keeps the k best valid ones; no sampling, no draw from any generator).  ``DEFAULT_SEARCH`` picks the
@@ -60,6 +64,16 @@ class GenerationOutput(NamedTuple):
     log_probas: Tensor
 
 
+class ItemGenerationOutput(NamedTuple):
+    """generate_items: the corpus items of the beams (item_ids [B, n] int64 and the source beam of each, beams [B, n] int32,
+    both -1 past count [B] int32), and generate's own beams (sem_ids [B, top_k, H], log_probas [B, top_k])."""
+    item_ids: Tensor
+    beams: Tensor
+    count: Tensor
+    sem_ids: Tensor
+    log_probas: Tensor
+
+
 def draw_exponential(probas: Tensor) -> Tensor:
     """The Exp(1) draw ``torch.multinomial(probas, n)`` (without replacement) makes from the default generator: sampling is
     then ``topk(probas / draw, n)``.  Patch this function to inject noise."""
@@ -97,6 +111,7 @@ class EncoderDecoderRetrievalModel(nn.Module):
         self.user_embedding = nn.Embedding(num_user_bins, t5_d_model) if num_user_bins else None
         self.sep_token = nn.Parameter(torch.randn(1, t5_d_model), requires_grad=True) if should_add_sep_token else None
         self._prefix_index_cache = None
+        self._item_table_cache = None
 
     @property
     def device(self) -> torch.device:
@@ -189,6 +204,15 @@ class EncoderDecoderRetrievalModel(nn.Module):
             self._prefix_index_cache = (key, index)
         return self._prefix_index_cache[1]
 
+    def _item_table(self, device: torch.device) -> ops.SidItemTable:
+        """The corpus item table (row n of codebooks is item n), cached on the same key as the prefix index."""
+        cb = self.codebooks
+        key = (id(cb), cb._version, cb.device, torch.device(device))
+        if self._item_table_cache is None or self._item_table_cache[0] != key:
+            table = ops.SidItemTable(cb[:, :self.num_hierarchies].to(device), self.num_embeddings_per_hierarchy)
+            self._item_table_cache = (key, table)
+        return self._item_table_cache[1]
+
     def _check_valid_prefix(self, prefix: Tensor, batch_size: int = 100000) -> Tensor:
         """bool [P]: some corpus row starts with prefix[p] (batch_size is accepted for the reference's signature)."""
         return self._prefix_index(prefix.device).check(prefix)
@@ -267,3 +291,21 @@ class EncoderDecoderRetrievalModel(nn.Module):
                                               input_ids=_strip_dedup_col(batch.sem_ids, H + 1, H), user_id=batch.user_ids,
                                               search=search)
         return GenerationOutput(sem_ids=generated, log_probas=log_probas)
+
+    @torch.no_grad()
+    def generate_items(self, batch: TokenizedSeqBatch, n: Optional[int] = None,
+                       search: Optional[str] = None) -> ItemGenerationOutput:
+        """The top corpus items for each history: ``generate_next_sem_id``'s beams, unchanged, then one launch that takes the
+        items of every finite beam whose ids are in the corpus, beam by beam in descending score order, each beam's items by
+        dedup rank, no item twice, at most n (default top_k_for_generation) per history."""
+        out = self.generate_next_sem_id(batch, search=search)
+        table = self._item_table(out.sem_ids.device)
+        items, beams, count = table.retrieve(out.sem_ids, out.log_probas, self.top_k_for_generation if n is None else n)
+        return ItemGenerationOutput(item_ids=items, beams=beams, count=count, sem_ids=out.sem_ids, log_probas=out.log_probas)
+
+    @torch.no_grad()
+    def item_of(self, sem_ids_fut: Tensor) -> Tensor:
+        """int64 [B]: the corpus item of each row of ``TokenizedSeqBatch.sem_ids_fut`` (its H ids and the dedup column), -1
+        when the tuple is not in the corpus or the dedup rank exceeds its items."""
+        H = self.num_hierarchies
+        return self._item_table(sem_ids_fut.device).lookup(sem_ids_fut[:, :H + 1], with_dedup=True)

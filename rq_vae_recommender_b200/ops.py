@@ -721,6 +721,100 @@ class SidPrefixIndex:
         return out_g, out_p, out_parent
 
 
+class SidItemTable:
+    """Item table of a corpus id table [N, C] (rqb200_sid_items_build): maps generated id tuples back to the corpus items (rows)
+    that carry them.  Row n is item n; the items of one tuple come in ascending row order, which is dedup rank 0, 1, 2, ....
+    A row holding an id outside [0, codebook_size) is never retrieved.  Built once per corpus, one launch per call."""
+
+    MAX_K, MAX_N = 1024, 4096
+
+    def __init__(self, cached_ids: torch.Tensor, codebook_size: int):
+        _need_cuda(cached_ids)
+        lib = _lib.load()
+        ids = cached_ids.to(torch.int64).contiguous()
+        self.N, self.C = ids.shape
+        self.K = int(codebook_size)
+        self.device = ids.device
+        nbytes = lib.rqb200_sid_items_workspace_bytes(self.N, self.C, self.K)
+        if nbytes == 0:
+            raise _lib.Rqb200Error(f"item table: {self.N} rows of {self.C} ids over {self.K} codes is outside its limits "
+                                   "(N < 2^31 - 1, C <= 8, K <= 65536)")
+        #: device bytes the table holds (its build scratch included)
+        self.nbytes = int(nbytes)
+        self.ws = torch.empty(nbytes, dtype=torch.uint8, device=ids.device)
+        with torch.cuda.device(ids.device):
+            _lib.check(lib.rqb200_sid_items_build(_p(ids), self.N, self.C, self.K, _p(self.ws), nbytes, _stream()),
+                       "sid_items_build")
+        _count(1)                                             # one build call (the sort and the scan are several kernels)
+
+    def lookup(self, ids: torch.Tensor, with_dedup: bool = False) -> torch.Tensor:
+        """int64 [...]: the item of each tuple ids[..., :C] -- its first item, or with ``with_dedup`` the item of dedup rank
+        ids[..., C] -- or -1 when the tuple is not in the corpus or the rank is outside [0, count)."""
+        _need_cuda(ids)
+        width = self.C + (1 if with_dedup else 0)
+        if ids.shape[-1] != width:
+            raise ValueError(f"lookup: expected {width} columns (C = {self.C}{' + the dedup rank' if with_dedup else ''}), "
+                             f"got {ids.shape[-1]}")
+        lead = ids.shape[:-1]
+        rows = ids.to(torch.int64).reshape(-1, width)
+        if rows.stride(-1) != 1 or (rows.shape[0] > 1 and rows.stride(0) < width):
+            rows = rows.contiguous()
+        P = rows.shape[0]
+        out = torch.empty(P, dtype=torch.int64, device=ids.device)
+        with torch.cuda.device(ids.device):
+            _lib.check(_lib.load().rqb200_sid_items_lookup(_p(self.ws), _p(rows), max(rows.stride(0), 1), P, int(with_dedup),
+                                                           _p(out), _stream()), "sid_items_lookup")
+        _count(1)
+        return out.reshape(lead)
+
+    def retrieve(self, generated: torch.Tensor, log_probas: Optional[torch.Tensor], n: int):
+        """generated [B, k, C], log_probas [B, k] or None -> (items [B, n] int64, beam [B, n] int32, count [B] int32): per
+        history, in beam order, the items of every beam whose log-probability is above -inf and whose tuple is in the corpus,
+        each beam's in dedup-rank order, no item twice, cut off at n; -1 pads items and beam.  k <= 1024, n <= 4096."""
+        _need_cuda(generated, log_probas)
+        B, k, C = generated.shape
+        if C != self.C:
+            raise ValueError(f"retrieve: generated has {C} ids per beam, the item table {self.C}")
+        n = int(n)
+        generated = generated.to(torch.int64).contiguous()
+        if log_probas is not None:
+            log_probas = log_probas.to(torch.float32).reshape(B, k).contiguous()
+        dev = generated.device
+        items = torch.empty((B, n), dtype=torch.int64, device=dev)
+        beam = torch.empty((B, n), dtype=torch.int32, device=dev)
+        count = torch.empty((B,), dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.load().rqb200_sid_items_retrieve(_p(self.ws), _p(generated), _p(log_probas), B, k, C, n, _p(items),
+                                                             _p(beam), _p(count), _stream()), "sid_items_retrieve")
+        _count(1)
+        return items, beam, count
+
+
+def sid_topk_rank_hist(actual: torch.Tensor, candidates: torch.Tensor, hist: torch.Tensor, item_mode: bool = False) -> None:
+    """Adds the rank of every row to hist (int64 [k + 1], on the device): the first candidate candidates[b, j] ([B, k, D]) equal
+    to actual[b] ([B, D]) in all D columns, k when none is (evaluate/metrics.py's rule).  ``item_mode``: -1 never matches.
+    One launch; never waits on the host."""
+    _need_cuda(actual, candidates, hist)
+    if candidates.dim() != 3 or actual.dim() != 2 or actual.shape[0] != candidates.shape[0] or \
+            actual.shape[1] != candidates.shape[2]:
+        raise ValueError(f"rank histogram: actual {tuple(actual.shape)} must be [B, D] and candidates "
+                         f"{tuple(candidates.shape)} [B, k, D]")
+    B, k, D = candidates.shape
+    if hist.dtype != torch.int64 or hist.numel() < k + 1 or not hist.is_contiguous():
+        raise ValueError(f"rank histogram: hist must be a contiguous int64 tensor of at least k + 1 = {k + 1} elements")
+    actual = actual.to(torch.int64)
+    if actual.stride(1) != 1 or actual.stride(0) < D:
+        actual = actual.contiguous()
+    candidates = candidates.to(torch.int64)
+    if candidates.stride(2) != 1 or candidates.stride(1) != D or candidates.stride(0) < k * D:
+        candidates = candidates.contiguous()
+    with torch.cuda.device(hist.device):
+        _lib.check(_lib.load().rqb200_sid_topk_rank_hist(_p(actual), max(actual.stride(0), D), _p(candidates),
+                                                         max(candidates.stride(0), k * D), B, k, D, int(item_mode), _p(hist),
+                                                         _stream()), "sid_topk_rank_hist")
+    _count(1)
+
+
 def sid_gather(cached_ids: torch.Tensor, item_ids: torch.Tensor, seq_mask: Optional[torch.Tensor] = None,
                want_token_type: bool = True):
     """cached_ids[item_ids] -> [B, S*C] with -1 under the padding mask, and token_type_ids (semids.py:112-146), one launch."""
