@@ -77,6 +77,9 @@ int rqb200_rq_backward(int mode, const float* x, int64_t ldx, const float* const
  * state_bytes grows as K^2 L(L-1)/2 (the Gram tables): ~80 MB at K = 2048, L = 3, D = 768; ~0.55 GB at L = 8. */
 size_t rqb200_tokenize_tc_state_bytes(int D, int K, int L);
 int rqb200_tokenize_tc_supported(int D, int K, int L);
+/* Host only: 32 KB codebook ring stages `run` gives a CTA at this shape (3 or 4, whatever fits in 227 KB of shared memory
+ * next to the x image and the candidate words), 0 for an unsupported shape. */
+int rqb200_tokenize_tc_ring_stages(int D, int K, int L);
 int rqb200_tokenize_tc_prepare(const float* const* codebooks, int D, int K, int L, void* state, size_t state_bytes,
                                void* stream);
 int rqb200_tokenize_tc_run(const float* x, int64_t ldx, int B, const void* state, int D, int K, int L,

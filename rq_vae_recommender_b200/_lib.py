@@ -42,6 +42,7 @@ _SIGNATURES = {
                                    c_vp, c_vp, c_vp]),
     "rqb200_tokenize_tc_state_bytes": (c_size, [c_int, c_int, c_int]),
     "rqb200_tokenize_tc_supported": (c_int, [c_int, c_int, c_int]),
+    "rqb200_tokenize_tc_ring_stages": (c_int, [c_int, c_int, c_int]),
     "rqb200_tokenize_tc_prepare": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_size, c_vp]),
     "rqb200_tokenize_tc_run": (c_int, [c_vp, c_i64, c_int, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
     "rqb200_kmeans_assign_accumulate": (c_int, [c_vp, c_i64, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp,

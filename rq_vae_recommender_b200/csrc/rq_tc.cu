@@ -19,6 +19,7 @@
 
 int tcx_run(const float* x, int64_t ldx, int B, const void* state, int D, int K, int L, int64_t* ids, int* stats, int sm_count,
             cudaStream_t st);
+int tcx_ring_stages(int D, int K, int L);
 
 extern "C" int rqb200_tokenize_tc_supported(int D, int K, int L) {
   return (K >= TC_K && K <= TC_MAX_K && K % TC_K == 0 && D >= TC_KC && D <= TC_MAX_D && D % TC_KC == 0 && L >= 1 &&
@@ -28,6 +29,11 @@ extern "C" int rqb200_tokenize_tc_supported(int D, int K, int L) {
 extern "C" size_t rqb200_tokenize_tc_state_bytes(int D, int K, int L) {
   if (!rqb200_tokenize_tc_supported(D, K, L)) return 0;
   return tc_state_size(D, K, L);
+}
+
+extern "C" int rqb200_tokenize_tc_ring_stages(int D, int K, int L) {
+  if (!rqb200_tokenize_tc_supported(D, K, L)) return 0;
+  return tcx_ring_stages(D, K, L);
 }
 
 // ------------------------------------------------------------------------------------------------ prepare

@@ -530,6 +530,15 @@ __global__ void __launch_bounds__(TX_THREADS, 1) rq_tcx_blocked_kernel(const __g
   }
 }
 
+// the ring gets as many 32 KB stages (<= TX_NB_MAX) as fit under the 227 KB limit: 4 at K = 256 for every D and L (120 bytes
+// to spare at D = 768, L = 8), 3 at K > 256 with D = 768 and at some K > 256 with D = 640 or 704, 4 elsewhere.  tcx_run and
+// rqb200_tokenize_tc_ring_stages both take the depth from here.
+int tcx_ring_stages(int D, int K, int L) {
+  int nbs = TX_NB_MAX;
+  while (nbs > 2 && tcx_smem_bytes(D, K, L, nbs) > TX_SMEM_LIMIT) --nbs;
+  return nbs;
+}
+
 int tcx_run(const float* x, int64_t ldx, int B, const void* state, int D, int K, int L, int64_t* ids, int* stats, int sm_count,
             cudaStream_t st) {
   const char* base = reinterpret_cast<const char*>(state);
@@ -543,12 +552,8 @@ int tcx_run(const float* x, int64_t ldx, int B, const void* state, int D, int K,
   p.cbf = reinterpret_cast<const float*>(base + tc_off_cbf(K, L));
   p.blob = reinterpret_cast<const unsigned char*>(base + tc_off_blob(D, K, L));
   p.ids = ids; p.stats = stats;
-  // the ring gets as many 32 KB stages (<= TX_NB_MAX) as fit under the 227 KB limit: 4 at K = 256 for every D and L (120 bytes
-  // to spare at D = 768, L = 8), 3 at K > 256 with D = 768 and at some K > 256 with D = 640 or 704, 4 elsewhere
-  int nbs = TX_NB_MAX;
-  while (nbs > 2 && tcx_smem_bytes(D, K, L, nbs) > TX_SMEM_LIMIT) --nbs;
-  p.nb = nbs;
-  const size_t smem = tcx_smem_bytes(D, K, L, nbs);
+  p.nb = tcx_ring_stages(D, K, L);
+  const size_t smem = tcx_smem_bytes(D, K, L, p.nb);
   // K = 256: one accumulator holds a level; larger K is scored in 256-code blocks
   void (*const kernel)(TxParams) = K == TC_K ? rq_tcx_kernel : rq_tcx_blocked_kernel;
   RQB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
