@@ -297,6 +297,35 @@ int rqb200_sid_items_retrieve(const void* workspace, const int64_t* generated, c
 int rqb200_sid_topk_rank_hist(const int64_t* actual, int64_t a_stride, const int64_t* cand, int64_t c_stride, int B, int k, int D,
                               int item_mode, int64_t* hist, void* stream);
 
+/* ---- one step of the generative-retrieval model's T5 decoder (modules/model.py, generate(decoder="fused")), csrc/t5dec.cu ----
+ * HF T5 numerics in eval mode: attention without 1/sqrt(d) scaling, fp32 softmax, d_kv = 64 per head (inner = heads * 64).
+ * The GEMMs around these calls are the caller's.  fp32 throughout; strides in elements.
+ * t5dec_cross_attention : attention over the encoder output with keys/values stored ONCE per history.  q [B * nq, inner] (row
+ *                         stride ldq; rows b * nq .. b * nq + nq - 1 belong to history b), k / v [B * S, inner] (row stride ldkv:
+ *                         key s of history b is row b * S + s), mask [B, S] or null (a key whose mask is 0 gets -FLT_MAX added,
+ *                         torch.finfo(float32).min as in HF's eager mask), out [B * nq, inner] (row stride ldo).  One CTA per
+ *                         (head, history) reads the history's keys/values once for all its queries; any S >= 1.
+ *                         Limits: nq <= 32, B <= 65535 (RQB_ERR_UNSUPPORTED).
+ * t5dec_self_attention  : the causal self-attention of query position h (< H <= 8) for R beam rows.  qkv [R, 3 inner] (q | k | v,
+ *                         row stride ldqkv).  cache_k / cache_v hold slot j (position j) of row x at [j * slot_stride + x * inner];
+ *                         the row's own k / v are written to slot h.  Earlier positions j < h of row r are read from row
+ *                         anc[r, j] of slot j, anc = int32 [rows, H]: anc = anc_in when parent is null; with parent (int64 [R], the
+ *                         previous level's row of each beam) anc[r, j] = anc_in[parent[r], j] for j < h - 1 and anc[r, h - 1] =
+ *                         parent[r], and this call writes it to anc_out (which must not alias anc_in).  bias [heads, H, H] is added
+ *                         to the score of (query h, key j).  out [R, inner] (row stride ldo).
+ * t5dec_add_norm        : one sublayer boundary, one warp per row of x [R, D] (contiguous, updated in place):
+ *                         emb != null : x[r] = emb[ids[r * ids_stride] + id_offset] (row 0 for all r when ids is null; an id outside
+ *                                       [0, n_emb) gives a NaN row) -- the step's input embedding;
+ *                         else        : x[r] += delta[r] (row stride ld_delta; null: x unchanged);
+ *                         then out[r] = weight * (x[r] * rsqrt(mean(x[r]^2) + eps)) (T5LayerNorm), out [R, D] contiguous. */
+int rqb200_t5dec_cross_attention(const float* q, int64_t ldq, const float* k, const float* v, int64_t ldkv, const float* mask, int B,
+                                 int nq, int S, int heads, float* out, int64_t ldo, void* stream);
+int rqb200_t5dec_self_attention(const float* qkv, int64_t ldqkv, float* cache_k, float* cache_v, int64_t slot_stride,
+                                const float* bias, const int* anc_in, const int64_t* parent, int* anc_out, int R, int heads, int h,
+                                int H, float* out, int64_t ldo, void* stream);
+int rqb200_t5dec_add_norm(float* x, const float* delta, int64_t ld_delta, const float* emb, const int64_t* ids, int64_t ids_stride,
+                          int64_t id_offset, int64_t n_emb, const float* weight, int R, int D, float eps, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -24,6 +24,10 @@ column) to the true next item.
 (``SidPrefixIndex.beam_topk``: per level the head and ONE kernel that scores all top_k x K extensions by log_softmax plus the
 parent's log-probability and keeps the k best valid ones; no sampling, no draw from any generator).  ``DEFAULT_SEARCH`` picks the
 search when ``generate`` / ``generate_next_sem_id`` are not given one (``dropin.install(search=...)`` sets it).
+
+``generate(..., decoder="fused")`` replaces only the decoder passes and their cache with ``FusedT5Decode`` (the decoder-step kernels
+of csrc/t5dec.cu between cuBLAS GEMMs, cross keys/values once per history, no cache copies); ``DEFAULT_DECODER`` ("hf") picks
+the decoder when none is given (``dropin.install(decoder=...)`` sets it).
 """
 from typing import NamedTuple
 from typing import Optional
@@ -49,6 +53,10 @@ MAX_CANDIDATES = 64
 #: the search generate() runs when it is not given one: "sample" (the reference's sampled beam search) or "beam" (exhaustive)
 DEFAULT_SEARCH = "sample"
 SEARCHES = ("sample", "beam")
+#: the decoder passes generate() runs when it is not given a decoder: "hf" (transformers' T5Stack with its cache, as the
+#: reference) or "fused" (FusedT5Decode: cross keys/values once per history, the decoder-step kernels of csrc/t5dec.cu)
+DEFAULT_DECODER = "hf"
+DECODERS = ("hf", "fused")
 _MULTINOMIAL_ERRORS = ("probability tensor contains either `inf`, `nan` or element < 0",
                        "invalid multinomial distribution (sum of probabilities <= 0)")
 
@@ -85,6 +93,69 @@ def _strip_dedup_col(tensor: Tensor, sem_ids_dim: int, n_layers: int) -> Tensor:
     B, width = tensor.shape
     items = width // sem_ids_dim
     return tensor.view(B, items, sem_ids_dim)[:, :, :n_layers].contiguous().view(B, items * n_layers)
+
+
+class FusedT5Decode:
+    """The decoder passes of one ``generate(decoder="fused")`` call: HF's T5Stack (eval mode, relu FFN, d_kv 64) restated as
+    cuBLAS GEMMs (``F.linear``) between the decoder-step kernels of csrc/t5dec.cu, with the key/value state laid out so that no
+    level copies it:
+      * cross-attention keys/values are projected ONCE, from the encoder output of the B histories, for every layer in one GEMM
+        (``cross_kv`` [B * S, layers * 2 * inner]), and each history's are read once per level for all of its beams;
+      * self-attention keys/values of position j live in slot j of ``cache`` [layers, 2, H, B * k, inner]; a beam reads its past
+        through an int32 ancestor table [B * k, H] that ``step`` advances from the search's parent_global (no reorder copy);
+      * level 1 reuses level 0's BOS keys/values: the BOS position depends only on the history.
+    ``step(h, generated, parent)`` returns the final-layer-normed hidden state [rows, d_model] of query position h."""
+
+    def __init__(self, model: "EncoderDecoderRetrievalModel", enc_out: Tensor, enc_mask: Tensor, k: int):
+        dec = model.t5_decoder
+        cfg = dec.config
+        if cfg.d_kv != ops.T5_DKV or cfg.is_gated_act or cfg.dense_act_fn != "relu":
+            raise Rqb200Error(f"decoder=\"fused\" needs d_kv = {ops.T5_DKV} and a relu feed-forward (d_kv = {cfg.d_kv}, "
+                              f"feed_forward_proj = {cfg.feed_forward_proj!r})")
+        self.model, self.k, self.H = model, k, model.num_hierarchies
+        self.heads, self.eps = cfg.num_heads, cfg.layer_norm_epsilon
+        self.blocks = [blk.layer for blk in dec.block]
+        self.norms = [w for lay in self.blocks for w in (lay[0].layer_norm.weight, lay[1].layer_norm.weight,
+                                                         lay[2].layer_norm.weight)] + [dec.final_layer_norm.weight]
+        self.w_qkv = [torch.cat([lay[0].SelfAttention.q.weight, lay[0].SelfAttention.k.weight, lay[0].SelfAttention.v.weight])
+                      for lay in self.blocks]
+        B, S, d = enc_out.shape
+        self.B, self.S, inner = B, S, self.heads * ops.T5_DKV
+        self.inner = inner
+        w_kv = torch.cat([w for lay in self.blocks for w in (lay[1].EncDecAttention.k.weight, lay[1].EncDecAttention.v.weight)])
+        #: [B * S, layers * 2 * inner]: layer l's cross keys at columns 2 l inner, its values at (2 l + 1) inner
+        self.cross_kv = F.linear(enc_out.reshape(B * S, d), w_kv)
+        self.mask = enc_mask.to(torch.float32).contiguous()
+        self.bias = dec.block[0].layer[0].SelfAttention.compute_bias(self.H, self.H)[0].contiguous()
+        self.cache = torch.empty((len(self.blocks), 2, self.H, B * k, inner), dtype=torch.float32, device=enc_out.device)
+        self.anc = torch.empty((B * k, self.H), dtype=torch.int32, device=enc_out.device)
+        self._anc_next = torch.empty_like(self.anc)
+
+    def step(self, h: int, generated: Optional[Tensor], parent: Optional[Tensor]) -> Tensor:
+        m, eps, inner = self.model, self.eps, self.inner
+        nq = 1 if h == 0 else self.k
+        R = self.B * nq
+        x = torch.empty((R, m.bos_token.shape[1]), dtype=torch.float32, device=self.cross_kv.device)
+        nrm = torch.empty_like(x)
+        if h == 0:
+            ops.t5dec_add_norm(x, None, self.norms[0], nrm, eps, emb=m.bos_token)
+        else:
+            ops.t5dec_add_norm(x, None, self.norms[0], nrm, eps, emb=m.item_sid_embedding_table.weight,
+                               ids=generated.reshape(R, h)[:, h - 1], offset=(h - 1) * m.num_embeddings_per_hierarchy)
+        for l, lay in enumerate(self.blocks):
+            advance = h > 0 and l == 0
+            a = ops.t5dec_self_attention(F.linear(nrm, self.w_qkv[l]), self.cache[l, 0], self.cache[l, 1], self.bias, h,
+                                         self.anc, parent if advance else None, self._anc_next if advance else None)
+            if advance:
+                self.anc, self._anc_next = self._anc_next, self.anc
+            ops.t5dec_add_norm(x, F.linear(a, lay[0].SelfAttention.o.weight), self.norms[3 * l + 1], nrm, eps)
+            kv = self.cross_kv[:, 2 * l * inner:(2 * l + 2) * inner]
+            a = ops.t5dec_cross_attention(F.linear(nrm, lay[1].EncDecAttention.q.weight), kv[:, :inner], kv[:, inner:],
+                                          self.mask, nq, self.heads)
+            ops.t5dec_add_norm(x, F.linear(a, lay[1].EncDecAttention.o.weight), self.norms[3 * l + 2], nrm, eps)
+            ff = lay[2].DenseReluDense
+            ops.t5dec_add_norm(x, F.linear(F.linear(nrm, ff.wi.weight).relu_(), ff.wo.weight), self.norms[3 * l + 3], nrm, eps)
+        return nrm
 
 
 class EncoderDecoderRetrievalModel(nn.Module):
@@ -235,37 +306,57 @@ class EncoderDecoderRetrievalModel(nn.Module):
         else:
             raise ValueError(f"generate: search must be one of {SEARCHES}, got {search!r}")
 
+    def _fused_decoder(self, enc_out: Tensor, enc_mask: Tensor, k: int) -> FusedT5Decode:
+        return FusedT5Decode(self, enc_out, enc_mask, k)
+
     @torch.no_grad()
-    def generate(self, attention_mask, input_ids, user_id=None, search: Optional[str] = None):
+    def generate(self, attention_mask, input_ids, user_id=None, search: Optional[str] = None, decoder: Optional[str] = None):
         """Top-k semantic ids by beam search restricted to id prefixes of the corpus.  ``search`` (default: the module's
         ``DEFAULT_SEARCH``, read at call time):
           "sample"  per level, n_cands = min(64, K) tokens sampled without replacement per beam, scored by cumulative
                     log-probability, prefixes absent from the corpus scored -inf, the k best kept (the reference's search);
           "beam"    per level, every code of every beam scored by cumulative log-probability, the k best valid extensions kept
                     (equal scores: lowest beam * K + code first); deterministic, draws no random numbers.
+        ``decoder`` (default: the module's ``DEFAULT_DECODER``, read at call time):
+          "hf"      transformers' T5Stack with an EncoderDecoderCache, as the reference drives it;
+          "fused"   ``FusedT5Decode``: the same T5 maths with cross keys/values once per history and the decoder-step kernels of
+                    csrc/t5dec.cu; eval mode only (HF would apply dropout in training mode).
         Returns generated [B, top_k, num_hierarchies] and log_probas [B, top_k]."""
         search = DEFAULT_SEARCH if search is None else search
+        decoder = DEFAULT_DECODER if decoder is None else decoder
+        if decoder not in DECODERS:
+            raise ValueError(f"generate: decoder must be one of {DECODERS}, got {decoder!r}")
+        if decoder == "fused" and self.training:
+            raise ValueError("generate: decoder=\"fused\" runs the decoder in eval mode only; call model.eval() first (in "
+                             "training mode HF's decoder applies dropout)")
         k = self.top_k_for_generation
         n_cands = min(MAX_CANDIDATES, self.num_embeddings_per_hierarchy)
         self._check_search_limits(search, k, n_cands)
         beam = search == "beam"
         enc_out, enc_mask = self.encoder_forward_pass(attention_mask=attention_mask, input_ids=input_ids, user_id=user_id)
         index = self._prefix_index(enc_out.device)
-        rep_enc, rep_mask = enc_out.repeat_interleave(k, dim=0), enc_mask.repeat_interleave(k, dim=0)
+        fused = self._fused_decoder(enc_out, enc_mask, k) if decoder == "fused" else None
+        if fused is None:
+            rep_enc, rep_mask = enc_out.repeat_interleave(k, dim=0), enc_mask.repeat_interleave(k, dim=0)
+            past_kv = EncoderDecoderCache(DynamicCache(), DynamicCache())
         reject = torch.zeros(1 if beam else 2, dtype=torch.int32, device=enc_out.device)
-        generated, log_probas = None, None
-        past_kv = EncoderDecoderCache(DynamicCache(), DynamicCache())
+        generated, log_probas, parent_global = None, None, None
         for h in range(self.num_hierarchies):
             first = generated is None
-            dec_out, past_kv = self.decoder_forward_pass(
-                future_ids=None if first else generated.reshape(-1, h), encoder_output=enc_out if first else rep_enc,
-                attention_mask_for_encoder=enc_mask if first else rep_mask, use_cache=True, past_key_values=past_kv)
-            logits = self.decoder_mlp[h](dec_out[:, -1, :])
+            if fused is not None:
+                logits = self.decoder_mlp[h](fused.step(h, generated, parent_global))
+            else:
+                dec_out, past_kv = self.decoder_forward_pass(
+                    future_ids=None if first else generated.reshape(-1, h), encoder_output=enc_out if first else rep_enc,
+                    attention_mask_for_encoder=enc_mask if first else rep_mask, use_cache=True, past_key_values=past_kv)
+                logits = self.decoder_mlp[h](dec_out[:, -1, :])
             if beam:
                 generated, log_probas, parent_global = index.beam_topk(logits, generated, log_probas, k, bad=reject)
             else:
                 generated, log_probas, parent_global = self._sample_and_select(index, F.softmax(logits, dim=-1), generated,
                                                                                log_probas, k, n_cands, reject)
+            if fused is not None:
+                continue
             if first:
                 past_kv = EncoderDecoderCache(DynamicCache(), DynamicCache())   # level 1 re-runs the decoder on B * k rows
             else:
@@ -285,20 +376,20 @@ class EncoderDecoderRetrievalModel(nn.Module):
 
     @torch.no_grad()
     def generate_next_sem_id(self, batch: TokenizedSeqBatch, top_k: bool = True, temperature: int = 1,
-                             search: Optional[str] = None) -> GenerationOutput:
+                             search: Optional[str] = None, decoder: Optional[str] = None) -> GenerationOutput:
         H = self.num_hierarchies
         generated, log_probas = self.generate(attention_mask=_strip_dedup_col(batch.seq_mask.long(), H + 1, H),
                                               input_ids=_strip_dedup_col(batch.sem_ids, H + 1, H), user_id=batch.user_ids,
-                                              search=search)
+                                              search=search, decoder=decoder)
         return GenerationOutput(sem_ids=generated, log_probas=log_probas)
 
     @torch.no_grad()
-    def generate_items(self, batch: TokenizedSeqBatch, n: Optional[int] = None,
-                       search: Optional[str] = None) -> ItemGenerationOutput:
+    def generate_items(self, batch: TokenizedSeqBatch, n: Optional[int] = None, search: Optional[str] = None,
+                       decoder: Optional[str] = None) -> ItemGenerationOutput:
         """The top corpus items for each history: ``generate_next_sem_id``'s beams, unchanged, then one launch that takes the
         items of every finite beam whose ids are in the corpus, beam by beam in descending score order, each beam's items by
         dedup rank, no item twice, at most n (default top_k_for_generation) per history."""
-        out = self.generate_next_sem_id(batch, search=search)
+        out = self.generate_next_sem_id(batch, search=search, decoder=decoder)
         table = self._item_table(out.sem_ids.device)
         items, beams, count = table.retrieve(out.sem_ids, out.log_probas, self.top_k_for_generation if n is None else n)
         return ItemGenerationOutput(item_ids=items, beams=beams, count=count, sem_ids=out.sem_ids, log_probas=out.log_probas)

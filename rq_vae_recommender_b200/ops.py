@@ -840,6 +840,116 @@ def sid_gather(cached_ids: torch.Tensor, item_ids: torch.Tensor, seq_mask: Optio
     return out, tt
 
 
+# ---------------------------------------------------------------------------------------------- fused T5 decoder step
+T5_DKV = 64       # d_kv the decoder-step kernels are built for (csrc/t5dec.cu)
+
+
+def _rows_of(t: torch.Tensor, width: int, what: str) -> torch.Tensor:
+    t = _rows(t)
+    if t.shape[1] != width:
+        raise ValueError(f"{what}: expected {width} columns, got {tuple(t.shape)}")
+    return t
+
+
+def t5dec_cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, mask: Optional[torch.Tensor], nq: int,
+                          heads: int) -> torch.Tensor:
+    """T5 cross-attention over keys/values stored once per history (rqb200_t5dec_cross_attention), one launch.
+    q [B * nq, heads * 64] (history b owns rows b * nq ...), k / v [B * S, heads * 64] (any row stride), mask [B, S] (0 masks a
+    key: -FLT_MAX is added to its score, as HF's eager mask) or None -> [B * nq, heads * 64]."""
+    _need_cuda(q, k, v, mask)
+    inner = heads * T5_DKV
+    q, k, v = _rows_of(q, inner, "q"), _rows_of(k, inner, "k"), _rows_of(v, inner, "v")
+    if q.shape[0] % nq:
+        raise ValueError(f"q has {q.shape[0]} rows, not a multiple of nq = {nq}")
+    B = q.shape[0] // nq
+    if B == 0 or k.shape != v.shape or k.shape[0] == 0 or k.shape[0] % B:
+        raise ValueError(f"k {tuple(k.shape)} / v {tuple(v.shape)} must both be [B * S, {inner}] with B = {B} > 0, S > 0")
+    if k.stride(0) != v.stride(0):
+        k, v = k.contiguous(), v.contiguous()
+    S = k.shape[0] // B
+    if mask is not None:
+        mask = _f32c(mask)
+        if mask.shape != (B, S):
+            raise ValueError(f"mask {tuple(mask.shape)} must be [B, S] = [{B}, {S}]")
+    out = torch.empty((q.shape[0], inner), dtype=torch.float32, device=q.device)
+    with torch.cuda.device(q.device):
+        _lib.check(_lib.load().rqb200_t5dec_cross_attention(_p(q), q.stride(0), _p(k), _p(v), k.stride(0), _p(mask), B, nq, S,
+                                                            heads, _p(out), out.stride(0), _stream()), "t5dec_cross_attention")
+    _count(1)
+    return out
+
+
+def t5dec_self_attention(qkv: torch.Tensor, cache_k: torch.Tensor, cache_v: torch.Tensor, bias: torch.Tensor, h: int,
+                         anc_in: Optional[torch.Tensor], parent: Optional[torch.Tensor] = None,
+                         anc_out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The causal T5 self-attention of query position h for R beam rows (rqb200_t5dec_self_attention), one launch.
+    qkv [R, 3 * heads * 64] (q | k | v); cache_k / cache_v [H, rows, heads * 64] contiguous, rows >= R: the rows' k / v are written
+    to slot h, position j < h of row r is read from row anc[r, j] of slot j; bias [heads, H, H] (HF's compute_bias(H, H)[0]).
+    anc = anc_in (int32 [*, H]) when parent is None; with parent (int64 [R]) anc[r] = anc_in[parent[r]] with position h - 1 set
+    to parent[r], written to anc_out (int32 [R', H], R' >= R, not anc_in).  Returns [R, heads * 64]."""
+    _need_cuda(qkv, cache_k, cache_v, bias, anc_in, parent, anc_out)
+    H, rows, inner = cache_k.shape
+    heads = inner // T5_DKV
+    qkv = _rows_of(qkv, 3 * inner, "qkv")
+    R = qkv.shape[0]
+    if cache_v.shape != cache_k.shape or not (cache_k.is_contiguous() and cache_v.is_contiguous()) or rows < R or \
+            cache_k.dtype != torch.float32 or cache_v.dtype != torch.float32:
+        raise ValueError(f"cache_k / cache_v must be contiguous fp32 [H, rows >= {R}, {inner}]")
+    bias = _f32c(bias)
+    if bias.shape != (heads, H, H):
+        raise ValueError(f"bias {tuple(bias.shape)} must be [{heads}, {H}, {H}]")
+    for name, t in (("anc_in", anc_in), ("anc_out", anc_out)):
+        if t is not None and (t.dtype != torch.int32 or t.dim() != 2 or t.shape[1] != H or not t.is_contiguous()):
+            raise ValueError(f"{name} must be a contiguous int32 [rows, {H}] tensor")
+    if parent is not None:
+        parent = parent.to(torch.int64).contiguous()
+        if parent.shape != (R,) or anc_out is None or anc_out.shape[0] < R or (anc_in is not None and
+                                                                               anc_out.data_ptr() == anc_in.data_ptr()):
+            raise ValueError("parent must be [R] and comes with an anc_out of at least R rows that is not anc_in")
+    elif anc_in is not None and anc_in.shape[0] < R:
+        raise ValueError(f"anc_in has {anc_in.shape[0]} rows, fewer than R = {R}")
+    out = torch.empty((R, inner), dtype=torch.float32, device=qkv.device)
+    with torch.cuda.device(qkv.device):
+        _lib.check(_lib.load().rqb200_t5dec_self_attention(_p(qkv), qkv.stride(0), _p(cache_k), _p(cache_v), rows * inner, _p(bias),
+                                                           _p(anc_in), _p(parent), _p(anc_out), R, heads, int(h), H, _p(out),
+                                                           out.stride(0), _stream()), "t5dec_self_attention")
+    _count(1)
+    return out
+
+
+def t5dec_add_norm(x: torch.Tensor, delta: Optional[torch.Tensor], weight: torch.Tensor, out: torch.Tensor, eps: float,
+                   emb: Optional[torch.Tensor] = None, ids: Optional[torch.Tensor] = None, offset: int = 0) -> torch.Tensor:
+    """A T5 sublayer boundary (rqb200_t5dec_add_norm), one launch: x += delta in place -- or, with emb [V, D], x = emb[ids + offset]
+    (ids int64 [R], any stride; emb[0] for every row when ids is None) -- then out = T5LayerNorm(x) * weight.  x, out [R, D]
+    contiguous fp32.  Returns out."""
+    _need_cuda(x, delta, weight, out, emb, ids)
+    R, D = x.shape
+    for name, t in (("x", x), ("out", out)):
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.shape != (R, D):
+            raise ValueError(f"{name} must be a contiguous fp32 [{R}, {D}] tensor")
+    weight = _f32c(weight)
+    if weight.shape != (D,):
+        raise ValueError(f"weight {tuple(weight.shape)} must be [{D}]")
+    if delta is not None:
+        delta = _rows_of(delta, D, "delta")
+        if delta.shape[0] != R:
+            raise ValueError(f"delta has {delta.shape[0]} rows, x {R}")
+    if emb is not None:
+        emb = _f32c(emb)
+        if emb.dim() != 2 or emb.shape[1] != D:
+            raise ValueError(f"emb {tuple(emb.shape)} must be [V, {D}]")
+    if ids is not None:
+        if ids.dtype != torch.int64 or ids.shape != (R,):
+            raise ValueError(f"ids must be int64 [{R}]")
+    with torch.cuda.device(x.device):
+        _lib.check(_lib.load().rqb200_t5dec_add_norm(_p(x), _p(delta), delta.stride(0) if delta is not None else 0, _p(emb), _p(ids),
+                                                     ids.stride(0) if ids is not None else 0, int(offset),
+                                                     emb.shape[0] if emb is not None else 0, _p(weight), R, D, float(eps), _p(out),
+                                                     _stream()), "t5dec_add_norm")
+    _count(1)
+    return out
+
+
 # ---------------------------------------------------------------------------------------------- tensor-core tokeniser
 def tc_supported(D: int, K: int, L: int) -> bool:
     return bool(_lib.load().rqb200_tokenize_tc_supported(D, K, L))
