@@ -39,6 +39,7 @@
 #define TX_SLOT_BYTES (TX_R * TC_KC * 2)          // one k chunk of the x image: 8 KB
 #define TX_THREADS 160
 #define TX_SMEM_LIMIT 232448                      // 227 KB of opt-in shared memory per block
+#define TX_GC 4                                   // column groups per chunk of Gram-row loads in tx_score (8 spills)
 
 struct TxSmem {
   uint64_t full[TX_NB_MAX], empty[TX_NB_MAX];
@@ -215,23 +216,37 @@ __device__ __forceinline__ void tx_score(float (&acc)[128], const TxParams& p, c
       acc[4 * jb + 2] = fmaf(acc[4 * jb + 2], ninv, t.x); acc[4 * jb + 3] = fmaf(acc[4 * jb + 3], ninv, t.y);
     }
   } else {
-    // Gram rows of the previous levels' ids, table (j, l) at gram + (l (l - 1) / 2 + j) K^2, summed in level order
-    const float* g0 = p.gram + (size_t)(l * (l - 1) / 2) * K * K + 2 * q4;
-    const float* a0 = g0 + (size_t)ids[r0] * K + col;
-    const float* a1 = g0 + (size_t)ids[r1] * K + col;
+    // Gram rows of the previous levels' ids, table (j, l) at gram + (l (l - 1) / 2 + j) K^2, summed in level order.  TX_GC
+    // column groups at a time: the loads of one table are independent, so a level costs l round trips to L2 per chunk rather
+    // than one per column group and table
+    const float* g0 = p.gram + (size_t)(l * (l - 1) / 2) * K * K + 2 * q4 + col;
+    const float* a0 = g0 + (size_t)ids[r0] * K;
+    const float* a1 = g0 + (size_t)ids[r1] * K;
 #pragma unroll
-    for (int jb = 0; jb < 32; ++jb) {
-      float2 t0 = __ldg(reinterpret_cast<const float2*>(a0 + 8 * jb));
-      float2 t1 = __ldg(reinterpret_cast<const float2*>(a1 + 8 * jb));
+    for (int jc = 0; jc < 32; jc += TX_GC) {
+      float2 t0[TX_GC], t1[TX_GC];
+#pragma unroll
+      for (int i = 0; i < TX_GC; ++i) {
+        t0[i] = __ldg(reinterpret_cast<const float2*>(a0 + 8 * (jc + i)));
+        t1[i] = __ldg(reinterpret_cast<const float2*>(a1 + 8 * (jc + i)));
+      }
 #pragma unroll 1
       for (int j = 1; j < l; ++j) {
-        const float* gj = g0 + (size_t)j * K * K + col + 8 * jb;
-        const float2 u0 = __ldg(reinterpret_cast<const float2*>(gj + (size_t)ids[j * TX_R + r0] * K));
-        const float2 u1 = __ldg(reinterpret_cast<const float2*>(gj + (size_t)ids[j * TX_R + r1] * K));
-        t0.x += u0.x; t0.y += u0.y; t1.x += u1.x; t1.y += u1.y;
+        const float* b0 = g0 + ((size_t)j * K + ids[j * TX_R + r0]) * K;
+        const float* b1 = g0 + ((size_t)j * K + ids[j * TX_R + r1]) * K;
+#pragma unroll
+        for (int i = 0; i < TX_GC; ++i) {
+          const float2 u0 = __ldg(reinterpret_cast<const float2*>(b0 + 8 * (jc + i)));
+          const float2 u1 = __ldg(reinterpret_cast<const float2*>(b1 + 8 * (jc + i)));
+          t0[i].x += u0.x; t0[i].y += u0.y; t1[i].x += u1.x; t1[i].y += u1.y;
+        }
       }
-      acc[4 * jb + 0] = fmaf(acc[4 * jb + 0], ninv, t0.x); acc[4 * jb + 1] = fmaf(acc[4 * jb + 1], ninv, t0.y);
-      acc[4 * jb + 2] = fmaf(acc[4 * jb + 2], ninv, t1.x); acc[4 * jb + 3] = fmaf(acc[4 * jb + 3], ninv, t1.y);
+#pragma unroll
+      for (int i = 0; i < TX_GC; ++i) {
+        const int jb = jc + i;
+        acc[4 * jb + 0] = fmaf(acc[4 * jb + 0], ninv, t0[i].x); acc[4 * jb + 1] = fmaf(acc[4 * jb + 1], ninv, t0[i].y);
+        acc[4 * jb + 2] = fmaf(acc[4 * jb + 2], ninv, t1[i].x); acc[4 * jb + 3] = fmaf(acc[4 * jb + 3], ninv, t1[i].y);
+      }
     }
   }
 }
