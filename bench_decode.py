@@ -73,7 +73,7 @@ def run_shape(torch, F, np, M, levels, w):
     ids = torch.from_numpy(rs.randint(0, K, size=(B, ITEMS * levels))).cuda()
     mask = torch.ones_like(ids)
     arms = [(dec, search) for search in ("sample", "beam") for dec in ("hf", "fused")]
-    res = {"levels": levels, "index": None}
+    res = {"levels": levels}
     outs = {}
     for dec, search in arms:
         m.generate(mask, ids, search=search, decoder=dec)    # warm-up (builds the index)
@@ -83,7 +83,6 @@ def run_shape(torch, F, np, M, levels, w):
         outs[dec, search] = m.generate(mask, ids, search=search, decoder=dec)
         torch.cuda.synchronize()
         res[f"{dec}_{search}_peak_bytes"] = torch.cuda.max_memory_allocated()
-    res["index"] = m._prefix_index(torch.device("cuda")).kind
     for search in ("sample", "beam"):
         (gh, ph), (gf, pf) = outs["hf", search], outs["fused", search]
         fin = torch.isfinite(ph) & torch.isfinite(pf)

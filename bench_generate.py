@@ -16,17 +16,16 @@ beam, K = 256 codes, 3 hierarchy levels), on a 12 101-row corpus (Amazon Beauty'
       beam_composed   torch: log_softmax, SidPrefixIndex.check of every extension, masked_fill, a stable descending sort,
                       gathers;
   * the two exhaustive arms again at top-k 32 and K = 2048 (65 536 candidates per history) on a 12 101-row corpus;
-  * the corpus prefix index: build ms and device bytes of the bitmap and of the trie (ops.SidPrefixIndex(kind=...)) on a
-    12 101-row corpus at K = 256, C = 3 (the shipped shape), K = 2048, C = 3 (1 GiB of bitmap) and K = 256, C = 4 (512 MiB);
-    and the fused and beam arms above again on the trie of the same corpora (fused_trie_ms, beam_trie_ms);
-  * per-level ms of sample_select (top-k 10, 64 candidates) and beam_topk (top-k 10) on the trie alone, where no bitmap fits:
-    K = 256 with C = 5 and 8, K = 1024 and 2048 with C = 4, and beam_topk at top-k 32 with K = 2048, C = 4 (65 536
+  * the corpus prefix index (the trie): build ms, the device bytes it keeps and the bytes of its build scratch, on a
+    12 101-row corpus at K = 256, C = 3 (the shipped shape), K = 2048, C = 3 and K = 256, C = 4, and on a 1 048 576-row
+    corpus at K = 256, C = 3;
+  * per-level ms of sample_select (top-k 10, 64 candidates) and beam_topk (top-k 10) at deeper hierarchies and larger
+    codebooks: K = 256 with C = 5 and 8, K = 1024 and 2048 with C = 4, and beam_topk at top-k 32 with K = 2048, C = 4 (65 536
     candidates per history), each on a 12 101-row corpus;
   * whole-generate ms of the drop-in EncoderDecoderRetrievalModel at the decoder_amazon.gin T5 shape (d_model 384, 6 heads,
     d_ff 1024, 4 layers, randomly initialised) on 20-item histories, of the same model with the composed arm in place of
     sample_select, under the same seed (their beams are compared), and of generate(search="beam"); three alternating windows
-    each; and generate(search="sample") and generate(search="beam") of the same T5 shape with 5 hierarchy levels at K = 256 (on
-    the trie).  Also the fraction of returned beams with a finite log-probability under each search (of this randomly
+    each; and generate(search="sample") and generate(search="beam") of the same T5 shape with 5 hierarchy levels at K = 256.  Also the fraction of returned beams with a finite log-probability under each search (of this randomly
     initialised model: it says how often a search runs out of valid prefixes, not how good its beams are).
 Every shape is warmed up, every timed window lasts at least --min-window-s seconds (CUDA events).  Prints the card's name,
 power limit and max SM clock, and one JSON line; writes nothing.
@@ -155,20 +154,24 @@ def beam_level_inputs(torch, index, k, codes, seed, levels=H):
     return out
 
 
-def build_ms(torch, ops, corpus, codes, kind, reps=5):
-    """Median ms of building the prefix index (host clock around the build and a device synchronise), and its bytes."""
+def build_ms(torch, ops, corpus, codes, reps=5):
+    """Median ms of building the prefix index (host clock around the build and a device synchronise), the bytes it keeps and
+    the bytes of its build scratch."""
     import time
+    from rq_vae_recommender_b200 import _lib
     times = []
     for _ in range(reps + 1):
         torch.cuda.synchronize()
         t0 = time.perf_counter()
-        index = ops.SidPrefixIndex(corpus, codes, kind=kind)
+        index = ops.SidPrefixIndex(corpus, codes)
         torch.cuda.synchronize()
         times.append((time.perf_counter() - t0) * 1e3)
         nbytes = index.nbytes
         del index
     times = sorted(times[1:])                                  # the first build loads the module
-    return {"build_ms": times[len(times) // 2], "bytes": nbytes}
+    rows, levels = corpus.shape
+    return {"build_ms": times[len(times) // 2], "bytes": nbytes,
+            "scratch_bytes": _lib.load().rqb200_sid_trie_scratch_bytes(rows, levels, codes)}
 
 
 def main():
@@ -186,20 +189,17 @@ def main():
     for name, rows in (("corpus_12101", 12101), ("corpus_1M", 1 << 20)):
         corpus = torch.from_numpy(corpus_of(np, rows, rows)).cuda()
         index = ops.SidPrefixIndex(corpus, K)
-        trie = ops.SidPrefixIndex(corpus, K, kind="trie")
         res = {}
         for h, (probas, logits, generated, log_probas) in enumerate(level_inputs(torch, F, index, 7)):
             arms = {"composed_ms": lambda: composed_level(torch, index, probas, generated, log_probas, TOP_K, NC),
                     "fused_ms": lambda: index.sample_select(probas, M.draw_exponential(probas), generated, log_probas, TOP_K, NC),
-                    "fused_trie_ms": lambda: trie.sample_select(probas, M.draw_exponential(probas), generated, log_probas, TOP_K, NC),
                     "beam_ms": lambda: index.beam_topk(logits, generated, log_probas, TOP_K),
-                    "beam_trie_ms": lambda: trie.beam_topk(logits, generated, log_probas, TOP_K),
                     "beam_composed_ms": lambda: beam_composed_level(torch, F, index, logits, generated, log_probas, TOP_K)}
             if rows < 100000:
                 arms["reference_ms"] = lambda: reference_level(torch, corpus, probas, generated, log_probas, TOP_K, NC)
             res[f"level{h}"] = {arm: timed_ms(torch, fn, w) for arm, fn in arms.items()}
         out[name] = res
-        del index, trie, corpus
+        del index, corpus
         torch.cuda.empty_cache()
     big_k, big_codes = 32, 2048                               # 65 536 candidates per history
     corpus = torch.from_numpy(corpus_of(np, 12101, 12101, big_codes)).cuda()
@@ -219,14 +219,17 @@ def main():
     builds = {}
     for codes, levels in ((K, 3), (2048, 3), (K, 4)):
         corpus = torch.from_numpy(corpus_of(np, 12101, 12101, codes, levels)).cuda()
-        builds[f"codes{codes}_levels{levels}"] = {kind: build_ms(torch, ops, corpus, codes, kind) for kind in ("bitmap", "trie")}
+        builds[f"codes{codes}_levels{levels}"] = build_ms(torch, ops, corpus, codes)
         torch.cuda.empty_cache()
     out["index_build_corpus_12101"] = builds
+    corpus = torch.from_numpy(corpus_of(np, 1 << 20, 1 << 20)).cuda()
+    out["index_build_corpus_1M"] = {f"codes{K}_levels{H}": build_ms(torch, ops, corpus, K)}
+    del corpus
+    torch.cuda.empty_cache()
     deep = {}
     for codes, levels in ((K, 5), (K, 8), (1024, 4), (2048, 4)):
         corpus = torch.from_numpy(corpus_of(np, 12101, 12101, codes, levels)).cuda()
         trie = ops.SidPrefixIndex(corpus, codes)
-        assert trie.kind == "trie"
         res = {}
         for h, (probas, logits, generated, log_probas) in enumerate(level_inputs(torch, F, trie, 9, codes, levels)):
             res[f"level{h}"] = {
@@ -272,7 +275,7 @@ def main():
                                                    "beam": float(torch.isfinite(p_b).float().mean())},
         "history_items": ITEMS, "t5": "d_model 384, 6 heads, d_ff 1024, 4 layers, random init, TF32 matmuls"}
     del fused, composed
-    deep_h = 5                                                # no bitmap fits K^5: the model builds the trie
+    deep_h = 5
     corpus5 = torch.from_numpy(corpus_of(np, 12101, 12101, K, deep_h))
     torch.manual_seed(0)
     model5 = M.EncoderDecoderRetrievalModel(codebooks=corpus5, **dict(shape, num_hierarchies=deep_h)).cuda().eval()
@@ -285,7 +288,7 @@ def main():
         sample5.append(timed_ms(torch, lambda: model5.generate(mask5, ids5), w))
         beam5.append(timed_ms(torch, lambda: model5.generate(mask5, ids5, search="beam"), w))
     out["generate_levels5"] = {
-        "index": model5._prefix_index(torch.device("cuda")).kind, "sample_ms": sample5, "beam_ms": beam5,
+        "sample_ms": sample5, "beam_ms": beam5,
         "finite_beam_fraction_random_init_model": {"sample": float(torch.isfinite(p_s5).float().mean()),
                                                    "beam": float(torch.isfinite(p_b5).float().mean())}}
     out["timed"] = ("CUDA events, windows >= %.1f s after warm-up; per-level arms start from the level's probabilities (beam arms: "

@@ -180,34 +180,26 @@ int rqb200_sid_gather(const int64_t* cached_ids, int64_t n_corpus, int C, const 
                       int64_t* token_type /* [B, S*C] or null */, void* stream);
 
 /* ---- constrained beam search, data side (modules/model.py:169-182 `_check_valid_prefix`, :340-376 the selection step) ----
- * Two indexes of the corpus id table [N, C] hold its valid prefixes: the prefixes of every row up to its first id outside
- * [0, K) (a prefix holding such an id is never valid; duplicated rows and N = 0 are legal).  Every search entry point exists
- * once per index, with the same arguments, limits and results: rqb200_sid_X on the bitmap, rqb200_sid_trie_X on the trie.
- *   bitmap  one bitmap per prefix length, K^l bits at length l (512 MiB at K = 256, l = 4); a check is one bit test.  Only
- *           for K^C <= 2^33 bits: sid_prefix_workspace_bytes returns 0 above that.
- *   trie    the distinct l-prefixes per level in lexicographic order, each node with its last code and the range of its
- *           children: O(N C) bytes for any K^C (N < 2^31 - 1, K <= 65536); a check is one binary search among a node's
- *           children per level.  The workspace holds the trie and its build scratch; the search calls need only the pointer.
- *           The build sorts on the stream (CUB radix sort and scans) and does not synchronise the host.
- * sid_prefix_build  : corpus id table [N, C] -> one bitmap per prefix length (workspace layout: levels 1..C, 256-byte aligned
- *                     regions; sid_prefix_workspace_bytes returns 0 when K^C exceeds 2^33 bits)
- * sid_trie_build    : the same table -> the trie (sid_trie_workspace_bytes returns 0 outside its limits or when the current
- *                     device cannot be queried)
- * sid_prefix_check  : valid[p] = some corpus row starts with prefix[p, :l]   (one bit test instead of the reference's
- *                     O(P N l) compare)
- * sid_beam_select   : one launch per hierarchy level h: score kp x nc candidate extensions per batch row (sampled token
- *                     log-probability + parent beam log-probability, -inf when the extended prefix is not in the corpus), keep
- *                     the k best in descending order, gather their ids into out_generated [B, k, h + 1] and return the parent
- *                     beam's global index b * kp + beam (the key/value-cache reorder index). */
-size_t rqb200_sid_prefix_workspace_bytes(int C, int K);
-int rqb200_sid_prefix_build(const int64_t* cached_ids, int64_t N, int C, int K, void* workspace, size_t ws_bytes, void* stream);
-int rqb200_sid_prefix_check(const int64_t* prefix, int64_t row_stride, int64_t P, int l, int C, int K, const void* workspace,
-                            unsigned char* valid, void* stream);
-int rqb200_sid_beam_select(const int64_t* samples, const float* samp_log_p, const int64_t* generated, const float* log_probas,
-                           int B, int kp, int nc, int h, int k, int C, int K, const void* prefix_workspace,
-                           int64_t* out_generated, float* out_log_probas, int64_t* out_parent, void* stream);
+ * A trie of the corpus id table [N, C] holds its valid prefixes: the prefixes of every row up to its first id outside [0, K)
+ * (a prefix holding such an id is never valid; duplicated rows and N = 0 are legal).  Level l holds the distinct l-prefixes in
+ * lexicographic order, each node with its last code and the range of its children.  Limits: N < 2^31 - 1, C <= 8, K <= 65536.
+ * sid_trie_workspace_bytes : bytes of the trie the search calls read, (4 (C - 1) + 2 C) N plus alignment; arithmetic only, no
+ *                            device.  0 outside the limits.
+ * sid_trie_scratch_bytes   : bytes of the build's scratch (the row sort and the per-level scans); queries CUB on the current
+ *                            device.  0 outside the limits or when the device cannot be queried.
+ * sid_trie_build           : corpus id table [N, C] -> the trie in `workspace`.  Sorts on the stream (CUB radix sort and scans)
+ *                            and does not synchronise the host; `scratch` may be reused once the stream has passed the build.
+ * sid_trie_check           : valid[p] = some corpus row starts with prefix[p, :l]   (one binary search among a node's children per
+ *                            level instead of the reference's O(P N l) compare)
+ * sid_trie_beam_select     : one launch per hierarchy level h: score kp x nc candidate extensions per batch row (sampled token
+ *                            log-probability + parent beam log-probability, -inf when the extended prefix is not in the corpus),
+ *                            keep the k best in descending order, gather their ids into out_generated [B, k, h + 1] and return
+ *                            the parent beam's global index b * kp + beam (the key/value-cache reorder index).
+ *                            Limits: kp * nc <= 1024, k <= 32, h < C <= 8. */
 size_t rqb200_sid_trie_workspace_bytes(int64_t N, int C, int K);
-int rqb200_sid_trie_build(const int64_t* cached_ids, int64_t N, int C, int K, void* workspace, size_t ws_bytes, void* stream);
+size_t rqb200_sid_trie_scratch_bytes(int64_t N, int C, int K);
+int rqb200_sid_trie_build(const int64_t* cached_ids, int64_t N, int C, int K, void* workspace, size_t ws_bytes, void* scratch,
+                          size_t scratch_bytes, void* stream);
 int rqb200_sid_trie_check(const int64_t* prefix, int64_t row_stride, int64_t P, int l, int C, int K, const void* workspace,
                           unsigned char* valid, void* stream);
 int rqb200_sid_trie_beam_select(const int64_t* samples, const float* samp_log_p, const int64_t* generated,
@@ -215,10 +207,10 @@ int rqb200_sid_trie_beam_select(const int64_t* samples, const float* samp_log_p,
                                 const void* prefix_workspace, int64_t* out_generated, float* out_log_probas, int64_t* out_parent,
                                 void* stream);
 
-/* sid_sample_select : the sampling step of the same beam search fused with sid_beam_select, one launch per level h
+/* sid_trie_sample_select : the sampling step of the same beam search fused with sid_trie_beam_select, one launch per level h
  *                     (modules/model.py:345-388 after the softmax).  torch.multinomial(p, nc) without replacement is
  *                     topk(p / q, nc) with q = empty_like(p).exponential_(1) from the same generator; given that q in `noise`,
- *                     this call reproduces its samples bit for bit and then selects exactly as sid_beam_select does:
+ *                     this call reproduces its samples bit for bit and then selects exactly as sid_trie_beam_select does:
  *   probas, noise    [B*kp, K] fp32, row strides in elements (kp = 1 at h = 0, where generated and log_probas are null)
  *   generated        [B, kp, h] int64, log_probas [B, kp] fp32: the beams entering the level
  *   per row          ratio = probas / noise (IEEE fp32 division), the nc largest ratios in torch.topk's order (descending, NaN
@@ -231,18 +223,14 @@ int rqb200_sid_trie_beam_select(const int64_t* samples, const float* samp_log_p,
  *                    rows whose probabilities are all zero -- the rows torch.multinomial would reject with "probability
  *                    tensor contains either `inf`, `nan` or element < 0" / "invalid multinomial distribution (sum of
  *                    probabilities <= 0)".  Such rows still complete, with unspecified samples in [0, K).
- *   limits           1 <= nc <= K <= 2048, kp * nc <= 1024, k <= 32, h < C <= 8, and for the bitmap K^C within its limit;
- *                    RQB_ERR_UNSUPPORTED otherwise.  Deterministic: no result depends on the order of atomics. */
-int rqb200_sid_sample_select(const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride,
-                             const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k, int C, int K,
-                             const void* prefix_workspace, int64_t* out_generated, float* out_log_probas, int64_t* out_parent,
-                             int64_t* samples, float* samp_log_p, int* reject, void* stream);
+ *   limits           1 <= nc <= K <= 2048, kp * nc <= 1024, k <= 32, h < C <= 8; RQB_ERR_UNSUPPORTED otherwise.
+ *                    Deterministic: no result depends on the order of atomics. */
 int rqb200_sid_trie_sample_select(const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride,
                                   const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k, int C,
                                   int K, const void* prefix_workspace, int64_t* out_generated, float* out_log_probas,
                                   int64_t* out_parent, int64_t* samples, float* samp_log_p, int* reject, void* stream);
 
-/* sid_beam_topk     : one level h of the exhaustive (deterministic) constrained beam search, from the head's logits, one launch:
+/* sid_trie_beam_topk : one level h of the exhaustive (deterministic) constrained beam search, from the head's logits, one launch:
  *   logits           [B*kp, K] fp32, row stride in elements (kp = 1 at h = 0, where generated and log_probas may be null)
  *   generated        [B, kp, h] int64, log_probas [B, kp] fp32: the beams entering the level
  *   per row          lse = m + logf(sum expf(x - m)) in fp32 (m the row maximum, fixed reduction order)
@@ -251,11 +239,8 @@ int rqb200_sid_trie_sample_select(const float* probas, int64_t probas_stride, co
  *                    lowest e) -> out_generated [B, k, h + 1], out_log_probas [B, k], out_parent [B*k] = b * kp + beam
  *   bad              optional int[1], ADDED to (never cleared): beam rows holding a NaN or +inf logit, or whose logits are all
  *                    -inf.  Such rows still complete; all their candidates score -inf.
- *   limits           K <= 2048, k <= 32, k <= K, kp <= 32, h < C <= 8, and for the bitmap K^C within its limit;
- *                    RQB_ERR_UNSUPPORTED otherwise.  B = 0 is a no-op.  Deterministic: no result depends on the order of atomics. */
-int rqb200_sid_beam_topk(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas, int B,
-                         int kp, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
-                         float* out_log_probas, int64_t* out_parent, int* bad, void* stream);
+ *   limits           K <= 2048, k <= 32, k <= K, kp <= 32, h < C <= 8; RQB_ERR_UNSUPPORTED otherwise.  B = 0 is a no-op.
+ *                    Deterministic: no result depends on the order of atomics. */
 int rqb200_sid_trie_beam_topk(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas, int B,
                               int kp, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
                               float* out_log_probas, int64_t* out_parent, int* bad, void* stream);

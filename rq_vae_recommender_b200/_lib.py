@@ -64,17 +64,9 @@ _SIGNATURES = {
     "rqb200_sid_dedup_workspace_bytes": (c_size, [c_int, c_int, c_int]),
     "rqb200_sid_dedup_rank": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_size, c_vp]),
     "rqb200_sid_gather": (c_int, [c_vp, c_i64, c_int, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_vp, c_vp, c_vp]),
-    "rqb200_sid_prefix_workspace_bytes": (c_size, [c_int, c_int]),
-    "rqb200_sid_prefix_build": (c_int, [c_vp, c_i64, c_int, c_int, c_vp, c_size, c_vp]),
-    "rqb200_sid_prefix_check": (c_int, [c_vp, c_i64, c_i64, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
-    "rqb200_sid_beam_select": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp,
-                                       c_vp, c_vp, c_vp]),
-    "rqb200_sid_sample_select": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
-                                         c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
-    "rqb200_sid_beam_topk": (c_int, [c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp,
-                                     c_vp, c_vp]),
     "rqb200_sid_trie_workspace_bytes": (c_size, [c_i64, c_int, c_int]),
-    "rqb200_sid_trie_build": (c_int, [c_vp, c_i64, c_int, c_int, c_vp, c_size, c_vp]),
+    "rqb200_sid_trie_scratch_bytes": (c_size, [c_i64, c_int, c_int]),
+    "rqb200_sid_trie_build": (c_int, [c_vp, c_i64, c_int, c_int, c_vp, c_size, c_vp, c_size, c_vp]),
     "rqb200_sid_trie_check": (c_int, [c_vp, c_i64, c_i64, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
     "rqb200_sid_trie_beam_select": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp,
                                             c_vp, c_vp, c_vp]),

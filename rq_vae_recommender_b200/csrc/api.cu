@@ -12,7 +12,7 @@ void rqb_set_error(const char* fmt, ...) {
 }
 
 extern "C" const char* rqb200_last_error(void) { return g_err; }
-extern "C" int rqb200_version(void) { return 100; }
+extern "C" int rqb200_version(void) { return 101; }
 
 // number of SMs / compute capability of the current device (host logic sizes persistent grids with it)
 extern "C" int rqb200_device_info(int* sm_count, int* cc_major, int* cc_minor) {

@@ -155,101 +155,21 @@ extern "C" int rqb200_sid_gather(const int64_t* cached_ids, int64_t n_corpus, in
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Valid-prefix indexes of the corpus id table (SURVEY 8(f)-4: modules/model.py:169-182 `_check_valid_prefix`, called once per
+// Valid-prefix index of the corpus id table (SURVEY 8(f)-4: modules/model.py:169-182 `_check_valid_prefix`, called once per
 // hierarchy level of the constrained beam search, :340-376).  The reference compares every candidate prefix with every corpus
 // row: O(P N l) per call (P = batch x beams x candidates = 163 840 at the shipped evaluation settings, N = corpus size).  Here
-// the corpus is turned ONCE into an index, and the search kernels below are templated on it (SidBitmap, SidTrie):
-//   bitmap  one bitmap per prefix length l (bit key = packed prefix, K^l bits: 32 B, 8 KB, 2 MB, 512 MB for K = 256,
-//           l = 1..4); a check is one bit test.  Only for K^C <= 2^33 bits.
-//   trie    the distinct l-prefixes of the corpus per level in lexicographic order (sid_trie_build below), O(N C) bytes for any
-//           K^C; a check is one binary search among a node's children per level.
-// Both hold exactly the prefixes of the corpus rows up to their first id outside [0, K): a prefix holding such an id is never
-// valid (it can never equal a candidate drawn from K logits).
-//   bitmap workspace layout: for l = 1..C the bitmap of ceil(K^l / 32) words, each region padded to 256 bytes, in this order.
-#define SID_PREFIX_MAX_BITS (1ll << 33)
-
-static int64_t sid_prefix_bits(int l, int K) {
-  int64_t s = 1;
-  for (int i = 0; i < l; ++i) {
-    s *= K;
-    if (s > SID_PREFIX_MAX_BITS) return 0;
-  }
-  return s;
-}
-static size_t sid_prefix_region(int l, int K) {            // bytes of level l's bitmap region (0: too large)
-  const int64_t bits = sid_prefix_bits(l, K);
-  if (bits == 0) return 0;
-  return (size_t)(((bits + 31) / 32 * 4 + 255) / 256 * 256);
-}
-
-extern "C" size_t rqb200_sid_prefix_workspace_bytes(int C, int K) {
-  if (C <= 0 || C > 8 || K <= 0) return 0;
-  size_t tot = 0;
-  for (int l = 1; l <= C; ++l) {
-    const size_t r = sid_prefix_region(l, K);
-    if (r == 0) return 0;                                   // key space too large for bitmaps: the corpus trie serves it
-    tot += r;
-  }
-  return tot;
-}
-
-struct SidPrefixOffsets { unsigned long long off[9]; };     // off[l] = byte offset of level l's bitmap (1-based)
-
-__global__ void sid_prefix_build_kernel(const int64_t* __restrict__ ids, int64_t N, int C, int K, unsigned int* ws, SidPrefixOffsets o) {
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < N; i += (int64_t)gridDim.x * blockDim.x) {
-    unsigned long long key = 0;
-    for (int l = 1; l <= C; ++l) {
-      const int64_t v = ids[i * C + l - 1];
-      if (v < 0 || v >= K) break;                           // an id outside [0, K) can never equal a candidate drawn from K logits
-      key = key * (unsigned long long)K + (unsigned long long)v;
-      atomicOr(ws + o.off[l] / 4 + (key >> 5), 1u << (key & 31));
-    }
-  }
-}
-
-static int sid_prefix_offsets(int C, int K, SidPrefixOffsets& o) {
-  size_t at = 0;
-  for (int l = 1; l <= C; ++l) {
-    const size_t r = sid_prefix_region(l, K);
-    if (r == 0) return 1;
-    o.off[l] = at;
-    at += r;
-  }
-  return 0;
-}
-
-extern "C" int rqb200_sid_prefix_build(const int64_t* cached_ids, int64_t N, int C, int K, void* workspace, size_t ws_bytes, void* stream) {
-  RQB_CHECK_ARG(N >= 0 && C > 0 && C <= 8 && K > 0 && workspace, "sid_prefix_build: bad argument");
-  const size_t need = rqb200_sid_prefix_workspace_bytes(C, K);
-  if (need == 0) {
-    rqb_set_error("sid_prefix_build: key space K^C = %d^%d exceeds the bitmap limit (2^33 bits)", K, C);
-    return RQB_ERR_UNSUPPORTED;
-  }
-  if (ws_bytes < need) {
-    rqb_set_error("sid_prefix_build: workspace too small");
-    return RQB_ERR_WORKSPACE;
-  }
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  RQB_CUDA(cudaMemsetAsync(workspace, 0, need, st));
-  if (N == 0) return RQB_OK;
-  RQB_CHECK_ARG(cached_ids, "sid_prefix_build: null pointer");
-  SidPrefixOffsets o{};
-  sid_prefix_offsets(C, K, o);
-  int grid = (int)((N + 255) / 256);
-  if (grid > 132 * 8) grid = 132 * 8;
-  sid_prefix_build_kernel<<<grid, 256, 0, st>>>(cached_ids, N, C, K, reinterpret_cast<unsigned int*>(workspace), o);
-  RQB_LAUNCH_CHECK();
-  return RQB_OK;
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// Corpus trie.  Level l (1..C) holds the n[l] distinct l-prefixes of the corpus rows in lexicographic order; node i of level l
+// the corpus is turned ONCE into a trie of its distinct prefixes, O(N C) bytes for any K^C, which the search kernels below
+// read.  It holds exactly the prefixes of the corpus rows up to their first id outside [0, K): a prefix holding such an id is
+// never valid (it can never equal a candidate drawn from K logits).
+//
+// Level l (1..C) holds the n[l] distinct l-prefixes of the corpus rows in lexicographic order; node i of level l
 // stores its last code code_l[i] and, for l < C, the range of its children in level l + 1, [child_l[i], child_l[i + 1]) (the
 // root is level 0: child_0 = {0, n[1]}).  Lexicographic order makes the children of a node contiguous and sorted by code, so
 // "node i extended by code c" is a binary search in at most K codes.  The workspace starts with a SidTrieHeader that locates
-// the arrays, so a search call needs no more arguments than with the bitmap.
-//   workspace layout: header | child_0 .. child_{C-1} (int [cap_l + 1]) | code_1 .. code_C (uint16 [N]) | build scratch, every
-//   region 256-byte aligned, cap_0 = 1 and cap_l = N (a level has at most N nodes).
+// the arrays, so a search call needs only the workspace pointer.
+//   workspace layout: header | child_0 .. child_{C-1} (int [cap_l + 1]) | code_1 .. code_C (uint16 [N]), every region
+//   256-byte aligned, cap_0 = 1 and cap_l = N (a level has at most N nodes).  The build's sort scratch (SidSortScratch) is a
+//   separate buffer, needed only while the build runs.
 // Build: rows are sorted lexicographically (stable LSD radix sort over 64-bit keys of as many columns as fit, ids outside
 // [0, K) and every id after them mapped to K so that they sort last), each sorted row flags the levels at which it starts a new
 // node (deeper than its common prefix with the row before, within its valid length), an inclusive scan per level numbers the
@@ -262,19 +182,21 @@ struct SidTrieHeader {
   unsigned long long code[9];                               // byte offset of code_l, l = 1..C
 };
 
-struct SidTrieLayout {
-  SidTrieHeader h;
-  size_t keys[2], perm[2], flag, scan, temp, temp_bytes, total;
-  int width, cols;                                          // bits per packed id, ids per 64-bit sort key
-};
-
 static size_t sid_align256(size_t b) { return (b + 255) / 256 * 256; }
 
-// The row sort shared by the trie and the item table: bits per packed id (K itself, the "no id" mark, fits), ids per 64-bit
-// sort key, and the CUB scratch bytes of a sort or a scan of N entries.  Nonzero when the sort's workspace query fails.
-static int sid_sort_plan(int64_t N, int K, int& width, int& cols, size_t& temp_bytes) {
-  width = 32 - __builtin_clz((unsigned)K);
-  cols = 64 / width;
+// bits per id in the packed sort keys of the trie and the item table (K itself, the "no id" mark, fits); 64 / width ids fit
+// one 64-bit key
+static int sid_id_bits(int K) { return 32 - __builtin_clz((unsigned)K); }
+
+// Scratch of the row sort shared by the trie and the item table, as byte offsets: two buffers of 64-bit sort keys and two of
+// row permutations (N each), `levels` arrays of N ints for the flags and as many for their scans, and CUB's temp storage for a
+// sort or a scan of N entries.
+struct SidSortScratch {
+  size_t keys[2], perm[2], flag, scan, temp, temp_bytes, end;
+};
+
+// Lays the sort scratch of N rows out from byte offset `at`.  Nonzero when the sort's workspace query fails.
+static int sid_sort_scratch(int64_t N, int levels, size_t at, SidSortScratch& s) {
   size_t sort_bytes = 0, scan_bytes = 0;
   const int n = (int)N > 0 ? (int)N : 1;
   if (cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
@@ -283,47 +205,56 @@ static int sid_sort_plan(int64_t N, int K, int& width, int& cols, size_t& temp_b
     cudaGetLastError();
     return 1;
   }
-  temp_bytes = sort_bytes > scan_bytes ? sort_bytes : scan_bytes;
-  return 0;
-}
-
-static int sid_trie_layout(int64_t N, int C, int K, SidTrieLayout& t) {
-  if (N < 0 || N >= 0x7fffffffll || C <= 0 || C > 8 || K <= 0 || K > 65536) return 1;
-  t = SidTrieLayout{};
-  t.h.C = C;
-  t.h.K = K;
-  t.h.N = N;
-  t.h.n[0] = 1;
-  size_t at = sid_align256(sizeof(SidTrieHeader));
-  for (int l = 0; l < C; ++l) {
-    t.h.child[l] = at;
-    at += sid_align256(((l == 0 ? 1 : (size_t)N) + 1) * sizeof(int));
-  }
-  for (int l = 1; l <= C; ++l) {
-    t.h.code[l] = at;
-    at += sid_align256((size_t)N * sizeof(unsigned short));
-  }
+  s.temp_bytes = sort_bytes > scan_bytes ? sort_bytes : scan_bytes;
   for (int i = 0; i < 2; ++i) {
-    t.keys[i] = at;
+    s.keys[i] = at;
     at += sid_align256((size_t)N * sizeof(unsigned long long));
   }
   for (int i = 0; i < 2; ++i) {
-    t.perm[i] = at;
+    s.perm[i] = at;
     at += sid_align256((size_t)N * sizeof(int));
   }
-  t.flag = at;
-  at += sid_align256((size_t)C * N * sizeof(int));
-  t.scan = at;
-  at += sid_align256((size_t)C * N * sizeof(int));
-  if (sid_sort_plan(N, K, t.width, t.cols, t.temp_bytes)) return 2;
-  t.temp = at;
-  t.total = at + sid_align256(t.temp_bytes);
+  s.flag = at;
+  at += sid_align256((size_t)levels * N * sizeof(int));
+  s.scan = at;
+  at += sid_align256((size_t)levels * N * sizeof(int));
+  s.temp = at;
+  s.end = at + sid_align256(s.temp_bytes);
+  return 0;
+}
+
+// The trie's header and workspace bytes: arithmetic only, no device.  Nonzero outside the trie's limits.
+static int sid_trie_layout(int64_t N, int C, int K, SidTrieHeader& h, size_t& bytes) {
+  if (N < 0 || N >= 0x7fffffffll || C <= 0 || C > 8 || K <= 0 || K > 65536) return 1;
+  h = SidTrieHeader{};
+  h.C = C;
+  h.K = K;
+  h.N = N;
+  h.n[0] = 1;
+  size_t at = sid_align256(sizeof(SidTrieHeader));
+  for (int l = 0; l < C; ++l) {
+    h.child[l] = at;
+    at += sid_align256(((l == 0 ? 1 : (size_t)N) + 1) * sizeof(int));
+  }
+  for (int l = 1; l <= C; ++l) {
+    h.code[l] = at;
+    at += sid_align256((size_t)N * sizeof(unsigned short));
+  }
+  bytes = at;
   return 0;
 }
 
 extern "C" size_t rqb200_sid_trie_workspace_bytes(int64_t N, int C, int K) {
-  SidTrieLayout t;
-  return sid_trie_layout(N, C, K, t) ? 0 : t.total;
+  SidTrieHeader h;
+  size_t bytes;
+  return sid_trie_layout(N, C, K, h, bytes) ? 0 : bytes;
+}
+
+extern "C" size_t rqb200_sid_trie_scratch_bytes(int64_t N, int C, int K) {
+  SidTrieHeader h;
+  size_t bytes;
+  SidSortScratch s;
+  return (sid_trie_layout(N, C, K, h, bytes) || sid_sort_scratch(N, C, 0, s)) ? 0 : s.end;
 }
 
 // number of leading ids of a row inside [0, K)
@@ -369,10 +300,15 @@ __global__ void sid_items_key_kernel(const int64_t* __restrict__ ids, int N, int
   }
 }
 
-// Stable LSD radix sort of the N rows on their packed tuple, least significant column group first (CUB, on the stream).
-// perm[0] ends holding the sorted row ids; with `whole` rows that hold an id outside [0, K) sort last, else the trie's order.
-static int sid_sort_rows(const int64_t* ids, int n, int C, int K, int width, int cols, bool whole, unsigned long long* keys[2],
-                         int* perm[2], void* temp, size_t temp_bytes, int grid, cudaStream_t st) {
+// Stable LSD radix sort of the N rows on their packed tuple, least significant column group first (CUB, on the stream), in the
+// sort scratch s at `scratch`.  `sorted` ends pointing at the sorted row ids; with `whole` rows that hold an id outside [0, K)
+// sort last, else the trie's order.
+static int sid_sort_rows(const int64_t* ids, int n, int C, int K, bool whole, unsigned char* scratch, const SidSortScratch& s,
+                         int grid, cudaStream_t st, int*& sorted) {
+  unsigned long long* keys[2] = {reinterpret_cast<unsigned long long*>(scratch + s.keys[0]),
+                                 reinterpret_cast<unsigned long long*>(scratch + s.keys[1])};
+  int* perm[2] = {reinterpret_cast<int*>(scratch + s.perm[0]), reinterpret_cast<int*>(scratch + s.perm[1])};
+  const int width = sid_id_bits(K), cols = 64 / width;
   sid_trie_iota_kernel<<<grid, 256, 0, st>>>(perm[0], n);
   RQB_LAUNCH_CHECK();
   const int groups = (C + cols - 1) / cols;
@@ -381,10 +317,11 @@ static int sid_sort_rows(const int64_t* ids, int n, int C, int K, int width, int
     if (whole) sid_items_key_kernel<<<grid, 256, 0, st>>>(ids, n, C, K, perm[0], c0, c1, width, keys[0]);
     else sid_trie_key_kernel<<<grid, 256, 0, st>>>(ids, n, C, K, perm[0], c0, c1, width, keys[0]);
     RQB_LAUNCH_CHECK();
-    size_t tb = temp_bytes;
-    RQB_CUDA(cub::DeviceRadixSort::SortPairs(temp, tb, keys[0], keys[1], perm[0], perm[1], n, 0, width * (c1 - c0), st));
+    size_t tb = s.temp_bytes;
+    RQB_CUDA(cub::DeviceRadixSort::SortPairs(scratch + s.temp, tb, keys[0], keys[1], perm[0], perm[1], n, 0, width * (c1 - c0), st));
     std::swap(perm[0], perm[1]);
   }
+  sorted = perm[0];
   return RQB_OK;
 }
 
@@ -433,89 +370,65 @@ __global__ void sid_trie_fill_kernel(const int64_t* __restrict__ ids, int N, int
   }
 }
 
-extern "C" int rqb200_sid_trie_build(const int64_t* cached_ids, int64_t N, int C, int K, void* workspace, size_t ws_bytes, void* stream) {
+extern "C" int rqb200_sid_trie_build(const int64_t* cached_ids, int64_t N, int C, int K, void* workspace, size_t ws_bytes,
+                                     void* scratch, size_t scratch_bytes, void* stream) {
   RQB_CHECK_ARG(N >= 0 && C > 0 && C <= 8 && K > 0 && workspace, "sid_trie_build: bad argument");
-  SidTrieLayout t;
-  const int rc = sid_trie_layout(N, C, K, t);
-  if (rc == 1) {
+  SidTrieHeader h;
+  size_t bytes;
+  if (sid_trie_layout(N, C, K, h, bytes)) {
     rqb_set_error("sid_trie_build: need N < 2^31 - 1 and K <= 65536 (N = %lld, K = %d)", (long long)N, K);
     return RQB_ERR_UNSUPPORTED;
   }
-  if (rc == 2) {
+  SidSortScratch s;
+  if (sid_sort_scratch(N, C, 0, s)) {
     rqb_set_error("sid_trie_build: the sort's workspace query failed (no CUDA device?)");
     return RQB_ERR_CUDA;
   }
-  if (ws_bytes < t.total) {
+  if (ws_bytes < bytes) {
     rqb_set_error("sid_trie_build: workspace too small");
+    return RQB_ERR_WORKSPACE;
+  }
+  if (scratch_bytes < s.end) {
+    rqb_set_error("sid_trie_build: scratch too small");
     return RQB_ERR_WORKSPACE;
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
-  sid_trie_header_kernel<<<1, 1, 0, st>>>(t.h, ws);
+  sid_trie_header_kernel<<<1, 1, 0, st>>>(h, ws);
   RQB_LAUNCH_CHECK();
   if (N == 0) return RQB_OK;
-  RQB_CHECK_ARG(cached_ids, "sid_trie_build: null pointer");
+  RQB_CHECK_ARG(cached_ids && scratch, "sid_trie_build: null pointer");
   const int n = (int)N;
   int grid = (n + 255) / 256;
   if (grid > 132 * 8) grid = 132 * 8;
-  unsigned long long* keys[2] = {reinterpret_cast<unsigned long long*>(ws + t.keys[0]),
-                                 reinterpret_cast<unsigned long long*>(ws + t.keys[1])};
-  int* perm[2] = {reinterpret_cast<int*>(ws + t.perm[0]), reinterpret_cast<int*>(ws + t.perm[1])};
-  int* flag = reinterpret_cast<int*>(ws + t.flag);
-  int* scan = reinterpret_cast<int*>(ws + t.scan);
-  const int sorted = sid_sort_rows(cached_ids, n, C, K, t.width, t.cols, false, keys, perm, ws + t.temp, t.temp_bytes, grid, st);
-  if (sorted != RQB_OK) return sorted;
-  sid_trie_flag_kernel<<<grid, 256, 0, st>>>(cached_ids, n, C, K, perm[0], flag);
+  unsigned char* sc = reinterpret_cast<unsigned char*>(scratch);
+  int* flag = reinterpret_cast<int*>(sc + s.flag);
+  int* scan = reinterpret_cast<int*>(sc + s.scan);
+  int* sorted = nullptr;
+  const int rc = sid_sort_rows(cached_ids, n, C, K, false, sc, s, grid, st, sorted);
+  if (rc != RQB_OK) return rc;
+  sid_trie_flag_kernel<<<grid, 256, 0, st>>>(cached_ids, n, C, K, sorted, flag);
   RQB_LAUNCH_CHECK();
   for (int l = 0; l < C; ++l) {
-    size_t temp_bytes = t.temp_bytes;
-    RQB_CUDA(cub::DeviceScan::InclusiveSum(ws + t.temp, temp_bytes, flag + (int64_t)l * n, scan + (int64_t)l * n, n, st));
+    size_t temp_bytes = s.temp_bytes;
+    RQB_CUDA(cub::DeviceScan::InclusiveSum(sc + s.temp, temp_bytes, flag + (int64_t)l * n, scan + (int64_t)l * n, n, st));
   }
-  sid_trie_fill_kernel<<<grid, 256, 0, st>>>(cached_ids, n, C, perm[0], flag, scan, ws);
+  sid_trie_fill_kernel<<<grid, 256, 0, st>>>(cached_ids, n, C, sorted, flag, scan, ws);
   RQB_LAUNCH_CHECK();
   return RQB_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Index policies of the search kernels.  Each kernel tests "the beam's prefix extended by code tok is a corpus prefix" through
-//   Parent              what a kernel keeps per beam, from parent(ids, h, K) (the beam's ids [0, h));
-//   has(parent, tok, K) the test of one extension;
-//   prefix(ids, l, K)   ids[0, l) is a corpus prefix (the check kernel);
-//   kWalk               the index resolves a beam by walking the trie: the kernels do it once per beam and keep the result
-//                       (beam_select in shared memory, beam_topk as a K-bit child mask per beam in shared memory).
-// An index object serves one prefix length: `level` = h + 1 in the search kernels, l in the check kernel.
-struct SidBitmap {                                          // the level's bitmap
-  const unsigned int* bits;
-  static constexpr bool kWalk = false;
-  struct Parent { const int64_t* ids; int h; };
-  __device__ __forceinline__ Parent parent(const int64_t* ids, int h, int) const { return {ids, h}; }
-  __device__ __forceinline__ bool has(const Parent& p, int64_t tok, int K) const {
-    unsigned long long key = 0;
-    bool ok = tok >= 0 && tok < K;
-    for (int j = 0; j < p.h; ++j) {
-      const int64_t v = p.ids[j];
-      ok = ok && v >= 0 && v < K;
-      key = key * (unsigned long long)K + (unsigned long long)(ok ? v : 0);
-    }
-    key = key * (unsigned long long)K + (unsigned long long)(ok ? tok : 0);
-    return ok && ((__ldg(bits + (key >> 5)) >> (key & 31)) & 1u);
-  }
-  __device__ __forceinline__ bool prefix(const int64_t* ids, int l, int K) const {
-    unsigned long long key = 0;
-    bool ok = true;
-    for (int j = 0; j < l; ++j) {
-      const int64_t v = ids[j];
-      ok = ok && v >= 0 && v < K;
-      key = key * (unsigned long long)K + (unsigned long long)(ok ? v : 0);
-    }
-    return ok && ((__ldg(bits + (key >> 5)) >> (key & 31)) & 1u);
-  }
-};
-
+// Lookups in the trie.  A search kernel tests "the beam's prefix extended by code tok is a corpus prefix" through
+//   parent(ids, h, K)    the walk from the root along the beam's ids [0, h): the range of its children at level h + 1;
+//   has(parent, tok, K)  one binary search among those children;
+//   prefix(ids, l, K)    ids[0, l) is a corpus prefix (the check kernel);
+//   sid_child_mask       the children's codes as a K-bit mask in shared memory, so that a candidate's test is one bit test
+//                        (sample_select and beam_topk, which hold one beam per warp at a time or every beam of a row).
+// A SidTrie object serves one prefix length: `level` = h + 1 in the search kernels, l in the check kernel.
 struct SidTrie {                                            // the whole trie workspace
   const unsigned char* ws;
   int level;
-  static constexpr bool kWalk = true;
   struct Parent { int lo, hi; };                            // the beam's children: nodes [lo, hi) of `level` (empty: not a prefix)
   __device__ __forceinline__ const SidTrieHeader* hdr() const { return reinterpret_cast<const SidTrieHeader*>(ws); }
   __device__ __forceinline__ const int* child(int l) const { return reinterpret_cast<const int*>(ws + __ldg(&hdr()->child[l])); }
@@ -551,69 +464,57 @@ struct SidTrie {                                            // the whole trie wo
   __device__ __forceinline__ bool prefix(const int64_t* ids, int l, int K) const { return has(parent(ids, l - 1, K), ids[l - 1], K); }
 };
 
+// One warp: mask[0, ceil(K / 32)) = bit c set for every child code c of the beam ids[0, h) (none when the beam is not a corpus
+// prefix).  The warp is synchronised on return.
+__device__ __forceinline__ void sid_child_mask(const SidTrie& trie, const int64_t* ids, int h, int K, unsigned int* mask, int lane) {
+  const SidTrie::Parent par = trie.parent(ids, h, K);
+  const unsigned short* code = trie.code(h + 1);
+  for (int i = lane; i < (K + 31) >> 5; i += 32) mask[i] = 0;
+  __syncwarp();
+  for (int i = par.lo + lane; i < par.hi; i += 32) {
+    const int c = __ldg(code + i);
+    atomicOr(&mask[c >> 5], 1u << (c & 31));
+  }
+  __syncwarp();
+}
+
+__device__ __forceinline__ bool sid_mask_has(const unsigned int* mask, int c) { return (mask[c >> 5] >> (c & 31)) & 1u; }
+
 // valid[p] = any corpus row whose first l ids equal prefix[p, :l]      (model.py:175-181)
-template <class Index>
-__global__ void sid_prefix_check_kernel(const int64_t* __restrict__ prefix, int64_t stride, int64_t P, int l, int K, Index idx,
+__global__ void sid_prefix_check_kernel(const int64_t* __restrict__ prefix, int64_t stride, int64_t P, int l, int K, SidTrie trie,
                                         unsigned char* __restrict__ valid) {
   for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < P; p += (int64_t)gridDim.x * blockDim.x)
-    valid[p] = idx.prefix(prefix + p * stride, l, K) ? 1 : 0;
-}
-
-static int sid_check_args(const char* fn, const int64_t* prefix, int64_t row_stride, int64_t P, int l, int C, int K,
-                          const void* workspace, unsigned char* valid) {
-  RQB_CHECK_ARG(P >= 0 && l > 0 && l <= C && C <= 8 && K > 0 && row_stride >= l, "%s: bad argument (l=%d C=%d)", fn, l, C);
-  if (P == 0) return RQB_OK;
-  RQB_CHECK_ARG(prefix && workspace && valid, "%s: null pointer", fn);
-  return RQB_OK;
-}
-
-template <class Index>
-static int sid_check_run(const int64_t* prefix, int64_t row_stride, int64_t P, int l, int K, Index idx, unsigned char* valid,
-                         void* stream) {
-  int grid = (int)((P + 255) / 256);
-  if (grid > 132 * 16) grid = 132 * 16;
-  sid_prefix_check_kernel<Index><<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(prefix, row_stride, P, l, K, idx, valid);
-  RQB_LAUNCH_CHECK();
-  return RQB_OK;
-}
-
-extern "C" int rqb200_sid_prefix_check(const int64_t* prefix, int64_t row_stride, int64_t P, int l, int C, int K, const void* workspace,
-                                       unsigned char* valid, void* stream) {
-  const int rc = sid_check_args("sid_prefix_check", prefix, row_stride, P, l, C, K, workspace, valid);
-  if (rc != RQB_OK || P == 0) return rc;
-  SidPrefixOffsets o{};
-  if (sid_prefix_offsets(C, K, o)) {
-    rqb_set_error("sid_prefix_check: key space too large");
-    return RQB_ERR_UNSUPPORTED;
-  }
-  return sid_check_run(prefix, row_stride, P, l, K,
-                       SidBitmap{reinterpret_cast<const unsigned int*>(reinterpret_cast<const char*>(workspace) + o.off[l])}, valid,
-                       stream);
+    valid[p] = trie.prefix(prefix + p * stride, l, K) ? 1 : 0;
 }
 
 extern "C" int rqb200_sid_trie_check(const int64_t* prefix, int64_t row_stride, int64_t P, int l, int C, int K, const void* workspace,
                                      unsigned char* valid, void* stream) {
-  const int rc = sid_check_args("sid_trie_check", prefix, row_stride, P, l, C, K, workspace, valid);
-  if (rc != RQB_OK || P == 0) return rc;
-  return sid_check_run(prefix, row_stride, P, l, K, SidTrie{reinterpret_cast<const unsigned char*>(workspace), l}, valid, stream);
+  RQB_CHECK_ARG(P >= 0 && l > 0 && l <= C && C <= 8 && K > 0 && row_stride >= l, "sid_trie_check: bad argument (l=%d C=%d)", l, C);
+  if (P == 0) return RQB_OK;
+  RQB_CHECK_ARG(prefix && workspace && valid, "sid_trie_check: null pointer");
+  int grid = (int)((P + 255) / 256);
+  if (grid > 132 * 16) grid = 132 * 16;
+  sid_prefix_check_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      prefix, row_stride, P, l, K, SidTrie{reinterpret_cast<const unsigned char*>(workspace), l}, valid);
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
 // One selection step of the constrained beam search (modules/model.py:340-376) in one launch: for every batch row the
 // kp x nc candidate extensions (kp live beams, nc sampled tokens each) are scored  log p(token) + log p(parent beam),  the
-// extensions whose id prefix does not occur in the corpus get -inf (the prefix index above: the reference's repeat_interleave +
-// cat + O(P N) compare + masked_fill), and the k best are taken in descending score order (the reference sorts all kp nc scores
-// and keeps k), with their ids gathered into the new beams and the parent beam's global index returned for the key/value-cache
+// extensions whose id prefix does not occur in the corpus get -inf (the trie above: the reference's repeat_interleave + cat +
+// O(P N) compare + masked_fill), and the k best are taken in descending score order (the reference sorts all kp nc scores and
+// keeps k), with their ids gathered into the new beams and the parent beam's global index returned for the key/value-cache
 // reorder.  Ties: lowest flat candidate index first (torch.sort is not stable: any order is legal).
-// One warp per batch row; kp * nc <= 1024, k <= 32.  With the trie each warp first resolves its row's kp beams (shared memory).
+// One warp per batch row; kp * nc <= 1024, k <= 32.  Each warp first resolves its row's kp beams in the trie (shared memory),
+// then tests each candidate with one binary search among its beam's children: a K-bit mask per beam would not fit for
+// 1024 beams.
 #define SID_BEAM_MAX_E 1024
 
 // Score of one candidate extension: lp (token log-probability + parent beam log-probability), or -inf when the prefix
-// parent ids + tok is not in the corpus (model.py:356,366) or lp is NaN (NaN ranks last here).
-template <class Index>
-__device__ __forceinline__ float sid_extension_score(const Index& idx, const typename Index::Parent& par, int64_t tok, int K, float lp) {
-  return (!idx.has(par, tok, K) || lp != lp) ? -INFINITY : lp;
-}
+// parent ids + tok is not in the corpus (!valid, model.py:356,366) or lp is NaN (NaN ranks last here).
+__device__ __forceinline__ float sid_extension_score(bool valid, float lp) { return (!valid || lp != lp) ? -INFINITY : lp; }
 
 // One warp keeps the k best of batch row b's E = kp * nc candidate scores sc[] in descending order: k rounds of a warp
 // arg-max over the candidates not yet taken (tk[], cleared by the caller).  tok[e] is candidate e's token (e = beam * nc + j).
@@ -649,11 +550,11 @@ __device__ __forceinline__ void sid_keep_best(const float* sc, unsigned char* tk
   }
 }
 
-template <class Index>
 __global__ void __launch_bounds__(128) sid_beam_select_kernel(
     const int64_t* __restrict__ samples, const float* __restrict__ samp_log_p, const int64_t* __restrict__ generated,
-    const float* __restrict__ log_probas, int B, int kp, int nc, int h, int k, int K, Index idx,
+    const float* __restrict__ log_probas, int B, int kp, int nc, int h, int k, int K, SidTrie trie,
     int64_t* __restrict__ out_generated, float* __restrict__ out_log_probas, int64_t* __restrict__ out_parent) {
+  extern __shared__ __align__(16) unsigned char sid_smem[];
   __shared__ float s_score[4][SID_BEAM_MAX_E];
   __shared__ unsigned char s_taken[4][SID_BEAM_MAX_E];
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -662,79 +563,39 @@ __global__ void __launch_bounds__(128) sid_beam_select_kernel(
   const int E = kp * nc;
   float* sc = s_score[w];
   unsigned char* tk = s_taken[w];
-  typename Index::Parent* s_par = nullptr;                  // [4][kp] with kWalk: the row's beams, resolved once
-  if constexpr (Index::kWalk) {
-    extern __shared__ __align__(16) unsigned char sid_smem[];
-    s_par = reinterpret_cast<typename Index::Parent*>(sid_smem) + w * kp;
-    for (int beam = lane; beam < kp; beam += 32) s_par[beam] = idx.parent(generated + ((int64_t)b * kp + beam) * h, h, K);
-    __syncwarp();
-  }
+  SidTrie::Parent* s_par = reinterpret_cast<SidTrie::Parent*>(sid_smem) + w * kp;   // [4][kp]: the row's beams, resolved once
+  for (int beam = lane; beam < kp; beam += 32) s_par[beam] = trie.parent(generated + ((int64_t)b * kp + beam) * h, h, K);
+  __syncwarp();
   for (int e = lane; e < E; e += 32) {
     const int beam = e / nc;
     const int64_t row = (int64_t)b * kp + beam;
     const float s = samp_log_p[row * nc + (e - beam * nc)] + (log_probas ? log_probas[row] : 0.f);
-    const typename Index::Parent par = Index::kWalk ? s_par[beam] : idx.parent(generated + row * h, h, K);
-    sc[e] = sid_extension_score(idx, par, samples[row * nc + (e - beam * nc)], K, s);
+    sc[e] = sid_extension_score(trie.has(s_par[beam], samples[row * nc + (e - beam * nc)], K), s);
     tk[e] = 0;
   }
   __syncwarp();
   sid_keep_best(sc, tk, samples + (int64_t)b * kp * nc, E, nc, b, kp, h, k, generated, out_generated, out_log_probas, out_parent, lane);
 }
 
-static int sid_beam_select_args(const char* fn, const int64_t* samples, const float* samp_log_p, const int64_t* generated, int B,
-                                int kp, int nc, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
-                                float* out_log_probas, int64_t* out_parent) {
-  RQB_CHECK_ARG(B >= 0 && kp > 0 && nc > 0 && h >= 0 && h < C && C <= 8 && k > 0 && K > 0, "%s: bad argument", fn);
-  if (kp * nc > SID_BEAM_MAX_E || k > 32) {
-    rqb_set_error("%s: kp * nc = %d (max %d), k = %d (max 32)", fn, kp * nc, SID_BEAM_MAX_E, k);
-    return RQB_ERR_UNSUPPORTED;
-  }
-  if (B == 0) return RQB_OK;
-  RQB_CHECK_ARG(samples && samp_log_p && prefix_workspace && out_generated && out_log_probas && out_parent && (h == 0 || generated),
-                "%s: null pointer", fn);
-  return RQB_OK;
-}
-
-template <class Index>
-static int sid_beam_select_run(const int64_t* samples, const float* samp_log_p, const int64_t* generated, const float* log_probas,
-                               int B, int kp, int nc, int h, int k, int K, Index idx, int64_t* out_generated,
-                               float* out_log_probas, int64_t* out_parent, void* stream) {
-  const size_t smem = Index::kWalk ? 4 * (size_t)kp * sizeof(typename Index::Parent) : 0;
-  if (Index::kWalk) RQB_CUDA(cudaFuncSetAttribute(sid_beam_select_kernel<Index>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  sid_beam_select_kernel<Index><<<(B + 3) / 4, 128, smem, reinterpret_cast<cudaStream_t>(stream)>>>(
-      samples, samp_log_p, generated, log_probas, B, kp, nc, h, k, K, idx, out_generated, out_log_probas, out_parent);
-  RQB_LAUNCH_CHECK();
-  return RQB_OK;
-}
-
-extern "C" int rqb200_sid_beam_select(const int64_t* samples, const float* samp_log_p, const int64_t* generated,
-                                      const float* log_probas, int B, int kp, int nc, int h, int k, int C, int K,
-                                      const void* prefix_workspace, int64_t* out_generated, float* out_log_probas,
-                                      int64_t* out_parent, void* stream) {
-  const int rc = sid_beam_select_args("sid_beam_select", samples, samp_log_p, generated, B, kp, nc, h, k, C, K, prefix_workspace,
-                                      out_generated, out_log_probas, out_parent);
-  if (rc != RQB_OK || B == 0) return rc;
-  SidPrefixOffsets o{};
-  if (sid_prefix_offsets(C, K, o)) {
-    rqb_set_error("sid_beam_select: key space too large");
-    return RQB_ERR_UNSUPPORTED;
-  }
-  return sid_beam_select_run(
-      samples, samp_log_p, generated, log_probas, B, kp, nc, h, k, K,
-      SidBitmap{reinterpret_cast<const unsigned int*>(reinterpret_cast<const char*>(prefix_workspace) + o.off[h + 1])}, out_generated,
-      out_log_probas, out_parent, stream);
-}
-
 extern "C" int rqb200_sid_trie_beam_select(const int64_t* samples, const float* samp_log_p, const int64_t* generated,
                                            const float* log_probas, int B, int kp, int nc, int h, int k, int C, int K,
                                            const void* prefix_workspace, int64_t* out_generated, float* out_log_probas,
                                            int64_t* out_parent, void* stream) {
-  const int rc = sid_beam_select_args("sid_trie_beam_select", samples, samp_log_p, generated, B, kp, nc, h, k, C, K,
-                                      prefix_workspace, out_generated, out_log_probas, out_parent);
-  if (rc != RQB_OK || B == 0) return rc;
-  return sid_beam_select_run(samples, samp_log_p, generated, log_probas, B, kp, nc, h, k, K,
-                             SidTrie{reinterpret_cast<const unsigned char*>(prefix_workspace), h + 1}, out_generated, out_log_probas,
-                             out_parent, stream);
+  RQB_CHECK_ARG(B >= 0 && kp > 0 && nc > 0 && h >= 0 && h < C && C <= 8 && k > 0 && K > 0, "sid_trie_beam_select: bad argument");
+  if (kp * nc > SID_BEAM_MAX_E || k > 32) {
+    rqb_set_error("sid_trie_beam_select: kp * nc = %d (max %d), k = %d (max 32)", kp * nc, SID_BEAM_MAX_E, k);
+    return RQB_ERR_UNSUPPORTED;
+  }
+  if (B == 0) return RQB_OK;
+  RQB_CHECK_ARG(samples && samp_log_p && prefix_workspace && out_generated && out_log_probas && out_parent && (h == 0 || generated),
+                "sid_trie_beam_select: null pointer");
+  const size_t smem = 4 * (size_t)kp * sizeof(SidTrie::Parent);
+  RQB_CUDA(cudaFuncSetAttribute(sid_beam_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  sid_beam_select_kernel<<<(B + 3) / 4, 128, smem, reinterpret_cast<cudaStream_t>(stream)>>>(
+      samples, samp_log_p, generated, log_probas, B, kp, nc, h, k, K,
+      SidTrie{reinterpret_cast<const unsigned char*>(prefix_workspace), h + 1}, out_generated, out_log_probas, out_parent);
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -743,10 +604,10 @@ extern "C" int rqb200_sid_trie_beam_select(const int64_t* samples, const float* 
 // generator; given that q, this kernel reproduces its samples bit for bit: ratio = p / q as an IEEE fp32 division (at::div),
 // the n largest ratios in torch.topk's order (descending; NaN above +inf and -0 below +0, as its radix selection ranks them;
 // equal ratios by ascending index, as its gather and stable sort leave them), samp_log_p = logf(p[sample]).  The candidates
-// then go through sid_extension_score / sid_keep_best exactly as in rqb200_sid_beam_select.
+// then go through sid_extension_score / sid_keep_best exactly as in rqb200_sid_trie_beam_select.
 // One CTA per batch row; warp w samples beams w, w + W, ... (W = min(kp, 16)) from its own shared-memory copy of the row's
-// ratio keys, resolving each beam in the index once; warp 0 then selects from the kp * nc candidates.  Nothing is ordered by
-// atomics: the results are deterministic.
+// ratio keys, expands each beam's children into its own K-bit mask (sid_child_mask) and tests its candidates against it; warp 0
+// then selects from the kp * nc candidates.  Nothing is ordered by atomics: the results are deterministic.
 #define SID_SAMPLE_MAX_WARPS 16
 #define SID_SAMPLE_MAX_K 2048
 
@@ -831,25 +692,25 @@ __device__ void sid_warp_top_n(const unsigned int* key, int K, int n, int* hist,
 static size_t sid_sample_smem(int kp, int nc, int K) {
   const int W = kp < SID_SAMPLE_MAX_WARPS ? kp : SID_SAMPLE_MAX_WARPS;
   const size_t E = (size_t)kp * nc;
-  return E * (sizeof(int64_t) + sizeof(float) + 1) + (size_t)W * (K + 256 + 2 * nc) * 4;
+  return E * (sizeof(int64_t) + sizeof(float) + 1) + (size_t)W * (K + 256 + 2 * nc + (K + 31) / 32) * 4;
 }
 
-template <class Index>
 __global__ void __launch_bounds__(SID_SAMPLE_MAX_WARPS * 32) sid_sample_select_kernel(
     const float* __restrict__ probas, int64_t p_stride, const float* __restrict__ noise, int64_t n_stride,
-    const int64_t* __restrict__ generated, const float* __restrict__ log_probas, int kp, int nc, int h, int k, int K, Index idx,
+    const int64_t* __restrict__ generated, const float* __restrict__ log_probas, int kp, int nc, int h, int k, int K, SidTrie trie,
     int64_t* __restrict__ out_generated, float* __restrict__ out_log_probas, int64_t* __restrict__ out_parent,
     int64_t* __restrict__ samples, float* __restrict__ samp_log_p, int* __restrict__ reject) {
   extern __shared__ __align__(16) unsigned char sid_smem[];
   const int W = blockDim.x >> 5, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int b = blockIdx.x, E = kp * nc;
+  const int b = blockIdx.x, E = kp * nc, KW = (K + 31) >> 5;
   int64_t* s_tok = reinterpret_cast<int64_t*>(sid_smem);                          // [E] candidate tokens
   float* s_score = reinterpret_cast<float*>(s_tok + E);                          // [E] candidate scores
   unsigned int* s_key = reinterpret_cast<unsigned int*>(s_score + E) + (size_t)w * K;                      // [W][K]
   int* s_hist = reinterpret_cast<int*>(reinterpret_cast<unsigned int*>(s_score + E) + (size_t)W * K) + w * 256;   // [W][256]
   unsigned int* s_sk = reinterpret_cast<unsigned int*>(s_hist - w * 256 + W * 256) + w * nc;               // [W][nc]
   int* s_si = reinterpret_cast<int*>(s_sk - w * nc + W * nc) + w * nc;                                     // [W][nc]
-  unsigned char* s_taken = reinterpret_cast<unsigned char*>(s_si - w * nc + W * nc);                      // [E]
+  unsigned int* s_mask = reinterpret_cast<unsigned int*>(s_si - w * nc + W * nc) + w * KW;                 // [W][KW]
+  unsigned char* s_taken = reinterpret_cast<unsigned char*>(s_mask - w * KW + W * KW);                    // [E]
   for (int beam = w; beam < kp; beam += W) {
     const int64_t row = (int64_t)b * kp + beam;
     const float* p = probas + row * p_stride;
@@ -866,14 +727,14 @@ __global__ void __launch_bounds__(SID_SAMPLE_MAX_WARPS * 32) sid_sample_select_k
     if (reject && lane == 0 && (bad || !nonzero)) atomicAdd(&reject[bad ? 0 : 1], 1);
     __syncwarp();
     sid_warp_top_n(s_key, K, nc, s_hist, s_sk, s_si, s_tok + beam * nc, lane);
+    sid_child_mask(trie, generated + row * h, h, K, s_mask, lane);
     const float plp = log_probas ? log_probas[row] : 0.f;
-    const typename Index::Parent par = idx.parent(generated + row * h, h, K);
     for (int r = lane; r < nc; r += 32) {
       const int64_t tok = s_tok[beam * nc + r];
       const float lp = logf(p[tok]);
       if (samples) samples[row * nc + r] = tok;
       if (samp_log_p) samp_log_p[row * nc + r] = lp;
-      s_score[beam * nc + r] = sid_extension_score(idx, par, tok, K, lp + plp);
+      s_score[beam * nc + r] = sid_extension_score(sid_mask_has(s_mask, (int)tok), lp + plp);
       s_taken[beam * nc + r] = 0;
     }
   }
@@ -882,67 +743,31 @@ __global__ void __launch_bounds__(SID_SAMPLE_MAX_WARPS * 32) sid_sample_select_k
     sid_keep_best(s_score, s_taken, s_tok, E, nc, b, kp, h, k, generated, out_generated, out_log_probas, out_parent, lane);
 }
 
-static int sid_sample_select_args(const char* fn, const float* probas, int64_t probas_stride, const float* noise,
-                                  int64_t noise_stride, const int64_t* generated, const float* log_probas, int B, int kp, int nc,
-                                  int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
-                                  float* out_log_probas, int64_t* out_parent) {
-  RQB_CHECK_ARG(B >= 0 && kp > 0 && nc > 0 && h >= 0 && h < C && C <= 8 && k > 0 && K > 0 && probas_stride >= K &&
-                    noise_stride >= K, "%s: bad argument (B=%d kp=%d nc=%d h=%d k=%d C=%d K=%d)", fn, B, kp, nc, h, k, C, K);
-  if (nc > K || K > SID_SAMPLE_MAX_K || kp * nc > SID_BEAM_MAX_E || k > 32) {
-    rqb_set_error("%s: need nc <= K <= %d, kp * nc <= %d, k <= 32 (nc = %d, K = %d, kp * nc = %d, k = %d)", fn,
-                  SID_SAMPLE_MAX_K, SID_BEAM_MAX_E, nc, K, kp * nc, k);
-    return RQB_ERR_UNSUPPORTED;
-  }
-  if (B == 0) return RQB_OK;
-  RQB_CHECK_ARG(probas && noise && prefix_workspace && out_generated && out_log_probas && out_parent && (h == 0 || generated) &&
-                    (h == 0 || log_probas), "%s: null pointer", fn);
-  return RQB_OK;
-}
-
-template <class Index>
-static int sid_sample_select_run(const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride,
-                                 const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k, int K,
-                                 Index idx, int64_t* out_generated, float* out_log_probas, int64_t* out_parent, int64_t* samples,
-                                 float* samp_log_p, int* reject, void* stream) {
-  const int W = kp < SID_SAMPLE_MAX_WARPS ? kp : SID_SAMPLE_MAX_WARPS;
-  const size_t smem = sid_sample_smem(kp, nc, K);
-  RQB_CUDA(cudaFuncSetAttribute(sid_sample_select_kernel<Index>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  sid_sample_select_kernel<Index><<<B, W * 32, smem, reinterpret_cast<cudaStream_t>(stream)>>>(
-      probas, probas_stride, noise, noise_stride, generated, log_probas, kp, nc, h, k, K, idx, out_generated, out_log_probas,
-      out_parent, samples, samp_log_p, reject);
-  RQB_LAUNCH_CHECK();
-  return RQB_OK;
-}
-
-extern "C" int rqb200_sid_sample_select(const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride,
-                                        const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k,
-                                        int C, int K, const void* prefix_workspace, int64_t* out_generated, float* out_log_probas,
-                                        int64_t* out_parent, int64_t* samples, float* samp_log_p, int* reject, void* stream) {
-  const int rc = sid_sample_select_args("sid_sample_select", probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp,
-                                        nc, h, k, C, K, prefix_workspace, out_generated, out_log_probas, out_parent);
-  if (rc != RQB_OK || B == 0) return rc;
-  SidPrefixOffsets o{};
-  if (sid_prefix_offsets(C, K, o)) {
-    rqb_set_error("sid_sample_select: key space %d^%d exceeds the bitmap limit (2^33 bits)", K, C);
-    return RQB_ERR_UNSUPPORTED;
-  }
-  return sid_sample_select_run(
-      probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, K,
-      SidBitmap{reinterpret_cast<const unsigned int*>(reinterpret_cast<const char*>(prefix_workspace) + o.off[h + 1])}, out_generated,
-      out_log_probas, out_parent, samples, samp_log_p, reject, stream);
-}
-
 extern "C" int rqb200_sid_trie_sample_select(const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride,
                                              const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k,
                                              int C, int K, const void* prefix_workspace, int64_t* out_generated,
                                              float* out_log_probas, int64_t* out_parent, int64_t* samples, float* samp_log_p,
                                              int* reject, void* stream) {
-  const int rc = sid_sample_select_args("sid_trie_sample_select", probas, probas_stride, noise, noise_stride, generated, log_probas,
-                                        B, kp, nc, h, k, C, K, prefix_workspace, out_generated, out_log_probas, out_parent);
-  if (rc != RQB_OK || B == 0) return rc;
-  return sid_sample_select_run(probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, K,
-                               SidTrie{reinterpret_cast<const unsigned char*>(prefix_workspace), h + 1}, out_generated,
-                               out_log_probas, out_parent, samples, samp_log_p, reject, stream);
+  RQB_CHECK_ARG(B >= 0 && kp > 0 && nc > 0 && h >= 0 && h < C && C <= 8 && k > 0 && K > 0 && probas_stride >= K &&
+                    noise_stride >= K, "sid_trie_sample_select: bad argument (B=%d kp=%d nc=%d h=%d k=%d C=%d K=%d)", B, kp, nc, h,
+                k, C, K);
+  if (nc > K || K > SID_SAMPLE_MAX_K || kp * nc > SID_BEAM_MAX_E || k > 32) {
+    rqb_set_error("sid_trie_sample_select: need nc <= K <= %d, kp * nc <= %d, k <= 32 (nc = %d, K = %d, kp * nc = %d, k = %d)",
+                  SID_SAMPLE_MAX_K, SID_BEAM_MAX_E, nc, K, kp * nc, k);
+    return RQB_ERR_UNSUPPORTED;
+  }
+  if (B == 0) return RQB_OK;
+  RQB_CHECK_ARG(probas && noise && prefix_workspace && out_generated && out_log_probas && out_parent && (h == 0 || generated) &&
+                    (h == 0 || log_probas), "sid_trie_sample_select: null pointer");
+  const int W = kp < SID_SAMPLE_MAX_WARPS ? kp : SID_SAMPLE_MAX_WARPS;
+  const size_t smem = sid_sample_smem(kp, nc, K);
+  RQB_CUDA(cudaFuncSetAttribute(sid_sample_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  sid_sample_select_kernel<<<B, W * 32, smem, reinterpret_cast<cudaStream_t>(stream)>>>(
+      probas, probas_stride, noise, noise_stride, generated, log_probas, kp, nc, h, k, K,
+      SidTrie{reinterpret_cast<const unsigned char*>(prefix_workspace), h + 1}, out_generated, out_log_probas, out_parent, samples,
+      samp_log_p, reject);
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -956,8 +781,8 @@ extern "C" int rqb200_sid_trie_sample_select(const float* probas, int64_t probas
 // finds the smallest kept key, the k keys at or above it are collected and each is ranked among them.  The histograms are
 // integer counts and the ranks compare distinct keys: no result depends on the order of atomics.  The 32-bit score keys stay
 // in shared memory when E <= SID_TOPK_SMEM_KEYS; above that every pass recomputes them from the logits.  The score is written
-// with explicit roundings (no contraction), so a recomputed key has the same bits as the first.  With the trie every beam's
-// children are first expanded into a K-bit mask in shared memory (after the keys), and a candidate's test is one bit test.
+// with explicit roundings (no contraction), so a recomputed key has the same bits as the first.  Every beam's children are
+// first expanded into a K-bit mask in shared memory (sid_child_mask, after the keys), and a candidate's test is one bit test.
 #define SID_TOPK_MAX_K 2048
 #define SID_TOPK_MAX_BEAMS 32
 #define SID_TOPK_MAX_THREADS 512
@@ -973,26 +798,19 @@ struct SidTopkShared {
   unsigned long long sel[32];
 };
 
-// candidate e's 32-bit score key; mask: the beams' child masks [kp][ceil(K / 32)] with kWalk
-template <class Index>
-__device__ __forceinline__ unsigned int sid_topk_candidate(const float* __restrict__ logits, int64_t ld, int64_t row0, int K, int h,
-                                                           int e, const SidTopkShared& s, const Index& idx, const unsigned int* mask) {
+// candidate e's 32-bit score key; mask: the beams' child masks [kp][ceil(K / 32)]
+__device__ __forceinline__ unsigned int sid_topk_candidate(const float* __restrict__ logits, int64_t ld, int64_t row0, int K, int e,
+                                                           const SidTopkShared& s, const unsigned int* mask) {
   const int beam = e / K, c = e - beam * K;
   const float lp = __fadd_rn(__fsub_rn(logits[(row0 + beam) * ld + c], s.lse[beam]), s.plp[beam]);
-  float sc;
-  if constexpr (Index::kWalk) {
-    const bool ok = (mask[beam * ((K + 31) >> 5) + (c >> 5)] >> (c & 31)) & 1u;
-    sc = (!ok || lp != lp) ? -INFINITY : lp;
-  } else {
-    sc = sid_extension_score(idx, idx.parent(s.gen + beam * h, h, K), c, K, lp);
-  }
+  const float sc = sid_extension_score(sid_mask_has(mask + beam * ((K + 31) >> 5), c), lp);
   return sid_topk_key(sc == 0.f ? 0.f : sc);
 }
 
-template <class Index, bool KEYS_IN_SMEM>
+template <bool KEYS_IN_SMEM>
 __global__ void __launch_bounds__(SID_TOPK_MAX_THREADS) sid_beam_topk_kernel(
     const float* __restrict__ logits, int64_t ld, const int64_t* __restrict__ generated, const float* __restrict__ log_probas,
-    int kp, int h, int k, int K, Index idx, int64_t* __restrict__ out_generated, float* __restrict__ out_log_probas,
+    int kp, int h, int k, int K, SidTrie trie, int64_t* __restrict__ out_generated, float* __restrict__ out_log_probas,
     int64_t* __restrict__ out_parent, int* __restrict__ bad) {
   extern __shared__ __align__(16) unsigned char sid_smem[];
   __shared__ SidTopkShared s;
@@ -1001,7 +819,7 @@ __global__ void __launch_bounds__(SID_TOPK_MAX_THREADS) sid_beam_topk_kernel(
   const unsigned int lt = (1u << lane) - 1u;
   const int b = blockIdx.x, E = kp * K;
   const int64_t row0 = (int64_t)b * kp;
-  unsigned int* s_mask = s_key + (KEYS_IN_SMEM ? E : 0);   // [kp][ceil(K / 32)] with kWalk
+  unsigned int* s_mask = s_key + (KEYS_IN_SMEM ? E : 0);   // [kp][ceil(K / 32)]
   for (int i = threadIdx.x; i < 256; i += nt) s.hist[i] = 0;
   for (int i = threadIdx.x; i < kp * h; i += nt) s.gen[i] = generated[row0 * h + i];
   if (threadIdx.x == 0) s.nsel = 0;
@@ -1028,21 +846,8 @@ __global__ void __launch_bounds__(SID_TOPK_MAX_THREADS) sid_beam_topk_kernel(
     }
   }
   __syncthreads();
-  if constexpr (Index::kWalk) {                             // warp per beam: walk the trie, set the bits of the children's codes
-    const int KW = (K + 31) >> 5;
-    const unsigned short* code = idx.code(idx.level);
-    for (int beam = w; beam < kp; beam += W) {
-      const typename Index::Parent par = idx.parent(s.gen + beam * h, h, K);
-      unsigned int* m = s_mask + beam * KW;
-      for (int i = lane; i < KW; i += 32) m[i] = 0;
-      __syncwarp();
-      for (int i = par.lo + lane; i < par.hi; i += 32) {
-        const int c = __ldg(code + i);
-        atomicOr(&m[c >> 5], 1u << (c & 31));
-      }
-    }
-    __syncthreads();
-  }
+  for (int beam = w; beam < kp; beam += W) sid_child_mask(trie, s.gen + beam * h, h, K, s_mask + beam * ((K + 31) >> 5), lane);
+  __syncthreads();
   unsigned long long prefix = 0, pmask = 0;
   int want = k;                                             // entries still needed among those matching the decided digits
   for (int shift = 40; shift >= 0; shift -= 8) {
@@ -1052,10 +857,10 @@ __global__ void __launch_bounds__(SID_TOPK_MAX_THREADS) sid_beam_topk_kernel(
       if (e < E) {
         unsigned int key;
         if (KEYS_IN_SMEM) {
-          if (shift == 40) s_key[e] = key = sid_topk_candidate(logits, ld, row0, K, h, e, s, idx, s_mask);
+          if (shift == 40) s_key[e] = key = sid_topk_candidate(logits, ld, row0, K, e, s, s_mask);
           else key = s_key[e];
         } else {
-          key = sid_topk_candidate(logits, ld, row0, K, h, e, s, idx, s_mask);
+          key = sid_topk_candidate(logits, ld, row0, K, e, s, s_mask);
         }
         const unsigned long long v = ((unsigned long long)key << 16) | (unsigned int)(0xffff - e);
         if ((v & pmask) == prefix) d = (int)((v >> shift) & 255u);
@@ -1100,7 +905,7 @@ __global__ void __launch_bounds__(SID_TOPK_MAX_THREADS) sid_beam_topk_kernel(
   }
   // the kept set: keys whose decided digits are above the prefix (k - want of them) or equal to it (want of them)
   for (int e = threadIdx.x; e < E; e += nt) {
-    const unsigned int key = KEYS_IN_SMEM ? s_key[e] : sid_topk_candidate(logits, ld, row0, K, h, e, s, idx, s_mask);
+    const unsigned int key = KEYS_IN_SMEM ? s_key[e] : sid_topk_candidate(logits, ld, row0, K, e, s, s_mask);
     const unsigned long long v = ((unsigned long long)key << 16) | (unsigned int)(0xffff - e);
     if ((v & pmask) >= prefix) s.sel[atomicAdd(&s.nsel, 1)] = v;
   }
@@ -1121,69 +926,35 @@ __global__ void __launch_bounds__(SID_TOPK_MAX_THREADS) sid_beam_topk_kernel(
   }
 }
 
-static int sid_beam_topk_args(const char* fn, const float* logits, int64_t logits_stride, const int64_t* generated,
-                              const float* log_probas, int B, int kp, int h, int k, int C, int K, const void* prefix_workspace,
-                              int64_t* out_generated, float* out_log_probas, int64_t* out_parent) {
+extern "C" int rqb200_sid_trie_beam_topk(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas,
+                                         int B, int kp, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
+                                         float* out_log_probas, int64_t* out_parent, int* bad, void* stream) {
   RQB_CHECK_ARG(B >= 0 && kp > 0 && h >= 0 && h < C && C <= 8 && k > 0 && K > 0 && logits_stride >= K,
-                "%s: bad argument (B=%d kp=%d h=%d k=%d C=%d K=%d)", fn, B, kp, h, k, C, K);
+                "sid_trie_beam_topk: bad argument (B=%d kp=%d h=%d k=%d C=%d K=%d)", B, kp, h, k, C, K);
   if (K > SID_TOPK_MAX_K || k > 32 || k > K || kp > SID_TOPK_MAX_BEAMS) {
-    rqb_set_error("%s: need K <= %d, k <= 32, k <= K, kp <= %d (K = %d, k = %d, kp = %d)", fn, SID_TOPK_MAX_K,
+    rqb_set_error("sid_trie_beam_topk: need K <= %d, k <= 32, k <= K, kp <= %d (K = %d, k = %d, kp = %d)", SID_TOPK_MAX_K,
                   SID_TOPK_MAX_BEAMS, K, k, kp);
     return RQB_ERR_UNSUPPORTED;
   }
   if (B == 0) return RQB_OK;
   RQB_CHECK_ARG(logits && prefix_workspace && out_generated && out_log_probas && out_parent && (h == 0 || generated) &&
-                    (h == 0 || log_probas), "%s: null pointer", fn);
-  return RQB_OK;
-}
-
-template <class Index>
-static int sid_beam_topk_run(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas, int B,
-                             int kp, int h, int k, int K, Index idx, int64_t* out_generated, float* out_log_probas,
-                             int64_t* out_parent, int* bad, void* stream) {
+                    (h == 0 || log_probas), "sid_trie_beam_topk: null pointer");
+  const SidTrie trie{reinterpret_cast<const unsigned char*>(prefix_workspace), h + 1};
   const int E = kp * K;
   const int nt = E >= 4096 ? SID_TOPK_MAX_THREADS : E >= 1024 ? 256 : 128;
-  const size_t mask = Index::kWalk ? (size_t)kp * ((K + 31) / 32) * sizeof(unsigned int) : 0;
+  const size_t mask = (size_t)kp * ((K + 31) / 32) * sizeof(unsigned int);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (E <= SID_TOPK_SMEM_KEYS) {
     const size_t smem = (size_t)E * sizeof(unsigned int) + mask;
-    RQB_CUDA(cudaFuncSetAttribute(sid_beam_topk_kernel<Index, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    sid_beam_topk_kernel<Index, true><<<B, nt, smem, st>>>(logits, logits_stride, generated, log_probas, kp, h, k, K, idx,
-                                                           out_generated, out_log_probas, out_parent, bad);
+    RQB_CUDA(cudaFuncSetAttribute(sid_beam_topk_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    sid_beam_topk_kernel<true><<<B, nt, smem, st>>>(logits, logits_stride, generated, log_probas, kp, h, k, K, trie, out_generated,
+                                                    out_log_probas, out_parent, bad);
   } else {
-    sid_beam_topk_kernel<Index, false><<<B, nt, mask, st>>>(logits, logits_stride, generated, log_probas, kp, h, k, K, idx,
-                                                            out_generated, out_log_probas, out_parent, bad);
+    sid_beam_topk_kernel<false><<<B, nt, mask, st>>>(logits, logits_stride, generated, log_probas, kp, h, k, K, trie, out_generated,
+                                                     out_log_probas, out_parent, bad);
   }
   RQB_LAUNCH_CHECK();
   return RQB_OK;
-}
-
-extern "C" int rqb200_sid_beam_topk(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas,
-                                    int B, int kp, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
-                                    float* out_log_probas, int64_t* out_parent, int* bad, void* stream) {
-  const int rc = sid_beam_topk_args("sid_beam_topk", logits, logits_stride, generated, log_probas, B, kp, h, k, C, K,
-                                    prefix_workspace, out_generated, out_log_probas, out_parent);
-  if (rc != RQB_OK || B == 0) return rc;
-  SidPrefixOffsets o{};
-  if (sid_prefix_offsets(C, K, o)) {
-    rqb_set_error("sid_beam_topk: key space %d^%d exceeds the bitmap limit (2^33 bits)", K, C);
-    return RQB_ERR_UNSUPPORTED;
-  }
-  return sid_beam_topk_run(
-      logits, logits_stride, generated, log_probas, B, kp, h, k, K,
-      SidBitmap{reinterpret_cast<const unsigned int*>(reinterpret_cast<const char*>(prefix_workspace) + o.off[h + 1])}, out_generated,
-      out_log_probas, out_parent, bad, stream);
-}
-
-extern "C" int rqb200_sid_trie_beam_topk(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas,
-                                         int B, int kp, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
-                                         float* out_log_probas, int64_t* out_parent, int* bad, void* stream) {
-  const int rc = sid_beam_topk_args("sid_trie_beam_topk", logits, logits_stride, generated, log_probas, B, kp, h, k, C, K,
-                                    prefix_workspace, out_generated, out_log_probas, out_parent);
-  if (rc != RQB_OK || B == 0) return rc;
-  return sid_beam_topk_run(logits, logits_stride, generated, log_probas, B, kp, h, k, K,
-                           SidTrie{reinterpret_cast<const unsigned char*>(prefix_workspace), h + 1}, out_generated, out_log_probas,
-                           out_parent, bad, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -1196,7 +967,8 @@ extern "C" int rqb200_sid_trie_beam_topk(const float* logits, int64_t logits_str
 //   key[U][G]     the U distinct retrievable tuples, packed as the sort packs them (G 64-bit words of `cols` ids each), ascending;
 //   start[U + 1]  tuple u's rows are row[start[u] .. start[u + 1]).
 // A lookup packs its tuple and binary-searches the keys.  A header at the start of the workspace locates the arrays.
-//   workspace layout: header | row (int [N]) | key (u64 [N * G]) | start (int [N + 1]) | build scratch, 256-byte aligned regions.
+//   workspace layout: header | row (int [N]) | key (u64 [N * G]) | start (int [N + 1]) | the sort's scratch (SidSortScratch),
+//   256-byte aligned regions.
 struct SidItemsHeader {
   int C, K;
   long long N;
@@ -1207,7 +979,7 @@ struct SidItemsHeader {
 
 struct SidItemsLayout {
   SidItemsHeader h;
-  size_t keys[2], perm[2], flag, scan, temp, temp_bytes, total;
+  SidSortScratch sort;                                      // sort.end: the workspace bytes
 };
 
 #define SID_ITEMS_MAX_G 3                                   // C <= 8 ids of at most 17 bits: 3 ids per word
@@ -1217,7 +989,8 @@ struct SidItemsLayout {
 static int sid_items_layout(int64_t N, int C, int K, SidItemsLayout& t) {
   if (N < 0 || N >= 0x7fffffffll || C <= 0 || C > 8 || K <= 0 || K > 65536) return 1;
   t = SidItemsLayout{};
-  if (sid_sort_plan(N, K, t.h.width, t.h.cols, t.temp_bytes)) return 2;
+  t.h.width = sid_id_bits(K);
+  t.h.cols = 64 / t.h.width;
   t.h.C = C;
   t.h.K = K;
   t.h.N = N;
@@ -1229,26 +1002,12 @@ static int sid_items_layout(int64_t N, int C, int K, SidItemsLayout& t) {
   at += sid_align256((size_t)N * t.h.G * sizeof(unsigned long long));
   t.h.start = at;
   at += sid_align256(((size_t)N + 1) * sizeof(int));
-  for (int i = 0; i < 2; ++i) {
-    t.keys[i] = at;
-    at += sid_align256((size_t)N * sizeof(unsigned long long));
-  }
-  for (int i = 0; i < 2; ++i) {
-    t.perm[i] = at;
-    at += sid_align256((size_t)N * sizeof(int));
-  }
-  t.flag = at;
-  at += sid_align256((size_t)N * sizeof(int));
-  t.scan = at;
-  at += sid_align256((size_t)N * sizeof(int));
-  t.temp = at;
-  t.total = at + sid_align256(t.temp_bytes);
-  return 0;
+  return sid_sort_scratch(N, 1, at, t.sort) ? 2 : 0;
 }
 
 extern "C" size_t rqb200_sid_items_workspace_bytes(int64_t N, int C, int K) {
   SidItemsLayout t;
-  return sid_items_layout(N, C, K, t) ? 0 : t.total;
+  return sid_items_layout(N, C, K, t) ? 0 : t.sort.end;
 }
 
 __global__ void sid_items_header_kernel(SidItemsHeader h, unsigned char* ws) {
@@ -1309,7 +1068,7 @@ extern "C" int rqb200_sid_items_build(const int64_t* cached_ids, int64_t N, int 
     rqb_set_error("sid_items_build: the sort's workspace query failed (no CUDA device?)");
     return RQB_ERR_CUDA;
   }
-  if (ws_bytes < t.total) {
+  if (ws_bytes < t.sort.end) {
     rqb_set_error("sid_items_build: workspace too small");
     return RQB_ERR_WORKSPACE;
   }
@@ -1322,18 +1081,16 @@ extern "C" int rqb200_sid_items_build(const int64_t* cached_ids, int64_t N, int 
   const int n = (int)N;
   int grid = (n + 255) / 256;
   if (grid > 132 * 8) grid = 132 * 8;
-  unsigned long long* keys[2] = {reinterpret_cast<unsigned long long*>(ws + t.keys[0]),
-                                 reinterpret_cast<unsigned long long*>(ws + t.keys[1])};
-  int* perm[2] = {reinterpret_cast<int*>(ws + t.perm[0]), reinterpret_cast<int*>(ws + t.perm[1])};
-  int* flag = reinterpret_cast<int*>(ws + t.flag);
-  int* scan = reinterpret_cast<int*>(ws + t.scan);
-  const int sorted = sid_sort_rows(cached_ids, n, C, K, t.h.width, t.h.cols, true, keys, perm, ws + t.temp, t.temp_bytes, grid, st);
-  if (sorted != RQB_OK) return sorted;
-  sid_items_flag_kernel<<<grid, 256, 0, st>>>(cached_ids, n, C, K, perm[0], flag);
+  int* flag = reinterpret_cast<int*>(ws + t.sort.flag);
+  int* scan = reinterpret_cast<int*>(ws + t.sort.scan);
+  int* sorted = nullptr;
+  const int sc = sid_sort_rows(cached_ids, n, C, K, true, ws, t.sort, grid, st, sorted);
+  if (sc != RQB_OK) return sc;
+  sid_items_flag_kernel<<<grid, 256, 0, st>>>(cached_ids, n, C, K, sorted, flag);
   RQB_LAUNCH_CHECK();
-  size_t temp_bytes = t.temp_bytes;
-  RQB_CUDA(cub::DeviceScan::InclusiveSum(ws + t.temp, temp_bytes, flag, scan, n, st));
-  sid_items_fill_kernel<<<grid, 256, 0, st>>>(cached_ids, n, perm[0], flag, scan, ws);
+  size_t temp_bytes = t.sort.temp_bytes;
+  RQB_CUDA(cub::DeviceScan::InclusiveSum(ws + t.sort.temp, temp_bytes, flag, scan, n, st));
+  sid_items_fill_kernel<<<grid, 256, 0, st>>>(cached_ids, n, sorted, flag, scan, ws);
   RQB_LAUNCH_CHECK();
   return RQB_OK;
 }

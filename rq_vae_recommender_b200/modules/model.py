@@ -4,10 +4,9 @@ the semantic-id kernels.
 Same names (``EncoderDecoderRetrievalModel``, ``ModelOutput``, ``GenerationOutput``, ``_strip_dedup_col``), constructor
 signature and ``state_dict`` keys, so decoder checkpoints load with ``strict=True``.  ``forward`` and the encoder / decoder
 passes are plain torch on HF T5, as in the reference.  What differs is the search in ``generate``:
-  * ``_check_valid_prefix`` is a lookup in a prefix index of the corpus id table (``ops.SidPrefixIndex``: a bitmap per prefix
-    length where K^num_hierarchies fits 2^33 bits, a trie of the corpus's prefixes otherwise), instead of a compare of every
-    prefix with every corpus row.  The index is built on first use and rebuilt when the ``codebooks`` buffer is replaced,
-    written to (``load_state_dict``) or moved;
+  * ``_check_valid_prefix`` is a lookup in a prefix index of the corpus id table (``ops.SidPrefixIndex``: a trie of the
+    corpus's prefixes), instead of a compare of every prefix with every corpus row.  The index is built on first use and
+    rebuilt when the ``codebooks`` buffer is replaced, written to (``load_state_dict``) or moved;
   * each hierarchy level runs the head, the softmax, ``draw_exponential`` and ONE kernel (``SidPrefixIndex.sample_select``)
     that samples, checks the prefixes, scores and keeps the k best.  ``torch.multinomial(p, n)`` without replacement is
     ``topk(p / q, n)`` with ``q = draw_exponential(p)`` from the same generator, so under the same seed the samples, beams and

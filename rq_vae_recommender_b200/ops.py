@@ -556,49 +556,29 @@ def sid_dedup_rank(ids: torch.Tensor, K: int):
 
 
 class SidPrefixIndex:
-    """Valid-prefix index of a corpus id table [N, C] (modules/model.py:169-182), built once per corpus: one bitmap per prefix
-    length (``kind == "bitmap"``, rqb200_sid_prefix_build) where K^C fits its 2^33-bit limit, else a trie of the corpus's
-    distinct prefixes (``kind == "trie"``, rqb200_sid_trie_build, O(N C) bytes).  ``check`` is the reference's
-    `_check_valid_prefix`; ``beam_select`` one selection step of its constrained beam search (model.py:340-376).  Every method
-    gives the same results on either index.  ``kind`` forces one (both indexes of one corpus are compared that way)."""
+    """Valid-prefix index of a corpus id table [N, C] (modules/model.py:169-182), built once per corpus: a trie of the corpus's
+    distinct prefixes (rqb200_sid_trie_build, O(N C) bytes for any K^C).  ``check`` is the reference's `_check_valid_prefix`;
+    ``beam_select`` one selection step of its constrained beam search (model.py:340-376)."""
 
-    KINDS = ("bitmap", "trie")
-    _ENTRY = {"bitmap": ("rqb200_sid_prefix_build", "rqb200_sid_prefix_check", "rqb200_sid_beam_select",
-                         "rqb200_sid_sample_select", "rqb200_sid_beam_topk"),
-              "trie": ("rqb200_sid_trie_build", "rqb200_sid_trie_check", "rqb200_sid_trie_beam_select",
-                       "rqb200_sid_trie_sample_select", "rqb200_sid_trie_beam_topk")}
-
-    @staticmethod
-    def kind_for(num_levels: int, codebook_size: int) -> str:
-        """The index a corpus of num_levels ids per row over codebook_size codes gets: the bitmap wherever it fits."""
-        return "bitmap" if _lib.load().rqb200_sid_prefix_workspace_bytes(int(num_levels), int(codebook_size)) else "trie"
-
-    def __init__(self, cached_ids: torch.Tensor, codebook_size: int, kind: Optional[str] = None):
+    def __init__(self, cached_ids: torch.Tensor, codebook_size: int):
         _need_cuda(cached_ids)
         lib = _lib.load()
         ids = cached_ids.to(torch.int64).contiguous()
         self.N, self.C = ids.shape
         self.K = int(codebook_size)
         self.device = ids.device
-        self.kind = self.kind_for(self.C, self.K) if kind is None else kind
-        if self.kind not in self.KINDS:
-            raise ValueError(f"prefix index: kind must be one of {self.KINDS}, got {kind!r}")
-        build, check, beam_select, sample_select, beam_topk = (getattr(lib, n) for n in self._ENTRY[self.kind])
-        self._check, self._beam_select, self._sample_select, self._beam_topk = check, beam_select, sample_select, beam_topk
         with torch.cuda.device(ids.device):
-            if self.kind == "bitmap":
-                nbytes = lib.rqb200_sid_prefix_workspace_bytes(self.C, self.K)
-                if nbytes == 0:
-                    raise _lib.Rqb200Error(f"prefix index: key space {self.K}^{self.C} exceeds the bitmap limit (2^33 bits)")
-            else:
-                nbytes = lib.rqb200_sid_trie_workspace_bytes(self.N, self.C, self.K)
-                if nbytes == 0:
-                    raise _lib.Rqb200Error(f"prefix index: a trie of {self.N} rows of {self.C} ids over {self.K} codes is "
-                                           "outside its limits (N < 2^31 - 1, C <= 8, K <= 65536)")
-            #: device bytes the index holds (the trie's include its build scratch)
+            nbytes = lib.rqb200_sid_trie_workspace_bytes(self.N, self.C, self.K)
+            scratch_bytes = lib.rqb200_sid_trie_scratch_bytes(self.N, self.C, self.K)
+            if nbytes == 0 or scratch_bytes == 0:
+                raise _lib.Rqb200Error(f"prefix index: a trie of {self.N} rows of {self.C} ids over {self.K} codes is outside "
+                                       "its limits (N < 2^31 - 1, C <= 8, K <= 65536)")
+            #: device bytes the index holds (the build's scratch is freed after the build)
             self.nbytes = int(nbytes)
             self.ws = torch.empty(nbytes, dtype=torch.uint8, device=ids.device)
-            _lib.check(build(_p(ids), self.N, self.C, self.K, _p(self.ws), nbytes, _stream()), self._ENTRY[self.kind][0][7:])
+            scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=ids.device)   # the allocator reuses it in stream order
+            _lib.check(lib.rqb200_sid_trie_build(_p(ids), self.N, self.C, self.K, _p(self.ws), nbytes, _p(scratch), scratch_bytes,
+                                                 _stream()), "sid_trie_build")
         _count(1)                                             # one build call (the trie's sort and scans are several kernels)
 
     def check(self, prefix: torch.Tensor) -> torch.Tensor:
@@ -613,8 +593,8 @@ class SidPrefixIndex:
             raise ValueError(f"prefix length {l} exceeds the id tuple length {self.C}")
         valid = torch.empty(P, dtype=torch.bool, device=prefix.device)
         with torch.cuda.device(prefix.device):
-            _lib.check(self._check(_p(prefix), prefix.stride(0), P, l, self.C, self.K, _p(self.ws), _p(valid),
-                                                   _stream()), "sid_prefix_check")
+            _lib.check(_lib.load().rqb200_sid_trie_check(_p(prefix), prefix.stride(0), P, l, self.C, self.K, _p(self.ws), _p(valid),
+                                                         _stream()), "sid_trie_check")
         _count(1)
         return valid
 
@@ -638,16 +618,16 @@ class SidPrefixIndex:
         out_p = torch.empty((B, k), dtype=torch.float32, device=dev)
         out_parent = torch.empty((B * k,), dtype=torch.int64, device=dev)
         with torch.cuda.device(dev):
-            _lib.check(self._beam_select(_p(samples), _p(samp_log_p), _p(generated), _p(log_probas), B, kp, nc, h, k,
-                                                  self.C, self.K, _p(self.ws), _p(out_g), _p(out_p), _p(out_parent), _stream()),
-                       "sid_beam_select")
+            _lib.check(_lib.load().rqb200_sid_trie_beam_select(_p(samples), _p(samp_log_p), _p(generated), _p(log_probas), B, kp,
+                                                               nc, h, k, self.C, self.K, _p(self.ws), _p(out_g), _p(out_p),
+                                                               _p(out_parent), _stream()), "sid_trie_beam_select")
         _count(1)
         return out_g, out_p, out_parent
 
     def sample_select(self, probas: torch.Tensor, noise: torch.Tensor, generated: Optional[torch.Tensor],
                       log_probas: Optional[torch.Tensor], k: int, nc: int, want_samples: bool = False,
                       reject: Optional[torch.Tensor] = None):
-        """The sampling step fused with ``beam_select`` (rqb200_sid_sample_select), one launch.  probas / noise [B * kp, K]
+        """The sampling step fused with ``beam_select`` (rqb200_sid_trie_sample_select), one launch.  probas / noise [B * kp, K]
         (kp = 1 on the first level; noise = the Exp(1) draw torch.multinomial makes, ``torch.empty_like(probas).exponential_(1)``),
         generated [B, kp, h] or None, log_probas [B, kp] or None -> (generated [B, k, h + 1], log_probas [B, k],
         parent_global [B * k]), plus (samples [B * kp, nc], samp_log_p [B * kp, nc]) when ``want_samples``: the samples are
@@ -676,10 +656,10 @@ class SidPrefixIndex:
         samples = torch.empty((B * kp, nc), dtype=torch.int64, device=dev) if want_samples else None
         samp_log_p = torch.empty((B * kp, nc), dtype=torch.float32, device=dev) if want_samples else None
         with torch.cuda.device(dev):
-            _lib.check(self._sample_select(_p(probas), probas.stride(0), _p(noise), noise.stride(0), _p(generated),
-                                                    _p(log_probas), B, kp, nc, h, k, self.C, self.K, _p(self.ws), _p(out_g),
-                                                    _p(out_p), _p(out_parent), _p(samples), _p(samp_log_p), _p(reject),
-                                                    _stream()), "sid_sample_select")
+            _lib.check(_lib.load().rqb200_sid_trie_sample_select(_p(probas), probas.stride(0), _p(noise), noise.stride(0),
+                                                                 _p(generated), _p(log_probas), B, kp, nc, h, k, self.C, self.K,
+                                                                 _p(self.ws), _p(out_g), _p(out_p), _p(out_parent), _p(samples),
+                                                                 _p(samp_log_p), _p(reject), _stream()), "sid_trie_sample_select")
         _count(1)
         if want_samples:
             return out_g, out_p, out_parent, samples, samp_log_p
@@ -687,7 +667,7 @@ class SidPrefixIndex:
 
     def beam_topk(self, logits: torch.Tensor, generated: Optional[torch.Tensor], log_probas: Optional[torch.Tensor], k: int,
                   bad: Optional[torch.Tensor] = None):
-        """One level of the exhaustive constrained beam search from the head's logits (rqb200_sid_beam_topk), one launch.
+        """One level of the exhaustive constrained beam search from the head's logits (rqb200_sid_trie_beam_topk), one launch.
         logits [B * kp, K] (kp = 1 on the first level), generated [B, kp, h] or None, log_probas [B, kp] or None ->
         (generated [B, k, h + 1], log_probas [B, k], parent_global [B * k]): of all kp * K extensions of each history, scored
         log_softmax(logits)[code] + the parent's log-probability (-inf when the extended prefix is not in the corpus), the k
@@ -714,9 +694,9 @@ class SidPrefixIndex:
         out_p = torch.empty((B, k), dtype=torch.float32, device=dev)
         out_parent = torch.empty((B * k,), dtype=torch.int64, device=dev)
         with torch.cuda.device(dev):
-            _lib.check(self._beam_topk(_p(logits), logits.stride(0), _p(generated), _p(log_probas), B, kp, h, k, self.C,
-                                                self.K, _p(self.ws), _p(out_g), _p(out_p), _p(out_parent), _p(bad), _stream()),
-                       "sid_beam_topk")
+            _lib.check(_lib.load().rqb200_sid_trie_beam_topk(_p(logits), logits.stride(0), _p(generated), _p(log_probas), B, kp,
+                                                             h, k, self.C, self.K, _p(self.ws), _p(out_g), _p(out_p),
+                                                             _p(out_parent), _p(bad), _stream()), "sid_trie_beam_topk")
         _count(1)
         return out_g, out_p, out_parent
 

@@ -1,7 +1,7 @@
-"""GPU tests of the corpus trie index (csrc/sid.cu: rqb200_sid_trie_*, ops.SidPrefixIndex(kind="trie")): check against
-oracle.rq_oracle.check_valid_prefix beyond the bitmap limit, bit-identical search results on the two indexes of one corpus,
-the sampled and exhaustive searches against their oracles at K^C above the bitmap limit, and the drop-in model at five
-hierarchy levels.  `pytest -m gpu`."""
+"""GPU tests of the corpus trie index (csrc/sid.cu: rqb200_sid_trie_*, ops.SidPrefixIndex): check against
+oracle.rq_oracle.check_valid_prefix up to K^C = 2^88, the three searches against their oracles and against each other (the
+sampled search's child masks against beam_select's walk), the sampled and exhaustive searches at K^C above 2^33, and the
+drop-in model at five hierarchy levels.  `pytest -m gpu`."""
 import numpy as np
 import pytest
 import torch
@@ -9,7 +9,9 @@ import torch.nn.functional as F
 
 import trie_oracle as T
 from oracle import rq_oracle as O
-from test_gpu_beam_search import assert_matches, oracle_level, torch_level
+import beam_search_oracle as BO
+import sample_oracle as SO
+from test_gpu_beam_search import TOL, assert_matches, oracle_level, torch_level
 from test_gpu_generate import composition, dev, history, level_logits, realistic_corpus, small_model
 from test_trie_oracle import prefixes, random_corpus
 
@@ -17,12 +19,11 @@ pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("K,C", [(16, 8), (256, 5), (512, 4), (2048, 4), (2048, 8)])
-def test_trie_check_vs_oracle(K, C):
+def test_check_matches_check_valid_prefix(K, C):
     from rq_vae_recommender_b200 import ops
     rs = np.random.RandomState(K + C)
     corpus = random_corpus(rs, 2000, C, K)
-    idx = ops.SidPrefixIndex(dev(corpus), K, kind="trie")
-    assert ops.SidPrefixIndex.kind_for(C, K) == ("bitmap" if K ** C <= 1 << 33 else "trie")
+    idx = ops.SidPrefixIndex(dev(corpus), K)
     for l in range(1, C + 1):
         p = prefixes(rs, corpus, l, K, n=1000)
         want = T.valid_prefixes(corpus, p, K)
@@ -33,21 +34,15 @@ def test_trie_check_vs_oracle(K, C):
 
 
 @pytest.mark.parametrize("N", [0, 1, 2])
-def test_trie_tiny_corpora(N):
+def test_check_on_tiny_corpora(N):
     from rq_vae_recommender_b200 import ops
     K, C = 256, 5
     corpus = np.array([[1, 2, 3, 4, 5], [1, 2, 300, 4, 5]], dtype=np.int64)[:N]
     idx = ops.SidPrefixIndex(dev(corpus.reshape(N, C)), K)
-    assert idx.kind == "trie"
     rs = np.random.RandomState(N)
     for l in range(1, C + 1):
         p = np.concatenate([np.array([[1, 2, 3, 4, 5], [1, 2, 300, 4, 5]])[:, :l], rs.randint(0, 4, size=(50, l))])
         assert np.array_equal(idx.check(dev(p)).cpu().numpy(), T.valid_prefixes(corpus.reshape(N, C), p, K)), l
-
-
-def both(corpus, K):
-    from rq_vae_recommender_b200 import ops
-    return ops.SidPrefixIndex(dev(corpus), K, kind="bitmap"), ops.SidPrefixIndex(dev(corpus), K, kind="trie")
 
 
 def same(a, b):
@@ -60,68 +55,86 @@ CASES = [(B, k, K) for B in (1, 7, 640) for k in (1, 10, 32) for K in (16, 256, 
 
 
 @pytest.mark.parametrize("B,k,K", CASES)
-def test_indexes_give_identical_results(B, k, K):
-    """Three levels of each search on both indexes of one corpus, each level fed the bitmap run's beams: outputs and the
-    reject / bad counts are bit-identical.  Logit rows with NaN, all -inf, and probability rows with zero sums are mixed in;
-    at k = 32, K = 2048 beam_topk recomputes its keys (65 536 candidates)."""
+def test_searches_agree_with_oracles_and_each_other(B, k, K):
+    """Three levels of each search on one corpus, each level fed the search's own beams.  Logit rows with NaN, all -inf, and
+    probability rows with a NaN or a zero sum are mixed in; at k = 32, K = 2048 beam_topk recomputes its keys (65 536
+    candidates).  sample_select (its candidates tested against a K-bit child mask per beam) is bit-identical to beam_select
+    (a binary search per candidate) over its own samples, which are sample_oracle's; check of every extension is
+    trie_oracle's; beam_topk matches beam_search_oracle and returns as many finite beams as there are valid finite
+    extensions, up to k.  The reject and bad counts are numpy's."""
+    from rq_vae_recommender_b200 import ops
     rs = np.random.RandomState(B * 7 + k * 131 + K)
     C = 3
     corpus = realistic_corpus(rs, 3000 if K == 16 else 12101, C, K)
-    bm, tr = both(corpus, K)
+    idx = ops.SidPrefixIndex(dev(corpus), K)
     nc = min(64, K, 1024 // k)
+    n = lambda t: None if t is None else t.cpu().numpy()
     gen_b = gen_s = lp_b = lp_s = None
     for h in range(C):
         kp = 1 if h == 0 else k
-        beams = None if h == 0 else gen_b.reshape(-1, h).cpu().numpy()
-        logits = dev(level_logits(rs, corpus, beams, B * kp, K))
+        beams = None if h == 0 else n(gen_b).reshape(-1, h)
+        logits = dev(np.clip(level_logits(rs, corpus, beams, B * kp, K), -60, 60))    # clipped as in test_beam_topk_vs_oracle
         if B * kp > 3:
             logits[1, 5] = float("nan")
             logits[2] = -float("inf")
-        counters = [torch.zeros(1, dtype=torch.int32, device="cuda") for _ in range(2)]
-        out = [i.beam_topk(logits, gen_b, lp_b, k, bad=c) for i, c in zip((bm, tr), counters)]
-        assert same(*out) and torch.equal(*counters)
+        bad = torch.zeros(1, dtype=torch.int32, device="cuda")
+        out = idx.beam_topk(logits, gen_b, lp_b, k, bad=bad)
+        x = n(logits)
+        assert int(bad) == int((np.isnan(x).any(1) | np.isposinf(x).any(1) | np.isneginf(x).all(1)).sum())
+        ref = oracle_level(corpus, logits, gen_b, lp_b, k)
+        assert_matches(*ref, out, k)
+        finite = np.isfinite(n(out[1]))
+        assert np.array_equal(finite.sum(1), np.minimum(k, np.isfinite(ref[3]).sum(1)))
+        assert T.valid_prefixes(corpus, n(out[0])[finite], K).all()
+
         probas = F.softmax(logits.nan_to_num(0.0), dim=-1)
         if B * kp > 3:
             probas[3] = 0.0
             probas[1, 2] = float("nan")
         noise = torch.empty_like(probas).exponential_(1)
-        rejects = [torch.zeros(2, dtype=torch.int32, device="cuda") for _ in range(2)]
-        samp = [i.sample_select(probas, noise, gen_s, lp_s, k, nc, want_samples=True, reject=r) for i, r in zip((bm, tr), rejects)]
-        assert same(*samp) and torch.equal(*rejects)
-        sel = [i.beam_select(samp[0][3], samp[0][4], gen_s, lp_s, k) for i in (bm, tr)]
-        assert same(*sel)
-        ext = torch.cat([samp[0][3].reshape(-1, 1) if h == 0 else
-                         torch.cat([gen_s.reshape(-1, h).repeat_interleave(nc, 0), samp[0][3].reshape(-1, 1)], 1)])
-        assert torch.equal(bm.check(ext), tr.check(ext))
-        gen_b, lp_b = out[0][0], out[0][1]
-        gen_s, lp_s = samp[0][0], samp[0][1]
+        reject = torch.zeros(2, dtype=torch.int32, device="cuda")
+        samp = idx.sample_select(probas, noise, gen_s, lp_s, k, nc, want_samples=True, reject=reject)
+        p = n(probas)
+        bad_rows = ~(p >= 0).all(1) | np.isinf(p).any(1)
+        assert n(reject).tolist() == [int(bad_rows.sum()), int((~bad_rows & (p == 0).all(1)).sum())]
+        assert np.array_equal(n(samp[3]), SO.sample_select(corpus, p, n(noise), n(gen_s), n(lp_s), k, nc)[3])
+        assert same(samp[:3], idx.beam_select(samp[3], samp[4], gen_s, lp_s, k))
+        ext = samp[3].reshape(-1, 1) if h == 0 else torch.cat([gen_s.reshape(-1, h).repeat_interleave(nc, 0),
+                                                                samp[3].reshape(-1, 1)], 1)
+        assert np.array_equal(n(idx.check(ext)), T.valid_prefixes(corpus, n(ext), K))
+        gen_b, lp_b = out[0], out[1]
+        gen_s, lp_s = samp[0], samp[1]
 
 
-def test_sparse_corpus_identical():
-    """Fewer valid extensions than k: -inf fillers in the same order on both indexes."""
+def test_sparse_corpus_fillers_in_oracle_order():
+    """Fewer valid extensions than k on all three levels: the valid ones first, then the -inf fillers in ascending flat index
+    (beam * K + code) with their parents and ids, exactly as beam_search_oracle has them."""
+    from rq_vae_recommender_b200 import ops
     K, k, B = 256, 10, 6
     corpus = np.array([[5, 1, 0], [5, 2, 0], [200, 7, 1]], dtype=np.int64)
-    bm, tr = both(corpus, K)
+    idx = ops.SidPrefixIndex(dev(corpus), K)
     rs = np.random.RandomState(22)
     g = lp = None
     for h in range(3):
-        logits = dev(rs.randn(B * (1 if h == 0 else k), K).astype(np.float32))
-        a, b = bm.beam_topk(logits, g, lp, k), tr.beam_topk(logits, g, lp, k)
-        assert same(a, b)
-        g, lp = a[0], a[1]
+        logits = rs.randn(B * (1 if h == 0 else k), K).astype(np.float32)
+        out = idx.beam_topk(dev(logits), g, lp, k)
+        og, op, opar = BO.beam_topk(corpus, logits, None if g is None else g.cpu().numpy(),
+                                    None if lp is None else lp.cpu().numpy(), k)
+        assert np.isneginf(op[:, -1]).all()
+        assert np.array_equal(out[0].cpu().numpy(), og) and np.array_equal(out[2].cpu().numpy().reshape(B, k), opar)
+        np.testing.assert_allclose(out[1].cpu().numpy(), op, rtol=TOL, atol=TOL)
+        g, lp = out[0], out[1]
 
 
-def test_sample_select_beyond_bitmap_limit():
+def test_sample_select_five_levels_vs_oracle():
     """K = 256, C = 5 (a 2^40-bit key space): per level the samples are torch.multinomial's under the same seed, and the
     selection is sample_oracle's (oracle.rq_oracle.beam_select over the samples and their log-probabilities)."""
-    import sample_oracle as SO
     from rq_vae_recommender_b200 import ops
     from rq_vae_recommender_b200.modules.model import draw_exponential
     K, C, B, k, nc = 256, 5, 24, 10, 64
     rs = np.random.RandomState(31)
     corpus = realistic_corpus(rs, 3000, C, K)
     idx = ops.SidPrefixIndex(dev(corpus), K)
-    assert idx.kind == "trie"
     generated = log_probas = None
     n_valid = 0
     for h in range(C):
@@ -146,14 +159,13 @@ def test_sample_select_beyond_bitmap_limit():
     assert n_valid > 0
 
 
-def test_beam_topk_beyond_bitmap_limit():
+def test_beam_topk_65536_candidates_four_levels_vs_oracle():
     """K = 2048, k = 32, C = 4 (2^44 keys): all four levels against beam_search_oracle, 65 536 candidates per history."""
     from rq_vae_recommender_b200 import ops
     K, C, B, k = 2048, 4, 7, 32
     rs = np.random.RandomState(32)
     corpus = realistic_corpus(rs, 12101, C, K)
     idx = ops.SidPrefixIndex(dev(corpus), K)
-    assert idx.kind == "trie"
     generated, log_probas = None, None
     for h in range(C):
         kp = 1 if h == 0 else k
@@ -164,8 +176,8 @@ def test_beam_topk_beyond_bitmap_limit():
         generated, log_probas = got[0], got[1]
 
 
-def test_generate_five_levels_both_searches():
-    """The drop-in model at five hierarchy levels (K = 256: no bitmap fits): one build then one launch per level, deterministic,
+def test_generate_five_levels_sample_and_beam():
+    """The drop-in model at five hierarchy levels (K = 256, 2^40 keys): one build then one launch per level, deterministic,
     the exhaustive search leaves the CUDA RNG state alone and agrees with the torch composition on hook-recorded logits, the
     sampled search equals torch.multinomial + beam_select under the same seed, and load_state_dict rebuilds the index."""
     from rq_vae_recommender_b200 import ops
@@ -180,7 +192,6 @@ def test_generate_five_levels_both_searches():
     rng = torch.cuda.get_rng_state()
     g1, p1 = m.generate(mask, ids, users, search="beam")
     assert ops.LAUNCHES - before == 1 + H
-    assert m._prefix_index_cache[1].kind == "trie"
     assert torch.equal(torch.cuda.get_rng_state(), rng)
     assert g1.shape == (B, k, H) and bool(torch.isfinite(p1).all())
     assert bool(torch.from_numpy(T.valid_prefixes(corpus, g1.reshape(-1, H).cpu().numpy(), K)).all())

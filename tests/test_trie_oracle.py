@@ -1,5 +1,5 @@
 """CPU tests of the corpus trie's numpy restatement (trie_oracle) against oracle.rq_oracle.check_valid_prefix on random corpora
-with duplicated rows and ids outside [0, K), and of the rule by which ops.SidPrefixIndex picks its index."""
+with duplicated rows and ids outside [0, K), and of the trie's size and index construction without a device."""
 import numpy as np
 import pytest
 
@@ -65,25 +65,19 @@ def test_duplicates_only_and_invalid_first_ids():
     assert T.lookup(trie, [[3, 4, 5], [3, 99, 1]]).tolist() == [True, False]
 
 
-@pytest.mark.parametrize("K", [16, 256, 512, 1024, 2048])
-@pytest.mark.parametrize("C", range(1, 9))
-def test_index_choice_follows_bitmap_limit(K, C):
-    """The bitmap wherever K^C fits its 2^33 bits (every shape that had an index before keeps it), the trie elsewhere."""
-    from rq_vae_recommender_b200 import ops
-    assert ops.SidPrefixIndex.kind_for(C, K) == ("bitmap" if K ** C <= 1 << 33 else "trie")
+def test_trie_bytes_without_a_device_below_the_corpus_table():
+    """The trie's persistent bytes are arithmetic (no device is queried) and, at the shipped shape and at a million rows, fewer
+    than those of the int64 corpus table [N, C] it indexes."""
+    from rq_vae_recommender_b200 import _lib
+    lib = _lib.load()
+    for N, C, K in ((12101, 3, 256), (1 << 20, 3, 256)):
+        nbytes = lib.rqb200_sid_trie_workspace_bytes(N, C, K)
+        assert 0 < nbytes < N * C * 8, (N, nbytes)
+    assert lib.rqb200_sid_trie_workspace_bytes(0x7fffffff, 3, 256) == 0                 # outside the trie's limits
 
 
-def test_index_choice_at_the_named_shapes():
-    from rq_vae_recommender_b200 import ops
-    kind = ops.SidPrefixIndex.kind_for
-    assert [kind(3, 256), kind(4, 256), kind(3, 2048), kind(8, 16)] == ["bitmap"] * 4
-    assert [kind(5, 256), kind(8, 256), kind(4, 512), kind(4, 2048), kind(8, 2048)] == ["trie"] * 5
-
-
-def test_index_rejects_cpu_tensors_and_unknown_kinds():
+def test_index_rejects_cpu_tensors():
     import torch
     from rq_vae_recommender_b200 import _lib, ops
     with pytest.raises(_lib.Rqb200Error):
         ops.SidPrefixIndex(torch.zeros((4, 5), dtype=torch.int64), 256)
-    with pytest.raises(_lib.Rqb200Error):
-        ops.SidPrefixIndex(torch.zeros((4, 5), dtype=torch.int64), 256, kind="trie")
