@@ -228,7 +228,8 @@ extern "C" int rqb200_tokenize_tc_run(const float* x, int64_t ldx, int B, const 
   int dev = 0, sm_count = 0;
   RQB_CUDA(cudaGetDevice(&dev));
   RQB_CUDA(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev));     // per call: the state may live on any device
-  // the converter reads x as float4: 16-byte aligned base and row pitch (ops.py copies other layouts)
+  // x's rows are bulk-copied to shared memory (16-byte aligned source and size): 16-byte aligned base and row pitch
+  // (ops.py copies other layouts)
   RQB_CHECK_ARG(((ldx & 3) == 0) && ((reinterpret_cast<uintptr_t>(x) & 15) == 0),
                 "tokenize_tc_run: x must be 16-byte aligned with a row stride that is a multiple of 4 floats");
   return tcx_run(x, ldx, B, state, D, K, L, ids, stats, sm_count, st);

@@ -11,14 +11,17 @@
 //   CUDA-core kernel (sequential fp32 residual, (xx + cc) - 2 dot, first index wins ties).
 //
 // One CTA per SM, persistent over 64-row tiles:
-//   warps 0-3 (one warpgroup)  convert the tile's rows to the fp16 image (K-major SWIZZLE_128B, resident for all levels) and
-//                              measure ||fp16(x) - x||^2 and ||x||^2 per row; per level and 256-code block: 4 x wgmma per 64-wide
-//                              k chunk into a 64 x 256 register accumulator, then score.  All 256 codes of a block sit in one
-//                              thread quad, so the block minimum and its candidate bits are quad shuffles; rows with more than
-//                              one candidate go to a shared queue that the four warps re-rank exactly.
-//   warp 4                     codebook producer: the prepared 16 KB blocks of codes [256 cb, 256 cb + 128) and [256 cb + 128,
-//                              256 cb + 256) of (level, k chunk) -> one 32 KB stage of a ring (bulk copies counted on an
-//                              mbarrier); it runs ahead into the next block, level and tile while the warpgroup scores and converts.
+//   warps 0-3 (one warpgroup)  convert the tile's rows from their x stages to the fp16 image (K-major SWIZZLE_128B, resident for
+//                              all levels) and measure ||fp16(x) - x||^2 and ||x||^2 per row; per level and 256-code block: 4 x
+//                              wgmma per 64-wide k chunk into a 64 x 256 register accumulator, then score.  All 256 codes of a
+//                              block sit in one thread quad, so the block minimum and its candidate bits are quad shuffles; rows
+//                              with more than one candidate go to a shared queue that the four warps re-rank exactly.
+//   warp 4                     producer of one 32 KB stage ring (bulk copies counted on an mbarrier per stage).  Per tile it
+//                              first stages the tile's fp32 rows, 128 columns per stage (one copy per row, spread over the
+//                              lanes), then for every (level, block, k chunk) the prepared 16 KB blocks of codes [256 cb,
+//                              256 cb + 128) and [256 cb + 128, 256 cb + 256).  It runs ahead into the next block, level and
+//                              tile while the warpgroup scores, so the next tile's rows are in flight while the last level of
+//                              this one is scored and re-ranked, and the conversion issues no global loads.
 //
 // Two kernels share every stage but the candidate selection:
 //   rq_tcx_kernel          K = 256: one accumulator holds the whole level, so the row minimum and the candidate words stay in
@@ -34,8 +37,11 @@
 #include "wgmma.cuh"
 
 #define TX_R 64                                   // rows per tile = wgmma M
-#define TX_NB_MAX 4                               // codebook ring stages
-#define TX_STAGE_BYTES (2 * TC_BSTAGE_BYTES)      // 256 codes x 64 k fp16 = 32 KB
+#define TX_NB_MAX 4                               // ring stages
+#define TX_STAGE_BYTES (2 * TC_BSTAGE_BYTES)      // 256 codes x 64 k fp16 = 32 KB = 64 rows x 128 columns of fp32 x
+#define TX_XCOLS 128                              // columns of x per stage: a 512-byte row
+#define TX_XROW_BYTES (TX_XCOLS * 4)
+#define TX_XGROUP 4                               // rows a converter warp reads from a stage at once
 #define TX_SLOT_BYTES (TX_R * TC_KC * 2)          // one k chunk of the x image: 8 KB
 #define TX_THREADS 160
 #define TX_SMEM_LIMIT 232448                      // 227 KB of opt-in shared memory per block
@@ -63,7 +69,7 @@ struct TxParams {
 };
 
 // Dynamic shared memory of a CTA, in order (tcx_smem_bytes sizes it):
-//   x image [nkc][8 KB] | codebook ring [nb][32 KB] | TxSmem |
+//   x image [nkc][8 KB] | ring [nb][32 KB] (x rows or codebook blocks) | TxSmem |
 //   cmask [TX_R][K / 32]   candidate bits (code 32 w + b -> word w, bit b): of the queued rows at K = 256, of every row above
 //   bmin  [TX_R][K / 256]  K > 256 only: per-block minimum, NaN if the block holds a NaN score
 //   ids   [L][TX_R]        ids of the tile: Id = uint8_t at K = 256 (16-bit ids would cost a ring stage at D = 768, L = 8),
@@ -113,12 +119,32 @@ __device__ __forceinline__ void tx_init(unsigned char* tsm, TxSmem* ms) {
   __syncthreads();
 }
 
-// codebook producer (one thread): stages in (tile, level, block, k chunk) order, the order the warpgroup consumes them
+// producer (warp 4): stages in the order the warpgroup consumes them -- per tile, its x stages, then (level, block, k chunk).
+// Lane 0 waits for a free slot and arms its mbarrier with the exact byte count.  X stage c holds columns [128 c, 128 c + 128)
+// (half of them when D % 128 == 64) of the tile's rows below B, 512 bytes per row whatever the width; each lane copies rows
+// lane and lane + 32.  Lane 0 copies the two 16 KB halves of a codebook stage.
 __device__ __forceinline__ void tx_produce(const TxParams& p, unsigned char* sC, TxSmem* ms, int nblk) {
-  const int nkc = p.nkc;
+  const int nkc = p.nkc, lane = threadIdx.x & 31, nxs = (p.D + TX_XCOLS - 1) / TX_XCOLS;
   const uint32_t nb = (uint32_t)p.nb;
   uint32_t s = 0;
-  for (int unit = blockIdx.x; unit < p.ntiles; unit += gridDim.x)
+  for (int unit = blockIdx.x; unit < p.ntiles; unit += gridDim.x) {
+    const int row0 = unit * TX_R, nrows = min(TX_R, p.B - row0);
+    for (int c = 0; c < nxs; ++c, ++s) {
+      const uint32_t st = s % nb, u = s / nb;
+      const uint32_t bytes = (uint32_t)min(TX_XCOLS, p.D - c * TX_XCOLS) * 4u;
+      if (lane == 0) {
+        mbar_wait_guarded(&ms->empty[st], (u & 1) ^ 1, 1);
+        mbar_expect_tx(&ms->full[st], (uint32_t)nrows * bytes);
+      }
+      __syncwarp();
+      unsigned char* dst = sC + st * TX_STAGE_BYTES;
+      for (int r = lane; r < nrows; r += 32)
+        bulk_g2s(dst + r * TX_XROW_BYTES, p.x + (int64_t)(row0 + r) * p.ldx + c * TX_XCOLS, bytes, &ms->full[st]);
+    }
+    if (lane != 0) {                   // the other lanes wait for lane 0 at the next tile's first x stage
+      s += (uint32_t)(p.L * nblk * nkc);
+      continue;
+    }
     for (int l = 0; l < p.L; ++l)
       for (int cb = 0; cb < nblk; ++cb)
         for (int kc = 0; kc < nkc; ++kc, ++s) {
@@ -130,42 +156,63 @@ __device__ __forceinline__ void tx_produce(const TxParams& p, unsigned char* sC,
           bulk_g2s(dst, p.blob + (h0 * nkc + kc) * TC_BSTAGE_BYTES, TC_BSTAGE_BYTES, &ms->full[st]);
           bulk_g2s(dst + TC_BSTAGE_BYTES, p.blob + ((h0 + 1) * nkc + kc) * TC_BSTAGE_BYTES, TC_BSTAGE_BYTES, &ms->full[st]);
         }
+  }
 }
 
-// fp16 image + row statistics of the tile at row0: warp w converts rows [16w, 16w + 16); lane = float4 column of every
-// 512-byte stretch.  The image is visible to the tensor core on return.
-__device__ __forceinline__ void tx_convert(const TxParams& p, TxSmem* ms, uint32_t x_base, int row0) {
+// fp16 image + row statistics of the tile at row0 from its x stages, the next ones of the ring (s counts the stages
+// consumed): warp w converts rows [16w, 16w + 16); lane = float4 column of every 512-byte stage row.  Each warp releases a
+// stage once its rows are read.  The per-lane sums of a row run over the columns in order, so the statistics do not depend
+// on the stage width.  Rows past B are zeros and are never read.  The image is visible to the tensor core on return.
+__device__ __forceinline__ void tx_convert(const TxParams& p, TxSmem* ms, uint32_t x_base, const unsigned char* sC, int row0,
+                                           uint32_t& s) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, lane4 = lane * 4, D = p.D;
-#pragma unroll 2
-  for (int i = 0; i < 16; ++i) {
-    const int R = warp * 16 + i, grow = row0 + R;
-    const float* xr = p.x + (int64_t)grow * p.ldx;
-    float4 v[6];
+  const int nxs = (D + TX_XCOLS - 1) / TX_XCOLS, nr = min(16, p.B - row0 - warp * 16);   // rows of this warp below B
+  const uint32_t nb = (uint32_t)p.nb;
+  float s2[16], e2[16];
 #pragma unroll
-    for (int c4 = 0; c4 < 6; ++c4) {
-      const int c = c4 * 128 + lane4;
-      v[c4] = (grow < p.B && c < D) ? __ldg(reinterpret_cast<const float4*>(xr + c)) : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    float s2 = 0.f, e2 = 0.f;
+  for (int i = 0; i < 16; ++i) { s2[i] = 0.f; e2[i] = 0.f; }
+#pragma unroll 1
+  for (int c4 = 0; c4 < nxs; ++c4, ++s) {
+    const uint32_t st = s % nb;
+    const int c = c4 * TX_XCOLS + lane4;
+    mbar_wait_guarded(&ms->full[st], (s / nb) & 1, 2);
+    const float4* srcp = reinterpret_cast<const float4*>(sC + st * TX_STAGE_BYTES + warp * 16 * TX_XROW_BYTES) + lane;
+    // TX_XGROUP rows at a time: the 128 accumulator registers stay allocated through the conversion, and with the 32
+    // partial sums more rows in flight spill in rq_tcx_blocked_kernel.  The image stores below carry no memory clobber, so
+    // the compiler may issue a group's stage loads ahead of the previous group's stores (they never overlap); the stage
+    // wait and release above and below are compiler barriers either way
 #pragma unroll
-    for (int c4 = 0; c4 < 6; ++c4) {
-      const int c = c4 * 128 + lane4;
-      if (c < D) {
-        const float4 a = v[c4];
+    for (int i0 = 0; i0 < 16; i0 += TX_XGROUP) {
+      float4 v[TX_XGROUP];
+#pragma unroll
+      for (int j = 0; j < TX_XGROUP; ++j) {
+        v[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (i0 + j < nr && c < D) v[j] = srcp[(i0 + j) * (TX_XROW_BYTES / 16)];
+      }
+      if (c >= D) continue;
+#pragma unroll
+      for (int j = 0; j < TX_XGROUP; ++j) {
+        const int i = i0 + j, R = warp * 16 + i;
+        const float4 a = v[j];
         const __half2 h0 = __floats2half2_rn(a.x, a.y), h1 = __floats2half2_rn(a.z, a.w);
         // the MEASURED rounding error of this row: fp16(x) - x is exact in fp32 (nearby values, or a flush to zero / inf)
         const float2 b0 = __half22float2(h0), b1 = __half22float2(h1);
         const float d0 = b0.x - a.x, d1 = b0.y - a.y, d2 = b1.x - a.z, d3 = b1.y - a.w;
-        s2 = fmaf(a.x, a.x, fmaf(a.y, a.y, fmaf(a.z, a.z, fmaf(a.w, a.w, s2))));
-        e2 = fmaf(d0, d0, fmaf(d1, d1, fmaf(d2, d2, fmaf(d3, d3, e2))));
+        s2[i] = fmaf(a.x, a.x, fmaf(a.y, a.y, fmaf(a.z, a.z, fmaf(a.w, a.w, s2[i]))));
+        e2[i] = fmaf(d0, d0, fmaf(d1, d1, fmaf(d2, d2, fmaf(d3, d3, e2[i]))));
         const uint32_t addr = x_base + (uint32_t)(c >> 6) * TX_SLOT_BYTES + (uint32_t)R * 128u +
                               ((((uint32_t)(c & 63) >> 3) ^ ((uint32_t)R & 7u)) << 4) + (uint32_t)(c & 7) * 2u;
         asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(*reinterpret_cast<const uint32_t*>(&h0)),
-                     "r"(*reinterpret_cast<const uint32_t*>(&h1)) : "memory");
+                     "r"(*reinterpret_cast<const uint32_t*>(&h1)));
       }
     }
-    s2 = warp_sum(s2); e2 = warp_sum(e2);
-    if (lane == 0) ms->rowinfo[R] = (tc_bf16_up(e2) << 16) | tc_bf16_up(s2);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&ms->empty[st]);
+  }
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    const float a = warp_sum(s2[i]), b = warp_sum(e2[i]);
+    if (lane == 0) ms->rowinfo[warp * 16 + i] = (tc_bf16_up(b) << 16) | tc_bf16_up(a);
   }
   fence_proxy_async();                 // generic-proxy smem writes -> visible to the tensor core (async proxy)
   tx_wg_sync();
@@ -419,7 +466,7 @@ __global__ void __launch_bounds__(TX_THREADS, 1) rq_tcx_kernel(const __grid_cons
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   tx_init(tsm, sh.ms);
   if (warp == 4) {
-    if (lane == 0) tx_produce(p, sh.sC, sh.ms, 1);
+    tx_produce(p, sh.sC, sh.ms, 1);
     return;
   }
   const int q4 = lane & 3;
@@ -429,7 +476,7 @@ __global__ void __launch_bounds__(TX_THREADS, 1) rq_tcx_kernel(const __grid_cons
 #pragma unroll 1
   for (int unit = blockIdx.x; unit < p.ntiles; unit += gridDim.x) {
     const int row0 = unit * TX_R;
-    tx_convert(p, sh.ms, x_base, row0);
+    tx_convert(p, sh.ms, x_base, sh.sC, row0, s);
 #pragma unroll 1
     for (int l = 0; l < p.L; ++l) {
       float acc[128];
@@ -468,7 +515,7 @@ __global__ void __launch_bounds__(TX_THREADS, 1) rq_tcx_blocked_kernel(const __g
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   tx_init(tsm, sh.ms);
   if (warp == 4) {
-    if (lane == 0) tx_produce(p, sh.sC, sh.ms, nblk);
+    tx_produce(p, sh.sC, sh.ms, nblk);
     return;
   }
   const int q4 = lane & 3;
@@ -478,7 +525,7 @@ __global__ void __launch_bounds__(TX_THREADS, 1) rq_tcx_blocked_kernel(const __g
 #pragma unroll 1
   for (int unit = blockIdx.x; unit < p.ntiles; unit += gridDim.x) {
     const int row0 = unit * TX_R;
-    tx_convert(p, sh.ms, x_base, row0);
+    tx_convert(p, sh.ms, x_base, sh.sC, row0, s);
 #pragma unroll 1
     for (int l = 0; l < p.L; ++l) {
       float run0 = INFINITY, run1 = INFINITY;                // running row minima over the blocks scored so far

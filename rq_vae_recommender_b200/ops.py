@@ -990,7 +990,7 @@ def rq_tokenize_tc(x: torch.Tensor, codebooks=None, state: Optional[TcState] = N
         raise _lib.Rqb200Error(f"rq_tokenize_tc: x is on {x.device}, the prepared state on {state.device}")
     if D != state.D:
         x = torch.nn.functional.pad(x, (0, state.D - D))
-    if x.data_ptr() % 16 or x.stride(0) % 4:        # the kernel reads x through TMA: 16-byte aligned base and row pitch
+    if x.data_ptr() % 16 or x.stride(0) % 4:        # the kernel bulk-copies x's rows: 16-byte aligned base and row pitch
         x = x.contiguous()
     ids = torch.empty((B, state.L), dtype=torch.int64, device=x.device)
     with torch.cuda.device(x.device):
