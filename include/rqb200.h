@@ -311,6 +311,33 @@ int rqb200_t5dec_self_attention(const float* qkv, int64_t ldqkv, float* cache_k,
 int rqb200_t5dec_add_norm(float* x, const float* delta, int64_t ld_delta, const float* emb, const int64_t* ids, int64_t ids_stride,
                           int64_t id_offset, int64_t n_emb, const float* weight, int R, int D, float eps, float* out, void* stream);
 
+/* ---- the generative-retrieval model's T5 encoder pass over kept tokens only (modules/model.py, generate(encoder="fused")),
+ * csrc/t5enc.cu ----
+ * The encoder input of a history of n = items * H ids (mask [B, n] fp32, ids [B, n] int64) has S = user + items * (H + sep)
+ * positions: the user row (user = 1), then per item its H ids and, with sep = 1, a separator carrying the mask of the item's last
+ * id.  A position is KEPT when its mask is nonzero (the user row always is); a history with no kept position keeps all S, and its
+ * keys then get -FLT_MAX added (HF's eager mask: the softmax averages every position).  Kept rows are packed history by history
+ * in position order; fp32 throughout, d_kv = 64 per head, sublayer boundaries are rqb200_t5dec_add_norm, GEMMs the caller's.
+ * t5enc_offsets  : offsets int32 [B + 1] (history b owns packed rows offsets[b] .. offsets[b + 1] - 1; offsets[B] = N, the
+ *                  packed row count) and key_mask fp32 [B] (0, or -FLT_MAX for a history without an unmasked position).  One CTA.
+ * t5enc_assemble : src int32 [N] = b * S + p of every packed row, slot int32 [B * S] = its packed row or -1 (dropped), and per
+ *                  packed row x = the input row -- user_table[remainder(user_ids[b * user_stride], n_users)] (user_table and
+ *                  user_ids both null: no user row), item_table[(ids[b, c] + (c % H) * K) * mask[b, c]] (an id outside
+ *                  [0, n_items) gives a NaN row), or sep_row (null: sep = 0) -- and out = T5LayerNorm(x) * weight; x, out [N, D].
+ * t5enc_attention: bidirectional self-attention among each history's packed rows.  qkv [N, 3 inner] (q | k | v, row stride
+ *                  ldqkv, a multiple of 4, 16-byte aligned), rel [heads, 2S - 1]: the score of query position i and key position
+ *                  j is q . k + (rel[n, j - i + S - 1] + key_mask[b]), no 1/sqrt(d) scaling, fp32 softmax.  out [N, inner] (row
+ *                  stride ldo, a multiple of 4, 16-byte aligned).  Any S.
+ * t5enc_scatter  : out[r] = rows[slot[r]] for r < n_out (= B * S), zeros where slot[r] = -1; rows [N, D], out [n_out, D]. */
+int rqb200_t5enc_offsets(const float* mask, int B, int n, int H, int sep, int user, int* offsets, float* key_mask, void* stream);
+int rqb200_t5enc_assemble(const float* mask, const int64_t* ids, int64_t ids_stride, const int64_t* user_ids, int64_t user_stride,
+                          const float* item_table, int64_t n_items, const float* sep_row, const float* user_table, int64_t n_users,
+                          int64_t K, int B, int n, int H, int D, const int* offsets, const float* weight, float eps, float* x,
+                          float* out, int* src, int* slot, void* stream);
+int rqb200_t5enc_attention(const float* qkv, int64_t ldqkv, const int* src, const int* offsets, const float* key_mask,
+                           const float* rel, int B, int S, int heads, float* out, int64_t ldo, void* stream);
+int rqb200_t5enc_scatter(const float* rows, const int* slot, int64_t n_out, int D, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

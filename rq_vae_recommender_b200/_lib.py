@@ -14,7 +14,7 @@ from typing import Optional
 PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "librqb200.so")
-SOURCES = ["api.cu", "rq_simt.cu", "dense.cu", "rq_tc.cu", "rq_tcx.cu", "gemm_tc.cu", "sid.cu", "t5dec.cu"]
+SOURCES = ["api.cu", "rq_simt.cu", "dense.cu", "rq_tc.cu", "rq_tcx.cu", "gemm_tc.cu", "sid.cu", "t5dec.cu", "t5enc.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-shared", "-Xcompiler", "-fPIC"]
 
@@ -84,6 +84,11 @@ _SIGNATURES = {
     "rqb200_t5dec_self_attention": (c_int, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int,
                                             c_vp, c_i64, c_vp]),
     "rqb200_t5dec_add_norm": (c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_vp, c_int, c_int, c_f32, c_vp, c_vp]),
+    "rqb200_t5enc_offsets": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
+    "rqb200_t5enc_assemble": (c_int, [c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i64, c_i64, c_int, c_int, c_int,
+                                      c_int, c_vp, c_vp, c_f32, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "rqb200_t5enc_attention": (c_int, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_i64, c_vp]),
+    "rqb200_t5enc_scatter": (c_int, [c_vp, c_vp, c_i64, c_int, c_vp, c_vp]),
     "rqb200_bf16_image_bytes": (c_size, [c_int, c_int]),
     "rqb200_f32_to_bf16_image": (c_int, [c_vp, c_i64, c_int, c_int, c_vp, c_vp]),
     "rqb200_gemm_bf16": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_i64, c_vp]),

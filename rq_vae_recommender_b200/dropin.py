@@ -11,7 +11,8 @@ tree untouched.  ``replace_model=True`` also aliases ``modules.model`` (train_de
 ``EncoderDecoderRetrievalModel.generate`` then runs its beam search on the fused sampling and selection kernel;
 ``search="beam"`` (with ``replace_model=True``) makes the exhaustive, deterministic beam search over every code its default, so
 an unmodified ``train_decoder.py`` evaluates with it; ``decoder="fused"`` (with ``replace_model=True``) likewise makes generate's
-decoder passes run on the fused decoder-step kernels (``FusedT5Decode``).  ``replace_metrics=True`` also aliases ``evaluate.metrics``
+decoder passes run on the fused decoder-step kernels (``FusedT5Decode``), and ``encoder="fused"`` its encoder pass over the
+unpadded positions only (``FusedT5Encode``).  ``replace_metrics=True`` also aliases ``evaluate.metrics``
 (train_decoder.py:13), whose ``TopKAccumulator`` accumulates on the device without waiting on the host.  Checkpoints pickle ``modules.quantize.Quantize`` etc. by module path,
 so ``torch.load(..., weights_only=False)`` of the shipped files also lands on the replacement classes.
 gin-config is not in this image: a small compatible shim is registered as ``gin`` when the real one is missing.
@@ -35,7 +36,7 @@ _METRICS = ("evaluate.metrics", "rq_vae_recommender_b200.evaluate.metrics")
 
 
 def install(reference_root=None, replace_tokenizer=True, gin_shim=True, replace_model=False, search="sample",
-            replace_metrics=False, decoder="hf"):
+            replace_metrics=False, decoder="hf", encoder="hf"):
     if search not in ("sample", "beam"):
         raise ValueError(f"search must be 'sample' or 'beam', got {search!r}")
     if search != "sample" and not replace_model:
@@ -44,6 +45,10 @@ def install(reference_root=None, replace_tokenizer=True, gin_shim=True, replace_
         raise ValueError(f"decoder must be 'hf' or 'fused', got {decoder!r}")
     if decoder != "hf" and not replace_model:
         raise ValueError(f"decoder={decoder!r} selects the replacement model's decoder passes: it needs replace_model=True")
+    if encoder not in ("hf", "fused"):
+        raise ValueError(f"encoder must be 'hf' or 'fused', got {encoder!r}")
+    if encoder != "hf" and not replace_model:
+        raise ValueError(f"encoder={encoder!r} selects the replacement model's encoder pass: it needs replace_model=True")
     if gin_shim and "gin" not in sys.modules:
         try:
             import gin  # noqa: F401
@@ -65,6 +70,7 @@ def install(reference_root=None, replace_tokenizer=True, gin_shim=True, replace_
         sys.modules[_MODEL[0]] = importlib.import_module(_MODEL[1])
         sys.modules[_MODEL[0]].DEFAULT_SEARCH = search
         sys.modules[_MODEL[0]].DEFAULT_DECODER = decoder
+        sys.modules[_MODEL[0]].DEFAULT_ENCODER = encoder
     if replace_metrics:
         sys.modules[_METRICS[0]] = importlib.import_module(_METRICS[1])
     return sorted(list(_ALIASES) + ([_TOKENIZER[0]] if replace_tokenizer else []) + ([_MODEL[0]] if replace_model else [])
@@ -80,3 +86,4 @@ def uninstall():
     if model is not None:
         model.DEFAULT_SEARCH = "sample"
         model.DEFAULT_DECODER = "hf"
+        model.DEFAULT_ENCODER = "hf"

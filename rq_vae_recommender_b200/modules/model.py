@@ -27,6 +27,10 @@ search when ``generate`` / ``generate_next_sem_id`` are not given one (``dropin.
 ``generate(..., decoder="fused")`` replaces only the decoder passes and their cache with ``FusedT5Decode`` (the decoder-step kernels
 of csrc/t5dec.cu between cuBLAS GEMMs, cross keys/values once per history, no cache copies); ``DEFAULT_DECODER`` ("hf") picks
 the decoder when none is given (``dropin.install(decoder=...)`` sets it).
+
+``generate(..., encoder="fused")`` replaces only the encoder pass with ``FusedT5Encode`` (the unpadded positions of each history
+only, packed, with the kernels of csrc/t5enc.cu between cuBLAS GEMMs); ``DEFAULT_ENCODER`` ("hf") picks the encoder when none is
+given (``dropin.install(encoder=...)`` sets it).
 """
 from typing import NamedTuple
 from typing import Optional
@@ -56,6 +60,10 @@ SEARCHES = ("sample", "beam")
 #: reference) or "fused" (FusedT5Decode: cross keys/values once per history, the decoder-step kernels of csrc/t5dec.cu)
 DEFAULT_DECODER = "hf"
 DECODERS = ("hf", "fused")
+#: the encoder pass generate() runs when it is not given an encoder: "hf" (transformers' T5EncoderModel over every padded
+#: position, as the reference) or "fused" (FusedT5Encode: the kept positions of each history only, the kernels of csrc/t5enc.cu)
+DEFAULT_ENCODER = "hf"
+ENCODERS = ("hf", "fused")
 _MULTINOMIAL_ERRORS = ("probability tensor contains either `inf`, `nan` or element < 0",
                        "invalid multinomial distribution (sum of probabilities <= 0)")
 
@@ -155,6 +163,67 @@ class FusedT5Decode:
             ff = lay[2].DenseReluDense
             ops.t5dec_add_norm(x, F.linear(F.linear(nrm, ff.wi.weight).relu_(), ff.wo.weight), self.norms[3 * l + 3], nrm, eps)
         return nrm
+
+
+def _read_n_kept(offsets: Tensor) -> int:
+    """The packed row count offsets[B], read on the host to size the encoder's GEMMs: the one host synchronisation of an
+    encoder="fused" pass."""
+    return int(offsets[-1])
+
+
+class FusedT5Encode:
+    """The encoder pass of ``generate(encoder="fused")``: ``encoder_forward_pass`` (HF's T5EncoderModel in eval mode, relu FFN,
+    d_kv 64) restated over the KEPT positions of each history only, as cuBLAS GEMMs (``F.linear``) between the kernels of
+    csrc/t5enc.cu and the decoder's ``t5dec_add_norm``:
+      * a position is kept when its mask is nonzero (the user row always is); a history with no unmasked position keeps all of
+        them, so HF's uniform average over its positions is reproduced.  Everywhere else a dropped position changes nothing:
+        HF's softmax gives a masked key the weight 0, and both decoders mask it again;
+      * kept rows are packed history by history; the GEMMs run on the packed [N, d_model] rows and self-attention adds HF's
+        relative-position bias at each row's ORIGINAL position (``compute_bias(S, S)`` of block 0, once per call);
+      * ``__call__`` returns what ``encoder_forward_pass`` returns: enc_out [B, S, d_model] with the rows of dropped positions
+        set to 0, and enc_mask [B, S] with the same values.
+    N is read on the host once per call (``_read_n_kept``) to size the GEMMs; it is the pass's only host synchronisation."""
+
+    def __init__(self, model: "EncoderDecoderRetrievalModel"):
+        enc = model.encoder.encoder
+        cfg = enc.config
+        if cfg.d_kv != ops.T5_DKV or cfg.is_gated_act or cfg.dense_act_fn != "relu":
+            raise Rqb200Error(f"encoder=\"fused\" needs d_kv = {ops.T5_DKV} and a relu feed-forward (d_kv = {cfg.d_kv}, "
+                              f"feed_forward_proj = {cfg.feed_forward_proj!r})")
+        self.model, self.eps = model, cfg.layer_norm_epsilon
+        self.blocks = [blk.layer for blk in enc.block]
+        self.w_qkv = [torch.cat([lay[0].SelfAttention.q.weight, lay[0].SelfAttention.k.weight, lay[0].SelfAttention.v.weight])
+                      for lay in self.blocks]
+        self.norms = [w for lay in self.blocks for w in (lay[0].layer_norm.weight, lay[1].layer_norm.weight)] + \
+            [enc.final_layer_norm.weight]
+        self.n_kept = None
+
+    def __call__(self, attention_mask: Tensor, input_ids: Tensor, user_id: Optional[Tensor] = None):
+        m, eps = self.model, self.eps
+        H = m.num_hierarchies
+        sep = m.sep_token is not None
+        user = user_id is not None and m.user_embedding is not None
+        B, n = attention_mask.shape
+        enc_mask = attention_mask
+        if sep:                                               # encoder_forward_pass's mask: the separator takes the item's last
+            items = enc_mask.view(B, n // H, H)
+            enc_mask = torch.cat([items, items[:, :, -1:]], dim=2).reshape(B, n // H * (H + 1))
+        if user:
+            enc_mask = torch.cat([torch.ones(B, 1, device=enc_mask.device), enc_mask], dim=1)
+        self.offsets, key_mask = ops.t5enc_offsets(attention_mask, H, sep, user)
+        self.n_kept = _read_n_kept(self.offsets)
+        x, nrm, self.src, slot = ops.t5enc_assemble(
+            attention_mask, input_ids, user_id if user else None, m.item_sid_embedding_table.weight, m.sep_token if sep else None,
+            m.user_embedding.weight if user else None, m.num_embeddings_per_hierarchy, H, self.offsets, self.n_kept,
+            self.norms[0], eps)
+        S = slot.shape[1]
+        rel = ops.t5enc_rel_bias(self.blocks[0][0].SelfAttention.compute_bias(S, S)[0])
+        for l, lay in enumerate(self.blocks):
+            a = ops.t5enc_attention(F.linear(nrm, self.w_qkv[l]), self.src, self.offsets, key_mask, rel, S)
+            ops.t5dec_add_norm(x, F.linear(a, lay[0].SelfAttention.o.weight), self.norms[2 * l + 1], nrm, eps)
+            ff = lay[1].DenseReluDense
+            ops.t5dec_add_norm(x, F.linear(F.linear(nrm, ff.wi.weight).relu_(), ff.wo.weight), self.norms[2 * l + 2], nrm, eps)
+        return ops.t5enc_scatter(nrm, slot), enc_mask
 
 
 class EncoderDecoderRetrievalModel(nn.Module):
@@ -308,8 +377,12 @@ class EncoderDecoderRetrievalModel(nn.Module):
     def _fused_decoder(self, enc_out: Tensor, enc_mask: Tensor, k: int) -> FusedT5Decode:
         return FusedT5Decode(self, enc_out, enc_mask, k)
 
+    def _fused_encoder(self) -> FusedT5Encode:
+        return FusedT5Encode(self)
+
     @torch.no_grad()
-    def generate(self, attention_mask, input_ids, user_id=None, search: Optional[str] = None, decoder: Optional[str] = None):
+    def generate(self, attention_mask, input_ids, user_id=None, search: Optional[str] = None, decoder: Optional[str] = None,
+                 encoder: Optional[str] = None):
         """Top-k semantic ids by beam search restricted to id prefixes of the corpus.  ``search`` (default: the module's
         ``DEFAULT_SEARCH``, read at call time):
           "sample"  per level, n_cands = min(64, K) tokens sampled without replacement per beam, scored by cumulative
@@ -320,19 +393,32 @@ class EncoderDecoderRetrievalModel(nn.Module):
           "hf"      transformers' T5Stack with an EncoderDecoderCache, as the reference drives it;
           "fused"   ``FusedT5Decode``: the same T5 maths with cross keys/values once per history and the decoder-step kernels of
                     csrc/t5dec.cu; eval mode only (HF would apply dropout in training mode).
+        ``encoder`` (default: the module's ``DEFAULT_ENCODER``, read at call time), independent of ``decoder`` and ``search``:
+          "hf"      ``encoder_forward_pass``: transformers' T5EncoderModel over every position, padded ones included;
+          "fused"   ``FusedT5Encode``: the same encoder output at every unpadded position (padded rows are 0) from the unpadded
+                    positions only; eval mode only.  It reads the packed row count on the host once, before the first level.
         Returns generated [B, top_k, num_hierarchies] and log_probas [B, top_k]."""
         search = DEFAULT_SEARCH if search is None else search
         decoder = DEFAULT_DECODER if decoder is None else decoder
+        encoder = DEFAULT_ENCODER if encoder is None else encoder
         if decoder not in DECODERS:
             raise ValueError(f"generate: decoder must be one of {DECODERS}, got {decoder!r}")
         if decoder == "fused" and self.training:
             raise ValueError("generate: decoder=\"fused\" runs the decoder in eval mode only; call model.eval() first (in "
                              "training mode HF's decoder applies dropout)")
+        if encoder not in ENCODERS:
+            raise ValueError(f"generate: encoder must be one of {ENCODERS}, got {encoder!r}")
+        if encoder == "fused" and self.training:
+            raise ValueError("generate: encoder=\"fused\" runs the encoder in eval mode only; call model.eval() first (in "
+                             "training mode HF's encoder applies dropout)")
         k = self.top_k_for_generation
         n_cands = min(MAX_CANDIDATES, self.num_embeddings_per_hierarchy)
         self._check_search_limits(search, k, n_cands)
         beam = search == "beam"
-        enc_out, enc_mask = self.encoder_forward_pass(attention_mask=attention_mask, input_ids=input_ids, user_id=user_id)
+        if encoder == "fused":
+            enc_out, enc_mask = self._fused_encoder()(attention_mask, input_ids, user_id)
+        else:
+            enc_out, enc_mask = self.encoder_forward_pass(attention_mask=attention_mask, input_ids=input_ids, user_id=user_id)
         index = self._prefix_index(enc_out.device)
         fused = self._fused_decoder(enc_out, enc_mask, k) if decoder == "fused" else None
         if fused is None:
@@ -375,20 +461,21 @@ class EncoderDecoderRetrievalModel(nn.Module):
 
     @torch.no_grad()
     def generate_next_sem_id(self, batch: TokenizedSeqBatch, top_k: bool = True, temperature: int = 1,
-                             search: Optional[str] = None, decoder: Optional[str] = None) -> GenerationOutput:
+                             search: Optional[str] = None, decoder: Optional[str] = None,
+                             encoder: Optional[str] = None) -> GenerationOutput:
         H = self.num_hierarchies
         generated, log_probas = self.generate(attention_mask=_strip_dedup_col(batch.seq_mask.long(), H + 1, H),
                                               input_ids=_strip_dedup_col(batch.sem_ids, H + 1, H), user_id=batch.user_ids,
-                                              search=search, decoder=decoder)
+                                              search=search, decoder=decoder, encoder=encoder)
         return GenerationOutput(sem_ids=generated, log_probas=log_probas)
 
     @torch.no_grad()
     def generate_items(self, batch: TokenizedSeqBatch, n: Optional[int] = None, search: Optional[str] = None,
-                       decoder: Optional[str] = None) -> ItemGenerationOutput:
+                       decoder: Optional[str] = None, encoder: Optional[str] = None) -> ItemGenerationOutput:
         """The top corpus items for each history: ``generate_next_sem_id``'s beams, unchanged, then one launch that takes the
         items of every finite beam whose ids are in the corpus, beam by beam in descending score order, each beam's items by
         dedup rank, no item twice, at most n (default top_k_for_generation) per history."""
-        out = self.generate_next_sem_id(batch, search=search, decoder=decoder)
+        out = self.generate_next_sem_id(batch, search=search, decoder=decoder, encoder=encoder)
         table = self._item_table(out.sem_ids.device)
         items, beams, count = table.retrieve(out.sem_ids, out.log_probas, self.top_k_for_generation if n is None else n)
         return ItemGenerationOutput(item_ids=items, beams=beams, count=count, sem_ids=out.sem_ids, log_probas=out.log_probas)

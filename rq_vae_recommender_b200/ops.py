@@ -930,6 +930,127 @@ def t5dec_add_norm(x: torch.Tensor, delta: Optional[torch.Tensor], weight: torch
     return out
 
 
+# ---------------------------------------------------------------------------------------------- fused T5 encoder pass
+def t5enc_len(n: int, H: int, sep: bool, user: bool) -> int:
+    """Positions of the encoder input of n = items * H ids: the user row, then per item its H ids and a separator."""
+    return int(user) + n // H * (H + int(sep))
+
+
+def t5enc_offsets(mask: torch.Tensor, H: int, sep: bool, user: bool):
+    """The kept positions of each history (rqb200_t5enc_offsets), one launch.  mask [B, n] (nonzero keeps the id; a separator
+    follows the mask of its item's last id, the user row is always kept; a history with nothing kept keeps every position) ->
+    (offsets int32 [B + 1], history b owning packed rows offsets[b] .. offsets[b + 1] - 1, and key_mask fp32 [B]: 0, or
+    -FLT_MAX for a history without an unmasked position)."""
+    _need_cuda(mask)
+    mask = _f32c(mask)
+    if mask.dim() != 2 or mask.shape[1] % H:
+        raise ValueError(f"mask {tuple(mask.shape)} must be [B, items * {H}]")
+    B, n = mask.shape
+    offsets = torch.empty(B + 1, dtype=torch.int32, device=mask.device)
+    key_mask = torch.empty(B, dtype=torch.float32, device=mask.device)
+    with torch.cuda.device(mask.device):
+        _lib.check(_lib.load().rqb200_t5enc_offsets(_p(mask), B, n, H, int(sep), int(user), _p(offsets), _p(key_mask), _stream()),
+                   "t5enc_offsets")
+    _count(1)
+    return offsets, key_mask
+
+
+def t5enc_assemble(mask: torch.Tensor, ids: torch.Tensor, user_ids: Optional[torch.Tensor], item_table: torch.Tensor,
+                   sep_row: Optional[torch.Tensor], user_table: Optional[torch.Tensor], K: int, H: int, offsets: torch.Tensor,
+                   n_kept: int, weight: torch.Tensor, eps: float):
+    """The packed encoder input and its first T5LayerNorm (rqb200_t5enc_assemble), one launch.  mask / ids [B, n] (ids int64, any
+    row stride), user_ids int64 [B, *] (column 0 is read) with user_table [U, D], or both None; item_table [V, D]; sep_row [D] or
+    None; offsets from ``t5enc_offsets`` with n_kept = offsets[B].  Returns x, out [n_kept, D] (the input rows and
+    T5LayerNorm(x) * weight), src int32 [n_kept] (b * S + p of each packed row) and slot int32 [B, S] (packed row or -1)."""
+    _need_cuda(mask, ids, user_ids, item_table, sep_row, user_table, offsets, weight)
+    if (user_ids is None) != (user_table is None):
+        raise ValueError("user_ids and user_table go together")
+    mask = _f32c(mask)
+    B, n = mask.shape
+    if ids.dtype != torch.int64 or ids.shape != (B, n) or ids.stride(1) != 1:
+        ids = ids.to(torch.int64).contiguous()
+        if ids.shape != (B, n):
+            raise ValueError(f"ids {tuple(ids.shape)} must be [{B}, {n}] like the mask")
+    item_table = _f32c(item_table)
+    D = item_table.shape[1]
+    if user_ids is not None:
+        if user_ids.dtype != torch.int64:
+            user_ids = user_ids.to(torch.int64)
+        if user_ids.dim() != 2 or user_ids.shape[0] != B:
+            raise ValueError(f"user_ids {tuple(user_ids.shape)} must be [{B}, *]")
+        user_table = _f32c(user_table)
+        if user_table.dim() != 2 or user_table.shape[1] != D:
+            raise ValueError(f"user_table {tuple(user_table.shape)} must be [U, {D}]")
+    if sep_row is not None:
+        sep_row = _f32c(sep_row).reshape(-1)
+        if sep_row.shape != (D,):
+            raise ValueError(f"sep_row must hold {D} values")
+    weight = _f32c(weight)
+    if weight.shape != (D,):
+        raise ValueError(f"weight {tuple(weight.shape)} must be [{D}]")
+    if offsets.dtype != torch.int32 or offsets.shape != (B + 1,):
+        raise ValueError(f"offsets must be int32 [{B + 1}]")
+    S = t5enc_len(n, H, sep_row is not None, user_table is not None)
+    x = torch.empty((n_kept, D), dtype=torch.float32, device=mask.device)
+    out = torch.empty_like(x)
+    src = torch.empty(n_kept, dtype=torch.int32, device=mask.device)
+    slot = torch.empty((B, S), dtype=torch.int32, device=mask.device)
+    with torch.cuda.device(mask.device):
+        _lib.check(_lib.load().rqb200_t5enc_assemble(
+            _p(mask), _p(ids), ids.stride(0), _p(user_ids), user_ids.stride(0) if user_ids is not None else 0, _p(item_table),
+            item_table.shape[0], _p(sep_row), _p(user_table), user_table.shape[0] if user_table is not None else 0, int(K), B, n, H,
+            D, _p(offsets), _p(weight), float(eps), _p(x), _p(out), _p(src), _p(slot), _stream()), "t5enc_assemble")
+    _count(1)
+    return x, out, src, slot
+
+
+def t5enc_rel_bias(bias: torch.Tensor) -> torch.Tensor:
+    """[heads, 2S - 1] from HF's compute_bias(S, S)[0] ([heads, S, S], a function of key - query position only): entry t is the
+    bias of distance t - (S - 1)."""
+    return torch.cat([bias[:, 1:, 0].flip(1), bias[:, 0, :]], dim=1).contiguous()
+
+
+def t5enc_attention(qkv: torch.Tensor, src: torch.Tensor, offsets: torch.Tensor, key_mask: torch.Tensor, rel: torch.Tensor,
+                    S: int) -> torch.Tensor:
+    """Bidirectional T5 self-attention among each history's packed rows (rqb200_t5enc_attention), one launch.  qkv [N, 3 inner]
+    (q | k | v), src / offsets / key_mask as ``t5enc_assemble`` / ``t5enc_offsets`` give them, rel [heads, 2S - 1] from
+    ``t5enc_rel_bias`` -> [N, inner]."""
+    _need_cuda(qkv, src, offsets, key_mask, rel)
+    rel = _f32c(rel)
+    heads = rel.shape[0]
+    if rel.shape != (heads, 2 * S - 1):
+        raise ValueError(f"rel {tuple(rel.shape)} must be [heads, {2 * S - 1}]")
+    inner = heads * T5_DKV
+    qkv = _rows_of(qkv, 3 * inner, "qkv")
+    if qkv.stride(0) % 4 or qkv.data_ptr() % 16:
+        qkv = qkv.contiguous()
+    B = offsets.shape[0] - 1
+    if offsets.dtype != torch.int32 or src.dtype != torch.int32 or src.shape != (qkv.shape[0],) or key_mask.shape != (B,):
+        raise ValueError("src must be int32 [N] with N = qkv rows, offsets int32 [B + 1], key_mask [B]")
+    key_mask = _f32c(key_mask)
+    out = torch.empty((qkv.shape[0], inner), dtype=torch.float32, device=qkv.device)
+    with torch.cuda.device(qkv.device):
+        _lib.check(_lib.load().rqb200_t5enc_attention(_p(qkv), qkv.stride(0), _p(src), _p(offsets), _p(key_mask), _p(rel), B, S,
+                                                      heads, _p(out), out.stride(0), _stream()), "t5enc_attention")
+    _count(1)
+    return out
+
+
+def t5enc_scatter(rows: torch.Tensor, slot: torch.Tensor) -> torch.Tensor:
+    """[B, S, D]: row slot[b, s] of rows [N, D], zeros where slot is -1 (rqb200_t5enc_scatter), one launch."""
+    _need_cuda(rows, slot)
+    rows = _f32c(rows)
+    if slot.dtype != torch.int32 or slot.dim() != 2 or not slot.is_contiguous():
+        raise ValueError("slot must be a contiguous int32 [B, S] tensor")
+    B, S = slot.shape
+    D = rows.shape[1]
+    out = torch.empty((B, S, D), dtype=torch.float32, device=rows.device)
+    with torch.cuda.device(rows.device):
+        _lib.check(_lib.load().rqb200_t5enc_scatter(_p(rows), _p(slot), B * S, D, _p(out), _stream()), "t5enc_scatter")
+    _count(1)
+    return out
+
+
 # ---------------------------------------------------------------------------------------------- tensor-core tokeniser
 def tc_supported(D: int, K: int, L: int) -> bool:
     return bool(_lib.load().rqb200_tokenize_tc_supported(D, K, L))
