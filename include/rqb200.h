@@ -145,7 +145,8 @@ int rqb200_gemm_bf16(const void* a_image, const void* w_image, int M, int N, int
  * two fp16 images hi + lo (22 significant bits); C = act(A B^T) costs three tcgen05.mma per k-step (hi.hi + lo.hi +
  * hi.lo, fp32 accumulate) and is written as fp32 rows.
  *   split_image_bytes  : bytes of one operand buffer [hi image][lo image][row scales] for a [rows, K] matrix
- *   f32_to_split_image : fp32 [rows, K] (ld = ldx) -> buffer; transposed != 0 reads the operand as x[K, rows]
+ *   f32_to_split_image : fp32 [rows, K] (ld = ldx) -> buffer, any K; transposed != 0 reads the operand as x[K, rows]
+ *                        (K <= 65535 * 64)
  *   gemm_split         : out[M, N] (ld = ldo) = act(A[M, K] . B[N, K]^T) from two such buffers; an optional mask[M, N]
  *                        zeroes the entries whose mask value is not > 0 (the ReLU' of a backward GEMM) */
 size_t rqb200_split_image_bytes(int rows, int K);

@@ -226,7 +226,8 @@ extern "C" int rqb200_gemm_bf16(const void* a_image, const void* w_image, int M,
 //                                                      is then 2^-25 absolute = 2^-39 of the row maximum)
 // and the product is three wgmma per k-step, hi.hi + lo.hi + hi.lo, each 64-wide k chunk promoted into an fp32 total (lo.lo is 2^-22
 // relative and dropped).  The epilogue multiplies by 2^-(e_row + e_col), both exact.  Measured against float64 the result is
-// as close as a plain fp32 FMA GEMM (tests/test_gpu_gemm_split.py states the bound that is asserted).
+// as close as a plain fp32 FMA GEMM (tests/test_gpu_gemm_split.py states the bound that is asserted).  Below K = 64 a plain fp32
+// GEMM is nearly exact and the format's worst case per product, 3 x 2^-22 of |a||b|, is the bound (tests/test_gpu_gemm_shapes.py).
 //
 // Image = the bf16 image's layout with fp16 elements: [row tile of 128][k chunk of 64][128 rows x 128 B swizzled]; one buffer
 // holds [hi image][lo image][row scales: 128 floats per row tile, value 2^-e].  K is padded with zeros to a multiple of 64, rows
@@ -238,7 +239,7 @@ extern "C" int rqb200_gemm_bf16(const void* a_image, const void* w_image, int M,
 #include <cuda_fp16.h>
 
 #define GS_STAGES 3
-#define GS_MAX_CHUNKS 12                   // 16-byte chunks per lane of the row splitter: K <= 32 * 8 * 12 = 3072
+#define GS_MAX_CHUNKS 12                   // 16-byte chunks per lane of the row splitter: K <= 32 * 8 * 12 = 3072 (wider: two passes)
 #define GS_STAGE_BYTES (4 * GT_BLK_BYTES)
 
 extern "C" size_t rqb200_split_image_bytes(int rows, int K) {
@@ -326,6 +327,56 @@ __global__ void __launch_bounds__(256) gs_split_rows_kernel(const float* __restr
   }
 }
 
+// Rows wider than the register-resident splitter takes (K > 32 * 8 * GS_MAX_CHUNKS): one warp per image row, two passes over
+// the row -- its maximum, then the split (the second read comes from L2: at most 8 rows of a CTA are in flight).  Same image
+// and scale as gs_split_rows_kernel.  grid = 16 per row tile (8 rows each), block = 256.
+__global__ void __launch_bounds__(256) gs_split_rows_wide_kernel(const float* __restrict__ x, int64_t ldx, int rows, int K,
+                                                                 unsigned char* img) {
+  const int nkc = (K + GT_KC - 1) / GT_KC, mtiles = gridDim.x / 16;
+  const int mt = blockIdx.x / 16, r = (blockIdx.x % 16) * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  const int row = mt * 128 + r;
+  unsigned char* hi_img = img;
+  unsigned char* lo_img = img + (size_t)mtiles * nkc * GT_BLK_BYTES;
+  float* scales = reinterpret_cast<float*>(img + 2 * (size_t)mtiles * nkc * GT_BLK_BYTES);
+  const int nchunks = nkc * 8;
+  const bool vec = (K % 8 == 0) && (ldx % 4 == 0) && ((reinterpret_cast<uintptr_t>(x) & 15) == 0);
+  // chunk c of the row (zeros past K and for rows >= rows): the splitters' 16-byte loads, or scalar loads off the vec layout
+  auto load = [&](int c, float (&v)[8]) {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) v[e] = 0.f;
+    if (row >= rows) return;
+    const float* src = x + (int64_t)row * ldx + c * 8;
+    if (vec && c * 8 + 8 <= K) {
+      const float4 a = __ldg(reinterpret_cast<const float4*>(src)), b = __ldg(reinterpret_cast<const float4*>(src) + 1);
+      v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+    } else {
+#pragma unroll
+      for (int e = 0; e < 8; ++e)
+        if (c * 8 + e < K) v[e] = __ldg(src + e);
+    }
+  };
+  float mx = 0.f;
+  for (int c = lane; c < nchunks; c += 32) {
+    float v[8];
+    load(c, v);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) mx = fmaxf(mx, fabsf(v[e]));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  const float s = gs_pow2_scale(mx);
+  if (lane == 0) scales[row] = 1.f / s;                          // exact: a power of two
+  for (int c = lane; c < nchunks; c += 32) {
+    float v[8];
+    load(c, v);
+    uint4 hi, lo;
+    gs_split8(v, s, hi, lo);
+    const size_t off = ((size_t)mt * nkc + (c >> 3)) * GT_BLK_BYTES + r * 128 + (((c & 7) ^ (r & 7)) << 4);
+    *reinterpret_cast<uint4*>(hi_img + off) = hi;
+    *reinterpret_cast<uint4*>(lo_img + off) = lo;
+  }
+}
+
 // Transposed source: image row r = column r of x[K, rows] (ld = ldx) -- the operand of x^T without materialising the transpose
 // (W^T for dgrad, C^T for W@C, g^T and h^T for the weight gradients whose contraction runs over the batch).  Three launches:
 //   gs_colmax_kernel    |column| maxima by atomicMax on the float bits (non-negative floats order like unsigned ints) into scales[]
@@ -399,10 +450,6 @@ extern "C" int rqb200_f32_to_split_image(const float* x, int64_t ldx, int rows, 
     RQB_LAUNCH_CHECK();
     gs_split_cols_kernel<<<dim3(mtiles, nkc), 256, 0, st>>>(x, ldx, rows, K, im);
   } else {
-    if (K > 32 * 8 * GS_MAX_CHUNKS) {
-      rqb_set_error("f32_to_split_image: K = %d > %d", K, 32 * 8 * GS_MAX_CHUNKS);
-      return RQB_ERR_UNSUPPORTED;
-    }
     unsigned char* im = reinterpret_cast<unsigned char*>(image);
     const int nchunks = ((K + GT_KC - 1) / GT_KC) * 8;
     if (nchunks <= 8) gs_split_rows_kernel<1, 8><<<mtiles, 256, 0, st>>>(x, ldx, rows, K, im);
@@ -411,7 +458,8 @@ extern "C" int rqb200_f32_to_split_image(const float* x, int64_t ldx, int rows, 
     else if (nchunks <= 64) gs_split_rows_kernel<2, 32><<<mtiles, 256, 0, st>>>(x, ldx, rows, K, im);
     else if (nchunks <= 96) gs_split_rows_kernel<3, 32><<<mtiles, 256, 0, st>>>(x, ldx, rows, K, im);
     else if (nchunks <= 128) gs_split_rows_kernel<4, 32><<<mtiles, 256, 0, st>>>(x, ldx, rows, K, im);
-    else gs_split_rows_kernel<GS_MAX_CHUNKS, 32><<<mtiles, 256, 0, st>>>(x, ldx, rows, K, im);
+    else if (nchunks <= 32 * GS_MAX_CHUNKS) gs_split_rows_kernel<GS_MAX_CHUNKS, 32><<<mtiles, 256, 0, st>>>(x, ldx, rows, K, im);
+    else gs_split_rows_wide_kernel<<<mtiles * 16, 256, 0, st>>>(x, ldx, rows, K, im);
   }
   RQB_LAUNCH_CHECK();
   return RQB_OK;

@@ -112,9 +112,18 @@ def _mlp_ref64(x, ws, normalize=False):
 def test_mlp_on_tensor_cores_forward_and_backward_vs_float64():
     """B = 4096 rows: every Linear of the shipped encoder shape runs on gs_gemm_kernel (forward and dgrad); outputs and all
     gradients are compared with float64 autograd, next to what plain fp32 torch achieves on the same inputs."""
+    _mlp_vs_float64(4096, [768, 512, 256, 128, 32])
+
+
+@pytest.mark.parametrize("B,dims", [(1024, [4096, 512, 256, 128, 32]), (1024, [32, 128, 256, 512, 4096])])
+def test_wide_mlp_on_tensor_cores_forward_and_backward_vs_float64(B, dims):
+    """An encoder and a decoder for 4096-wide items: the 4096-wide operands (encoder input, decoder output gradient) take the
+    two-pass row splitter, and every Linear still runs on gs_gemm_kernel."""
+    _mlp_vs_float64(B, dims)
+
+
+def _mlp_vs_float64(B, dims):
     from rq_vae_recommender_b200 import ops
-    dims = [768, 512, 256, 128, 32]
-    B = 4096
     x = dev(I.randn(530, B, dims[0]) * 0.05).requires_grad_(True)
     ws = [dev(w).requires_grad_(True) for w in I.mlp_weights(531, dims)]
     gy = dev(I.randn(532, B, dims[-1]))
