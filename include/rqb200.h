@@ -339,6 +339,38 @@ int rqb200_t5enc_attention(const float* qkv, int64_t ldqkv, const int* src, cons
                            const float* rel, int B, int S, int heads, float* out, int64_t ldo, void* stream);
 int rqb200_t5enc_scatter(const float* rows, const int* slot, int64_t n_out, int D, float* out, void* stream);
 
+/* ---- training the encoder pass over kept tokens (modules/model.py, forward(encoder="fused")), csrc/t5enc.cu ----
+ * Shapes and packing as above.  Attention-weight dropout with probability p (0 <= p < 1) keeps the weight of (history b, head n,
+ * query position i, key position j) when the first word of Philox4x32-10(counter {j, i, n, b}, key {seed lo, seed hi}) is at least
+ * floor(p * 2^32); seed is int64 [1] in device memory.  Kept weights are scaled by 1 / (1 - p).
+ * t5enc_attention_train   : t5enc_attention's output with that dropout, out = sum_j (P_ij keep_ij / (1 - p)) v_j, plus lse [N, heads]
+ *                           = (m - key_mask[b]) + log l, the log-sum-exp of the row's scores less key_mask (l the undropped sum).
+ * t5enc_attention_backward: from out (the forward's), dout [N, inner] and lse: dS = P (dP keep / (1 - p) - D) with
+ *                           D_i = dout_i . out_i written to delta [N, heads]; dqkv [N, 3 inner] (row stride ldd: dQ | dK | dV, every
+ *                           column written) and drel_part [B, t5enc_attention_backward_tiles(S), heads, 2S - 1], partial sums of
+ *                           d rel whose sum over the first two axes is d rel.  Two launches, no atomics: bit-reproducible.
+ *                           S <= 5120 (one shared-memory bin array of 2S - 1 floats per warp).
+ * t5enc_dropout_keep      : keep uint8 [B, heads, S, S] (0 / 1), the bits above for every position pair.
+ * t5enc_add_norm_fwd      : one warp per row: x_out = x + delta (delta null: x), out = weight * (x_out * inv), inv_rms [R] = inv =
+ *                           rsqrt(mean(x_out^2) + eps); x, x_out, out [R, D] contiguous.
+ * t5enc_add_norm_bwd      : from d_out [R, D] and d_res [R, D] (the gradient reaching x_out directly; null: 0): dx = d_x_out [R, D]
+ *                           (also the gradient of delta) and dw_part [t5enc_add_norm_bwd_parts(R), D], partial sums of d weight in
+ *                           a fixed order.  D <= 5120. */
+int rqb200_t5enc_attention_train(const float* qkv, int64_t ldqkv, const int* src, const int* offsets, const float* key_mask,
+                                 const float* rel, int B, int S, int heads, const int64_t* seed, float p, float* out, int64_t ldo,
+                                 float* lse, void* stream);
+int rqb200_t5enc_attention_backward_tiles(int S);
+int rqb200_t5enc_attention_backward(const float* qkv, int64_t ldqkv, const float* out, int64_t ldo, const float* dout, int64_t lddo,
+                                    const float* lse, const int* src, const int* offsets, const float* key_mask, const float* rel,
+                                    int B, int S, int heads, const int64_t* seed, float p, float* delta, float* dqkv, int64_t ldd,
+                                    float* drel_part, void* stream);
+int rqb200_t5enc_dropout_keep(const int64_t* seed, float p, int B, int heads, int S, uint8_t* keep, void* stream);
+int rqb200_t5enc_add_norm_fwd(const float* x, const float* delta, int64_t ld_delta, const float* weight, int R, int D, float eps,
+                              float* x_out, float* out, float* inv_rms, void* stream);
+int rqb200_t5enc_add_norm_bwd_parts(int R);
+int rqb200_t5enc_add_norm_bwd(const float* d_out, const float* d_res, const float* x_out, const float* inv_rms, const float* weight,
+                              int R, int D, float* dx, float* dw_part, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

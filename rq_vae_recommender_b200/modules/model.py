@@ -31,6 +31,10 @@ the decoder when none is given (``dropin.install(decoder=...)`` sets it).
 ``generate(..., encoder="fused")`` replaces only the encoder pass with ``FusedT5Encode`` (the unpadded positions of each history
 only, packed, with the kernels of csrc/t5enc.cu between cuBLAS GEMMs); ``DEFAULT_ENCODER`` ("hf") picks the encoder when none is
 given (``dropin.install(encoder=...)`` sets it).
+
+``forward(batch, encoder="fused")``, the training pass, runs the encoder as ``FusedT5EncodeTrain``: the same packed pass with a
+backward and HF's dropout; ``DEFAULT_FORWARD_ENCODER`` ("hf") picks it when none is given (``dropin.install(forward_encoder=...)``
+sets it).  The decoder of ``forward`` stays HF's T5Stack.
 """
 from typing import NamedTuple
 from typing import Optional
@@ -64,6 +68,9 @@ DECODERS = ("hf", "fused")
 #: position, as the reference) or "fused" (FusedT5Encode: the kept positions of each history only, the kernels of csrc/t5enc.cu)
 DEFAULT_ENCODER = "hf"
 ENCODERS = ("hf", "fused")
+#: the encoder pass forward() (the training pass) runs when it is not given an encoder: "hf" (transformers' T5EncoderModel) or
+#: "fused" (FusedT5EncodeTrain: the kept positions only, with the training kernels of csrc/t5enc.cu and HF's dropout)
+DEFAULT_FORWARD_ENCODER = "hf"
 _MULTINOMIAL_ERRORS = ("probability tensor contains either `inf`, `nan` or element < 0",
                        "invalid multinomial distribution (sum of probabilities <= 0)")
 
@@ -93,6 +100,12 @@ def draw_exponential(probas: Tensor) -> Tensor:
     """The Exp(1) draw ``torch.multinomial(probas, n)`` (without replacement) makes from the default generator: sampling is
     then ``topk(probas / draw, n)``.  Patch this function to inject noise."""
     return torch.empty_like(probas).exponential_(1)
+
+
+def dropout_rows(x: Tensor, p: float) -> Tensor:
+    """HF's nn.Dropout at the token-wise sites of the fused training encoder (embedding, attention output, feed-forward inner
+    and output, final output), drawn from torch's generator.  Patch this function to inject masks."""
+    return F.dropout(x, p, training=True) if p > 0 else x
 
 
 def _strip_dedup_col(tensor: Tensor, sem_ids_dim: int, n_layers: int) -> Tensor:
@@ -226,6 +239,171 @@ class FusedT5Encode:
         return ops.t5enc_scatter(nrm, slot), enc_mask
 
 
+def _encoder_layout(n: int, H: int, sep: bool, user: bool, device) -> Tensor:
+    """[3, S] per encoder position: kind (0 user row, 1 item id, 2 separator), the column of the [B, n] inputs it reads and the id's
+    level -- the layout encoder_forward_pass builds."""
+    W = H + int(sep)
+    q = torch.arange(n // H * W, device=device)
+    item, j = q // W, q % W
+    kind = torch.where(j < H, 1, 2)
+    col = item * H + torch.clamp(j, max=H - 1)
+    lvl = torch.where(j < H, j, 0)
+    out = torch.stack([kind, col, lvl])
+    if user:
+        out = torch.cat([torch.zeros((3, 1), dtype=out.dtype, device=device), out], dim=1)
+    return out
+
+
+class _AssembleFunction(torch.autograd.Function):
+    """The packed input rows x [N, D] of ``ops.t5enc_assemble``, with the backward of the gather: each packed row's gradient is
+    added (``index_put_`` with accumulate, a sorted and therefore deterministic sum) to the table row it was read from."""
+
+    @staticmethod
+    def forward(ctx, item_w, sep_row, user_w, mask, ids, user_ids, K, H, offsets, n_kept, norm_w, eps):
+        x, _, src, slot = ops.t5enc_assemble(mask, ids, user_ids, item_w, sep_row, user_w, K, H, offsets, n_kept, norm_w, eps)
+        ctx.save_for_backward(src, mask, ids, user_ids)
+        ctx.K, ctx.H, ctx.S, ctx.sep, ctx.user = K, H, slot.shape[1], sep_row is not None, user_w is not None
+        ctx.shapes = (item_w.shape[0], user_w.shape[0] if user_w is not None else 0)
+        ctx.mark_non_differentiable(src, slot)
+        return x, src, slot
+
+    @staticmethod
+    def backward(ctx, dx, _src, _slot):
+        src, mask, ids, user_ids = ctx.saved_tensors
+        V, U = ctx.shapes
+        lay = _encoder_layout(mask.shape[1], ctx.H, ctx.sep, ctx.user, dx.device)
+        src = src.long()
+        b, pos = src // ctx.S, src % ctx.S
+        kind, col, lvl = lay[0, pos], lay[1, pos], lay[2, pos]
+        d_item = d_sep = d_user = None
+        if ctx.needs_input_grad[0]:
+            row = (ids[b, col].long() + lvl * ctx.K) * mask[b, col].float().long()   # the kernel's id: masked ids read row 0
+            row = torch.where((kind == 1) & (row >= 0) & (row < V), row, V)
+            d_item = dx.new_zeros((V + 1, dx.shape[1])).index_put_((row,), dx, accumulate=True)[:V]
+        if ctx.sep and ctx.needs_input_grad[1]:
+            d_sep = (dx * (kind == 2).to(dx.dtype)[:, None]).sum(0, keepdim=True)
+        if ctx.user and ctx.needs_input_grad[2]:
+            row = torch.where(kind == 0, torch.remainder(user_ids[b, 0], U), U)
+            d_user = dx.new_zeros((U + 1, dx.shape[1])).index_put_((row,), dx, accumulate=True)[:U]
+        return d_item, d_sep, d_user, None, None, None, None, None, None, None, None, None
+
+
+class _ScatterFunction(torch.autograd.Function):
+    """``ops.t5enc_scatter`` with its backward: the packed rows' gradient is the output's gradient gathered at src."""
+
+    @staticmethod
+    def forward(ctx, rows, slot, src):
+        ctx.save_for_backward(src)
+        return ops.t5enc_scatter(rows, slot)
+
+    @staticmethod
+    def backward(ctx, dout):
+        (src,) = ctx.saved_tensors
+        return dout.reshape(-1, dout.shape[-1]).index_select(0, src.long()), None, None
+
+
+class _RelBiasFunction(torch.autograd.Function):
+    """``t5enc_rel_bias(compute_bias(S, S)[0])`` of a bidirectional T5Attention: rel [heads, 2S - 1] = table[bucket(t - (S - 1))]^T,
+    the same values.  Its backward adds d_rel into the table with ``index_put_`` (accumulate, a sorted sum), so the table's
+    gradient is bit-reproducible; compute_bias's embedding backward is not."""
+
+    @staticmethod
+    def forward(ctx, table, buckets):
+        ctx.save_for_backward(buckets)
+        ctx.rows = table.shape[0]
+        return table.index_select(0, buckets).t().contiguous()
+
+    @staticmethod
+    def backward(ctx, drel):
+        (buckets,) = ctx.saved_tensors
+        return drel.new_zeros((ctx.rows, drel.shape[0])).index_put_((buckets,), drel.t(), accumulate=True), None
+
+
+def _rel_bias(att, S: int) -> Tensor:
+    dist = torch.arange(-(S - 1), S, device=att.relative_attention_bias.weight.device)
+    buckets = att._relative_position_bucket(dist, bidirectional=not att.is_decoder, num_buckets=att.relative_attention_num_buckets,
+                                            max_distance=att.relative_attention_max_distance)
+    return _RelBiasFunction.apply(att.relative_attention_bias.weight, buckets.long())
+
+
+def _check_encoder_config(cfg, what: str) -> None:
+    if cfg.d_kv != ops.T5_DKV or cfg.is_gated_act or cfg.dense_act_fn != "relu":
+        raise Rqb200Error(f"{what} needs d_kv = {ops.T5_DKV} and a relu feed-forward (d_kv = {cfg.d_kv}, "
+                          f"feed_forward_proj = {cfg.feed_forward_proj!r})")
+
+
+#: longest encoder sequence the training attention's backward takes (one shared-memory bin array of 2S - 1 floats per warp)
+MAX_TRAIN_ENCODER_LEN = 5120
+
+
+class FusedT5EncodeTrain:
+    """The encoder pass of ``forward(encoder="fused")``: ``FusedT5Encode``'s packed pass (kept positions only, HF's relative bias
+    at the original positions) made trainable.  Autograd runs through
+      * ``_AssembleFunction`` (gradient into ``item_sid_embedding_table``, ``sep_token`` and ``user_embedding``),
+      * ``ops.T5EncAddNormFunction`` at every norm (out of place: the residual row and its inverse RMS are saved),
+      * ``ops.T5EncAttentionFunction`` (attention-weight dropout from a Philox stream keyed on a seed drawn per layer from torch's
+        generator, log-sum-exp saved; the backward recomputes P),
+      * ``F.linear`` for every GEMM and ``_ScatterFunction`` back to [B, S, d_model];
+    ``rel`` holds the values of ``t5enc_rel_bias(compute_bias(S, S)[0])`` of block 0 (``_rel_bias``: a gather of
+    ``relative_attention_bias`` at the buckets of distances -(S - 1) .. S - 1), so its gradient reaches that table summed over the
+    layers, as in HF, through a deterministic sum.  Dropout follows HF: embedding, attention weights, attention output, feed-forward inner and
+    output, final output, each with its module's probability read at call time when that module is in training mode (0 else).
+    The token-wise sites call ``dropout_rows``.  fp32 parameters only; an active autocast region raises ``ValueError``."""
+
+    def __init__(self, model: "EncoderDecoderRetrievalModel"):
+        enc = model.encoder.encoder
+        _check_encoder_config(enc.config, "encoder=\"fused\"")
+        if any(t.dtype != torch.float32 for t in model.parameters()):
+            raise Rqb200Error("forward(encoder=\"fused\") needs fp32 parameters")
+        self.model, self.enc, self.eps = model, enc, enc.config.layer_norm_epsilon
+        self.blocks = [blk.layer for blk in enc.block]
+        self.norms = [w for lay in self.blocks for w in (lay[0].layer_norm.weight, lay[1].layer_norm.weight)] + \
+            [enc.final_layer_norm.weight]
+
+    @staticmethod
+    def _p(mod) -> float:
+        return float(mod.p) if mod.training else 0.0
+
+    def __call__(self, attention_mask: Tensor, input_ids: Tensor, user_id: Optional[Tensor] = None):
+        if torch.is_autocast_enabled("cuda"):
+            raise ValueError("forward(encoder=\"fused\") runs fp32 kernels: it cannot run inside an autocast region")
+        m, enc, eps = self.model, self.enc, self.eps
+        H = m.num_hierarchies
+        sep = m.sep_token is not None
+        user = user_id is not None and m.user_embedding is not None
+        B, n = attention_mask.shape
+        S = ops.t5enc_len(n, H, sep, user)
+        if S > MAX_TRAIN_ENCODER_LEN:
+            raise Rqb200Error(f"forward(encoder=\"fused\"): {S} encoder positions exceed {MAX_TRAIN_ENCODER_LEN}")
+        enc_mask = attention_mask
+        if sep:
+            items = enc_mask.view(B, n // H, H)
+            enc_mask = torch.cat([items, items[:, :, -1:]], dim=2).reshape(B, n // H * (H + 1))
+        if user:
+            enc_mask = torch.cat([torch.ones(B, 1, device=enc_mask.device), enc_mask], dim=1)
+        offsets, key_mask = ops.t5enc_offsets(attention_mask, H, sep, user)
+        n_kept = _read_n_kept(offsets)
+        x, src, slot = _AssembleFunction.apply(
+            m.item_sid_embedding_table.weight, m.sep_token if sep else None, m.user_embedding.weight if user else None,
+            attention_mask, input_ids, user_id if user else None, m.num_embeddings_per_hierarchy, H, offsets, n_kept,
+            self.norms[0], eps)
+        x, nrm = ops.T5EncAddNormFunction.apply(dropout_rows(x, self._p(enc.dropout)), None, self.norms[0], eps)
+        rel = _rel_bias(self.blocks[0][0].SelfAttention, S)
+        for l, lay in enumerate(self.blocks):
+            att = lay[0].SelfAttention
+            p_att = float(att.dropout) if att.training else 0.0
+            seed = ops.t5enc_dropout_seed(x.device) if p_att > 0 else torch.zeros(1, dtype=torch.int64, device=x.device)
+            qkv = F.linear(nrm, torch.cat([att.q.weight, att.k.weight, att.v.weight]))
+            a = ops.T5EncAttentionFunction.apply(qkv, rel, src, offsets, key_mask, S, seed, p_att)
+            x, nrm = ops.T5EncAddNormFunction.apply(x, dropout_rows(F.linear(a, att.o.weight), self._p(lay[0].dropout)),
+                                                    self.norms[2 * l + 1], eps)
+            ff = lay[1].DenseReluDense
+            h = dropout_rows(F.relu(F.linear(nrm, ff.wi.weight)), self._p(ff.dropout))
+            x, nrm = ops.T5EncAddNormFunction.apply(x, dropout_rows(F.linear(h, ff.wo.weight), self._p(lay[1].dropout)),
+                                                    self.norms[2 * l + 2], eps)
+        return _ScatterFunction.apply(dropout_rows(nrm, self._p(enc.dropout)), slot, src), enc_mask
+
+
 class EncoderDecoderRetrievalModel(nn.Module):
     """T5 encoder over the history's semantic ids, T5 decoder stack plus one Linear head per hierarchy level for the next
     item's ids; ``generate`` is a sampled beam search restricted to id prefixes that occur in the corpus (``codebooks``)."""
@@ -316,12 +494,27 @@ class EncoderDecoderRetrievalModel(nn.Module):
             return out.last_hidden_state, out.past_key_values
         return out.last_hidden_state
 
-    def forward(self, batch: TokenizedSeqBatch) -> ModelOutput:
+    @torch.compiler.disable
+    def _fused_train_encoder_pass(self, attention_mask, input_ids, user_id):
+        """FusedT5EncodeTrain runs outside torch.compile's graphs (ctypes launches): a graph break, with backward through it."""
+        return FusedT5EncodeTrain(self)(attention_mask, input_ids, user_id)
+
+    def forward(self, batch: TokenizedSeqBatch, encoder: Optional[str] = None) -> ModelOutput:
+        """The training loss.  ``encoder`` (default: the module's ``DEFAULT_FORWARD_ENCODER``, read at call time):
+          "hf"      ``encoder_forward_pass``: transformers' T5EncoderModel over every position, as the reference;
+          "fused"   ``FusedT5EncodeTrain``: the kept positions only, with HF's dropout in training mode and none in eval mode;
+                    gradients in both.  It reads the packed row count on the host once."""
+        encoder = DEFAULT_FORWARD_ENCODER if encoder is None else encoder
+        if encoder not in ENCODERS:
+            raise ValueError(f"forward: encoder must be one of {ENCODERS}, got {encoder!r}")
         H = self.num_hierarchies
         input_ids = _strip_dedup_col(batch.sem_ids, H + 1, H)
         attention_mask = _strip_dedup_col(batch.seq_mask.long(), H + 1, H)
         fut_ids = batch.sem_ids_fut[:, :H]
-        enc, enc_mask = self.encoder_forward_pass(attention_mask=attention_mask, input_ids=input_ids, user_id=batch.user_ids)
+        if encoder == "fused":
+            enc, enc_mask = self._fused_train_encoder_pass(attention_mask, input_ids, batch.user_ids)
+        else:
+            enc, enc_mask = self.encoder_forward_pass(attention_mask=attention_mask, input_ids=input_ids, user_id=batch.user_ids)
         dec = self.decoder_forward_pass(future_ids=fut_ids, encoder_output=enc, attention_mask_for_encoder=enc_mask,
                                         use_cache=False)[:, :-1]
         loss = torch.tensor(0.0, device=dec.device)

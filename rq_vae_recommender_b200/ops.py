@@ -1051,6 +1051,172 @@ def t5enc_scatter(rows: torch.Tensor, slot: torch.Tensor) -> torch.Tensor:
     return out
 
 
+# ---------------------------------------------------------------------------------------------- training the T5 encoder pass
+def t5enc_dropout_seed(device) -> torch.Tensor:
+    """int64 [1] on the device: a fresh attention-dropout seed drawn from torch's generator of that device (no host read), so
+    ``torch.manual_seed`` reproduces the keep bits."""
+    return torch.empty(1, dtype=torch.int64, device=device).random_()
+
+
+def _check_p(p: float) -> float:
+    if not 0.0 <= p < 1.0:
+        raise ValueError(f"dropout probability {p} must be in [0, 1)")
+    return float(p)
+
+
+def t5enc_dropout_keep(seed: torch.Tensor, p: float, B: int, heads: int, S: int) -> torch.Tensor:
+    """uint8 [B, heads, S, S]: the attention-dropout keep bits (rqb200_t5enc_dropout_keep) that ``t5enc_attention_train`` applies
+    with this seed, indexed by (history, head, query position, key position), one launch."""
+    _need_cuda(seed)
+    if seed.dtype != torch.int64 or seed.numel() != 1:
+        raise ValueError("seed must be an int64 tensor of one element")
+    keep = torch.empty((B, heads, S, S), dtype=torch.uint8, device=seed.device)
+    with torch.cuda.device(seed.device):
+        _lib.check(_lib.load().rqb200_t5enc_dropout_keep(_p(seed), _check_p(p), B, heads, S, _p(keep), _stream()),
+                   "t5enc_dropout_keep")
+    _count(1)
+    return keep
+
+
+def t5enc_attention_train(qkv: torch.Tensor, src: torch.Tensor, offsets: torch.Tensor, key_mask: torch.Tensor, rel: torch.Tensor,
+                          S: int, seed: torch.Tensor, p: float):
+    """``t5enc_attention`` with HF's attention-weight dropout (probability p, keep bits from ``seed``) that also returns the
+    log-sum-exp the backward needs (rqb200_t5enc_attention_train), one launch -> (out [N, inner], lse [N, heads])."""
+    _need_cuda(qkv, src, offsets, key_mask, rel, seed)
+    rel = _f32c(rel)
+    heads = rel.shape[0]
+    if rel.shape != (heads, 2 * S - 1):
+        raise ValueError(f"rel {tuple(rel.shape)} must be [heads, {2 * S - 1}]")
+    qkv = _rows_of(qkv, 3 * heads * T5_DKV, "qkv")
+    if qkv.stride(0) % 4 or qkv.data_ptr() % 16:
+        qkv = qkv.contiguous()
+    B = offsets.shape[0] - 1
+    if offsets.dtype != torch.int32 or src.dtype != torch.int32 or src.shape != (qkv.shape[0],) or key_mask.shape != (B,):
+        raise ValueError("src must be int32 [N] with N = qkv rows, offsets int32 [B + 1], key_mask [B]")
+    if seed.dtype != torch.int64 or seed.numel() != 1:
+        raise ValueError("seed must be an int64 tensor of one element")
+    key_mask = _f32c(key_mask)
+    N = qkv.shape[0]
+    out = torch.empty((N, heads * T5_DKV), dtype=torch.float32, device=qkv.device)
+    lse = torch.empty((N, heads), dtype=torch.float32, device=qkv.device)
+    with torch.cuda.device(qkv.device):
+        _lib.check(_lib.load().rqb200_t5enc_attention_train(_p(qkv), qkv.stride(0), _p(src), _p(offsets), _p(key_mask), _p(rel), B,
+                                                            S, heads, _p(seed), _check_p(p), _p(out), out.stride(0), _p(lse),
+                                                            _stream()), "t5enc_attention_train")
+    _count(1)
+    return out, lse
+
+
+def t5enc_attention_backward(qkv: torch.Tensor, out: torch.Tensor, dout: torch.Tensor, lse: torch.Tensor, src: torch.Tensor,
+                             offsets: torch.Tensor, key_mask: torch.Tensor, rel: torch.Tensor, S: int, seed: torch.Tensor, p: float):
+    """The backward of ``t5enc_attention_train`` (rqb200_t5enc_attention_backward), two launches and one fixed-order sum ->
+    (d_qkv [N, 3 inner], d_rel [heads, 2S - 1]).  Bit-reproducible."""
+    _need_cuda(qkv, out, dout, lse, src, offsets, key_mask, rel, seed)
+    heads = rel.shape[0]
+    inner = heads * T5_DKV
+    qkv, out, dout = _rows_of(qkv, 3 * inner, "qkv"), _rows_of(out, inner, "out"), _rows_of(dout, inner, "dout")
+    qkv, out, dout = (t if t.stride(0) % 4 == 0 and t.data_ptr() % 16 == 0 else t.contiguous() for t in (qkv, out, dout))
+    lse, rel, key_mask = _f32c(lse), _f32c(rel), _f32c(key_mask)
+    B, N = offsets.shape[0] - 1, qkv.shape[0]
+    if out.shape[0] != N or dout.shape[0] != N or lse.shape != (N, heads) or rel.shape != (heads, 2 * S - 1):
+        raise ValueError("out / dout [N, inner], lse [N, heads] and rel [heads, 2S - 1] must match qkv [N, 3 inner]")
+    lib = _lib.load()
+    tiles = lib.rqb200_t5enc_attention_backward_tiles(S)
+    delta = torch.empty((N, heads), dtype=torch.float32, device=qkv.device)
+    dqkv = torch.empty((N, 3 * inner), dtype=torch.float32, device=qkv.device)
+    part = torch.empty((B * tiles, heads, 2 * S - 1), dtype=torch.float32, device=qkv.device)
+    with torch.cuda.device(qkv.device):
+        _lib.check(lib.rqb200_t5enc_attention_backward(_p(qkv), qkv.stride(0), _p(out), out.stride(0), _p(dout), dout.stride(0),
+                                                       _p(lse), _p(src), _p(offsets), _p(key_mask), _p(rel), B, S, heads, _p(seed),
+                                                       _check_p(p), _p(delta), _p(dqkv), dqkv.stride(0), _p(part), _stream()),
+                   "t5enc_attention_backward")
+    _count(2)
+    return dqkv, part.sum(0)
+
+
+def t5enc_add_norm_fwd(x: torch.Tensor, delta: Optional[torch.Tensor], weight: torch.Tensor, eps: float):
+    """Out-of-place add + T5LayerNorm (rqb200_t5enc_add_norm_fwd), one launch: x [R, D] and delta [R, D] or None ->
+    (x_out = x + delta, out = T5LayerNorm(x_out) * weight, inv_rms [R])."""
+    _need_cuda(x, delta, weight)
+    x = _f32c(x)
+    R, D = x.shape
+    weight = _f32c(weight)
+    if weight.shape != (D,):
+        raise ValueError(f"weight {tuple(weight.shape)} must be [{D}]")
+    if delta is not None:
+        delta = _rows_of(delta, D, "delta")
+        if delta.shape[0] != R:
+            raise ValueError(f"delta has {delta.shape[0]} rows, x {R}")
+    x_out, out = torch.empty_like(x), torch.empty_like(x)
+    inv = torch.empty(R, dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        _lib.check(_lib.load().rqb200_t5enc_add_norm_fwd(_p(x), _p(delta), delta.stride(0) if delta is not None else 0, _p(weight),
+                                                         R, D, float(eps), _p(x_out), _p(out), _p(inv), _stream()),
+                   "t5enc_add_norm_fwd")
+    _count(1)
+    return x_out, out, inv
+
+
+def t5enc_add_norm_bwd(d_out: torch.Tensor, d_res: Optional[torch.Tensor], x_out: torch.Tensor, inv_rms: torch.Tensor,
+                       weight: torch.Tensor):
+    """The backward of ``t5enc_add_norm_fwd`` (rqb200_t5enc_add_norm_bwd), one launch and one fixed-order sum: d_out [R, D] (the
+    norm output's gradient) and d_res [R, D] or None (x_out's own) -> (dx [R, D], the gradient of x and delta, d_weight [D])."""
+    _need_cuda(d_out, d_res, x_out, inv_rms, weight)
+    x_out, d_out, inv_rms, weight = _f32c(x_out), _f32c(d_out), _f32c(inv_rms), _f32c(weight)
+    R, D = x_out.shape
+    if d_res is not None:
+        d_res = _f32c(d_res)
+    for name, t in (("d_out", d_out), ("d_res", d_res)):
+        if t is not None and t.shape != (R, D):
+            raise ValueError(f"{name} {tuple(t.shape)} must be [{R}, {D}]")
+    lib = _lib.load()
+    dx = torch.empty_like(x_out)
+    part = torch.empty((lib.rqb200_t5enc_add_norm_bwd_parts(R), D), dtype=torch.float32, device=x_out.device)
+    with torch.cuda.device(x_out.device):
+        _lib.check(lib.rqb200_t5enc_add_norm_bwd(_p(d_out), _p(d_res), _p(x_out), _p(inv_rms), _p(weight), R, D, _p(dx), _p(part),
+                                                 _stream()), "t5enc_add_norm_bwd")
+    _count(1)
+    return dx, part.sum(0)
+
+
+class T5EncAttentionFunction(torch.autograd.Function):
+    """Autograd of the training attention: ``apply(qkv, rel, src, offsets, key_mask, S, seed, p)`` -> out [N, inner]; gradients
+    for qkv and rel."""
+
+    @staticmethod
+    def forward(ctx, qkv, rel, src, offsets, key_mask, S, seed, p):
+        qkv = qkv.contiguous()
+        out, lse = t5enc_attention_train(qkv, src, offsets, key_mask, rel, S, seed, p)
+        ctx.save_for_backward(qkv, rel, src, offsets, key_mask, seed, out, lse)
+        ctx.S, ctx.p = S, p
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        qkv, rel, src, offsets, key_mask, seed, out, lse = ctx.saved_tensors
+        dqkv, drel = t5enc_attention_backward(qkv, out, dout, lse, src, offsets, key_mask, rel, ctx.S, seed, ctx.p)
+        return dqkv, drel, None, None, None, None, None, None
+
+
+class T5EncAddNormFunction(torch.autograd.Function):
+    """Autograd of the training add + norm: ``apply(x, delta, weight, eps)`` (delta may be None) -> (x_out, out)."""
+
+    @staticmethod
+    def forward(ctx, x, delta, weight, eps):
+        x_out, out, inv = t5enc_add_norm_fwd(x, delta, weight, eps)
+        ctx.save_for_backward(x_out, inv, weight)
+        ctx.has_delta = delta is not None
+        return x_out, out
+
+    @staticmethod
+    def backward(ctx, d_x_out, d_out):
+        x_out, inv, weight = ctx.saved_tensors
+        if d_out is None:
+            d_out = torch.zeros_like(x_out)
+        dx, dw = t5enc_add_norm_bwd(d_out, d_x_out, x_out, inv, weight)
+        return dx, dx if ctx.has_delta else None, dw, None
+
+
 # ---------------------------------------------------------------------------------------------- tensor-core tokeniser
 def tc_supported(D: int, K: int, L: int) -> bool:
     return bool(_lib.load().rqb200_tokenize_tc_supported(D, K, L))
