@@ -1,5 +1,6 @@
 #!/usr/bin/env python
-"""bench_train_decoder.py -- the generative-retrieval model's training step with HF's encoder against the packed fused encoder.
+"""bench_train_decoder.py -- the generative-retrieval model's training step for every (encoder, decoder) pair of HF's passes and the
+fused ones.
 
     python bench_train_decoder.py [--min-window-s 1.0] [--windows 3]
 
@@ -9,11 +10,13 @@ training mode with HF's dropout 0.1, the module's matmul precision "high", TF32)
   * "full":    batch 640, every history 20 items;
   * "ml1m":    batch 64, every history 200 items (ML-1M's max_seq_len; 801 encoder positions);
 it reports:
-  * ms per training step -- ``model(batch, encoder=...)``, ``loss.backward()``, ``AdamW.step()`` and ``zero_grad`` -- for encoder
-    "hf" against "fused", alternating the arms, --windows windows of at least --min-window-s seconds each (CUDA events);
+  * ms per training step -- ``model(batch, encoder=..., decoder=...)``, ``loss.backward()``, ``AdamW.step()`` and ``zero_grad`` --
+    for the four arms (encoder, decoder) in {hf, fused}^2, alternating the arms, --windows windows of at least --min-window-s
+    seconds each (CUDA events);
   * torch.cuda.max_memory_allocated during one step of each arm (model, optimizer state and inputs included);
-  * a CUDA-event split of the fused step: encoder forward, encoder backward (the encoder output's gradient through the packed
-    pass), and the rest (decoder and heads forward and backward, optimizer);
+  * a CUDA-event split of each arm's step: encoder forward, decoder + heads forward, decoder + heads backward, encoder backward
+    (the encoder output's gradient through the encoder) and optimizer.  The split cuts the step at the encoder output, so it
+    runs the fused pair as two graph breaks instead of one;
 Prints the card's name, power limit and max SM clock, read in the same run, and one JSON line; writes nothing.
 """
 import argparse
@@ -45,44 +48,60 @@ def batch_of(torch, rs, B, items, lengths):
                              token_type_ids=torch.zeros_like(sem), token_type_ids_fut=torch.zeros_like(fut))
 
 
-def step_fn(m, opt, batch, encoder):
+ARMS = [("hf", "hf"), ("fused", "hf"), ("hf", "fused"), ("fused", "fused")]
+
+
+def step_fn(m, opt, batch, encoder, decoder):
     def step():
-        out = m(batch, encoder=encoder)
+        out = m(batch, encoder=encoder, decoder=decoder)
         out.loss.backward()
         opt.step()
         opt.zero_grad(set_to_none=True)
     return step
 
 
-def fused_split(torch, M, m, opt, batch, reps=10):
-    """Mean ms of the fused step's encoder forward, encoder backward and the rest, over reps steps with CUDA events."""
+def step_split(torch, M, m, opt, batch, encoder, decoder, reps=10):
+    """Mean ms of the step's encoder forward, decoder + heads forward, decoder + heads backward, encoder backward and optimizer,
+    over reps steps with CUDA events."""
     Hh = m.num_hierarchies
-    tot = [0.0, 0.0, 0.0]
+    names = ("encoder_forward_ms", "decoder_forward_ms", "decoder_backward_ms", "encoder_backward_ms", "optimizer_ms")
+    tot = [0.0] * len(names)
     for rep in range(reps + 1):
-        ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(len(names) + 1)]
         ev[0].record()
         mask = M._strip_dedup_col(batch.seq_mask.long(), Hh + 1, Hh)
         ids = M._strip_dedup_col(batch.sem_ids, Hh + 1, Hh)
-        enc, enc_mask = m._fused_train_encoder_pass(mask, ids, batch.user_ids)
-        ev[1].record()
-        leaf = enc.detach().requires_grad_()
         fut = batch.sem_ids_fut[:, :Hh]
-        dec = m.decoder_forward_pass(future_ids=fut, encoder_output=leaf, attention_mask_for_encoder=enc_mask)[:, :-1]
+        if encoder == "fused" and decoder == "fused":
+            packed = M.FusedT5EncodeTrain(m).packed(mask, ids, batch.user_ids)
+            out = packed.rows
+        elif encoder == "fused":
+            out, enc_mask = m._fused_train_encoder_pass(mask, ids, batch.user_ids)
+        else:
+            out, enc_mask = m.encoder_forward_pass(attention_mask=mask, input_ids=ids, user_id=batch.user_ids)
+        ev[1].record()
+        leaf = out.detach().requires_grad_()
+        if encoder == "fused" and decoder == "fused":
+            key_mask = packed.key_mask.index_select(0, torch.div(packed.src, packed.S, rounding_mode="floor").long())
+            dec = M.FusedT5DecodeTrain(m)(fut, leaf, packed.offsets, key_mask, packed.src, packed.S)
+        elif decoder == "fused":
+            dec = m._fused_train_decoder_pass(fut, leaf, enc_mask)
+        else:
+            dec = m.decoder_forward_pass(future_ids=fut, encoder_output=leaf, attention_mask_for_encoder=enc_mask)[:, :-1]
         loss = sum(torch.nn.functional.cross_entropy(m.decoder_mlp[h](dec[:, h]), fut[:, h].long()) for h in range(Hh))
-        loss.backward()
         ev[2].record()
-        enc.backward(leaf.grad)
+        loss.backward()
         ev[3].record()
+        out.backward(leaf.grad)
+        ev[4].record()
         opt.step()
         opt.zero_grad(set_to_none=True)
-        ev_end = torch.cuda.Event(enable_timing=True)
-        ev_end.record()
+        ev[5].record()
         torch.cuda.synchronize()
         if rep:
-            tot[0] += ev[0].elapsed_time(ev[1])
-            tot[1] += ev[2].elapsed_time(ev[3])
-            tot[2] += ev[1].elapsed_time(ev[2]) + ev[3].elapsed_time(ev_end)
-    return {"encoder_forward_ms": tot[0] / reps, "encoder_backward_ms": tot[1] / reps, "rest_ms": tot[2] / reps}
+            for i in range(len(names)):
+                tot[i] += ev[i].elapsed_time(ev[i + 1])
+    return {name: t / reps for name, t in zip(names, tot)}
 
 
 def main():
@@ -106,7 +125,7 @@ def main():
         m = M.EncoderDecoderRetrievalModel(codebooks=torch.from_numpy(corpus_of(np, 3000, 1, K, H)), **SHAPE).cuda().train()
         opt = torch.optim.AdamW(m.parameters(), lr=1e-4)
         batch = batch_of(torch, rs, B, items, lengths)
-        steps = {enc: step_fn(m, opt, batch, enc) for enc in ("hf", "fused")}
+        steps = {f"{enc}/{dec}": step_fn(m, opt, batch, enc, dec) for enc, dec in ARMS}
         mem = {}
         for enc, fn in steps.items():
             fn()
@@ -119,16 +138,18 @@ def main():
         for _ in range(args.windows):
             for enc, fn in steps.items():
                 times[enc].append(timed_ms(torch, fn, args.min_window_s))
-        split = fused_split(torch, M, m, opt, batch)
+        split = {f"{enc}/{dec}": step_split(torch, M, m, opt, batch, enc, dec) for enc, dec in ARMS}
         kept = float(batch.seq_mask.float().mean())
         row = {"batch": B, "items": items, "lengths": "uniform %d..%d" % lengths if lengths else "all %d" % items,
                "kept_fraction_of_ids": round(kept, 3),
                "step_ms": {enc: [round(t, 2) for t in ts] for enc, ts in times.items()},
                "peak_mib": {enc: round(v, 1) for enc, v in mem.items()},
-               "fused_split_ms": {k: round(v, 2) for k, v in split.items()}}
-        row["speedup_median"] = round(float(np.median(times["hf"]) / np.median(times["fused"])), 3)
-        print(f"{name}: B={B} items={items} {row['lengths']}: step ms hf {row['step_ms']['hf']} fused {row['step_ms']['fused']} "
-              f"(x{row['speedup_median']}), peak MiB {row['peak_mib']}, fused split {row['fused_split_ms']}")
+               "split_ms": {arm: {k: round(v, 2) for k, v in sp.items()} for arm, sp in split.items()}}
+        row["speedup_median_vs_hf"] = {arm: round(float(np.median(times["hf/hf"]) / np.median(ts)), 3) for arm, ts in times.items()}
+        print(f"{name}: B={B} items={items} {row['lengths']}")
+        for arm in steps:
+            print(f"  {arm:12s} step ms {row['step_ms'][arm]} (x{row['speedup_median_vs_hf'][arm]} vs hf/hf), peak MiB "
+                  f"{row['peak_mib'][arm]}, split {row['split_ms'][arm]}")
         result["sets"][name] = row
         del m, opt, batch, steps
         torch.cuda.empty_cache()

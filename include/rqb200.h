@@ -371,6 +371,39 @@ int rqb200_t5enc_add_norm_bwd_parts(int R);
 int rqb200_t5enc_add_norm_bwd(const float* d_out, const float* d_res, const float* x_out, const float* inv_rms, const float* weight,
                               int R, int D, float* dx, float* dw_part, void* stream);
 
+/* ---- training the decoder pass (modules/model.py, forward(decoder="fused")), csrc/t5dec.cu ----
+ * T (<= 8, else RQB_ERR_UNSUPPORTED) decoder positions per history: row b * T + t of q / qkv / out / dout holds position t of
+ * history b; inner = heads * 64, fp32, strides in elements, no 1/sqrt(d) scaling.  Attention-weight dropout as the encoder's:
+ * the weight of (history b, head n, query position t, key position j) is kept when the first word of Philox4x32-10(counter
+ * {j, t, n, b}, key {seed lo, seed hi}) is at least floor(p * 2^32), kept weights scaled by 1 / (1 - p); seed int64 [1] in device
+ * memory.  No atomics: the backwards are bit-reproducible.
+ * t5dec_self_attention_train   : causal self-attention, qkv [B * T, 3 inner] (q | k | v), rel [heads, 2T - 1] (the bias of key j
+ *                                for query t is rel[n, j - t + T - 1]); keys j > t get weight 0.  out [B * T, inner], lse
+ *                                [B * T, heads] = m + log l of the undropped scores.
+ * t5dec_self_attention_backward: from out (the forward's), dout and lse: dqkv [B * T, 3 inner] (dQ | dK | dV) and drel_part
+ *                                [B, heads, 2T - 1], partial sums of d rel whose sum over the first axis is d rel.
+ * t5dec_cross_attention_train  : attention of q [B * T, inner] over key rows offsets[b] .. offsets[b + 1] - 1 (int32 [B + 1]) of k / v
+ *                                (row stride ldkv), score q . k + key_mask[row] (key_mask fp32 [rows]: 0, or -FLT_MAX to mask).
+ *                                The key's position j in the dropout counter is src[row] - b * S (src int32 [rows], the packed
+ *                                encoder's b * S + p) or, with src null, row - offsets[b].  out [B * T, inner], lse [B * T, heads] =
+ *                                (m - base) + log l with base the history's largest key_mask (finite when every key is masked).  A
+ *                                history without keys gets zeros.
+ * t5dec_cross_attention_backward: from out, dout and lse: dq [B * T, inner] (row stride lddq) and dk / dv (row stride lddkv, the rows
+ *                                of k / v; rows no history owns are not written). */
+int rqb200_t5dec_self_attention_train(const float* qkv, int64_t ldqkv, const float* rel, int B, int T, int heads, const int64_t* seed,
+                                      float p, float* out, int64_t ldo, float* lse, void* stream);
+int rqb200_t5dec_self_attention_backward(const float* qkv, int64_t ldqkv, const float* out, int64_t ldo, const float* dout,
+                                         int64_t lddo, const float* lse, const float* rel, int B, int T, int heads,
+                                         const int64_t* seed, float p, float* dqkv, int64_t ldd, float* drel_part, void* stream);
+int rqb200_t5dec_cross_attention_train(const float* q, int64_t ldq, const float* k, const float* v, int64_t ldkv, const int* offsets,
+                                       const float* key_mask, const int* src, int B, int S, int T, int heads, const int64_t* seed,
+                                       float p, float* out, int64_t ldo, float* lse, void* stream);
+int rqb200_t5dec_cross_attention_backward(const float* q, int64_t ldq, const float* k, const float* v, int64_t ldkv, const float* out,
+                                          int64_t ldo, const float* dout, int64_t lddo, const float* lse, const int* offsets,
+                                          const float* key_mask, const int* src, int B, int S, int T, int heads,
+                                          const int64_t* seed, float p, float* dq, int64_t lddq, float* dk, float* dv, int64_t lddkv,
+                                          void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -98,7 +98,15 @@ _SIGNATURES = {
     "rqb200_t5enc_add_norm_fwd": (c_int, [c_vp, c_vp, c_i64, c_vp, c_int, c_int, c_f32, c_vp, c_vp, c_vp, c_vp]),
     "rqb200_t5enc_add_norm_bwd_parts": (c_int, [c_int]),
     "rqb200_t5enc_add_norm_bwd": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp]),
-    "rqb200_bf16_image_bytes": (c_size, [c_int, c_int]),
+    "rqb200_t5dec_self_attention_train": (c_int, [c_vp, c_i64, c_vp, c_int, c_int, c_int, c_vp, c_f32, c_vp, c_i64, c_vp, c_vp]),
+    "rqb200_t5dec_self_attention_backward": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_vp,
+                                                     c_f32, c_vp, c_i64, c_vp, c_vp]),
+    "rqb200_t5dec_cross_attention_train": (c_int, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int,
+                                                   c_vp, c_f32, c_vp, c_i64, c_vp, c_vp]),
+    "rqb200_t5dec_cross_attention_backward": (c_int, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp,
+                                                      c_vp, c_int, c_int, c_int, c_int, c_vp, c_f32, c_vp, c_i64, c_vp, c_vp, c_i64,
+                                                      c_vp]),
+    "rqb200_bf16_image_bytes":(c_size, [c_int, c_int]),
     "rqb200_f32_to_bf16_image": (c_int, [c_vp, c_i64, c_int, c_int, c_vp, c_vp]),
     "rqb200_gemm_bf16": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_i64, c_vp]),
     "rqb200_split_image_bytes": (c_size, [c_int, c_int]),

@@ -33,9 +33,8 @@
 // Numerics are HF's: no 1/sqrt(d) scaling, fp32 softmax, RMS norm in fp32.
 #include <cfloat>
 
-#include <curand_kernel.h>
-
 #include "common.cuh"
+#include "t5_dropout.cuh"
 
 #define TE_DKV 64           // d_kv, as in csrc/t5dec.cu
 #define TE_SCAN 1024        // threads of the offsets kernel (histories per chunk)
@@ -167,17 +166,7 @@ __global__ void __launch_bounds__(TE_ASM) t5enc_assemble_kernel(
 }
 
 // ------------------------------------------------------------------------------------------------ self-attention
-// Keep bit of the attention weight of (history b, head n, query position pi, key position pj): one Philox4x32-10 draw, kept when
-// its first word is at least thresh = p * 2^32 (so thresh = 0 keeps everything).
-__device__ __forceinline__ bool te_keep(uint2 key, int b, int n, int pi, int pj, uint32_t thresh) {
-  return curand_Philox4x32_10(make_uint4((unsigned)pj, (unsigned)pi, (unsigned)n, (unsigned)b), key).x >= thresh;
-}
-
-__device__ __forceinline__ uint2 te_seed_key(const int64_t* seed) {
-  const uint64_t s = (uint64_t)seed[0];
-  return make_uint2((unsigned)s, (unsigned)(s >> 32));
-}
-
+// The attention-weight dropout's keep bits are te_keep of csrc/t5_dropout.cuh.
 // grid (B, heads, ceil(S / TE_AQ)).  qkv row r: q at n * 64, k at inner + n * 64, v at 2 inner + n * 64.  rel [heads, 2S - 1]:
 // the bias of key position pj for query position pi is rel[n, pj - pi + S - 1].  TRAIN adds the dropout of the attention weights
 // (thresh != 0: a dropped weight leaves the sum of values, a kept one is scaled by `scale` = 1 / (1 - p); l stays the undropped
@@ -652,12 +641,6 @@ extern "C" int rqb200_t5enc_scatter(const float* rows, const int* slot, int64_t 
   t5enc_scatter_kernel<<<(unsigned)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(rows, slot, n_out, D, out);
   RQB_LAUNCH_CHECK();
   return RQB_OK;
-}
-
-// 0 <= p < 1 -> the Philox threshold and the kept weights' scale
-static void dropout_params(float p, uint32_t* thresh, float* scale) {
-  *thresh = (uint32_t)((double)p * 4294967296.0);
-  *scale = *thresh ? 1.f / (1.f - p) : 1.f;
 }
 
 static int attention_train_args(const float* qkv, int64_t ldqkv, int B, int S, int heads, float p, const char* what) {

@@ -13,7 +13,8 @@ tree untouched.  ``replace_model=True`` also aliases ``modules.model`` (train_de
 an unmodified ``train_decoder.py`` evaluates with it; ``decoder="fused"`` (with ``replace_model=True``) likewise makes generate's
 decoder passes run on the fused decoder-step kernels (``FusedT5Decode``), and ``encoder="fused"`` its encoder pass over the
 unpadded positions only (``FusedT5Encode``); ``forward_encoder="fused"`` makes the training pass ``forward`` run its encoder on
-the trainable packed pass (``FusedT5EncodeTrain``).  ``replace_metrics=True`` also aliases ``evaluate.metrics``
+the trainable packed pass (``FusedT5EncodeTrain``), and ``forward_decoder="fused"`` its decoder on the fused training
+decoder (``FusedT5DecodeTrain``).  ``replace_metrics=True`` also aliases ``evaluate.metrics``
 (train_decoder.py:13), whose ``TopKAccumulator`` accumulates on the device without waiting on the host.  Checkpoints pickle ``modules.quantize.Quantize`` etc. by module path,
 so ``torch.load(..., weights_only=False)`` of the shipped files also lands on the replacement classes.
 gin-config is not in this image: a small compatible shim is registered as ``gin`` when the real one is missing.
@@ -37,7 +38,7 @@ _METRICS = ("evaluate.metrics", "rq_vae_recommender_b200.evaluate.metrics")
 
 
 def install(reference_root=None, replace_tokenizer=True, gin_shim=True, replace_model=False, search="sample",
-            replace_metrics=False, decoder="hf", encoder="hf", forward_encoder="hf"):
+            replace_metrics=False, decoder="hf", encoder="hf", forward_encoder="hf", forward_decoder="hf"):
     if search not in ("sample", "beam"):
         raise ValueError(f"search must be 'sample' or 'beam', got {search!r}")
     if search != "sample" and not replace_model:
@@ -54,6 +55,11 @@ def install(reference_root=None, replace_tokenizer=True, gin_shim=True, replace_
         raise ValueError(f"forward_encoder must be 'hf' or 'fused', got {forward_encoder!r}")
     if forward_encoder != "hf" and not replace_model:
         raise ValueError(f"forward_encoder={forward_encoder!r} selects the replacement model's training encoder pass: it needs "
+                         "replace_model=True")
+    if forward_decoder not in ("hf", "fused"):
+        raise ValueError(f"forward_decoder must be 'hf' or 'fused', got {forward_decoder!r}")
+    if forward_decoder != "hf" and not replace_model:
+        raise ValueError(f"forward_decoder={forward_decoder!r} selects the replacement model's training decoder pass: it needs "
                          "replace_model=True")
     if gin_shim and "gin" not in sys.modules:
         try:
@@ -78,6 +84,7 @@ def install(reference_root=None, replace_tokenizer=True, gin_shim=True, replace_
         sys.modules[_MODEL[0]].DEFAULT_DECODER = decoder
         sys.modules[_MODEL[0]].DEFAULT_ENCODER = encoder
         sys.modules[_MODEL[0]].DEFAULT_FORWARD_ENCODER = forward_encoder
+        sys.modules[_MODEL[0]].DEFAULT_FORWARD_DECODER = forward_decoder
     if replace_metrics:
         sys.modules[_METRICS[0]] = importlib.import_module(_METRICS[1])
     return sorted(list(_ALIASES) + ([_TOKENIZER[0]] if replace_tokenizer else []) + ([_MODEL[0]] if replace_model else [])
@@ -95,3 +102,4 @@ def uninstall():
         model.DEFAULT_DECODER = "hf"
         model.DEFAULT_ENCODER = "hf"
         model.DEFAULT_FORWARD_ENCODER = "hf"
+        model.DEFAULT_FORWARD_DECODER = "hf"

@@ -34,7 +34,9 @@ given (``dropin.install(encoder=...)`` sets it).
 
 ``forward(batch, encoder="fused")``, the training pass, runs the encoder as ``FusedT5EncodeTrain``: the same packed pass with a
 backward and HF's dropout; ``DEFAULT_FORWARD_ENCODER`` ("hf") picks it when none is given (``dropin.install(forward_encoder=...)``
-sets it).  The decoder of ``forward`` stays HF's T5Stack.
+sets it).  ``forward(batch, decoder="fused")`` runs the decoder as ``FusedT5DecodeTrain``: the H positions the loss reads, on the
+decoder training kernels of csrc/t5dec.cu with HF's dropout; ``DEFAULT_FORWARD_DECODER`` ("hf") picks it when none is given
+(``dropin.install(forward_decoder=...)`` sets it).  With both fused, the decoder attends to the encoder's packed rows.
 """
 from typing import NamedTuple
 from typing import Optional
@@ -71,6 +73,9 @@ ENCODERS = ("hf", "fused")
 #: the encoder pass forward() (the training pass) runs when it is not given an encoder: "hf" (transformers' T5EncoderModel) or
 #: "fused" (FusedT5EncodeTrain: the kept positions only, with the training kernels of csrc/t5enc.cu and HF's dropout)
 DEFAULT_FORWARD_ENCODER = "hf"
+#: the decoder pass forward() runs when it is not given a decoder: "hf" (transformers' T5Stack) or "fused" (FusedT5DecodeTrain:
+#: the H positions the loss reads, with the training kernels of csrc/t5dec.cu and HF's dropout)
+DEFAULT_FORWARD_DECODER = "hf"
 _MULTINOMIAL_ERRORS = ("probability tensor contains either `inf`, `nan` or element < 0",
                        "invalid multinomial distribution (sum of probabilities <= 0)")
 
@@ -365,22 +370,31 @@ class FusedT5EncodeTrain:
         return float(mod.p) if mod.training else 0.0
 
     def __call__(self, attention_mask: Tensor, input_ids: Tensor, user_id: Optional[Tensor] = None):
+        """(enc_out [B, S, d_model] with the rows of dropped positions 0, enc_mask [B, S]), as ``encoder_forward_pass``."""
+        out = self.packed(attention_mask, input_ids, user_id)
+        H = self.model.num_hierarchies
+        sep = self.model.sep_token is not None
+        B, n = attention_mask.shape
+        enc_mask = attention_mask
+        if sep:
+            items = enc_mask.view(B, n // H, H)
+            enc_mask = torch.cat([items, items[:, :, -1:]], dim=2).reshape(B, n // H * (H + 1))
+        if user_id is not None and self.model.user_embedding is not None:
+            enc_mask = torch.cat([torch.ones(B, 1, device=enc_mask.device), enc_mask], dim=1)
+        return _ScatterFunction.apply(out.rows, out.slot, out.src), enc_mask
+
+    def packed(self, attention_mask: Tensor, input_ids: Tensor, user_id: Optional[Tensor] = None) -> "PackedEncoderOutput":
+        """The pass without the scatter: the kept rows [N, d_model] (the encoder's final dropout applied) and their layout."""
         if torch.is_autocast_enabled("cuda"):
             raise ValueError("forward(encoder=\"fused\") runs fp32 kernels: it cannot run inside an autocast region")
         m, enc, eps = self.model, self.enc, self.eps
         H = m.num_hierarchies
         sep = m.sep_token is not None
         user = user_id is not None and m.user_embedding is not None
-        B, n = attention_mask.shape
+        n = attention_mask.shape[1]
         S = ops.t5enc_len(n, H, sep, user)
         if S > MAX_TRAIN_ENCODER_LEN:
             raise Rqb200Error(f"forward(encoder=\"fused\"): {S} encoder positions exceed {MAX_TRAIN_ENCODER_LEN}")
-        enc_mask = attention_mask
-        if sep:
-            items = enc_mask.view(B, n // H, H)
-            enc_mask = torch.cat([items, items[:, :, -1:]], dim=2).reshape(B, n // H * (H + 1))
-        if user:
-            enc_mask = torch.cat([torch.ones(B, 1, device=enc_mask.device), enc_mask], dim=1)
         offsets, key_mask = ops.t5enc_offsets(attention_mask, H, sep, user)
         n_kept = _read_n_kept(offsets)
         x, src, slot = _AssembleFunction.apply(
@@ -401,7 +415,114 @@ class FusedT5EncodeTrain:
             h = dropout_rows(F.relu(F.linear(nrm, ff.wi.weight)), self._p(ff.dropout))
             x, nrm = ops.T5EncAddNormFunction.apply(x, dropout_rows(F.linear(h, ff.wo.weight), self._p(lay[1].dropout)),
                                                     self.norms[2 * l + 2], eps)
-        return _ScatterFunction.apply(dropout_rows(nrm, self._p(enc.dropout)), slot, src), enc_mask
+        return PackedEncoderOutput(dropout_rows(nrm, self._p(enc.dropout)), offsets, key_mask, src, slot, S)
+
+
+class PackedEncoderOutput(NamedTuple):
+    """``FusedT5EncodeTrain.packed``: rows [N, d_model] (history b's kept positions are rows offsets[b] .. offsets[b + 1] - 1, in
+    position order), offsets int32 [B + 1], key_mask fp32 [B] (finfo(float32).min for a history without an unmasked position),
+    src int32 [N] (b * S + position of each row), slot int32 [B, S] (row of each position or -1) and S."""
+    rows: Tensor
+    offsets: Tensor
+    key_mask: Tensor
+    src: Tensor
+    slot: Tensor
+    S: int
+
+
+class _DecoderInputFunction(torch.autograd.Function):
+    """The decoder's input rows x [B * T, d]: row b * T + t is bos for t = 0 and table[ids[b, t - 1] + (t - 1) K] after.  The
+    backward adds each row's gradient to the table row it was read from with ``index_put_`` (accumulate, a sorted and therefore
+    deterministic sum) and sums bos's rows in order."""
+
+    @staticmethod
+    def forward(ctx, table, bos, ids, K, T):
+        B, d = ids.shape[0], table.shape[1]
+        rows = ids[:, :T - 1].long() + torch.arange(T - 1, device=ids.device) * K
+        x = torch.cat([bos.expand(B, 1, d), table.index_select(0, rows.reshape(-1)).view(B, T - 1, d)], dim=1)
+        ctx.save_for_backward(rows)
+        ctx.V, ctx.T = table.shape[0], T
+        return x.reshape(B * T, d)
+
+    @staticmethod
+    def backward(ctx, dx):
+        (rows,) = ctx.saved_tensors
+        dx = dx.view(-1, ctx.T, dx.shape[1])
+        d_table = d_bos = None
+        if ctx.needs_input_grad[0]:
+            d_table = dx.new_zeros((ctx.V, dx.shape[2])).index_put_((rows.reshape(-1),), dx[:, 1:].reshape(-1, dx.shape[2]),
+                                                                    accumulate=True)
+        if ctx.needs_input_grad[1]:
+            d_bos = dx[:, 0].sum(0, keepdim=True)
+        return d_table, d_bos, None, None, None
+
+
+class FusedT5DecodeTrain:
+    """The decoder pass of ``forward(decoder="fused")``: HF's T5Stack decoder (relu FFN, d_kv 64) over the T = H positions the loss
+    reads (causality makes them independent of HF's extra last position), as cuBLAS GEMMs (``F.linear``) between the training
+    kernels of csrc/t5dec.cu.  Autograd runs through
+      * ``_DecoderInputFunction`` (gradient into ``item_sid_embedding_table`` and ``bos_token``, deterministic),
+      * ``ops.T5EncAddNormFunction`` at every norm,
+      * ``ops.T5DecSelfAttentionFunction`` (causal, block 0's unidirectional relative bias from ``_rel_bias``) and
+        ``ops.T5DecCrossAttentionFunction`` over the encoder rows given by ``offsets`` and a per-key additive mask: the packed rows
+        of ``FusedT5EncodeTrain.packed`` or the [B * S] rows of HF's encoder.  Cross keys and values are one GEMM per layer on
+        those rows.  Attention-weight dropout draws one seed per attention site and layer from torch's generator, the bits keyed
+        on the key's ORIGINAL encoder position, so both encoders give the same bits under one seed;
+      * HF's token-wise dropout sites through ``dropout_rows``.
+    ``__call__`` returns the final-normed, dropped-out hidden state [B, T, d_model].  fp32 parameters only; an active autocast
+    region raises ``ValueError``."""
+
+    def __init__(self, model: "EncoderDecoderRetrievalModel"):
+        dec = model.t5_decoder
+        _check_encoder_config(dec.config, "decoder=\"fused\"")
+        if model.num_hierarchies > MAX_TRAIN_DECODER_LEN:
+            raise Rqb200Error(f"forward(decoder=\"fused\"): {model.num_hierarchies} levels exceed {MAX_TRAIN_DECODER_LEN}")
+        if any(t.dtype != torch.float32 for t in model.parameters()):
+            raise Rqb200Error("forward(decoder=\"fused\") needs fp32 parameters")
+        self.model, self.dec, self.eps = model, dec, dec.config.layer_norm_epsilon
+        self.blocks = [blk.layer for blk in dec.block]
+        self.norms = [w for lay in self.blocks for w in (lay[0].layer_norm.weight, lay[1].layer_norm.weight,
+                                                         lay[2].layer_norm.weight)] + [dec.final_layer_norm.weight]
+
+    _p = staticmethod(FusedT5EncodeTrain._p)
+
+    @staticmethod
+    def _seed(att, device):
+        p = float(att.dropout) if att.training else 0.0
+        return p, ops.t5enc_dropout_seed(device) if p > 0 else torch.zeros(1, dtype=torch.int64, device=device)
+
+    def __call__(self, fut_ids: Tensor, rows: Tensor, offsets: Tensor, key_mask: Tensor, src: Optional[Tensor], S: int) -> Tensor:
+        """fut_ids [B, >= T - 1]; rows [*, d_model] the encoder rows, history b's keys rows offsets[b] .. offsets[b + 1] - 1 with
+        additive key_mask [rows]; src [rows] (b * S + position) or None (row - offsets[b] is the position)."""
+        if torch.is_autocast_enabled("cuda"):
+            raise ValueError("forward(decoder=\"fused\") runs fp32 kernels: it cannot run inside an autocast region")
+        m, dec, eps = self.model, self.dec, self.eps
+        T, B = m.num_hierarchies, fut_ids.shape[0]
+        x = _DecoderInputFunction.apply(m.item_sid_embedding_table.weight, m.bos_token, fut_ids, m.num_embeddings_per_hierarchy, T)
+        x, nrm = ops.T5EncAddNormFunction.apply(dropout_rows(x, self._p(dec.dropout)), None, self.norms[0], eps)
+        rel = _rel_bias(self.blocks[0][0].SelfAttention, T)
+        for l, lay in enumerate(self.blocks):
+            att = lay[0].SelfAttention
+            p_att, seed = self._seed(att, x.device)
+            a = ops.T5DecSelfAttentionFunction.apply(F.linear(nrm, torch.cat([att.q.weight, att.k.weight, att.v.weight])), rel, T,
+                                                     seed, p_att)
+            x, nrm = ops.T5EncAddNormFunction.apply(x, dropout_rows(F.linear(a, att.o.weight), self._p(lay[0].dropout)),
+                                                    self.norms[3 * l + 1], eps)
+            ca = lay[1].EncDecAttention
+            p_ca, seed = self._seed(ca, x.device)
+            kv = F.linear(rows, torch.cat([ca.k.weight, ca.v.weight]))
+            a = ops.T5DecCrossAttentionFunction.apply(F.linear(nrm, ca.q.weight), kv, offsets, key_mask, src, S, T, seed, p_ca)
+            x, nrm = ops.T5EncAddNormFunction.apply(x, dropout_rows(F.linear(a, ca.o.weight), self._p(lay[1].dropout)),
+                                                    self.norms[3 * l + 2], eps)
+            ff = lay[2].DenseReluDense
+            h = dropout_rows(F.relu(F.linear(nrm, ff.wi.weight)), self._p(ff.dropout))
+            x, nrm = ops.T5EncAddNormFunction.apply(x, dropout_rows(F.linear(h, ff.wo.weight), self._p(lay[2].dropout)),
+                                                    self.norms[3 * l + 3], eps)
+        return dropout_rows(nrm, self._p(dec.dropout)).view(B, T, -1)
+
+
+#: most decoder positions (hierarchy levels) the decoder's training kernels take
+MAX_TRAIN_DECODER_LEN = 8
 
 
 class EncoderDecoderRetrievalModel(nn.Module):
@@ -499,24 +620,53 @@ class EncoderDecoderRetrievalModel(nn.Module):
         """FusedT5EncodeTrain runs outside torch.compile's graphs (ctypes launches): a graph break, with backward through it."""
         return FusedT5EncodeTrain(self)(attention_mask, input_ids, user_id)
 
-    def forward(self, batch: TokenizedSeqBatch, encoder: Optional[str] = None) -> ModelOutput:
+    @torch.compiler.disable
+    def _fused_train_passes(self, attention_mask, input_ids, user_id, fut_ids):
+        """Both fused passes in one graph break: the decoder attends to the encoder's packed rows (no scatter to [B, S, d])."""
+        enc = FusedT5EncodeTrain(self).packed(attention_mask, input_ids, user_id)
+        key_mask = enc.key_mask.index_select(0, torch.div(enc.src, enc.S, rounding_mode="floor").long())
+        return FusedT5DecodeTrain(self)(fut_ids, enc.rows, enc.offsets, key_mask, enc.src, enc.S)
+
+    @torch.compiler.disable
+    def _fused_train_decoder_pass(self, fut_ids, enc_out, enc_mask):
+        """The fused decoder pass over HF's encoder output: history b's keys are rows b * S .. b * S + S - 1 of [B * S, d_model]."""
+        B, S, d = enc_out.shape
+        key_mask = torch.where(enc_mask == 0, torch.finfo(torch.float32).min, 0.0).to(torch.float32).reshape(B * S)
+        offsets = torch.arange(0, (B + 1) * S, S, dtype=torch.int32, device=enc_out.device)
+        return FusedT5DecodeTrain(self)(fut_ids, enc_out.reshape(B * S, d), offsets, key_mask, None, S)
+
+    def forward(self, batch: TokenizedSeqBatch, encoder: Optional[str] = None, decoder: Optional[str] = None) -> ModelOutput:
         """The training loss.  ``encoder`` (default: the module's ``DEFAULT_FORWARD_ENCODER``, read at call time):
           "hf"      ``encoder_forward_pass``: transformers' T5EncoderModel over every position, as the reference;
           "fused"   ``FusedT5EncodeTrain``: the kept positions only, with HF's dropout in training mode and none in eval mode;
-                    gradients in both.  It reads the packed row count on the host once."""
+                    gradients in both.  It reads the packed row count on the host once.
+        ``decoder`` (default: the module's ``DEFAULT_FORWARD_DECODER``, read at call time):
+          "hf"      ``decoder_forward_pass``: transformers' T5Stack over BOS and the H future ids, as the reference;
+          "fused"   ``FusedT5DecodeTrain``: the H positions the loss reads, with HF's dropout in training mode and none in eval
+                    mode; gradients in both.  With encoder="fused" it attends to the encoder's packed rows directly."""
         encoder = DEFAULT_FORWARD_ENCODER if encoder is None else encoder
+        decoder = DEFAULT_FORWARD_DECODER if decoder is None else decoder
         if encoder not in ENCODERS:
             raise ValueError(f"forward: encoder must be one of {ENCODERS}, got {encoder!r}")
+        if decoder not in DECODERS:
+            raise ValueError(f"forward: decoder must be one of {DECODERS}, got {decoder!r}")
         H = self.num_hierarchies
         input_ids = _strip_dedup_col(batch.sem_ids, H + 1, H)
         attention_mask = _strip_dedup_col(batch.seq_mask.long(), H + 1, H)
         fut_ids = batch.sem_ids_fut[:, :H]
-        if encoder == "fused":
-            enc, enc_mask = self._fused_train_encoder_pass(attention_mask, input_ids, batch.user_ids)
+        if encoder == "fused" and decoder == "fused":
+            dec = self._fused_train_passes(attention_mask, input_ids, batch.user_ids, fut_ids)
         else:
-            enc, enc_mask = self.encoder_forward_pass(attention_mask=attention_mask, input_ids=input_ids, user_id=batch.user_ids)
-        dec = self.decoder_forward_pass(future_ids=fut_ids, encoder_output=enc, attention_mask_for_encoder=enc_mask,
-                                        use_cache=False)[:, :-1]
+            if encoder == "fused":
+                enc, enc_mask = self._fused_train_encoder_pass(attention_mask, input_ids, batch.user_ids)
+            else:
+                enc, enc_mask = self.encoder_forward_pass(attention_mask=attention_mask, input_ids=input_ids,
+                                                          user_id=batch.user_ids)
+            if decoder == "fused":
+                dec = self._fused_train_decoder_pass(fut_ids, enc, enc_mask)
+            else:
+                dec = self.decoder_forward_pass(future_ids=fut_ids, encoder_output=enc, attention_mask_for_encoder=enc_mask,
+                                                use_cache=False)[:, :-1]
         loss = torch.tensor(0.0, device=dec.device)
         per_level = []
         for h in range(H):

@@ -1217,6 +1217,160 @@ class T5EncAddNormFunction(torch.autograd.Function):
         return dx, dx if ctx.has_delta else None, dw, None
 
 
+# ---------------------------------------------------------------------------------------------- training the T5 decoder pass
+def _check_seed(seed: torch.Tensor) -> None:
+    if seed.dtype != torch.int64 or seed.numel() != 1:
+        raise ValueError("seed must be an int64 tensor of one element")
+
+
+def t5dec_self_attention_train(qkv: torch.Tensor, rel: torch.Tensor, T: int, seed: torch.Tensor, p: float):
+    """Causal T5 self-attention of T decoder positions per history with HF's attention-weight dropout
+    (rqb200_t5dec_self_attention_train), one launch.  qkv [B * T, 3 inner] (row b * T + t: position t of history b; q | k | v),
+    rel [heads, 2T - 1] (``t5enc_rel_bias`` layout) -> (out [B * T, inner], lse [B * T, heads])."""
+    _need_cuda(qkv, rel, seed)
+    _check_seed(seed)
+    rel = _f32c(rel)
+    heads = rel.shape[0]
+    if rel.shape != (heads, 2 * T - 1):
+        raise ValueError(f"rel {tuple(rel.shape)} must be [heads, {2 * T - 1}]")
+    qkv = _rows_of(qkv, 3 * heads * T5_DKV, "qkv")
+    if qkv.shape[0] % T:
+        raise ValueError(f"qkv has {qkv.shape[0]} rows, not a multiple of T = {T}")
+    B = qkv.shape[0] // T
+    out = torch.empty((B * T, heads * T5_DKV), dtype=torch.float32, device=qkv.device)
+    lse = torch.empty((B * T, heads), dtype=torch.float32, device=qkv.device)
+    with torch.cuda.device(qkv.device):
+        _lib.check(_lib.load().rqb200_t5dec_self_attention_train(_p(qkv), qkv.stride(0), _p(rel), B, T, heads, _p(seed), _check_p(p),
+                                                                 _p(out), out.stride(0), _p(lse), _stream()),
+                   "t5dec_self_attention_train")
+    _count(1)
+    return out, lse
+
+
+def t5dec_self_attention_backward(qkv: torch.Tensor, out: torch.Tensor, dout: torch.Tensor, lse: torch.Tensor, rel: torch.Tensor,
+                                  T: int, seed: torch.Tensor, p: float):
+    """The backward of ``t5dec_self_attention_train`` (rqb200_t5dec_self_attention_backward), one launch and one fixed-order sum ->
+    (d_qkv [B * T, 3 inner], d_rel [heads, 2T - 1]).  Bit-reproducible."""
+    _need_cuda(qkv, out, dout, lse, rel, seed)
+    _check_seed(seed)
+    rel = _f32c(rel)
+    heads = rel.shape[0]
+    inner = heads * T5_DKV
+    qkv, out, dout, lse = _rows_of(qkv, 3 * inner, "qkv"), _rows_of(out, inner, "out"), _rows_of(dout, inner, "dout"), _f32c(lse)
+    N = qkv.shape[0]
+    if N % T or out.shape[0] != N or dout.shape[0] != N or lse.shape != (N, heads) or rel.shape != (heads, 2 * T - 1):
+        raise ValueError("qkv [B * T, 3 inner], out / dout [B * T, inner], lse [B * T, heads] and rel [heads, 2T - 1] must match")
+    B = N // T
+    dqkv = torch.empty((N, 3 * inner), dtype=torch.float32, device=qkv.device)
+    part = torch.empty((B, heads, 2 * T - 1), dtype=torch.float32, device=qkv.device)
+    with torch.cuda.device(qkv.device):
+        _lib.check(_lib.load().rqb200_t5dec_self_attention_backward(
+            _p(qkv), qkv.stride(0), _p(out), out.stride(0), _p(dout), dout.stride(0), _p(lse), _p(rel), B, T, heads, _p(seed),
+            _check_p(p), _p(dqkv), dqkv.stride(0), _p(part), _stream()), "t5dec_self_attention_backward")
+    _count(1)
+    return dqkv, part.sum(0)
+
+
+def _cross_layout(q, kv, offsets, key_mask, src, T, heads):
+    inner = heads * T5_DKV
+    q, kv = _rows_of(q, inner, "q"), _rows_of(kv, 2 * inner, "kv")
+    if q.shape[0] % T:
+        raise ValueError(f"q has {q.shape[0]} rows, not a multiple of T = {T}")
+    B = q.shape[0] // T
+    if offsets.dtype != torch.int32 or offsets.shape != (B + 1,):
+        raise ValueError(f"offsets must be int32 [{B + 1}]")
+    key_mask = _f32c(key_mask)
+    if key_mask.shape != (kv.shape[0],):
+        raise ValueError(f"key_mask {tuple(key_mask.shape)} must hold one value per key row ({kv.shape[0]})")
+    if src is not None and (src.dtype != torch.int32 or src.shape != (kv.shape[0],) or not src.is_contiguous()):
+        raise ValueError(f"src must be a contiguous int32 [{kv.shape[0]}] tensor")
+    return q, kv, key_mask, B
+
+
+def t5dec_cross_attention_train(q: torch.Tensor, kv: torch.Tensor, offsets: torch.Tensor, key_mask: torch.Tensor,
+                                src: Optional[torch.Tensor], S: int, T: int, seed: torch.Tensor, p: float):
+    """T5 cross-attention of T decoder positions per history over its encoder rows, with HF's attention-weight dropout
+    (rqb200_t5dec_cross_attention_train), one launch.  q [B * T, inner]; kv [rows, 2 inner] (k | v); history b's keys are rows
+    offsets[b] .. offsets[b + 1] - 1 (int32 [B + 1]) with additive key_mask [rows] (0 or finfo(float32).min); a key's position in
+    the dropout bits is src[row] - b * S (packed encoder rows) or row - offsets[b] (src None: [B * S] rows).
+    -> (out [B * T, inner], lse [B * T, heads])."""
+    _need_cuda(q, kv, offsets, key_mask, src, seed)
+    _check_seed(seed)
+    heads = q.shape[1] // T5_DKV
+    q, kv, key_mask, B = _cross_layout(q, kv, offsets, key_mask, src, T, heads)
+    inner = heads * T5_DKV
+    out = torch.empty((B * T, inner), dtype=torch.float32, device=q.device)
+    lse = torch.empty((B * T, heads), dtype=torch.float32, device=q.device)
+    with torch.cuda.device(q.device):
+        _lib.check(_lib.load().rqb200_t5dec_cross_attention_train(
+            _p(q), q.stride(0), _p(kv), kv.data_ptr() + 4 * inner, kv.stride(0), _p(offsets), _p(key_mask), _p(src), B, int(S), T,
+            heads, _p(seed), _check_p(p), _p(out), out.stride(0), _p(lse), _stream()), "t5dec_cross_attention_train")
+    _count(1)
+    return out, lse
+
+
+def t5dec_cross_attention_backward(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, dout: torch.Tensor, lse: torch.Tensor,
+                                   offsets: torch.Tensor, key_mask: torch.Tensor, src: Optional[torch.Tensor], S: int, T: int,
+                                   seed: torch.Tensor, p: float):
+    """The backward of ``t5dec_cross_attention_train`` (rqb200_t5dec_cross_attention_backward), one launch -> (d_q [B * T, inner],
+    d_kv [rows, 2 inner], zero in rows no history owns).  Bit-reproducible."""
+    _need_cuda(q, kv, out, dout, lse, offsets, key_mask, src, seed)
+    _check_seed(seed)
+    heads = q.shape[1] // T5_DKV
+    q, kv, key_mask, B = _cross_layout(q, kv, offsets, key_mask, src, T, heads)
+    inner = heads * T5_DKV
+    out, dout, lse = _rows_of(out, inner, "out"), _rows_of(dout, inner, "dout"), _f32c(lse)
+    if out.shape[0] != B * T or dout.shape[0] != B * T or lse.shape != (B * T, heads):
+        raise ValueError("out / dout [B * T, inner] and lse [B * T, heads] must match q")
+    dq = torch.empty_like(out)
+    dkv = torch.zeros((kv.shape[0], 2 * inner), dtype=torch.float32, device=q.device)
+    with torch.cuda.device(q.device):
+        _lib.check(_lib.load().rqb200_t5dec_cross_attention_backward(
+            _p(q), q.stride(0), _p(kv), kv.data_ptr() + 4 * inner, kv.stride(0), _p(out), out.stride(0), _p(dout), dout.stride(0),
+            _p(lse), _p(offsets), _p(key_mask), _p(src), B, int(S), T, heads, _p(seed), _check_p(p), _p(dq), dq.stride(0), _p(dkv),
+            dkv.data_ptr() + 4 * inner, dkv.stride(0), _stream()), "t5dec_cross_attention_backward")
+    _count(1)
+    return dq, dkv
+
+
+class T5DecSelfAttentionFunction(torch.autograd.Function):
+    """Autograd of the decoder's training self-attention: ``apply(qkv, rel, T, seed, p)`` -> out [B * T, inner]; gradients for
+    qkv and rel."""
+
+    @staticmethod
+    def forward(ctx, qkv, rel, T, seed, p):
+        qkv = qkv.contiguous()
+        out, lse = t5dec_self_attention_train(qkv, rel, T, seed, p)
+        ctx.save_for_backward(qkv, rel, seed, out, lse)
+        ctx.T, ctx.p = T, p
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        qkv, rel, seed, out, lse = ctx.saved_tensors
+        dqkv, drel = t5dec_self_attention_backward(qkv, out, dout, lse, rel, ctx.T, seed, ctx.p)
+        return dqkv, drel, None, None, None
+
+
+class T5DecCrossAttentionFunction(torch.autograd.Function):
+    """Autograd of the decoder's training cross-attention: ``apply(q, kv, offsets, key_mask, src, S, T, seed, p)`` -> out
+    [B * T, inner]; gradients for q and kv."""
+
+    @staticmethod
+    def forward(ctx, q, kv, offsets, key_mask, src, S, T, seed, p):
+        q, kv = q.contiguous(), kv.contiguous()
+        out, lse = t5dec_cross_attention_train(q, kv, offsets, key_mask, src, S, T, seed, p)
+        ctx.save_for_backward(q, kv, offsets, key_mask, src, seed, out, lse)
+        ctx.S, ctx.T, ctx.p = S, T, p
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        q, kv, offsets, key_mask, src, seed, out, lse = ctx.saved_tensors
+        dq, dkv = t5dec_cross_attention_backward(q, kv, out, dout, lse, offsets, key_mask, src, ctx.S, ctx.T, seed, ctx.p)
+        return dq, dkv, None, None, None, None, None, None, None
+
+
 # ---------------------------------------------------------------------------------------------- tensor-core tokeniser
 def tc_supported(D: int, K: int, L: int) -> bool:
     return bool(_lib.load().rqb200_tokenize_tc_supported(D, K, L))
