@@ -60,9 +60,9 @@ def step_fn(m, opt, batch, encoder, decoder):
     return step
 
 
-def step_split(torch, M, m, opt, batch, encoder, decoder, reps=10):
+def step_split(torch, M, m, opt, batch, encoder, decoder, reps=10, attention="fp32"):
     """Mean ms of the step's encoder forward, decoder + heads forward, decoder + heads backward, encoder backward and optimizer,
-    over reps steps with CUDA events."""
+    over reps steps with CUDA events; ``attention`` is the fused encoder's attention precision."""
     Hh = m.num_hierarchies
     names = ("encoder_forward_ms", "decoder_forward_ms", "decoder_backward_ms", "encoder_backward_ms", "optimizer_ms")
     tot = [0.0] * len(names)
@@ -73,10 +73,10 @@ def step_split(torch, M, m, opt, batch, encoder, decoder, reps=10):
         ids = M._strip_dedup_col(batch.sem_ids, Hh + 1, Hh)
         fut = batch.sem_ids_fut[:, :Hh]
         if encoder == "fused" and decoder == "fused":
-            packed = M.FusedT5EncodeTrain(m).packed(mask, ids, batch.user_ids)
+            packed = M.FusedT5EncodeTrain(m, attention).packed(mask, ids, batch.user_ids)
             out = packed.rows
         elif encoder == "fused":
-            out, enc_mask = m._fused_train_encoder_pass(mask, ids, batch.user_ids)
+            out, enc_mask = m._fused_train_encoder_pass(mask, ids, batch.user_ids, attention)
         else:
             out, enc_mask = m.encoder_forward_pass(attention_mask=mask, input_ids=ids, user_id=batch.user_ids)
         ev[1].record()

@@ -371,6 +371,22 @@ int rqb200_t5enc_add_norm_bwd_parts(int R);
 int rqb200_t5enc_add_norm_bwd(const float* d_out, const float* d_res, const float* x_out, const float* inv_rms, const float* weight,
                               int R, int D, float* dx, float* dw_part, void* stream);
 
+/* ---- TF32 tensor-core encoder self-attention (encoder_attention="tf32"), csrc/t5enc_tc.cu ----
+ * The entry points above with the same arguments, layouts, dropout bits and outputs, whose products (scores, P.V, dP and the
+ * gradient products) run as wgmma TF32 with fp32 accumulation, operands rounded to TF32.  Softmax, bias, mask and dropout are fp32.
+ * t5enc_attention_tc_backward's drel_part is [B, t5enc_attention_tc_backward_tiles(S), heads, 2S - 1]; two launches, no atomics,
+ * bit-reproducible; S <= 8336 (two shared-memory bin arrays of 2S - 1 floats). */
+int rqb200_t5enc_attention_tc(const float* qkv, int64_t ldqkv, const int* src, const int* offsets, const float* key_mask,
+                              const float* rel, int B, int S, int heads, float* out, int64_t ldo, void* stream);
+int rqb200_t5enc_attention_tc_train(const float* qkv, int64_t ldqkv, const int* src, const int* offsets, const float* key_mask,
+                                    const float* rel, int B, int S, int heads, const int64_t* seed, float p, float* out, int64_t ldo,
+                                    float* lse, void* stream);
+int rqb200_t5enc_attention_tc_backward_tiles(int S);
+int rqb200_t5enc_attention_tc_backward(const float* qkv, int64_t ldqkv, const float* out, int64_t ldo, const float* dout,
+                                       int64_t lddo, const float* lse, const int* src, const int* offsets, const float* key_mask,
+                                       const float* rel, int B, int S, int heads, const int64_t* seed, float p, float* delta,
+                                       float* dqkv, int64_t ldd, float* drel_part, void* stream);
+
 /* ---- training the decoder pass (modules/model.py, forward(decoder="fused")), csrc/t5dec.cu ----
  * T (<= 8, else RQB_ERR_UNSUPPORTED) decoder positions per history: row b * T + t of q / qkv / out / dout holds position t of
  * history b; inner = heads * 64, fp32, strides in elements, no 1/sqrt(d) scaling.  Attention-weight dropout as the encoder's:

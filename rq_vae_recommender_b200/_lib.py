@@ -14,7 +14,7 @@ from typing import Optional
 PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "librqb200.so")
-SOURCES = ["api.cu", "rq_simt.cu", "dense.cu", "rq_tc.cu", "rq_tcx.cu", "gemm_tc.cu", "sid.cu", "t5dec.cu", "t5enc.cu"]
+SOURCES = ["api.cu", "rq_simt.cu", "dense.cu", "rq_tc.cu", "rq_tcx.cu", "gemm_tc.cu", "sid.cu", "t5dec.cu", "t5enc.cu", "t5enc_tc.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-shared", "-Xcompiler", "-fPIC"]
 
@@ -94,7 +94,13 @@ _SIGNATURES = {
     "rqb200_t5enc_attention_backward_tiles": (c_int, [c_int]),
     "rqb200_t5enc_attention_backward": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int,
                                                 c_int, c_vp, c_f32, c_vp, c_vp, c_i64, c_vp, c_vp]),
-    "rqb200_t5enc_dropout_keep": (c_int, [c_vp, c_f32, c_int, c_int, c_int, c_vp, c_vp]),
+    "rqb200_t5enc_attention_tc": (c_int, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_i64, c_vp]),
+    "rqb200_t5enc_attention_tc_train": (c_int, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_f32, c_vp, c_i64,
+                                                c_vp, c_vp]),
+    "rqb200_t5enc_attention_tc_backward_tiles": (c_int, [c_int]),
+    "rqb200_t5enc_attention_tc_backward": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_int,
+                                                   c_int, c_int, c_vp, c_f32, c_vp, c_vp, c_i64, c_vp, c_vp]),
+    "rqb200_t5enc_dropout_keep":(c_int, [c_vp, c_f32, c_int, c_int, c_int, c_vp, c_vp]),
     "rqb200_t5enc_add_norm_fwd": (c_int, [c_vp, c_vp, c_i64, c_vp, c_int, c_int, c_f32, c_vp, c_vp, c_vp, c_vp]),
     "rqb200_t5enc_add_norm_bwd_parts": (c_int, [c_int]),
     "rqb200_t5enc_add_norm_bwd": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp]),

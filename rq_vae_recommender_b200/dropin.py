@@ -14,7 +14,8 @@ an unmodified ``train_decoder.py`` evaluates with it; ``decoder="fused"`` (with 
 decoder passes run on the fused decoder-step kernels (``FusedT5Decode``), and ``encoder="fused"`` its encoder pass over the
 unpadded positions only (``FusedT5Encode``); ``forward_encoder="fused"`` makes the training pass ``forward`` run its encoder on
 the trainable packed pass (``FusedT5EncodeTrain``), and ``forward_decoder="fused"`` its decoder on the fused training
-decoder (``FusedT5DecodeTrain``).  ``replace_metrics=True`` also aliases ``evaluate.metrics``
+decoder (``FusedT5DecodeTrain``).  ``encoder_attention="tf32"`` makes the fused encoder passes (of ``generate`` and
+``forward``) run their self-attention on the TF32 tensor-core kernels.  ``replace_metrics=True`` also aliases ``evaluate.metrics``
 (train_decoder.py:13), whose ``TopKAccumulator`` accumulates on the device without waiting on the host.  Checkpoints pickle ``modules.quantize.Quantize`` etc. by module path,
 so ``torch.load(..., weights_only=False)`` of the shipped files also lands on the replacement classes.
 gin-config is not in this image: a small compatible shim is registered as ``gin`` when the real one is missing.
@@ -38,7 +39,8 @@ _METRICS = ("evaluate.metrics", "rq_vae_recommender_b200.evaluate.metrics")
 
 
 def install(reference_root=None, replace_tokenizer=True, gin_shim=True, replace_model=False, search="sample",
-            replace_metrics=False, decoder="hf", encoder="hf", forward_encoder="hf", forward_decoder="hf"):
+            replace_metrics=False, decoder="hf", encoder="hf", forward_encoder="hf", forward_decoder="hf",
+            encoder_attention="fp32"):
     if search not in ("sample", "beam"):
         raise ValueError(f"search must be 'sample' or 'beam', got {search!r}")
     if search != "sample" and not replace_model:
@@ -61,6 +63,11 @@ def install(reference_root=None, replace_tokenizer=True, gin_shim=True, replace_
     if forward_decoder != "hf" and not replace_model:
         raise ValueError(f"forward_decoder={forward_decoder!r} selects the replacement model's training decoder pass: it needs "
                          "replace_model=True")
+    if encoder_attention not in ("fp32", "tf32"):
+        raise ValueError(f"encoder_attention must be 'fp32' or 'tf32', got {encoder_attention!r}")
+    if encoder_attention != "fp32" and not replace_model:
+        raise ValueError(f"encoder_attention={encoder_attention!r} selects the replacement model's fused encoder attention: it "
+                         "needs replace_model=True")
     if gin_shim and "gin" not in sys.modules:
         try:
             import gin  # noqa: F401
@@ -85,6 +92,7 @@ def install(reference_root=None, replace_tokenizer=True, gin_shim=True, replace_
         sys.modules[_MODEL[0]].DEFAULT_ENCODER = encoder
         sys.modules[_MODEL[0]].DEFAULT_FORWARD_ENCODER = forward_encoder
         sys.modules[_MODEL[0]].DEFAULT_FORWARD_DECODER = forward_decoder
+        sys.modules[_MODEL[0]].DEFAULT_ENCODER_ATTENTION = encoder_attention
     if replace_metrics:
         sys.modules[_METRICS[0]] = importlib.import_module(_METRICS[1])
     return sorted(list(_ALIASES) + ([_TOKENIZER[0]] if replace_tokenizer else []) + ([_MODEL[0]] if replace_model else [])
@@ -103,3 +111,4 @@ def uninstall():
         model.DEFAULT_ENCODER = "hf"
         model.DEFAULT_FORWARD_ENCODER = "hf"
         model.DEFAULT_FORWARD_DECODER = "hf"
+        model.DEFAULT_ENCODER_ATTENTION = "fp32"

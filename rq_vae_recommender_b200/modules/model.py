@@ -76,6 +76,11 @@ DEFAULT_FORWARD_ENCODER = "hf"
 #: the decoder pass forward() runs when it is not given a decoder: "hf" (transformers' T5Stack) or "fused" (FusedT5DecodeTrain:
 #: the H positions the loss reads, with the training kernels of csrc/t5dec.cu and HF's dropout)
 DEFAULT_FORWARD_DECODER = "hf"
+#: the precision of the fused encoder's self-attention when a call gives none (read at call time): "fp32" (csrc/t5enc.cu, fp32 on
+#: the CUDA cores) or "tf32" (csrc/t5enc_tc.cu: scores, P.V and the gradient products on TF32 tensor cores, softmax in fp32).  It
+#: applies to encoder="fused" passes only; HF's encoder follows torch's matmul precision.
+DEFAULT_ENCODER_ATTENTION = "fp32"
+ENCODER_ATTENTIONS = ("fp32", "tf32")
 _MULTINOMIAL_ERRORS = ("probability tensor contains either `inf`, `nan` or element < 0",
                        "invalid multinomial distribution (sum of probabilities <= 0)")
 
@@ -183,6 +188,24 @@ class FusedT5Decode:
         return nrm
 
 
+def _encoder_attention(encoder: str, encoder_attention: Optional[str], what: str) -> str:
+    """The fused encoder's attention precision of one call: ``encoder_attention``, else ``DEFAULT_ENCODER_ATTENTION``.  An explicit
+    "tf32" with encoder="hf" raises: HF's attention runs at torch's matmul precision, and the switch would be ignored."""
+    att = DEFAULT_ENCODER_ATTENTION if encoder_attention is None else encoder_attention
+    if att not in ENCODER_ATTENTIONS:
+        raise ValueError(f"{what}: encoder_attention must be one of {ENCODER_ATTENTIONS}, got {att!r}")
+    if encoder_attention == "tf32" and encoder != "fused":
+        raise ValueError(f"{what}: encoder_attention=\"tf32\" selects the fused encoder's attention kernels; with "
+                         f"encoder={encoder!r} the attention follows torch.get_float32_matmul_precision()")
+    return att
+
+
+def _check_attention(attention: str) -> str:
+    if attention not in ENCODER_ATTENTIONS:
+        raise ValueError(f"encoder attention must be one of {ENCODER_ATTENTIONS}, got {attention!r}")
+    return attention
+
+
 def _read_n_kept(offsets: Tensor) -> int:
     """The packed row count offsets[B], read on the host to size the encoder's GEMMs: the one host synchronisation of an
     encoder="fused" pass."""
@@ -200,15 +223,17 @@ class FusedT5Encode:
         relative-position bias at each row's ORIGINAL position (``compute_bias(S, S)`` of block 0, once per call);
       * ``__call__`` returns what ``encoder_forward_pass`` returns: enc_out [B, S, d_model] with the rows of dropped positions
         set to 0, and enc_mask [B, S] with the same values.
-    N is read on the host once per call (``_read_n_kept``) to size the GEMMs; it is the pass's only host synchronisation."""
+    N is read on the host once per call (``_read_n_kept``) to size the GEMMs; it is the pass's only host synchronisation.
+    ``attention`` picks the self-attention kernel: "fp32" (``ops.t5enc_attention``) or "tf32" (``ops.t5enc_attention_tc``)."""
 
-    def __init__(self, model: "EncoderDecoderRetrievalModel"):
+    def __init__(self, model: "EncoderDecoderRetrievalModel", attention: str = "fp32"):
         enc = model.encoder.encoder
         cfg = enc.config
         if cfg.d_kv != ops.T5_DKV or cfg.is_gated_act or cfg.dense_act_fn != "relu":
             raise Rqb200Error(f"encoder=\"fused\" needs d_kv = {ops.T5_DKV} and a relu feed-forward (d_kv = {cfg.d_kv}, "
                               f"feed_forward_proj = {cfg.feed_forward_proj!r})")
         self.model, self.eps = model, cfg.layer_norm_epsilon
+        self.attention = ops.t5enc_attention_tc if _check_attention(attention) == "tf32" else ops.t5enc_attention
         self.blocks = [blk.layer for blk in enc.block]
         self.w_qkv = [torch.cat([lay[0].SelfAttention.q.weight, lay[0].SelfAttention.k.weight, lay[0].SelfAttention.v.weight])
                       for lay in self.blocks]
@@ -237,7 +262,7 @@ class FusedT5Encode:
         S = slot.shape[1]
         rel = ops.t5enc_rel_bias(self.blocks[0][0].SelfAttention.compute_bias(S, S)[0])
         for l, lay in enumerate(self.blocks):
-            a = ops.t5enc_attention(F.linear(nrm, self.w_qkv[l]), self.src, self.offsets, key_mask, rel, S)
+            a = self.attention(F.linear(nrm, self.w_qkv[l]), self.src, self.offsets, key_mask, rel, S)
             ops.t5dec_add_norm(x, F.linear(a, lay[0].SelfAttention.o.weight), self.norms[2 * l + 1], nrm, eps)
             ff = lay[1].DenseReluDense
             ops.t5dec_add_norm(x, F.linear(F.linear(nrm, ff.wi.weight).relu_(), ff.wo.weight), self.norms[2 * l + 2], nrm, eps)
@@ -353,14 +378,17 @@ class FusedT5EncodeTrain:
     ``relative_attention_bias`` at the buckets of distances -(S - 1) .. S - 1), so its gradient reaches that table summed over the
     layers, as in HF, through a deterministic sum.  Dropout follows HF: embedding, attention weights, attention output, feed-forward inner and
     output, final output, each with its module's probability read at call time when that module is in training mode (0 else).
-    The token-wise sites call ``dropout_rows``.  fp32 parameters only; an active autocast region raises ``ValueError``."""
+    The token-wise sites call ``dropout_rows``.  fp32 parameters only; an active autocast region raises ``ValueError``.
+    ``attention`` picks the attention kernels: "fp32" (``ops.T5EncAttentionFunction``) or "tf32"
+    (``ops.T5EncAttentionTCFunction``, the same keep bits under the same seed)."""
 
-    def __init__(self, model: "EncoderDecoderRetrievalModel"):
+    def __init__(self, model: "EncoderDecoderRetrievalModel", attention: str = "fp32"):
         enc = model.encoder.encoder
         _check_encoder_config(enc.config, "encoder=\"fused\"")
         if any(t.dtype != torch.float32 for t in model.parameters()):
             raise Rqb200Error("forward(encoder=\"fused\") needs fp32 parameters")
         self.model, self.enc, self.eps = model, enc, enc.config.layer_norm_epsilon
+        self.attention = ops.T5EncAttentionTCFunction if _check_attention(attention) == "tf32" else ops.T5EncAttentionFunction
         self.blocks = [blk.layer for blk in enc.block]
         self.norms = [w for lay in self.blocks for w in (lay[0].layer_norm.weight, lay[1].layer_norm.weight)] + \
             [enc.final_layer_norm.weight]
@@ -408,7 +436,7 @@ class FusedT5EncodeTrain:
             p_att = float(att.dropout) if att.training else 0.0
             seed = ops.t5enc_dropout_seed(x.device) if p_att > 0 else torch.zeros(1, dtype=torch.int64, device=x.device)
             qkv = F.linear(nrm, torch.cat([att.q.weight, att.k.weight, att.v.weight]))
-            a = ops.T5EncAttentionFunction.apply(qkv, rel, src, offsets, key_mask, S, seed, p_att)
+            a = self.attention.apply(qkv, rel, src, offsets, key_mask, S, seed, p_att)
             x, nrm = ops.T5EncAddNormFunction.apply(x, dropout_rows(F.linear(a, att.o.weight), self._p(lay[0].dropout)),
                                                     self.norms[2 * l + 1], eps)
             ff = lay[1].DenseReluDense
@@ -616,14 +644,14 @@ class EncoderDecoderRetrievalModel(nn.Module):
         return out.last_hidden_state
 
     @torch.compiler.disable
-    def _fused_train_encoder_pass(self, attention_mask, input_ids, user_id):
+    def _fused_train_encoder_pass(self, attention_mask, input_ids, user_id, attention="fp32"):
         """FusedT5EncodeTrain runs outside torch.compile's graphs (ctypes launches): a graph break, with backward through it."""
-        return FusedT5EncodeTrain(self)(attention_mask, input_ids, user_id)
+        return FusedT5EncodeTrain(self, attention)(attention_mask, input_ids, user_id)
 
     @torch.compiler.disable
-    def _fused_train_passes(self, attention_mask, input_ids, user_id, fut_ids):
+    def _fused_train_passes(self, attention_mask, input_ids, user_id, fut_ids, attention="fp32"):
         """Both fused passes in one graph break: the decoder attends to the encoder's packed rows (no scatter to [B, S, d])."""
-        enc = FusedT5EncodeTrain(self).packed(attention_mask, input_ids, user_id)
+        enc = FusedT5EncodeTrain(self, attention).packed(attention_mask, input_ids, user_id)
         key_mask = enc.key_mask.index_select(0, torch.div(enc.src, enc.S, rounding_mode="floor").long())
         return FusedT5DecodeTrain(self)(fut_ids, enc.rows, enc.offsets, key_mask, enc.src, enc.S)
 
@@ -635,7 +663,8 @@ class EncoderDecoderRetrievalModel(nn.Module):
         offsets = torch.arange(0, (B + 1) * S, S, dtype=torch.int32, device=enc_out.device)
         return FusedT5DecodeTrain(self)(fut_ids, enc_out.reshape(B * S, d), offsets, key_mask, None, S)
 
-    def forward(self, batch: TokenizedSeqBatch, encoder: Optional[str] = None, decoder: Optional[str] = None) -> ModelOutput:
+    def forward(self, batch: TokenizedSeqBatch, encoder: Optional[str] = None, decoder: Optional[str] = None,
+                encoder_attention: Optional[str] = None) -> ModelOutput:
         """The training loss.  ``encoder`` (default: the module's ``DEFAULT_FORWARD_ENCODER``, read at call time):
           "hf"      ``encoder_forward_pass``: transformers' T5EncoderModel over every position, as the reference;
           "fused"   ``FusedT5EncodeTrain``: the kept positions only, with HF's dropout in training mode and none in eval mode;
@@ -643,22 +672,25 @@ class EncoderDecoderRetrievalModel(nn.Module):
         ``decoder`` (default: the module's ``DEFAULT_FORWARD_DECODER``, read at call time):
           "hf"      ``decoder_forward_pass``: transformers' T5Stack over BOS and the H future ids, as the reference;
           "fused"   ``FusedT5DecodeTrain``: the H positions the loss reads, with HF's dropout in training mode and none in eval
-                    mode; gradients in both.  With encoder="fused" it attends to the encoder's packed rows directly."""
+                    mode; gradients in both.  With encoder="fused" it attends to the encoder's packed rows directly.
+        ``encoder_attention`` (default: the module's ``DEFAULT_ENCODER_ATTENTION``, read at call time) picks the fused encoder's
+        attention kernels: "fp32" or "tf32" (TF32 tensor-core products, the same dropout bits).  "tf32" needs encoder="fused"."""
         encoder = DEFAULT_FORWARD_ENCODER if encoder is None else encoder
         decoder = DEFAULT_FORWARD_DECODER if decoder is None else decoder
         if encoder not in ENCODERS:
             raise ValueError(f"forward: encoder must be one of {ENCODERS}, got {encoder!r}")
         if decoder not in DECODERS:
             raise ValueError(f"forward: decoder must be one of {DECODERS}, got {decoder!r}")
+        att = _encoder_attention(encoder, encoder_attention, "forward")
         H = self.num_hierarchies
         input_ids = _strip_dedup_col(batch.sem_ids, H + 1, H)
         attention_mask = _strip_dedup_col(batch.seq_mask.long(), H + 1, H)
         fut_ids = batch.sem_ids_fut[:, :H]
         if encoder == "fused" and decoder == "fused":
-            dec = self._fused_train_passes(attention_mask, input_ids, batch.user_ids, fut_ids)
+            dec = self._fused_train_passes(attention_mask, input_ids, batch.user_ids, fut_ids, att)
         else:
             if encoder == "fused":
-                enc, enc_mask = self._fused_train_encoder_pass(attention_mask, input_ids, batch.user_ids)
+                enc, enc_mask = self._fused_train_encoder_pass(attention_mask, input_ids, batch.user_ids, att)
             else:
                 enc, enc_mask = self.encoder_forward_pass(attention_mask=attention_mask, input_ids=input_ids,
                                                           user_id=batch.user_ids)
@@ -720,12 +752,12 @@ class EncoderDecoderRetrievalModel(nn.Module):
     def _fused_decoder(self, enc_out: Tensor, enc_mask: Tensor, k: int) -> FusedT5Decode:
         return FusedT5Decode(self, enc_out, enc_mask, k)
 
-    def _fused_encoder(self) -> FusedT5Encode:
-        return FusedT5Encode(self)
+    def _fused_encoder(self, attention: str = "fp32") -> FusedT5Encode:
+        return FusedT5Encode(self, attention)
 
     @torch.no_grad()
     def generate(self, attention_mask, input_ids, user_id=None, search: Optional[str] = None, decoder: Optional[str] = None,
-                 encoder: Optional[str] = None):
+                 encoder: Optional[str] = None, encoder_attention: Optional[str] = None):
         """Top-k semantic ids by beam search restricted to id prefixes of the corpus.  ``search`` (default: the module's
         ``DEFAULT_SEARCH``, read at call time):
           "sample"  per level, n_cands = min(64, K) tokens sampled without replacement per beam, scored by cumulative
@@ -740,6 +772,8 @@ class EncoderDecoderRetrievalModel(nn.Module):
           "hf"      ``encoder_forward_pass``: transformers' T5EncoderModel over every position, padded ones included;
           "fused"   ``FusedT5Encode``: the same encoder output at every unpadded position (padded rows are 0) from the unpadded
                     positions only; eval mode only.  It reads the packed row count on the host once, before the first level.
+        ``encoder_attention`` (default: the module's ``DEFAULT_ENCODER_ATTENTION``, read at call time) picks the fused encoder's
+        attention kernel: "fp32" or "tf32" (TF32 tensor-core products).  "tf32" needs encoder="fused".
         Returns generated [B, top_k, num_hierarchies] and log_probas [B, top_k]."""
         search = DEFAULT_SEARCH if search is None else search
         decoder = DEFAULT_DECODER if decoder is None else decoder
@@ -751,6 +785,7 @@ class EncoderDecoderRetrievalModel(nn.Module):
                              "training mode HF's decoder applies dropout)")
         if encoder not in ENCODERS:
             raise ValueError(f"generate: encoder must be one of {ENCODERS}, got {encoder!r}")
+        att = _encoder_attention(encoder, encoder_attention, "generate")
         if encoder == "fused" and self.training:
             raise ValueError("generate: encoder=\"fused\" runs the encoder in eval mode only; call model.eval() first (in "
                              "training mode HF's encoder applies dropout)")
@@ -759,7 +794,8 @@ class EncoderDecoderRetrievalModel(nn.Module):
         self._check_search_limits(search, k, n_cands)
         beam = search == "beam"
         if encoder == "fused":
-            enc_out, enc_mask = self._fused_encoder()(attention_mask, input_ids, user_id)
+            fused_encoder = self._fused_encoder() if att == "fp32" else self._fused_encoder(att)
+            enc_out, enc_mask = fused_encoder(attention_mask, input_ids, user_id)
         else:
             enc_out, enc_mask = self.encoder_forward_pass(attention_mask=attention_mask, input_ids=input_ids, user_id=user_id)
         index = self._prefix_index(enc_out.device)
@@ -805,20 +841,23 @@ class EncoderDecoderRetrievalModel(nn.Module):
     @torch.no_grad()
     def generate_next_sem_id(self, batch: TokenizedSeqBatch, top_k: bool = True, temperature: int = 1,
                              search: Optional[str] = None, decoder: Optional[str] = None,
-                             encoder: Optional[str] = None) -> GenerationOutput:
+                             encoder: Optional[str] = None, encoder_attention: Optional[str] = None) -> GenerationOutput:
         H = self.num_hierarchies
         generated, log_probas = self.generate(attention_mask=_strip_dedup_col(batch.seq_mask.long(), H + 1, H),
                                               input_ids=_strip_dedup_col(batch.sem_ids, H + 1, H), user_id=batch.user_ids,
-                                              search=search, decoder=decoder, encoder=encoder)
+                                              search=search, decoder=decoder, encoder=encoder,
+                                              encoder_attention=encoder_attention)
         return GenerationOutput(sem_ids=generated, log_probas=log_probas)
 
     @torch.no_grad()
     def generate_items(self, batch: TokenizedSeqBatch, n: Optional[int] = None, search: Optional[str] = None,
-                       decoder: Optional[str] = None, encoder: Optional[str] = None) -> ItemGenerationOutput:
+                       decoder: Optional[str] = None, encoder: Optional[str] = None,
+                       encoder_attention: Optional[str] = None) -> ItemGenerationOutput:
         """The top corpus items for each history: ``generate_next_sem_id``'s beams, unchanged, then one launch that takes the
         items of every finite beam whose ids are in the corpus, beam by beam in descending score order, each beam's items by
         dedup rank, no item twice, at most n (default top_k_for_generation) per history."""
-        out = self.generate_next_sem_id(batch, search=search, decoder=decoder, encoder=encoder)
+        out = self.generate_next_sem_id(batch, search=search, decoder=decoder, encoder=encoder,
+                                        encoder_attention=encoder_attention)
         table = self._item_table(out.sem_ids.device)
         items, beams, count = table.retrieve(out.sem_ids, out.log_probas, self.top_k_for_generation if n is None else n)
         return ItemGenerationOutput(item_ids=items, beams=beams, count=count, sem_ids=out.sem_ids, log_probas=out.log_probas)

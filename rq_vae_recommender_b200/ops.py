@@ -1015,6 +1015,16 @@ def t5enc_attention(qkv: torch.Tensor, src: torch.Tensor, offsets: torch.Tensor,
     """Bidirectional T5 self-attention among each history's packed rows (rqb200_t5enc_attention), one launch.  qkv [N, 3 inner]
     (q | k | v), src / offsets / key_mask as ``t5enc_assemble`` / ``t5enc_offsets`` give them, rel [heads, 2S - 1] from
     ``t5enc_rel_bias`` -> [N, inner]."""
+    return _t5enc_attention_eval("t5enc_attention", qkv, src, offsets, key_mask, rel, S)
+
+
+def t5enc_attention_tc(qkv: torch.Tensor, src: torch.Tensor, offsets: torch.Tensor, key_mask: torch.Tensor, rel: torch.Tensor,
+                       S: int) -> torch.Tensor:
+    """``t5enc_attention`` with its products on TF32 tensor cores (rqb200_t5enc_attention_tc, csrc/t5enc_tc.cu), one launch."""
+    return _t5enc_attention_eval("t5enc_attention_tc", qkv, src, offsets, key_mask, rel, S)
+
+
+def _t5enc_attention_eval(name, qkv, src, offsets, key_mask, rel, S):
     _need_cuda(qkv, src, offsets, key_mask, rel)
     rel = _f32c(rel)
     heads = rel.shape[0]
@@ -1030,8 +1040,8 @@ def t5enc_attention(qkv: torch.Tensor, src: torch.Tensor, offsets: torch.Tensor,
     key_mask = _f32c(key_mask)
     out = torch.empty((qkv.shape[0], inner), dtype=torch.float32, device=qkv.device)
     with torch.cuda.device(qkv.device):
-        _lib.check(_lib.load().rqb200_t5enc_attention(_p(qkv), qkv.stride(0), _p(src), _p(offsets), _p(key_mask), _p(rel), B, S,
-                                                      heads, _p(out), out.stride(0), _stream()), "t5enc_attention")
+        _lib.check(getattr(_lib.load(), "rqb200_" + name)(_p(qkv), qkv.stride(0), _p(src), _p(offsets), _p(key_mask), _p(rel), B,
+                                                         S, heads, _p(out), out.stride(0), _stream()), name)
     _count(1)
     return out
 
@@ -1082,6 +1092,17 @@ def t5enc_attention_train(qkv: torch.Tensor, src: torch.Tensor, offsets: torch.T
                           S: int, seed: torch.Tensor, p: float):
     """``t5enc_attention`` with HF's attention-weight dropout (probability p, keep bits from ``seed``) that also returns the
     log-sum-exp the backward needs (rqb200_t5enc_attention_train), one launch -> (out [N, inner], lse [N, heads])."""
+    return _t5enc_attention_train("t5enc_attention_train", qkv, src, offsets, key_mask, rel, S, seed, p)
+
+
+def t5enc_attention_tc_train(qkv: torch.Tensor, src: torch.Tensor, offsets: torch.Tensor, key_mask: torch.Tensor,
+                             rel: torch.Tensor, S: int, seed: torch.Tensor, p: float):
+    """``t5enc_attention_train`` with its products on TF32 tensor cores (rqb200_t5enc_attention_tc_train), one launch; the same
+    keep bits under the same seed."""
+    return _t5enc_attention_train("t5enc_attention_tc_train", qkv, src, offsets, key_mask, rel, S, seed, p)
+
+
+def _t5enc_attention_train(name, qkv, src, offsets, key_mask, rel, S, seed, p):
     _need_cuda(qkv, src, offsets, key_mask, rel, seed)
     rel = _f32c(rel)
     heads = rel.shape[0]
@@ -1100,9 +1121,9 @@ def t5enc_attention_train(qkv: torch.Tensor, src: torch.Tensor, offsets: torch.T
     out = torch.empty((N, heads * T5_DKV), dtype=torch.float32, device=qkv.device)
     lse = torch.empty((N, heads), dtype=torch.float32, device=qkv.device)
     with torch.cuda.device(qkv.device):
-        _lib.check(_lib.load().rqb200_t5enc_attention_train(_p(qkv), qkv.stride(0), _p(src), _p(offsets), _p(key_mask), _p(rel), B,
-                                                            S, heads, _p(seed), _check_p(p), _p(out), out.stride(0), _p(lse),
-                                                            _stream()), "t5enc_attention_train")
+        _lib.check(getattr(_lib.load(), "rqb200_" + name)(_p(qkv), qkv.stride(0), _p(src), _p(offsets), _p(key_mask), _p(rel), B,
+                                                         S, heads, _p(seed), _check_p(p), _p(out), out.stride(0), _p(lse),
+                                                         _stream()), name)
     _count(1)
     return out, lse
 
@@ -1111,6 +1132,18 @@ def t5enc_attention_backward(qkv: torch.Tensor, out: torch.Tensor, dout: torch.T
                              offsets: torch.Tensor, key_mask: torch.Tensor, rel: torch.Tensor, S: int, seed: torch.Tensor, p: float):
     """The backward of ``t5enc_attention_train`` (rqb200_t5enc_attention_backward), two launches and one fixed-order sum ->
     (d_qkv [N, 3 inner], d_rel [heads, 2S - 1]).  Bit-reproducible."""
+    return _t5enc_attention_backward("t5enc_attention_backward", qkv, out, dout, lse, src, offsets, key_mask, rel, S, seed, p)
+
+
+def t5enc_attention_tc_backward(qkv: torch.Tensor, out: torch.Tensor, dout: torch.Tensor, lse: torch.Tensor, src: torch.Tensor,
+                                offsets: torch.Tensor, key_mask: torch.Tensor, rel: torch.Tensor, S: int, seed: torch.Tensor,
+                                p: float):
+    """The backward of ``t5enc_attention_tc_train`` on TF32 tensor cores (rqb200_t5enc_attention_tc_backward), two launches and
+    one fixed-order sum -> (d_qkv [N, 3 inner], d_rel [heads, 2S - 1]).  Bit-reproducible."""
+    return _t5enc_attention_backward("t5enc_attention_tc_backward", qkv, out, dout, lse, src, offsets, key_mask, rel, S, seed, p)
+
+
+def _t5enc_attention_backward(name, qkv, out, dout, lse, src, offsets, key_mask, rel, S, seed, p):
     _need_cuda(qkv, out, dout, lse, src, offsets, key_mask, rel, seed)
     heads = rel.shape[0]
     inner = heads * T5_DKV
@@ -1121,15 +1154,14 @@ def t5enc_attention_backward(qkv: torch.Tensor, out: torch.Tensor, dout: torch.T
     if out.shape[0] != N or dout.shape[0] != N or lse.shape != (N, heads) or rel.shape != (heads, 2 * S - 1):
         raise ValueError("out / dout [N, inner], lse [N, heads] and rel [heads, 2S - 1] must match qkv [N, 3 inner]")
     lib = _lib.load()
-    tiles = lib.rqb200_t5enc_attention_backward_tiles(S)
+    tiles = getattr(lib, "rqb200_" + name + "_tiles")(S)
     delta = torch.empty((N, heads), dtype=torch.float32, device=qkv.device)
     dqkv = torch.empty((N, 3 * inner), dtype=torch.float32, device=qkv.device)
     part = torch.empty((B * tiles, heads, 2 * S - 1), dtype=torch.float32, device=qkv.device)
     with torch.cuda.device(qkv.device):
-        _lib.check(lib.rqb200_t5enc_attention_backward(_p(qkv), qkv.stride(0), _p(out), out.stride(0), _p(dout), dout.stride(0),
-                                                       _p(lse), _p(src), _p(offsets), _p(key_mask), _p(rel), B, S, heads, _p(seed),
-                                                       _check_p(p), _p(delta), _p(dqkv), dqkv.stride(0), _p(part), _stream()),
-                   "t5enc_attention_backward")
+        _lib.check(getattr(lib, "rqb200_" + name)(_p(qkv), qkv.stride(0), _p(out), out.stride(0), _p(dout), dout.stride(0),
+                                                 _p(lse), _p(src), _p(offsets), _p(key_mask), _p(rel), B, S, heads, _p(seed),
+                                                 _check_p(p), _p(delta), _p(dqkv), dqkv.stride(0), _p(part), _stream()), name)
     _count(2)
     return dqkv, part.sum(0)
 
@@ -1195,6 +1227,25 @@ class T5EncAttentionFunction(torch.autograd.Function):
     def backward(ctx, dout):
         qkv, rel, src, offsets, key_mask, seed, out, lse = ctx.saved_tensors
         dqkv, drel = t5enc_attention_backward(qkv, out, dout, lse, src, offsets, key_mask, rel, ctx.S, seed, ctx.p)
+        return dqkv, drel, None, None, None, None, None, None
+
+
+class T5EncAttentionTCFunction(torch.autograd.Function):
+    """``T5EncAttentionFunction`` on the TF32 tensor-core kernels (``t5enc_attention_tc_train`` / ``_tc_backward``), the same
+    arguments and gradients."""
+
+    @staticmethod
+    def forward(ctx, qkv, rel, src, offsets, key_mask, S, seed, p):
+        qkv = qkv.contiguous()
+        out, lse = t5enc_attention_tc_train(qkv, src, offsets, key_mask, rel, S, seed, p)
+        ctx.save_for_backward(qkv, rel, src, offsets, key_mask, seed, out, lse)
+        ctx.S, ctx.p = S, p
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        qkv, rel, src, offsets, key_mask, seed, out, lse = ctx.saved_tensors
+        dqkv, drel = t5enc_attention_tc_backward(qkv, out, dout, lse, src, offsets, key_mask, rel, ctx.S, seed, ctx.p)
         return dqkv, drel, None, None, None, None, None, None
 
 
