@@ -10,18 +10,33 @@
 //   one candidate -> it is the exact argmin;  else the candidates are re-scored with the exact fp32 arithmetic of the
 //   CUDA-core kernel (sequential fp32 residual, (xx + cc) - 2 dot, first index wins ties).
 //
-// One CTA per SM, persistent over 64-row tiles:
-//   warps 0-3 (one warpgroup)  convert the tile's rows from their x stages to the fp16 image (K-major SWIZZLE_128B, resident for
-//                              all levels) and measure ||fp16(x) - x||^2 and ||x||^2 per row; per level and 256-code block: 4 x
-//                              wgmma per 64-wide k chunk into a 64 x 256 register accumulator, then score.  All 256 codes of a
-//                              block sit in one thread quad, so the block minimum and its candidate bits are quad shuffles; rows
-//                              with more than one candidate go to a shared queue that the four warps re-rank exactly.
-//   warp 4                     producer of one 32 KB stage ring (bulk copies counted on an mbarrier per stage).  Per tile it
-//                              first stages the tile's fp32 rows, 128 columns per stage (one copy per row, spread over the
-//                              lanes), then for every (level, block, k chunk) the prepared 16 KB blocks of codes [256 cb,
-//                              256 cb + 128) and [256 cb + 128, 256 cb + 256).  It runs ahead into the next block, level and
-//                              tile while the warpgroup scores, so the next tile's rows are in flight while the last level of
-//                              this one is scored and re-ranked, and the conversion issues no global loads.
+// One CTA per SM, persistent over 64-row tiles, three warpgroups with their own register budgets (setmaxnreg):
+//   WG0, warps 0-3   MMA and scoring: per level and 256-code block, 4 x wgmma per 64-wide k chunk into a 64 x 256 register
+//     (scorer)       accumulator, then score.  All 256 codes of a block sit in one thread quad, so the block minimum and its
+//                    candidate bits are quad shuffles; a row with one candidate takes it, rows with more go to a shared queue.
+//                    It never converts and never re-ranks.
+//   WG1, warps 4-7   convert the next tile's rows from their x stages to the fp16 image (K-major SWIZZLE_128B, resident for
+//     (helper)       all levels of a tile) and measure ||fp16(x) - x||^2 and ||x||^2 per row; re-rank the queued rows of each
+//                    level exactly, any warp taking the next queued row.
+//   WG2, warp 8      producer of one 32 KB stage ring (bulk copies counted on an mbarrier per stage).  Per tile it first
+//                    stages the tile's fp32 rows, 128 columns per stage (one copy per row, spread over the lanes), then for
+//                    every (level, block, k chunk) the prepared 16 KB blocks of codes [256 cb, 256 cb + 128) and
+//                    [256 cb + 128, 256 cb + 256).  Warps 9-11 exit at once.  The helper consumes the x stages and the scorer
+//                    the codebook stages; each walks the same stage counter and skips the other's stages.
+//
+// Hand-offs of tile t, on four mbarriers that every thread of the signalling warpgroup arrives on:
+//   scorer  waits IMG_FULL(t); per level l: MMA(l) (after the last level's MMAs complete it arrives on IMG_FREE(t)), waits
+//           RR_DONE of the level before (for l = 0: level L-1 of tile t-1), scores and selects, arrives on Q_READY(l).
+//   helper  waits IMG_FREE(t-1) and converts tile t, keeping the row statistics in registers; waits Q_READY(L-1) of tile t-1
+//           (the scorer no longer reads rowinfo), writes rowinfo, arrives on IMG_FULL(t); re-ranks level L-1 of tile t-1 and
+//           arrives on RR_DONE; then for l = 0 .. L-2 waits Q_READY(l), re-ranks level l of tile t, arrives on RR_DONE.
+// So the scorer writes the ids, candidate words and queue of a level only once the previous level's re-rank has drained
+// them, and the helper writes the image and rowinfo only once the scorer is done with them: none of them is doubled, and the
+// shared memory is the single-warpgroup layout's plus four mbarriers.  Each barrier's waiter is never more than one phase
+// behind (every arrival needs the other side's previous wait), so parity waits are exact.  The ring cannot deadlock at any
+// depth: the producer issues a tile's x stages after the previous tile's last codebook stage, and the helper consumes them
+// only after IMG_FREE, which needs nothing but earlier stages.  Each level's re-rank runs under the next level's MMAs, the
+// conversion under the last level's scoring.
 //
 // Two kernels share every stage but the candidate selection:
 //   rq_tcx_kernel          K = 256: one accumulator holds the whole level, so the row minimum and the candidate words stay in
@@ -41,14 +56,23 @@
 #define TX_STAGE_BYTES (2 * TC_BSTAGE_BYTES)      // 256 codes x 64 k fp16 = 32 KB = 64 rows x 128 columns of fp32 x
 #define TX_XCOLS 128                              // columns of x per stage: a 512-byte row
 #define TX_XROW_BYTES (TX_XCOLS * 4)
-#define TX_XGROUP 4                               // rows a converter warp reads from a stage at once
+#define TX_XGROUP 8                               // rows a converter warp reads from a stage at once
 #define TX_SLOT_BYTES (TX_R * TC_KC * 2)          // one k chunk of the x image: 8 KB
-#define TX_THREADS 160
+#define TX_THREADS 384                            // scorer, helper and producer warpgroups
+#define TX_REG_LAUNCH 168                         // registers per thread at launch: 65536 / 384, rounded down to 8
+#define TX_REG_SCORER 240                         // setmaxnreg of each role: the scorer raises, the others lower
+#define TX_REG_HELPER 160
+#define TX_REG_PRODUCER 40
+static_assert(TX_REG_LAUNCH * TX_THREADS <= 65536 && TX_REG_SCORER >= TX_REG_LAUNCH && TX_REG_HELPER <= TX_REG_LAUNCH &&
+                  TX_REG_PRODUCER <= TX_REG_LAUNCH && TX_REG_SCORER + TX_REG_HELPER + TX_REG_PRODUCER <= 3 * TX_REG_LAUNCH,
+              "setmaxnreg budgets must fit the registers the CTA is launched with");
 #define TX_SMEM_LIMIT 232448                      // 227 KB of opt-in shared memory per block
 #define TX_GC 4                                   // column groups per chunk of Gram-row loads in tx_score (8 spills)
 
 struct TxSmem {
   uint64_t full[TX_NB_MAX], empty[TX_NB_MAX];
+  uint64_t img_full, img_free;                    // the image of a tile written (helper) / last read (scorer)
+  uint64_t q_ready, rr_done;                      // a level's queue complete (scorer) / its re-rank done (helper)
   uint32_t fl_count, fl_next;                     // queue of rows that need the exact re-rank
   uint32_t rowinfo[TX_R];                         // bf16_up(||fp16(x)-x||^2) << 16 | bf16_up(||x||^2)
   unsigned char flist[TX_R];
@@ -101,25 +125,29 @@ static size_t tcx_smem_bytes(int D, int K, int L, int nb) {
 __device__ __forceinline__ float tx_margin(const TcLevelConst& lc, uint32_t ri) {
   return 2.f * tc_eps(lc, __uint_as_float(ri & 0xffff0000u), __uint_as_float(ri << 16)) * 1.0000153f;
 }
-__device__ __forceinline__ void tx_wg_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }   // the 4 warps of the warpgroup
+__device__ __forceinline__ void tx_helper_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }   // the helper's 4 warps
+template <uint32_t N> __device__ __forceinline__ void tx_reg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <uint32_t N> __device__ __forceinline__ void tx_reg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 __device__ __forceinline__ float tx_min_nan(float a, float b) {       // NaN if either is NaN
   float r;
   asm("min.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
   return r;
 }
 
-// ring barriers and an empty re-rank queue, visible to all five warps on return
+// ring and hand-off barriers and an empty re-rank queue, visible to all warps on return
 __device__ __forceinline__ void tx_init(unsigned char* tsm, TxSmem* ms) {
   if (threadIdx.x == 0) {
     if ((smem_u32(tsm) & 1023u) != 0) __trap();              // the swizzle pattern needs a 1024-byte aligned base
     for (int i = 0; i < TX_NB_MAX; ++i) { mbar_init(&ms->full[i], 1); mbar_init(&ms->empty[i], 4); }
+    mbar_init(&ms->img_full, 128); mbar_init(&ms->img_free, 128);
+    mbar_init(&ms->q_ready, 128); mbar_init(&ms->rr_done, 128);
     ms->fl_count = 0; ms->fl_next = 0;
     fence_mbar_init();
   }
   __syncthreads();
 }
 
-// producer (warp 4): stages in the order the warpgroup consumes them -- per tile, its x stages, then (level, block, k chunk).
+// producer (warp 8): per tile, its x stages (the helper's), then (level, block, k chunk) (the scorer's).
 // Lane 0 waits for a free slot and arms its mbarrier with the exact byte count.  X stage c holds columns [128 c, 128 c + 128)
 // (half of them when D % 128 == 64) of the tile's rows below B, 512 bytes per row whatever the width; each lane copies rows
 // lane and lane + 32.  Lane 0 copies the two 16 KB halves of a codebook stage.
@@ -160,12 +188,13 @@ __device__ __forceinline__ void tx_produce(const TxParams& p, unsigned char* sC,
 }
 
 // fp16 image + row statistics of the tile at row0 from its x stages, the next ones of the ring (s counts the stages
-// consumed): warp w converts rows [16w, 16w + 16); lane = float4 column of every 512-byte stage row.  Each warp releases a
-// stage once its rows are read.  The per-lane sums of a row run over the columns in order, so the statistics do not depend
-// on the stage width.  Rows past B are zeros and are never read.  The image is visible to the tensor core on return.
-__device__ __forceinline__ void tx_convert(const TxParams& p, TxSmem* ms, uint32_t x_base, const unsigned char* sC, int row0,
-                                           uint32_t& s) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, lane4 = lane * 4, D = p.D;
+// consumed): helper warp w converts rows [16w, 16w + 16); lane = float4 column of every 512-byte stage row.  Each warp
+// releases a stage once its rows are read.  The per-lane sums of a row run over the columns in order, so the statistics do
+// not depend on the stage width.  Rows past B are zeros and are never read.  Returns, in lane i < 16, the rowinfo word of
+// row 16w + i; the caller publishes it and makes the image visible to the tensor core.
+__device__ __forceinline__ uint32_t tx_convert(const TxParams& p, TxSmem* ms, uint32_t x_base, const unsigned char* sC, int row0,
+                                               uint32_t& s) {
+  const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31, lane4 = lane * 4, D = p.D;
   const int nxs = (D + TX_XCOLS - 1) / TX_XCOLS, nr = min(16, p.B - row0 - warp * 16);   // rows of this warp below B
   const uint32_t nb = (uint32_t)p.nb;
   float s2[16], e2[16];
@@ -177,10 +206,9 @@ __device__ __forceinline__ void tx_convert(const TxParams& p, TxSmem* ms, uint32
     const int c = c4 * TX_XCOLS + lane4;
     mbar_wait_guarded(&ms->full[st], (s / nb) & 1, 2);
     const float4* srcp = reinterpret_cast<const float4*>(sC + st * TX_STAGE_BYTES + warp * 16 * TX_XROW_BYTES) + lane;
-    // TX_XGROUP rows at a time: the 128 accumulator registers stay allocated through the conversion, and with the 32
-    // partial sums more rows in flight spill in rq_tcx_blocked_kernel.  The image stores below carry no memory clobber, so
-    // the compiler may issue a group's stage loads ahead of the previous group's stores (they never overlap); the stage
-    // wait and release above and below are compiler barriers either way
+    // TX_XGROUP rows at a time.  The image stores below carry no memory clobber, so the compiler may issue a group's stage
+    // loads ahead of the previous group's stores (they never overlap); the stage wait and release above and below are
+    // compiler barriers either way
 #pragma unroll
     for (int i0 = 0; i0 < 16; i0 += TX_XGROUP) {
       float4 v[TX_XGROUP];
@@ -209,13 +237,13 @@ __device__ __forceinline__ void tx_convert(const TxParams& p, TxSmem* ms, uint32
     __syncwarp();
     if (lane == 0) mbar_arrive(&ms->empty[st]);
   }
+  uint32_t ri = 0;
 #pragma unroll
   for (int i = 0; i < 16; ++i) {
     const float a = warp_sum(s2[i]), b = warp_sum(e2[i]);
-    if (lane == 0) ms->rowinfo[warp * 16 + i] = (tc_bf16_up(b) << 16) | tc_bf16_up(a);
+    if (lane == i) ri = (tc_bf16_up(b) << 16) | tc_bf16_up(a);
   }
-  fence_proxy_async();                 // generic-proxy smem writes -> visible to the tensor core (async proxy)
-  tx_wg_sync();
+  return ri;
 }
 
 // S = X . C^T of one 256-code block over the next nkc ring stages (s counts the stages consumed); a stage is released as
@@ -347,16 +375,15 @@ __device__ __forceinline__ bool tx_settle(const TxParams& p, TxSmem* ms, Id* ids
   return false;
 }
 
-// Exact re-rank of the tile's queued rows at level l once every row is settled or queued; any warp takes the next row (same
-// arithmetic as rq_simt.cu: sequential fp32 residual, (xx + cc) - 2 dot, candidates in ascending index order with a strict
-// '<': first index wins ties).  Lane covers elements 128 i + 4 lane .. +3 of a row (6 x LDG.128 per row).  On return every id
-// of the level is in ids[] and the queue is empty again.  p is taken by value: by reference, ptxas spills a tile counter of
-// rq_tcx_kernel (both kernels sit at 255 registers).
+// Exact re-rank, by the helper, of the tile's queued rows at level l once the scorer has settled or queued every row
+// (Q_READY); any warp takes the next row (same arithmetic as rq_simt.cu: sequential fp32 residual, (xx + cc) - 2 dot,
+// candidates in ascending index order with a strict '<': first index wins ties).  Lane covers elements 128 i + 4 lane .. +3
+// of a row (6 x LDG.128 per row).  On return every id of the level is in ids[] and the queue is empty again, for the scorer
+// once the helper has arrived on RR_DONE.
 template <class Id>
-__device__ __forceinline__ void tx_rerank(const TxParams p, const TxShared<Id>& sh, int l, int row0, int K) {
+__device__ __forceinline__ void tx_rerank(const TxParams& p, const TxShared<Id>& sh, int l, int row0, int K) {
   const int lane = threadIdx.x & 31, lane4 = lane * 4, D = p.D, nw = K / 32;
   TxSmem* const ms = sh.ms;
-  tx_wg_sync();                                             // the re-rank queue of the tile is complete
   const float* ccl = p.cc + (size_t)l * K;
   const float* cl = p.cbf + (size_t)l * K * D;
   const uint32_t nfl = *reinterpret_cast<volatile uint32_t*>(&ms->fl_count);
@@ -455,32 +482,90 @@ __device__ __forceinline__ void tx_rerank(const TxParams p, const TxShared<Id>& 
     atomicAdd(p.stats + 1, n_cand);
     atomicAdd(p.stats + 2, n_many);
   }
-  tx_wg_sync();                                             // every id of the level is in ids[]; the queue is drained
-  if (threadIdx.x == 0) { ms->fl_count = 0; ms->fl_next = 0; }
-  tx_wg_sync();
+  tx_helper_sync();                                         // every id of the level is in ids[]; the queue is drained
+  // the reset reaches the scorer with this thread's RR_DONE arrival, and the other helper warps through the scorer's next
+  // Q_READY, so no second barrier
+  if ((threadIdx.x & 127) == 0) { ms->fl_count = 0; ms->fl_next = 0; }
+}
+
+// helper warpgroup: converts each tile into the image and re-ranks its levels, in the hand-off order of the header comment
+// (n counts the tiles, so the Q_READY / RR_DONE completion of level l of tile n is the (n L + l)-th)
+template <class Id>
+__device__ __forceinline__ void tx_helper(const TxParams& p, const TxShared<Id>& sh, uint32_t x_base, int K) {
+  TxSmem* const ms = sh.ms;
+  const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
+  const uint32_t L = (uint32_t)p.L, ncs = L * (uint32_t)((K / TC_K) * p.nkc);   // codebook stages of a tile: the scorer's
+  uint32_t s = 0, n = 0;
+  int prev0 = 0;                                            // row0 of the previous tile
+#pragma unroll 1
+  for (int unit = blockIdx.x; unit < p.ntiles; unit += gridDim.x, ++n) {
+    const int row0 = unit * TX_R;
+    if (n > 0) mbar_wait_guarded(&ms->img_free, (n - 1) & 1, 3);
+    const uint32_t ri = tx_convert(p, ms, x_base, sh.sC, row0, s);
+    s += ncs;
+    if (n > 0) mbar_wait_guarded(&ms->q_ready, (n * L - 1) & 1, 4);   // the scorer is done with the last tile's rowinfo
+    if (lane < 16) ms->rowinfo[warp * 16 + lane] = ri;
+    fence_proxy_async();                                    // generic-proxy image stores -> visible to the tensor core
+    mbar_arrive(&ms->img_full);
+    if (n > 0) {
+      tx_rerank(p, sh, (int)L - 1, prev0, K);
+      mbar_arrive(&ms->rr_done);
+    }
+#pragma unroll 1
+    for (uint32_t l = 0; l + 1 < L; ++l) {
+      mbar_wait_guarded(&ms->q_ready, (n * L + l) & 1, 4);
+      tx_rerank(p, sh, (int)l, row0, K);
+      mbar_arrive(&ms->rr_done);
+    }
+    prev0 = row0;
+  }
+  if (n > 0) {
+    mbar_wait_guarded(&ms->q_ready, (n * L - 1) & 1, 4);
+    tx_rerank(p, sh, (int)L - 1, prev0, K);
+  }
+}
+
+// the helper and producer warpgroups of either kernel, each at its register budget; returns false in the scorer warpgroup,
+// which has raised its own
+template <class Id>
+__device__ __forceinline__ bool tx_side_roles(const TxParams& p, const TxShared<Id>& sh, uint32_t x_base, int K) {
+  const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);
+  if (wg == 2) {
+    tx_reg_dec<TX_REG_PRODUCER>();
+    if (threadIdx.x < 9 * 32) tx_produce(p, sh.sC, sh.ms, K / TC_K);   // warp 8; warps 9-11 have nothing to do
+    return true;
+  }
+  if (wg == 1) {
+    tx_reg_dec<TX_REG_HELPER>();
+    tx_helper(p, sh, x_base, K);
+    return true;
+  }
+  tx_reg_inc<TX_REG_SCORER>();
+  return false;
 }
 
 __global__ void __launch_bounds__(TX_THREADS, 1) rq_tcx_kernel(const __grid_constant__ TxParams p) {
   extern __shared__ __align__(1024) unsigned char tsm[];
   const TxShared<uint8_t> sh = tx_shared<uint8_t>(tsm, p, TC_K);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  tx_init(tsm, sh.ms);
-  if (warp == 4) {
-    tx_produce(p, sh.sC, sh.ms, 1);
-    return;
-  }
-  const int q4 = lane & 3;
-  const int r0 = warp * 16 + (lane >> 2), r1 = r0 + 8;      // accumulator rows of this thread
   const uint32_t x_base = smem_u32(tsm), c_base = smem_u32(sh.sC);
-  uint32_t s = 0;
+  tx_init(tsm, sh.ms);
+  if (tx_side_roles(p, sh, x_base, TC_K)) return;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, q4 = lane & 3;
+  const int r0 = warp * 16 + (lane >> 2), r1 = r0 + 8;      // accumulator rows of this thread
+  const uint32_t nxs = (uint32_t)((p.D + TX_XCOLS - 1) / TX_XCOLS), L = (uint32_t)p.L;
+  uint32_t s = 0, n = 0;
 #pragma unroll 1
-  for (int unit = blockIdx.x; unit < p.ntiles; unit += gridDim.x) {
+  for (int unit = blockIdx.x; unit < p.ntiles; unit += gridDim.x, ++n) {
     const int row0 = unit * TX_R;
-    tx_convert(p, sh.ms, x_base, sh.sC, row0, s);
+    s += nxs;                                               // the tile's x stages: the helper's
+    mbar_wait_guarded(&sh.ms->img_full, n & 1, 5);
 #pragma unroll 1
-    for (int l = 0; l < p.L; ++l) {
+    for (uint32_t l = 0; l < L; ++l) {
       float acc[128];
       tx_mma(acc, sh.ms, x_base, c_base, p.nkc, (uint32_t)p.nb, s);
+      if (l + 1 == L) mbar_arrive(&sh.ms->img_free);       // the helper may convert the next tile
+      // ids, candidate words and queue of the level before are drained by its re-rank
+      if (n | l) mbar_wait_guarded(&sh.ms->rr_done, (n * L + l - 1) & 1, 6);
       const TcLevelConst lc = p.hdr->lv[l];
       tx_score(acc, p, lc, l, 0, TC_K, sh.ids, r0, r1);
       // ---- candidates: the row minimum, then the 8 candidate words in registers; only a queued row stores its words
@@ -503,7 +588,7 @@ __global__ void __launch_bounds__(TX_THREADS, 1) rq_tcx_kernel(const __grid_cons
           for (int w = 0; w < 8; ++w) sh.cmask[r * 8 + w] = q4 ? w1[w] : w0[w];
         }
       }
-      tx_rerank(p, sh, l, row0, TC_K);
+      mbar_arrive(&sh.ms->q_ready);                         // every row of the level is settled or queued
     }
   }
 }
@@ -512,28 +597,29 @@ __global__ void __launch_bounds__(TX_THREADS, 1) rq_tcx_blocked_kernel(const __g
   extern __shared__ __align__(1024) unsigned char tsm[];
   const int K = p.K, nblk = p.nblk, nw = K / 32;
   const TxShared<uint16_t> sh = tx_shared<uint16_t>(tsm, p, K);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  tx_init(tsm, sh.ms);
-  if (warp == 4) {
-    tx_produce(p, sh.sC, sh.ms, nblk);
-    return;
-  }
-  const int q4 = lane & 3;
-  const int r0 = warp * 16 + (lane >> 2), r1 = r0 + 8;      // accumulator rows of this thread
   const uint32_t x_base = smem_u32(tsm), c_base = smem_u32(sh.sC);
-  uint32_t s = 0;
+  tx_init(tsm, sh.ms);
+  if (tx_side_roles(p, sh, x_base, K)) return;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, q4 = lane & 3;
+  const int r0 = warp * 16 + (lane >> 2), r1 = r0 + 8;      // accumulator rows of this thread
+  const uint32_t nxs = (uint32_t)((p.D + TX_XCOLS - 1) / TX_XCOLS), L = (uint32_t)p.L;
+  uint32_t s = 0, n = 0;
 #pragma unroll 1
-  for (int unit = blockIdx.x; unit < p.ntiles; unit += gridDim.x) {
+  for (int unit = blockIdx.x; unit < p.ntiles; unit += gridDim.x, ++n) {
     const int row0 = unit * TX_R;
-    tx_convert(p, sh.ms, x_base, sh.sC, row0, s);
+    s += nxs;                                               // the tile's x stages: the helper's
+    mbar_wait_guarded(&sh.ms->img_full, n & 1, 5);
 #pragma unroll 1
-    for (int l = 0; l < p.L; ++l) {
+    for (uint32_t l = 0; l < L; ++l) {
       float run0 = INFINITY, run1 = INFINITY;                // running row minima over the blocks scored so far
       float thr0 = 0.f, thr1 = 0.f;                          // candidate thresholds of the latest block: the final ones after it
 #pragma unroll 1
       for (int cb = 0; cb < nblk; ++cb) {
         float acc[128];
         tx_mma(acc, sh.ms, x_base, c_base, p.nkc, (uint32_t)p.nb, s);
+        if (l + 1 == L && cb + 1 == nblk) mbar_arrive(&sh.ms->img_free);   // the helper may convert the next tile
+        // ids, candidate words and queue of the level before are drained by its re-rank
+        if (cb == 0 && (n | l)) mbar_wait_guarded(&sh.ms->rr_done, (n * L + l - 1) & 1, 6);
         const TcLevelConst lc = p.hdr->lv[l];
         tx_score(acc, p, lc, l, cb * TC_K, K, sh.ids, r0, r1);
         // ---- candidates: the block minimum, the running minimum, then the block's candidate words to shared memory
@@ -587,12 +673,12 @@ __global__ void __launch_bounds__(TX_THREADS, 1) rq_tcx_blocked_kernel(const __g
         }
         tx_settle(p, sh.ms, sh.ids, l, row0, r, cnt, first, K);
       }
-      tx_rerank(p, sh, l, row0, K);
+      mbar_arrive(&sh.ms->q_ready);                         // every row of the level is settled or queued
     }
   }
 }
 
-// the ring gets as many 32 KB stages (<= TX_NB_MAX) as fit under the 227 KB limit: 4 at K = 256 for every D and L (120 bytes
+// the ring gets as many 32 KB stages (<= TX_NB_MAX) as fit under the 227 KB limit: 4 at K = 256 for every D and L (88 bytes
 // to spare at D = 768, L = 8), 3 at K > 256 with D = 768 and at some K > 256 with D = 640 or 704, 4 elsewhere.  tcx_run and
 // rqb200_tokenize_tc_ring_stages both take the depth from here.
 int tcx_ring_stages(int D, int K, int L) {
