@@ -246,6 +246,15 @@ int rqb200_sid_trie_beam_topk(const float* logits, int64_t logits_stride, const 
                               int kp, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
                               float* out_log_probas, int64_t* out_parent, int* bad, void* stream);
 
+/* The trie's level arrays as plain device arrays (the exact ranking decodes one row per node).
+ * sid_trie_counts : counts int32 [C + 1] = the node count of every level (counts[0] = 1, the root); one tiny launch.
+ * sid_trie_level  : for level l (1..C) of n_l nodes below n_prev parents: code int32 [n_l] (each node's last id), parent int32
+ *                   [n_l] (its node in level l - 1) and, for l < C, child int32 [n_l + 1] (node i's children in level l + 1 are
+ *                   child[i] .. child[i + 1] - 1; null when l = C).  n_l and n_prev must be the counts above. */
+int rqb200_sid_trie_counts(const void* workspace, int* counts, void* stream);
+int rqb200_sid_trie_level(const void* workspace, int C, int l, int n_l, int n_prev, int* code, int* parent, int* child,
+                          void* stream);
+
 /* ---- from generated id tuples to corpus items ----
  * Row n of the corpus id table [N, C] is item n; rows with equal tuples are told apart by their dedup rank (the tokeniser's last
  * column: how many earlier rows carry the same tuple).  The item table maps a tuple back to its rows.  A row is retrievable
@@ -272,6 +281,9 @@ int rqb200_sid_items_lookup(const void* workspace, const int64_t* ids, int64_t i
                             int64_t* out_item /* [P] */, void* stream);
 int rqb200_sid_items_retrieve(const void* workspace, const int64_t* generated, const float* log_probas, int B, int k, int C, int n,
                               int64_t* out_items, int* out_beam, int* out_count, void* stream);
+/* sid_items_offsets   : byte offsets of row (int32 [N]) and start (int32 [N + 1]) in the item table's workspace; arithmetic only.
+ *                       RQB_ERR_UNSUPPORTED outside the table's limits. */
+int rqb200_sid_items_offsets(int64_t N, int C, int K, size_t* row, size_t* start);
 
 /* sid_topk_rank_hist  : evaluate/metrics.py's TopKAccumulator rule, accumulated on the device.  Row b's rank is its first
  *                       candidate cand[b, j, 0:D] equal to actual[b, 0:D] in all D columns (`.all(-1).max(-1)`); hist[rank] += 1,
@@ -282,6 +294,37 @@ int rqb200_sid_items_retrieve(const void* workspace, const int64_t* generated, c
  *                       (elements).  B = 0 is a no-op. */
 int rqb200_sid_topk_rank_hist(const int64_t* actual, int64_t a_stride, const int64_t* cand, int64_t c_stride, int B, int k, int D,
                               int item_mode, int64_t* hist, void* stream);
+/* sid_rank_hist       : hist[rank[b]] += 1 for an exact rank in [0, k), hist[k] += 1 otherwise (-1: the item is not ranked).
+ *                       rank int64 [B], hist int64 [k + 1], ADDED to.  B = 0 is a no-op. */
+int rqb200_sid_rank_hist(const int64_t* rank, int B, int64_t k, int64_t* hist, void* stream);
+
+/* ---- exact ranking of every corpus item (modules/model.py rank_sem_ids / rank_items), csrc/t5rank.cu ----
+ * t5rank_cross_attention : T5 cross-attention (no 1/sqrt(d) scaling, fp32 softmax) of Q queries per history: q [B * Q, inner] (row
+ *                          stride ldq; history b's queries are rows b * Q ..), keys / values of history b the rows offsets[b] ..
+ *                          offsets[b + 1] - 1 of k / v (row stride ldkv; offsets int32 [B + 1], absolute rows), score q . k +
+ *                          key_mask[row] (fp32 [rows]: 0, or -FLT_MAX to mask; null: 0).  out [B * Q, inner] (row stride ldo);
+ *                          a history without keys gets zeros.  Limits: B, heads <= 65535.
+ * t5rank_cross_attention_tc : the same call with S = Q K^T and P V as wgmma m64n64k8 TF32 (operands rounded to TF32, fp32
+ *                          accumulate), softmax and mask in fp32; q, k, v 16-byte aligned with row strides a multiple of 4.
+ * t5rank_children        : logits [R, K] (row stride ld) of R = B * n_h node rows of one trie level (row b * n_h + i); per row
+ *                          lse = m + logf(sum expf(x - m)) exactly as sid_trie_beam_topk, and for every child j of node i (child
+ *                          int32 [n_h + 1]: child[i] <= j < child[i + 1]) out[b * n_next + j] = (x[code[j]] - lse) + parent[r]
+ *                          (parent fp32 [R], null: 0; code int32 [n_next]).  A row holding a NaN or +inf logit, or all -inf, adds 1
+ *                          to bad (int32 [1], optional) and gives its children NaN.
+ * t5rank_select          : one CTA per history over its U leaf scores (scores fp32 [B, U], leaf u = item-table tuple u; row / start
+ *                          the item table's arrays, sid_items_offsets).  Order: score descending, then leaf ascending, NaN last;
+ *                          each leaf's items in dedup order.  out_items int64 [B, n] / out_scores fp32 [B, n] (the item's leaf
+ *                          score): the first n items, -1 / -inf past the corpus.  out_rank int64 [B]: the position in that order of
+ *                          item t_dedup[b] of leaf t_leaf[b] (int64 [B] each), -1 when t_leaf is outside [0, U) or the dedup rank
+ *                          outside the leaf's items.  n <= 1024 (RQB_ERR_UNSUPPORTED).  No global atomics: deterministic. */
+int rqb200_t5rank_cross_attention(const float* q, int64_t ldq, const float* k, const float* v, int64_t ldkv, const int* offsets,
+                                  const float* key_mask, int B, int Q, int heads, float* out, int64_t ldo, void* stream);
+int rqb200_t5rank_cross_attention_tc(const float* q, int64_t ldq, const float* k, const float* v, int64_t ldkv, const int* offsets,
+                                     const float* key_mask, int B, int Q, int heads, float* out, int64_t ldo, void* stream);
+int rqb200_t5rank_children(const float* logits, int64_t ld, int R, int K, int n_h, const float* parent, const int* child,
+                           const int* code, int n_next, float* out, int* bad, void* stream);
+int rqb200_t5rank_select(const float* scores, int B, int U, const int* row, const int* start, const int64_t* t_leaf,
+                         const int64_t* t_dedup, int n, int64_t* out_items, float* out_scores, int64_t* out_rank, void* stream);
 
 /* ---- one step of the generative-retrieval model's T5 decoder (modules/model.py, generate(decoder="fused")), csrc/t5dec.cu ----
  * HF T5 numerics in eval mode: attention without 1/sqrt(d) scaling, fp32 softmax, d_kv = 64 per head (inner = heads * 64).

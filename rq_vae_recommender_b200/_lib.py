@@ -14,7 +14,8 @@ from typing import Optional
 PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "librqb200.so")
-SOURCES = ["api.cu", "rq_simt.cu", "dense.cu", "rq_tc.cu", "rq_tcx.cu", "gemm_tc.cu", "sid.cu", "t5dec.cu", "t5enc.cu", "t5enc_tc.cu"]
+SOURCES = ["api.cu", "rq_simt.cu", "dense.cu", "rq_tc.cu", "rq_tcx.cu", "gemm_tc.cu", "sid.cu", "t5dec.cu", "t5enc.cu", "t5enc_tc.cu",
+           "t5rank.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-shared", "-Xcompiler", "-fPIC"]
 
@@ -79,6 +80,16 @@ _SIGNATURES = {
     "rqb200_sid_items_lookup": (c_int, [c_vp, c_vp, c_i64, c_i64, c_int, c_vp, c_vp]),
     "rqb200_sid_items_retrieve": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp]),
     "rqb200_sid_topk_rank_hist": (c_int, [c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_vp, c_vp]),
+    "rqb200_sid_rank_hist": (c_int, [c_vp, c_int, c_i64, c_vp, c_vp]),
+    "rqb200_sid_trie_counts": (c_int, [c_vp, c_vp, c_vp]),
+    "rqb200_sid_trie_level": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp]),
+    "rqb200_sid_items_offsets": (c_int, [c_i64, c_int, c_int, ctypes.POINTER(c_size), ctypes.POINTER(c_size)]),
+    "rqb200_t5rank_cross_attention": (c_int, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_i64,
+                                              c_vp]),
+    "rqb200_t5rank_cross_attention_tc": (c_int, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_i64,
+                                                 c_vp]),
+    "rqb200_t5rank_children": (c_int, [c_vp, c_i64, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp]),
+    "rqb200_t5rank_select": (c_int, [c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp]),
     "rqb200_t5dec_cross_attention": (c_int, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_int, c_int, c_int, c_int, c_vp, c_i64,
                                              c_vp]),
     "rqb200_t5dec_self_attention": (c_int, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int,

@@ -418,6 +418,51 @@ extern "C" int rqb200_sid_trie_build(const int64_t* cached_ids, int64_t N, int C
   return RQB_OK;
 }
 
+// The trie's level arrays as plain device arrays, for the exact ranking of modules/model.py (rank_sem_ids), which decodes one
+// row per trie node.  rqb200_sid_trie_counts copies the node counts n[0..C] to a device array (the caller reads them once per
+// index); rqb200_sid_trie_level writes, for level l (1..C), each node's code, its parent in level l - 1 (from the parent's
+// child range) and, for l < C, its child range in level l + 1 (child[n_l + 1]).
+__global__ void sid_trie_counts_kernel(const unsigned char* __restrict__ ws, int* __restrict__ counts) {
+  const SidTrieHeader* hdr = reinterpret_cast<const SidTrieHeader*>(ws);
+  for (int l = threadIdx.x; l <= hdr->C; l += blockDim.x) counts[l] = hdr->n[l];
+}
+
+__global__ void sid_trie_level_kernel(const unsigned char* __restrict__ ws, int l, int n_l, int n_prev, int* __restrict__ code,
+                                      int* __restrict__ parent, int* __restrict__ child) {
+  const SidTrieHeader* hdr = reinterpret_cast<const SidTrieHeader*>(ws);
+  const unsigned short* c = reinterpret_cast<const unsigned short*>(ws + hdr->code[l]);
+  const int* up = reinterpret_cast<const int*>(ws + hdr->child[l - 1]);
+  const int* down = l < hdr->C ? reinterpret_cast<const int*>(ws + hdr->child[l]) : nullptr;
+  const int stride = gridDim.x * blockDim.x;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i <= n_l; i += stride) {
+    if (i < n_l) code[i] = c[i];
+    if (child) child[i] = down ? down[i] : 0;
+  }
+  for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < n_prev; p += stride)
+    for (int j = up[p]; j < up[p + 1]; ++j) parent[j] = p;
+}
+
+extern "C" int rqb200_sid_trie_counts(const void* workspace, int* counts, void* stream) {
+  RQB_CHECK_ARG(workspace && counts, "sid_trie_counts: null pointer");
+  sid_trie_counts_kernel<<<1, 32, 0, reinterpret_cast<cudaStream_t>(stream)>>>(reinterpret_cast<const unsigned char*>(workspace),
+                                                                             counts);
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
+}
+
+extern "C" int rqb200_sid_trie_level(const void* workspace, int C, int l, int n_l, int n_prev, int* code, int* parent, int* child,
+                                     void* stream) {
+  RQB_CHECK_ARG(C > 0 && C <= 8 && l >= 1 && l <= C && n_l >= 0 && n_prev >= 0,
+                "sid_trie_level: bad argument (C = %d, l = %d, n_l = %d, n_prev = %d)", C, l, n_l, n_prev);
+  RQB_CHECK_ARG(workspace && code && parent && (l == C || child), "sid_trie_level: null pointer");
+  int grid = (n_l + 256) / 256;
+  if (grid > 132 * 8) grid = 132 * 8;
+  sid_trie_level_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<const unsigned char*>(workspace), l, n_l, n_prev, code, parent, l < C ? child : nullptr);
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 // Lookups in the trie.  A search kernel tests "the beam's prefix extended by code tok is a corpus prefix" through
 //   parent(ids, h, K)    the walk from the root along the beam's ids [0, h): the range of its children at level h + 1;
@@ -1010,6 +1055,20 @@ extern "C" size_t rqb200_sid_items_workspace_bytes(int64_t N, int C, int K) {
   return sid_items_layout(N, C, K, t) ? 0 : t.sort.end;
 }
 
+// Byte offsets of the row[N] and start[N + 1] arrays in an item table's workspace (host arithmetic, no device): the exact
+// ranking expands its chosen tuples to items through them.  Nonzero outside the table's limits.
+extern "C" int rqb200_sid_items_offsets(int64_t N, int C, int K, size_t* row, size_t* start) {
+  SidItemsLayout t;
+  RQB_CHECK_ARG(row && start, "sid_items_offsets: null pointer");
+  if (sid_items_layout(N, C, K, t) == 1) {                  // 2 (no device to size the sort's scratch) still lays out both
+    rqb_set_error("sid_items_offsets: N = %lld, C = %d, K = %d is outside the item table's limits", (long long)N, C, K);
+    return RQB_ERR_UNSUPPORTED;
+  }
+  *row = t.h.row;
+  *start = t.h.start;
+  return RQB_OK;
+}
+
 __global__ void sid_items_header_kernel(SidItemsHeader h, unsigned char* ws) {
   *reinterpret_cast<SidItemsHeader*>(ws) = h;               // U = 0 and start[0] = 0: the fill pass overwrites both when a row is valid
   reinterpret_cast<int*>(ws + h.start)[0] = 0;
@@ -1270,6 +1329,26 @@ extern "C" int rqb200_sid_topk_rank_hist(const int64_t* actual, int64_t a_stride
   if (grid > 132 * 8) grid = 132 * 8;
   sid_topk_rank_hist_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       actual, a_stride, cand, c_stride, B, k, D, item_mode, reinterpret_cast<unsigned long long*>(hist));
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
+}
+
+// The same histogram from exact ranks (rank_items' target_rank): hist[rank] += 1 for rank in [0, k), hist[k] += 1 otherwise.
+__global__ void sid_rank_hist_kernel(const int64_t* __restrict__ rank, int B, int64_t k, unsigned long long* __restrict__ hist) {
+  for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < B; b += gridDim.x * blockDim.x) {
+    const int64_t r = rank[b];
+    atomicAdd(hist + ((r >= 0 && r < k) ? r : k), 1ull);
+  }
+}
+
+extern "C" int rqb200_sid_rank_hist(const int64_t* rank, int B, int64_t k, int64_t* hist, void* stream) {
+  RQB_CHECK_ARG(B >= 0 && k > 0, "sid_rank_hist: bad argument (B = %d, k = %lld)", B, (long long)k);
+  if (B == 0) return RQB_OK;
+  RQB_CHECK_ARG(rank && hist, "sid_rank_hist: null pointer");
+  int grid = (B + 255) / 256;
+  if (grid > 132 * 8) grid = 132 * 8;
+  sid_rank_hist_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(rank, B, k,
+                                                                                reinterpret_cast<unsigned long long*>(hist));
   RQB_LAUNCH_CHECK();
   return RQB_OK;
 }

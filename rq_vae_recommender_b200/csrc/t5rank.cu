@@ -1,0 +1,522 @@
+// Exact ranking of every corpus item for each history (modules/model.py EncoderDecoderRetrievalModel.rank_sem_ids / rank_items).
+// Items that share an l-prefix share the causal decoder's state at positions 0..l, so one decoder row per node of the corpus
+// trie (ops.SidPrefixIndex, per history) scores every corpus tuple.  The GEMMs are the split-precision tensor-core GEMM of
+// csrc/gemm_tc.cu and the decoder step kernels of csrc/t5dec.cu (add-norm, self-attention through an ancestor table) are reused;
+// these kernels do the rest:
+//
+//   rqb200_t5rank_cross_attention[_tc]  T5 cross-attention of Q queries per history (a trie level: up to tens of thousands) over
+//                                  that history's encoder rows, t5rank_cross_attention_kernel<TF32>: one warpgroup per (64-query
+//                                  tile, head, history), keys streamed through shared memory with an online fp32 softmax.  TF32:
+//                                  64-key tiles, S = Q K^T by wgmma m64n64k8 from shared memory, O += P V with P as the register A
+//                                  operand (the staging of csrc/t5_tc.cuh: a transposing V copy in the 0,2,4,6,1,3,5,7 key order).
+//                                  fp32: the same query tiles on the CUDA cores, 32 keys per tile, the reference of the TF32 one.
+//   rqb200_t5rank_children         after the level's head GEMM: one warp per node row computes the log-sum-exp exactly as
+//                                  sid_beam_topk_kernel does (same formula, same reduction order), then writes every child's
+//                                  score = parent score + (x[code] - lse).  A row with a NaN or +inf logit, or all -inf, is
+//                                  counted and gives its children NaN.
+//   rqb200_t5rank_select           one CTA per history over its U leaf scores: block radix selection of the n best leaves keyed
+//                                  on (score descending, leaf ascending, NaN last), expansion of the chosen leaves to their items
+//                                  in dedup order cut off at n, and the target item's rank as a block count.  No global atomics.
+//
+// Numerics are HF's T5 in eval mode: no 1/sqrt(d) scaling, an additive per-key mask (-FLT_MAX masks a key, as HF's eager mask).
+#include <cfloat>
+
+#include <cub/block/block_reduce.cuh>
+#include <cub/block/block_scan.cuh>
+
+#include "common.cuh"
+#include "t5_tc.cuh"
+
+#define RK_DKV 64
+#define RK_QTILE 64         // queries per CTA
+#define RK_KTILE 32         // keys per shared-memory tile
+#define RK_WARPS 4
+#define RK_QPW (RK_QTILE / RK_WARPS)
+
+__device__ __forceinline__ float rk_warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// ------------------------------------------------------------------------------------------------ cross-attention
+// grid (ceil(Q / 64), heads, B).  Query i of history b is row b * Q + i of q (head n at column n * 64); history b's keys are rows
+// offsets[b] .. offsets[b + 1] - 1 of k / v, with additive key_mask[row] (null: 0).  Warp w owns queries w, w + 4, ... of the tile;
+// in a key tile lane j scores key j, then lane d accumulates output dims d and d + 32.
+template <bool TF32>
+__global__ void __launch_bounds__(RK_WARPS * 32) t5rank_cross_attention_kernel(
+    const float* __restrict__ q, int64_t ldq, const float* __restrict__ k, const float* __restrict__ v, int64_t ldkv,
+    const int* __restrict__ offsets, const float* __restrict__ key_mask, int Q, float* __restrict__ out, int64_t ldo);
+
+template <>
+__global__ void __launch_bounds__(RK_WARPS * 32) t5rank_cross_attention_kernel<false>(
+    const float* __restrict__ q, int64_t ldq, const float* __restrict__ k, const float* __restrict__ v, int64_t ldkv,
+    const int* __restrict__ offsets, const float* __restrict__ key_mask, int Q, float* __restrict__ out, int64_t ldo) {
+  __shared__ float sq[RK_QTILE][RK_DKV];
+  __shared__ float sk[RK_KTILE][RK_DKV + 1];   // +1: lane j reads row j, column d -> distinct banks
+  __shared__ float sv[RK_KTILE][RK_DKV];
+  __shared__ float sbias[RK_KTILE];
+  const int q0 = blockIdx.x * RK_QTILE, n = blockIdx.y, b = blockIdx.z;
+  const int nq = min(RK_QTILE, Q - q0);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t col = (int64_t)n * RK_DKV, qrow0 = (int64_t)b * Q + q0;
+  for (int i = threadIdx.x; i < RK_QTILE * RK_DKV; i += blockDim.x) {
+    const int r = i / RK_DKV, d = i % RK_DKV;
+    sq[r][d] = r < nq ? q[(qrow0 + r) * ldq + col + d] : 0.f;
+  }
+  const int r0 = offsets[b], S = offsets[b + 1] - r0;
+
+  float m[RK_QPW], l[RK_QPW], acc0[RK_QPW], acc1[RK_QPW];
+#pragma unroll
+  for (int t = 0; t < RK_QPW; ++t) { m[t] = -INFINITY; l[t] = 0.f; acc0[t] = 0.f; acc1[t] = 0.f; }
+
+  const float* kb = k + (int64_t)r0 * ldkv + col;
+  const float* vb = v + (int64_t)r0 * ldkv + col;
+  for (int s0 = 0; s0 < S; s0 += RK_KTILE) {
+    __syncthreads();                                        // the previous tile is consumed (and sq is written)
+    for (int i = threadIdx.x; i < RK_KTILE * RK_DKV; i += blockDim.x) {
+      const int j = i / RK_DKV, d = i % RK_DKV, s = s0 + j;
+      sk[j][d] = s < S ? kb[(int64_t)s * ldkv + d] : 0.f;
+      sv[j][d] = s < S ? vb[(int64_t)s * ldkv + d] : 0.f;
+    }
+    if (threadIdx.x < RK_KTILE) {
+      const int s = s0 + threadIdx.x;
+      sbias[threadIdx.x] = s >= S ? -INFINITY : (key_mask ? key_mask[r0 + s] : 0.f);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int t = 0; t < RK_QPW; ++t) {
+      const int qi = warp + t * RK_WARPS;
+      if (qi >= nq) continue;
+      float dot = 0.f;
+#pragma unroll 16
+      for (int d = 0; d < RK_DKV; ++d) dot = fmaf(sq[qi][d], sk[lane][d], dot);
+      const float bias = sbias[lane];
+      const float sc = bias == -INFINITY ? -INFINITY : dot + bias;   // a key past S contributes exp(-inf) = 0
+      const float m_new = fmaxf(m[t], rk_warp_max(sc));              // finite: every tile holds at least one key < S
+      const float alpha = expf(m[t] - m_new);
+      const float p = expf(sc - m_new);
+      l[t] = l[t] * alpha + warp_sum(p);
+      float a0 = acc0[t] * alpha, a1 = acc1[t] * alpha;
+#pragma unroll 8
+      for (int j = 0; j < RK_KTILE; ++j) {
+        const float pj = __shfl_sync(0xffffffffu, p, j);
+        a0 = fmaf(pj, sv[j][lane], a0);
+        a1 = fmaf(pj, sv[j][lane + 32], a1);
+      }
+      acc0[t] = a0;
+      acc1[t] = a1;
+      m[t] = m_new;
+    }
+  }
+#pragma unroll
+  for (int t = 0; t < RK_QPW; ++t) {
+    const int qi = warp + t * RK_WARPS;
+    if (qi >= nq) continue;
+    float* o = out + (qrow0 + qi) * ldo + col;
+    o[lane] = l[t] > 0.f ? acc0[t] / l[t] : 0.f;            // a history without keys gets zeros
+    o[lane + 32] = l[t] > 0.f ? acc1[t] / l[t] : 0.f;
+  }
+}
+
+
+// The TF32 instantiation: the same grid and query tile, dynamic smem 3 tiles (Q, K, transposed V).  Thread (warp w, lane
+// 4 g + t) holds query rows 16 w + g and 16 w + g + 8 of the tile and, of each 8-key block j, key columns 8 j + 2 t, 8 j + 2 t + 1.
+// q, k, v rows must be 16-byte aligned with row strides a multiple of 4 floats.
+extern __shared__ __align__(128) float rk_tc_smem[];
+
+template <>
+__global__ void __launch_bounds__(TC_THREADS) t5rank_cross_attention_kernel<true>(
+    const float* __restrict__ q, int64_t ldq, const float* __restrict__ k, const float* __restrict__ v, int64_t ldkv,
+    const int* __restrict__ offsets, const float* __restrict__ key_mask, int Q, float* __restrict__ out, int64_t ldo) {
+  float* sQ = rk_tc_smem;
+  float* sK = sQ + TC_TILE;
+  float* sVt = sK + TC_TILE;
+  __shared__ float sbias[TC_T];
+  const int q0 = blockIdx.x * TC_T, n = blockIdx.y, b = blockIdx.z;
+  const int nq = min(TC_T, Q - q0);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const int row[2] = {16 * warp + g, 16 * warp + g + 8};
+  const int64_t qrow0 = (int64_t)b * Q + q0;
+  const int r0 = offsets[b], S = offsets[b + 1] - r0;
+  tc_stage(sQ, q + qrow0 * ldq + n * 64, ldq, nq);
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  for (int t0 = 0; t0 < S; t0 += TC_T) {
+    const int nk = min(TC_T, S - t0);
+    __syncthreads();                                          // the previous tile's MMAs have completed in every warp
+    tc_stage(sK, k + (int64_t)(r0 + t0) * ldkv + n * 64, ldkv, nk);
+    tc_stage_t(sVt, v + (int64_t)(r0 + t0) * ldkv + n * 64, ldkv, nk);
+    if (threadIdx.x < TC_T)
+      sbias[threadIdx.x] = (int)threadIdx.x < nk ? (key_mask ? key_mask[r0 + t0 + threadIdx.x] : 0.f) : -INFINITY;
+    tc_proxy_fence();
+    __syncthreads();
+    float s[32];
+    tc_fence();
+    tc_gemm_ss(s, sQ, sK);
+    tc_commit();
+    tc_wait();
+    tc_pin(s);
+    float mt[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const float bias = sbias[8 * j + 2 * t + e];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float& x = s[4 * j + 2 * h + e];
+          x = bias == -INFINITY ? -INFINITY : x + bias;       // a key past the history contributes exp(-inf) = 0
+          mt[h] = fmaxf(mt[h], x);
+        }
+      }
+    float alpha[2], lt[2] = {0.f, 0.f};
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      mt[h] = fmaxf(mt[h], __shfl_xor_sync(0xffffffffu, mt[h], 1));
+      mt[h] = fmaxf(mt[h], __shfl_xor_sync(0xffffffffu, mt[h], 2));
+      const float m_new = fmaxf(m[h], mt[h]);                 // finite: every tile holds at least one key of the history
+      alpha[h] = expf(m[h] - m_new);
+      m[h] = m_new;
+    }
+    uint32_t a[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      const float p = expf(s[i] - m[(i >> 1) & 1]);
+      lt[(i >> 1) & 1] += p;
+      a[i] = tf32_bits(p);
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) l[h] = fmaf(l[h], alpha[h], lt[h]);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      o[4 * j] *= alpha[0];
+      o[4 * j + 1] *= alpha[0];
+      o[4 * j + 2] *= alpha[1];
+      o[4 * j + 3] *= alpha[1];
+    }
+    tc_fence();
+    tc_gemm_rs(o, a, sVt);
+    tc_commit();
+    tc_wait();
+    tc_pin(o);
+    tc_pin(a);
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    l[h] += __shfl_xor_sync(0xffffffffu, l[h], 1);
+    l[h] += __shfl_xor_sync(0xffffffffu, l[h], 2);
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    if (row[h] >= nq) continue;
+    float* orow = out + (qrow0 + row[h]) * ldo + n * 64 + 2 * t;
+    const float inv_ok = l[h] > 0.f ? 1.f : 0.f;              // a history without keys gets zeros
+    const float den = l[h] > 0.f ? l[h] : 1.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      *reinterpret_cast<float2*>(orow + 8 * j) = make_float2(o[4 * j + 2 * h] / den * inv_ok, o[4 * j + 2 * h + 1] / den * inv_ok);
+  }
+}
+
+// cudaFuncSetAttribute once per device and kernel (bit d of *done: device d)
+static int rk_set_smem_once(const void* fn, int bytes, unsigned long long* done) {
+  int dev = 0;
+  RQB_CUDA(cudaGetDevice(&dev));
+  if (dev < 64 && (*done >> dev) & 1ull) return RQB_OK;
+  RQB_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+  if (dev < 64) *done |= 1ull << dev;
+  return RQB_OK;
+}
+
+static int rk_cross_attention(bool tf32, const char* what, const float* q, int64_t ldq, const float* k, const float* v, int64_t ldkv,
+                              const int* offsets, const float* key_mask, int B, int Q, int heads, float* out, int64_t ldo,
+                              void* stream) {
+  RQB_CHECK_ARG(B >= 0 && Q >= 0 && heads > 0 && ldq >= (int64_t)heads * RK_DKV && ldkv >= (int64_t)heads * RK_DKV &&
+                    ldo >= (int64_t)heads * RK_DKV,
+                "%s: bad argument (B = %d, Q = %d, heads = %d)", what, B, Q, heads);
+  if (B > 65535 || heads > 65535) {
+    rqb_set_error("%s: need B <= 65535 and heads <= 65535 (B = %d, heads = %d)", what, B, heads);
+    return RQB_ERR_UNSUPPORTED;
+  }
+  if (B == 0 || Q == 0) return RQB_OK;
+  RQB_CHECK_ARG(q && k && v && offsets && out, "%s: null pointer", what);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const dim3 grid((unsigned)((Q + RK_QTILE - 1) / RK_QTILE), (unsigned)heads, (unsigned)B);
+  if (tf32) {
+    RQB_CHECK_ARG(ldq % 4 == 0 && ldkv % 4 == 0 && ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) |
+                                                      reinterpret_cast<uintptr_t>(v)) & 15) == 0,
+                  "%s: q, k, v must be 16-byte aligned with row strides a multiple of 4", what);
+    static unsigned long long done = 0;
+    const int smem = 3 * TC_TILE * (int)sizeof(float);
+    const int rc = rk_set_smem_once(reinterpret_cast<const void*>(t5rank_cross_attention_kernel<true>), smem, &done);
+    if (rc != RQB_OK) return rc;
+    t5rank_cross_attention_kernel<true><<<grid, TC_THREADS, smem, st>>>(q, ldq, k, v, ldkv, offsets, key_mask, Q, out, ldo);
+  } else {
+    t5rank_cross_attention_kernel<false><<<grid, RK_WARPS * 32, 0, st>>>(q, ldq, k, v, ldkv, offsets, key_mask, Q, out, ldo);
+  }
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
+}
+
+extern "C" int rqb200_t5rank_cross_attention(const float* q, int64_t ldq, const float* k, const float* v, int64_t ldkv,
+                                             const int* offsets, const float* key_mask, int B, int Q, int heads, float* out,
+                                             int64_t ldo, void* stream) {
+  return rk_cross_attention(false, "t5rank_cross_attention", q, ldq, k, v, ldkv, offsets, key_mask, B, Q, heads, out, ldo, stream);
+}
+
+extern "C" int rqb200_t5rank_cross_attention_tc(const float* q, int64_t ldq, const float* k, const float* v, int64_t ldkv,
+                                                const int* offsets, const float* key_mask, int B, int Q, int heads, float* out,
+                                                int64_t ldo, void* stream) {
+  return rk_cross_attention(true, "t5rank_cross_attention_tc", q, ldq, k, v, ldkv, offsets, key_mask, B, Q, heads, out, ldo,
+                            stream);
+}
+
+// ------------------------------------------------------------------------------------------------ children scores
+// One warp per node row r = b * n_h + i of logits [R, K].  lse as sid_beam_topk_kernel: m = max, sum of expf(x - m) over c = lane,
+// lane + 32, ... then an xor butterfly (every lane ends with the same bits), lse = m + logf(sum).  Child j of node i (child[i] <=
+// j < child[i + 1], a node of level h + 1) gets out[b * n_next + j] = (x[code[j]] - lse) + parent[r] with explicit roundings.
+__global__ void __launch_bounds__(256) t5rank_children_kernel(const float* __restrict__ logits, int64_t ld, int R, int K, int n_h,
+                                                              const float* __restrict__ parent, const int* __restrict__ child,
+                                                              const int* __restrict__ code, int n_next, float* __restrict__ out,
+                                                              int* __restrict__ bad) {
+  const int64_t r = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (r >= R) return;
+  const int64_t b = r / n_h;
+  const int i = (int)(r - b * n_h);
+  const float* x = logits + r * ld;
+  float m = -INFINITY;
+  bool odd = false;
+  for (int c = lane; c < K; c += 32) {
+    const float val = x[c];
+    m = fmaxf(m, val);
+    odd |= val != val || val == INFINITY;
+  }
+  m = rk_warp_max(m);
+  odd = __any_sync(0xffffffffu, odd);
+  float sum = 0.f;
+  for (int c = lane; c < K; c += 32) sum += expf(x[c] - m);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+  const float lse = m + logf(sum);
+  const bool nonfinite = odd || m == -INFINITY;
+  if (nonfinite && lane == 0 && bad) atomicAdd(bad, 1);
+  const float ps = parent ? parent[r] : 0.f;
+  float* o = out + b * n_next;
+  for (int j = child[i] + lane; j < child[i + 1]; j += 32)
+    o[j] = nonfinite ? __int_as_float(0x7fffffff) : __fadd_rn(__fsub_rn(x[code[j]], lse), ps);
+}
+
+extern "C" int rqb200_t5rank_children(const float* logits, int64_t ld, int R, int K, int n_h, const float* parent, const int* child,
+                                      const int* code, int n_next, float* out, int* bad, void* stream) {
+  RQB_CHECK_ARG(R >= 0 && K > 0 && n_h > 0 && n_next >= 0 && ld >= K && R % n_h == 0,
+                "t5rank_children: bad argument (R = %d, K = %d, n_h = %d, n_next = %d)", R, K, n_h, n_next);
+  if (R == 0) return RQB_OK;
+  RQB_CHECK_ARG(logits && child && code && out, "t5rank_children: null pointer");
+  const int rows_per_block = 8;
+  t5rank_children_kernel<<<(R + rows_per_block - 1) / rows_per_block, rows_per_block * 32, 0,
+                           reinterpret_cast<cudaStream_t>(stream)>>>(logits, ld, R, K, n_h, parent, child, code, n_next, out, bad);
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ per-history selection
+// Order key of a leaf: its score's order-preserving 32-bit image (-0 folded into +0, NaN mapped to 0, below every number) above
+// 0xffffffff - leaf, so keys are distinct and "descending key" is (score descending, leaf ascending, NaN last).
+#define RK_SEL_THREADS 512
+#define RK_SEL_MAX_N 1024
+#define RK_SEL_SMEM_KEYS (24 * 1024)
+
+__device__ __forceinline__ unsigned int rk_score_key(float v) {
+  if (v != v) return 0u;
+  const unsigned int x = __float_as_uint(v == 0.f ? 0.f : v);
+  return x ^ ((x & 0x80000000u) ? 0xffffffffu : 0x80000000u);
+}
+
+__device__ __forceinline__ unsigned long long rk_key64(unsigned int key, int leaf) {
+  return ((unsigned long long)key << 32) | (unsigned int)(0xffffffffu - (unsigned int)leaf);
+}
+
+template <bool KEYS_IN_SMEM>
+__global__ void __launch_bounds__(RK_SEL_THREADS) t5rank_select_kernel(
+    const float* __restrict__ scores, int U, const int* __restrict__ row, const int* __restrict__ start,
+    const int64_t* __restrict__ t_leaf, const int64_t* __restrict__ t_dedup, int n, int64_t* __restrict__ out_items,
+    float* __restrict__ out_scores, int64_t* __restrict__ out_rank) {
+  using Scan = cub::BlockScan<int, RK_SEL_THREADS>;
+  using Reduce = cub::BlockReduce<long long, RK_SEL_THREADS>;
+  __shared__ union {
+    typename Scan::TempStorage scan;
+    typename Reduce::TempStorage reduce;
+  } tmp;
+  __shared__ int hist[256];
+  __shared__ int ctl[3];                                    // chosen digit, entries above its bin, entries in its bin
+  __shared__ int nsel_at, ties_base;
+  __shared__ unsigned long long sel[RK_SEL_MAX_N];
+  __shared__ int s_leaf[RK_SEL_MAX_N];
+  __shared__ int s_off[RK_SEL_MAX_N + 1];
+  extern __shared__ __align__(16) unsigned int s_key[];     // [U] when KEYS_IN_SMEM
+  const int nt = RK_SEL_THREADS, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const unsigned int lt = (1u << lane) - 1u;
+  const int64_t b = blockIdx.x;
+  const float* sc = scores + b * U;
+  const int nsel = min(n, U);
+  for (int i = threadIdx.x; i < 256; i += nt) hist[i] = 0;
+  if (threadIdx.x == 0) {
+    nsel_at = 0;
+    ties_base = 0;
+  }
+  if (KEYS_IN_SMEM)
+    for (int u = threadIdx.x; u < U; u += nt) s_key[u] = rk_score_key(sc[u]);
+  __syncthreads();
+  // radix selection of the nsel-th largest 32-bit score key (8-bit digits, stops once the chosen bin is taken whole)
+  unsigned int prefix = 0, pmask = 0;
+  int want = nsel;
+  for (int shift = 24; shift >= 0 && nsel > 0; shift -= 8) {
+    for (int base = 0; base < U; base += nt) {
+      const int u = base + threadIdx.x;
+      int d = 256;
+      if (u < U) {
+        const unsigned int key = KEYS_IN_SMEM ? s_key[u] : rk_score_key(sc[u]);
+        if ((key & pmask) == prefix) d = (int)((key >> shift) & 255u);
+      }
+      const unsigned int same = __match_any_sync(0xffffffffu, d);
+      if (d < 256 && (same & lt) == 0) atomicAdd(&hist[d], __popc(same));   // integer counts: order does not matter
+    }
+    __syncthreads();
+    if (w == 0) {
+      int c[8], sum = 0;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        c[j] = hist[lane * 8 + j];
+        hist[lane * 8 + j] = 0;
+        sum += c[j];
+      }
+      int suf = sum;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_down_sync(0xffffffffu, suf, o);
+        if (lane + o < 32) suf += t;
+      }
+      const int owner = 31 - __clz(__ballot_sync(0xffffffffu, suf >= want));
+      if (lane == owner) {
+        int acc = suf - sum;
+        for (int j = 7; j >= 0; --j) {
+          if (acc + c[j] >= want) {
+            ctl[0] = lane * 8 + j;
+            ctl[1] = acc;
+            ctl[2] = c[j];
+            break;
+          }
+          acc += c[j];
+        }
+      }
+    }
+    __syncthreads();
+    want -= ctl[1];
+    prefix |= (unsigned int)ctl[0] << shift;
+    pmask |= 255u << shift;
+    const bool whole = ctl[2] == want;
+    __syncthreads();                                        // ctl is read by every thread before the next pass writes it
+    if (whole) break;
+  }
+  // keep every leaf above the threshold and the `want` lowest-index leaves at it (an ordered block scan over the ties), and count
+  // the items of the leaves that sort before the target
+  const int64_t tl = t_leaf[b];
+  const int64_t td = t_dedup[b];
+  const bool t_ok = tl >= 0 && tl < U && td >= 0 && td < (int64_t)(start[tl + 1] - start[tl]);
+  const unsigned long long t_key = t_ok ? rk_key64(KEYS_IN_SMEM ? s_key[tl] : rk_score_key(sc[tl]), (int)tl) : 0ull;
+  long long before = 0;
+  for (int base = 0; base < U; base += nt) {
+    const int u = base + threadIdx.x;
+    unsigned int key = 0;
+    if (u < U) key = KEYS_IN_SMEM ? s_key[u] : rk_score_key(sc[u]);
+    const bool in = u < U && nsel > 0;
+    const bool above = in && (key & pmask) > prefix;
+    const int tie = (in && (key & pmask) == prefix) ? 1 : 0;
+    int excl, total;
+    Scan(tmp.scan).ExclusiveSum(tie, excl, total);
+    const bool take = above || (tie && ties_base + excl < want);
+    if (take) {
+      const int at = atomicAdd(&nsel_at, 1);                // a slot only: the final order is each key's rank below
+      sel[at] = rk_key64(key, u);
+    }
+    if (t_ok && u < U && rk_key64(key, u) > t_key) before += start[u + 1] - start[u];
+    __syncthreads();                                        // scan storage and ties_base reused
+    if (threadIdx.x == 0) ties_base += total;
+    __syncthreads();
+  }
+  const long long items_before = Reduce(tmp.reduce).Sum(before);
+  __syncthreads();
+  // rank each kept key among the kept ones (distinct keys), then each leaf's item count, scanned in rank order
+  for (int i = threadIdx.x; i < nsel; i += nt) {
+    const unsigned long long key = sel[i];
+    int r = 0;
+    for (int j = 0; j < nsel; ++j) r += sel[j] > key;
+    s_leaf[r] = (int)(0xffffffffu - (unsigned int)(key & 0xffffffffull));
+  }
+  __syncthreads();
+  constexpr int PER = RK_SEL_MAX_N / RK_SEL_THREADS;
+  int cnt[PER], off[PER], total;
+#pragma unroll
+  for (int i = 0; i < PER; ++i) {
+    const int j = threadIdx.x * PER + i;
+    cnt[i] = j < nsel ? start[s_leaf[j] + 1] - start[s_leaf[j]] : 0;
+  }
+  Scan(tmp.scan).ExclusiveSum(cnt, off, total);
+#pragma unroll
+  for (int i = 0; i < PER; ++i) {
+    const int j = threadIdx.x * PER + i;
+    if (j < nsel) s_off[j] = off[i];
+  }
+  __syncthreads();
+  const int mcount = min(total, n);
+  for (int o = threadIdx.x; o < n; o += nt) {
+    int64_t item = -1;
+    float s = -INFINITY;
+    if (o < mcount) {                                       // s_off[lo] <= o < s_off[lo + 1]: leaf lo holds slot o
+      int lo = 0, hi = nsel;
+      while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (s_off[mid] <= o) lo = mid;
+        else hi = mid;
+      }
+      const int leaf = s_leaf[lo];
+      item = row[start[leaf] + (o - s_off[lo])];
+      s = sc[leaf];
+    }
+    out_items[b * n + o] = item;
+    out_scores[b * n + o] = s;
+  }
+  if (threadIdx.x == 0) out_rank[b] = t_ok ? (int64_t)items_before + td : -1;
+}
+
+extern "C" int rqb200_t5rank_select(const float* scores, int B, int U, const int* row, const int* start, const int64_t* t_leaf,
+                                    const int64_t* t_dedup, int n, int64_t* out_items, float* out_scores, int64_t* out_rank,
+                                    void* stream) {
+  RQB_CHECK_ARG(B >= 0 && U >= 0 && n > 0, "t5rank_select: bad argument (B = %d, U = %d, n = %d)", B, U, n);
+  if (n > RK_SEL_MAX_N) {
+    rqb_set_error("t5rank_select: need n <= %d (n = %d)", RK_SEL_MAX_N, n);
+    return RQB_ERR_UNSUPPORTED;
+  }
+  if (B == 0) return RQB_OK;
+  RQB_CHECK_ARG((scores || U == 0) && start && (row || U == 0) && t_leaf && t_dedup && out_items && out_scores && out_rank,
+                "t5rank_select: null pointer");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (U <= RK_SEL_SMEM_KEYS) {
+    const size_t smem = (size_t)U * sizeof(unsigned int);
+    static unsigned long long done = 0;
+    const int rc = rk_set_smem_once(reinterpret_cast<const void*>(t5rank_select_kernel<true>),
+                                    RK_SEL_SMEM_KEYS * (int)sizeof(unsigned int), &done);
+    if (rc != RQB_OK) return rc;
+    t5rank_select_kernel<true><<<B, RK_SEL_THREADS, smem, st>>>(scores, U, row, start, t_leaf, t_dedup, n, out_items, out_scores,
+                                                               out_rank);
+  } else {
+    t5rank_select_kernel<false><<<B, RK_SEL_THREADS, 0, st>>>(scores, U, row, start, t_leaf, t_dedup, n, out_items, out_scores,
+                                                             out_rank);
+  }
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
+}

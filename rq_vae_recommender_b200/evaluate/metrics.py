@@ -8,7 +8,9 @@ none is -- to an int64 histogram on the device in one launch (``ops.sid_topk_ran
     ndcg = sum_r hist[r] / log2(r + 2) / total,    h@j = sum_{r < j} hist[r] / total.
 ``accumulate_items`` is an addition: it scores lists of corpus items (``EncoderDecoderRetrievalModel.generate_items``) against the
 true next item (``EncoderDecoderRetrievalModel.item_of``) in separate histograms, reported as ``item_ndcg`` and ``item_h@{k}``.
-There a -1 (padding, an item that could not be resolved) never matches.  The reference's keys are unchanged.
+There a -1 (padding, an item that could not be resolved) never matches.  ``accumulate_ranks`` is another addition: exact ranks
+(``EncoderDecoderRetrievalModel.rank_items``' target_rank, -1 a miss) in a third histogram, reported as ``exact_ndcg`` and
+``exact_h@{k}``.  The reference's keys are unchanged.
 """
 from typing import Dict
 from typing import Sequence
@@ -39,7 +41,8 @@ class TopKAccumulator:
     def reset(self):
         self.total = 0
         self.item_total = 0
-        self._hists = {}                                     # (item_mode, k, device) -> int64 [k + 1] device histogram
+        self.exact_total = 0
+        self._hists = {}                                     # (mode, k, device) -> int64 [k + 1] device histogram
 
     def _add(self, actual: Tensor, candidates: Tensor, item_mode: bool) -> None:
         key = (item_mode, candidates.shape[1], candidates.device)
@@ -61,6 +64,17 @@ class TopKAccumulator:
         self._add(actual, retrieved_items.reshape(actual.shape[0], -1).unsqueeze(-1), True)
         self.item_total += actual.shape[0]
 
+    def accumulate_ranks(self, rank: Tensor, num_items: int) -> None:
+        """rank [B] int64: exact 0-based ranks among num_items ranked items (-1: a miss), e.g. ``rank_items``' target_rank and
+        num_items.  One launch into a histogram of num_items + 1 bins, no host synchronisation."""
+        rank = rank.reshape(-1)
+        key = ("exact", max(1, int(num_items)), rank.device)
+        hist = self._hists.get(key)
+        if hist is None:
+            hist = self._hists[key] = torch.zeros(key[1] + 1, dtype=torch.int64, device=rank.device)
+        ops.sid_rank_hist(rank, hist)
+        self.exact_total += rank.shape[0]
+
     def reduce(self) -> dict:
         if not self._hists:
             return {}
@@ -68,7 +82,8 @@ class TopKAccumulator:
         dev = keys[0][2]
         flat = torch.cat([self._hists[key].to(dev) for key in keys]).cpu().numpy()   # the one wait on the device
         out = {}
-        for item_mode, prefix, total in ((False, "", self.total), (True, "item_", self.item_total)):
+        for item_mode, prefix, total in ((False, "", self.total), (True, "item_", self.item_total),
+                                         ("exact", "exact_", self.exact_total)):
             parts, at = [], 0
             for key in keys:
                 k = key[1]

@@ -37,6 +37,9 @@ backward and HF's dropout; ``DEFAULT_FORWARD_ENCODER`` ("hf") picks it when none
 sets it).  ``forward(batch, decoder="fused")`` runs the decoder as ``FusedT5DecodeTrain``: the H positions the loss reads, on the
 decoder training kernels of csrc/t5dec.cu with HF's dropout; ``DEFAULT_FORWARD_DECODER`` ("hf") picks it when none is given
 (``dropin.install(forward_decoder=...)`` sets it).  With both fused, the decoder attends to the encoder's packed rows.
+
+``rank_items`` / ``rank_sem_ids`` are an evaluation tool with no search: every corpus item is scored by its exact
+log-probability, one decoder row per corpus-trie node per history (``FusedT5Rank``, csrc/t5rank.cu), and ranked.
 """
 from typing import NamedTuple
 from typing import Optional
@@ -188,6 +191,111 @@ class FusedT5Decode:
         return nrm
 
 
+class ItemRankingOutput(NamedTuple):
+    """rank_items: the n best corpus items of each history by exact log-probability (item_ids [B, n] int64, -1 past the corpus),
+    their log-probabilities (scores [B, n] fp32, -inf past the corpus), the true next item's 0-based rank among every retrievable
+    item (target_rank [B] int64, -1 when it is not retrievable) and the number of retrievable items ranked (num_items)."""
+    item_ids: Tensor
+    scores: Tensor
+    target_rank: Tensor
+    num_items: int
+
+
+#: device bytes one chunk of histories of rank_sem_ids / rank_items is sized to when max_rows is not given
+RANK_BYTE_BUDGET = 4 << 30
+#: most items rank_items returns per history
+MAX_RANK_ITEMS = 1024
+
+
+class FusedT5Rank:
+    """The decoder passes of ``rank_sem_ids``: one decoder row per node of the corpus trie per history.  Items that share an
+    l-prefix share the causal decoder's state at positions 0..l, so level h's rows (one per h-prefix node; the root at h = 0) give
+    every child's log-probability, and a leaf's score is the sum along its path.  The maths are ``FusedT5Decode``'s (eval mode,
+    no 1/sqrt(d), block 0's relative bias), with
+      * ``t5dec_add_norm`` gathering ``item_sid_embedding_table[code + (h - 1) K]`` for node rows;
+      * ``t5dec_self_attention`` reading ancestors through the table that each level advances from the node parents, with cache
+        slots sized to the largest level of the chunk;
+      * every GEMM on the split-precision tensor-core GEMM (``ops.gemm_split``: fp32-accurate, each output row a function of its
+        input row alone), so the chunking of histories does not change a bit;
+      * cross keys and values projected once for all histories (one GEMM per call), and ``t5rank_cross_attention`` for the level's
+        n_h queries per history over the encoder rows given by offsets and an additive per-row key mask, fp32 on the CUDA cores or
+        (``attention="tf32"``) its products on the TF32 tensor cores;
+      * after each level's head, ``t5rank_children`` (log-sum-exp as the beam search, child score = parent + log-probability)."""
+
+    def __init__(self, model: "EncoderDecoderRetrievalModel", levels: ops.SidTrieLevels, rows: Tensor, offsets: Tensor,
+                 key_mask: Tensor, attention: str = "fp32"):
+        dec = model.t5_decoder
+        _check_encoder_config(dec.config, "rank_sem_ids")
+        self.model, self.levels, self.H = model, levels, model.num_hierarchies
+        self.tf32 = _check_attention(attention) == "tf32"
+        self.heads, self.eps = dec.config.num_heads, dec.config.layer_norm_epsilon
+        self.inner = self.heads * ops.T5_DKV
+        self.blocks = [blk.layer for blk in dec.block]
+        self.norms = [w for lay in self.blocks for w in (lay[0].layer_norm.weight, lay[1].layer_norm.weight,
+                                                         lay[2].layer_norm.weight)] + [dec.final_layer_norm.weight]
+        w = ops.SplitOperand
+        #: per layer, the split images of (qkv, self o, cross q, cross o, wi, wo); then each level's head
+        self.w = [(w(torch.cat([lay[0].SelfAttention.q.weight, lay[0].SelfAttention.k.weight, lay[0].SelfAttention.v.weight])),
+                   w(lay[0].SelfAttention.o.weight), w(lay[1].EncDecAttention.q.weight), w(lay[1].EncDecAttention.o.weight),
+                   w(lay[2].DenseReluDense.wi.weight), w(lay[2].DenseReluDense.wo.weight)) for lay in self.blocks]
+        self.heads_w = [w(mlp.weight) for mlp in model.decoder_mlp]
+        w_kv = torch.cat([t for lay in self.blocks for t in (lay[1].EncDecAttention.k.weight, lay[1].EncDecAttention.v.weight)])
+        #: [rows, layers * 2 * inner]: layer l's cross keys at columns 2 l inner, its values at (2 l + 1) inner
+        self.cross_kv = ops.gemm_split(rows, w(w_kv))
+        self.offsets, self.key_mask = offsets, key_mask
+        self.bias = dec.block[0].layer[0].SelfAttention.compute_bias(self.H, self.H)[0].contiguous()
+        self.width = max(levels.n[:self.H])
+        self.codes = [None] + [levels.code[h].long() for h in range(1, self.H)]
+
+    @staticmethod
+    def row_bytes(model: "EncoderDecoderRetrievalModel") -> int:
+        """Device bytes one node row of the widest level holds while a chunk runs: its self-attention cache (layers x k, v x H
+        slots x inner fp32), the activations of one layer (x, norm, qkv, attention, projection, feed-forward, head logits) and
+        its ids, parent and ancestor entries."""
+        cfg = model.t5_decoder.config
+        inner, d, H = cfg.num_heads * ops.T5_DKV, cfg.d_model, model.num_hierarchies
+        floats = cfg.num_layers * 2 * H * inner + 3 * d + 5 * inner + cfg.d_ff + model.num_embeddings_per_hierarchy + 1
+        return 4 * floats + 16 + 8 * H
+
+    def run(self, b0: int, b1: int, out: Tensor, bad: Tensor) -> None:
+        """Leaf scores of histories b0 .. b1 - 1 into out[b0:b1] ([B, U])."""
+        m, eps, inner, lv, H = self.model, self.eps, self.inner, self.levels, self.H
+        Bc, dev = b1 - b0, self.cross_kv.device
+        rows = Bc * self.width
+        cache = torch.empty((len(self.blocks), 2, H, rows, inner), dtype=torch.float32, device=dev)
+        anc = torch.zeros((rows, H), dtype=torch.int32, device=dev)
+        anc_next = torch.empty_like(anc)
+        offsets = self.offsets[b0:b1 + 1]
+        score = None
+        for h in range(H):
+            n_h = lv.n[h]
+            R = Bc * n_h
+            x = torch.empty((R, m.bos_token.shape[1]), dtype=torch.float32, device=dev)
+            nrm = torch.empty_like(x)
+            parent = None
+            if h == 0:
+                ops.t5dec_add_norm(x, None, self.norms[0], nrm, eps, emb=m.bos_token)
+            else:
+                ops.t5dec_add_norm(x, None, self.norms[0], nrm, eps, emb=m.item_sid_embedding_table.weight,
+                                   ids=self.codes[h].repeat(Bc), offset=(h - 1) * m.num_embeddings_per_hierarchy)
+                parent = (torch.arange(Bc, device=dev)[:, None] * lv.n[h - 1] + lv.parent[h].long()[None, :]).reshape(R)
+            for l, (w_qkv, w_o, w_q, w_xo, w_i, w_fo) in enumerate(self.w):
+                advance = parent is not None and l == 0
+                a = ops.t5dec_self_attention(ops.gemm_split(nrm, w_qkv), cache[l, 0], cache[l, 1], self.bias, h, anc,
+                                             parent if advance else None, anc_next if advance else None)
+                if advance:
+                    anc, anc_next = anc_next, anc
+                ops.t5dec_add_norm(x, ops.gemm_split(a, w_o), self.norms[3 * l + 1], nrm, eps)
+                kv = self.cross_kv[:, 2 * l * inner:(2 * l + 2) * inner]
+                a = ops.t5rank_cross_attention(ops.gemm_split(nrm, w_q), kv[:, :inner], kv[:, inner:], offsets, self.key_mask,
+                                               n_h, self.heads, tf32=self.tf32)
+                ops.t5dec_add_norm(x, ops.gemm_split(a, w_xo), self.norms[3 * l + 2], nrm, eps)
+                ops.t5dec_add_norm(x, ops.gemm_split(ops.gemm_split(nrm, w_i, relu=True), w_fo), self.norms[3 * l + 3], nrm, eps)
+            nxt = out[b0:b1] if h == H - 1 else torch.empty((Bc, lv.n[h + 1]), dtype=torch.float32, device=dev)
+            ops.t5rank_children(ops.gemm_split(nrm, self.heads_w[h]), score, lv.child[h], lv.code[h + 1], n_h, nxt, bad)
+            score = nxt
+
+
 def _encoder_attention(encoder: str, encoder_attention: Optional[str], what: str) -> str:
     """The fused encoder's attention precision of one call: ``encoder_attention``, else ``DEFAULT_ENCODER_ATTENTION``.  An explicit
     "tf32" with encoder="hf" raises: HF's attention runs at torch's matmul precision, and the switch would be ignored."""
@@ -242,6 +350,12 @@ class FusedT5Encode:
         self.n_kept = None
 
     def __call__(self, attention_mask: Tensor, input_ids: Tensor, user_id: Optional[Tensor] = None):
+        nrm, slot, enc_mask = self.packed(attention_mask, input_ids, user_id)
+        return ops.t5enc_scatter(nrm, slot), enc_mask
+
+    def packed(self, attention_mask: Tensor, input_ids: Tensor, user_id: Optional[Tensor] = None):
+        """The pass without the scatter: (the kept rows [N, d_model], slot [B, S], enc_mask [B, S]); ``offsets``, ``key_mask``
+        and ``src`` of the packing are left on the object."""
         m, eps = self.model, self.eps
         H = m.num_hierarchies
         sep = m.sep_token is not None
@@ -253,7 +367,8 @@ class FusedT5Encode:
             enc_mask = torch.cat([items, items[:, :, -1:]], dim=2).reshape(B, n // H * (H + 1))
         if user:
             enc_mask = torch.cat([torch.ones(B, 1, device=enc_mask.device), enc_mask], dim=1)
-        self.offsets, key_mask = ops.t5enc_offsets(attention_mask, H, sep, user)
+        self.offsets, self.key_mask = ops.t5enc_offsets(attention_mask, H, sep, user)
+        key_mask = self.key_mask
         self.n_kept = _read_n_kept(self.offsets)
         x, nrm, self.src, slot = ops.t5enc_assemble(
             attention_mask, input_ids, user_id if user else None, m.item_sid_embedding_table.weight, m.sep_token if sep else None,
@@ -266,7 +381,7 @@ class FusedT5Encode:
             ops.t5dec_add_norm(x, F.linear(a, lay[0].SelfAttention.o.weight), self.norms[2 * l + 1], nrm, eps)
             ff = lay[1].DenseReluDense
             ops.t5dec_add_norm(x, F.linear(F.linear(nrm, ff.wi.weight).relu_(), ff.wo.weight), self.norms[2 * l + 2], nrm, eps)
-        return ops.t5enc_scatter(nrm, slot), enc_mask
+        return nrm, slot, enc_mask
 
 
 def _encoder_layout(n: int, H: int, sep: bool, user: bool, device) -> Tensor:
@@ -868,3 +983,127 @@ class EncoderDecoderRetrievalModel(nn.Module):
         when the tuple is not in the corpus or the dedup rank exceeds its items."""
         H = self.num_hierarchies
         return self._item_table(sem_ids_fut.device).lookup(sem_ids_fut[:, :H + 1], with_dedup=True)
+
+    # ------------------------------------------------------------------------------------------------ exact ranking
+    def _rank_levels(self, device: torch.device):
+        """(trie levels, leaf keys int64 [U], retrievable items) of the prefix index, built once per index and cached on it.  The
+        node counts and the item count are read on the host here, in one read.  The leaves of level H are the item table's U
+        tuples in the same (lexicographic) order: both hold the distinct tuples of the rows whose first H ids are in [0, K)."""
+        index = self._prefix_index(device)
+        H, K = self.num_hierarchies, self.num_embeddings_per_hierarchy
+        state = getattr(index, "_rank_state", None)
+        if state is None or state[0] != H:
+            if index.C < H:
+                raise Rqb200Error(f"rank_sem_ids: the corpus table has {index.C} id columns, fewer than {H} levels")
+            if H * max(1, (K - 1).bit_length()) > 62:
+                raise Rqb200Error(f"rank_sem_ids: {H} levels of {K} codes do not pack into a 64-bit tuple key")
+            cb = self.codebooks[:, :H].to(device)
+            n_items = ((cb >= 0) & (cb < K)).all(1).sum()
+            host = torch.cat([index.counts().long(), n_items.view(1)]).tolist()   # the one host read of the ranking
+            levels = index.levels(host[:-1])
+            key = levels.code[1].long()
+            for l in range(2, H + 1):
+                key = key[levels.parent[l].long()] * K + levels.code[l]
+            state = index._rank_state = (H, levels, key, int(host[-1]))
+        return state[1:]
+
+    def _leaf_of(self, tuples: Tensor, leaf_key: Tensor) -> Tensor:
+        """int64 [B]: the leaf (item-table tuple) of each row of tuples [B, H], -1 when it holds an id outside [0, K) or is not in
+        the corpus."""
+        K, U = self.num_embeddings_per_hierarchy, leaf_key.shape[0]
+        t = tuples.long()
+        if U == 0:
+            return torch.full((t.shape[0],), -1, dtype=torch.int64, device=t.device)
+        valid = ((t >= 0) & (t < K)).all(1)
+        key = torch.zeros(t.shape[0], dtype=torch.int64, device=t.device)
+        for h in range(t.shape[1]):
+            key = key * K + t[:, h].clamp(0, K - 1)
+        idx = torch.searchsorted(leaf_key, key).clamp_(max=U - 1)
+        return torch.where(valid & (leaf_key[idx] == key), idx, -1)
+
+    def _leaf_scores(self, attention_mask, input_ids, user_id, encoder, encoder_attention, attention, max_rows, what: str):
+        if self.training:
+            raise ValueError(f"{what} runs the model in eval mode only; call model.eval() first (in training mode HF's passes "
+                             "apply dropout)")
+        if torch.is_autocast_enabled("cuda"):
+            raise ValueError(f"{what} runs fp32 kernels: it cannot run inside an autocast region")
+        encoder = DEFAULT_ENCODER if encoder is None else encoder
+        if encoder not in ENCODERS:
+            raise ValueError(f"{what}: encoder must be one of {ENCODERS}, got {encoder!r}")
+        att = _encoder_attention(encoder, encoder_attention, what)
+        attention = "fp32" if attention is None else attention
+        if attention not in ENCODER_ATTENTIONS:
+            raise ValueError(f"{what}: attention must be one of {ENCODER_ATTENTIONS}, got {attention!r}")
+        dev = attention_mask.device
+        levels, leaf_key, n_items = self._rank_levels(dev)
+        H, B = self.num_hierarchies, attention_mask.shape[0]
+        U = levels.n[H]
+        per_history = sum(levels.n[:H])
+        if max_rows is None:
+            max_rows = max(per_history, RANK_BYTE_BUDGET // FusedT5Rank.row_bytes(self))
+        elif max_rows < per_history:
+            raise ValueError(f"{what}: max_rows = {max_rows} is below the {per_history} decoder rows of one history")
+        bad = torch.zeros(1, dtype=torch.int32, device=dev)
+        scores = torch.empty((B, U), dtype=torch.float32, device=dev)
+        if B == 0 or U == 0:
+            return scores, bad, leaf_key, n_items
+        if encoder == "fused":
+            enc = self._fused_encoder(att)
+            rows, slot, _ = enc.packed(attention_mask, input_ids, user_id)
+            offsets = enc.offsets
+            key_mask = enc.key_mask.index_select(0, torch.div(enc.src, slot.shape[1], rounding_mode="floor").long())
+        else:
+            enc_out, enc_mask = self.encoder_forward_pass(attention_mask=attention_mask, input_ids=input_ids, user_id=user_id)
+            S, d = enc_out.shape[1], enc_out.shape[2]
+            rows = enc_out.reshape(B * S, d)
+            offsets = torch.arange(0, (B + 1) * S, S, dtype=torch.int32, device=dev)
+            key_mask = torch.where(enc_mask == 0, torch.finfo(torch.float32).min, 0.0).to(torch.float32).reshape(B * S)
+        ranker = FusedT5Rank(self, levels, rows, offsets, key_mask, attention)
+        chunk = max_rows // per_history
+        for b0 in range(0, B, chunk):
+            ranker.run(b0, min(B, b0 + chunk), scores, bad)
+        return scores, bad, leaf_key, n_items
+
+    @staticmethod
+    def _raise_bad(bad: Tensor, what: str) -> None:
+        n_bad = int(bad[0])
+        if n_bad:
+            raise RuntimeError(f"{what}: {n_bad} decoder row(s) of the head's logits hold a NaN or +inf or are all -inf; the "
+                               "items below them score NaN")
+
+    @torch.no_grad()
+    def rank_sem_ids(self, attention_mask, input_ids, user_id=None, encoder: Optional[str] = None,
+                     encoder_attention: Optional[str] = None, attention: Optional[str] = None,
+                     max_rows: Optional[int] = None) -> Tensor:
+        """fp32 [B, U]: the exact log-probability of every retrievable corpus tuple (U distinct tuples, in the item table's
+        lexicographic order) for each history: sum over levels of log_softmax(decoder_mlp[h](dec_h))[c_h], with the per-row
+        log-sum-exp of the beam search.  One decoder row per corpus-trie node per history (``FusedT5Rank``), histories in chunks of
+        at most ``max_rows`` decoder rows (default: ``RANK_BYTE_BUDGET`` bytes of decoder state); chunking does not change a bit.
+        ``encoder`` / ``encoder_attention`` as in ``generate``; ``attention`` the cross-attention's precision: "fp32" (default) or
+        "tf32" (its products on the TF32 tensor cores).  The GEMMs are fp32-accurate whatever torch's matmul precision.  Eval mode only, no autocast, no random draws.  Raises
+        ``RuntimeError`` after the pass when some head row was not finite (its items score NaN).  An evaluation tool: it runs a
+        decoder row per trie node, thousands of times ``generate``'s work."""
+        scores, bad, _, _ = self._leaf_scores(attention_mask, input_ids, user_id, encoder, encoder_attention, attention,
+                                               max_rows, "rank_sem_ids")
+        self._raise_bad(bad, "rank_sem_ids")
+        return scores
+
+    @torch.no_grad()
+    def rank_items(self, batch: TokenizedSeqBatch, n: Optional[int] = None, encoder: Optional[str] = None,
+                   encoder_attention: Optional[str] = None, attention: Optional[str] = None,
+                   max_rows: Optional[int] = None) -> ItemRankingOutput:
+        """Every retrievable corpus item ranked for each history by the model's exact log-probability (``rank_sem_ids``): the n
+        best (default top_k_for_generation, at most ``MAX_RANK_ITEMS``) and the rank of ``item_of(batch.sem_ids_fut)``.  Order:
+        score descending, then tuple (lexicographic), then dedup rank; NaN last.  One selection launch after the decoder."""
+        n = self.top_k_for_generation if n is None else int(n)
+        if not 1 <= n <= MAX_RANK_ITEMS:
+            raise ValueError(f"rank_items: n = {n} must be in [1, {MAX_RANK_ITEMS}]")
+        H = self.num_hierarchies
+        scores, bad, leaf_key, n_items = self._leaf_scores(
+            _strip_dedup_col(batch.seq_mask.long(), H + 1, H), _strip_dedup_col(batch.sem_ids, H + 1, H), batch.user_ids,
+            encoder, encoder_attention, attention, max_rows, "rank_items")
+        fut = batch.sem_ids_fut
+        row, start = self._item_table(scores.device).arrays()
+        items, item_scores, rank = ops.t5rank_select(scores, row, start, self._leaf_of(fut[:, :H], leaf_key), fut[:, H], n)
+        self._raise_bad(bad, "rank_items")
+        return ItemRankingOutput(item_ids=items, scores=item_scores, target_rank=rank, num_items=n_items)

@@ -7,7 +7,7 @@ from __future__ import annotations
 
 import ctypes
 import weakref
-from typing import List, Optional, Sequence
+from typing import List, NamedTuple, Optional, Sequence
 
 import torch
 
@@ -700,6 +700,48 @@ class SidPrefixIndex:
         _count(1)
         return out_g, out_p, out_parent
 
+    def counts(self) -> torch.Tensor:
+        """int32 [C + 1] on the device: the node count of every level (the root's 1 first), one launch, no host read."""
+        counts = torch.empty(self.C + 1, dtype=torch.int32, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().rqb200_sid_trie_counts(_p(self.ws), _p(counts), _stream()), "sid_trie_counts")
+        _count(1)
+        return counts
+
+    def levels(self, n: Sequence[int]) -> "SidTrieLevels":
+        """The level arrays of levels 1..C as device tensors, given the node counts n = ``counts()`` read on the host; one launch
+        per level.  Built once and cached on the index."""
+        if getattr(self, "_levels", None) is None:
+            n = [int(v) for v in n]
+            if len(n) != self.C + 1 or n[0] != 1:
+                raise ValueError(f"levels: n must be the {self.C + 1} node counts of counts(), got {n}")
+            code, parent, child = [None], [None], [torch.tensor([0, n[1]], dtype=torch.int32, device=self.device)]
+            lib = _lib.load()
+            for l in range(1, self.C + 1):
+                c = torch.empty(n[l], dtype=torch.int32, device=self.device)
+                p = torch.empty(n[l], dtype=torch.int32, device=self.device)
+                ch = torch.zeros(n[l] + 1, dtype=torch.int32, device=self.device) if l < self.C else None
+                if n[l] > 0:
+                    with torch.cuda.device(self.device):
+                        _lib.check(lib.rqb200_sid_trie_level(_p(self.ws), self.C, l, n[l], n[l - 1], _p(c), _p(p), _p(ch),
+                                                             _stream()), "sid_trie_level")
+                    _count(1)
+                code.append(c)
+                parent.append(p)
+                child.append(ch)
+            self._levels = SidTrieLevels(n, code, parent, child)
+        return self._levels
+
+
+class SidTrieLevels(NamedTuple):
+    """A trie's levels: n[l] nodes in level l (n[0] = 1, the root); for l >= 1 code[l] / parent[l] int32 [n[l]] (each node's last
+    id and its node in level l - 1); child[l] int32 [n[l] + 1] for l < C (node i's children in level l + 1 are child[l][i] ..
+    child[l][i + 1] - 1; child[0] = [0, n[1]]).  Nodes of one level are in lexicographic order of their prefixes."""
+    n: List[int]
+    code: List[Optional[torch.Tensor]]
+    parent: List[Optional[torch.Tensor]]
+    child: List[Optional[torch.Tensor]]
+
 
 class SidItemTable:
     """Item table of a corpus id table [N, C] (rqb200_sid_items_build): maps generated id tuples back to the corpus items (rows)
@@ -768,6 +810,29 @@ class SidItemTable:
                                                              _p(beam), _p(count), _stream()), "sid_items_retrieve")
         _count(1)
         return items, beam, count
+
+    def arrays(self):
+        """(row int32 [N], start int32 [N + 1]): views of the table's workspace.  Tuple u's items are row[start[u] .. start[u + 1])
+        in dedup order; only the first U + 1 entries of start are written (U: the distinct retrievable tuples)."""
+        row_off, start_off = ctypes.c_size_t(), ctypes.c_size_t()
+        _lib.check(_lib.load().rqb200_sid_items_offsets(self.N, self.C, self.K, ctypes.byref(row_off), ctypes.byref(start_off)),
+                   "sid_items_offsets")
+        row = self.ws[row_off.value:row_off.value + 4 * self.N].view(torch.int32)
+        start = self.ws[start_off.value:start_off.value + 4 * (self.N + 1)].view(torch.int32)
+        return row, start
+
+
+def sid_rank_hist(rank: torch.Tensor, hist: torch.Tensor) -> None:
+    """Adds exact ranks (int64 [B], -1: not ranked) to hist (int64 [k + 1]): hist[rank] for rank < k, hist[k] otherwise.  One
+    launch; never waits on the host."""
+    _need_cuda(rank, hist)
+    if hist.dtype != torch.int64 or hist.dim() != 1 or hist.numel() < 2 or not hist.is_contiguous():
+        raise ValueError("rank histogram: hist must be a contiguous int64 tensor of k + 1 >= 2 elements")
+    rank = rank.reshape(-1).to(torch.int64).contiguous()
+    with torch.cuda.device(hist.device):
+        _lib.check(_lib.load().rqb200_sid_rank_hist(_p(rank), rank.numel(), hist.numel() - 1, _p(hist), _stream()),
+                   "sid_rank_hist")
+    _count(1)
 
 
 def sid_topk_rank_hist(actual: torch.Tensor, candidates: torch.Tensor, hist: torch.Tensor, item_mode: bool = False) -> None:
@@ -928,6 +993,104 @@ def t5dec_add_norm(x: torch.Tensor, delta: Optional[torch.Tensor], weight: torch
                                                      _stream()), "t5dec_add_norm")
     _count(1)
     return out
+
+
+# ---------------------------------------------------------------------------------------------- exact ranking (csrc/t5rank.cu)
+def _int32_vec(t: torch.Tensor, n: int, what: str) -> torch.Tensor:
+    if t.dtype != torch.int32 or t.dim() != 1 or t.shape[0] < n or not t.is_contiguous():
+        raise ValueError(f"{what} must be a contiguous int32 vector of at least {n} entries")
+    return t
+
+
+def t5rank_cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, offsets: torch.Tensor,
+                           key_mask: Optional[torch.Tensor], Q: int, heads: int, tf32: bool = False) -> torch.Tensor:
+    """T5 cross-attention of Q queries per history (rqb200_t5rank_cross_attention, fp32 on the CUDA cores, or with ``tf32``
+    rqb200_t5rank_cross_attention_tc, the products on the TF32 tensor cores), one launch.  q [B * Q, heads * 64] (history b
+    owns rows b * Q ...), k / v [rows, heads * 64] (any row stride, equal), history b's keys rows offsets[b] .. offsets[b + 1] - 1
+    (int32 [B + 1], absolute), key_mask fp32 [rows] added to the scores (None: 0) -> [B * Q, heads * 64]."""
+    _need_cuda(q, k, v, offsets, key_mask)
+    inner = heads * T5_DKV
+    q, k, v = _rows_of(q, inner, "q"), _rows_of(k, inner, "k"), _rows_of(v, inner, "v")
+    if Q <= 0 or q.shape[0] % Q:
+        raise ValueError(f"q has {q.shape[0]} rows, not a multiple of Q = {Q}")
+    B = q.shape[0] // Q
+    _int32_vec(offsets, B + 1, "offsets")
+    if k.shape != v.shape:
+        raise ValueError(f"k {tuple(k.shape)} and v {tuple(v.shape)} must have one shape")
+    if k.stride(0) != v.stride(0):
+        k, v = k.contiguous(), v.contiguous()
+    if key_mask is not None:
+        key_mask = _f32c(key_mask)
+        if key_mask.dim() != 1 or key_mask.shape[0] != k.shape[0]:
+            raise ValueError(f"key_mask {tuple(key_mask.shape)} must be [{k.shape[0]}], one entry per key row")
+    if tf32 and any(t.data_ptr() % 16 or t.stride(0) % 4 for t in (q, k)):
+        q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
+    out = torch.empty((q.shape[0], inner), dtype=torch.float32, device=q.device)
+    name = "t5rank_cross_attention_tc" if tf32 else "t5rank_cross_attention"
+    with torch.cuda.device(q.device):
+        _lib.check(getattr(_lib.load(), "rqb200_" + name)(_p(q), q.stride(0), _p(k), _p(v), k.stride(0), _p(offsets), _p(key_mask),
+                                                          B, Q, heads, _p(out), out.stride(0), _stream()), name)
+    _count(1)
+    return out
+
+
+def t5rank_children(logits: torch.Tensor, parent: Optional[torch.Tensor], child: torch.Tensor, code: torch.Tensor, n_h: int,
+                    out: torch.Tensor, bad: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Child scores of one trie level (rqb200_t5rank_children), one launch: logits [B * n_h, K] of the level's node rows, parent
+    fp32 [B * n_h] (the nodes' scores; None: 0), child int32 [n_h + 1], code int32 [n_next] -> out fp32 [B, n_next] (written):
+    out[b, j] = (logits[b * n_h + i, code[j]] - lse) + parent[b * n_h + i] for every child j of node i.  ``bad`` (int32, on the
+    device) is ADDED the rows holding a NaN or +inf logit or all -inf; their children score NaN."""
+    _need_cuda(logits, parent, child, code, out, bad)
+    logits = _rows(logits)
+    R, K = logits.shape
+    if n_h <= 0 or R % n_h:
+        raise ValueError(f"logits has {R} rows, not a multiple of n_h = {n_h}")
+    B = R // n_h
+    _int32_vec(child, n_h + 1, "child")
+    n_next = code.shape[0]
+    _int32_vec(code, n_next, "code")
+    if out.dtype != torch.float32 or out.shape != (B, n_next) or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous fp32 [{B}, {n_next}] tensor")
+    if parent is not None:
+        parent = _f32c(parent).reshape(-1)
+        if parent.shape[0] != R:
+            raise ValueError(f"parent has {parent.shape[0]} entries, logits {R} rows")
+    if bad is not None and (bad.dtype != torch.int32 or bad.numel() < 1 or not bad.is_contiguous()):
+        raise ValueError("bad must be a contiguous int32 tensor")
+    with torch.cuda.device(logits.device):
+        _lib.check(_lib.load().rqb200_t5rank_children(_p(logits), logits.stride(0), R, K, n_h, _p(parent), _p(child), _p(code),
+                                                      n_next, _p(out), _p(bad), _stream()), "t5rank_children")
+    _count(1)
+    return out
+
+
+def t5rank_select(scores: torch.Tensor, row: torch.Tensor, start: torch.Tensor, t_leaf: torch.Tensor, t_dedup: torch.Tensor,
+                  n: int):
+    """The n best items of each history from its leaf scores (rqb200_t5rank_select), one launch.  scores fp32 [B, U] (leaf u =
+    item-table tuple u), (row, start) = ``SidItemTable.arrays()``, t_leaf / t_dedup int64 [B] (the target's tuple, -1 when it has
+    none, and dedup rank) -> (items int64 [B, n], item scores fp32 [B, n], target rank int64 [B]): items by score descending, then
+    tuple, then dedup rank, NaN last; -1 / -inf pad; rank -1 when the target is not ranked.  n <= 1024."""
+    _need_cuda(scores, row, start, t_leaf, t_dedup)
+    scores = _f32c(scores)
+    if scores.dim() != 2:
+        raise ValueError(f"scores {tuple(scores.shape)} must be [B, U]")
+    B, U = scores.shape
+    _int32_vec(start, U + 1, "start")
+    _int32_vec(row, 0, "row")
+    t_leaf = t_leaf.to(torch.int64).reshape(-1).contiguous()
+    t_dedup = t_dedup.to(torch.int64).reshape(-1).contiguous()
+    if t_leaf.shape[0] != B or t_dedup.shape[0] != B:
+        raise ValueError(f"t_leaf / t_dedup must have B = {B} entries")
+    n = int(n)
+    dev = scores.device
+    items = torch.empty((B, n), dtype=torch.int64, device=dev)
+    item_scores = torch.empty((B, n), dtype=torch.float32, device=dev)
+    rank = torch.empty((B,), dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.load().rqb200_t5rank_select(_p(scores), B, U, _p(row), _p(start), _p(t_leaf), _p(t_dedup), n, _p(items),
+                                                    _p(item_scores), _p(rank), _stream()), "t5rank_select")
+    _count(1)
+    return items, item_scores, rank
 
 
 # ---------------------------------------------------------------------------------------------- fused T5 encoder pass
