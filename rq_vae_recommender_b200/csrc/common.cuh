@@ -153,4 +153,13 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
       "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
       : "memory");
 }
+// tiled tensor copy global -> shared of the box at (c0, c1) of a 2-D tensor map (a __grid_constant__ kernel parameter);
+// 128-byte aligned destination.  SASS UTMALDG
+__device__ __forceinline__ void tensor_g2s_2d(void* smem_dst, const void* tmap, int c0, int c1, uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
+          smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(c0), "r"(c1), "r"(smem_u32(bar))
+      : "memory");
+}
 #endif  // __CUDACC__

@@ -19,10 +19,11 @@
 //     (helper)       all levels of a tile) and measure ||fp16(x) - x||^2 and ||x||^2 per row; re-rank the queued rows of each
 //                    level exactly, any warp taking the next queued row.
 //   WG2, warp 8      producer of one 32 KB stage ring (bulk copies counted on an mbarrier per stage).  Per tile it first
-//                    stages the tile's fp32 rows, 128 columns per stage (one copy per row, spread over the lanes), then for
+//                    stages the tile's fp32 rows, 128 columns per stage (one tensor copy of the 64 x 128 box), then for
 //                    every (level, block, k chunk) the prepared 16 KB blocks of codes [256 cb, 256 cb + 128) and
-//                    [256 cb + 128, 256 cb + 256).  Warps 9-11 exit at once.  The helper consumes the x stages and the scorer
-//                    the codebook stages; each walks the same stage counter and skips the other's stages.
+//                    [256 cb + 128, 256 cb + 256).  Only its lane 0 issues copies; warps 9-11 exit at once.  The helper
+//                    consumes the x stages and the scorer the codebook stages; each walks the same stage counter and skips
+//                    the other's stages.
 //
 // Hand-offs of tile t, on four mbarriers that every thread of the signalling warpgroup arrives on:
 //   scorer  waits IMG_FULL(t); per level l: MMA(l) (after the last level's MMAs complete it arrives on IMG_FREE(t)), waits
@@ -48,6 +49,9 @@
 //                          ends with exactly that code, so the re-rank rate is the unblocked filter's (tests/tc_blocked_model.py).
 //                          Candidate words of every row go to shared memory and ids are 16-bit.
 // One kernel with a runtime block loop for every K was 2-4 % slower at K = 256 on the H100, even specialised by template.
+#include <cuda.h>
+#include <cudaTypedefs.h>
+
 #include "tc_common.cuh"
 #include "wgmma.cuh"
 
@@ -79,6 +83,7 @@ struct TxSmem {
 };
 
 struct TxParams {
+  CUtensorMap xmap;              // x as a [B][D] fp32 tensor (row pitch ldx), boxes of TX_R rows x TX_XCOLS columns
   const float* x;
   int64_t ldx;
   int B, D, K, L, nkc, nblk, ntiles, nb;
@@ -147,31 +152,22 @@ __device__ __forceinline__ void tx_init(unsigned char* tsm, TxSmem* ms) {
   __syncthreads();
 }
 
-// producer (warp 8): per tile, its x stages (the helper's), then (level, block, k chunk) (the scorer's).
-// Lane 0 waits for a free slot and arms its mbarrier with the exact byte count.  X stage c holds columns [128 c, 128 c + 128)
-// (half of them when D % 128 == 64) of the tile's rows below B, 512 bytes per row whatever the width; each lane copies rows
-// lane and lane + 32.  Lane 0 copies the two 16 KB halves of a codebook stage.
+// producer (lane 0 of warp 8): per tile, its x stages (the helper's), then (level, block, k chunk) (the scorer's).  It
+// waits for a free slot and arms its mbarrier with the stage's byte count.  X stage c is ONE tensor copy of the box of rows
+// [row0, row0 + 64) and columns [128 c, 128 c + 128): 512 bytes per row, with zeros past B and past D (when D % 128 == 64)
+// that the converter never reads; the copy counts the whole box.  One copy per stage rather than 64 bulk copies of a
+// 512-byte row each: the step is 14-18 % shorter on the H100 (README).  A codebook stage is two 16 KB bulk copies.
 __device__ __forceinline__ void tx_produce(const TxParams& p, unsigned char* sC, TxSmem* ms, int nblk) {
-  const int nkc = p.nkc, lane = threadIdx.x & 31, nxs = (p.D + TX_XCOLS - 1) / TX_XCOLS;
+  const int nkc = p.nkc, nxs = (p.D + TX_XCOLS - 1) / TX_XCOLS;
   const uint32_t nb = (uint32_t)p.nb;
   uint32_t s = 0;
   for (int unit = blockIdx.x; unit < p.ntiles; unit += gridDim.x) {
-    const int row0 = unit * TX_R, nrows = min(TX_R, p.B - row0);
+    const int row0 = unit * TX_R;
     for (int c = 0; c < nxs; ++c, ++s) {
       const uint32_t st = s % nb, u = s / nb;
-      const uint32_t bytes = (uint32_t)min(TX_XCOLS, p.D - c * TX_XCOLS) * 4u;
-      if (lane == 0) {
-        mbar_wait_guarded(&ms->empty[st], (u & 1) ^ 1, 1);
-        mbar_expect_tx(&ms->full[st], (uint32_t)nrows * bytes);
-      }
-      __syncwarp();
-      unsigned char* dst = sC + st * TX_STAGE_BYTES;
-      for (int r = lane; r < nrows; r += 32)
-        bulk_g2s(dst + r * TX_XROW_BYTES, p.x + (int64_t)(row0 + r) * p.ldx + c * TX_XCOLS, bytes, &ms->full[st]);
-    }
-    if (lane != 0) {                   // the other lanes wait for lane 0 at the next tile's first x stage
-      s += (uint32_t)(p.L * nblk * nkc);
-      continue;
+      mbar_wait_guarded(&ms->empty[st], (u & 1) ^ 1, 1);
+      mbar_expect_tx(&ms->full[st], TX_STAGE_BYTES);
+      tensor_g2s_2d(sC + st * TX_STAGE_BYTES, &p.xmap, c * TX_XCOLS, row0, &ms->full[st]);
     }
     for (int l = 0; l < p.L; ++l)
       for (int cb = 0; cb < nblk; ++cb)
@@ -532,7 +528,7 @@ __device__ __forceinline__ bool tx_side_roles(const TxParams& p, const TxShared<
   const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);
   if (wg == 2) {
     tx_reg_dec<TX_REG_PRODUCER>();
-    if (threadIdx.x < 9 * 32) tx_produce(p, sh.sC, sh.ms, K / TC_K);   // warp 8; warps 9-11 have nothing to do
+    if (threadIdx.x == 8 * 32) tx_produce(p, sh.sC, sh.ms, K / TC_K);   // lane 0 of warp 8; the rest have nothing to do
     return true;
   }
   if (wg == 1) {
@@ -701,6 +697,27 @@ int tcx_run(const float* x, int64_t ldx, int B, const void* state, int D, int K,
   p.blob = reinterpret_cast<const unsigned char*>(base + tc_off_blob(D, K, L));
   p.ids = ids; p.stats = stats;
   p.nb = tcx_ring_stages(D, K, L);
+  // the x tensor map: dimension 0 = the D columns (row pitch ldx floats), dimension 1 = the B rows; reads outside it
+  // (columns past D, rows past B) fill the box with zeros
+  static PFN_cuTensorMapEncodeTiled_v12000 encode = nullptr;
+  if (!encode) {
+    cudaDriverEntryPointQueryResult q;
+    void* fn = nullptr;
+    RQB_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q));
+    if (q != cudaDriverEntryPointSuccess || !fn) {
+      rqb_set_error("tokenize_tc_run: the driver has no cuTensorMapEncodeTiled");
+      return RQB_ERR_CUDA;
+    }
+    encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fn);
+  }
+  const cuuint64_t dims[2] = {(cuuint64_t)D, (cuuint64_t)B}, strides[1] = {(cuuint64_t)ldx * 4u};
+  const cuuint32_t box[2] = {TX_XCOLS, TX_R}, estr[2] = {1, 1};
+  if (encode(&p.xmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(x), dims, strides, box, estr,
+             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS) {
+    rqb_set_error("tokenize_tc_run: cuTensorMapEncodeTiled failed (B=%d D=%d ldx=%lld)", B, D, (long long)ldx);
+    return RQB_ERR_CUDA;
+  }
   const size_t smem = tcx_smem_bytes(D, K, L, p.nb);
   // K = 256: one accumulator holds a level; larger K is scored in 256-code blocks
   void (*const kernel)(TxParams) = K == TC_K ? rq_tcx_kernel : rq_tcx_blocked_kernel;
