@@ -325,6 +325,17 @@ int rqb200_t5rank_children(const float* logits, int64_t ld, int R, int K, int n_
                            const int* code, int n_next, float* out, int* bad, void* stream);
 int rqb200_t5rank_select(const float* scores, int B, int U, const int* row, const int* start, const int64_t* t_leaf,
                          const int64_t* t_dedup, int n, int64_t* out_items, float* out_scores, int64_t* out_rank, void* stream);
+/* t5score_trie_build     : the trie of each history's own candidate tuples (modules/model.py score_sem_ids / score_items), one CTA per
+ *                          history.  ids int64 [B, C, H] (candidate c of history b: ids[(b * C + c) * H ..]); a tuple holding an id
+ *                          outside [0, K) is invalid.  Per history b and level l = 1..H (the distinct l-prefixes of its valid tuples,
+ *                          in lexicographic order): counts int32 [B, H] (entry l - 1: the node count n_l), code / parent int32
+ *                          [B, H, C] (entry (l - 1, i): node i's last id and its node in level l - 1; 0 and 0 for i >= n_l), child
+ *                          int32 [B, H, C + 1] (entry (l, i) for l = 0..H - 1: node i's children in level l + 1 are child[l][i] ..
+ *                          child[l][i + 1] - 1; n_{l + 1} for i >= n_l), leaf int32 [B, C] (each candidate's node in level H, -1 when
+ *                          invalid; equal tuples share it).  C <= 4096, H <= 8, H * bits(K - 1) <= 62 (RQB_ERR_UNSUPPORTED).  No
+ *                          atomics: the output is a function of the input. */
+int rqb200_t5score_trie_build(const int64_t* ids, int B, int C, int H, int K, int* counts, int* code, int* parent, int* child,
+                              int* leaf, void* stream);
 
 /* ---- one step of the generative-retrieval model's T5 decoder (modules/model.py, generate(decoder="fused")), csrc/t5dec.cu ----
  * HF T5 numerics in eval mode: attention without 1/sqrt(d) scaling, fp32 softmax, d_kv = 64 per head (inner = heads * 64).

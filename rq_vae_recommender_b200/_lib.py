@@ -90,6 +90,7 @@ _SIGNATURES = {
                                                  c_vp]),
     "rqb200_t5rank_children": (c_int, [c_vp, c_i64, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp]),
     "rqb200_t5rank_select": (c_int, [c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp]),
+    "rqb200_t5score_trie_build": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "rqb200_t5dec_cross_attention": (c_int, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_int, c_int, c_int, c_int, c_vp, c_i64,
                                              c_vp]),
     "rqb200_t5dec_self_attention": (c_int, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int,

@@ -21,6 +21,7 @@
 // Numerics are HF's T5 in eval mode: no 1/sqrt(d) scaling, an additive per-key mask (-FLT_MAX masks a key, as HF's eager mask).
 #include <cfloat>
 
+#include <cub/block/block_radix_sort.cuh>
 #include <cub/block/block_reduce.cuh>
 #include <cub/block/block_scan.cuh>
 
@@ -517,6 +518,132 @@ extern "C" int rqb200_t5rank_select(const float* scores, int B, int U, const int
     t5rank_select_kernel<false><<<B, RK_SEL_THREADS, 0, st>>>(scores, U, row, start, t_leaf, t_dedup, n, out_items, out_scores,
                                                              out_rank);
   }
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ per-history candidate trie
+// Exact scoring of given tuples (modules/model.py score_sem_ids / score_items) decodes, per history, the trie of that history's
+// C candidates instead of the corpus's.  One CTA per history: each candidate packs into a 64-bit key (bits = bits(K - 1) per id,
+// the first id highest, so key order is lexicographic); a tuple with an id outside [0, K) gets the key 1 << (H bits), above every
+// valid key.  A block radix sort (stable: equal keys stay in candidate order) over bits 0 .. H bits, then per level l = 1..H the
+// distinct l-prefixes are flagged and numbered by a block scan.  Writes are plain stores to distinct addresses: no atomics, the
+// output is a function of the input alone.
+#define SC_THREADS 512
+#define SC_MAX_C 4096
+
+template <int IPT>
+__global__ void __launch_bounds__(SC_THREADS) t5score_trie_kernel(const int64_t* __restrict__ ids, int C, int H, int K, int bits,
+                                                                  int* __restrict__ counts, int* __restrict__ code,
+                                                                  int* __restrict__ parent, int* __restrict__ child,
+                                                                  int* __restrict__ leaf) {
+  using Sort = cub::BlockRadixSort<unsigned long long, SC_THREADS, IPT, int>;
+  using Scan = cub::BlockScan<int, SC_THREADS>;
+  __shared__ union {
+    typename Sort::TempStorage sort;
+    typename Scan::TempStorage scan;
+  } tmp;
+  __shared__ unsigned long long s_last[SC_THREADS];
+  const int64_t b = blockIdx.x;
+  const int tid = threadIdx.x;
+  const int vbits = H * bits;
+  const unsigned long long invalid = 1ull << vbits;
+  const int64_t* in = ids + b * (int64_t)C * H;
+  unsigned long long key[IPT];
+  int idx[IPT];
+#pragma unroll
+  for (int j = 0; j < IPT; ++j) {                           // blocked: thread t holds candidates t IPT .. t IPT + IPT - 1
+    const int c = tid * IPT + j;
+    idx[j] = c;
+    key[j] = invalid;
+    if (c < C) {
+      unsigned long long k = 0;
+      bool ok = true;
+      for (int h = 0; h < H; ++h) {
+        const int64_t v = in[(int64_t)c * H + h];
+        ok &= v >= 0 && v < K;
+        k = (k << bits) | (unsigned long long)(ok ? v : 0);
+      }
+      if (ok) key[j] = k;
+    }
+  }
+  Sort(tmp.sort).Sort(key, idx, 0, vbits + 1);
+  __syncthreads();
+  s_last[tid] = key[IPT - 1];
+  __syncthreads();
+  const unsigned long long before = tid > 0 ? s_last[tid - 1] : invalid;
+  int* cnt_out = counts + b * H;
+  int prev_node[IPT], cnt_prev = 1;                         // level l - 1: every valid candidate's node; the root is node 0
+  bool prev_flag[IPT];
+#pragma unroll
+  for (int j = 0; j < IPT; ++j) {
+    prev_node[j] = 0;
+    prev_flag[j] = false;
+  }
+  if (tid == 0) child[b * H * (C + 1)] = 0;                 // the root's children start at node 0 of level 1
+  for (int l = 1; l <= H; ++l) {
+    const int shift = (H - l) * bits;
+    int flag[IPT], node[IPT], total;
+#pragma unroll
+    for (int j = 0; j < IPT; ++j) {
+      const unsigned long long prev = j > 0 ? key[j - 1] : before;
+      const bool valid = key[j] < invalid;
+      flag[j] = valid && (prev >= invalid || (prev >> shift) != (key[j] >> shift)) ? 1 : 0;
+    }
+    Scan(tmp.scan).InclusiveSum(flag, node, total);
+    __syncthreads();                                        // scan storage is reused by the next level
+    int* lcode = code + (b * H + (l - 1)) * (int64_t)C;
+    int* lpar = parent + (b * H + (l - 1)) * (int64_t)C;
+    int* pchild = child + (b * H + (l - 1)) * (int64_t)(C + 1);   // level l - 1's child ranges
+#pragma unroll
+    for (int j = 0; j < IPT; ++j) {
+      node[j] -= 1;
+      if (flag[j]) {
+        lcode[node[j]] = (int)((key[j] >> shift) & ((1ull << bits) - 1ull));
+        lpar[node[j]] = prev_node[j];
+        if (l > 1 && prev_flag[j]) pchild[prev_node[j]] = node[j];   // the first child of a new (l - 1)-prefix
+      }
+    }
+    for (int i = total + tid; i < C; i += SC_THREADS) {     // padding nodes: a valid code and parent
+      lcode[i] = 0;
+      lpar[i] = 0;
+    }
+    for (int i = cnt_prev + tid; i <= C; i += SC_THREADS) pchild[i] = total;
+    if (tid == 0) cnt_out[l - 1] = total;
+#pragma unroll
+    for (int j = 0; j < IPT; ++j) {
+      prev_node[j] = node[j];
+      prev_flag[j] = flag[j] != 0;
+    }
+    cnt_prev = total;
+  }
+  int* lf = leaf + b * C;
+#pragma unroll
+  for (int j = 0; j < IPT; ++j)
+    if (idx[j] < C) lf[idx[j]] = key[j] < invalid ? prev_node[j] : -1;
+}
+
+extern "C" int rqb200_t5score_trie_build(const int64_t* ids, int B, int C, int H, int K, int* counts, int* code, int* parent,
+                                         int* child, int* leaf, void* stream) {
+  RQB_CHECK_ARG(B >= 0 && C > 0 && H > 0 && K > 0, "t5score_trie_build: bad argument (B = %d, C = %d, H = %d, K = %d)", B, C, H, K);
+  int bits = 1;
+  while (bits < 31 && (1 << bits) < K) ++bits;              // bits(K - 1), at least 1
+  if (C > SC_MAX_C || H > RQB_MAX_LEVELS || H * bits > 62) {
+    rqb_set_error("t5score_trie_build: need C <= %d, H <= %d and H * bits(K - 1) <= 62 (C = %d, H = %d, K = %d)", SC_MAX_C,
+                  RQB_MAX_LEVELS, C, H, K);
+    return RQB_ERR_UNSUPPORTED;
+  }
+  if (B == 0) return RQB_OK;
+  RQB_CHECK_ARG(ids && counts && code && parent && child && leaf, "t5score_trie_build: null pointer");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (C <= SC_THREADS)
+    t5score_trie_kernel<1><<<B, SC_THREADS, 0, st>>>(ids, C, H, K, bits, counts, code, parent, child, leaf);
+  else if (C <= 2 * SC_THREADS)
+    t5score_trie_kernel<2><<<B, SC_THREADS, 0, st>>>(ids, C, H, K, bits, counts, code, parent, child, leaf);
+  else if (C <= 4 * SC_THREADS)
+    t5score_trie_kernel<4><<<B, SC_THREADS, 0, st>>>(ids, C, H, K, bits, counts, code, parent, child, leaf);
+  else
+    t5score_trie_kernel<8><<<B, SC_THREADS, 0, st>>>(ids, C, H, K, bits, counts, code, parent, child, leaf);
   RQB_LAUNCH_CHECK();
   return RQB_OK;
 }

@@ -40,7 +40,10 @@ decoder training kernels of csrc/t5dec.cu with HF's dropout; ``DEFAULT_FORWARD_D
 
 ``rank_items`` / ``rank_sem_ids`` are an evaluation tool with no search: every corpus item is scored by its exact
 log-probability, one decoder row per corpus-trie node per history (``FusedT5Rank``, csrc/t5rank.cu), and ranked.
+``score_items`` / ``score_sem_ids`` give the same exact log-probability for items the caller chooses, decoding per history the trie
+of its own candidates with the same kernels.
 """
+from typing import List
 from typing import NamedTuple
 from typing import Optional
 
@@ -201,7 +204,15 @@ class ItemRankingOutput(NamedTuple):
     num_items: int
 
 
-#: device bytes one chunk of histories of rank_sem_ids / rank_items is sized to when max_rows is not given
+class ItemScoreOutput(NamedTuple):
+    """score_items: the exact log-probability of each given item (scores [B, C] fp32, -inf for padding and for items whose
+    tuple holds an id outside [0, K)) and the 0-based position of the true next item among the row's items in rank_items' order
+    (target_rank [B] int64, -1 when it is not among them)."""
+    scores: Tensor
+    target_rank: Tensor
+
+
+#: device bytes one chunk of histories of rank_sem_ids / rank_items / score_sem_ids is sized to when max_rows is not given
 RANK_BYTE_BUDGET = 4 << 30
 #: most items rank_items returns per history
 MAX_RANK_ITEMS = 1024
@@ -222,11 +233,11 @@ class FusedT5Rank:
         (``attention="tf32"``) its products on the TF32 tensor cores;
       * after each level's head, ``t5rank_children`` (log-sum-exp as the beam search, child score = parent + log-probability)."""
 
-    def __init__(self, model: "EncoderDecoderRetrievalModel", levels: ops.SidTrieLevels, rows: Tensor, offsets: Tensor,
-                 key_mask: Tensor, attention: str = "fp32"):
+    def __init__(self, model: "EncoderDecoderRetrievalModel", rows: Tensor, offsets: Tensor, key_mask: Tensor,
+                 attention: str = "fp32"):
         dec = model.t5_decoder
         _check_encoder_config(dec.config, "rank_sem_ids")
-        self.model, self.levels, self.H = model, levels, model.num_hierarchies
+        self.model, self.H = model, model.num_hierarchies
         self.tf32 = _check_attention(attention) == "tf32"
         self.heads, self.eps = dec.config.num_heads, dec.config.layer_norm_epsilon
         self.inner = self.heads * ops.T5_DKV
@@ -244,8 +255,6 @@ class FusedT5Rank:
         self.cross_kv = ops.gemm_split(rows, w(w_kv))
         self.offsets, self.key_mask = offsets, key_mask
         self.bias = dec.block[0].layer[0].SelfAttention.compute_bias(self.H, self.H)[0].contiguous()
-        self.width = max(levels.n[:self.H])
-        self.codes = [None] + [levels.code[h].long() for h in range(1, self.H)]
 
     @staticmethod
     def row_bytes(model: "EncoderDecoderRetrievalModel") -> int:
@@ -257,32 +266,63 @@ class FusedT5Rank:
         floats = cfg.num_layers * 2 * H * inner + 3 * d + 5 * inner + cfg.d_ff + model.num_embeddings_per_hierarchy + 1
         return 4 * floats + 16 + 8 * H
 
-    def run(self, b0: int, b1: int, out: Tensor, bad: Tensor) -> None:
-        """Leaf scores of histories b0 .. b1 - 1 into out[b0:b1] ([B, U])."""
-        m, eps, inner, lv, H = self.model, self.eps, self.inner, self.levels, self.H
+    def run(self, b0: int, b1: int, levels: ops.SidTrieLevels, out: Tensor, bad: Tensor) -> None:
+        """Leaf scores of histories b0 .. b1 - 1 over the corpus trie into out[b0:b1] ([B, U]): every history decodes every node."""
+        H, Bc, dev = self.H, b1 - b0, self.cross_kv.device
+        first = torch.arange(Bc, device=dev)[:, None]
+        ids = [None] + [levels.code[h].long().repeat(Bc) for h in range(1, H)]
+        parent = [None] + [(first * levels.n[h - 1] + levels.parent[h].long()[None, :]).reshape(-1) for h in range(1, H)]
+        nxt = [torch.empty((Bc, levels.n[h + 1]), dtype=torch.float32, device=dev) for h in range(H - 1)] + [out[b0:b1]]
+        self.decode(b0, b1, levels.n[:H], ids, parent, levels.child[:H], levels.code[1:H + 1], nxt, bad)
+
+    def run_candidates(self, b0: int, b1: int, n: List[int], trie: ops.CandidateTrie, out: Tensor, bad: Tensor) -> None:
+        """Candidate scores of histories b0 .. b1 - 1 over their own tries (``ops.t5score_trie_build``) into out[b0:b1] ([B, C];
+        -inf for a candidate holding an id outside [0, K)).  Level h is padded to n[h] rows per history, the chunk's largest
+        count (at least 1).  A padding row decodes code 0 under its history's row 0 of the level above, so its values are finite;
+        it has no children, except that the last row of a history owns the padding slots of the level below it, which keeps the
+        chunk's child ranges one ascending array.  No padding score is read."""
+        H, Bc, dev = self.H, b1 - b0, self.cross_kv.device
+        first = torch.arange(Bc, device=dev)[:, None]
+        ids = [None] + [trie.code[b0:b1, h - 1, :n[h]].reshape(-1).long() for h in range(1, H)]
+        parent = [None] + [(first * n[h - 1] + trie.parent[b0:b1, h - 1, :n[h]]).reshape(-1) for h in range(1, H)]
+        # the chunk as one group of Bc * n[h] rows: child ranges offset to the chunk's slots of level h + 1
+        child = [torch.cat([(first * n[h + 1] + trie.child[b0:b1, h, :n[h]]).reshape(-1),
+                            torch.full((1,), Bc * n[h + 1], dtype=torch.int64, device=dev)]).to(torch.int32) for h in range(H)]
+        code = [trie.code[b0:b1, h, :n[h + 1]].reshape(-1).contiguous() for h in range(H)]
+        nxt = [torch.empty((1, Bc * n[h + 1]), dtype=torch.float32, device=dev) for h in range(H)]
+        self.decode(b0, b1, n[:H], ids, parent, child, code, nxt, bad)
+        leaf = trie.leaf[b0:b1].long()
+        out[b0:b1] = torch.where(leaf >= 0, nxt[H - 1].view(-1)[first * n[H] + leaf.clamp(min=0)], float("-inf"))
+
+    def decode(self, b0: int, b1: int, n: List[int], ids: List[Optional[Tensor]], parent: List[Optional[Tensor]],
+               child: List[Tensor], code: List[Tensor], nxt: List[Tensor], bad: Tensor) -> None:
+        """The level loop of histories b0 .. b1 - 1 over given trie levels.  Level h runs n[h] decoder rows per history (row
+        b * n[h] + i; n[0] = 1, BOS); for h >= 1 ids[h] / parent[h] (int64 [Bc * n[h]]) are each row's last code and its row in
+        level h - 1.  After the level's head, ``t5rank_children`` writes the children's scores to nxt[h] ([G, n_next]: the level's
+        rows as G equal groups, child[h] int32 the child ranges of one group's rows, code[h] int32 [n_next] the children's last
+        codes, nxt[h - 1] the rows' own scores)."""
+        m, eps, inner, H = self.model, self.eps, self.inner, self.H
         Bc, dev = b1 - b0, self.cross_kv.device
-        rows = Bc * self.width
+        rows = Bc * max(n)
         cache = torch.empty((len(self.blocks), 2, H, rows, inner), dtype=torch.float32, device=dev)
         anc = torch.zeros((rows, H), dtype=torch.int32, device=dev)
         anc_next = torch.empty_like(anc)
         offsets = self.offsets[b0:b1 + 1]
         score = None
         for h in range(H):
-            n_h = lv.n[h]
+            n_h = n[h]
             R = Bc * n_h
             x = torch.empty((R, m.bos_token.shape[1]), dtype=torch.float32, device=dev)
             nrm = torch.empty_like(x)
-            parent = None
             if h == 0:
                 ops.t5dec_add_norm(x, None, self.norms[0], nrm, eps, emb=m.bos_token)
             else:
-                ops.t5dec_add_norm(x, None, self.norms[0], nrm, eps, emb=m.item_sid_embedding_table.weight,
-                                   ids=self.codes[h].repeat(Bc), offset=(h - 1) * m.num_embeddings_per_hierarchy)
-                parent = (torch.arange(Bc, device=dev)[:, None] * lv.n[h - 1] + lv.parent[h].long()[None, :]).reshape(R)
+                ops.t5dec_add_norm(x, None, self.norms[0], nrm, eps, emb=m.item_sid_embedding_table.weight, ids=ids[h],
+                                   offset=(h - 1) * m.num_embeddings_per_hierarchy)
             for l, (w_qkv, w_o, w_q, w_xo, w_i, w_fo) in enumerate(self.w):
-                advance = parent is not None and l == 0
+                advance = h > 0 and l == 0
                 a = ops.t5dec_self_attention(ops.gemm_split(nrm, w_qkv), cache[l, 0], cache[l, 1], self.bias, h, anc,
-                                             parent if advance else None, anc_next if advance else None)
+                                             parent[h] if advance else None, anc_next if advance else None)
                 if advance:
                     anc, anc_next = anc_next, anc
                 ops.t5dec_add_norm(x, ops.gemm_split(a, w_o), self.norms[3 * l + 1], nrm, eps)
@@ -291,9 +331,8 @@ class FusedT5Rank:
                                                n_h, self.heads, tf32=self.tf32)
                 ops.t5dec_add_norm(x, ops.gemm_split(a, w_xo), self.norms[3 * l + 2], nrm, eps)
                 ops.t5dec_add_norm(x, ops.gemm_split(ops.gemm_split(nrm, w_i, relu=True), w_fo), self.norms[3 * l + 3], nrm, eps)
-            nxt = out[b0:b1] if h == H - 1 else torch.empty((Bc, lv.n[h + 1]), dtype=torch.float32, device=dev)
-            ops.t5rank_children(ops.gemm_split(nrm, self.heads_w[h]), score, lv.child[h], lv.code[h + 1], n_h, nxt, bad)
-            score = nxt
+            ops.t5rank_children(ops.gemm_split(nrm, self.heads_w[h]), score, child[h], code[h], R // nxt[h].shape[0], nxt[h], bad)
+            score = nxt[h]
 
 
 def _encoder_attention(encoder: str, encoder_attention: Optional[str], what: str) -> str:
@@ -318,6 +357,12 @@ def _read_n_kept(offsets: Tensor) -> int:
     """The packed row count offsets[B], read on the host to size the encoder's GEMMs: the one host synchronisation of an
     encoder="fused" pass."""
     return int(offsets[-1])
+
+
+def _read_node_counts(counts: Tensor) -> List[List[int]]:
+    """The candidate tries' node counts [B, H], read on the host to size the padded levels and the chunks: the first of the two
+    host reads of score_sem_ids / score_items."""
+    return counts.tolist()
 
 
 class FusedT5Encode:
@@ -1021,7 +1066,8 @@ class EncoderDecoderRetrievalModel(nn.Module):
         idx = torch.searchsorted(leaf_key, key).clamp_(max=U - 1)
         return torch.where(valid & (leaf_key[idx] == key), idx, -1)
 
-    def _leaf_scores(self, attention_mask, input_ids, user_id, encoder, encoder_attention, attention, max_rows, what: str):
+    def _check_rank_call(self, encoder, encoder_attention, attention, what: str):
+        """(encoder, its attention, the decoder's cross-attention) of an exact-scoring call, after its mode checks."""
         if self.training:
             raise ValueError(f"{what} runs the model in eval mode only; call model.eval() first (in training mode HF's passes "
                              "apply dropout)")
@@ -1034,6 +1080,24 @@ class EncoderDecoderRetrievalModel(nn.Module):
         attention = "fp32" if attention is None else attention
         if attention not in ENCODER_ATTENTIONS:
             raise ValueError(f"{what}: attention must be one of {ENCODER_ATTENTIONS}, got {attention!r}")
+        return encoder, att, attention
+
+    def _rank_encoder(self, attention_mask, input_ids, user_id, encoder: str, att: str):
+        """The encoder rows the exact scoring attends to: (rows [*, d_model], offsets int32 [B + 1], additive key mask [*])."""
+        B, dev = attention_mask.shape[0], attention_mask.device
+        if encoder == "fused":
+            enc = self._fused_encoder(att)
+            rows, slot, _ = enc.packed(attention_mask, input_ids, user_id)
+            key_mask = enc.key_mask.index_select(0, torch.div(enc.src, slot.shape[1], rounding_mode="floor").long())
+            return rows, enc.offsets, key_mask
+        enc_out, enc_mask = self.encoder_forward_pass(attention_mask=attention_mask, input_ids=input_ids, user_id=user_id)
+        S, d = enc_out.shape[1], enc_out.shape[2]
+        offsets = torch.arange(0, (B + 1) * S, S, dtype=torch.int32, device=dev)
+        key_mask = torch.where(enc_mask == 0, torch.finfo(torch.float32).min, 0.0).to(torch.float32).reshape(B * S)
+        return enc_out.reshape(B * S, d), offsets, key_mask
+
+    def _leaf_scores(self, attention_mask, input_ids, user_id, encoder, encoder_attention, attention, max_rows, what: str):
+        encoder, att, attention = self._check_rank_call(encoder, encoder_attention, attention, what)
         dev = attention_mask.device
         levels, leaf_key, n_items = self._rank_levels(dev)
         H, B = self.num_hierarchies, attention_mask.shape[0]
@@ -1047,21 +1111,10 @@ class EncoderDecoderRetrievalModel(nn.Module):
         scores = torch.empty((B, U), dtype=torch.float32, device=dev)
         if B == 0 or U == 0:
             return scores, bad, leaf_key, n_items
-        if encoder == "fused":
-            enc = self._fused_encoder(att)
-            rows, slot, _ = enc.packed(attention_mask, input_ids, user_id)
-            offsets = enc.offsets
-            key_mask = enc.key_mask.index_select(0, torch.div(enc.src, slot.shape[1], rounding_mode="floor").long())
-        else:
-            enc_out, enc_mask = self.encoder_forward_pass(attention_mask=attention_mask, input_ids=input_ids, user_id=user_id)
-            S, d = enc_out.shape[1], enc_out.shape[2]
-            rows = enc_out.reshape(B * S, d)
-            offsets = torch.arange(0, (B + 1) * S, S, dtype=torch.int32, device=dev)
-            key_mask = torch.where(enc_mask == 0, torch.finfo(torch.float32).min, 0.0).to(torch.float32).reshape(B * S)
-        ranker = FusedT5Rank(self, levels, rows, offsets, key_mask, attention)
+        ranker = FusedT5Rank(self, *self._rank_encoder(attention_mask, input_ids, user_id, encoder, att), attention)
         chunk = max_rows // per_history
         for b0 in range(0, B, chunk):
-            ranker.run(b0, min(B, b0 + chunk), scores, bad)
+            ranker.run(b0, min(B, b0 + chunk), levels, scores, bad)
         return scores, bad, leaf_key, n_items
 
     @staticmethod
@@ -1107,3 +1160,113 @@ class EncoderDecoderRetrievalModel(nn.Module):
         items, item_scores, rank = ops.t5rank_select(scores, row, start, self._leaf_of(fut[:, :H], leaf_key), fut[:, H], n)
         self._raise_bad(bad, "rank_items")
         return ItemRankingOutput(item_ids=items, scores=item_scores, target_rank=rank, num_items=n_items)
+
+    # ------------------------------------------------------------------------------------------------ scoring given items
+    def _candidate_scores(self, attention_mask, input_ids, user_id, sem_ids: Tensor, encoder, encoder_attention, attention,
+                          max_rows, bad: Tensor, what: str) -> Tensor:
+        """fp32 [B, C]: each candidate tuple's exact log-probability, decoding per history the trie of its own candidates
+        (``ops.t5score_trie_build``, ``FusedT5Rank.run_candidates``); NaN-row counts are added to bad[0]."""
+        encoder, att, attention = self._check_rank_call(encoder, encoder_attention, attention, what)
+        H, K = self.num_hierarchies, self.num_embeddings_per_hierarchy
+        if H > 8 or H * max(1, (K - 1).bit_length()) > 62:
+            raise Rqb200Error(f"{what}: {H} levels of {K} codes do not pack into a 64-bit tuple key (at most 8 levels)")
+        B = attention_mask.shape[0]
+        if sem_ids.dim() != 3 or sem_ids.shape[0] != B or sem_ids.shape[2] != H:
+            raise ValueError(f"{what}: sem_ids {tuple(sem_ids.shape)} must be [B = {B}, C, H = {H}]")
+        C = sem_ids.shape[1]
+        if not 1 <= C <= ops.SCORE_MAX_CANDIDATES:
+            raise ValueError(f"{what}: C = {C} candidates per history must be in [1, {ops.SCORE_MAX_CANDIDATES}]")
+        trie = ops.t5score_trie_build(sem_ids, K)
+        need = [[1] + [max(1, c) for c in row] for row in _read_node_counts(trie.counts)]   # rows per level, n[0] = 1 (BOS)
+        own = max((sum(n[:H]) for n in need), default=0)
+        if max_rows is None:
+            max_rows = max(own, RANK_BYTE_BUDGET // FusedT5Rank.row_bytes(self))
+        elif max_rows < own:
+            raise ValueError(f"{what}: max_rows = {max_rows} is below the {own} decoder rows of one history")
+        scores = torch.empty((B, C), dtype=torch.float32, device=sem_ids.device)
+        if B == 0:
+            return scores
+        chunks, b0 = [], 0                  # histories in order, each chunk as long as its padded levels fit in max_rows
+        while b0 < B:
+            n, b1 = need[b0], b0 + 1
+            while b1 < B:
+                wider = [max(a, c) for a, c in zip(n, need[b1])]
+                if (b1 + 1 - b0) * sum(wider[:H]) > max_rows:
+                    break
+                n, b1 = wider, b1 + 1
+            chunks.append((b0, b1, n))
+            b0 = b1
+        ranker = FusedT5Rank(self, *self._rank_encoder(attention_mask, input_ids, user_id, encoder, att), attention)
+        for b0, b1, n in chunks:
+            ranker.run_candidates(b0, b1, n, trie, scores, bad)
+        return scores
+
+    @staticmethod
+    def _raise_score_errors(counters: Tensor, what: str) -> None:
+        """The one host read at the end of score_sem_ids / score_items: counters[0] the head rows that were not finite,
+        counters[1] the item ids outside [-1, N)."""
+        n_bad, n_items = counters.tolist()
+        if n_items:
+            raise ValueError(f"{what}: {n_items} item id(s) outside [-1, N) where N is the number of corpus rows")
+        if n_bad:
+            raise RuntimeError(f"{what}: {n_bad} decoder row(s) of the head's logits hold a NaN or +inf or are all -inf; the "
+                               "items below them score NaN")
+
+    @torch.no_grad()
+    def score_sem_ids(self, attention_mask, input_ids, user_id=None, sem_ids: Optional[Tensor] = None,
+                      encoder: Optional[str] = None, encoder_attention: Optional[str] = None, attention: Optional[str] = None,
+                      max_rows: Optional[int] = None) -> Tensor:
+        """fp32 [B, C]: the exact log-probability of each of the C candidate tuples (sem_ids integer [B, C, H]) of each history,
+        the quantity ``rank_sem_ids`` gives a corpus tuple (the same kernels, the same log-sum-exp, bit for bit).  A tuple whose
+        ids are all in [0, K) is scored whether or not the corpus holds it; one holding an id outside [0, K) (-1 pads ragged
+        candidate lists) scores -inf; equal tuples score the same.  Each history decodes the trie of its own candidates, one decoder
+        row per node: at most 1 + C (H - 1) rows per history.  ``encoder``, ``encoder_attention``, ``attention`` and ``max_rows``
+        as in ``rank_sem_ids``; C <= ``ops.SCORE_MAX_CANDIDATES``.  Two host reads: the tries' node counts after their build, and
+        the non-finite row count at the end (``RuntimeError`` when some head row was not finite)."""
+        if sem_ids is None:
+            raise ValueError("score_sem_ids: sem_ids [B, C, H] is required")
+        counters = torch.zeros(2, dtype=torch.int32, device=attention_mask.device)
+        scores = self._candidate_scores(attention_mask, input_ids, user_id, sem_ids, encoder, encoder_attention, attention,
+                                        max_rows, counters, "score_sem_ids")
+        self._raise_score_errors(counters, "score_sem_ids")
+        return scores
+
+    @torch.no_grad()
+    def score_items(self, batch: TokenizedSeqBatch, item_ids: Tensor, encoder: Optional[str] = None,
+                    encoder_attention: Optional[str] = None, attention: Optional[str] = None,
+                    max_rows: Optional[int] = None) -> ItemScoreOutput:
+        """The exact log-probability of given corpus items (item_ids int64 [B, C], corpus rows, -1 pads) for each history,
+        through their tuples codebooks[item, :H] (``score_sem_ids``), and the position of ``item_of(batch.sem_ids_fut)`` among the
+        row's items in ``rank_items``' order: score descending, then tuple, then item id (dedup order), NaN last; -1 when the
+        target is not among them.  With the target among C sampled items, ``TopKAccumulator.accumulate_ranks(target_rank, C)``
+        gives the sampled-candidate metrics.  Item ids outside [-1, N) are counted on the device and raise ``ValueError`` after
+        the pass; the host reads are those of ``score_sem_ids``."""
+        ops._need_cuda(item_ids)
+        H, K = self.num_hierarchies, self.num_embeddings_per_hierarchy
+        B = batch.sem_ids.shape[0]
+        if item_ids.dim() != 2 or item_ids.shape[0] != B or item_ids.dtype.is_floating_point or item_ids.dtype == torch.bool:
+            raise ValueError(f"score_items: item_ids must be an integer [B = {B}, C] tensor, got {item_ids.dtype} "
+                             f"{tuple(item_ids.shape)}")
+        items = item_ids.long()
+        cb = self.codebooks[:, :H].to(items.device).long()
+        N = cb.shape[0]
+        ok = (items >= 0) & (items < N)
+        counters = torch.zeros(2, dtype=torch.int32, device=items.device)
+        counters[1:] = (~ok & (items != -1)).sum().view(1)
+        tuples = torch.where(ok[..., None], cb[items.clamp(0, max(N - 1, 0))], -1)
+        scores = self._candidate_scores(
+            _strip_dedup_col(batch.seq_mask.long(), H + 1, H), _strip_dedup_col(batch.sem_ids, H + 1, H), batch.user_ids, tuples,
+            encoder, encoder_attention, attention, max_rows, counters, "score_items")
+        target = self.item_of(batch.sem_ids_fut)[:, None]
+        key = torch.zeros_like(items)
+        for h in range(H):
+            key = key * K + tuples[..., h].clamp(0, K - 1)
+        match = ok & (items == target)
+        pos = match.int().argmax(1, keepdim=True)
+        s_t, key_t = scores.gather(1, pos), key.gather(1, pos)
+        nan, nan_t = scores.isnan(), s_t.isnan()
+        tie = (scores == s_t) | (nan & nan_t)
+        before = ok & ((~nan & nan_t) | (scores > s_t) | (tie & ((key < key_t) | ((key == key_t) & (items < target)))))
+        rank = torch.where(match.any(1), before.sum(1), -1)
+        self._raise_score_errors(counters, "score_items")
+        return ItemScoreOutput(scores=scores, target_rank=rank)

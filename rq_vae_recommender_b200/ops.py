@@ -1093,6 +1093,44 @@ def t5rank_select(scores: torch.Tensor, row: torch.Tensor, start: torch.Tensor, 
     return items, item_scores, rank
 
 
+#: most candidate tuples per history t5score_trie_build takes (its block sort holds them in shared memory)
+SCORE_MAX_CANDIDATES = 4096
+
+
+class CandidateTrie(NamedTuple):
+    """The trie of each history's own candidate tuples (``t5score_trie_build``).  counts int32 [B, H]: entry l - 1 the node count
+    n_l of level l; code / parent int32 [B, H, C]: entry (l - 1, i) node i's last id and its node in level l - 1 (0, 0 for
+    i >= n_l); child int32 [B, H, C + 1]: entry (l, i) for l < H the start of node i's children in level l + 1 (n_{l + 1} for
+    i >= n_l, so node i's children are child[l][i] .. child[l][i + 1] - 1); leaf int32 [B, C]: each candidate's node in level H,
+    -1 when it holds an id outside [0, K).  Nodes of one level are in lexicographic order of their prefixes."""
+    counts: torch.Tensor
+    code: torch.Tensor
+    parent: torch.Tensor
+    child: torch.Tensor
+    leaf: torch.Tensor
+
+
+def t5score_trie_build(ids: torch.Tensor, K: int) -> CandidateTrie:
+    """The candidate trie of every history (rqb200_t5score_trie_build), one launch: ids integer [B, C, H] (C candidate tuples per
+    history) over K codes per level.  C <= ``SCORE_MAX_CANDIDATES``, H <= 8, H * bits(K - 1) <= 62."""
+    _need_cuda(ids)
+    if ids.dim() != 3 or ids.dtype.is_floating_point or ids.dtype.is_complex or ids.dtype == torch.bool:
+        raise ValueError(f"ids must be an integer [B, C, H] tensor, got {ids.dtype} {tuple(ids.shape)}")
+    B, C, H = ids.shape
+    ids = ids.to(torch.int64).contiguous()
+    dev = ids.device
+    counts = torch.empty((B, H), dtype=torch.int32, device=dev)
+    code = torch.empty((B, H, C), dtype=torch.int32, device=dev)
+    parent = torch.empty((B, H, C), dtype=torch.int32, device=dev)
+    child = torch.empty((B, H, C + 1), dtype=torch.int32, device=dev)
+    leaf = torch.empty((B, C), dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.load().rqb200_t5score_trie_build(_p(ids), B, C, H, int(K), _p(counts), _p(code), _p(parent), _p(child),
+                                                         _p(leaf), _stream()), "t5score_trie_build")
+    _count(1)
+    return CandidateTrie(counts, code, parent, child, leaf)
+
+
 # ---------------------------------------------------------------------------------------------- fused T5 encoder pass
 def t5enc_len(n: int, H: int, sep: bool, user: bool) -> int:
     """Positions of the encoder input of n = items * H ids: the user row, then per item its H ids and a separator."""
