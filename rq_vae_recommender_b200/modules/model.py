@@ -3,45 +3,31 @@ the semantic-id kernels.
 
 Same names (``EncoderDecoderRetrievalModel``, ``ModelOutput``, ``GenerationOutput``, ``_strip_dedup_col``), constructor
 signature and ``state_dict`` keys, so decoder checkpoints load with ``strict=True``.  ``forward`` and the encoder / decoder
-passes are plain torch on HF T5, as in the reference.  What differs is the search in ``generate``:
-  * ``_check_valid_prefix`` is a lookup in a prefix index of the corpus id table (``ops.SidPrefixIndex``: a trie of the
-    corpus's prefixes), instead of a compare of every prefix with every corpus row.  The index is built on first use and
+passes are plain torch on HF T5 unless a call (or the ``DEFAULT_*`` switch it falls back to, which ``dropin.install`` sets)
+picks a fused pass.  Shapes outside a kernel's limits raise ``Rqb200Error``; nothing falls back to the reference's code.
+
+The search (``generate``, ``generate_items``):
+  * ``_check_valid_prefix`` is a lookup in a trie of the corpus's id prefixes (``ops.SidPrefixIndex``), built on first use and
     rebuilt when the ``codebooks`` buffer is replaced, written to (``load_state_dict``) or moved;
-  * each hierarchy level runs the head, the softmax, ``draw_exponential`` and ONE kernel (``SidPrefixIndex.sample_select``)
-    that samples, checks the prefixes, scores and keeps the k best.  ``torch.multinomial(p, n)`` without replacement is
-    ``topk(p / q, n)`` with ``q = draw_exponential(p)`` from the same generator, so under the same seed the samples, beams and
-    log-probabilities are the reference's.  Nothing in the level loop waits for the device: rows ``torch.multinomial`` would
-    reject are counted on the device and raise its error after the last level.
-Shapes outside the kernel's limits (codebooks above 2048 codes, top_k * 64 candidates above 1024, top_k above 32) raise
-``Rqb200Error``; there is no fallback to the reference's search.
+  * ``search="sample"``: per level the head, the softmax, ``draw_exponential`` and ONE kernel that samples, checks the prefixes,
+    scores and keeps the k best.  ``torch.multinomial(p, n)`` without replacement is ``topk(p / q, n)`` with
+    ``q = draw_exponential(p)`` from the same generator, so under the same seed the samples, beams and log-probabilities are the
+    reference's.  Nothing in the level loop waits for the device: rows ``torch.multinomial`` would reject are counted on the
+    device and raise its error after the last level;
+  * ``search="beam"``: an exhaustive, deterministic beam search over every code (``SidPrefixIndex.beam_topk``), no sampling;
+  * ``generate_items`` resolves the beams to corpus items with one more launch (``ops.SidItemTable.retrieve``); ``item_of``
+    resolves ``sem_ids_fut`` to the true next item.
 
-``generate_items`` turns the beams into corpus items: one more launch (``ops.SidItemTable.retrieve``) after ``generate``, through
-an item table of ``codebooks`` that is cached like the prefix index.  ``item_of`` resolves ``sem_ids_fut`` (ids plus the dedup
-column) to the true next item.
-
-``generate(..., search="beam")`` runs a different search instead: an exhaustive, deterministic beam search over every code
-(``SidPrefixIndex.beam_topk``: per level the head and ONE kernel that scores all top_k x K extensions by log_softmax plus the
-parent's log-probability and keeps the k best valid ones; no sampling, no draw from any generator).  ``DEFAULT_SEARCH`` picks the
-search when ``generate`` / ``generate_next_sem_id`` are not given one (``dropin.install(search=...)`` sets it).
-
-``generate(..., decoder="fused")`` replaces only the decoder passes and their cache with ``FusedT5Decode`` (the decoder-step kernels
-of csrc/t5dec.cu between cuBLAS GEMMs, cross keys/values once per history, no cache copies); ``DEFAULT_DECODER`` ("hf") picks
-the decoder when none is given (``dropin.install(decoder=...)`` sets it).
-
-``generate(..., encoder="fused")`` replaces only the encoder pass with ``FusedT5Encode`` (the unpadded positions of each history
-only, packed, with the kernels of csrc/t5enc.cu between cuBLAS GEMMs); ``DEFAULT_ENCODER`` ("hf") picks the encoder when none is
-given (``dropin.install(encoder=...)`` sets it).
-
-``forward(batch, encoder="fused")``, the training pass, runs the encoder as ``FusedT5EncodeTrain``: the same packed pass with a
-backward and HF's dropout; ``DEFAULT_FORWARD_ENCODER`` ("hf") picks it when none is given (``dropin.install(forward_encoder=...)``
-sets it).  ``forward(batch, decoder="fused")`` runs the decoder as ``FusedT5DecodeTrain``: the H positions the loss reads, on the
-decoder training kernels of csrc/t5dec.cu with HF's dropout; ``DEFAULT_FORWARD_DECODER`` ("hf") picks it when none is given
-(``dropin.install(forward_decoder=...)`` sets it).  With both fused, the decoder attends to the encoder's packed rows.
+The fused T5 passes, each HF's maths as GEMMs between this project's kernels, described once by ``_T5Weights``:
+  * ``FusedT5Decode`` (``generate(decoder="fused")``) and ``FusedT5Rank`` (exact scoring) run the incremental decoder of
+    ``_T5DecoderLevels``; ``FusedT5Encode`` (``generate(encoder="fused")``) runs the unpadded positions of each history only;
+  * ``FusedT5EncodeTrain`` / ``FusedT5DecodeTrain`` (``forward(encoder="fused")`` / ``forward(decoder="fused")``) are the same
+    passes with a backward and HF's dropout;
+  * ``PackedEncoderOutput`` is the one layout of encoder rows that every offsets-based cross-attention reads.
 
 ``rank_items`` / ``rank_sem_ids`` are an evaluation tool with no search: every corpus item is scored by its exact
-log-probability, one decoder row per corpus-trie node per history (``FusedT5Rank``, csrc/t5rank.cu), and ranked.
-``score_items`` / ``score_sem_ids`` give the same exact log-probability for items the caller chooses, decoding per history the trie
-of its own candidates with the same kernels.
+log-probability, one decoder row per corpus-trie node per history, and ranked.  ``score_items`` / ``score_sem_ids`` give the same
+exact log-probability for items the caller chooses, decoding per history the trie of its own candidates with the same kernels.
 """
 from typing import List
 from typing import NamedTuple
@@ -131,68 +117,122 @@ def _strip_dedup_col(tensor: Tensor, sem_ids_dim: int, n_layers: int) -> Tensor:
     return tensor.view(B, items, sem_ids_dim)[:, :, :n_layers].contiguous().view(B, items * n_layers)
 
 
-class FusedT5Decode:
+
+def _choice(value: Optional[str], default: Optional[str], allowed, what: str, name: str) -> str:
+    """An option string of one call: ``value``, else ``default``; ``ValueError`` when it is not one of ``allowed``."""
+    value = default if value is None else value
+    if value not in allowed:
+        raise ValueError(f"{what}: {name} must be one of {allowed}, got {value!r}")
+    return value
+
+
+def _check_no_autocast(what: str) -> None:
+    if torch.is_autocast_enabled("cuda"):
+        raise ValueError(f"{what} runs fp32 kernels: it cannot run inside an autocast region")
+
+
+class _T5Weights:
+    """One T5 stack (``model.t5_decoder`` or ``model.encoder.encoder``) as the fused passes read it: ``blocks`` (each block's
+    sub-layers), ``norms`` (every sub-layer's T5LayerNorm weight in pass order, then the final norm's), ``heads``, ``eps`` and
+    ``inner`` = heads * d_kv.  The kernels are built for d_kv = 64 and a relu feed-forward: any other config raises."""
+
+    def __init__(self, stack, what: str):
+        cfg = stack.config
+        if cfg.d_kv != ops.T5_DKV or cfg.is_gated_act or cfg.dense_act_fn != "relu":
+            raise Rqb200Error(f"{what} needs d_kv = {ops.T5_DKV} and a relu feed-forward (d_kv = {cfg.d_kv}, "
+                              f"feed_forward_proj = {cfg.feed_forward_proj!r})")
+        self.stack = stack
+        self.blocks = [blk.layer for blk in stack.block]
+        self.norms = [sub.layer_norm.weight for lay in self.blocks for sub in lay] + [stack.final_layer_norm.weight]
+        self.heads, self.eps, self.inner = cfg.num_heads, cfg.layer_norm_epsilon, cfg.num_heads * ops.T5_DKV
+
+    def qkv(self, l: int) -> Tensor:
+        """Layer l's q | k | v self-attention weight, concatenated here: a training pass calls this per step, so autograd reaches
+        the three parameters."""
+        att = self.blocks[l][0].SelfAttention
+        return torch.cat([att.q.weight, att.k.weight, att.v.weight])
+
+    def layer(self, l: int) -> tuple:
+        """Layer l's GEMM weights in pass order: q|k|v, self-attention o, (decoders: cross-attention q, o), wi, wo."""
+        lay = self.blocks[l]
+        cross = (lay[1].EncDecAttention.q.weight, lay[1].EncDecAttention.o.weight) if len(lay) == 3 else ()
+        ff = lay[-1].DenseReluDense
+        return (self.qkv(l), lay[0].SelfAttention.o.weight, *cross, ff.wi.weight, ff.wo.weight)
+
+
+def _linear(x: Tensor, w: Tensor, relu: bool = False) -> Tensor:
+    """x w^T on cuBLAS, the feed-forward's relu in place."""
+    y = F.linear(x, w)
+    return y.relu_() if relu else y
+
+
+class _T5DecoderLevels:
+    """The incremental T5 decoder (eval mode, no 1/sqrt(d), block 0's relative bias) that ``FusedT5Decode`` and ``FusedT5Rank``
+    share: one query position per call of ``level``, between the decoder-step kernels of csrc/t5dec.cu.  The two differ in the
+    GEMM (``linear(x, w, relu=False)`` over weights wrapped by ``operand``) and in the cross-attention kernel, and in nothing
+    else.  Cross keys and values are projected here ONCE from the encoder ``rows``, for every layer in one GEMM: ``cross_kv``
+    [rows, layers * 2 * inner], layer l's keys at columns 2 l inner, its values at (2 l + 1) inner."""
+
+    def __init__(self, model: "EncoderDecoderRetrievalModel", what: str, rows: Tensor, linear, operand=lambda w: w):
+        self.model, self.H, self.linear = model, model.num_hierarchies, linear
+        self.t5 = t5 = _T5Weights(model.t5_decoder, what)
+        self.w = [tuple(operand(w) for w in t5.layer(l)) for l in range(len(t5.blocks))]
+        w_kv = torch.cat([w for lay in t5.blocks for w in (lay[1].EncDecAttention.k.weight, lay[1].EncDecAttention.v.weight)])
+        self.cross_kv = linear(rows, operand(w_kv))
+        self.bias = t5.blocks[0][0].SelfAttention.compute_bias(self.H, self.H)[0].contiguous()
+
+    def level(self, h: int, R: int, ids: Optional[Tensor], parent: Optional[Tensor], cache: Tensor, anc: List[Tensor],
+              cross) -> Tensor:
+        """The final-layer-normed hidden state [R, d_model] of query position h for R rows.  ids [R] are the rows' last codes
+        (None at h = 0: BOS).  Self-attention keys/values of position j live in slot j of ``cache`` [layers, 2, H, >= R, inner];
+        a row reads its past through the int32 ancestor table anc[0] [>= R, H], which this call advances from ``parent`` [R]
+        (each row's row at level h - 1) into anc[1] and then swaps the pair, so no level copies the cache.
+        ``cross(q, k, v)`` is the cross-attention of the R queries over one layer's keys and values."""
+        m, linear, eps, norms, inner = self.model, self.linear, self.t5.eps, self.t5.norms, self.t5.inner
+        x = torch.empty((R, m.bos_token.shape[1]), dtype=torch.float32, device=self.cross_kv.device)
+        nrm = torch.empty_like(x)
+        if ids is None:
+            ops.t5dec_add_norm(x, None, norms[0], nrm, eps, emb=m.bos_token)
+        else:
+            ops.t5dec_add_norm(x, None, norms[0], nrm, eps, emb=m.item_sid_embedding_table.weight, ids=ids,
+                               offset=(h - 1) * m.num_embeddings_per_hierarchy)
+        for l, (w_qkv, w_o, w_q, w_xo, w_i, w_fo) in enumerate(self.w):
+            advance = h > 0 and l == 0
+            a = ops.t5dec_self_attention(linear(nrm, w_qkv), cache[l, 0], cache[l, 1], self.bias, h, anc[0],
+                                         parent if advance else None, anc[1] if advance else None)
+            if advance:
+                anc.reverse()
+            ops.t5dec_add_norm(x, linear(a, w_o), norms[3 * l + 1], nrm, eps)
+            kv = self.cross_kv[:, 2 * l * inner:(2 * l + 2) * inner]
+            a = cross(linear(nrm, w_q), kv[:, :inner], kv[:, inner:])
+            ops.t5dec_add_norm(x, linear(a, w_xo), norms[3 * l + 2], nrm, eps)
+            ops.t5dec_add_norm(x, linear(linear(nrm, w_i, relu=True), w_fo), norms[3 * l + 3], nrm, eps)
+        return nrm
+
+
+class FusedT5Decode(_T5DecoderLevels):
     """The decoder passes of one ``generate(decoder="fused")`` call: HF's T5Stack (eval mode, relu FFN, d_kv 64) restated as
-    cuBLAS GEMMs (``F.linear``) between the decoder-step kernels of csrc/t5dec.cu, with the key/value state laid out so that no
-    level copies it:
-      * cross-attention keys/values are projected ONCE, from the encoder output of the B histories, for every layer in one GEMM
-        (``cross_kv`` [B * S, layers * 2 * inner]), and each history's are read once per level for all of its beams;
-      * self-attention keys/values of position j live in slot j of ``cache`` [layers, 2, H, B * k, inner]; a beam reads its past
-        through an int32 ancestor table [B * k, H] that ``step`` advances from the search's parent_global (no reorder copy);
+    cuBLAS GEMMs (``F.linear``) between the decoder-step kernels, with the key/value state laid out so that no level copies it:
+      * cross-attention keys/values are projected once from the encoder output of the B histories (``cross_kv`` [B * S, ...]),
+        and each history's are read once per level for all of its beams (``t5dec_cross_attention``);
+      * ``cache`` [layers, 2, H, B * k, inner] and the ancestor tables live across the levels; ``step`` advances the tables from
+        the search's parent_global (no reorder copy);
       * level 1 reuses level 0's BOS keys/values: the BOS position depends only on the history.
     ``step(h, generated, parent)`` returns the final-layer-normed hidden state [rows, d_model] of query position h."""
 
     def __init__(self, model: "EncoderDecoderRetrievalModel", enc_out: Tensor, enc_mask: Tensor, k: int):
-        dec = model.t5_decoder
-        cfg = dec.config
-        if cfg.d_kv != ops.T5_DKV or cfg.is_gated_act or cfg.dense_act_fn != "relu":
-            raise Rqb200Error(f"decoder=\"fused\" needs d_kv = {ops.T5_DKV} and a relu feed-forward (d_kv = {cfg.d_kv}, "
-                              f"feed_forward_proj = {cfg.feed_forward_proj!r})")
-        self.model, self.k, self.H = model, k, model.num_hierarchies
-        self.heads, self.eps = cfg.num_heads, cfg.layer_norm_epsilon
-        self.blocks = [blk.layer for blk in dec.block]
-        self.norms = [w for lay in self.blocks for w in (lay[0].layer_norm.weight, lay[1].layer_norm.weight,
-                                                         lay[2].layer_norm.weight)] + [dec.final_layer_norm.weight]
-        self.w_qkv = [torch.cat([lay[0].SelfAttention.q.weight, lay[0].SelfAttention.k.weight, lay[0].SelfAttention.v.weight])
-                      for lay in self.blocks]
         B, S, d = enc_out.shape
-        self.B, self.S, inner = B, S, self.heads * ops.T5_DKV
-        self.inner = inner
-        w_kv = torch.cat([w for lay in self.blocks for w in (lay[1].EncDecAttention.k.weight, lay[1].EncDecAttention.v.weight)])
-        #: [B * S, layers * 2 * inner]: layer l's cross keys at columns 2 l inner, its values at (2 l + 1) inner
-        self.cross_kv = F.linear(enc_out.reshape(B * S, d), w_kv)
+        super().__init__(model, "decoder=\"fused\"", enc_out.reshape(B * S, d), _linear)
+        self.k, self.B, self.S, self.inner = k, B, S, self.t5.inner
         self.mask = enc_mask.to(torch.float32).contiguous()
-        self.bias = dec.block[0].layer[0].SelfAttention.compute_bias(self.H, self.H)[0].contiguous()
-        self.cache = torch.empty((len(self.blocks), 2, self.H, B * k, inner), dtype=torch.float32, device=enc_out.device)
-        self.anc = torch.empty((B * k, self.H), dtype=torch.int32, device=enc_out.device)
-        self._anc_next = torch.empty_like(self.anc)
+        self.cache = torch.empty((len(self.w), 2, self.H, B * k, self.inner), dtype=torch.float32, device=enc_out.device)
+        self.anc = [torch.empty((B * k, self.H), dtype=torch.int32, device=enc_out.device) for _ in range(2)]
 
     def step(self, h: int, generated: Optional[Tensor], parent: Optional[Tensor]) -> Tensor:
-        m, eps, inner = self.model, self.eps, self.inner
         nq = 1 if h == 0 else self.k
         R = self.B * nq
-        x = torch.empty((R, m.bos_token.shape[1]), dtype=torch.float32, device=self.cross_kv.device)
-        nrm = torch.empty_like(x)
-        if h == 0:
-            ops.t5dec_add_norm(x, None, self.norms[0], nrm, eps, emb=m.bos_token)
-        else:
-            ops.t5dec_add_norm(x, None, self.norms[0], nrm, eps, emb=m.item_sid_embedding_table.weight,
-                               ids=generated.reshape(R, h)[:, h - 1], offset=(h - 1) * m.num_embeddings_per_hierarchy)
-        for l, lay in enumerate(self.blocks):
-            advance = h > 0 and l == 0
-            a = ops.t5dec_self_attention(F.linear(nrm, self.w_qkv[l]), self.cache[l, 0], self.cache[l, 1], self.bias, h,
-                                         self.anc, parent if advance else None, self._anc_next if advance else None)
-            if advance:
-                self.anc, self._anc_next = self._anc_next, self.anc
-            ops.t5dec_add_norm(x, F.linear(a, lay[0].SelfAttention.o.weight), self.norms[3 * l + 1], nrm, eps)
-            kv = self.cross_kv[:, 2 * l * inner:(2 * l + 2) * inner]
-            a = ops.t5dec_cross_attention(F.linear(nrm, lay[1].EncDecAttention.q.weight), kv[:, :inner], kv[:, inner:],
-                                          self.mask, nq, self.heads)
-            ops.t5dec_add_norm(x, F.linear(a, lay[1].EncDecAttention.o.weight), self.norms[3 * l + 2], nrm, eps)
-            ff = lay[2].DenseReluDense
-            ops.t5dec_add_norm(x, F.linear(F.linear(nrm, ff.wi.weight).relu_(), ff.wo.weight), self.norms[3 * l + 3], nrm, eps)
-        return nrm
-
+        return self.level(h, R, None if h == 0 else generated.reshape(R, h)[:, h - 1], parent, self.cache, self.anc,
+                          lambda q, k, v: ops.t5dec_cross_attention(q, k, v, self.mask, nq, self.t5.heads))
 
 class ItemRankingOutput(NamedTuple):
     """rank_items: the n best corpus items of each history by exact log-probability (item_ids [B, n] int64, -1 past the corpus),
@@ -218,43 +258,23 @@ RANK_BYTE_BUDGET = 4 << 30
 MAX_RANK_ITEMS = 1024
 
 
-class FusedT5Rank:
+class FusedT5Rank(_T5DecoderLevels):
     """The decoder passes of ``rank_sem_ids``: one decoder row per node of the corpus trie per history.  Items that share an
     l-prefix share the causal decoder's state at positions 0..l, so level h's rows (one per h-prefix node; the root at h = 0) give
-    every child's log-probability, and a leaf's score is the sum along its path.  The maths are ``FusedT5Decode``'s (eval mode,
-    no 1/sqrt(d), block 0's relative bias), with
-      * ``t5dec_add_norm`` gathering ``item_sid_embedding_table[code + (h - 1) K]`` for node rows;
-      * ``t5dec_self_attention`` reading ancestors through the table that each level advances from the node parents, with cache
-        slots sized to the largest level of the chunk;
+    every child's log-probability, and a leaf's score is the sum along its path.  The maths are ``FusedT5Decode``'s, with
+      * node rows' ids and parents taken from the trie, and cache slots sized to the largest level of the chunk;
       * every GEMM on the split-precision tensor-core GEMM (``ops.gemm_split``: fp32-accurate, each output row a function of its
-        input row alone), so the chunking of histories does not change a bit;
-      * cross keys and values projected once for all histories (one GEMM per call), and ``t5rank_cross_attention`` for the level's
-        n_h queries per history over the encoder rows given by offsets and an additive per-row key mask, fp32 on the CUDA cores or
-        (``attention="tf32"``) its products on the TF32 tensor cores;
+        input row alone), so the chunking of histories does not change a bit; the weights' split images are built once per call;
+      * ``t5rank_cross_attention`` for the level's n_h queries per history over the encoder rows given by offsets and an additive
+        per-row key mask, fp32 on the CUDA cores or (``attention="tf32"``) its products on the TF32 tensor cores;
       * after each level's head, ``t5rank_children`` (log-sum-exp as the beam search, child score = parent + log-probability)."""
 
     def __init__(self, model: "EncoderDecoderRetrievalModel", rows: Tensor, offsets: Tensor, key_mask: Tensor,
                  attention: str = "fp32"):
-        dec = model.t5_decoder
-        _check_encoder_config(dec.config, "rank_sem_ids")
-        self.model, self.H = model, model.num_hierarchies
-        self.tf32 = _check_attention(attention) == "tf32"
-        self.heads, self.eps = dec.config.num_heads, dec.config.layer_norm_epsilon
-        self.inner = self.heads * ops.T5_DKV
-        self.blocks = [blk.layer for blk in dec.block]
-        self.norms = [w for lay in self.blocks for w in (lay[0].layer_norm.weight, lay[1].layer_norm.weight,
-                                                         lay[2].layer_norm.weight)] + [dec.final_layer_norm.weight]
-        w = ops.SplitOperand
-        #: per layer, the split images of (qkv, self o, cross q, cross o, wi, wo); then each level's head
-        self.w = [(w(torch.cat([lay[0].SelfAttention.q.weight, lay[0].SelfAttention.k.weight, lay[0].SelfAttention.v.weight])),
-                   w(lay[0].SelfAttention.o.weight), w(lay[1].EncDecAttention.q.weight), w(lay[1].EncDecAttention.o.weight),
-                   w(lay[2].DenseReluDense.wi.weight), w(lay[2].DenseReluDense.wo.weight)) for lay in self.blocks]
-        self.heads_w = [w(mlp.weight) for mlp in model.decoder_mlp]
-        w_kv = torch.cat([t for lay in self.blocks for t in (lay[1].EncDecAttention.k.weight, lay[1].EncDecAttention.v.weight)])
-        #: [rows, layers * 2 * inner]: layer l's cross keys at columns 2 l inner, its values at (2 l + 1) inner
-        self.cross_kv = ops.gemm_split(rows, w(w_kv))
+        super().__init__(model, "rank_sem_ids", rows, ops.gemm_split, ops.SplitOperand)
+        self.tf32 = _choice(attention, None, ENCODER_ATTENTIONS, "FusedT5Rank", "attention") == "tf32"
+        self.heads_w = [ops.SplitOperand(mlp.weight) for mlp in model.decoder_mlp]
         self.offsets, self.key_mask = offsets, key_mask
-        self.bias = dec.block[0].layer[0].SelfAttention.compute_bias(self.H, self.H)[0].contiguous()
 
     @staticmethod
     def row_bytes(model: "EncoderDecoderRetrievalModel") -> int:
@@ -301,36 +321,19 @@ class FusedT5Rank:
         level h - 1.  After the level's head, ``t5rank_children`` writes the children's scores to nxt[h] ([G, n_next]: the level's
         rows as G equal groups, child[h] int32 the child ranges of one group's rows, code[h] int32 [n_next] the children's last
         codes, nxt[h - 1] the rows' own scores)."""
-        m, eps, inner, H = self.model, self.eps, self.inner, self.H
         Bc, dev = b1 - b0, self.cross_kv.device
         rows = Bc * max(n)
-        cache = torch.empty((len(self.blocks), 2, H, rows, inner), dtype=torch.float32, device=dev)
-        anc = torch.zeros((rows, H), dtype=torch.int32, device=dev)
-        anc_next = torch.empty_like(anc)
+        cache = torch.empty((len(self.w), 2, self.H, rows, self.t5.inner), dtype=torch.float32, device=dev)
+        anc = [torch.zeros((rows, self.H), dtype=torch.int32, device=dev)]
+        anc.append(torch.empty_like(anc[0]))
         offsets = self.offsets[b0:b1 + 1]
         score = None
-        for h in range(H):
+        for h in range(self.H):
             n_h = n[h]
             R = Bc * n_h
-            x = torch.empty((R, m.bos_token.shape[1]), dtype=torch.float32, device=dev)
-            nrm = torch.empty_like(x)
-            if h == 0:
-                ops.t5dec_add_norm(x, None, self.norms[0], nrm, eps, emb=m.bos_token)
-            else:
-                ops.t5dec_add_norm(x, None, self.norms[0], nrm, eps, emb=m.item_sid_embedding_table.weight, ids=ids[h],
-                                   offset=(h - 1) * m.num_embeddings_per_hierarchy)
-            for l, (w_qkv, w_o, w_q, w_xo, w_i, w_fo) in enumerate(self.w):
-                advance = h > 0 and l == 0
-                a = ops.t5dec_self_attention(ops.gemm_split(nrm, w_qkv), cache[l, 0], cache[l, 1], self.bias, h, anc,
-                                             parent[h] if advance else None, anc_next if advance else None)
-                if advance:
-                    anc, anc_next = anc_next, anc
-                ops.t5dec_add_norm(x, ops.gemm_split(a, w_o), self.norms[3 * l + 1], nrm, eps)
-                kv = self.cross_kv[:, 2 * l * inner:(2 * l + 2) * inner]
-                a = ops.t5rank_cross_attention(ops.gemm_split(nrm, w_q), kv[:, :inner], kv[:, inner:], offsets, self.key_mask,
-                                               n_h, self.heads, tf32=self.tf32)
-                ops.t5dec_add_norm(x, ops.gemm_split(a, w_xo), self.norms[3 * l + 2], nrm, eps)
-                ops.t5dec_add_norm(x, ops.gemm_split(ops.gemm_split(nrm, w_i, relu=True), w_fo), self.norms[3 * l + 3], nrm, eps)
+            nrm = self.level(h, R, ids[h], parent[h], cache, anc,
+                             lambda q, k, v: ops.t5rank_cross_attention(q, k, v, offsets, self.key_mask, n_h, self.t5.heads,
+                                                                        tf32=self.tf32))
             ops.t5rank_children(ops.gemm_split(nrm, self.heads_w[h]), score, child[h], code[h], R // nxt[h].shape[0], nxt[h], bad)
             score = nxt[h]
 
@@ -338,19 +341,11 @@ class FusedT5Rank:
 def _encoder_attention(encoder: str, encoder_attention: Optional[str], what: str) -> str:
     """The fused encoder's attention precision of one call: ``encoder_attention``, else ``DEFAULT_ENCODER_ATTENTION``.  An explicit
     "tf32" with encoder="hf" raises: HF's attention runs at torch's matmul precision, and the switch would be ignored."""
-    att = DEFAULT_ENCODER_ATTENTION if encoder_attention is None else encoder_attention
-    if att not in ENCODER_ATTENTIONS:
-        raise ValueError(f"{what}: encoder_attention must be one of {ENCODER_ATTENTIONS}, got {att!r}")
+    att = _choice(encoder_attention, DEFAULT_ENCODER_ATTENTION, ENCODER_ATTENTIONS, what, "encoder_attention")
     if encoder_attention == "tf32" and encoder != "fused":
         raise ValueError(f"{what}: encoder_attention=\"tf32\" selects the fused encoder's attention kernels; with "
                          f"encoder={encoder!r} the attention follows torch.get_float32_matmul_precision()")
     return att
-
-
-def _check_attention(attention: str) -> str:
-    if attention not in ENCODER_ATTENTIONS:
-        raise ValueError(f"encoder attention must be one of {ENCODER_ATTENTIONS}, got {attention!r}")
-    return attention
 
 
 def _read_n_kept(offsets: Tensor) -> int:
@@ -365,6 +360,51 @@ def _read_node_counts(counts: Tensor) -> List[List[int]]:
     return counts.tolist()
 
 
+class PackedEncoderOutput(NamedTuple):
+    """An encoder pass as rows: rows [N, d_model] (history b's are rows offsets[b] .. offsets[b + 1] - 1, in position order),
+    offsets int32 [B + 1], S encoder positions per history and enc_mask [B, S], the mask ``encoder_forward_pass`` returns.
+    ``packed`` of the fused encoders keeps only some positions and adds key_mask fp32 [B] (finfo(float32).min for a history
+    without an unmasked position), src int32 [N] (b * S + position of each row) and slot int32 [B, S] (row of each position or
+    -1); ``of_padded`` (every position a row) leaves the three None."""
+    rows: Tensor
+    offsets: Tensor
+    key_mask: Optional[Tensor]
+    src: Optional[Tensor]
+    slot: Optional[Tensor]
+    S: int
+    enc_mask: Tensor
+
+    @classmethod
+    def of_padded(cls, enc_out: Tensor, enc_mask: Tensor) -> "PackedEncoderOutput":
+        """HF's encoder output [B, S, d_model] and its mask [B, S]: history b's rows are b * S .. b * S + S - 1."""
+        B, S, d = enc_out.shape
+        offsets = torch.arange(0, (B + 1) * S, S, dtype=torch.int32, device=enc_out.device)
+        return cls(enc_out.reshape(B * S, d), offsets, None, None, None, S, enc_mask)
+
+    def keys(self):
+        """(rows, offsets, additive key mask fp32 [N], src, S): what the offsets-based cross-attentions take.  A padded layout
+        masks the rows whose enc_mask is 0; a packed one holds kept positions only, so a row takes its history's key_mask."""
+        if self.src is None:
+            key_mask = torch.where(self.enc_mask == 0, torch.finfo(torch.float32).min, 0.0).to(torch.float32).reshape(-1)
+        else:
+            key_mask = self.key_mask.index_select(0, torch.div(self.src, self.S, rounding_mode="floor").long())
+        return self.rows, self.offsets, key_mask, self.src, self.S
+
+
+def _encoder_mask(model: "EncoderDecoderRetrievalModel", attention_mask: Tensor, user: bool) -> Tensor:
+    """``encoder_forward_pass``'s mask [B, S] of the ids' mask [B, n]: each item's separator takes the mask of the item's last
+    id, and the user column is ones."""
+    B, n = attention_mask.shape
+    H = model.num_hierarchies
+    enc_mask = attention_mask
+    if model.sep_token is not None:
+        items = enc_mask.view(B, n // H, H)
+        enc_mask = torch.cat([items, items[:, :, -1:]], dim=2).reshape(B, n // H * (H + 1))
+    if user:
+        enc_mask = torch.cat([torch.ones(B, 1, device=enc_mask.device), enc_mask], dim=1)
+    return enc_mask
+
+
 class FusedT5Encode:
     """The encoder pass of ``generate(encoder="fused")``: ``encoder_forward_pass`` (HF's T5EncoderModel in eval mode, relu FFN,
     d_kv 64) restated over the KEPT positions of each history only, as cuBLAS GEMMs (``F.linear``) between the kernels of
@@ -376,58 +416,41 @@ class FusedT5Encode:
         relative-position bias at each row's ORIGINAL position (``compute_bias(S, S)`` of block 0, once per call);
       * ``__call__`` returns what ``encoder_forward_pass`` returns: enc_out [B, S, d_model] with the rows of dropped positions
         set to 0, and enc_mask [B, S] with the same values.
-    N is read on the host once per call (``_read_n_kept``) to size the GEMMs; it is the pass's only host synchronisation.
-    ``attention`` picks the self-attention kernel: "fp32" (``ops.t5enc_attention``) or "tf32" (``ops.t5enc_attention_tc``)."""
+    N is read on the host once per call (``_read_n_kept``) to size the GEMMs; it is the pass's only host synchronisation, and
+    ``n_kept`` keeps the last call's.  ``attention`` picks the self-attention kernel: "fp32" (``ops.t5enc_attention``) or "tf32"
+    (``ops.t5enc_attention_tc``)."""
 
     def __init__(self, model: "EncoderDecoderRetrievalModel", attention: str = "fp32"):
-        enc = model.encoder.encoder
-        cfg = enc.config
-        if cfg.d_kv != ops.T5_DKV or cfg.is_gated_act or cfg.dense_act_fn != "relu":
-            raise Rqb200Error(f"encoder=\"fused\" needs d_kv = {ops.T5_DKV} and a relu feed-forward (d_kv = {cfg.d_kv}, "
-                              f"feed_forward_proj = {cfg.feed_forward_proj!r})")
-        self.model, self.eps = model, cfg.layer_norm_epsilon
-        self.attention = ops.t5enc_attention_tc if _check_attention(attention) == "tf32" else ops.t5enc_attention
-        self.blocks = [blk.layer for blk in enc.block]
-        self.w_qkv = [torch.cat([lay[0].SelfAttention.q.weight, lay[0].SelfAttention.k.weight, lay[0].SelfAttention.v.weight])
-                      for lay in self.blocks]
-        self.norms = [w for lay in self.blocks for w in (lay[0].layer_norm.weight, lay[1].layer_norm.weight)] + \
-            [enc.final_layer_norm.weight]
+        self.model = model
+        self.t5 = _T5Weights(model.encoder.encoder, "encoder=\"fused\"")
+        tf32 = _choice(attention, None, ENCODER_ATTENTIONS, "FusedT5Encode", "attention") == "tf32"
+        self.attention = ops.t5enc_attention_tc if tf32 else ops.t5enc_attention
+        self.w = [self.t5.layer(l) for l in range(len(self.t5.blocks))]
         self.n_kept = None
 
     def __call__(self, attention_mask: Tensor, input_ids: Tensor, user_id: Optional[Tensor] = None):
-        nrm, slot, enc_mask = self.packed(attention_mask, input_ids, user_id)
-        return ops.t5enc_scatter(nrm, slot), enc_mask
+        out = self.packed(attention_mask, input_ids, user_id)
+        return ops.t5enc_scatter(out.rows, out.slot), out.enc_mask
 
-    def packed(self, attention_mask: Tensor, input_ids: Tensor, user_id: Optional[Tensor] = None):
-        """The pass without the scatter: (the kept rows [N, d_model], slot [B, S], enc_mask [B, S]); ``offsets``, ``key_mask``
-        and ``src`` of the packing are left on the object."""
-        m, eps = self.model, self.eps
+    def packed(self, attention_mask: Tensor, input_ids: Tensor, user_id: Optional[Tensor] = None) -> PackedEncoderOutput:
+        """The pass without the scatter: the kept rows [N, d_model] and their layout."""
+        m, eps, norms = self.model, self.t5.eps, self.t5.norms
         H = m.num_hierarchies
         sep = m.sep_token is not None
         user = user_id is not None and m.user_embedding is not None
-        B, n = attention_mask.shape
-        enc_mask = attention_mask
-        if sep:                                               # encoder_forward_pass's mask: the separator takes the item's last
-            items = enc_mask.view(B, n // H, H)
-            enc_mask = torch.cat([items, items[:, :, -1:]], dim=2).reshape(B, n // H * (H + 1))
-        if user:
-            enc_mask = torch.cat([torch.ones(B, 1, device=enc_mask.device), enc_mask], dim=1)
-        self.offsets, self.key_mask = ops.t5enc_offsets(attention_mask, H, sep, user)
-        key_mask = self.key_mask
-        self.n_kept = _read_n_kept(self.offsets)
-        x, nrm, self.src, slot = ops.t5enc_assemble(
+        enc_mask = _encoder_mask(m, attention_mask, user)
+        offsets, key_mask = ops.t5enc_offsets(attention_mask, H, sep, user)
+        self.n_kept = _read_n_kept(offsets)
+        x, nrm, src, slot = ops.t5enc_assemble(
             attention_mask, input_ids, user_id if user else None, m.item_sid_embedding_table.weight, m.sep_token if sep else None,
-            m.user_embedding.weight if user else None, m.num_embeddings_per_hierarchy, H, self.offsets, self.n_kept,
-            self.norms[0], eps)
+            m.user_embedding.weight if user else None, m.num_embeddings_per_hierarchy, H, offsets, self.n_kept, norms[0], eps)
         S = slot.shape[1]
-        rel = ops.t5enc_rel_bias(self.blocks[0][0].SelfAttention.compute_bias(S, S)[0])
-        for l, lay in enumerate(self.blocks):
-            a = self.attention(F.linear(nrm, self.w_qkv[l]), self.src, self.offsets, key_mask, rel, S)
-            ops.t5dec_add_norm(x, F.linear(a, lay[0].SelfAttention.o.weight), self.norms[2 * l + 1], nrm, eps)
-            ff = lay[1].DenseReluDense
-            ops.t5dec_add_norm(x, F.linear(F.linear(nrm, ff.wi.weight).relu_(), ff.wo.weight), self.norms[2 * l + 2], nrm, eps)
-        return nrm, slot, enc_mask
-
+        rel = ops.t5enc_rel_bias(self.t5.blocks[0][0].SelfAttention.compute_bias(S, S)[0])
+        for l, (w_qkv, w_o, w_i, w_fo) in enumerate(self.w):
+            a = self.attention(F.linear(nrm, w_qkv), src, offsets, key_mask, rel, S)
+            ops.t5dec_add_norm(x, F.linear(a, w_o), norms[2 * l + 1], nrm, eps)
+            ops.t5dec_add_norm(x, F.linear(_linear(nrm, w_i, relu=True), w_fo), norms[2 * l + 2], nrm, eps)
+        return PackedEncoderOutput(nrm, offsets, key_mask, src, slot, S, enc_mask)
 
 def _encoder_layout(n: int, H: int, sep: bool, user: bool, device) -> Tensor:
     """[3, S] per encoder position: kind (0 user row, 1 item id, 2 separator), the column of the [B, n] inputs it reads and the id's
@@ -516,14 +539,38 @@ def _rel_bias(att, S: int) -> Tensor:
     return _RelBiasFunction.apply(att.relative_attention_bias.weight, buckets.long())
 
 
-def _check_encoder_config(cfg, what: str) -> None:
-    if cfg.d_kv != ops.T5_DKV or cfg.is_gated_act or cfg.dense_act_fn != "relu":
-        raise Rqb200Error(f"{what} needs d_kv = {ops.T5_DKV} and a relu feed-forward (d_kv = {cfg.d_kv}, "
-                          f"feed_forward_proj = {cfg.feed_forward_proj!r})")
-
-
 #: longest encoder sequence the training attention's backward takes (one shared-memory bin array of 2S - 1 floats per warp)
 MAX_TRAIN_ENCODER_LEN = 5120
+
+
+# What the two training passes share.  Dropout follows HF: each site's probability is read at call time from its module when that
+# module is in training mode (0 else), and the draws come from torch's generator in HF's order.
+def _p(mod) -> float:
+    return float(mod.p) if mod.training else 0.0
+
+
+def _attention_dropout(att, device):
+    """(p, seed) of one attention site: the attention-weight dropout's probability and, when it is on, a fresh seed for the
+    kernel's Philox stream drawn from torch's generator."""
+    p = float(att.dropout) if att.training else 0.0
+    return p, ops.t5enc_dropout_seed(device) if p > 0 else torch.zeros(1, dtype=torch.int64, device=device)
+
+
+def _train_sublayer(x: Tensor, out: Tensor, sub, weight: Tensor, eps: float):
+    """The end of sub-layer ``sub``: x + dropout(out), then the next T5LayerNorm -> (x, nrm)."""
+    return ops.T5EncAddNormFunction.apply(x, dropout_rows(out, _p(sub.dropout)), weight, eps)
+
+
+def _train_feed_forward(x: Tensor, nrm: Tensor, sub, weight: Tensor, eps: float):
+    """The feed-forward sub-layer ``sub``: wi, relu, dropout, wo, then ``_train_sublayer``."""
+    ff = sub.DenseReluDense
+    h = dropout_rows(F.relu(F.linear(nrm, ff.wi.weight)), _p(ff.dropout))
+    return _train_sublayer(x, F.linear(h, ff.wo.weight), sub, weight, eps)
+
+
+def _check_fp32_parameters(model: nn.Module, what: str) -> None:
+    if any(t.dtype != torch.float32 for t in model.parameters()):
+        raise Rqb200Error(f"{what} needs fp32 parameters")
 
 
 class FusedT5EncodeTrain:
@@ -536,51 +583,32 @@ class FusedT5EncodeTrain:
       * ``F.linear`` for every GEMM and ``_ScatterFunction`` back to [B, S, d_model];
     ``rel`` holds the values of ``t5enc_rel_bias(compute_bias(S, S)[0])`` of block 0 (``_rel_bias``: a gather of
     ``relative_attention_bias`` at the buckets of distances -(S - 1) .. S - 1), so its gradient reaches that table summed over the
-    layers, as in HF, through a deterministic sum.  Dropout follows HF: embedding, attention weights, attention output, feed-forward inner and
-    output, final output, each with its module's probability read at call time when that module is in training mode (0 else).
-    The token-wise sites call ``dropout_rows``.  fp32 parameters only; an active autocast region raises ``ValueError``.
-    ``attention`` picks the attention kernels: "fp32" (``ops.T5EncAttentionFunction``) or "tf32"
+    layers, as in HF, through a deterministic sum.  Dropout sites: embedding, attention weights, attention output, feed-forward
+    inner and output, final output.  The token-wise sites call ``dropout_rows``.  fp32 parameters only; an active autocast region
+    raises ``ValueError``.  ``attention`` picks the attention kernels: "fp32" (``ops.T5EncAttentionFunction``) or "tf32"
     (``ops.T5EncAttentionTCFunction``, the same keep bits under the same seed)."""
 
     def __init__(self, model: "EncoderDecoderRetrievalModel", attention: str = "fp32"):
-        enc = model.encoder.encoder
-        _check_encoder_config(enc.config, "encoder=\"fused\"")
-        if any(t.dtype != torch.float32 for t in model.parameters()):
-            raise Rqb200Error("forward(encoder=\"fused\") needs fp32 parameters")
-        self.model, self.enc, self.eps = model, enc, enc.config.layer_norm_epsilon
-        self.attention = ops.T5EncAttentionTCFunction if _check_attention(attention) == "tf32" else ops.T5EncAttentionFunction
-        self.blocks = [blk.layer for blk in enc.block]
-        self.norms = [w for lay in self.blocks for w in (lay[0].layer_norm.weight, lay[1].layer_norm.weight)] + \
-            [enc.final_layer_norm.weight]
-
-    @staticmethod
-    def _p(mod) -> float:
-        return float(mod.p) if mod.training else 0.0
+        self.model = model
+        self.t5 = _T5Weights(model.encoder.encoder, "encoder=\"fused\"")
+        _check_fp32_parameters(model, "forward(encoder=\"fused\")")
+        tf32 = _choice(attention, None, ENCODER_ATTENTIONS, "FusedT5EncodeTrain", "attention") == "tf32"
+        self.attention = ops.T5EncAttentionTCFunction if tf32 else ops.T5EncAttentionFunction
 
     def __call__(self, attention_mask: Tensor, input_ids: Tensor, user_id: Optional[Tensor] = None):
         """(enc_out [B, S, d_model] with the rows of dropped positions 0, enc_mask [B, S]), as ``encoder_forward_pass``."""
         out = self.packed(attention_mask, input_ids, user_id)
-        H = self.model.num_hierarchies
-        sep = self.model.sep_token is not None
-        B, n = attention_mask.shape
-        enc_mask = attention_mask
-        if sep:
-            items = enc_mask.view(B, n // H, H)
-            enc_mask = torch.cat([items, items[:, :, -1:]], dim=2).reshape(B, n // H * (H + 1))
-        if user_id is not None and self.model.user_embedding is not None:
-            enc_mask = torch.cat([torch.ones(B, 1, device=enc_mask.device), enc_mask], dim=1)
-        return _ScatterFunction.apply(out.rows, out.slot, out.src), enc_mask
+        return _ScatterFunction.apply(out.rows, out.slot, out.src), out.enc_mask
 
-    def packed(self, attention_mask: Tensor, input_ids: Tensor, user_id: Optional[Tensor] = None) -> "PackedEncoderOutput":
+    def packed(self, attention_mask: Tensor, input_ids: Tensor, user_id: Optional[Tensor] = None) -> PackedEncoderOutput:
         """The pass without the scatter: the kept rows [N, d_model] (the encoder's final dropout applied) and their layout."""
-        if torch.is_autocast_enabled("cuda"):
-            raise ValueError("forward(encoder=\"fused\") runs fp32 kernels: it cannot run inside an autocast region")
-        m, enc, eps = self.model, self.enc, self.eps
+        _check_no_autocast("forward(encoder=\"fused\")")
+        m, t5, eps, norms = self.model, self.t5, self.t5.eps, self.t5.norms
+        enc = t5.stack
         H = m.num_hierarchies
         sep = m.sep_token is not None
         user = user_id is not None and m.user_embedding is not None
-        n = attention_mask.shape[1]
-        S = ops.t5enc_len(n, H, sep, user)
+        S = ops.t5enc_len(attention_mask.shape[1], H, sep, user)
         if S > MAX_TRAIN_ENCODER_LEN:
             raise Rqb200Error(f"forward(encoder=\"fused\"): {S} encoder positions exceed {MAX_TRAIN_ENCODER_LEN}")
         offsets, key_mask = ops.t5enc_offsets(attention_mask, H, sep, user)
@@ -588,35 +616,16 @@ class FusedT5EncodeTrain:
         x, src, slot = _AssembleFunction.apply(
             m.item_sid_embedding_table.weight, m.sep_token if sep else None, m.user_embedding.weight if user else None,
             attention_mask, input_ids, user_id if user else None, m.num_embeddings_per_hierarchy, H, offsets, n_kept,
-            self.norms[0], eps)
-        x, nrm = ops.T5EncAddNormFunction.apply(dropout_rows(x, self._p(enc.dropout)), None, self.norms[0], eps)
-        rel = _rel_bias(self.blocks[0][0].SelfAttention, S)
-        for l, lay in enumerate(self.blocks):
-            att = lay[0].SelfAttention
-            p_att = float(att.dropout) if att.training else 0.0
-            seed = ops.t5enc_dropout_seed(x.device) if p_att > 0 else torch.zeros(1, dtype=torch.int64, device=x.device)
-            qkv = F.linear(nrm, torch.cat([att.q.weight, att.k.weight, att.v.weight]))
-            a = self.attention.apply(qkv, rel, src, offsets, key_mask, S, seed, p_att)
-            x, nrm = ops.T5EncAddNormFunction.apply(x, dropout_rows(F.linear(a, att.o.weight), self._p(lay[0].dropout)),
-                                                    self.norms[2 * l + 1], eps)
-            ff = lay[1].DenseReluDense
-            h = dropout_rows(F.relu(F.linear(nrm, ff.wi.weight)), self._p(ff.dropout))
-            x, nrm = ops.T5EncAddNormFunction.apply(x, dropout_rows(F.linear(h, ff.wo.weight), self._p(lay[1].dropout)),
-                                                    self.norms[2 * l + 2], eps)
-        return PackedEncoderOutput(dropout_rows(nrm, self._p(enc.dropout)), offsets, key_mask, src, slot, S)
-
-
-class PackedEncoderOutput(NamedTuple):
-    """``FusedT5EncodeTrain.packed``: rows [N, d_model] (history b's kept positions are rows offsets[b] .. offsets[b + 1] - 1, in
-    position order), offsets int32 [B + 1], key_mask fp32 [B] (finfo(float32).min for a history without an unmasked position),
-    src int32 [N] (b * S + position of each row), slot int32 [B, S] (row of each position or -1) and S."""
-    rows: Tensor
-    offsets: Tensor
-    key_mask: Tensor
-    src: Tensor
-    slot: Tensor
-    S: int
-
+            norms[0], eps)
+        x, nrm = ops.T5EncAddNormFunction.apply(dropout_rows(x, _p(enc.dropout)), None, norms[0], eps)
+        rel = _rel_bias(t5.blocks[0][0].SelfAttention, S)
+        for l, lay in enumerate(t5.blocks):
+            p_att, seed = _attention_dropout(lay[0].SelfAttention, x.device)
+            a = self.attention.apply(F.linear(nrm, t5.qkv(l)), rel, src, offsets, key_mask, S, seed, p_att)
+            x, nrm = _train_sublayer(x, F.linear(a, lay[0].SelfAttention.o.weight), lay[0], norms[2 * l + 1], eps)
+            x, nrm = _train_feed_forward(x, nrm, lay[1], norms[2 * l + 2], eps)
+        return PackedEncoderOutput(dropout_rows(nrm, _p(enc.dropout)), offsets, key_mask, src, slot, S,
+                                   _encoder_mask(m, attention_mask, user))
 
 class _DecoderInputFunction(torch.autograd.Function):
     """The decoder's input rows x [B * T, d]: row b * T + t is bos for t = 0 and table[ids[b, t - 1] + (t - 1) K] after.  The
@@ -645,6 +654,10 @@ class _DecoderInputFunction(torch.autograd.Function):
         return d_table, d_bos, None, None, None
 
 
+#: most decoder positions (hierarchy levels) the decoder's training kernels take
+MAX_TRAIN_DECODER_LEN = 8
+
+
 class FusedT5DecodeTrain:
     """The decoder pass of ``forward(decoder="fused")``: HF's T5Stack decoder (relu FFN, d_kv 64) over the T = H positions the loss
     reads (causality makes them independent of HF's extra last position), as cuBLAS GEMMs (``F.linear``) between the training
@@ -652,8 +665,8 @@ class FusedT5DecodeTrain:
       * ``_DecoderInputFunction`` (gradient into ``item_sid_embedding_table`` and ``bos_token``, deterministic),
       * ``ops.T5EncAddNormFunction`` at every norm,
       * ``ops.T5DecSelfAttentionFunction`` (causal, block 0's unidirectional relative bias from ``_rel_bias``) and
-        ``ops.T5DecCrossAttentionFunction`` over the encoder rows given by ``offsets`` and a per-key additive mask: the packed rows
-        of ``FusedT5EncodeTrain.packed`` or the [B * S] rows of HF's encoder.  Cross keys and values are one GEMM per layer on
+        ``ops.T5DecCrossAttentionFunction`` over the encoder rows of ``PackedEncoderOutput.keys``: the packed rows of
+        ``FusedT5EncodeTrain.packed`` or the [B * S] rows of HF's encoder.  Cross keys and values are one GEMM per layer on
         those rows.  Attention-weight dropout draws one seed per attention site and layer from torch's generator, the bits keyed
         on the key's ORIGINAL encoder position, so both encoders give the same bits under one seed;
       * HF's token-wise dropout sites through ``dropout_rows``.
@@ -661,57 +674,54 @@ class FusedT5DecodeTrain:
     region raises ``ValueError``."""
 
     def __init__(self, model: "EncoderDecoderRetrievalModel"):
-        dec = model.t5_decoder
-        _check_encoder_config(dec.config, "decoder=\"fused\"")
+        self.model = model
+        self.t5 = _T5Weights(model.t5_decoder, "decoder=\"fused\"")
         if model.num_hierarchies > MAX_TRAIN_DECODER_LEN:
             raise Rqb200Error(f"forward(decoder=\"fused\"): {model.num_hierarchies} levels exceed {MAX_TRAIN_DECODER_LEN}")
-        if any(t.dtype != torch.float32 for t in model.parameters()):
-            raise Rqb200Error("forward(decoder=\"fused\") needs fp32 parameters")
-        self.model, self.dec, self.eps = model, dec, dec.config.layer_norm_epsilon
-        self.blocks = [blk.layer for blk in dec.block]
-        self.norms = [w for lay in self.blocks for w in (lay[0].layer_norm.weight, lay[1].layer_norm.weight,
-                                                         lay[2].layer_norm.weight)] + [dec.final_layer_norm.weight]
-
-    _p = staticmethod(FusedT5EncodeTrain._p)
-
-    @staticmethod
-    def _seed(att, device):
-        p = float(att.dropout) if att.training else 0.0
-        return p, ops.t5enc_dropout_seed(device) if p > 0 else torch.zeros(1, dtype=torch.int64, device=device)
+        _check_fp32_parameters(model, "forward(decoder=\"fused\")")
 
     def __call__(self, fut_ids: Tensor, rows: Tensor, offsets: Tensor, key_mask: Tensor, src: Optional[Tensor], S: int) -> Tensor:
         """fut_ids [B, >= T - 1]; rows [*, d_model] the encoder rows, history b's keys rows offsets[b] .. offsets[b + 1] - 1 with
         additive key_mask [rows]; src [rows] (b * S + position) or None (row - offsets[b] is the position)."""
-        if torch.is_autocast_enabled("cuda"):
-            raise ValueError("forward(decoder=\"fused\") runs fp32 kernels: it cannot run inside an autocast region")
-        m, dec, eps = self.model, self.dec, self.eps
+        _check_no_autocast("forward(decoder=\"fused\")")
+        m, t5, eps, norms = self.model, self.t5, self.t5.eps, self.t5.norms
+        dec = t5.stack
         T, B = m.num_hierarchies, fut_ids.shape[0]
         x = _DecoderInputFunction.apply(m.item_sid_embedding_table.weight, m.bos_token, fut_ids, m.num_embeddings_per_hierarchy, T)
-        x, nrm = ops.T5EncAddNormFunction.apply(dropout_rows(x, self._p(dec.dropout)), None, self.norms[0], eps)
-        rel = _rel_bias(self.blocks[0][0].SelfAttention, T)
-        for l, lay in enumerate(self.blocks):
-            att = lay[0].SelfAttention
-            p_att, seed = self._seed(att, x.device)
-            a = ops.T5DecSelfAttentionFunction.apply(F.linear(nrm, torch.cat([att.q.weight, att.k.weight, att.v.weight])), rel, T,
-                                                     seed, p_att)
-            x, nrm = ops.T5EncAddNormFunction.apply(x, dropout_rows(F.linear(a, att.o.weight), self._p(lay[0].dropout)),
-                                                    self.norms[3 * l + 1], eps)
+        x, nrm = ops.T5EncAddNormFunction.apply(dropout_rows(x, _p(dec.dropout)), None, norms[0], eps)
+        rel = _rel_bias(t5.blocks[0][0].SelfAttention, T)
+        for l, lay in enumerate(t5.blocks):
+            p_att, seed = _attention_dropout(lay[0].SelfAttention, x.device)
+            a = ops.T5DecSelfAttentionFunction.apply(F.linear(nrm, t5.qkv(l)), rel, T, seed, p_att)
+            x, nrm = _train_sublayer(x, F.linear(a, lay[0].SelfAttention.o.weight), lay[0], norms[3 * l + 1], eps)
             ca = lay[1].EncDecAttention
-            p_ca, seed = self._seed(ca, x.device)
+            p_ca, seed = _attention_dropout(ca, x.device)
             kv = F.linear(rows, torch.cat([ca.k.weight, ca.v.weight]))
             a = ops.T5DecCrossAttentionFunction.apply(F.linear(nrm, ca.q.weight), kv, offsets, key_mask, src, S, T, seed, p_ca)
-            x, nrm = ops.T5EncAddNormFunction.apply(x, dropout_rows(F.linear(a, ca.o.weight), self._p(lay[1].dropout)),
-                                                    self.norms[3 * l + 2], eps)
-            ff = lay[2].DenseReluDense
-            h = dropout_rows(F.relu(F.linear(nrm, ff.wi.weight)), self._p(ff.dropout))
-            x, nrm = ops.T5EncAddNormFunction.apply(x, dropout_rows(F.linear(h, ff.wo.weight), self._p(lay[2].dropout)),
-                                                    self.norms[3 * l + 3], eps)
-        return dropout_rows(nrm, self._p(dec.dropout)).view(B, T, -1)
+            x, nrm = _train_sublayer(x, F.linear(a, ca.o.weight), lay[1], norms[3 * l + 2], eps)
+            x, nrm = _train_feed_forward(x, nrm, lay[2], norms[3 * l + 3], eps)
+        return dropout_rows(nrm, _p(dec.dropout)).view(B, T, -1)
 
 
-#: most decoder positions (hierarchy levels) the decoder's training kernels take
-MAX_TRAIN_DECODER_LEN = 8
+def _tuple_key(tuples: Tensor, K: int) -> Tensor:
+    """int64 [...]: the ids of tuples [..., H] packed into one key, level 0 most significant, so keys order as the tuples do
+    (lexicographically).  Ids outside [0, K) are clamped: the caller tracks which tuples are valid."""
+    key = torch.zeros(tuples.shape[:-1], dtype=torch.int64, device=tuples.device)
+    for h in range(tuples.shape[-1]):
+        key = key * K + tuples[..., h].clamp(0, K - 1)
+    return key
 
+
+def _check_tuple_key(H: int, K: int, what: str, max_levels: Optional[int] = None) -> None:
+    """``_tuple_key`` of H levels of K codes must fit in 62 bits (and H in max_levels, when the caller's kernels bound it)."""
+    if H * max(1, (K - 1).bit_length()) > 62 or (max_levels is not None and H > max_levels):
+        raise Rqb200Error(f"{what}: {H} levels of {K} codes do not pack into a 64-bit tuple key"
+                          + (f" (at most {max_levels} levels)" if max_levels is not None else ""))
+
+
+def _non_finite_error(what: str, n_bad: int) -> RuntimeError:
+    return RuntimeError(f"{what}: {n_bad} decoder row(s) of the head's logits "
+                        "hold a NaN or +inf or are all -inf; the items below them score NaN")
 
 class EncoderDecoderRetrievalModel(nn.Module):
     """T5 encoder over the history's semantic ids, T5 decoder stack plus one Linear head per hierarchy level for the next
@@ -812,16 +822,12 @@ class EncoderDecoderRetrievalModel(nn.Module):
     def _fused_train_passes(self, attention_mask, input_ids, user_id, fut_ids, attention="fp32"):
         """Both fused passes in one graph break: the decoder attends to the encoder's packed rows (no scatter to [B, S, d])."""
         enc = FusedT5EncodeTrain(self, attention).packed(attention_mask, input_ids, user_id)
-        key_mask = enc.key_mask.index_select(0, torch.div(enc.src, enc.S, rounding_mode="floor").long())
-        return FusedT5DecodeTrain(self)(fut_ids, enc.rows, enc.offsets, key_mask, enc.src, enc.S)
+        return FusedT5DecodeTrain(self)(fut_ids, *enc.keys())
 
     @torch.compiler.disable
     def _fused_train_decoder_pass(self, fut_ids, enc_out, enc_mask):
-        """The fused decoder pass over HF's encoder output: history b's keys are rows b * S .. b * S + S - 1 of [B * S, d_model]."""
-        B, S, d = enc_out.shape
-        key_mask = torch.where(enc_mask == 0, torch.finfo(torch.float32).min, 0.0).to(torch.float32).reshape(B * S)
-        offsets = torch.arange(0, (B + 1) * S, S, dtype=torch.int32, device=enc_out.device)
-        return FusedT5DecodeTrain(self)(fut_ids, enc_out.reshape(B * S, d), offsets, key_mask, None, S)
+        """The fused decoder pass over HF's encoder output, every position a key row."""
+        return FusedT5DecodeTrain(self)(fut_ids, *PackedEncoderOutput.of_padded(enc_out, enc_mask).keys())
 
     def forward(self, batch: TokenizedSeqBatch, encoder: Optional[str] = None, decoder: Optional[str] = None,
                 encoder_attention: Optional[str] = None) -> ModelOutput:
@@ -835,12 +841,8 @@ class EncoderDecoderRetrievalModel(nn.Module):
                     mode; gradients in both.  With encoder="fused" it attends to the encoder's packed rows directly.
         ``encoder_attention`` (default: the module's ``DEFAULT_ENCODER_ATTENTION``, read at call time) picks the fused encoder's
         attention kernels: "fp32" or "tf32" (TF32 tensor-core products, the same dropout bits).  "tf32" needs encoder="fused"."""
-        encoder = DEFAULT_FORWARD_ENCODER if encoder is None else encoder
-        decoder = DEFAULT_FORWARD_DECODER if decoder is None else decoder
-        if encoder not in ENCODERS:
-            raise ValueError(f"forward: encoder must be one of {ENCODERS}, got {encoder!r}")
-        if decoder not in DECODERS:
-            raise ValueError(f"forward: decoder must be one of {DECODERS}, got {decoder!r}")
+        encoder = _choice(encoder, DEFAULT_FORWARD_ENCODER, ENCODERS, "forward", "encoder")
+        decoder = _choice(decoder, DEFAULT_FORWARD_DECODER, DECODERS, "forward", "decoder")
         att = _encoder_attention(encoder, encoder_attention, "forward")
         H = self.num_hierarchies
         input_ids = _strip_dedup_col(batch.sem_ids, H + 1, H)
@@ -902,12 +904,9 @@ class EncoderDecoderRetrievalModel(nn.Module):
             if k > 32 or k * n_cands > 1024 or K > 2048:
                 raise Rqb200Error(f"generate: top_k_for_generation = {k} (at most 32, and top_k * {n_cands} candidates at most "
                                   f"1024) with {K} codes per level (at most 2048) is outside the sampling kernel's limits")
-        elif search == "beam":
-            if k > 32 or k > K or K > 2048:
-                raise Rqb200Error(f"generate: top_k_for_generation = {k} (at most 32 and at most the number of codes) with {K} "
-                                  "codes per level (at most 2048) is outside the beam search kernel's limits")
-        else:
-            raise ValueError(f"generate: search must be one of {SEARCHES}, got {search!r}")
+        elif k > 32 or k > K or K > 2048:
+            raise Rqb200Error(f"generate: top_k_for_generation = {k} (at most 32 and at most the number of codes) with {K} "
+                              "codes per level (at most 2048) is outside the beam search kernel's limits")
 
     def _fused_decoder(self, enc_out: Tensor, enc_mask: Tensor, k: int) -> FusedT5Decode:
         return FusedT5Decode(self, enc_out, enc_mask, k)
@@ -935,25 +934,22 @@ class EncoderDecoderRetrievalModel(nn.Module):
         ``encoder_attention`` (default: the module's ``DEFAULT_ENCODER_ATTENTION``, read at call time) picks the fused encoder's
         attention kernel: "fp32" or "tf32" (TF32 tensor-core products).  "tf32" needs encoder="fused".
         Returns generated [B, top_k, num_hierarchies] and log_probas [B, top_k]."""
-        search = DEFAULT_SEARCH if search is None else search
-        decoder = DEFAULT_DECODER if decoder is None else decoder
-        encoder = DEFAULT_ENCODER if encoder is None else encoder
-        if decoder not in DECODERS:
-            raise ValueError(f"generate: decoder must be one of {DECODERS}, got {decoder!r}")
+        decoder = _choice(decoder, DEFAULT_DECODER, DECODERS, "generate", "decoder")
         if decoder == "fused" and self.training:
             raise ValueError("generate: decoder=\"fused\" runs the decoder in eval mode only; call model.eval() first (in "
                              "training mode HF's decoder applies dropout)")
-        if encoder not in ENCODERS:
-            raise ValueError(f"generate: encoder must be one of {ENCODERS}, got {encoder!r}")
+        encoder = _choice(encoder, DEFAULT_ENCODER, ENCODERS, "generate", "encoder")
         att = _encoder_attention(encoder, encoder_attention, "generate")
         if encoder == "fused" and self.training:
             raise ValueError("generate: encoder=\"fused\" runs the encoder in eval mode only; call model.eval() first (in "
                              "training mode HF's encoder applies dropout)")
+        search = _choice(search, DEFAULT_SEARCH, SEARCHES, "generate", "search")
         k = self.top_k_for_generation
         n_cands = min(MAX_CANDIDATES, self.num_embeddings_per_hierarchy)
         self._check_search_limits(search, k, n_cands)
         beam = search == "beam"
         if encoder == "fused":
+            # "fp32" without an argument: a caller may have replaced _fused_encoder with a function of none
             fused_encoder = self._fused_encoder() if att == "fp32" else self._fused_encoder(att)
             enc_out, enc_mask = fused_encoder(attention_mask, input_ids, user_id)
         else:
@@ -1040,13 +1036,12 @@ class EncoderDecoderRetrievalModel(nn.Module):
         if state is None or state[0] != H:
             if index.C < H:
                 raise Rqb200Error(f"rank_sem_ids: the corpus table has {index.C} id columns, fewer than {H} levels")
-            if H * max(1, (K - 1).bit_length()) > 62:
-                raise Rqb200Error(f"rank_sem_ids: {H} levels of {K} codes do not pack into a 64-bit tuple key")
+            _check_tuple_key(H, K, "rank_sem_ids")
             cb = self.codebooks[:, :H].to(device)
             n_items = ((cb >= 0) & (cb < K)).all(1).sum()
             host = torch.cat([index.counts().long(), n_items.view(1)]).tolist()   # the one host read of the ranking
             levels = index.levels(host[:-1])
-            key = levels.code[1].long()
+            key = levels.code[1].long()                                           # _tuple_key of each leaf, along its path
             for l in range(2, H + 1):
                 key = key[levels.parent[l].long()] * K + levels.code[l]
             state = index._rank_state = (H, levels, key, int(host[-1]))
@@ -1060,9 +1055,7 @@ class EncoderDecoderRetrievalModel(nn.Module):
         if U == 0:
             return torch.full((t.shape[0],), -1, dtype=torch.int64, device=t.device)
         valid = ((t >= 0) & (t < K)).all(1)
-        key = torch.zeros(t.shape[0], dtype=torch.int64, device=t.device)
-        for h in range(t.shape[1]):
-            key = key * K + t[:, h].clamp(0, K - 1)
+        key = _tuple_key(t, K)
         idx = torch.searchsorted(leaf_key, key).clamp_(max=U - 1)
         return torch.where(valid & (leaf_key[idx] == key), idx, -1)
 
@@ -1071,30 +1064,28 @@ class EncoderDecoderRetrievalModel(nn.Module):
         if self.training:
             raise ValueError(f"{what} runs the model in eval mode only; call model.eval() first (in training mode HF's passes "
                              "apply dropout)")
-        if torch.is_autocast_enabled("cuda"):
-            raise ValueError(f"{what} runs fp32 kernels: it cannot run inside an autocast region")
-        encoder = DEFAULT_ENCODER if encoder is None else encoder
-        if encoder not in ENCODERS:
-            raise ValueError(f"{what}: encoder must be one of {ENCODERS}, got {encoder!r}")
+        _check_no_autocast(what)
+        encoder = _choice(encoder, DEFAULT_ENCODER, ENCODERS, what, "encoder")
         att = _encoder_attention(encoder, encoder_attention, what)
-        attention = "fp32" if attention is None else attention
-        if attention not in ENCODER_ATTENTIONS:
-            raise ValueError(f"{what}: attention must be one of {ENCODER_ATTENTIONS}, got {attention!r}")
-        return encoder, att, attention
+        return encoder, att, _choice(attention, "fp32", ENCODER_ATTENTIONS, what, "attention")
 
     def _rank_encoder(self, attention_mask, input_ids, user_id, encoder: str, att: str):
         """The encoder rows the exact scoring attends to: (rows [*, d_model], offsets int32 [B + 1], additive key mask [*])."""
-        B, dev = attention_mask.shape[0], attention_mask.device
         if encoder == "fused":
-            enc = self._fused_encoder(att)
-            rows, slot, _ = enc.packed(attention_mask, input_ids, user_id)
-            key_mask = enc.key_mask.index_select(0, torch.div(enc.src, slot.shape[1], rounding_mode="floor").long())
-            return rows, enc.offsets, key_mask
-        enc_out, enc_mask = self.encoder_forward_pass(attention_mask=attention_mask, input_ids=input_ids, user_id=user_id)
-        S, d = enc_out.shape[1], enc_out.shape[2]
-        offsets = torch.arange(0, (B + 1) * S, S, dtype=torch.int32, device=dev)
-        key_mask = torch.where(enc_mask == 0, torch.finfo(torch.float32).min, 0.0).to(torch.float32).reshape(B * S)
-        return enc_out.reshape(B * S, d), offsets, key_mask
+            enc = self._fused_encoder(att).packed(attention_mask, input_ids, user_id)
+        else:
+            enc = PackedEncoderOutput.of_padded(*self.encoder_forward_pass(attention_mask=attention_mask, input_ids=input_ids,
+                                                                           user_id=user_id))
+        return enc.keys()[:3]
+
+    def _row_budget(self, max_rows: Optional[int], per_history: int, what: str) -> int:
+        """Most decoder rows one chunk of histories runs: ``max_rows`` (at least one history's), else what ``RANK_BYTE_BUDGET``
+        bytes of decoder state hold."""
+        if max_rows is None:
+            return max(per_history, RANK_BYTE_BUDGET // FusedT5Rank.row_bytes(self))
+        if max_rows < per_history:
+            raise ValueError(f"{what}: max_rows = {max_rows} is below the {per_history} decoder rows of one history")
+        return max_rows
 
     def _leaf_scores(self, attention_mask, input_ids, user_id, encoder, encoder_attention, attention, max_rows, what: str):
         encoder, att, attention = self._check_rank_call(encoder, encoder_attention, attention, what)
@@ -1103,10 +1094,7 @@ class EncoderDecoderRetrievalModel(nn.Module):
         H, B = self.num_hierarchies, attention_mask.shape[0]
         U = levels.n[H]
         per_history = sum(levels.n[:H])
-        if max_rows is None:
-            max_rows = max(per_history, RANK_BYTE_BUDGET // FusedT5Rank.row_bytes(self))
-        elif max_rows < per_history:
-            raise ValueError(f"{what}: max_rows = {max_rows} is below the {per_history} decoder rows of one history")
+        max_rows = self._row_budget(max_rows, per_history, what)
         bad = torch.zeros(1, dtype=torch.int32, device=dev)
         scores = torch.empty((B, U), dtype=torch.float32, device=dev)
         if B == 0 or U == 0:
@@ -1121,8 +1109,7 @@ class EncoderDecoderRetrievalModel(nn.Module):
     def _raise_bad(bad: Tensor, what: str) -> None:
         n_bad = int(bad[0])
         if n_bad:
-            raise RuntimeError(f"{what}: {n_bad} decoder row(s) of the head's logits hold a NaN or +inf or are all -inf; the "
-                               "items below them score NaN")
+            raise _non_finite_error(what, n_bad)
 
     @torch.no_grad()
     def rank_sem_ids(self, attention_mask, input_ids, user_id=None, encoder: Optional[str] = None,
@@ -1168,8 +1155,7 @@ class EncoderDecoderRetrievalModel(nn.Module):
         (``ops.t5score_trie_build``, ``FusedT5Rank.run_candidates``); NaN-row counts are added to bad[0]."""
         encoder, att, attention = self._check_rank_call(encoder, encoder_attention, attention, what)
         H, K = self.num_hierarchies, self.num_embeddings_per_hierarchy
-        if H > 8 or H * max(1, (K - 1).bit_length()) > 62:
-            raise Rqb200Error(f"{what}: {H} levels of {K} codes do not pack into a 64-bit tuple key (at most 8 levels)")
+        _check_tuple_key(H, K, what, max_levels=8)
         B = attention_mask.shape[0]
         if sem_ids.dim() != 3 or sem_ids.shape[0] != B or sem_ids.shape[2] != H:
             raise ValueError(f"{what}: sem_ids {tuple(sem_ids.shape)} must be [B = {B}, C, H = {H}]")
@@ -1178,11 +1164,7 @@ class EncoderDecoderRetrievalModel(nn.Module):
             raise ValueError(f"{what}: C = {C} candidates per history must be in [1, {ops.SCORE_MAX_CANDIDATES}]")
         trie = ops.t5score_trie_build(sem_ids, K)
         need = [[1] + [max(1, c) for c in row] for row in _read_node_counts(trie.counts)]   # rows per level, n[0] = 1 (BOS)
-        own = max((sum(n[:H]) for n in need), default=0)
-        if max_rows is None:
-            max_rows = max(own, RANK_BYTE_BUDGET // FusedT5Rank.row_bytes(self))
-        elif max_rows < own:
-            raise ValueError(f"{what}: max_rows = {max_rows} is below the {own} decoder rows of one history")
+        max_rows = self._row_budget(max_rows, max((sum(n[:H]) for n in need), default=0), what)
         scores = torch.empty((B, C), dtype=torch.float32, device=sem_ids.device)
         if B == 0:
             return scores
@@ -1209,8 +1191,7 @@ class EncoderDecoderRetrievalModel(nn.Module):
         if n_items:
             raise ValueError(f"{what}: {n_items} item id(s) outside [-1, N) where N is the number of corpus rows")
         if n_bad:
-            raise RuntimeError(f"{what}: {n_bad} decoder row(s) of the head's logits hold a NaN or +inf or are all -inf; the "
-                               "items below them score NaN")
+            raise _non_finite_error(what, n_bad)
 
     @torch.no_grad()
     def score_sem_ids(self, attention_mask, input_ids, user_id=None, sem_ids: Optional[Tensor] = None,
@@ -1258,9 +1239,7 @@ class EncoderDecoderRetrievalModel(nn.Module):
             _strip_dedup_col(batch.seq_mask.long(), H + 1, H), _strip_dedup_col(batch.sem_ids, H + 1, H), batch.user_ids, tuples,
             encoder, encoder_attention, attention, max_rows, counters, "score_items")
         target = self.item_of(batch.sem_ids_fut)[:, None]
-        key = torch.zeros_like(items)
-        for h in range(H):
-            key = key * K + tuples[..., h].clamp(0, K - 1)
+        key = _tuple_key(tuples, K)
         match = ok & (items == target)
         pos = match.int().argmax(1, keepdim=True)
         s_t, key_t = scores.gather(1, pos), key.gather(1, pos)

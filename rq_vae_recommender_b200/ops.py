@@ -1225,6 +1225,12 @@ def t5enc_attention_tc(qkv: torch.Tensor, src: torch.Tensor, offsets: torch.Tens
     return _t5enc_attention_eval("t5enc_attention_tc", qkv, src, offsets, key_mask, rel, S)
 
 
+def _rows_of16(t: torch.Tensor, width: int, what: str) -> torch.Tensor:
+    """``_rows_of`` for the encoder attention kernels' 16-byte row loads: a copy when the row pitch or the base is not aligned."""
+    t = _rows_of(t, width, what)
+    return t.contiguous() if t.stride(0) % 4 or t.data_ptr() % 16 else t
+
+
 def _t5enc_attention_eval(name, qkv, src, offsets, key_mask, rel, S):
     _need_cuda(qkv, src, offsets, key_mask, rel)
     rel = _f32c(rel)
@@ -1232,9 +1238,7 @@ def _t5enc_attention_eval(name, qkv, src, offsets, key_mask, rel, S):
     if rel.shape != (heads, 2 * S - 1):
         raise ValueError(f"rel {tuple(rel.shape)} must be [heads, {2 * S - 1}]")
     inner = heads * T5_DKV
-    qkv = _rows_of(qkv, 3 * inner, "qkv")
-    if qkv.stride(0) % 4 or qkv.data_ptr() % 16:
-        qkv = qkv.contiguous()
+    qkv = _rows_of16(qkv, 3 * inner, "qkv")
     B = offsets.shape[0] - 1
     if offsets.dtype != torch.int32 or src.dtype != torch.int32 or src.shape != (qkv.shape[0],) or key_mask.shape != (B,):
         raise ValueError("src must be int32 [N] with N = qkv rows, offsets int32 [B + 1], key_mask [B]")
@@ -1275,12 +1279,16 @@ def _check_p(p: float) -> float:
     return float(p)
 
 
+def _check_seed(seed: torch.Tensor) -> None:
+    if seed.dtype != torch.int64 or seed.numel() != 1:
+        raise ValueError("seed must be an int64 tensor of one element")
+
+
 def t5enc_dropout_keep(seed: torch.Tensor, p: float, B: int, heads: int, S: int) -> torch.Tensor:
     """uint8 [B, heads, S, S]: the attention-dropout keep bits (rqb200_t5enc_dropout_keep) that ``t5enc_attention_train`` applies
     with this seed, indexed by (history, head, query position, key position), one launch."""
     _need_cuda(seed)
-    if seed.dtype != torch.int64 or seed.numel() != 1:
-        raise ValueError("seed must be an int64 tensor of one element")
+    _check_seed(seed)
     keep = torch.empty((B, heads, S, S), dtype=torch.uint8, device=seed.device)
     with torch.cuda.device(seed.device):
         _lib.check(_lib.load().rqb200_t5enc_dropout_keep(_p(seed), _check_p(p), B, heads, S, _p(keep), _stream()),
@@ -1309,14 +1317,11 @@ def _t5enc_attention_train(name, qkv, src, offsets, key_mask, rel, S, seed, p):
     heads = rel.shape[0]
     if rel.shape != (heads, 2 * S - 1):
         raise ValueError(f"rel {tuple(rel.shape)} must be [heads, {2 * S - 1}]")
-    qkv = _rows_of(qkv, 3 * heads * T5_DKV, "qkv")
-    if qkv.stride(0) % 4 or qkv.data_ptr() % 16:
-        qkv = qkv.contiguous()
+    qkv = _rows_of16(qkv, 3 * heads * T5_DKV, "qkv")
     B = offsets.shape[0] - 1
     if offsets.dtype != torch.int32 or src.dtype != torch.int32 or src.shape != (qkv.shape[0],) or key_mask.shape != (B,):
         raise ValueError("src must be int32 [N] with N = qkv rows, offsets int32 [B + 1], key_mask [B]")
-    if seed.dtype != torch.int64 or seed.numel() != 1:
-        raise ValueError("seed must be an int64 tensor of one element")
+    _check_seed(seed)
     key_mask = _f32c(key_mask)
     N = qkv.shape[0]
     out = torch.empty((N, heads * T5_DKV), dtype=torch.float32, device=qkv.device)
@@ -1348,8 +1353,7 @@ def _t5enc_attention_backward(name, qkv, out, dout, lse, src, offsets, key_mask,
     _need_cuda(qkv, out, dout, lse, src, offsets, key_mask, rel, seed)
     heads = rel.shape[0]
     inner = heads * T5_DKV
-    qkv, out, dout = _rows_of(qkv, 3 * inner, "qkv"), _rows_of(out, inner, "out"), _rows_of(dout, inner, "dout")
-    qkv, out, dout = (t if t.stride(0) % 4 == 0 and t.data_ptr() % 16 == 0 else t.contiguous() for t in (qkv, out, dout))
+    qkv, out, dout = _rows_of16(qkv, 3 * inner, "qkv"), _rows_of16(out, inner, "out"), _rows_of16(dout, inner, "dout")
     lse, rel, key_mask = _f32c(lse), _f32c(rel), _f32c(key_mask)
     B, N = offsets.shape[0] - 1, qkv.shape[0]
     if out.shape[0] != N or dout.shape[0] != N or lse.shape != (N, heads) or rel.shape != (heads, 2 * S - 1):
@@ -1412,42 +1416,33 @@ def t5enc_add_norm_bwd(d_out: torch.Tensor, d_res: Optional[torch.Tensor], x_out
     return dx, part.sum(0)
 
 
-class T5EncAttentionFunction(torch.autograd.Function):
-    """Autograd of the training attention: ``apply(qkv, rel, src, offsets, key_mask, S, seed, p)`` -> out [N, inner]; gradients
-    for qkv and rel."""
+def _t5enc_attention_function(name: str, train, backward, doc: str):
+    """The autograd.Function class ``name`` of a training attention whose kernels are the wrappers ``train`` and ``backward``."""
 
-    @staticmethod
-    def forward(ctx, qkv, rel, src, offsets, key_mask, S, seed, p):
+    def forward_(ctx, qkv, rel, src, offsets, key_mask, S, seed, p):
         qkv = qkv.contiguous()
-        out, lse = t5enc_attention_train(qkv, src, offsets, key_mask, rel, S, seed, p)
+        out, lse = train(qkv, src, offsets, key_mask, rel, S, seed, p)
         ctx.save_for_backward(qkv, rel, src, offsets, key_mask, seed, out, lse)
         ctx.S, ctx.p = S, p
         return out
 
-    @staticmethod
-    def backward(ctx, dout):
+    def backward_(ctx, dout):
         qkv, rel, src, offsets, key_mask, seed, out, lse = ctx.saved_tensors
-        dqkv, drel = t5enc_attention_backward(qkv, out, dout, lse, src, offsets, key_mask, rel, ctx.S, seed, ctx.p)
+        dqkv, drel = backward(qkv, out, dout, lse, src, offsets, key_mask, rel, ctx.S, seed, ctx.p)
         return dqkv, drel, None, None, None, None, None, None
 
+    return type(name, (torch.autograd.Function,), {"forward": staticmethod(forward_), "backward": staticmethod(backward_),
+                                                   "__doc__": doc, "__module__": __name__})
 
-class T5EncAttentionTCFunction(torch.autograd.Function):
-    """``T5EncAttentionFunction`` on the TF32 tensor-core kernels (``t5enc_attention_tc_train`` / ``_tc_backward``), the same
-    arguments and gradients."""
 
-    @staticmethod
-    def forward(ctx, qkv, rel, src, offsets, key_mask, S, seed, p):
-        qkv = qkv.contiguous()
-        out, lse = t5enc_attention_tc_train(qkv, src, offsets, key_mask, rel, S, seed, p)
-        ctx.save_for_backward(qkv, rel, src, offsets, key_mask, seed, out, lse)
-        ctx.S, ctx.p = S, p
-        return out
-
-    @staticmethod
-    def backward(ctx, dout):
-        qkv, rel, src, offsets, key_mask, seed, out, lse = ctx.saved_tensors
-        dqkv, drel = t5enc_attention_tc_backward(qkv, out, dout, lse, src, offsets, key_mask, rel, ctx.S, seed, ctx.p)
-        return dqkv, drel, None, None, None, None, None, None
+T5EncAttentionFunction = _t5enc_attention_function(
+    "T5EncAttentionFunction", t5enc_attention_train, t5enc_attention_backward,
+    "Autograd of the training attention: ``apply(qkv, rel, src, offsets, key_mask, S, seed, p)`` -> out [N, inner]; gradients "
+    "for qkv and rel.")
+T5EncAttentionTCFunction = _t5enc_attention_function(
+    "T5EncAttentionTCFunction", t5enc_attention_tc_train, t5enc_attention_tc_backward,
+    "``T5EncAttentionFunction`` on the TF32 tensor-core kernels (``t5enc_attention_tc_train`` / ``_tc_backward``), the same "
+    "arguments and gradients.")
 
 
 class T5EncAddNormFunction(torch.autograd.Function):
@@ -1470,11 +1465,6 @@ class T5EncAddNormFunction(torch.autograd.Function):
 
 
 # ---------------------------------------------------------------------------------------------- training the T5 decoder pass
-def _check_seed(seed: torch.Tensor) -> None:
-    if seed.dtype != torch.int64 or seed.numel() != 1:
-        raise ValueError("seed must be an int64 tensor of one element")
-
-
 def t5dec_self_attention_train(qkv: torch.Tensor, rel: torch.Tensor, T: int, seed: torch.Tensor, p: float):
     """Causal T5 self-attention of T decoder positions per history with HF's attention-weight dropout
     (rqb200_t5dec_self_attention_train), one launch.  qkv [B * T, 3 inner] (row b * T + t: position t of history b; q | k | v),

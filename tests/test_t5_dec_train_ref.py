@@ -138,6 +138,24 @@ def test_forward_decoder_argument_errors():
         M.FusedT5DecodeTrain(m)(fut, rows, offs, torch.zeros(B * S), None, S)
 
 
+def test_encoder_rows_layout():
+    """``PackedEncoderOutput.keys``: the rows, offsets and per-row key mask the offsets-based cross-attentions read, from HF's
+    padded output (every position a row) and from a packed pass (a row takes its history's key mask)."""
+    from rq_vae_recommender_b200.modules import model as M
+    B, S, d = 3, 4, 5
+    fmin = torch.finfo(torch.float32).min
+    enc_out = torch.arange(B * S * d, dtype=torch.float32).view(B, S, d)
+    enc_mask = torch.tensor([[1., 1, 0, 1], [0, 0, 0, 0], [1, 1, 1, 1]])
+    rows, offsets, key_mask, src, S_ = M.PackedEncoderOutput.of_padded(enc_out, enc_mask).keys()
+    assert src is None and S_ == S
+    assert torch.equal(rows, enc_out.reshape(B * S, d))                             # history b's rows: b * S .. b * S + S - 1
+    assert offsets.dtype == torch.int32 and offsets.tolist() == [0, 4, 8, 12]
+    assert key_mask.dtype == torch.float32 and key_mask.tolist() == [0, 0, fmin, 0] + [fmin] * 4 + [0] * 4
+    packed = M.PackedEncoderOutput(rows[:5], torch.tensor([0, 2, 4, 5], dtype=torch.int32), torch.tensor([0., fmin, 0.]),
+                                   torch.tensor([0, 3, 4, 5, 8], dtype=torch.int32), None, S, enc_mask)
+    assert packed.keys()[2].tolist() == [0, 0, fmin, fmin, 0] and packed.keys()[3] is packed.src
+
+
 def test_install_forward_decoder_switch():
     import sys
 
