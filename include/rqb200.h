@@ -230,6 +230,16 @@ int rqb200_sid_trie_sample_select(const float* probas, int64_t probas_stride, co
                                   const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k, int C,
                                   int K, const void* prefix_workspace, int64_t* out_generated, float* out_log_probas,
                                   int64_t* out_parent, int64_t* samples, float* samp_log_p, int* reject, void* stream);
+/* sid_trie_sample_select_excluding : the same call with each history's exclusion set (sid_exclusion_build; ex_count null: none).
+ *                    After the beam's children are expanded, those that are blocked for its history (level h + 1 of ex_blocked)
+ *                    are invalid, exactly like a prefix the corpus lacks.  The noise, samples and samp_log_p are unchanged.
+ *                    Needs ex_H > h and ex_M <= 4096. */
+int rqb200_sid_trie_sample_select_excluding(const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride,
+                                            const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k,
+                                            int C, int K, const void* prefix_workspace, int64_t* out_generated,
+                                            float* out_log_probas, int64_t* out_parent, int64_t* samples, float* samp_log_p,
+                                            int* reject, const int* ex_pos, const int64_t* ex_blocked, const int* ex_count, int ex_M,
+                                            int ex_H, void* stream);
 
 /* sid_trie_beam_topk : one level h of the exhaustive (deterministic) constrained beam search, from the head's logits, one launch:
  *   logits           [B*kp, K] fp32, row stride in elements (kp = 1 at h = 0, where generated and log_probas may be null)
@@ -245,6 +255,13 @@ int rqb200_sid_trie_sample_select(const float* probas, int64_t probas_stride, co
 int rqb200_sid_trie_beam_topk(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas, int B,
                               int kp, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
                               float* out_log_probas, int64_t* out_parent, int* bad, void* stream);
+/* sid_trie_beam_topk_excluding : the same call with each history's exclusion set, as sid_trie_sample_select_excluding: a blocked
+ *                    extension scores -inf like one the corpus lacks. */
+int rqb200_sid_trie_beam_topk_excluding(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas,
+                                        int B, int kp, int h, int k, int C, int K, const void* prefix_workspace,
+                                        int64_t* out_generated, float* out_log_probas, int64_t* out_parent, int* bad,
+                                        const int* ex_pos, const int64_t* ex_blocked, const int* ex_count, int ex_M, int ex_H,
+                                        void* stream);
 
 /* The trie's level arrays as plain device arrays (the exact ranking decodes one row per node).
  * sid_trie_counts : counts int32 [C + 1] = the node count of every level (counts[0] = 1, the root); one tiny launch.
@@ -281,6 +298,25 @@ int rqb200_sid_items_lookup(const void* workspace, const int64_t* ids, int64_t i
                             int64_t* out_item /* [P] */, void* stream);
 int rqb200_sid_items_retrieve(const void* workspace, const int64_t* generated, const float* log_probas, int B, int k, int C, int n,
                               int64_t* out_items, int* out_beam, int* out_count, void* stream);
+/* sid_items_retrieve_excluding : the same call with each history's exclusion set (sid_exclusion_build, on this table): a beam
+ *                       counts its tuple's items that are not excluded, in dedup order; an excluded item is never written. */
+int rqb200_sid_items_retrieve_excluding(const void* workspace, const int64_t* generated, const float* log_probas, int B, int k, int C,
+                                        int n, int64_t* out_items, int* out_beam, int* out_count, const int* ex_pos,
+                                        const int64_t* ex_blocked, const int* ex_count, int ex_M, int ex_H, void* stream);
+/* sid_exclusion_build : each history's exclusion set, one CTA per history.  items int64 [B, M] (corpus rows; -1 pads, repeats
+ *                       allowed; M <= 4096), inv int32 [N] (item -> its position in the table's row array), start int32 [U + 1]
+ *                       (sid_items_offsets), leaf_key int64 [U] (the table's U tuples packed K-ary, level 0 most significant,
+ *                       ascending), H the tuple length (H * bits(K - 1) <= 62).  Writes
+ *                         pos int32 [B, M]          the distinct positions of the retrievable excluded items, ascending (-1 after);
+ *                         blocked int64 [B, H, M]   per level l = 1..H the packed keys of the blocked l-prefixes, ascending (-1
+ *                                                   after): prefixes holding an excluded item under which every retrievable item
+ *                                                   is excluded;
+ *                         count int32 [B, H + 2]    [0] the positions, [l] the blocked l-prefixes, [H + 1] the entries outside
+ *                                                   [-1, N) (otherwise ignored).
+ *                       Unretrievable rows (positions from start[U] on) are ignored.  Plain stores: the output is a function
+ *                       of the input.  B = 0 is a no-op. */
+int rqb200_sid_exclusion_build(const int64_t* items, int B, int M, int64_t N, const int* inv, const int* start,
+                               const int64_t* leaf_key, int U, int H, int K, int* pos, int64_t* blocked, int* count, void* stream);
 /* sid_items_offsets   : byte offsets of row (int32 [N]) and start (int32 [N + 1]) in the item table's workspace; arithmetic only.
  *                       RQB_ERR_UNSUPPORTED outside the table's limits. */
 int rqb200_sid_items_offsets(int64_t N, int C, int K, size_t* row, size_t* start);
@@ -325,6 +361,13 @@ int rqb200_t5rank_children(const float* logits, int64_t ld, int R, int K, int n_
                            const int* code, int n_next, float* out, int* bad, void* stream);
 int rqb200_t5rank_select(const float* scores, int B, int U, const int* row, const int* start, const int64_t* t_leaf,
                          const int64_t* t_dedup, int n, int64_t* out_items, float* out_scores, int64_t* out_rank, void* stream);
+/* t5rank_select_excluding : the same call with each history's exclusion set (sid_exclusion_build): excluded items are skipped,
+ *                          leaves whose items are all excluded take no part, out_rank is the target's position among the items
+ *                          that are not excluded (-1 when it is excluded). */
+int rqb200_t5rank_select_excluding(const float* scores, int B, int U, const int* row, const int* start, const int64_t* t_leaf,
+                                   const int64_t* t_dedup, int n, int64_t* out_items, float* out_scores, int64_t* out_rank,
+                                   const int* ex_pos, const int64_t* ex_blocked, const int* ex_count, int ex_M, int ex_H,
+                                   void* stream);
 /* t5score_trie_build     : the trie of each history's own candidate tuples (modules/model.py score_sem_ids / score_items), one CTA per
  *                          history.  ids int64 [B, C, H] (candidate c of history b: ids[(b * C + c) * H ..]); a tuple holding an id
  *                          outside [0, K) is invalid.  Per history b and level l = 1..H (the distinct l-prefixes of its valid tuples,

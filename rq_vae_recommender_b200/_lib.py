@@ -75,10 +75,19 @@ _SIGNATURES = {
                                               c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "rqb200_sid_trie_beam_topk": (c_int, [c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp,
                                           c_vp, c_vp, c_vp]),
+    "rqb200_sid_trie_sample_select_excluding": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int,
+                                                        c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                                        c_int, c_int, c_vp]),
+    "rqb200_sid_trie_beam_topk_excluding": (c_int, [c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp,
+                                                    c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
     "rqb200_sid_items_workspace_bytes": (c_size, [c_i64, c_int, c_int]),
     "rqb200_sid_items_build": (c_int, [c_vp, c_i64, c_int, c_int, c_vp, c_size, c_vp]),
     "rqb200_sid_items_lookup": (c_int, [c_vp, c_vp, c_i64, c_i64, c_int, c_vp, c_vp]),
     "rqb200_sid_items_retrieve": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp]),
+    "rqb200_sid_items_retrieve_excluding": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                                    c_vp, c_int, c_int, c_vp]),
+    "rqb200_sid_exclusion_build": (c_int, [c_vp, c_int, c_int, c_i64, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp,
+                                           c_vp]),
     "rqb200_sid_topk_rank_hist": (c_int, [c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "rqb200_sid_rank_hist": (c_int, [c_vp, c_int, c_i64, c_vp, c_vp]),
     "rqb200_sid_trie_counts": (c_int, [c_vp, c_vp, c_vp]),
@@ -90,6 +99,8 @@ _SIGNATURES = {
                                                  c_vp]),
     "rqb200_t5rank_children": (c_int, [c_vp, c_i64, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp]),
     "rqb200_t5rank_select": (c_int, [c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp]),
+    "rqb200_t5rank_select_excluding": (c_int, [c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                               c_vp, c_int, c_int, c_vp]),
     "rqb200_t5score_trie_build": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "rqb200_t5dec_cross_attention": (c_int, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_int, c_int, c_int, c_int, c_vp, c_i64,
                                              c_vp]),

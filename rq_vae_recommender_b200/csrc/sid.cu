@@ -13,11 +13,13 @@
 // and never worse than the reference's O(N^2).
 #include <utility>
 
+#include <cub/block/block_radix_sort.cuh>
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/block/block_scan.cuh>
 #include <cub/device/device_scan.cuh>
 
 #include "common.cuh"
+#include "sid_excl.cuh"
 
 #define SID_MAX_KEYS (1ll << 26)
 
@@ -525,6 +527,27 @@ __device__ __forceinline__ void sid_child_mask(const SidTrie& trie, const int64_
 
 __device__ __forceinline__ bool sid_mask_has(const unsigned int* mask, int c) { return (mask[c >> 5] >> (c & 31)) & 1u; }
 
+// One warp, after sid_child_mask: clears the bits of the beam's children that are blocked for history b (SidExcl), the keys
+// [key(ids[0, h)) K, key(ids[0, h)) K + K) of level h + 1's blocked list.  Nothing to do without an exclusion.  The warp is
+// synchronised on return.
+__device__ __forceinline__ void sid_mask_unblock(const SidExcl& ex, int64_t b, const int64_t* ids, int h, int K, unsigned int* mask,
+                                                 int lane) {
+  if (!ex.on()) return;
+  long long key = 0;
+  for (int j = 0; j < h; ++j) {
+    const int64_t v = ids[j];
+    key = key * K + (v < 0 ? 0 : v >= K ? K - 1 : v);       // a beam holding such an id is no corpus prefix: its mask is empty
+  }
+  const long long lo = key * K, hi = lo + K;
+  const long long* list = ex.blocked_of(b, h + 1);
+  const int n = ex.nblocked(b, h + 1);
+  for (int i = sid_lower_bound(list, n, lo) + lane; i < n && __ldg(list + i) < hi; i += 32) {
+    const int c = (int)(__ldg(list + i) - lo);
+    atomicAnd(&mask[c >> 5], ~(1u << (c & 31)));
+  }
+  __syncwarp();
+}
+
 // valid[p] = any corpus row whose first l ids equal prefix[p, :l]      (model.py:175-181)
 __global__ void sid_prefix_check_kernel(const int64_t* __restrict__ prefix, int64_t stride, int64_t P, int l, int K, SidTrie trie,
                                         unsigned char* __restrict__ valid) {
@@ -740,11 +763,12 @@ static size_t sid_sample_smem(int kp, int nc, int K) {
   return E * (sizeof(int64_t) + sizeof(float) + 1) + (size_t)W * (K + 256 + 2 * nc + (K + 31) / 32) * 4;
 }
 
+template <bool EXCL>                                        // EXCL: with an exclusion (the mask clearing is compiled only then)
 __global__ void __launch_bounds__(SID_SAMPLE_MAX_WARPS * 32) sid_sample_select_kernel(
     const float* __restrict__ probas, int64_t p_stride, const float* __restrict__ noise, int64_t n_stride,
     const int64_t* __restrict__ generated, const float* __restrict__ log_probas, int kp, int nc, int h, int k, int K, SidTrie trie,
     int64_t* __restrict__ out_generated, float* __restrict__ out_log_probas, int64_t* __restrict__ out_parent,
-    int64_t* __restrict__ samples, float* __restrict__ samp_log_p, int* __restrict__ reject) {
+    int64_t* __restrict__ samples, float* __restrict__ samp_log_p, int* __restrict__ reject, SidExcl ex) {
   extern __shared__ __align__(16) unsigned char sid_smem[];
   const int W = blockDim.x >> 5, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int b = blockIdx.x, E = kp * nc, KW = (K + 31) >> 5;
@@ -773,6 +797,7 @@ __global__ void __launch_bounds__(SID_SAMPLE_MAX_WARPS * 32) sid_sample_select_k
     __syncwarp();
     sid_warp_top_n(s_key, K, nc, s_hist, s_sk, s_si, s_tok + beam * nc, lane);
     sid_child_mask(trie, generated + row * h, h, K, s_mask, lane);
+    if (EXCL) sid_mask_unblock(ex, b, generated + row * h, h, K, s_mask, lane);
     const float plp = log_probas ? log_probas[row] : 0.f;
     for (int r = lane; r < nc; r += 32) {
       const int64_t tok = s_tok[beam * nc + r];
@@ -788,11 +813,20 @@ __global__ void __launch_bounds__(SID_SAMPLE_MAX_WARPS * 32) sid_sample_select_k
     sid_keep_best(s_score, s_taken, s_tok, E, nc, b, kp, h, k, generated, out_generated, out_log_probas, out_parent, lane);
 }
 
-extern "C" int rqb200_sid_trie_sample_select(const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride,
-                                             const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k,
-                                             int C, int K, const void* prefix_workspace, int64_t* out_generated,
-                                             float* out_log_probas, int64_t* out_parent, int64_t* samples, float* samp_log_p,
-                                             int* reject, void* stream) {
+// The exclusion arguments of the *_excluding entry points: the arrays of rqb200_sid_exclusion_build (count null: none).
+static int sid_excl_of(const int* pos, const int64_t* blocked, const int* count, int M, int H, int levels, const char* what,
+                       SidExcl& ex) {
+  ex = SidExcl{pos, reinterpret_cast<const long long*>(blocked), count, M, H};
+  if (!count) return RQB_OK;
+  RQB_CHECK_ARG(pos && blocked && M > 0 && M <= SID_EXCL_MAX_M && H >= levels && H <= RQB_MAX_LEVELS,
+                "%s: bad exclusion (M = %d, H = %d, need M <= %d and H >= %d)", what, M, H, SID_EXCL_MAX_M, levels);
+  return RQB_OK;
+}
+
+static int sid_sample_select(const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride,
+                             const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k, int C, int K,
+                             const void* prefix_workspace, int64_t* out_generated, float* out_log_probas, int64_t* out_parent,
+                             int64_t* samples, float* samp_log_p, int* reject, const SidExcl& ex, void* stream) {
   RQB_CHECK_ARG(B >= 0 && kp > 0 && nc > 0 && h >= 0 && h < C && C <= 8 && k > 0 && K > 0 && probas_stride >= K &&
                     noise_stride >= K, "sid_trie_sample_select: bad argument (B=%d kp=%d nc=%d h=%d k=%d C=%d K=%d)", B, kp, nc, h,
                 k, C, K);
@@ -806,13 +840,35 @@ extern "C" int rqb200_sid_trie_sample_select(const float* probas, int64_t probas
                     (h == 0 || log_probas), "sid_trie_sample_select: null pointer");
   const int W = kp < SID_SAMPLE_MAX_WARPS ? kp : SID_SAMPLE_MAX_WARPS;
   const size_t smem = sid_sample_smem(kp, nc, K);
-  RQB_CUDA(cudaFuncSetAttribute(sid_sample_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  sid_sample_select_kernel<<<B, W * 32, smem, reinterpret_cast<cudaStream_t>(stream)>>>(
+  auto kernel = ex.count ? sid_sample_select_kernel<true> : sid_sample_select_kernel<false>;
+  RQB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kernel<<<B, W * 32, smem, reinterpret_cast<cudaStream_t>(stream)>>>(
       probas, probas_stride, noise, noise_stride, generated, log_probas, kp, nc, h, k, K,
       SidTrie{reinterpret_cast<const unsigned char*>(prefix_workspace), h + 1}, out_generated, out_log_probas, out_parent, samples,
-      samp_log_p, reject);
+      samp_log_p, reject, ex);
   RQB_LAUNCH_CHECK();
   return RQB_OK;
+}
+
+extern "C" int rqb200_sid_trie_sample_select(const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride,
+                                             const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k,
+                                             int C, int K, const void* prefix_workspace, int64_t* out_generated,
+                                             float* out_log_probas, int64_t* out_parent, int64_t* samples, float* samp_log_p,
+                                             int* reject, void* stream) {
+  return sid_sample_select(probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K, prefix_workspace,
+                           out_generated, out_log_probas, out_parent, samples, samp_log_p, reject, SidExcl{}, stream);
+}
+
+extern "C" int rqb200_sid_trie_sample_select_excluding(
+    const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride, const int64_t* generated,
+    const float* log_probas, int B, int kp, int nc, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
+    float* out_log_probas, int64_t* out_parent, int64_t* samples, float* samp_log_p, int* reject, const int* ex_pos,
+    const int64_t* ex_blocked, const int* ex_count, int ex_M, int ex_H, void* stream) {
+  SidExcl ex;
+  const int rc = sid_excl_of(ex_pos, ex_blocked, ex_count, ex_M, ex_H, h + 1, "sid_trie_sample_select_excluding", ex);
+  if (rc != RQB_OK) return rc;
+  return sid_sample_select(probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K, prefix_workspace,
+                           out_generated, out_log_probas, out_parent, samples, samp_log_p, reject, ex, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -856,7 +912,7 @@ template <bool KEYS_IN_SMEM>
 __global__ void __launch_bounds__(SID_TOPK_MAX_THREADS) sid_beam_topk_kernel(
     const float* __restrict__ logits, int64_t ld, const int64_t* __restrict__ generated, const float* __restrict__ log_probas,
     int kp, int h, int k, int K, SidTrie trie, int64_t* __restrict__ out_generated, float* __restrict__ out_log_probas,
-    int64_t* __restrict__ out_parent, int* __restrict__ bad) {
+    int64_t* __restrict__ out_parent, int* __restrict__ bad, SidExcl ex) {
   extern __shared__ __align__(16) unsigned char sid_smem[];
   __shared__ SidTopkShared s;
   unsigned int* s_key = reinterpret_cast<unsigned int*>(sid_smem);                // [E] when KEYS_IN_SMEM
@@ -891,7 +947,10 @@ __global__ void __launch_bounds__(SID_TOPK_MAX_THREADS) sid_beam_topk_kernel(
     }
   }
   __syncthreads();
-  for (int beam = w; beam < kp; beam += W) sid_child_mask(trie, s.gen + beam * h, h, K, s_mask + beam * ((K + 31) >> 5), lane);
+  for (int beam = w; beam < kp; beam += W) {
+    sid_child_mask(trie, s.gen + beam * h, h, K, s_mask + beam * ((K + 31) >> 5), lane);
+    sid_mask_unblock(ex, b, s.gen + beam * h, h, K, s_mask + beam * ((K + 31) >> 5), lane);
+  }
   __syncthreads();
   unsigned long long prefix = 0, pmask = 0;
   int want = k;                                             // entries still needed among those matching the decided digits
@@ -971,9 +1030,9 @@ __global__ void __launch_bounds__(SID_TOPK_MAX_THREADS) sid_beam_topk_kernel(
   }
 }
 
-extern "C" int rqb200_sid_trie_beam_topk(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas,
-                                         int B, int kp, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
-                                         float* out_log_probas, int64_t* out_parent, int* bad, void* stream) {
+static int sid_beam_topk(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas, int B, int kp,
+                         int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated, float* out_log_probas,
+                         int64_t* out_parent, int* bad, const SidExcl& ex, void* stream) {
   RQB_CHECK_ARG(B >= 0 && kp > 0 && h >= 0 && h < C && C <= 8 && k > 0 && K > 0 && logits_stride >= K,
                 "sid_trie_beam_topk: bad argument (B=%d kp=%d h=%d k=%d C=%d K=%d)", B, kp, h, k, C, K);
   if (K > SID_TOPK_MAX_K || k > 32 || k > K || kp > SID_TOPK_MAX_BEAMS) {
@@ -993,13 +1052,32 @@ extern "C" int rqb200_sid_trie_beam_topk(const float* logits, int64_t logits_str
     const size_t smem = (size_t)E * sizeof(unsigned int) + mask;
     RQB_CUDA(cudaFuncSetAttribute(sid_beam_topk_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     sid_beam_topk_kernel<true><<<B, nt, smem, st>>>(logits, logits_stride, generated, log_probas, kp, h, k, K, trie, out_generated,
-                                                    out_log_probas, out_parent, bad);
+                                                    out_log_probas, out_parent, bad, ex);
   } else {
     sid_beam_topk_kernel<false><<<B, nt, mask, st>>>(logits, logits_stride, generated, log_probas, kp, h, k, K, trie, out_generated,
-                                                     out_log_probas, out_parent, bad);
+                                                     out_log_probas, out_parent, bad, ex);
   }
   RQB_LAUNCH_CHECK();
   return RQB_OK;
+}
+
+extern "C" int rqb200_sid_trie_beam_topk(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas,
+                                         int B, int kp, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
+                                         float* out_log_probas, int64_t* out_parent, int* bad, void* stream) {
+  return sid_beam_topk(logits, logits_stride, generated, log_probas, B, kp, h, k, C, K, prefix_workspace, out_generated,
+                       out_log_probas, out_parent, bad, SidExcl{}, stream);
+}
+
+extern "C" int rqb200_sid_trie_beam_topk_excluding(const float* logits, int64_t logits_stride, const int64_t* generated,
+                                                   const float* log_probas, int B, int kp, int h, int k, int C, int K,
+                                                   const void* prefix_workspace, int64_t* out_generated, float* out_log_probas,
+                                                   int64_t* out_parent, int* bad, const int* ex_pos, const int64_t* ex_blocked,
+                                                   const int* ex_count, int ex_M, int ex_H, void* stream) {
+  SidExcl ex;
+  const int rc = sid_excl_of(ex_pos, ex_blocked, ex_count, ex_M, ex_H, h + 1, "sid_trie_beam_topk_excluding", ex);
+  if (rc != RQB_OK) return rc;
+  return sid_beam_topk(logits, logits_stride, generated, log_probas, B, kp, h, k, C, K, prefix_workspace, out_generated,
+                       out_log_probas, out_parent, bad, ex, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -1226,7 +1304,7 @@ extern "C" int rqb200_sid_items_lookup(const void* workspace, const int64_t* ids
 
 __global__ void __launch_bounds__(SID_ITEMS_THREADS) sid_items_retrieve_kernel(
     const unsigned char* __restrict__ ws, const int64_t* __restrict__ generated, const float* __restrict__ log_probas, int k, int C,
-    int n, int64_t* __restrict__ out_items, int* __restrict__ out_beam, int* __restrict__ out_count) {
+    int n, int64_t* __restrict__ out_items, int* __restrict__ out_beam, int* __restrict__ out_count, SidExcl ex) {
   using Scan = cub::BlockScan<int, SID_ITEMS_THREADS>;
   __shared__ typename Scan::TempStorage scan_tmp;
   __shared__ int s_u[SID_ITEMS_MAX_K];
@@ -1235,6 +1313,8 @@ __global__ void __launch_bounds__(SID_ITEMS_THREADS) sid_items_retrieve_kernel(
   const int* row = reinterpret_cast<const int*>(ws + h.row);
   const int* start = reinterpret_cast<const int*>(ws + h.start);
   const int b = blockIdx.x;
+  const int* xp = ex.on() ? ex.pos_of(b) : nullptr;         // the history's excluded positions, ascending
+  const int nx = ex.on() ? ex.npos(b) : 0;
   for (int j = threadIdx.x; j < k; j += SID_ITEMS_THREADS) {
     const int64_t bj = (int64_t)b * k + j;
     const bool live = log_probas == nullptr || log_probas[bj] > -INFINITY;   // NaN is not above -inf either
@@ -1250,7 +1330,10 @@ __global__ void __launch_bounds__(SID_ITEMS_THREADS) sid_items_retrieve_kernel(
       const int u = s_u[j];
       bool seen = false;
       for (int q = 0; q < j && !seen; ++q) seen = s_u[q] == u;
-      if (!seen) cnt[i] = __ldg(start + u + 1) - __ldg(start + u);
+      if (!seen) {
+        const int s = __ldg(start + u), e = __ldg(start + u + 1);
+        cnt[i] = e - s - (xp ? sid_excluded_in(xp, nx, s, e) : 0);
+      }
     }
   }
   int off[SID_ITEMS_PER_THREAD], total;
@@ -1274,7 +1357,8 @@ __global__ void __launch_bounds__(SID_ITEMS_THREADS) sid_items_retrieve_kernel(
         else hi = mid;
       }
       beam = lo;
-      item = __ldg(row + __ldg(start + s_u[lo]) + (o - s_off[lo]));
+      const int s = __ldg(start + s_u[lo]), d = o - s_off[lo];
+      item = __ldg(row + (xp ? sid_nth_kept(xp, nx, s, d) : s + d));
     }
     out_items[(int64_t)b * n + o] = item;
     out_beam[(int64_t)b * n + o] = beam;
@@ -1282,8 +1366,8 @@ __global__ void __launch_bounds__(SID_ITEMS_THREADS) sid_items_retrieve_kernel(
   if (threadIdx.x == 0) out_count[b] = m;
 }
 
-extern "C" int rqb200_sid_items_retrieve(const void* workspace, const int64_t* generated, const float* log_probas, int B, int k, int C,
-                                         int n, int64_t* out_items, int* out_beam, int* out_count, void* stream) {
+static int sid_items_retrieve(const void* workspace, const int64_t* generated, const float* log_probas, int B, int k, int C, int n,
+                              int64_t* out_items, int* out_beam, int* out_count, const SidExcl& ex, void* stream) {
   RQB_CHECK_ARG(B >= 0 && k > 0 && C > 0 && n > 0, "sid_items_retrieve: bad argument (B = %d, k = %d, C = %d, n = %d)", B, k, C, n);
   if (k > SID_ITEMS_MAX_K || n > SID_ITEMS_MAX_N) {
     rqb_set_error("sid_items_retrieve: need k <= %d and n <= %d (k = %d, n = %d)", SID_ITEMS_MAX_K, SID_ITEMS_MAX_N, k, n);
@@ -1292,7 +1376,169 @@ extern "C" int rqb200_sid_items_retrieve(const void* workspace, const int64_t* g
   if (B == 0) return RQB_OK;
   RQB_CHECK_ARG(workspace && generated && out_items && out_beam && out_count, "sid_items_retrieve: null pointer");
   sid_items_retrieve_kernel<<<B, SID_ITEMS_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<const unsigned char*>(workspace), generated, log_probas, k, C, n, out_items, out_beam, out_count);
+      reinterpret_cast<const unsigned char*>(workspace), generated, log_probas, k, C, n, out_items, out_beam, out_count, ex);
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
+}
+
+extern "C" int rqb200_sid_items_retrieve(const void* workspace, const int64_t* generated, const float* log_probas, int B, int k, int C,
+                                         int n, int64_t* out_items, int* out_beam, int* out_count, void* stream) {
+  return sid_items_retrieve(workspace, generated, log_probas, B, k, C, n, out_items, out_beam, out_count, SidExcl{}, stream);
+}
+
+extern "C" int rqb200_sid_items_retrieve_excluding(const void* workspace, const int64_t* generated, const float* log_probas, int B,
+                                                   int k, int C, int n, int64_t* out_items, int* out_beam, int* out_count,
+                                                   const int* ex_pos, const int64_t* ex_blocked, const int* ex_count, int ex_M,
+                                                   int ex_H, void* stream) {
+  SidExcl ex;
+  const int rc = sid_excl_of(ex_pos, ex_blocked, ex_count, ex_M, ex_H, 0, "sid_items_retrieve_excluding", ex);
+  if (rc != RQB_OK) return rc;
+  return sid_items_retrieve(workspace, generated, log_probas, B, k, C, n, out_items, out_beam, out_count, ex, stream);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Per-history exclusion sets (csrc/sid_excl.cuh for the layout): "do not return these items" for the search kernels above, the
+// item retrieval and the exact ranking's selection.  One CTA per history over its M entries (items, -1 pads): each item maps to
+// its sorted position in the item table (inv, the inverse of the table's row array; positions from start[U] on are unretrievable
+// rows and dropped), a block radix sort orders the positions and a block scan drops repeats.  The table's order is
+// lexicographic, so the excluded items under an l-prefix p are one run of the sorted positions, and p's retrievable rows are
+// start[lo] .. start[hi] with [lo, hi) the leaves whose keys (leaf_key, the packed tuples of the table's U leaves, ascending)
+// begin with p: two binary searches.  The first position of each run flags p as blocked when the run covers all those rows;
+// a block scan per level numbers the blocked prefixes.  Plain stores to distinct addresses; the cost depends on M and H only.
+#define SID_EXCL_THREADS 512
+
+template <int IPT>
+__global__ void __launch_bounds__(SID_EXCL_THREADS) sid_exclusion_kernel(
+    const int64_t* __restrict__ items, int M, int64_t N, const int* __restrict__ inv, const int* __restrict__ start,
+    const long long* __restrict__ leaf_key, int U, int H, int K, int* __restrict__ pos, long long* __restrict__ blocked,
+    int* __restrict__ count) {
+  using Sort = cub::BlockRadixSort<unsigned int, SID_EXCL_THREADS, IPT>;
+  using Scan = cub::BlockScan<int, SID_EXCL_THREADS>;
+  __shared__ union {
+    typename Sort::TempStorage sort;
+    typename Scan::TempStorage scan;
+  } tmp;
+  __shared__ int s_pos[SID_EXCL_THREADS * IPT];
+  __shared__ unsigned int s_last[SID_EXCL_THREADS];
+  __shared__ long long s_last_key[SID_EXCL_THREADS];
+  __shared__ int s_bad;
+  const unsigned int none = 0xffffffffu;
+  const int64_t b = blockIdx.x;
+  const int tid = threadIdx.x;
+  const int n_items = U > 0 ? __ldg(start + U) : 0;
+  if (tid == 0) s_bad = 0;
+  unsigned int key[IPT];
+  int bad = 0;
+#pragma unroll
+  for (int j = 0; j < IPT; ++j) {                           // blocked: thread t holds entries t IPT .. t IPT + IPT - 1
+    const int c = tid * IPT + j;
+    key[j] = none;
+    if (c < M) {
+      const int64_t v = items[b * M + c];
+      if (v < -1 || v >= N) ++bad;
+      else if (v >= 0) {
+        const int r = __ldg(inv + v);
+        if (r < n_items) key[j] = (unsigned int)r;
+      }
+    }
+  }
+  Sort(tmp.sort).Sort(key);
+  __syncthreads();
+  s_last[tid] = key[IPT - 1];
+  if (bad) atomicAdd(&s_bad, bad);                          // an integer count: its value does not depend on the order
+  __syncthreads();
+  int flag[IPT], idx[IPT], total;
+#pragma unroll
+  for (int j = 0; j < IPT; ++j) {
+    const unsigned int prev = j > 0 ? key[j - 1] : tid > 0 ? s_last[tid - 1] : none;
+    flag[j] = key[j] != none && key[j] != prev ? 1 : 0;
+  }
+  Scan(tmp.scan).InclusiveSum(flag, idx, total);
+  __syncthreads();
+#pragma unroll
+  for (int j = 0; j < IPT; ++j)
+    if (flag[j]) s_pos[idx[j] - 1] = (int)key[j];
+  __syncthreads();
+  int* out_pos = pos + b * M;
+  for (int i = tid; i < M; i += SID_EXCL_THREADS) out_pos[i] = i < total ? s_pos[i] : -1;
+  long long lk[IPT];                                        // the leaf key of distinct position i = t IPT + j
+#pragma unroll
+  for (int j = 0; j < IPT; ++j) {
+    const int i = tid * IPT + j;
+    lk[j] = -1;
+    if (i < total) {
+      int lo = 0, hi = U;                                   // the leaf u with start[u] <= position < start[u + 1]
+      while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (__ldg(start + mid) <= s_pos[i]) lo = mid;
+        else hi = mid;
+      }
+      lk[j] = __ldg(leaf_key + lo);
+    }
+  }
+  s_last_key[tid] = lk[IPT - 1];
+  __syncthreads();
+  const long long prev_key = tid > 0 ? s_last_key[tid - 1] : -1;
+  int* out_count = count + b * (H + 2);
+  long long div = 1;                                        // K^(H - l): a leaf key over div is its l-prefix's key
+  for (int l = 1; l < H; ++l) div *= K;
+  for (int l = 1; l <= H; ++l) {
+    long long p[IPT];
+#pragma unroll
+    for (int j = 0; j < IPT; ++j) {
+      const int i = tid * IPT + j;
+      p[j] = i < total ? lk[j] / div : -1;
+      flag[j] = 0;
+      const long long before = j > 0 ? lk[j - 1] : prev_key;
+      if (i < total && (before < 0 || before / div != p[j])) {   // the first excluded position under prefix p[j]
+        const int lo = sid_lower_bound(leaf_key, U, p[j] * div), hi = sid_lower_bound(leaf_key, U, (p[j] + 1) * div);
+        const int s = __ldg(start + lo), e = __ldg(start + hi);
+        flag[j] = sid_lower_bound(s_pos, total, e) - i == e - s ? 1 : 0;
+      }
+    }
+    int nb;
+    Scan(tmp.scan).InclusiveSum(flag, idx, nb);
+    __syncthreads();                                        // scan storage is reused by the next level
+    long long* out_blocked = blocked + (b * H + (l - 1)) * M;
+#pragma unroll
+    for (int j = 0; j < IPT; ++j)
+      if (flag[j]) out_blocked[idx[j] - 1] = p[j];
+    for (int i = nb + tid; i < M; i += SID_EXCL_THREADS) out_blocked[i] = -1;
+    if (tid == 0) out_count[l] = nb;
+    div /= K;
+  }
+  if (tid == 0) {
+    out_count[0] = total;
+    out_count[H + 1] = s_bad;
+  }
+}
+
+extern "C" int rqb200_sid_exclusion_build(const int64_t* items, int B, int M, int64_t N, const int* inv, const int* start,
+                                          const int64_t* leaf_key, int U, int H, int K, int* pos, int64_t* blocked, int* count,
+                                          void* stream) {
+  RQB_CHECK_ARG(B >= 0 && M > 0 && N >= 0 && N < 0x7fffffffll && U >= 0 && U <= N && H > 0 && K > 0,
+                "sid_exclusion_build: bad argument (B = %d, M = %d, N = %lld, U = %d, H = %d, K = %d)", B, M, (long long)N, U, H, K);
+  int bits = 1;
+  while (bits < 31 && (1 << bits) < K) ++bits;              // bits(K - 1), at least 1
+  if (M > SID_EXCL_MAX_M || H > RQB_MAX_LEVELS || H * bits > 62) {
+    rqb_set_error("sid_exclusion_build: need M <= %d, H <= %d and H * bits(K - 1) <= 62 (M = %d, H = %d, K = %d)", SID_EXCL_MAX_M,
+                  RQB_MAX_LEVELS, M, H, K);
+    return RQB_ERR_UNSUPPORTED;
+  }
+  if (B == 0) return RQB_OK;
+  RQB_CHECK_ARG(items && start && (inv || N == 0) && (leaf_key || U == 0) && pos && blocked && count,
+                "sid_exclusion_build: null pointer");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const long long* lk = reinterpret_cast<const long long*>(leaf_key);
+  long long* bl = reinterpret_cast<long long*>(blocked);
+  if (M <= SID_EXCL_THREADS)
+    sid_exclusion_kernel<1><<<B, SID_EXCL_THREADS, 0, st>>>(items, M, N, inv, start, lk, U, H, K, pos, bl, count);
+  else if (M <= 2 * SID_EXCL_THREADS)
+    sid_exclusion_kernel<2><<<B, SID_EXCL_THREADS, 0, st>>>(items, M, N, inv, start, lk, U, H, K, pos, bl, count);
+  else if (M <= 4 * SID_EXCL_THREADS)
+    sid_exclusion_kernel<4><<<B, SID_EXCL_THREADS, 0, st>>>(items, M, N, inv, start, lk, U, H, K, pos, bl, count);
+  else
+    sid_exclusion_kernel<8><<<B, SID_EXCL_THREADS, 0, st>>>(items, M, N, inv, start, lk, U, H, K, pos, bl, count);
   RQB_LAUNCH_CHECK();
   return RQB_OK;
 }

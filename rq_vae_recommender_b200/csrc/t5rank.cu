@@ -26,6 +26,7 @@
 #include <cub/block/block_scan.cuh>
 
 #include "common.cuh"
+#include "sid_excl.cuh"
 #include "t5_tc.cuh"
 
 #define RK_DKV 64
@@ -341,11 +342,24 @@ __device__ __forceinline__ unsigned long long rk_key64(unsigned int key, int lea
   return ((unsigned long long)key << 32) | (unsigned int)(0xffffffffu - (unsigned int)leaf);
 }
 
-template <bool KEYS_IN_SMEM>
+// With an exclusion (EXCL): a leaf whose items are all excluded takes the key RK_BLOCKED, which rk_score_key never returns, and
+// no part in the selection.  Thread-strided passes meet leaves in ascending order, so a thread finds whether its leaf is blocked
+// with a cursor over the excluded positions' leaves (ascending): O(U / threads + excluded) per pass.
+#define RK_BLOCKED 1u
+
+struct RkBlockedCursor {
+  int c = 0;
+  __device__ __forceinline__ bool at(int u, const int* x_leaf, const unsigned char* x_full, int nx) {
+    while (c < nx && x_leaf[c] < u) ++c;
+    return c < nx && x_leaf[c] == u && x_full[c];
+  }
+};
+
+template <bool KEYS_IN_SMEM, bool EXCL>
 __global__ void __launch_bounds__(RK_SEL_THREADS) t5rank_select_kernel(
     const float* __restrict__ scores, int U, const int* __restrict__ row, const int* __restrict__ start,
     const int64_t* __restrict__ t_leaf, const int64_t* __restrict__ t_dedup, int n, int64_t* __restrict__ out_items,
-    float* __restrict__ out_scores, int64_t* __restrict__ out_rank) {
+    float* __restrict__ out_scores, int64_t* __restrict__ out_rank, SidExcl ex) {
   using Scan = cub::BlockScan<int, RK_SEL_THREADS>;
   using Reduce = cub::BlockReduce<long long, RK_SEL_THREADS>;
   __shared__ union {
@@ -358,30 +372,58 @@ __global__ void __launch_bounds__(RK_SEL_THREADS) t5rank_select_kernel(
   __shared__ unsigned long long sel[RK_SEL_MAX_N];
   __shared__ int s_leaf[RK_SEL_MAX_N];
   __shared__ int s_off[RK_SEL_MAX_N + 1];
+  __shared__ int x_leaf[EXCL ? SID_EXCL_MAX_M : 1];         // the leaf of each excluded position
+  __shared__ unsigned char x_full[EXCL ? SID_EXCL_MAX_M : 1];   // ... and whether that leaf's items are all excluded
+  __shared__ int n_blocked;
   extern __shared__ __align__(16) unsigned int s_key[];     // [U] when KEYS_IN_SMEM
   const int nt = RK_SEL_THREADS, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const unsigned int lt = (1u << lane) - 1u;
   const int64_t b = blockIdx.x;
   const float* sc = scores + b * U;
-  const int nsel = min(n, U);
+  const int* xp = EXCL ? ex.pos_of(b) : nullptr;            // the history's excluded positions, ascending
+  const int nx = EXCL ? ex.npos(b) : 0;
   for (int i = threadIdx.x; i < 256; i += nt) hist[i] = 0;
   if (threadIdx.x == 0) {
     nsel_at = 0;
     ties_base = 0;
+    n_blocked = 0;
   }
-  if (KEYS_IN_SMEM)
-    for (int u = threadIdx.x; u < U; u += nt) s_key[u] = rk_score_key(sc[u]);
+  if (EXCL) {
+    __syncthreads();
+    for (int i = threadIdx.x; i < nx; i += nt) {
+      const int r = xp[i];
+      int lo = 0, hi = U;                                   // the leaf u with start[u] <= r < start[u + 1]
+      while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (start[mid] <= r) lo = mid;
+        else hi = mid;
+      }
+      const int s = start[lo], e = start[lo + 1];
+      const bool full = sid_excluded_in(xp, nx, s, e) == e - s;
+      x_leaf[i] = lo;
+      x_full[i] = full ? 1 : 0;
+      if (full && (i == 0 || xp[i - 1] < s)) atomicAdd(&n_blocked, 1);   // an integer count: order does not matter
+    }
+    __syncthreads();
+  }
+  const int nsel = min(n, U - (EXCL ? n_blocked : 0));
+  if (KEYS_IN_SMEM) {
+    RkBlockedCursor cur;
+    for (int u = threadIdx.x; u < U; u += nt)
+      s_key[u] = (EXCL && cur.at(u, x_leaf, x_full, nx)) ? RK_BLOCKED : rk_score_key(sc[u]);
+  }
   __syncthreads();
   // radix selection of the nsel-th largest 32-bit score key (8-bit digits, stops once the chosen bin is taken whole)
   unsigned int prefix = 0, pmask = 0;
   int want = nsel;
   for (int shift = 24; shift >= 0 && nsel > 0; shift -= 8) {
+    RkBlockedCursor cur;
     for (int base = 0; base < U; base += nt) {
       const int u = base + threadIdx.x;
       int d = 256;
       if (u < U) {
-        const unsigned int key = KEYS_IN_SMEM ? s_key[u] : rk_score_key(sc[u]);
-        if ((key & pmask) == prefix) d = (int)((key >> shift) & 255u);
+        const unsigned int key = KEYS_IN_SMEM ? s_key[u] : (EXCL && cur.at(u, x_leaf, x_full, nx)) ? RK_BLOCKED : rk_score_key(sc[u]);
+        if ((key & pmask) == prefix && !(EXCL && key == RK_BLOCKED)) d = (int)((key >> shift) & 255u);
       }
       const unsigned int same = __match_any_sync(0xffffffffu, d);
       if (d < 256 && (same & lt) == 0) atomicAdd(&hist[d], __popc(same));   // integer counts: order does not matter
@@ -426,15 +468,28 @@ __global__ void __launch_bounds__(RK_SEL_THREADS) t5rank_select_kernel(
   // keep every leaf above the threshold and the `want` lowest-index leaves at it (an ordered block scan over the ties), and count
   // the items of the leaves that sort before the target
   const int64_t tl = t_leaf[b];
-  const int64_t td = t_dedup[b];
-  const bool t_ok = tl >= 0 && tl < U && td >= 0 && td < (int64_t)(start[tl + 1] - start[tl]);
+  int64_t td = t_dedup[b];
+  bool t_ok = tl >= 0 && tl < U && td >= 0 && td < (int64_t)(start[tl + 1] - start[tl]);
+  if (EXCL && t_ok) {                                       // the target's position among its leaf's items that are not excluded
+    const int r = start[tl] + (int)td;
+    const int at = sid_lower_bound(xp, nx, r);
+    t_ok = !(at < nx && xp[at] == r);
+    td -= at - sid_lower_bound(xp, nx, start[tl]);
+  }
   const unsigned long long t_key = t_ok ? rk_key64(KEYS_IN_SMEM ? s_key[tl] : rk_score_key(sc[tl]), (int)tl) : 0ull;
   long long before = 0;
+  if (EXCL && t_ok)                                         // the excluded items of the leaves counted below
+    for (int i = threadIdx.x; i < nx; i += nt) {
+      const int u = x_leaf[i];
+      const unsigned int key = KEYS_IN_SMEM ? s_key[u] : x_full[i] ? RK_BLOCKED : rk_score_key(sc[u]);
+      if (rk_key64(key, u) > t_key) --before;
+    }
+  RkBlockedCursor cur;
   for (int base = 0; base < U; base += nt) {
     const int u = base + threadIdx.x;
     unsigned int key = 0;
-    if (u < U) key = KEYS_IN_SMEM ? s_key[u] : rk_score_key(sc[u]);
-    const bool in = u < U && nsel > 0;
+    if (u < U) key = KEYS_IN_SMEM ? s_key[u] : (EXCL && cur.at(u, x_leaf, x_full, nx)) ? RK_BLOCKED : rk_score_key(sc[u]);
+    const bool in = u < U && nsel > 0 && !(EXCL && key == RK_BLOCKED);
     const bool above = in && (key & pmask) > prefix;
     const int tie = (in && (key & pmask) == prefix) ? 1 : 0;
     int excl, total;
@@ -464,7 +519,11 @@ __global__ void __launch_bounds__(RK_SEL_THREADS) t5rank_select_kernel(
 #pragma unroll
   for (int i = 0; i < PER; ++i) {
     const int j = threadIdx.x * PER + i;
-    cnt[i] = j < nsel ? start[s_leaf[j] + 1] - start[s_leaf[j]] : 0;
+    cnt[i] = 0;
+    if (j < nsel) {
+      const int s = start[s_leaf[j]], e = start[s_leaf[j] + 1];
+      cnt[i] = e - s - (EXCL ? sid_excluded_in(xp, nx, s, e) : 0);
+    }
   }
   Scan(tmp.scan).ExclusiveSum(cnt, off, total);
 #pragma unroll
@@ -485,7 +544,7 @@ __global__ void __launch_bounds__(RK_SEL_THREADS) t5rank_select_kernel(
         else hi = mid;
       }
       const int leaf = s_leaf[lo];
-      item = row[start[leaf] + (o - s_off[lo])];
+      item = row[EXCL ? sid_nth_kept(xp, nx, start[leaf], o - s_off[lo]) : start[leaf] + (o - s_off[lo])];
       s = sc[leaf];
     }
     out_items[b * n + o] = item;
@@ -494,9 +553,9 @@ __global__ void __launch_bounds__(RK_SEL_THREADS) t5rank_select_kernel(
   if (threadIdx.x == 0) out_rank[b] = t_ok ? (int64_t)items_before + td : -1;
 }
 
-extern "C" int rqb200_t5rank_select(const float* scores, int B, int U, const int* row, const int* start, const int64_t* t_leaf,
-                                    const int64_t* t_dedup, int n, int64_t* out_items, float* out_scores, int64_t* out_rank,
-                                    void* stream) {
+template <bool EXCL>
+static int rk_select(const float* scores, int B, int U, const int* row, const int* start, const int64_t* t_leaf, const int64_t* t_dedup,
+                     int n, int64_t* out_items, float* out_scores, int64_t* out_rank, const SidExcl& ex, void* stream) {
   RQB_CHECK_ARG(B >= 0 && U >= 0 && n > 0, "t5rank_select: bad argument (B = %d, U = %d, n = %d)", B, U, n);
   if (n > RK_SEL_MAX_N) {
     rqb_set_error("t5rank_select: need n <= %d (n = %d)", RK_SEL_MAX_N, n);
@@ -509,17 +568,33 @@ extern "C" int rqb200_t5rank_select(const float* scores, int B, int U, const int
   if (U <= RK_SEL_SMEM_KEYS) {
     const size_t smem = (size_t)U * sizeof(unsigned int);
     static unsigned long long done = 0;
-    const int rc = rk_set_smem_once(reinterpret_cast<const void*>(t5rank_select_kernel<true>),
+    const int rc = rk_set_smem_once(reinterpret_cast<const void*>(t5rank_select_kernel<true, EXCL>),
                                     RK_SEL_SMEM_KEYS * (int)sizeof(unsigned int), &done);
     if (rc != RQB_OK) return rc;
-    t5rank_select_kernel<true><<<B, RK_SEL_THREADS, smem, st>>>(scores, U, row, start, t_leaf, t_dedup, n, out_items, out_scores,
-                                                               out_rank);
+    t5rank_select_kernel<true, EXCL><<<B, RK_SEL_THREADS, smem, st>>>(scores, U, row, start, t_leaf, t_dedup, n, out_items,
+                                                                     out_scores, out_rank, ex);
   } else {
-    t5rank_select_kernel<false><<<B, RK_SEL_THREADS, 0, st>>>(scores, U, row, start, t_leaf, t_dedup, n, out_items, out_scores,
-                                                             out_rank);
+    t5rank_select_kernel<false, EXCL><<<B, RK_SEL_THREADS, 0, st>>>(scores, U, row, start, t_leaf, t_dedup, n, out_items,
+                                                                   out_scores, out_rank, ex);
   }
   RQB_LAUNCH_CHECK();
   return RQB_OK;
+}
+
+extern "C" int rqb200_t5rank_select(const float* scores, int B, int U, const int* row, const int* start, const int64_t* t_leaf,
+                                    const int64_t* t_dedup, int n, int64_t* out_items, float* out_scores, int64_t* out_rank,
+                                    void* stream) {
+  return rk_select<false>(scores, B, U, row, start, t_leaf, t_dedup, n, out_items, out_scores, out_rank, SidExcl{}, stream);
+}
+
+extern "C" int rqb200_t5rank_select_excluding(const float* scores, int B, int U, const int* row, const int* start,
+                                              const int64_t* t_leaf, const int64_t* t_dedup, int n, int64_t* out_items,
+                                              float* out_scores, int64_t* out_rank, const int* ex_pos, const int64_t* ex_blocked,
+                                              const int* ex_count, int ex_M, int ex_H, void* stream) {
+  RQB_CHECK_ARG(ex_pos && ex_count && ex_M > 0 && ex_M <= SID_EXCL_MAX_M && ex_H > 0 && ex_H <= RQB_MAX_LEVELS,
+                "t5rank_select_excluding: bad exclusion (M = %d, H = %d, need M <= %d)", ex_M, ex_H, SID_EXCL_MAX_M);
+  const SidExcl ex{ex_pos, reinterpret_cast<const long long*>(ex_blocked), ex_count, ex_M, ex_H};
+  return rk_select<true>(scores, B, U, row, start, t_leaf, t_dedup, n, out_items, out_scores, out_rank, ex, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ per-history candidate trie

@@ -15,7 +15,9 @@ decoder passes run on the fused decoder-step kernels (``FusedT5Decode``), and ``
 unpadded positions only (``FusedT5Encode``); ``forward_encoder="fused"`` makes the training pass ``forward`` run its encoder on
 the trainable packed pass (``FusedT5EncodeTrain``), and ``forward_decoder="fused"`` its decoder on the fused training
 decoder (``FusedT5DecodeTrain``).  ``encoder_attention="tf32"`` makes the fused encoder passes (of ``generate`` and
-``forward``) run their self-attention on the TF32 tensor-core kernels.  ``replace_metrics=True`` also aliases ``evaluate.metrics``
+``forward``) run their self-attention on the TF32 tensor-core kernels.  ``exclude_history=True`` (with ``replace_model=True``)
+makes ``generate_next_sem_id``, ``generate_items`` and ``rank_items`` leave each history's own items out by default, so an
+unmodified ``train_decoder.py`` evaluates with seen items masked.  ``replace_metrics=True`` also aliases ``evaluate.metrics``
 (train_decoder.py:13), whose ``TopKAccumulator`` accumulates on the device without waiting on the host.  Checkpoints pickle ``modules.quantize.Quantize`` etc. by module path,
 so ``torch.load(..., weights_only=False)`` of the shipped files also lands on the replacement classes.
 gin-config is not in this image: a small compatible shim is registered as ``gin`` when the real one is missing.
@@ -40,7 +42,7 @@ _METRICS = ("evaluate.metrics", "rq_vae_recommender_b200.evaluate.metrics")
 
 def install(reference_root=None, replace_tokenizer=True, gin_shim=True, replace_model=False, search="sample",
             replace_metrics=False, decoder="hf", encoder="hf", forward_encoder="hf", forward_decoder="hf",
-            encoder_attention="fp32"):
+            encoder_attention="fp32", exclude_history=False):
     if search not in ("sample", "beam"):
         raise ValueError(f"search must be 'sample' or 'beam', got {search!r}")
     if search != "sample" and not replace_model:
@@ -68,6 +70,10 @@ def install(reference_root=None, replace_tokenizer=True, gin_shim=True, replace_
     if encoder_attention != "fp32" and not replace_model:
         raise ValueError(f"encoder_attention={encoder_attention!r} selects the replacement model's fused encoder attention: it "
                          "needs replace_model=True")
+    if exclude_history not in (False, True):
+        raise ValueError(f"exclude_history must be True or False, got {exclude_history!r}")
+    if exclude_history and not replace_model:
+        raise ValueError("exclude_history=True selects the replacement model's exclusion of seen items: it needs replace_model=True")
     if gin_shim and "gin" not in sys.modules:
         try:
             import gin  # noqa: F401
@@ -93,6 +99,7 @@ def install(reference_root=None, replace_tokenizer=True, gin_shim=True, replace_
         sys.modules[_MODEL[0]].DEFAULT_FORWARD_ENCODER = forward_encoder
         sys.modules[_MODEL[0]].DEFAULT_FORWARD_DECODER = forward_decoder
         sys.modules[_MODEL[0]].DEFAULT_ENCODER_ATTENTION = encoder_attention
+        sys.modules[_MODEL[0]].DEFAULT_EXCLUDE_HISTORY = exclude_history
     if replace_metrics:
         sys.modules[_METRICS[0]] = importlib.import_module(_METRICS[1])
     return sorted(list(_ALIASES) + ([_TOKENIZER[0]] if replace_tokenizer else []) + ([_MODEL[0]] if replace_model else [])
@@ -112,3 +119,4 @@ def uninstall():
         model.DEFAULT_FORWARD_ENCODER = "hf"
         model.DEFAULT_FORWARD_DECODER = "hf"
         model.DEFAULT_ENCODER_ATTENTION = "fp32"
+        model.DEFAULT_EXCLUDE_HISTORY = False

@@ -16,7 +16,10 @@ The search (``generate``, ``generate_items``):
     device and raise its error after the last level;
   * ``search="beam"``: an exhaustive, deterministic beam search over every code (``SidPrefixIndex.beam_topk``), no sampling;
   * ``generate_items`` resolves the beams to corpus items with one more launch (``ops.SidItemTable.retrieve``); ``item_of``
-    resolves ``sem_ids_fut`` to the true next item.
+    resolves ``sem_ids_fut`` to the true next item;
+  * ``exclude_items`` / ``exclude_history`` leave given items (or each history's own) out of the search, the retrieval and
+    ``rank_items``: a prefix under which every retrievable item is excluded is invalid for that history, like one the corpus
+    lacks (``ops.sid_exclusion_build``).
 
 The fused T5 passes, each HF's maths as GEMMs between this project's kernels, described once by ``_T5Weights``:
   * ``FusedT5Decode`` (``generate(decoder="fused")``) and ``FusedT5Rank`` (exact scoring) run the incremental decoder of
@@ -73,6 +76,9 @@ DEFAULT_FORWARD_DECODER = "hf"
 #: applies to encoder="fused" passes only; HF's encoder follows torch's matmul precision.
 DEFAULT_ENCODER_ATTENTION = "fp32"
 ENCODER_ATTENTIONS = ("fp32", "tf32")
+#: whether generate_next_sem_id, generate_items and rank_items leave out the items of each history (``exclude_history``) when a
+#: call does not say (read at call time)
+DEFAULT_EXCLUDE_HISTORY = False
 _MULTINOMIAL_ERRORS = ("probability tensor contains either `inf`, `nan` or element < 0",
                        "invalid multinomial distribution (sum of probabilities <= 0)")
 
@@ -894,9 +900,11 @@ class EncoderDecoderRetrievalModel(nn.Module):
         return self._prefix_index(prefix.device).check(prefix)
 
     def _sample_and_select(self, index: ops.SidPrefixIndex, probas: Tensor, generated: Optional[Tensor],
-                           log_probas: Optional[Tensor], k: int, n_cands: int, reject: Tensor):
+                           log_probas: Optional[Tensor], k: int, n_cands: int, reject: Tensor,
+                           exclude: Optional[ops.SidExclusion] = None):
         """One level of the search after the softmax: n_cands samples per beam, prefix check, scores, the k best beams."""
-        return index.sample_select(probas, draw_exponential(probas), generated, log_probas, k, n_cands, reject=reject)
+        excl = {} if exclude is None else {"exclude": exclude}
+        return index.sample_select(probas, draw_exponential(probas), generated, log_probas, k, n_cands, reject=reject, **excl)
 
     def _check_search_limits(self, search: str, k: int, n_cands: int) -> None:
         K = self.num_embeddings_per_hierarchy
@@ -914,9 +922,58 @@ class EncoderDecoderRetrievalModel(nn.Module):
     def _fused_encoder(self, attention: str = "fp32") -> FusedT5Encode:
         return FusedT5Encode(self, attention)
 
+    def _excluded_items(self, batch: TokenizedSeqBatch, exclude_items: Optional[Tensor],
+                        exclude_history: Optional[bool]) -> Optional[Tensor]:
+        """int64 [B, M]: exclude_items joined with the batch's own items when ``exclude_history`` (default
+        ``DEFAULT_EXCLUDE_HISTORY``); None when there is nothing to exclude."""
+        exclude_history = DEFAULT_EXCLUDE_HISTORY if exclude_history is None else exclude_history
+        parts = [] if exclude_items is None else [exclude_items]
+        if exclude_history:
+            parts.append(self.history_items(batch))
+        if not parts:
+            return None
+        B = batch.sem_ids.shape[0]
+        return torch.cat([self._check_exclude_items(t, B) for t in parts], dim=1)
+
+    @staticmethod
+    def _check_exclude_items(items: Tensor, B: int) -> Tensor:
+        ops._need_cuda(items)
+        if items.dim() != 2 or items.shape[0] != B or items.dtype.is_floating_point or items.dtype == torch.bool:
+            raise ValueError(f"exclude_items must be an integer [B = {B}, M] tensor of corpus rows, got {items.dtype} "
+                             f"{tuple(items.shape)}")
+        return items.long()
+
+    def _exclusion(self, items: Optional[Tensor], B: int, device: torch.device) -> Optional[ops.SidExclusion]:
+        """The exclusion sets of one call (``ops.sid_exclusion_build`` on the corpus item table), None without items."""
+        if items is None:
+            return None
+        items = self._check_exclude_items(items, B)
+        _, leaf_key, _ = self._rank_levels(device)
+        return ops.sid_exclusion_build(items.to(device), self._item_table(device), leaf_key)
+
+    @staticmethod
+    def _read_counters(counters: Tensor, exclusion: Optional[ops.SidExclusion], what: str) -> List[int]:
+        """The one host read at the end of a call: its counters, after which the excluded ids outside [-1, N) raise."""
+        if exclusion is None:
+            return counters.tolist()
+        *values, n_ids = torch.cat([counters.int(), exclusion.count[:, -1].sum(dtype=torch.int32).view(1)]).tolist()
+        if n_ids:
+            raise ValueError(f"{what}: {n_ids} excluded item id(s) outside [-1, N) where N is the number of corpus rows")
+        return values
+
+    @torch.no_grad()
+    def history_items(self, batch: TokenizedSeqBatch) -> Tensor:
+        """int64 [B, S]: the corpus item of each (H ids, dedup) group of ``batch.sem_ids`` (``item_of``), -1 where the group is
+        masked or does not resolve."""
+        H = self.num_hierarchies
+        B = batch.sem_ids.shape[0]
+        groups = batch.sem_ids.reshape(B, -1, H + 1)
+        items = self.item_of(groups.reshape(-1, H + 1)).view(B, -1)
+        return torch.where(batch.seq_mask.reshape(B, -1, H + 1)[:, :, :H].bool().all(-1), items, -1)
+
     @torch.no_grad()
     def generate(self, attention_mask, input_ids, user_id=None, search: Optional[str] = None, decoder: Optional[str] = None,
-                 encoder: Optional[str] = None, encoder_attention: Optional[str] = None):
+                 encoder: Optional[str] = None, encoder_attention: Optional[str] = None, exclude_items: Optional[Tensor] = None):
         """Top-k semantic ids by beam search restricted to id prefixes of the corpus.  ``search`` (default: the module's
         ``DEFAULT_SEARCH``, read at call time):
           "sample"  per level, n_cands = min(64, K) tokens sampled without replacement per beam, scored by cumulative
@@ -933,7 +990,15 @@ class EncoderDecoderRetrievalModel(nn.Module):
                     positions only; eval mode only.  It reads the packed row count on the host once, before the first level.
         ``encoder_attention`` (default: the module's ``DEFAULT_ENCODER_ATTENTION``, read at call time) picks the fused encoder's
         attention kernel: "fp32" or "tf32" (TF32 tensor-core products).  "tf32" needs encoder="fused".
+        ``exclude_items`` (integer [B, M], corpus rows, -1 pads, M <= ``ops.EXCLUDE_MAX_ITEMS``): no beam leads only to excluded
+        items of its history; an extension under which every retrievable item is excluded is invalid, like a prefix the corpus
+        lacks.  It adds one launch and no host read; ids outside [-1, N) raise ``ValueError`` after the search.
         Returns generated [B, top_k, num_hierarchies] and log_probas [B, top_k]."""
+        return self._generate(attention_mask, input_ids, user_id, search, decoder, encoder, encoder_attention,
+                              self._exclusion(exclude_items, attention_mask.shape[0], attention_mask.device))
+
+    def _generate(self, attention_mask, input_ids, user_id, search, decoder, encoder, encoder_attention,
+                  exclusion: Optional[ops.SidExclusion]):
         decoder = _choice(decoder, DEFAULT_DECODER, DECODERS, "generate", "decoder")
         if decoder == "fused" and self.training:
             raise ValueError("generate: decoder=\"fused\" runs the decoder in eval mode only; call model.eval() first (in "
@@ -960,6 +1025,7 @@ class EncoderDecoderRetrievalModel(nn.Module):
             rep_enc, rep_mask = enc_out.repeat_interleave(k, dim=0), enc_mask.repeat_interleave(k, dim=0)
             past_kv = EncoderDecoderCache(DynamicCache(), DynamicCache())
         reject = torch.zeros(1 if beam else 2, dtype=torch.int32, device=enc_out.device)
+        excl = {} if exclusion is None else {"exclude": exclusion}
         generated, log_probas, parent_global = None, None, None
         for h in range(self.num_hierarchies):
             first = generated is None
@@ -971,10 +1037,10 @@ class EncoderDecoderRetrievalModel(nn.Module):
                     attention_mask_for_encoder=enc_mask if first else rep_mask, use_cache=True, past_key_values=past_kv)
                 logits = self.decoder_mlp[h](dec_out[:, -1, :])
             if beam:
-                generated, log_probas, parent_global = index.beam_topk(logits, generated, log_probas, k, bad=reject)
+                generated, log_probas, parent_global = index.beam_topk(logits, generated, log_probas, k, bad=reject, **excl)
             else:
                 generated, log_probas, parent_global = self._sample_and_select(index, F.softmax(logits, dim=-1), generated,
-                                                                               log_probas, k, n_cands, reject)
+                                                                               log_probas, k, n_cands, reject, **excl)
             if fused is not None:
                 continue
             if first:
@@ -982,40 +1048,54 @@ class EncoderDecoderRetrievalModel(nn.Module):
             else:
                 past_kv.reorder_cache(parent_global)
         if beam:
-            n_bad = int(reject[0])
+            n_bad = int(reject[0]) if exclusion is None else self._read_counters(reject, exclusion, "generate")[0]
             if n_bad:
                 raise RuntimeError(f"generate: {n_bad} beam row(s) of the decoder head's logits hold a NaN or +inf or are all "
                                    "-inf; the beam search cannot rank them")
             return generated, log_probas
-        bad, zero_sum = reject.tolist()
+        bad, zero_sum = self._read_counters(reject, exclusion, "generate")
         if bad:
             raise RuntimeError(_MULTINOMIAL_ERRORS[0])
         if zero_sum:
             raise RuntimeError(_MULTINOMIAL_ERRORS[1])
         return generated, log_probas
 
+    def _batch_exclusion(self, batch: TokenizedSeqBatch, exclude_items, exclude_history) -> Optional[ops.SidExclusion]:
+        return self._exclusion(self._excluded_items(batch, exclude_items, exclude_history), batch.sem_ids.shape[0],
+                               batch.sem_ids.device)
+
+    def _generate_batch(self, batch: TokenizedSeqBatch, search, decoder, encoder, encoder_attention,
+                        exclusion: Optional[ops.SidExclusion]) -> GenerationOutput:
+        H = self.num_hierarchies
+        generated, log_probas = self._generate(_strip_dedup_col(batch.seq_mask.long(), H + 1, H),
+                                               _strip_dedup_col(batch.sem_ids, H + 1, H), batch.user_ids, search, decoder,
+                                               encoder, encoder_attention, exclusion)
+        return GenerationOutput(sem_ids=generated, log_probas=log_probas)
+
     @torch.no_grad()
     def generate_next_sem_id(self, batch: TokenizedSeqBatch, top_k: bool = True, temperature: int = 1,
                              search: Optional[str] = None, decoder: Optional[str] = None,
-                             encoder: Optional[str] = None, encoder_attention: Optional[str] = None) -> GenerationOutput:
-        H = self.num_hierarchies
-        generated, log_probas = self.generate(attention_mask=_strip_dedup_col(batch.seq_mask.long(), H + 1, H),
-                                              input_ids=_strip_dedup_col(batch.sem_ids, H + 1, H), user_id=batch.user_ids,
-                                              search=search, decoder=decoder, encoder=encoder,
-                                              encoder_attention=encoder_attention)
-        return GenerationOutput(sem_ids=generated, log_probas=log_probas)
+                             encoder: Optional[str] = None, encoder_attention: Optional[str] = None,
+                             exclude_items: Optional[Tensor] = None, exclude_history: Optional[bool] = None) -> GenerationOutput:
+        """``generate`` on the batch's histories.  ``exclude_items`` as in ``generate``; ``exclude_history`` (default
+        ``DEFAULT_EXCLUDE_HISTORY``, read at call time) also excludes each history's own items (``history_items``)."""
+        return self._generate_batch(batch, search, decoder, encoder, encoder_attention,
+                                    self._batch_exclusion(batch, exclude_items, exclude_history))
 
     @torch.no_grad()
     def generate_items(self, batch: TokenizedSeqBatch, n: Optional[int] = None, search: Optional[str] = None,
                        decoder: Optional[str] = None, encoder: Optional[str] = None,
-                       encoder_attention: Optional[str] = None) -> ItemGenerationOutput:
+                       encoder_attention: Optional[str] = None, exclude_items: Optional[Tensor] = None,
+                       exclude_history: Optional[bool] = None) -> ItemGenerationOutput:
         """The top corpus items for each history: ``generate_next_sem_id``'s beams, unchanged, then one launch that takes the
         items of every finite beam whose ids are in the corpus, beam by beam in descending score order, each beam's items by
-        dedup rank, no item twice, at most n (default top_k_for_generation) per history."""
-        out = self.generate_next_sem_id(batch, search=search, decoder=decoder, encoder=encoder,
-                                        encoder_attention=encoder_attention)
+        dedup rank, no item twice, at most n (default top_k_for_generation) per history.  ``exclude_items`` /
+        ``exclude_history`` as in ``generate_next_sem_id``: the search and the retrieval both leave the excluded items out."""
+        exclusion = self._batch_exclusion(batch, exclude_items, exclude_history)
+        out = self._generate_batch(batch, search, decoder, encoder, encoder_attention, exclusion)
         table = self._item_table(out.sem_ids.device)
-        items, beams, count = table.retrieve(out.sem_ids, out.log_probas, self.top_k_for_generation if n is None else n)
+        excl = {} if exclusion is None else {"exclude": exclusion}
+        items, beams, count = table.retrieve(out.sem_ids, out.log_probas, self.top_k_for_generation if n is None else n, **excl)
         return ItemGenerationOutput(item_ids=items, beams=beams, count=count, sem_ids=out.sem_ids, log_probas=out.log_probas)
 
     @torch.no_grad()
@@ -1131,21 +1211,32 @@ class EncoderDecoderRetrievalModel(nn.Module):
     @torch.no_grad()
     def rank_items(self, batch: TokenizedSeqBatch, n: Optional[int] = None, encoder: Optional[str] = None,
                    encoder_attention: Optional[str] = None, attention: Optional[str] = None,
-                   max_rows: Optional[int] = None) -> ItemRankingOutput:
+                   max_rows: Optional[int] = None, exclude_items: Optional[Tensor] = None,
+                   exclude_history: Optional[bool] = None) -> ItemRankingOutput:
         """Every retrievable corpus item ranked for each history by the model's exact log-probability (``rank_sem_ids``): the n
         best (default top_k_for_generation, at most ``MAX_RANK_ITEMS``) and the rank of ``item_of(batch.sem_ids_fut)``.  Order:
-        score descending, then tuple (lexicographic), then dedup rank; NaN last.  One selection launch after the decoder."""
+        score descending, then tuple (lexicographic), then dedup rank; NaN last.  One selection launch after the decoder.
+        ``exclude_items`` / ``exclude_history`` as in ``generate_next_sem_id``: excluded items are not returned and the target's
+        rank counts only the items that are not excluded (-1 when the target itself is excluded), the masked full-ranking
+        protocol; ``num_items`` stays the corpus's count."""
         n = self.top_k_for_generation if n is None else int(n)
         if not 1 <= n <= MAX_RANK_ITEMS:
             raise ValueError(f"rank_items: n = {n} must be in [1, {MAX_RANK_ITEMS}]")
         H = self.num_hierarchies
+        exclusion = self._batch_exclusion(batch, exclude_items, exclude_history)
         scores, bad, leaf_key, n_items = self._leaf_scores(
             _strip_dedup_col(batch.seq_mask.long(), H + 1, H), _strip_dedup_col(batch.sem_ids, H + 1, H), batch.user_ids,
             encoder, encoder_attention, attention, max_rows, "rank_items")
         fut = batch.sem_ids_fut
         row, start = self._item_table(scores.device).arrays()
-        items, item_scores, rank = ops.t5rank_select(scores, row, start, self._leaf_of(fut[:, :H], leaf_key), fut[:, H], n)
-        self._raise_bad(bad, "rank_items")
+        items, item_scores, rank = ops.t5rank_select(scores, row, start, self._leaf_of(fut[:, :H], leaf_key), fut[:, H], n,
+                                                     exclude=exclusion)
+        if exclusion is None:
+            self._raise_bad(bad, "rank_items")
+        else:
+            n_bad, = self._read_counters(bad, exclusion, "rank_items")
+            if n_bad:
+                raise _non_finite_error("rank_items", n_bad)
         return ItemRankingOutput(item_ids=items, scores=item_scores, target_rank=rank, num_items=n_items)
 
     # ------------------------------------------------------------------------------------------------ scoring given items

@@ -626,13 +626,15 @@ class SidPrefixIndex:
 
     def sample_select(self, probas: torch.Tensor, noise: torch.Tensor, generated: Optional[torch.Tensor],
                       log_probas: Optional[torch.Tensor], k: int, nc: int, want_samples: bool = False,
-                      reject: Optional[torch.Tensor] = None):
+                      reject: Optional[torch.Tensor] = None, exclude: Optional["SidExclusion"] = None):
         """The sampling step fused with ``beam_select`` (rqb200_sid_trie_sample_select), one launch.  probas / noise [B * kp, K]
         (kp = 1 on the first level; noise = the Exp(1) draw torch.multinomial makes, ``torch.empty_like(probas).exponential_(1)``),
         generated [B, kp, h] or None, log_probas [B, kp] or None -> (generated [B, k, h + 1], log_probas [B, k],
         parent_global [B * k]), plus (samples [B * kp, nc], samp_log_p [B * kp, nc]) when ``want_samples``: the samples are
         ``torch.multinomial(probas, nc)``'s under the same generator state.  ``reject``, an int32 [2] device tensor, is ADDED the
-        number of rows torch.multinomial would reject: [0] with a NaN, +-inf or negative entry, [1] otherwise all zero."""
+        number of rows torch.multinomial would reject: [0] with a NaN, +-inf or negative entry, [1] otherwise all zero.
+        ``exclude`` (``sid_exclusion_build``, one set per history): extensions to a prefix blocked for the history are invalid,
+        exactly like prefixes the corpus lacks; the samples do not change."""
         _need_cuda(probas, noise, reject)
         if generated is None:
             B, kp, h = probas.shape[0], 1, 0
@@ -656,23 +658,30 @@ class SidPrefixIndex:
         samples = torch.empty((B * kp, nc), dtype=torch.int64, device=dev) if want_samples else None
         samp_log_p = torch.empty((B * kp, nc), dtype=torch.float32, device=dev) if want_samples else None
         with torch.cuda.device(dev):
-            _lib.check(_lib.load().rqb200_sid_trie_sample_select(_p(probas), probas.stride(0), _p(noise), noise.stride(0),
-                                                                 _p(generated), _p(log_probas), B, kp, nc, h, k, self.C, self.K,
-                                                                 _p(self.ws), _p(out_g), _p(out_p), _p(out_parent), _p(samples),
-                                                                 _p(samp_log_p), _p(reject), _stream()), "sid_trie_sample_select")
+            if exclude is None:
+                _lib.check(_lib.load().rqb200_sid_trie_sample_select(
+                    _p(probas), probas.stride(0), _p(noise), noise.stride(0), _p(generated), _p(log_probas), B, kp, nc, h, k,
+                    self.C, self.K, _p(self.ws), _p(out_g), _p(out_p), _p(out_parent), _p(samples), _p(samp_log_p), _p(reject),
+                    _stream()), "sid_trie_sample_select")
+            else:
+                _lib.check(_lib.load().rqb200_sid_trie_sample_select_excluding(
+                    _p(probas), probas.stride(0), _p(noise), noise.stride(0), _p(generated), _p(log_probas), B, kp, nc, h, k,
+                    self.C, self.K, _p(self.ws), _p(out_g), _p(out_p), _p(out_parent), _p(samples), _p(samp_log_p), _p(reject),
+                    *exclude.args(B, h + 1, "sample_select"), _stream()), "sid_trie_sample_select_excluding")
         _count(1)
         if want_samples:
             return out_g, out_p, out_parent, samples, samp_log_p
         return out_g, out_p, out_parent
 
     def beam_topk(self, logits: torch.Tensor, generated: Optional[torch.Tensor], log_probas: Optional[torch.Tensor], k: int,
-                  bad: Optional[torch.Tensor] = None):
+                  bad: Optional[torch.Tensor] = None, exclude: Optional["SidExclusion"] = None):
         """One level of the exhaustive constrained beam search from the head's logits (rqb200_sid_trie_beam_topk), one launch.
         logits [B * kp, K] (kp = 1 on the first level), generated [B, kp, h] or None, log_probas [B, kp] or None ->
         (generated [B, k, h + 1], log_probas [B, k], parent_global [B * k]): of all kp * K extensions of each history, scored
         log_softmax(logits)[code] + the parent's log-probability (-inf when the extended prefix is not in the corpus), the k
         best in descending order, equal scores by ascending beam * K + code.  Deterministic.  ``bad``, an int32 device tensor,
-        is ADDED the number of beam rows whose logits hold a NaN or +inf or are all -inf."""
+        is ADDED the number of beam rows whose logits hold a NaN or +inf or are all -inf.  ``exclude`` as in ``sample_select``:
+        extensions to a prefix blocked for the history score -inf."""
         _need_cuda(logits, bad)
         if generated is None:
             B, kp, h = logits.shape[0], 1, 0
@@ -694,9 +703,15 @@ class SidPrefixIndex:
         out_p = torch.empty((B, k), dtype=torch.float32, device=dev)
         out_parent = torch.empty((B * k,), dtype=torch.int64, device=dev)
         with torch.cuda.device(dev):
-            _lib.check(_lib.load().rqb200_sid_trie_beam_topk(_p(logits), logits.stride(0), _p(generated), _p(log_probas), B, kp,
-                                                             h, k, self.C, self.K, _p(self.ws), _p(out_g), _p(out_p),
-                                                             _p(out_parent), _p(bad), _stream()), "sid_trie_beam_topk")
+            if exclude is None:
+                _lib.check(_lib.load().rqb200_sid_trie_beam_topk(_p(logits), logits.stride(0), _p(generated), _p(log_probas), B,
+                                                                 kp, h, k, self.C, self.K, _p(self.ws), _p(out_g), _p(out_p),
+                                                                 _p(out_parent), _p(bad), _stream()), "sid_trie_beam_topk")
+            else:
+                _lib.check(_lib.load().rqb200_sid_trie_beam_topk_excluding(
+                    _p(logits), logits.stride(0), _p(generated), _p(log_probas), B, kp, h, k, self.C, self.K, _p(self.ws), _p(out_g),
+                    _p(out_p), _p(out_parent), _p(bad), *exclude.args(B, h + 1, "beam_topk"), _stream()),
+                    "sid_trie_beam_topk_excluding")
         _count(1)
         return out_g, out_p, out_parent
 
@@ -789,10 +804,12 @@ class SidItemTable:
         _count(1)
         return out.reshape(lead)
 
-    def retrieve(self, generated: torch.Tensor, log_probas: Optional[torch.Tensor], n: int):
+    def retrieve(self, generated: torch.Tensor, log_probas: Optional[torch.Tensor], n: int,
+                 exclude: Optional["SidExclusion"] = None):
         """generated [B, k, C], log_probas [B, k] or None -> (items [B, n] int64, beam [B, n] int32, count [B] int32): per
         history, in beam order, the items of every beam whose log-probability is above -inf and whose tuple is in the corpus,
-        each beam's in dedup-rank order, no item twice, cut off at n; -1 pads items and beam.  k <= 1024, n <= 4096."""
+        each beam's in dedup-rank order, no item twice, cut off at n; -1 pads items and beam.  k <= 1024, n <= 4096.
+        ``exclude`` (``sid_exclusion_build`` on this table): the history's excluded items are skipped."""
         _need_cuda(generated, log_probas)
         B, k, C = generated.shape
         if C != self.C:
@@ -806,8 +823,13 @@ class SidItemTable:
         beam = torch.empty((B, n), dtype=torch.int32, device=dev)
         count = torch.empty((B,), dtype=torch.int32, device=dev)
         with torch.cuda.device(dev):
-            _lib.check(_lib.load().rqb200_sid_items_retrieve(_p(self.ws), _p(generated), _p(log_probas), B, k, C, n, _p(items),
-                                                             _p(beam), _p(count), _stream()), "sid_items_retrieve")
+            if exclude is None:
+                _lib.check(_lib.load().rqb200_sid_items_retrieve(_p(self.ws), _p(generated), _p(log_probas), B, k, C, n,
+                                                                 _p(items), _p(beam), _p(count), _stream()), "sid_items_retrieve")
+            else:
+                _lib.check(_lib.load().rqb200_sid_items_retrieve_excluding(
+                    _p(self.ws), _p(generated), _p(log_probas), B, k, C, n, _p(items), _p(beam), _p(count),
+                    *exclude.args(B, 0, "retrieve"), _stream()), "sid_items_retrieve_excluding")
         _count(1)
         return items, beam, count
 
@@ -820,6 +842,72 @@ class SidItemTable:
         row = self.ws[row_off.value:row_off.value + 4 * self.N].view(torch.int32)
         start = self.ws[start_off.value:start_off.value + 4 * (self.N + 1)].view(torch.int32)
         return row, start
+
+    def positions(self) -> torch.Tensor:
+        """int32 [N]: each item's position in the table's row array (the inverse permutation of ``arrays()[0]``), built once
+        and cached on the table."""
+        if getattr(self, "_positions", None) is None:
+            row, _ = self.arrays()
+            inv = torch.empty(self.N, dtype=torch.int32, device=self.device)
+            inv[row.long()] = torch.arange(self.N, dtype=torch.int32, device=self.device)
+            self._positions = inv
+        return self._positions
+
+
+#: most entries per history an exclusion set takes (sid_exclusion_build sorts them in shared memory)
+EXCLUDE_MAX_ITEMS = 4096
+
+
+class SidExclusion(NamedTuple):
+    """Each history's exclusion set (``sid_exclusion_build``).  pos int32 [B, M]: the distinct excluded retrievable items as
+    positions in the item table's row array, ascending; blocked int64 [B, H, M]: per level l = 1..H the keys (``_tuple_key``
+    of the prefix) of the blocked l-prefixes, ascending -- prefixes holding an excluded item under which every retrievable
+    item is excluded; count int32 [B, H + 2]: [0] the positions, [l] the blocked l-prefixes, [H + 1] the entries outside
+    [-1, N).  Entries past a count are -1."""
+    pos: torch.Tensor
+    blocked: torch.Tensor
+    count: torch.Tensor
+
+    def args(self, B: int, levels: int, what: str):
+        """The exclusion arguments of the *_excluding entry points, for B histories and a level up to ``levels``."""
+        _need_cuda(self.pos)
+        H = self.blocked.shape[1]
+        if self.pos.shape[0] != B:
+            raise ValueError(f"{what}: the exclusion holds {self.pos.shape[0]} histories, the call {B}")
+        if levels > H:
+            raise ValueError(f"{what}: level {levels} is deeper than the exclusion's {H} levels")
+        return _p(self.pos), _p(self.blocked), _p(self.count), self.pos.shape[1], H
+
+
+def sid_exclusion_build(items: torch.Tensor, table: SidItemTable, leaf_key: torch.Tensor) -> SidExclusion:
+    """Each history's exclusion set (rqb200_sid_exclusion_build), one launch, no host read.  items integer [B, M] (corpus rows,
+    -1 pads, repeats allowed, M <= ``EXCLUDE_MAX_ITEMS``), table the corpus's ``SidItemTable`` (H = its C ids per tuple),
+    leaf_key int64 [U]: the table's U distinct retrievable tuples packed K-ary (level 0 most significant), ascending.  Rows
+    that are not retrievable are ignored; ids outside [-1, N) are counted in count[:, H + 1]."""
+    _need_cuda(items, leaf_key)
+    if items.dim() != 2 or items.dtype.is_floating_point or items.dtype.is_complex or items.dtype == torch.bool:
+        raise ValueError(f"exclusion: items must be an integer [B, M] tensor, got {items.dtype} {tuple(items.shape)}")
+    B, M = items.shape
+    if M > EXCLUDE_MAX_ITEMS:
+        raise ValueError(f"exclusion: M = {M} items per history exceeds {EXCLUDE_MAX_ITEMS}")
+    dev = items.device
+    items = items.to(torch.int64)
+    if M == 0:
+        items, M = torch.full((B, 1), -1, dtype=torch.int64, device=dev), 1
+    items = items.contiguous()
+    leaf_key = leaf_key.to(torch.int64).contiguous()
+    H, U = table.C, leaf_key.shape[0]
+    _, start = table.arrays()
+    pos = torch.empty((B, M), dtype=torch.int32, device=dev)
+    blocked = torch.empty((B, H, M), dtype=torch.int64, device=dev)
+    count = torch.empty((B, H + 2), dtype=torch.int32, device=dev)
+    inv = table.positions()
+    with torch.cuda.device(dev):
+        _lib.check(_lib.load().rqb200_sid_exclusion_build(_p(items), B, M, table.N, _p(inv), _p(start), _p(leaf_key), U, H,
+                                                          table.K, _p(pos), _p(blocked), _p(count), _stream()),
+                   "sid_exclusion_build")
+    _count(1)
+    return SidExclusion(pos, blocked, count)
 
 
 def sid_rank_hist(rank: torch.Tensor, hist: torch.Tensor) -> None:
@@ -1065,11 +1153,13 @@ def t5rank_children(logits: torch.Tensor, parent: Optional[torch.Tensor], child:
 
 
 def t5rank_select(scores: torch.Tensor, row: torch.Tensor, start: torch.Tensor, t_leaf: torch.Tensor, t_dedup: torch.Tensor,
-                  n: int):
+                  n: int, exclude: Optional[SidExclusion] = None):
     """The n best items of each history from its leaf scores (rqb200_t5rank_select), one launch.  scores fp32 [B, U] (leaf u =
     item-table tuple u), (row, start) = ``SidItemTable.arrays()``, t_leaf / t_dedup int64 [B] (the target's tuple, -1 when it has
     none, and dedup rank) -> (items int64 [B, n], item scores fp32 [B, n], target rank int64 [B]): items by score descending, then
-    tuple, then dedup rank, NaN last; -1 / -inf pad; rank -1 when the target is not ranked.  n <= 1024."""
+    tuple, then dedup rank, NaN last; -1 / -inf pad; rank -1 when the target is not ranked.  n <= 1024.  ``exclude``
+    (``sid_exclusion_build`` on the same table): the history's excluded items are skipped and the rank counts only the items
+    that are not excluded (-1 when the target is excluded)."""
     _need_cuda(scores, row, start, t_leaf, t_dedup)
     scores = _f32c(scores)
     if scores.dim() != 2:
@@ -1087,8 +1177,14 @@ def t5rank_select(scores: torch.Tensor, row: torch.Tensor, start: torch.Tensor, 
     item_scores = torch.empty((B, n), dtype=torch.float32, device=dev)
     rank = torch.empty((B,), dtype=torch.int64, device=dev)
     with torch.cuda.device(dev):
-        _lib.check(_lib.load().rqb200_t5rank_select(_p(scores), B, U, _p(row), _p(start), _p(t_leaf), _p(t_dedup), n, _p(items),
-                                                    _p(item_scores), _p(rank), _stream()), "t5rank_select")
+        if exclude is None:
+            _lib.check(_lib.load().rqb200_t5rank_select(_p(scores), B, U, _p(row), _p(start), _p(t_leaf), _p(t_dedup), n,
+                                                        _p(items), _p(item_scores), _p(rank), _stream()), "t5rank_select")
+        else:
+            _lib.check(_lib.load().rqb200_t5rank_select_excluding(_p(scores), B, U, _p(row), _p(start), _p(t_leaf), _p(t_dedup), n,
+                                                                  _p(items), _p(item_scores), _p(rank),
+                                                                  *exclude.args(B, 0, "t5rank_select"), _stream()),
+                       "t5rank_select_excluding")
     _count(1)
     return items, item_scores, rank
 
