@@ -240,6 +240,16 @@ int rqb200_sid_trie_sample_select_excluding(const float* probas, int64_t probas_
                                             float* out_log_probas, int64_t* out_parent, int64_t* samples, float* samp_log_p,
                                             int* reject, const int* ex_pos, const int64_t* ex_blocked, const int* ex_count, int ex_M,
                                             int ex_H, void* stream);
+/* sid_trie_sample_select_including : the same call with each history's allow-list (sid_inclusion_build; in_count null: none).
+ *                    A beam's children are the keys of level h + 1 of in_keys under its prefix (the prefixes holding an eligible
+ *                    item); every other extension is invalid, exactly like a prefix the corpus lacks.  The noise, samples and
+ *                    samp_log_p are unchanged.  Needs in_H > h and in_M <= 4096. */
+int rqb200_sid_trie_sample_select_including(const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride,
+                                            const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k,
+                                            int C, int K, const void* prefix_workspace, int64_t* out_generated,
+                                            float* out_log_probas, int64_t* out_parent, int64_t* samples, float* samp_log_p,
+                                            int* reject, const int* in_pos, const int64_t* in_keys, const int* in_count, int in_M,
+                                            int in_H, void* stream);
 
 /* sid_trie_beam_topk : one level h of the exhaustive (deterministic) constrained beam search, from the head's logits, one launch:
  *   logits           [B*kp, K] fp32, row stride in elements (kp = 1 at h = 0, where generated and log_probas may be null)
@@ -261,6 +271,13 @@ int rqb200_sid_trie_beam_topk_excluding(const float* logits, int64_t logits_stri
                                         int B, int kp, int h, int k, int C, int K, const void* prefix_workspace,
                                         int64_t* out_generated, float* out_log_probas, int64_t* out_parent, int* bad,
                                         const int* ex_pos, const int64_t* ex_blocked, const int* ex_count, int ex_M, int ex_H,
+                                        void* stream);
+/* sid_trie_beam_topk_including : the same call with each history's allow-list, as sid_trie_sample_select_including: an extension
+ *                    to a prefix without an eligible item scores -inf like one the corpus lacks. */
+int rqb200_sid_trie_beam_topk_including(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas,
+                                        int B, int kp, int h, int k, int C, int K, const void* prefix_workspace,
+                                        int64_t* out_generated, float* out_log_probas, int64_t* out_parent, int* bad,
+                                        const int* in_pos, const int64_t* in_keys, const int* in_count, int in_M, int in_H,
                                         void* stream);
 
 /* The trie's level arrays as plain device arrays (the exact ranking decodes one row per node).
@@ -317,6 +334,24 @@ int rqb200_sid_items_retrieve_excluding(const void* workspace, const int64_t* ge
  *                       of the input.  B = 0 is a no-op. */
 int rqb200_sid_exclusion_build(const int64_t* items, int B, int M, int64_t N, const int* inv, const int* start,
                                const int64_t* leaf_key, int U, int H, int K, int* pos, int64_t* blocked, int* count, void* stream);
+/* sid_items_retrieve_including : the same call with each history's allow-list (sid_inclusion_build, on this table): a beam counts
+ *                       its tuple's eligible items, in dedup order; no other item is written. */
+int rqb200_sid_items_retrieve_including(const void* workspace, const int64_t* generated, const float* log_probas, int B, int k, int C,
+                                        int n, int64_t* out_items, int* out_beam, int* out_count, const int* in_pos,
+                                        const int64_t* in_keys, const int* in_count, int in_M, int in_H, void* stream);
+/* sid_inclusion_build : each history's allow-list, one CTA per history, with the arguments of sid_exclusion_build plus an optional
+ *                       exclusion of the same histories (its arrays; ex_count null: none), which is folded in.  items are the
+ *                       allowed corpus rows (-1 pads, repeats allowed, M <= 4096).  An item is eligible when it is allowed,
+ *                       retrievable and not excluded.  Writes
+ *                         pos int32 [B, M]          the distinct positions of the eligible items, ascending (-1 after);
+ *                         keys int64 [B, H, M]      per level l = 1..H the packed keys of the distinct l-prefixes of the eligible
+ *                                                   items (the valid l-prefixes), ascending (-1 after);
+ *                         count int32 [B, H + 2]    [0] the positions, [l] the valid l-prefixes, [H + 1] the entries of items
+ *                                                   outside [-1, N) (otherwise ignored).
+ *                       Plain stores: the output is a function of the input.  B = 0 is a no-op. */
+int rqb200_sid_inclusion_build(const int64_t* items, int B, int M, int64_t N, const int* inv, const int* start,
+                               const int64_t* leaf_key, int U, int H, int K, int* pos, int64_t* keys, int* count,
+                               const int* ex_pos, const int64_t* ex_blocked, const int* ex_count, int ex_M, int ex_H, void* stream);
 /* sid_items_offsets   : byte offsets of row (int32 [N]) and start (int32 [N + 1]) in the item table's workspace; arithmetic only.
  *                       RQB_ERR_UNSUPPORTED outside the table's limits. */
 int rqb200_sid_items_offsets(int64_t N, int C, int K, size_t* row, size_t* start);

@@ -80,6 +80,11 @@ _SIGNATURES = {
                                                         c_int, c_int, c_vp]),
     "rqb200_sid_trie_beam_topk_excluding": (c_int, [c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp,
                                                     c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
+    "rqb200_sid_trie_sample_select_including": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int,
+                                                        c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                                        c_int, c_int, c_vp]),
+    "rqb200_sid_trie_beam_topk_including": (c_int, [c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp,
+                                                    c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
     "rqb200_sid_items_workspace_bytes": (c_size, [c_i64, c_int, c_int]),
     "rqb200_sid_items_build": (c_int, [c_vp, c_i64, c_int, c_int, c_vp, c_size, c_vp]),
     "rqb200_sid_items_lookup": (c_int, [c_vp, c_vp, c_i64, c_i64, c_int, c_vp, c_vp]),
@@ -88,6 +93,10 @@ _SIGNATURES = {
                                                     c_vp, c_int, c_int, c_vp]),
     "rqb200_sid_exclusion_build": (c_int, [c_vp, c_int, c_int, c_i64, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp,
                                            c_vp]),
+    "rqb200_sid_items_retrieve_including": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                                    c_vp, c_int, c_int, c_vp]),
+    "rqb200_sid_inclusion_build": (c_int, [c_vp, c_int, c_int, c_i64, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp,
+                                           c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
     "rqb200_sid_topk_rank_hist": (c_int, [c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "rqb200_sid_rank_hist": (c_int, [c_vp, c_int, c_i64, c_vp, c_vp]),
     "rqb200_sid_trie_counts": (c_int, [c_vp, c_vp, c_vp]),

@@ -539,13 +539,58 @@ __device__ __forceinline__ void sid_mask_unblock(const SidExcl& ex, int64_t b, c
     key = key * K + (v < 0 ? 0 : v >= K ? K - 1 : v);       // a beam holding such an id is no corpus prefix: its mask is empty
   }
   const long long lo = key * K, hi = lo + K;
-  const long long* list = ex.blocked_of(b, h + 1);
-  const int n = ex.nblocked(b, h + 1);
+  const long long* list = ex.keys_of(b, h + 1);
+  const int n = ex.nkeys(b, h + 1);
   for (int i = sid_lower_bound(list, n, lo) + lane; i < n && __ldg(list + i) < hi; i += 32) {
     const int c = (int)(__ldg(list + i) - lo);
     atomicAnd(&mask[c >> 5], ~(1u << (c & 31)));
   }
   __syncwarp();
+}
+
+// One warp, with an allow-list (SidExcl::include): mask = bit c set for every child code c of the beam ids[0, h) that is valid
+// for history b, the keys [key(ids[0, h)) K, key(ids[0, h)) K + K) of level h + 1's allowed list (two binary searches).  The
+// allowed keys are corpus prefixes, so the trie is not read.  The warp is synchronised on return.
+__device__ __forceinline__ void sid_allowed_mask(const SidExcl& in, int64_t b, const int64_t* ids, int h, int K, unsigned int* mask,
+                                                 int lane) {
+  for (int i = lane; i < (K + 31) >> 5; i += 32) mask[i] = 0;
+  long long key = 0;
+  bool ok = true;                                           // a beam holding an id outside [0, K) has no valid child
+  for (int j = 0; j < h; ++j) {
+    const int64_t v = ids[j];
+    ok &= v >= 0 && v < K;
+    key = key * K + (ok ? v : 0);
+  }
+  __syncwarp();
+  if (ok) {
+    const long long lo = key * K;
+    const long long* list = in.keys_of(b, h + 1);
+    const int n = in.nkeys(b, h + 1);
+    const int end = sid_lower_bound(list, n, lo + K);
+    for (int i = sid_lower_bound(list, n, lo) + lane; i < end; i += 32) {
+      const int c = (int)(__ldg(list + i) - lo);
+      atomicOr(&mask[c >> 5], 1u << (c & 31));
+    }
+  }
+  __syncwarp();
+}
+
+// One warp: the K-bit mask of the beam's valid children under the consumer's filter mode (SidFilterMode): the trie's children,
+// less the blocked ones with an exclusion, or the allowed ones with an inclusion.  The warp is synchronised on return.
+template <int FILTER>
+__device__ __forceinline__ void sid_beam_mask(const SidTrie& trie, const SidExcl& f, int64_t b, const int64_t* ids, int h, int K,
+                                              unsigned int* mask, int lane) {
+  if (FILTER == SID_FILTER_INCLUDE) {
+    sid_allowed_mask(f, b, ids, h, K, mask, lane);
+    return;
+  }
+  sid_child_mask(trie, ids, h, K, mask, lane);
+  if (FILTER == SID_FILTER_EXCLUDE) sid_mask_unblock(f, b, ids, h, K, mask, lane);
+}
+
+// the filter mode of a filter argument (count null: none)
+__host__ __forceinline__ int sid_filter_mode(const SidExcl& f) {
+  return !f.count ? SID_FILTER_NONE : f.include ? SID_FILTER_INCLUDE : SID_FILTER_EXCLUDE;
 }
 
 // valid[p] = any corpus row whose first l ids equal prefix[p, :l]      (model.py:175-181)
@@ -763,7 +808,7 @@ static size_t sid_sample_smem(int kp, int nc, int K) {
   return E * (sizeof(int64_t) + sizeof(float) + 1) + (size_t)W * (K + 256 + 2 * nc + (K + 31) / 32) * 4;
 }
 
-template <bool EXCL>                                        // EXCL: with an exclusion (the mask clearing is compiled only then)
+template <int FILTER>                                       // SidFilterMode: the filter's code is compiled only with one
 __global__ void __launch_bounds__(SID_SAMPLE_MAX_WARPS * 32) sid_sample_select_kernel(
     const float* __restrict__ probas, int64_t p_stride, const float* __restrict__ noise, int64_t n_stride,
     const int64_t* __restrict__ generated, const float* __restrict__ log_probas, int kp, int nc, int h, int k, int K, SidTrie trie,
@@ -796,8 +841,7 @@ __global__ void __launch_bounds__(SID_SAMPLE_MAX_WARPS * 32) sid_sample_select_k
     if (reject && lane == 0 && (bad || !nonzero)) atomicAdd(&reject[bad ? 0 : 1], 1);
     __syncwarp();
     sid_warp_top_n(s_key, K, nc, s_hist, s_sk, s_si, s_tok + beam * nc, lane);
-    sid_child_mask(trie, generated + row * h, h, K, s_mask, lane);
-    if (EXCL) sid_mask_unblock(ex, b, generated + row * h, h, K, s_mask, lane);
+    sid_beam_mask<FILTER>(trie, ex, b, generated + row * h, h, K, s_mask, lane);
     const float plp = log_probas ? log_probas[row] : 0.f;
     for (int r = lane; r < nc; r += 32) {
       const int64_t tok = s_tok[beam * nc + r];
@@ -813,13 +857,15 @@ __global__ void __launch_bounds__(SID_SAMPLE_MAX_WARPS * 32) sid_sample_select_k
     sid_keep_best(s_score, s_taken, s_tok, E, nc, b, kp, h, k, generated, out_generated, out_log_probas, out_parent, lane);
 }
 
-// The exclusion arguments of the *_excluding entry points: the arrays of rqb200_sid_exclusion_build (count null: none).
-static int sid_excl_of(const int* pos, const int64_t* blocked, const int* count, int M, int H, int levels, const char* what,
-                       SidExcl& ex) {
-  ex = SidExcl{pos, reinterpret_cast<const long long*>(blocked), count, M, H};
+// The filter arguments of the *_excluding / *_including entry points: the arrays of rqb200_sid_exclusion_build /
+// rqb200_sid_inclusion_build (count null: none).
+static int sid_excl_of(const int* pos, const int64_t* keys, const int* count, int M, int H, int levels, const char* what,
+                       SidExcl& ex, bool include = false) {
+  ex = SidExcl{pos, reinterpret_cast<const long long*>(keys), count, M, H, include};
   if (!count) return RQB_OK;
-  RQB_CHECK_ARG(pos && blocked && M > 0 && M <= SID_EXCL_MAX_M && H >= levels && H <= RQB_MAX_LEVELS,
-                "%s: bad exclusion (M = %d, H = %d, need M <= %d and H >= %d)", what, M, H, SID_EXCL_MAX_M, levels);
+  RQB_CHECK_ARG(pos && keys && M > 0 && M <= SID_EXCL_MAX_M && H >= levels && H <= RQB_MAX_LEVELS,
+                "%s: bad %s (M = %d, H = %d, need M <= %d and H >= %d)", what, include ? "inclusion" : "exclusion", M, H,
+                SID_EXCL_MAX_M, levels);
   return RQB_OK;
 }
 
@@ -840,7 +886,10 @@ static int sid_sample_select(const float* probas, int64_t probas_stride, const f
                     (h == 0 || log_probas), "sid_trie_sample_select: null pointer");
   const int W = kp < SID_SAMPLE_MAX_WARPS ? kp : SID_SAMPLE_MAX_WARPS;
   const size_t smem = sid_sample_smem(kp, nc, K);
-  auto kernel = ex.count ? sid_sample_select_kernel<true> : sid_sample_select_kernel<false>;
+  const int mode = sid_filter_mode(ex);
+  auto kernel = mode == SID_FILTER_INCLUDE ? sid_sample_select_kernel<SID_FILTER_INCLUDE>
+                : mode == SID_FILTER_EXCLUDE ? sid_sample_select_kernel<SID_FILTER_EXCLUDE>
+                                             : sid_sample_select_kernel<SID_FILTER_NONE>;
   RQB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kernel<<<B, W * 32, smem, reinterpret_cast<cudaStream_t>(stream)>>>(
       probas, probas_stride, noise, noise_stride, generated, log_probas, kp, nc, h, k, K,
@@ -869,6 +918,18 @@ extern "C" int rqb200_sid_trie_sample_select_excluding(
   if (rc != RQB_OK) return rc;
   return sid_sample_select(probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K, prefix_workspace,
                            out_generated, out_log_probas, out_parent, samples, samp_log_p, reject, ex, stream);
+}
+
+extern "C" int rqb200_sid_trie_sample_select_including(
+    const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride, const int64_t* generated,
+    const float* log_probas, int B, int kp, int nc, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
+    float* out_log_probas, int64_t* out_parent, int64_t* samples, float* samp_log_p, int* reject, const int* in_pos,
+    const int64_t* in_keys, const int* in_count, int in_M, int in_H, void* stream) {
+  SidExcl in;
+  const int rc = sid_excl_of(in_pos, in_keys, in_count, in_M, in_H, h + 1, "sid_trie_sample_select_including", in, true);
+  if (rc != RQB_OK) return rc;
+  return sid_sample_select(probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K, prefix_workspace,
+                           out_generated, out_log_probas, out_parent, samples, samp_log_p, reject, in, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -908,7 +969,7 @@ __device__ __forceinline__ unsigned int sid_topk_candidate(const float* __restri
   return sid_topk_key(sc == 0.f ? 0.f : sc);
 }
 
-template <bool KEYS_IN_SMEM>
+template <bool KEYS_IN_SMEM, int FILTER>                    // FILTER: SidFilterMode
 __global__ void __launch_bounds__(SID_TOPK_MAX_THREADS) sid_beam_topk_kernel(
     const float* __restrict__ logits, int64_t ld, const int64_t* __restrict__ generated, const float* __restrict__ log_probas,
     int kp, int h, int k, int K, SidTrie trie, int64_t* __restrict__ out_generated, float* __restrict__ out_log_probas,
@@ -947,10 +1008,8 @@ __global__ void __launch_bounds__(SID_TOPK_MAX_THREADS) sid_beam_topk_kernel(
     }
   }
   __syncthreads();
-  for (int beam = w; beam < kp; beam += W) {
-    sid_child_mask(trie, s.gen + beam * h, h, K, s_mask + beam * ((K + 31) >> 5), lane);
-    sid_mask_unblock(ex, b, s.gen + beam * h, h, K, s_mask + beam * ((K + 31) >> 5), lane);
-  }
+  for (int beam = w; beam < kp; beam += W)
+    sid_beam_mask<FILTER>(trie, ex, b, s.gen + beam * h, h, K, s_mask + beam * ((K + 31) >> 5), lane);
   __syncthreads();
   unsigned long long prefix = 0, pmask = 0;
   int want = k;                                             // entries still needed among those matching the decided digits
@@ -1030,6 +1089,26 @@ __global__ void __launch_bounds__(SID_TOPK_MAX_THREADS) sid_beam_topk_kernel(
   }
 }
 
+template <int FILTER>
+static int sid_beam_topk_launch(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas,
+                                int B, int kp, int h, int k, int K, const SidTrie& trie, int64_t* out_generated,
+                                float* out_log_probas, int64_t* out_parent, int* bad, const SidExcl& ex, cudaStream_t st) {
+  const int E = kp * K;
+  const int nt = E >= 4096 ? SID_TOPK_MAX_THREADS : E >= 1024 ? 256 : 128;
+  const size_t mask = (size_t)kp * ((K + 31) / 32) * sizeof(unsigned int);
+  if (E <= SID_TOPK_SMEM_KEYS) {
+    const size_t smem = (size_t)E * sizeof(unsigned int) + mask;
+    RQB_CUDA(cudaFuncSetAttribute(sid_beam_topk_kernel<true, FILTER>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    sid_beam_topk_kernel<true, FILTER><<<B, nt, smem, st>>>(logits, logits_stride, generated, log_probas, kp, h, k, K, trie,
+                                                            out_generated, out_log_probas, out_parent, bad, ex);
+  } else {
+    sid_beam_topk_kernel<false, FILTER><<<B, nt, mask, st>>>(logits, logits_stride, generated, log_probas, kp, h, k, K, trie,
+                                                             out_generated, out_log_probas, out_parent, bad, ex);
+  }
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
+}
+
 static int sid_beam_topk(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas, int B, int kp,
                          int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated, float* out_log_probas,
                          int64_t* out_parent, int* bad, const SidExcl& ex, void* stream) {
@@ -1044,21 +1123,18 @@ static int sid_beam_topk(const float* logits, int64_t logits_stride, const int64
   RQB_CHECK_ARG(logits && prefix_workspace && out_generated && out_log_probas && out_parent && (h == 0 || generated) &&
                     (h == 0 || log_probas), "sid_trie_beam_topk: null pointer");
   const SidTrie trie{reinterpret_cast<const unsigned char*>(prefix_workspace), h + 1};
-  const int E = kp * K;
-  const int nt = E >= 4096 ? SID_TOPK_MAX_THREADS : E >= 1024 ? 256 : 128;
-  const size_t mask = (size_t)kp * ((K + 31) / 32) * sizeof(unsigned int);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (E <= SID_TOPK_SMEM_KEYS) {
-    const size_t smem = (size_t)E * sizeof(unsigned int) + mask;
-    RQB_CUDA(cudaFuncSetAttribute(sid_beam_topk_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    sid_beam_topk_kernel<true><<<B, nt, smem, st>>>(logits, logits_stride, generated, log_probas, kp, h, k, K, trie, out_generated,
-                                                    out_log_probas, out_parent, bad, ex);
-  } else {
-    sid_beam_topk_kernel<false><<<B, nt, mask, st>>>(logits, logits_stride, generated, log_probas, kp, h, k, K, trie, out_generated,
-                                                     out_log_probas, out_parent, bad, ex);
+  switch (sid_filter_mode(ex)) {
+    case SID_FILTER_INCLUDE:
+      return sid_beam_topk_launch<SID_FILTER_INCLUDE>(logits, logits_stride, generated, log_probas, B, kp, h, k, K, trie,
+                                                      out_generated, out_log_probas, out_parent, bad, ex, st);
+    case SID_FILTER_EXCLUDE:
+      return sid_beam_topk_launch<SID_FILTER_EXCLUDE>(logits, logits_stride, generated, log_probas, B, kp, h, k, K, trie,
+                                                      out_generated, out_log_probas, out_parent, bad, ex, st);
+    default:
+      return sid_beam_topk_launch<SID_FILTER_NONE>(logits, logits_stride, generated, log_probas, B, kp, h, k, K, trie,
+                                                   out_generated, out_log_probas, out_parent, bad, ex, st);
   }
-  RQB_LAUNCH_CHECK();
-  return RQB_OK;
 }
 
 extern "C" int rqb200_sid_trie_beam_topk(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas,
@@ -1078,6 +1154,18 @@ extern "C" int rqb200_sid_trie_beam_topk_excluding(const float* logits, int64_t 
   if (rc != RQB_OK) return rc;
   return sid_beam_topk(logits, logits_stride, generated, log_probas, B, kp, h, k, C, K, prefix_workspace, out_generated,
                        out_log_probas, out_parent, bad, ex, stream);
+}
+
+extern "C" int rqb200_sid_trie_beam_topk_including(const float* logits, int64_t logits_stride, const int64_t* generated,
+                                                   const float* log_probas, int B, int kp, int h, int k, int C, int K,
+                                                   const void* prefix_workspace, int64_t* out_generated, float* out_log_probas,
+                                                   int64_t* out_parent, int* bad, const int* in_pos, const int64_t* in_keys,
+                                                   const int* in_count, int in_M, int in_H, void* stream) {
+  SidExcl in;
+  const int rc = sid_excl_of(in_pos, in_keys, in_count, in_M, in_H, h + 1, "sid_trie_beam_topk_including", in, true);
+  if (rc != RQB_OK) return rc;
+  return sid_beam_topk(logits, logits_stride, generated, log_probas, B, kp, h, k, C, K, prefix_workspace, out_generated,
+                       out_log_probas, out_parent, bad, in, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -1298,10 +1386,13 @@ extern "C" int rqb200_sid_items_lookup(const void* workspace, const int64_t* ids
 // One CTA per history b: each beam that is finite (log_probas null, or above -inf) and whose tuple is in the corpus resolves to
 // tuple u; a beam whose tuple an earlier beam carries counts 0 items, every other resolved beam its tuple's row count; an
 // exclusive block scan of the k counts places each beam's rows, in beam order, and output slot o takes the row of the beam
-// whose range holds it (a binary search in the scanned offsets).  No result depends on the order of atomics.
+// whose range holds it (a binary search in the scanned offsets).  No result depends on the order of atomics.  With an exclusion a
+// beam skips its tuple's excluded rows; with an allow-list its tuple's rows are the eligible positions in [start[u], start[u + 1])
+// (two binary searches), and its d-th item is the d-th of them.
 #define SID_ITEMS_THREADS 256
 #define SID_ITEMS_PER_THREAD (SID_ITEMS_MAX_K / SID_ITEMS_THREADS)
 
+template <bool INCLUDE>                                     // with an allow-list (else no filter or an exclusion, as ex says)
 __global__ void __launch_bounds__(SID_ITEMS_THREADS) sid_items_retrieve_kernel(
     const unsigned char* __restrict__ ws, const int64_t* __restrict__ generated, const float* __restrict__ log_probas, int k, int C,
     int n, int64_t* __restrict__ out_items, int* __restrict__ out_beam, int* __restrict__ out_count, SidExcl ex) {
@@ -1309,12 +1400,13 @@ __global__ void __launch_bounds__(SID_ITEMS_THREADS) sid_items_retrieve_kernel(
   __shared__ typename Scan::TempStorage scan_tmp;
   __shared__ int s_u[SID_ITEMS_MAX_K];
   __shared__ int s_off[SID_ITEMS_MAX_K + 1];
+  __shared__ int s_first[INCLUDE ? SID_ITEMS_MAX_K : 1];   // INCLUDE: each beam's first eligible position's index in xp
   const SidItemsHeader h = *reinterpret_cast<const SidItemsHeader*>(ws);
   const int* row = reinterpret_cast<const int*>(ws + h.row);
   const int* start = reinterpret_cast<const int*>(ws + h.start);
   const int b = blockIdx.x;
-  const int* xp = ex.on() ? ex.pos_of(b) : nullptr;         // the history's excluded positions, ascending
-  const int nx = ex.on() ? ex.npos(b) : 0;
+  const int* xp = INCLUDE || ex.on() ? ex.pos_of(b) : nullptr;   // the history's excluded (INCLUDE: eligible) positions, ascending
+  const int nx = INCLUDE || ex.on() ? ex.npos(b) : 0;
   for (int j = threadIdx.x; j < k; j += SID_ITEMS_THREADS) {
     const int64_t bj = (int64_t)b * k + j;
     const bool live = log_probas == nullptr || log_probas[bj] > -INFINITY;   // NaN is not above -inf either
@@ -1332,7 +1424,12 @@ __global__ void __launch_bounds__(SID_ITEMS_THREADS) sid_items_retrieve_kernel(
       for (int q = 0; q < j && !seen; ++q) seen = s_u[q] == u;
       if (!seen) {
         const int s = __ldg(start + u), e = __ldg(start + u + 1);
-        cnt[i] = e - s - (xp ? sid_excluded_in(xp, nx, s, e) : 0);
+        if (INCLUDE) {
+          s_first[j] = sid_lower_bound(xp, nx, s);
+          cnt[i] = sid_lower_bound(xp, nx, e) - s_first[j];
+        } else {
+          cnt[i] = e - s - (xp ? sid_excluded_in(xp, nx, s, e) : 0);
+        }
       }
     }
   }
@@ -1357,8 +1454,13 @@ __global__ void __launch_bounds__(SID_ITEMS_THREADS) sid_items_retrieve_kernel(
         else hi = mid;
       }
       beam = lo;
-      const int s = __ldg(start + s_u[lo]), d = o - s_off[lo];
-      item = __ldg(row + (xp ? sid_nth_kept(xp, nx, s, d) : s + d));
+      const int d = o - s_off[lo];
+      if (INCLUDE) {
+        item = __ldg(row + xp[s_first[lo] + d]);
+      } else {
+        const int s = __ldg(start + s_u[lo]);
+        item = __ldg(row + (xp ? sid_nth_kept(xp, nx, s, d) : s + d));
+      }
     }
     out_items[(int64_t)b * n + o] = item;
     out_beam[(int64_t)b * n + o] = beam;
@@ -1375,7 +1477,8 @@ static int sid_items_retrieve(const void* workspace, const int64_t* generated, c
   }
   if (B == 0) return RQB_OK;
   RQB_CHECK_ARG(workspace && generated && out_items && out_beam && out_count, "sid_items_retrieve: null pointer");
-  sid_items_retrieve_kernel<<<B, SID_ITEMS_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+  auto kernel = sid_filter_mode(ex) == SID_FILTER_INCLUDE ? sid_items_retrieve_kernel<true> : sid_items_retrieve_kernel<false>;
+  kernel<<<B, SID_ITEMS_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const unsigned char*>(workspace), generated, log_probas, k, C, n, out_items, out_beam, out_count, ex);
   RQB_LAUNCH_CHECK();
   return RQB_OK;
@@ -1396,6 +1499,16 @@ extern "C" int rqb200_sid_items_retrieve_excluding(const void* workspace, const 
   return sid_items_retrieve(workspace, generated, log_probas, B, k, C, n, out_items, out_beam, out_count, ex, stream);
 }
 
+extern "C" int rqb200_sid_items_retrieve_including(const void* workspace, const int64_t* generated, const float* log_probas, int B,
+                                                   int k, int C, int n, int64_t* out_items, int* out_beam, int* out_count,
+                                                   const int* in_pos, const int64_t* in_keys, const int* in_count, int in_M,
+                                                   int in_H, void* stream) {
+  SidExcl in;
+  const int rc = sid_excl_of(in_pos, in_keys, in_count, in_M, in_H, 0, "sid_items_retrieve_including", in, true);
+  if (rc != RQB_OK) return rc;
+  return sid_items_retrieve(workspace, generated, log_probas, B, k, C, n, out_items, out_beam, out_count, in, stream);
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 // Per-history exclusion sets (csrc/sid_excl.cuh for the layout): "do not return these items" for the search kernels above, the
 // item retrieval and the exact ranking's selection.  One CTA per history over its M entries (items, -1 pads): each item maps to
@@ -1405,13 +1518,18 @@ extern "C" int rqb200_sid_items_retrieve_excluding(const void* workspace, const 
 // start[lo] .. start[hi] with [lo, hi) the leaves whose keys (leaf_key, the packed tuples of the table's U leaves, ascending)
 // begin with p: two binary searches.  The first position of each run flags p as blocked when the run covers all those rows;
 // a block scan per level numbers the blocked prefixes.  Plain stores to distinct addresses; the cost depends on M and H only.
+//
+// Per-history allow-lists ("return only these items") come from the same body (INCLUDE): the positions are sorted and
+// de-duplicated alike, those found in an exclusion's sorted positions (ex, one binary search each) are dropped as well, and the
+// first position of each run flags its l-prefix as valid, so each level's keys are the distinct l-prefixes of the eligible
+// positions, ascending because the positions are.
 #define SID_EXCL_THREADS 512
 
-template <int IPT>
-__global__ void __launch_bounds__(SID_EXCL_THREADS) sid_exclusion_kernel(
+template <int IPT, bool INCLUDE>
+__global__ void __launch_bounds__(SID_EXCL_THREADS) sid_filter_kernel(
     const int64_t* __restrict__ items, int M, int64_t N, const int* __restrict__ inv, const int* __restrict__ start,
     const long long* __restrict__ leaf_key, int U, int H, int K, int* __restrict__ pos, long long* __restrict__ blocked,
-    int* __restrict__ count) {
+    int* __restrict__ count, SidExcl ex) {
   using Sort = cub::BlockRadixSort<unsigned int, SID_EXCL_THREADS, IPT>;
   using Scan = cub::BlockScan<int, SID_EXCL_THREADS>;
   __shared__ union {
@@ -1452,6 +1570,11 @@ __global__ void __launch_bounds__(SID_EXCL_THREADS) sid_exclusion_kernel(
   for (int j = 0; j < IPT; ++j) {
     const unsigned int prev = j > 0 ? key[j - 1] : tid > 0 ? s_last[tid - 1] : none;
     flag[j] = key[j] != none && key[j] != prev ? 1 : 0;
+    if (INCLUDE && flag[j] && ex.on()) {                    // an excluded position is not eligible
+      const int* xp = ex.pos_of(b);
+      const int nx = ex.npos(b), at = sid_lower_bound(xp, nx, (int)key[j]);
+      if (at < nx && xp[at] == (int)key[j]) flag[j] = 0;
+    }
   }
   Scan(tmp.scan).InclusiveSum(flag, idx, total);
   __syncthreads();
@@ -1490,10 +1613,14 @@ __global__ void __launch_bounds__(SID_EXCL_THREADS) sid_exclusion_kernel(
       p[j] = i < total ? lk[j] / div : -1;
       flag[j] = 0;
       const long long before = j > 0 ? lk[j - 1] : prev_key;
-      if (i < total && (before < 0 || before / div != p[j])) {   // the first excluded position under prefix p[j]
-        const int lo = sid_lower_bound(leaf_key, U, p[j] * div), hi = sid_lower_bound(leaf_key, U, (p[j] + 1) * div);
-        const int s = __ldg(start + lo), e = __ldg(start + hi);
-        flag[j] = sid_lower_bound(s_pos, total, e) - i == e - s ? 1 : 0;
+      if (i < total && (before < 0 || before / div != p[j])) {   // the first position under prefix p[j]
+        if (INCLUDE) {
+          flag[j] = 1;
+        } else {
+          const int lo = sid_lower_bound(leaf_key, U, p[j] * div), hi = sid_lower_bound(leaf_key, U, (p[j] + 1) * div);
+          const int s = __ldg(start + lo), e = __ldg(start + hi);
+          flag[j] = sid_lower_bound(s_pos, total, e) - i == e - s ? 1 : 0;
+        }
       }
     }
     int nb;
@@ -1513,34 +1640,51 @@ __global__ void __launch_bounds__(SID_EXCL_THREADS) sid_exclusion_kernel(
   }
 }
 
-extern "C" int rqb200_sid_exclusion_build(const int64_t* items, int B, int M, int64_t N, const int* inv, const int* start,
-                                          const int64_t* leaf_key, int U, int H, int K, int* pos, int64_t* blocked, int* count,
-                                          void* stream) {
+static int sid_filter_build(const int64_t* items, int B, int M, int64_t N, const int* inv, const int* start, const int64_t* leaf_key,
+                            int U, int H, int K, int* pos, int64_t* keys, int* count, const SidExcl& ex, bool include,
+                            const char* what, void* stream) {
   RQB_CHECK_ARG(B >= 0 && M > 0 && N >= 0 && N < 0x7fffffffll && U >= 0 && U <= N && H > 0 && K > 0,
-                "sid_exclusion_build: bad argument (B = %d, M = %d, N = %lld, U = %d, H = %d, K = %d)", B, M, (long long)N, U, H, K);
+                "%s: bad argument (B = %d, M = %d, N = %lld, U = %d, H = %d, K = %d)", what, B, M, (long long)N, U, H, K);
   int bits = 1;
   while (bits < 31 && (1 << bits) < K) ++bits;              // bits(K - 1), at least 1
   if (M > SID_EXCL_MAX_M || H > RQB_MAX_LEVELS || H * bits > 62) {
-    rqb_set_error("sid_exclusion_build: need M <= %d, H <= %d and H * bits(K - 1) <= 62 (M = %d, H = %d, K = %d)", SID_EXCL_MAX_M,
+    rqb_set_error("%s: need M <= %d, H <= %d and H * bits(K - 1) <= 62 (M = %d, H = %d, K = %d)", what, SID_EXCL_MAX_M,
                   RQB_MAX_LEVELS, M, H, K);
     return RQB_ERR_UNSUPPORTED;
   }
   if (B == 0) return RQB_OK;
-  RQB_CHECK_ARG(items && start && (inv || N == 0) && (leaf_key || U == 0) && pos && blocked && count,
-                "sid_exclusion_build: null pointer");
+  RQB_CHECK_ARG(items && start && (inv || N == 0) && (leaf_key || U == 0) && pos && keys && count, "%s: null pointer", what);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const long long* lk = reinterpret_cast<const long long*>(leaf_key);
-  long long* bl = reinterpret_cast<long long*>(blocked);
-  if (M <= SID_EXCL_THREADS)
-    sid_exclusion_kernel<1><<<B, SID_EXCL_THREADS, 0, st>>>(items, M, N, inv, start, lk, U, H, K, pos, bl, count);
-  else if (M <= 2 * SID_EXCL_THREADS)
-    sid_exclusion_kernel<2><<<B, SID_EXCL_THREADS, 0, st>>>(items, M, N, inv, start, lk, U, H, K, pos, bl, count);
-  else if (M <= 4 * SID_EXCL_THREADS)
-    sid_exclusion_kernel<4><<<B, SID_EXCL_THREADS, 0, st>>>(items, M, N, inv, start, lk, U, H, K, pos, bl, count);
-  else
-    sid_exclusion_kernel<8><<<B, SID_EXCL_THREADS, 0, st>>>(items, M, N, inv, start, lk, U, H, K, pos, bl, count);
+  long long* kk = reinterpret_cast<long long*>(keys);
+  auto kernel = include ? (M <= SID_EXCL_THREADS       ? sid_filter_kernel<1, true>
+                           : M <= 2 * SID_EXCL_THREADS ? sid_filter_kernel<2, true>
+                           : M <= 4 * SID_EXCL_THREADS ? sid_filter_kernel<4, true>
+                                                       : sid_filter_kernel<8, true>)
+                        : (M <= SID_EXCL_THREADS       ? sid_filter_kernel<1, false>
+                           : M <= 2 * SID_EXCL_THREADS ? sid_filter_kernel<2, false>
+                           : M <= 4 * SID_EXCL_THREADS ? sid_filter_kernel<4, false>
+                                                       : sid_filter_kernel<8, false>);
+  kernel<<<B, SID_EXCL_THREADS, 0, st>>>(items, M, N, inv, start, lk, U, H, K, pos, kk, count, ex);
   RQB_LAUNCH_CHECK();
   return RQB_OK;
+}
+
+extern "C" int rqb200_sid_exclusion_build(const int64_t* items, int B, int M, int64_t N, const int* inv, const int* start,
+                                          const int64_t* leaf_key, int U, int H, int K, int* pos, int64_t* blocked, int* count,
+                                          void* stream) {
+  return sid_filter_build(items, B, M, N, inv, start, leaf_key, U, H, K, pos, blocked, count, SidExcl{}, false,
+                          "sid_exclusion_build", stream);
+}
+
+extern "C" int rqb200_sid_inclusion_build(const int64_t* items, int B, int M, int64_t N, const int* inv, const int* start,
+                                          const int64_t* leaf_key, int U, int H, int K, int* pos, int64_t* keys, int* count,
+                                          const int* ex_pos, const int64_t* ex_blocked, const int* ex_count, int ex_M, int ex_H,
+                                          void* stream) {
+  SidExcl ex;
+  const int rc = sid_excl_of(ex_pos, ex_blocked, ex_count, ex_M, ex_H, 0, "sid_inclusion_build", ex);
+  if (rc != RQB_OK) return rc;
+  return sid_filter_build(items, B, M, N, inv, start, leaf_key, U, H, K, pos, keys, count, ex, true, "sid_inclusion_build", stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

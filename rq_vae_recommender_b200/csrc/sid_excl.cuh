@@ -1,29 +1,36 @@
-// Per-history exclusion sets of the semantic-id search, item retrieval and exact ranking (rqb200_sid_exclusion_build in
-// csrc/sid.cu writes them; the search kernels of sid.cu and t5rank_select_kernel of t5rank.cu read them).
+// Per-history item filters of the semantic-id search, item retrieval and exact ranking: exclusion sets
+// (rqb200_sid_exclusion_build in csrc/sid.cu writes them; the search kernels of sid.cu and t5rank_select_kernel of t5rank.cu read
+// them) and allow-lists (rqb200_sid_inclusion_build; the search and retrieval kernels of sid.cu read them).  Both have one layout.
 //
 // For history b of B, with M entries per history and H levels:
-//   pos[b][0 .. n)          the distinct excluded items as positions in the item table's sorted row array, ascending
-//                           (n = count[b][0]); the table's order is lexicographic, so the excluded items under one trie prefix are
-//                           one run of them;
-//   blocked[b][l - 1][0 .. m)  the packed keys (level 0 most significant, K-ary) of the l-prefixes under which every retrievable
-//                           item is excluded, ascending (m = count[b][l], l = 1..H);
+//   pos[b][0 .. n)          exclusion: the distinct excluded items, inclusion: the eligible items (allowed, retrievable and not
+//                           excluded), as positions in the item table's sorted row array, ascending (n = count[b][0]); the table's
+//                           order is lexicographic, so the items under one trie prefix are one run of them;
+//   keys[b][l - 1][0 .. m)  the packed keys (level 0 most significant, K-ary) of l-prefixes, ascending (m = count[b][l],
+//                           l = 1..H): exclusion, the blocked prefixes (every retrievable item under them is excluded); inclusion,
+//                           the valid prefixes (at least one eligible item under them);
 //   count[b][H + 1]         the entries outside [-1, N) (counted, otherwise ignored).
-// A null count pointer means "no exclusion": every consumer then runs its code without it.
+// A null count pointer means "no filter": every consumer then runs its code without it.  A consumer takes one filter: an
+// inclusion has the exclusion folded in.
 #pragma once
 #include <cstdint>
 
 #define SID_EXCL_MAX_M 4096
 
+// the compile-time filter mode of a consumer kernel
+enum SidFilterMode { SID_FILTER_NONE = 0, SID_FILTER_EXCLUDE = 1, SID_FILTER_INCLUDE = 2 };
+
 struct SidExcl {
   const int* pos;
-  const long long* blocked;
+  const long long* keys;
   const int* count;
   int M, H;
+  bool include;                                             // an allow-list (rqb200_sid_inclusion_build), else an exclusion set
   __device__ __forceinline__ bool on() const { return count != nullptr; }
   __device__ __forceinline__ const int* pos_of(int64_t b) const { return pos + b * M; }
   __device__ __forceinline__ int npos(int64_t b) const { return __ldg(count + b * (H + 2)); }
-  __device__ __forceinline__ const long long* blocked_of(int64_t b, int l) const { return blocked + (b * H + (l - 1)) * M; }
-  __device__ __forceinline__ int nblocked(int64_t b, int l) const { return __ldg(count + b * (H + 2) + l); }
+  __device__ __forceinline__ const long long* keys_of(int64_t b, int l) const { return keys + (b * H + (l - 1)) * M; }
+  __device__ __forceinline__ int nkeys(int64_t b, int l) const { return __ldg(count + b * (H + 2) + l); }
 };
 
 // first i in [0, n) with a[i] >= v (n when none)

@@ -19,7 +19,9 @@ The search (``generate``, ``generate_items``):
     resolves ``sem_ids_fut`` to the true next item;
   * ``exclude_items`` / ``exclude_history`` leave given items (or each history's own) out of the search, the retrieval and
     ``rank_items``: a prefix under which every retrievable item is excluded is invalid for that history, like one the corpus
-    lacks (``ops.sid_exclusion_build``).
+    lacks (``ops.sid_exclusion_build``);
+  * ``include_items`` restricts the search and the retrieval to each history's allowed items: a prefix without an eligible item
+    (allowed, retrievable, not excluded) under it is invalid for that history (``ops.sid_inclusion_build``).
 
 The fused T5 passes, each HF's maths as GEMMs between this project's kernels, described once by ``_T5Weights``:
   * ``FusedT5Decode`` (``generate(decoder="fused")``) and ``FusedT5Rank`` (exact scoring) run the incremental decoder of
@@ -901,10 +903,12 @@ class EncoderDecoderRetrievalModel(nn.Module):
 
     def _sample_and_select(self, index: ops.SidPrefixIndex, probas: Tensor, generated: Optional[Tensor],
                            log_probas: Optional[Tensor], k: int, n_cands: int, reject: Tensor,
-                           exclude: Optional[ops.SidExclusion] = None):
+                           exclude: Optional[ops.SidExclusion] = None, include: Optional[ops.SidInclusion] = None):
         """One level of the search after the softmax: n_cands samples per beam, prefix check, scores, the k best beams."""
-        excl = {} if exclude is None else {"exclude": exclude}
-        return index.sample_select(probas, draw_exponential(probas), generated, log_probas, k, n_cands, reject=reject, **excl)
+        filt = {} if exclude is None else {"exclude": exclude}
+        if include is not None:
+            filt["include"] = include
+        return index.sample_select(probas, draw_exponential(probas), generated, log_probas, k, n_cands, reject=reject, **filt)
 
     def _check_search_limits(self, search: str, k: int, n_cands: int) -> None:
         K = self.num_embeddings_per_hierarchy
@@ -936,10 +940,10 @@ class EncoderDecoderRetrievalModel(nn.Module):
         return torch.cat([self._check_exclude_items(t, B) for t in parts], dim=1)
 
     @staticmethod
-    def _check_exclude_items(items: Tensor, B: int) -> Tensor:
+    def _check_exclude_items(items: Tensor, B: int, name: str = "exclude_items") -> Tensor:
         ops._need_cuda(items)
         if items.dim() != 2 or items.shape[0] != B or items.dtype.is_floating_point or items.dtype == torch.bool:
-            raise ValueError(f"exclude_items must be an integer [B = {B}, M] tensor of corpus rows, got {items.dtype} "
+            raise ValueError(f"{name} must be an integer [B = {B}, M] tensor of corpus rows, got {items.dtype} "
                              f"{tuple(items.shape)}")
         return items.long()
 
@@ -951,14 +955,37 @@ class EncoderDecoderRetrievalModel(nn.Module):
         _, leaf_key, _ = self._rank_levels(device)
         return ops.sid_exclusion_build(items.to(device), self._item_table(device), leaf_key)
 
+    def _filters(self, exclude_items: Optional[Tensor], include_items: Optional[Tensor], B: int,
+                 device: torch.device) -> list:
+        """The item filters of one call, in build order: the exclusion (``_exclusion``), then the allow-list built on it
+        (``ops.sid_inclusion_build``); empty without either.  The consumers take the last one (``_filter_kwargs``)."""
+        exclusion = self._exclusion(exclude_items, B, device)
+        filters = [] if exclusion is None else [exclusion]
+        if include_items is not None:
+            items = self._check_exclude_items(include_items, B, "include_items")
+            _, leaf_key, _ = self._rank_levels(device)
+            filters.append(ops.sid_inclusion_build(items.to(device), self._item_table(device), leaf_key, exclude=exclusion))
+        return filters
+
     @staticmethod
-    def _read_counters(counters: Tensor, exclusion: Optional[ops.SidExclusion], what: str) -> List[int]:
-        """The one host read at the end of a call: its counters, after which the excluded ids outside [-1, N) raise."""
-        if exclusion is None:
+    def _filter_kwargs(filters: list) -> dict:
+        """The filter argument of the search and retrieval calls: an allow-list holds the exclusion folded in."""
+        if not filters:
+            return {}
+        return {"include" if isinstance(filters[-1], ops.SidInclusion) else "exclude": filters[-1]}
+
+    @staticmethod
+    def _read_counters(counters: Tensor, filters: list, what: str) -> List[int]:
+        """The one host read at the end of a call: its counters, after which the excluded or allowed ids outside [-1, N) of
+        the call's filters (``_filters``) raise."""
+        if not filters:
             return counters.tolist()
-        *values, n_ids = torch.cat([counters.int(), exclusion.count[:, -1].sum(dtype=torch.int32).view(1)]).tolist()
-        if n_ids:
-            raise ValueError(f"{what}: {n_ids} excluded item id(s) outside [-1, N) where N is the number of corpus rows")
+        values = torch.cat([counters.int()] + [f.count[:, -1].sum(dtype=torch.int32).view(1) for f in filters]).tolist()
+        values, n_ids = values[:counters.numel()], values[counters.numel():]
+        for f, n in zip(filters, n_ids):
+            if n:
+                kind = "allowed" if isinstance(f, ops.SidInclusion) else "excluded"
+                raise ValueError(f"{what}: {n} {kind} item id(s) outside [-1, N) where N is the number of corpus rows")
         return values
 
     @torch.no_grad()
@@ -973,7 +1000,8 @@ class EncoderDecoderRetrievalModel(nn.Module):
 
     @torch.no_grad()
     def generate(self, attention_mask, input_ids, user_id=None, search: Optional[str] = None, decoder: Optional[str] = None,
-                 encoder: Optional[str] = None, encoder_attention: Optional[str] = None, exclude_items: Optional[Tensor] = None):
+                 encoder: Optional[str] = None, encoder_attention: Optional[str] = None, exclude_items: Optional[Tensor] = None,
+                 include_items: Optional[Tensor] = None):
         """Top-k semantic ids by beam search restricted to id prefixes of the corpus.  ``search`` (default: the module's
         ``DEFAULT_SEARCH``, read at call time):
           "sample"  per level, n_cands = min(64, K) tokens sampled without replacement per beam, scored by cumulative
@@ -993,12 +1021,15 @@ class EncoderDecoderRetrievalModel(nn.Module):
         ``exclude_items`` (integer [B, M], corpus rows, -1 pads, M <= ``ops.EXCLUDE_MAX_ITEMS``): no beam leads only to excluded
         items of its history; an extension under which every retrievable item is excluded is invalid, like a prefix the corpus
         lacks.  It adds one launch and no host read; ids outside [-1, N) raise ``ValueError`` after the search.
+        ``include_items`` (integer [B, M], corpus rows, -1 pads, M <= ``ops.INCLUDE_MAX_ITEMS``): every beam leads to an eligible
+        item of its history -- one in its allow-list, retrievable and not excluded; an extension without one under it is
+        invalid, like a prefix the corpus lacks.  None means no restriction; a row without an eligible item gets -inf fillers
+        only.  It adds one launch and no host read; ids outside [-1, N) raise ``ValueError`` after the search.
         Returns generated [B, top_k, num_hierarchies] and log_probas [B, top_k]."""
         return self._generate(attention_mask, input_ids, user_id, search, decoder, encoder, encoder_attention,
-                              self._exclusion(exclude_items, attention_mask.shape[0], attention_mask.device))
+                              self._filters(exclude_items, include_items, attention_mask.shape[0], attention_mask.device))
 
-    def _generate(self, attention_mask, input_ids, user_id, search, decoder, encoder, encoder_attention,
-                  exclusion: Optional[ops.SidExclusion]):
+    def _generate(self, attention_mask, input_ids, user_id, search, decoder, encoder, encoder_attention, filters: list):
         decoder = _choice(decoder, DEFAULT_DECODER, DECODERS, "generate", "decoder")
         if decoder == "fused" and self.training:
             raise ValueError("generate: decoder=\"fused\" runs the decoder in eval mode only; call model.eval() first (in "
@@ -1025,7 +1056,7 @@ class EncoderDecoderRetrievalModel(nn.Module):
             rep_enc, rep_mask = enc_out.repeat_interleave(k, dim=0), enc_mask.repeat_interleave(k, dim=0)
             past_kv = EncoderDecoderCache(DynamicCache(), DynamicCache())
         reject = torch.zeros(1 if beam else 2, dtype=torch.int32, device=enc_out.device)
-        excl = {} if exclusion is None else {"exclude": exclusion}
+        filt = self._filter_kwargs(filters)
         generated, log_probas, parent_global = None, None, None
         for h in range(self.num_hierarchies):
             first = generated is None
@@ -1037,10 +1068,10 @@ class EncoderDecoderRetrievalModel(nn.Module):
                     attention_mask_for_encoder=enc_mask if first else rep_mask, use_cache=True, past_key_values=past_kv)
                 logits = self.decoder_mlp[h](dec_out[:, -1, :])
             if beam:
-                generated, log_probas, parent_global = index.beam_topk(logits, generated, log_probas, k, bad=reject, **excl)
+                generated, log_probas, parent_global = index.beam_topk(logits, generated, log_probas, k, bad=reject, **filt)
             else:
                 generated, log_probas, parent_global = self._sample_and_select(index, F.softmax(logits, dim=-1), generated,
-                                                                               log_probas, k, n_cands, reject, **excl)
+                                                                               log_probas, k, n_cands, reject, **filt)
             if fused is not None:
                 continue
             if first:
@@ -1048,12 +1079,12 @@ class EncoderDecoderRetrievalModel(nn.Module):
             else:
                 past_kv.reorder_cache(parent_global)
         if beam:
-            n_bad = int(reject[0]) if exclusion is None else self._read_counters(reject, exclusion, "generate")[0]
+            n_bad = int(reject[0]) if not filters else self._read_counters(reject, filters, "generate")[0]
             if n_bad:
                 raise RuntimeError(f"generate: {n_bad} beam row(s) of the decoder head's logits hold a NaN or +inf or are all "
                                    "-inf; the beam search cannot rank them")
             return generated, log_probas
-        bad, zero_sum = self._read_counters(reject, exclusion, "generate")
+        bad, zero_sum = self._read_counters(reject, filters, "generate")
         if bad:
             raise RuntimeError(_MULTINOMIAL_ERRORS[0])
         if zero_sum:
@@ -1064,38 +1095,45 @@ class EncoderDecoderRetrievalModel(nn.Module):
         return self._exclusion(self._excluded_items(batch, exclude_items, exclude_history), batch.sem_ids.shape[0],
                                batch.sem_ids.device)
 
+    def _batch_filters(self, batch: TokenizedSeqBatch, exclude_items, exclude_history, include_items) -> list:
+        return self._filters(self._excluded_items(batch, exclude_items, exclude_history), include_items, batch.sem_ids.shape[0],
+                             batch.sem_ids.device)
+
     def _generate_batch(self, batch: TokenizedSeqBatch, search, decoder, encoder, encoder_attention,
-                        exclusion: Optional[ops.SidExclusion]) -> GenerationOutput:
+                        filters: list) -> GenerationOutput:
         H = self.num_hierarchies
         generated, log_probas = self._generate(_strip_dedup_col(batch.seq_mask.long(), H + 1, H),
                                                _strip_dedup_col(batch.sem_ids, H + 1, H), batch.user_ids, search, decoder,
-                                               encoder, encoder_attention, exclusion)
+                                               encoder, encoder_attention, filters)
         return GenerationOutput(sem_ids=generated, log_probas=log_probas)
 
     @torch.no_grad()
     def generate_next_sem_id(self, batch: TokenizedSeqBatch, top_k: bool = True, temperature: int = 1,
                              search: Optional[str] = None, decoder: Optional[str] = None,
                              encoder: Optional[str] = None, encoder_attention: Optional[str] = None,
-                             exclude_items: Optional[Tensor] = None, exclude_history: Optional[bool] = None) -> GenerationOutput:
-        """``generate`` on the batch's histories.  ``exclude_items`` as in ``generate``; ``exclude_history`` (default
-        ``DEFAULT_EXCLUDE_HISTORY``, read at call time) also excludes each history's own items (``history_items``)."""
+                             exclude_items: Optional[Tensor] = None, exclude_history: Optional[bool] = None,
+                             include_items: Optional[Tensor] = None) -> GenerationOutput:
+        """``generate`` on the batch's histories.  ``exclude_items`` and ``include_items`` as in ``generate``;
+        ``exclude_history`` (default ``DEFAULT_EXCLUDE_HISTORY``, read at call time) also excludes each history's own items
+        (``history_items``)."""
         return self._generate_batch(batch, search, decoder, encoder, encoder_attention,
-                                    self._batch_exclusion(batch, exclude_items, exclude_history))
+                                    self._batch_filters(batch, exclude_items, exclude_history, include_items))
 
     @torch.no_grad()
     def generate_items(self, batch: TokenizedSeqBatch, n: Optional[int] = None, search: Optional[str] = None,
                        decoder: Optional[str] = None, encoder: Optional[str] = None,
                        encoder_attention: Optional[str] = None, exclude_items: Optional[Tensor] = None,
-                       exclude_history: Optional[bool] = None) -> ItemGenerationOutput:
+                       exclude_history: Optional[bool] = None, include_items: Optional[Tensor] = None) -> ItemGenerationOutput:
         """The top corpus items for each history: ``generate_next_sem_id``'s beams, unchanged, then one launch that takes the
         items of every finite beam whose ids are in the corpus, beam by beam in descending score order, each beam's items by
         dedup rank, no item twice, at most n (default top_k_for_generation) per history.  ``exclude_items`` /
-        ``exclude_history`` as in ``generate_next_sem_id``: the search and the retrieval both leave the excluded items out."""
-        exclusion = self._batch_exclusion(batch, exclude_items, exclude_history)
-        out = self._generate_batch(batch, search, decoder, encoder, encoder_attention, exclusion)
+        ``exclude_history`` as in ``generate_next_sem_id``: the search and the retrieval both leave the excluded items out.
+        ``include_items`` as in ``generate``: the search and the retrieval both return only each history's eligible items."""
+        filters = self._batch_filters(batch, exclude_items, exclude_history, include_items)
+        out = self._generate_batch(batch, search, decoder, encoder, encoder_attention, filters)
         table = self._item_table(out.sem_ids.device)
-        excl = {} if exclusion is None else {"exclude": exclusion}
-        items, beams, count = table.retrieve(out.sem_ids, out.log_probas, self.top_k_for_generation if n is None else n, **excl)
+        items, beams, count = table.retrieve(out.sem_ids, out.log_probas, self.top_k_for_generation if n is None else n,
+                                             **self._filter_kwargs(filters))
         return ItemGenerationOutput(item_ids=items, beams=beams, count=count, sem_ids=out.sem_ids, log_probas=out.log_probas)
 
     @torch.no_grad()
@@ -1234,7 +1272,7 @@ class EncoderDecoderRetrievalModel(nn.Module):
         if exclusion is None:
             self._raise_bad(bad, "rank_items")
         else:
-            n_bad, = self._read_counters(bad, exclusion, "rank_items")
+            n_bad, = self._read_counters(bad, [exclusion], "rank_items")
             if n_bad:
                 raise _non_finite_error("rank_items", n_bad)
         return ItemRankingOutput(item_ids=items, scores=item_scores, target_rank=rank, num_items=n_items)

@@ -626,7 +626,8 @@ class SidPrefixIndex:
 
     def sample_select(self, probas: torch.Tensor, noise: torch.Tensor, generated: Optional[torch.Tensor],
                       log_probas: Optional[torch.Tensor], k: int, nc: int, want_samples: bool = False,
-                      reject: Optional[torch.Tensor] = None, exclude: Optional["SidExclusion"] = None):
+                      reject: Optional[torch.Tensor] = None, exclude: Optional["SidExclusion"] = None,
+                      include: Optional["SidInclusion"] = None):
         """The sampling step fused with ``beam_select`` (rqb200_sid_trie_sample_select), one launch.  probas / noise [B * kp, K]
         (kp = 1 on the first level; noise = the Exp(1) draw torch.multinomial makes, ``torch.empty_like(probas).exponential_(1)``),
         generated [B, kp, h] or None, log_probas [B, kp] or None -> (generated [B, k, h + 1], log_probas [B, k],
@@ -634,7 +635,9 @@ class SidPrefixIndex:
         ``torch.multinomial(probas, nc)``'s under the same generator state.  ``reject``, an int32 [2] device tensor, is ADDED the
         number of rows torch.multinomial would reject: [0] with a NaN, +-inf or negative entry, [1] otherwise all zero.
         ``exclude`` (``sid_exclusion_build``, one set per history): extensions to a prefix blocked for the history are invalid,
-        exactly like prefixes the corpus lacks; the samples do not change."""
+        exactly like prefixes the corpus lacks; the samples do not change.  ``include`` (``sid_inclusion_build``, one allow-list
+        per history, any exclusion folded in; not with ``exclude``): extensions to a prefix without an eligible item of the
+        history are invalid alike."""
         _need_cuda(probas, noise, reject)
         if generated is None:
             B, kp, h = probas.shape[0], 1, 0
@@ -657,31 +660,27 @@ class SidPrefixIndex:
         out_parent = torch.empty((B * k,), dtype=torch.int64, device=dev)
         samples = torch.empty((B * kp, nc), dtype=torch.int64, device=dev) if want_samples else None
         samp_log_p = torch.empty((B * kp, nc), dtype=torch.float32, device=dev) if want_samples else None
+        name, filt = _filter_entry("sid_trie_sample_select", exclude, include, B, h + 1, "sample_select")
         with torch.cuda.device(dev):
-            if exclude is None:
-                _lib.check(_lib.load().rqb200_sid_trie_sample_select(
-                    _p(probas), probas.stride(0), _p(noise), noise.stride(0), _p(generated), _p(log_probas), B, kp, nc, h, k,
-                    self.C, self.K, _p(self.ws), _p(out_g), _p(out_p), _p(out_parent), _p(samples), _p(samp_log_p), _p(reject),
-                    _stream()), "sid_trie_sample_select")
-            else:
-                _lib.check(_lib.load().rqb200_sid_trie_sample_select_excluding(
-                    _p(probas), probas.stride(0), _p(noise), noise.stride(0), _p(generated), _p(log_probas), B, kp, nc, h, k,
-                    self.C, self.K, _p(self.ws), _p(out_g), _p(out_p), _p(out_parent), _p(samples), _p(samp_log_p), _p(reject),
-                    *exclude.args(B, h + 1, "sample_select"), _stream()), "sid_trie_sample_select_excluding")
+            _lib.check(getattr(_lib.load(), "rqb200_" + name)(
+                _p(probas), probas.stride(0), _p(noise), noise.stride(0), _p(generated), _p(log_probas), B, kp, nc, h, k, self.C,
+                self.K, _p(self.ws), _p(out_g), _p(out_p), _p(out_parent), _p(samples), _p(samp_log_p), _p(reject), *filt,
+                _stream()), name)
         _count(1)
         if want_samples:
             return out_g, out_p, out_parent, samples, samp_log_p
         return out_g, out_p, out_parent
 
     def beam_topk(self, logits: torch.Tensor, generated: Optional[torch.Tensor], log_probas: Optional[torch.Tensor], k: int,
-                  bad: Optional[torch.Tensor] = None, exclude: Optional["SidExclusion"] = None):
+                  bad: Optional[torch.Tensor] = None, exclude: Optional["SidExclusion"] = None,
+                  include: Optional["SidInclusion"] = None):
         """One level of the exhaustive constrained beam search from the head's logits (rqb200_sid_trie_beam_topk), one launch.
         logits [B * kp, K] (kp = 1 on the first level), generated [B, kp, h] or None, log_probas [B, kp] or None ->
         (generated [B, k, h + 1], log_probas [B, k], parent_global [B * k]): of all kp * K extensions of each history, scored
         log_softmax(logits)[code] + the parent's log-probability (-inf when the extended prefix is not in the corpus), the k
         best in descending order, equal scores by ascending beam * K + code.  Deterministic.  ``bad``, an int32 device tensor,
-        is ADDED the number of beam rows whose logits hold a NaN or +inf or are all -inf.  ``exclude`` as in ``sample_select``:
-        extensions to a prefix blocked for the history score -inf."""
+        is ADDED the number of beam rows whose logits hold a NaN or +inf or are all -inf.  ``exclude`` / ``include`` as in
+        ``sample_select``: extensions to a prefix blocked for the history, or without an eligible item of it, score -inf."""
         _need_cuda(logits, bad)
         if generated is None:
             B, kp, h = logits.shape[0], 1, 0
@@ -702,16 +701,11 @@ class SidPrefixIndex:
         out_g = torch.empty((B, k, h + 1), dtype=torch.int64, device=dev)
         out_p = torch.empty((B, k), dtype=torch.float32, device=dev)
         out_parent = torch.empty((B * k,), dtype=torch.int64, device=dev)
+        name, filt = _filter_entry("sid_trie_beam_topk", exclude, include, B, h + 1, "beam_topk")
         with torch.cuda.device(dev):
-            if exclude is None:
-                _lib.check(_lib.load().rqb200_sid_trie_beam_topk(_p(logits), logits.stride(0), _p(generated), _p(log_probas), B,
-                                                                 kp, h, k, self.C, self.K, _p(self.ws), _p(out_g), _p(out_p),
-                                                                 _p(out_parent), _p(bad), _stream()), "sid_trie_beam_topk")
-            else:
-                _lib.check(_lib.load().rqb200_sid_trie_beam_topk_excluding(
-                    _p(logits), logits.stride(0), _p(generated), _p(log_probas), B, kp, h, k, self.C, self.K, _p(self.ws), _p(out_g),
-                    _p(out_p), _p(out_parent), _p(bad), *exclude.args(B, h + 1, "beam_topk"), _stream()),
-                    "sid_trie_beam_topk_excluding")
+            _lib.check(getattr(_lib.load(), "rqb200_" + name)(
+                _p(logits), logits.stride(0), _p(generated), _p(log_probas), B, kp, h, k, self.C, self.K, _p(self.ws), _p(out_g),
+                _p(out_p), _p(out_parent), _p(bad), *filt, _stream()), name)
         _count(1)
         return out_g, out_p, out_parent
 
@@ -805,11 +799,12 @@ class SidItemTable:
         return out.reshape(lead)
 
     def retrieve(self, generated: torch.Tensor, log_probas: Optional[torch.Tensor], n: int,
-                 exclude: Optional["SidExclusion"] = None):
+                 exclude: Optional["SidExclusion"] = None, include: Optional["SidInclusion"] = None):
         """generated [B, k, C], log_probas [B, k] or None -> (items [B, n] int64, beam [B, n] int32, count [B] int32): per
         history, in beam order, the items of every beam whose log-probability is above -inf and whose tuple is in the corpus,
         each beam's in dedup-rank order, no item twice, cut off at n; -1 pads items and beam.  k <= 1024, n <= 4096.
-        ``exclude`` (``sid_exclusion_build`` on this table): the history's excluded items are skipped."""
+        ``exclude`` (``sid_exclusion_build`` on this table): the history's excluded items are skipped.  ``include``
+        (``sid_inclusion_build`` on this table; not with ``exclude``): only the history's eligible items are taken."""
         _need_cuda(generated, log_probas)
         B, k, C = generated.shape
         if C != self.C:
@@ -822,14 +817,10 @@ class SidItemTable:
         items = torch.empty((B, n), dtype=torch.int64, device=dev)
         beam = torch.empty((B, n), dtype=torch.int32, device=dev)
         count = torch.empty((B,), dtype=torch.int32, device=dev)
+        name, filt = _filter_entry("sid_items_retrieve", exclude, include, B, 0, "retrieve")
         with torch.cuda.device(dev):
-            if exclude is None:
-                _lib.check(_lib.load().rqb200_sid_items_retrieve(_p(self.ws), _p(generated), _p(log_probas), B, k, C, n,
-                                                                 _p(items), _p(beam), _p(count), _stream()), "sid_items_retrieve")
-            else:
-                _lib.check(_lib.load().rqb200_sid_items_retrieve_excluding(
-                    _p(self.ws), _p(generated), _p(log_probas), B, k, C, n, _p(items), _p(beam), _p(count),
-                    *exclude.args(B, 0, "retrieve"), _stream()), "sid_items_retrieve_excluding")
+            _lib.check(getattr(_lib.load(), "rqb200_" + name)(_p(self.ws), _p(generated), _p(log_probas), B, k, C, n, _p(items),
+                                                              _p(beam), _p(count), *filt, _stream()), name)
         _count(1)
         return items, beam, count
 
@@ -856,6 +847,33 @@ class SidItemTable:
 
 #: most entries per history an exclusion set takes (sid_exclusion_build sorts them in shared memory)
 EXCLUDE_MAX_ITEMS = 4096
+#: most entries per history an allow-list takes (sid_inclusion_build, the same kernel)
+INCLUDE_MAX_ITEMS = EXCLUDE_MAX_ITEMS
+
+
+def _filter_args(f, kind: str, B: int, levels: int, what: str):
+    """The filter arguments (pos, keys, count, M, H) of the *_excluding / *_including entry points, for B histories and a level
+    up to ``levels``."""
+    _need_cuda(f.pos)
+    H = f[1].shape[1]
+    if f.pos.shape[0] != B:
+        raise ValueError(f"{what}: the {kind} holds {f.pos.shape[0]} histories, the call {B}")
+    if levels > H:
+        raise ValueError(f"{what}: level {levels} is deeper than the {kind}'s {H} levels")
+    return _p(f.pos), _p(f[1]), _p(f.count), f.pos.shape[1], H
+
+
+def _filter_entry(entry: str, exclude, include, B: int, levels: int, what: str):
+    """(entry point name, filter arguments) of a consumer call: ``entry`` without a filter, ``entry``_excluding /
+    ``entry``_including with one.  An inclusion has the exclusion folded in, so a call takes at most one."""
+    if exclude is not None and include is not None:
+        raise ValueError(f"{what}: pass exclude or include, not both (sid_inclusion_build folds an exclusion into the "
+                         "inclusion)")
+    if include is not None:
+        return entry + "_including", include.args(B, levels, what)
+    if exclude is not None:
+        return entry + "_excluding", exclude.args(B, levels, what)
+    return entry, ()
 
 
 class SidExclusion(NamedTuple):
@@ -870,13 +888,62 @@ class SidExclusion(NamedTuple):
 
     def args(self, B: int, levels: int, what: str):
         """The exclusion arguments of the *_excluding entry points, for B histories and a level up to ``levels``."""
-        _need_cuda(self.pos)
-        H = self.blocked.shape[1]
-        if self.pos.shape[0] != B:
-            raise ValueError(f"{what}: the exclusion holds {self.pos.shape[0]} histories, the call {B}")
-        if levels > H:
-            raise ValueError(f"{what}: level {levels} is deeper than the exclusion's {H} levels")
-        return _p(self.pos), _p(self.blocked), _p(self.count), self.pos.shape[1], H
+        return _filter_args(self, "exclusion", B, levels, what)
+
+
+class SidInclusion(NamedTuple):
+    """Each history's allow-list (``sid_inclusion_build``), in ``SidExclusion``'s layout.  pos int32 [B, M]: the distinct
+    eligible items (allowed, retrievable, not excluded) as positions in the item table's row array, ascending; keys int64
+    [B, H, M]: per level l = 1..H the keys (``_tuple_key`` of the prefix) of the valid l-prefixes -- those with an eligible item
+    under them -- ascending; count int32 [B, H + 2]: [0] the positions, [l] the valid l-prefixes, [H + 1] the allowed ids
+    outside [-1, N).  Entries past a count are -1."""
+    pos: torch.Tensor
+    keys: torch.Tensor
+    count: torch.Tensor
+
+    def args(self, B: int, levels: int, what: str):
+        """The inclusion arguments of the *_including entry points, for B histories and a level up to ``levels``."""
+        return _filter_args(self, "inclusion", B, levels, what)
+
+
+def _filter_items(items: torch.Tensor, kind: str, limit: int):
+    """items as a contiguous int64 [B, max(M, 1)] (an empty row is one -1), after the checks of a filter build."""
+    if items.dim() != 2 or items.dtype.is_floating_point or items.dtype.is_complex or items.dtype == torch.bool:
+        raise ValueError(f"{kind}: items must be an integer [B, M] tensor, got {items.dtype} {tuple(items.shape)}")
+    B, M = items.shape
+    if M > limit:
+        raise ValueError(f"{kind}: M = {M} items per history exceeds {limit}")
+    if M == 0:
+        return torch.full((B, 1), -1, dtype=torch.int64, device=items.device)
+    return items.to(torch.int64).contiguous()
+
+
+def sid_inclusion_build(items: torch.Tensor, table: SidItemTable, leaf_key: torch.Tensor,
+                        exclude: Optional[SidExclusion] = None) -> SidInclusion:
+    """Each history's allow-list (rqb200_sid_inclusion_build), one launch, no host read.  items integer [B, M] (corpus rows,
+    -1 pads, repeats allowed, M <= ``INCLUDE_MAX_ITEMS``), table and leaf_key as in ``sid_exclusion_build``, exclude an
+    exclusion of the same B histories on the same table, folded in: an item is eligible when it is allowed, retrievable and
+    not excluded.  Ids outside [-1, N) are counted in count[:, H + 1]."""
+    _need_cuda(items, leaf_key)
+    items = _filter_items(items, "inclusion", INCLUDE_MAX_ITEMS)
+    B, M = items.shape
+    dev = items.device
+    leaf_key = leaf_key.to(torch.int64).contiguous()
+    H, U = table.C, leaf_key.shape[0]
+    if exclude is not None and exclude.blocked.shape[1] != H:
+        raise ValueError(f"inclusion: the exclusion has {exclude.blocked.shape[1]} levels, the item table {H}")
+    filt = (None, None, None, 0, 0) if exclude is None else exclude.args(B, H, "inclusion")
+    _, start = table.arrays()
+    pos = torch.empty((B, M), dtype=torch.int32, device=dev)
+    keys = torch.empty((B, H, M), dtype=torch.int64, device=dev)
+    count = torch.empty((B, H + 2), dtype=torch.int32, device=dev)
+    inv = table.positions()
+    with torch.cuda.device(dev):
+        _lib.check(_lib.load().rqb200_sid_inclusion_build(_p(items), B, M, table.N, _p(inv), _p(start), _p(leaf_key), U, H,
+                                                          table.K, _p(pos), _p(keys), _p(count), *filt, _stream()),
+                   "sid_inclusion_build")
+    _count(1)
+    return SidInclusion(pos, keys, count)
 
 
 def sid_exclusion_build(items: torch.Tensor, table: SidItemTable, leaf_key: torch.Tensor) -> SidExclusion:
@@ -885,16 +952,9 @@ def sid_exclusion_build(items: torch.Tensor, table: SidItemTable, leaf_key: torc
     leaf_key int64 [U]: the table's U distinct retrievable tuples packed K-ary (level 0 most significant), ascending.  Rows
     that are not retrievable are ignored; ids outside [-1, N) are counted in count[:, H + 1]."""
     _need_cuda(items, leaf_key)
-    if items.dim() != 2 or items.dtype.is_floating_point or items.dtype.is_complex or items.dtype == torch.bool:
-        raise ValueError(f"exclusion: items must be an integer [B, M] tensor, got {items.dtype} {tuple(items.shape)}")
+    items = _filter_items(items, "exclusion", EXCLUDE_MAX_ITEMS)
     B, M = items.shape
-    if M > EXCLUDE_MAX_ITEMS:
-        raise ValueError(f"exclusion: M = {M} items per history exceeds {EXCLUDE_MAX_ITEMS}")
     dev = items.device
-    items = items.to(torch.int64)
-    if M == 0:
-        items, M = torch.full((B, 1), -1, dtype=torch.int64, device=dev), 1
-    items = items.contiguous()
     leaf_key = leaf_key.to(torch.int64).contiguous()
     H, U = table.C, leaf_key.shape[0]
     _, start = table.arrays()
