@@ -69,14 +69,16 @@ def cross_attention_train(q, kv, offs, key_mask, kpos, T, keep=None, p=0.0):
     return torch.cat(outs)
 
 
-def decode_train(model, fut_ids, rows, offs, key_mask, kpos, masks=None, p=0.0):
+def decode_train(model, fut_ids, rows, offs, key_mask, kpos, masks=None, p=0.0, relu=None, pre=None):
     """The decoder pass: [B, T, d] (the final norm's output after its dropout), differentiable in every parameter and in rows.
-    masks: HF-order keep masks (``random_masks``) or None for no dropout."""
+    masks: HF-order keep masks (``random_masks``) or None for no dropout.  relu: one [B, T + 1, d_ff] mask per feed-forward, in
+    call order, nonzero where its relu passes (the first T positions are read): the pass computes ``pre * mask`` in place of
+    ``F.relu(pre)``; None uses F.relu.  pre: a list each feed-forward's pre-activation [B * T, d_ff] is appended to, or None."""
     dec = model.t5_decoder
     T, K, eps = model.num_hierarchies, model.num_embeddings_per_hierarchy, dec.config.layer_norm_epsilon
     B, d = fut_ids.shape[0], model.bos_token.shape[1]
     table = model.item_sid_embedding_table.weight
-    idx = fut_ids[:, :T - 1].long() + torch.arange(T - 1) * K
+    idx = fut_ids[:, :T - 1].long() + torch.arange(T - 1, device=fut_ids.device) * K
     x = torch.cat([model.bos_token.expand(B, 1, d), table[idx]], dim=1).reshape(B * T, d)
     queue = list(masks) if masks is not None else None
 
@@ -87,6 +89,15 @@ def decode_train(model, fut_ids, rows, offs, key_mask, kpos, masks=None, p=0.0):
 
     def keep():
         return queue.pop(0) if queue is not None else None
+
+    relus = list(relu) if relu is not None else None
+
+    def act(t):                                             # a feed-forward relu: F.relu, or the first T positions of the next mask
+        if pre is not None:
+            pre.append(t.detach())
+        if relus is None:
+            return F.relu(t)
+        return t * relus.pop(0)[:, :T].reshape(B * T, -1).to(t.dtype)
 
     blocks = [blk.layer for blk in dec.block]
     rel = E.rel_bias(blocks[0][0].SelfAttention.compute_bias(T, T)[0])
@@ -100,20 +111,19 @@ def decode_train(model, fut_ids, rows, offs, key_mask, kpos, masks=None, p=0.0):
         kv = F.linear(rows, torch.cat([ca.k.weight, ca.v.weight]))
         x = x + drop(F.linear(cross_attention_train(q, kv, offs, key_mask, kpos, T, keep(), p), ca.o.weight))
         ff = lay[2].DenseReluDense
-        h = drop(F.relu(F.linear(t5_norm(x, lay[2].layer_norm.weight, eps), ff.wi.weight)))
+        h = drop(act(F.linear(t5_norm(x, lay[2].layer_norm.weight, eps), ff.wi.weight)))
         x = x + drop(F.linear(h, ff.wo.weight))
     out = drop(t5_norm(x, dec.final_layer_norm.weight, eps))
-    if queue is not None:
-        assert not queue
+    assert not queue and not relus
     return out.reshape(B, T, d)
 
 
 def padded_layout(enc_out, enc_mask):
     """HF's encoder output as decoder key rows: (rows [B * S, d], offsets, key_mask [B * S], kpos [B * S])."""
     B, S, d = enc_out.shape
-    offs = torch.arange(0, (B + 1) * S, S, dtype=torch.int32)
+    offs = torch.arange(0, (B + 1) * S, S, dtype=torch.int32, device=enc_out.device)
     key_mask = torch.where(enc_mask == 0, NEG, 0.0).to(enc_out.dtype).reshape(B * S)
-    return enc_out.reshape(B * S, d), offs, key_mask, torch.arange(S).repeat(B)
+    return enc_out.reshape(B * S, d), offs, key_mask, torch.arange(S, device=enc_out.device).repeat(B)
 
 
 def packed_layout(enc_out, attention_mask, H, sep, user):

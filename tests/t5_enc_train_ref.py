@@ -71,9 +71,11 @@ def t5_norm(x, weight, eps):
     return weight * (x * torch.rsqrt(x.pow(2).mean(-1, keepdim=True) + eps))
 
 
-def encode_train(model, attention_mask, input_ids, user_id=None, masks=None, p=0.0):
+def encode_train(model, attention_mask, input_ids, user_id=None, masks=None, p=0.0, relu=None, pre=None):
     """The packed training pass: (enc_out [B, S, d] with dropped rows 0, enc_mask [B, S]), differentiable in every parameter.
-    masks: HF-order keep masks (``random_masks``) or None for no dropout."""
+    masks: HF-order keep masks (``random_masks``) or None for no dropout.  relu: one [B, S, d_ff] mask per feed-forward, in call
+    order, nonzero where its relu passes: the pass computes ``pre * mask`` in place of ``F.relu(pre)``, so it can follow another
+    pass's relu decisions; None uses F.relu.  pre: a list each feed-forward's pre-activation [N, d_ff] is appended to, or None."""
     enc = model.encoder.encoder
     H, eps = model.num_hierarchies, enc.config.layer_norm_epsilon
     sep = model.sep_token is not None
@@ -101,6 +103,15 @@ def encode_train(model, attention_mask, input_ids, user_id=None, masks=None, p=0
         m = queue.pop(0)
         return t * m.reshape(B * S, -1)[rows].to(t.dtype) / (1 - p)
 
+    relus = list(relu) if relu is not None else None
+
+    def act(t):                                            # a feed-forward relu: F.relu, or the kept rows of the next relu mask
+        if pre is not None:
+            pre.append(t.detach())
+        if relus is None:
+            return F.relu(t)
+        return t * relus.pop(0).reshape(B * S, -1)[rows].to(t.dtype)
+
     blocks = [blk.layer for blk in enc.block]
     rel = E.rel_bias(blocks[0][0].SelfAttention.compute_bias(S, S)[0])
     x = drop(x)
@@ -111,9 +122,8 @@ def encode_train(model, attention_mask, input_ids, user_id=None, masks=None, p=0
         a = attention_train(qkv, src, offs, key_mask, rel, S, keep, p)
         x = x + drop(F.linear(a, att.o.weight))
         ff = lay[1].DenseReluDense
-        h = drop(F.relu(F.linear(t5_norm(x, lay[1].layer_norm.weight, eps), ff.wi.weight)))
+        h = drop(act(F.linear(t5_norm(x, lay[1].layer_norm.weight, eps), ff.wi.weight)))
         x = x + drop(F.linear(h, ff.wo.weight))
     out = drop(t5_norm(x, enc.final_layer_norm.weight, eps))
-    if queue is not None:
-        assert not queue
+    assert not queue and not relus
     return E.scatter(out, slot), enc_mask

@@ -167,7 +167,10 @@ def assert_matches_hf(m, batch, fn=None):
     print(f"largest gradient difference, relative to the parameter's largest entry: {errs[worst]:.2e} ({worst})")
     # The two passes round differently in fp32, so a feed-forward pre-activation within rounding of 0 can pass relu on one side
     # only, and that moves a whole row of wi's gradient.  At 64 x 81 positions an H100 measured up to 3.5e-3 of the largest
-    # entry, in block 0's wi; through torch.compile at 32 histories, 1.9e-6.  The loss agrees within 1e-5.
+    # entry, in block 0's wi; through torch.compile at 32 histories, 1.9e-6.  The loss agrees within 1e-5.  Measured against
+    # the float64 statement at 64 full 20-item histories (tests/test_gpu_train_statement.py, an H100 at 700 W), the fused pass
+    # flips 3 relus, each within 1.6 fp32 units of its layer's largest pre-activation; they move encoder block 3's wi gradient
+    # by 1.2e-3 of its largest entry, and with its relu decisions followed the statement is within 2e-6.
     for name, err in errs.items():
         assert err <= 1e-2, (name, err)
 
