@@ -37,6 +37,11 @@ extern "C" int rqb200_tokenize_tc_ring_stages(int D, int K, int L) {
 }
 
 // ------------------------------------------------------------------------------------------------ prepare
+// cbptr[l]: level l of the state's fp32 codebook copy
+__global__ void tc_prep_ptrs_kernel(const float** cbptr, const float* cbf, size_t level_elems, int L) {
+  if (threadIdx.x < L) cbptr[threadIdx.x] = cbf + threadIdx.x * level_elems;
+}
+
 // hcc[l][k] = cc/2 from a float64 sum (the filter's table); amax and c2max of the level
 __global__ void tc_prep_stats_kernel(const float* const* cbs, int D, int K, TcHeader* hdr, float* hcc) {
   const int l = blockIdx.y;
@@ -187,12 +192,12 @@ extern "C" int rqb200_tokenize_tc_prepare(const float* const* codebooks, int D, 
   RQB_CUDA(cudaMemsetAsync(hdr, 0, sizeof(TcHeader), st));
   // fp32 copy for the exact re-rank: 256-byte aligned rows whatever the caller's tensors look like, and the prepared state
   // no longer references caller memory after this call returns (stream order); every prepare kernel reads the copy
-  const float* cbfp[RQB_MAX_LEVELS] = {};
-  for (int l = 0; l < L; ++l) {
+  for (int l = 0; l < L; ++l)
     RQB_CUDA(cudaMemcpyAsync(cbf + (size_t)l * K * D, codebooks[l], sizeof(float) * K * D, cudaMemcpyDeviceToDevice, st));
-    cbfp[l] = cbf + (size_t)l * K * D;
-  }
-  RQB_CUDA(cudaMemcpyAsync(cbptr, cbfp, sizeof(float*) * L, cudaMemcpyHostToDevice, st));   // pageable source: staged before the call returns
+  // the level pointer table is written on the device: a copy from pageable host memory may wait for the stream's earlier work,
+  // and the prepare must never block the host
+  tc_prep_ptrs_kernel<<<1, 32, 0, st>>>(cbptr, cbf, (size_t)K * D, L);
+  RQB_LAUNCH_CHECK();
   tc_prep_stats_kernel<<<dim3(K / 8, L), 256, 0, st>>>(cbptr, D, K, hdr, hcc);
   RQB_LAUNCH_CHECK();
   tc_prep_cc_kernel<<<dim3(K / 8, L), 256, 0, st>>>(cbptr, D, K, cc);

@@ -52,8 +52,10 @@ class MLP(nn.Module):
         key = tuple((w.data_ptr(), w._version) for w in weights)
         cache = getattr(self, "_wimg_cache", None)
         if cache is None or cache[0] != key:
-            cache = (key, [ops.to_bf16_image(w.detach()) for w in weights])
+            images = [ops.to_bf16_image(w.detach()) for w in weights]
+            cache = (key, images, ops.StreamBuild(*images))
             object.__setattr__(self, "_wimg_cache", cache)
+        cache[2].ready()
         return cache[1]
 
     def forward(self, x: Tensor) -> Tensor:

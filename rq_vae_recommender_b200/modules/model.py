@@ -886,7 +886,7 @@ class EncoderDecoderRetrievalModel(nn.Module):
         if self._prefix_index_cache is None or self._prefix_index_cache[0] != key:
             index = ops.SidPrefixIndex(cb.to(device), self.num_embeddings_per_hierarchy)
             self._prefix_index_cache = (key, index)
-        return self._prefix_index_cache[1]
+        return self._prefix_index_cache[1].ready()
 
     def _item_table(self, device: torch.device) -> ops.SidItemTable:
         """The corpus item table (row n of codebooks is item n), cached on the same key as the prefix index."""
@@ -895,7 +895,7 @@ class EncoderDecoderRetrievalModel(nn.Module):
         if self._item_table_cache is None or self._item_table_cache[0] != key:
             table = ops.SidItemTable(cb[:, :self.num_hierarchies].to(device), self.num_embeddings_per_hierarchy)
             self._item_table_cache = (key, table)
-        return self._item_table_cache[1]
+        return self._item_table_cache[1].ready()
 
     def _check_valid_prefix(self, prefix: Tensor, batch_size: int = 100000) -> Tensor:
         """bool [P]: some corpus row starts with prefix[p] (batch_size is accepted for the reference's signature)."""
@@ -1162,8 +1162,9 @@ class EncoderDecoderRetrievalModel(nn.Module):
             key = levels.code[1].long()                                           # _tuple_key of each leaf, along its path
             for l in range(2, H + 1):
                 key = key[levels.parent[l].long()] * K + levels.code[l]
-            state = index._rank_state = (H, levels, key, int(host[-1]))
-        return state[1:]
+            state = index._rank_state = (H, levels, key, int(host[-1]), ops.StreamBuild(key))
+        state[4].ready()
+        return state[1:4]
 
     def _leaf_of(self, tuples: Tensor, leaf_key: Tensor) -> Tensor:
         """int64 [B]: the leaf (item-table tuple) of each row of tuples [B, H], -1 when it holds an id outside [0, K) or is not in

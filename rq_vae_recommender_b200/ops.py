@@ -66,6 +66,36 @@ def _ptr_array(ts: Sequence[Optional[torch.Tensor]]):
     return arr
 
 
+class StreamBuild:
+    """The build of cached device state (prepared codebooks, operand images, tries, item tables): kernels enqueued on the stream
+    current at construction, with no host sync.  Later calls reuse the state from whatever stream is current then, so each reuse
+    goes through ``ready()``: it orders the current stream after the build (an event wait, no host sync; nothing on the build
+    stream or on a stream that already waited) and marks the state's tensors as used on that stream, so that freeing them -- a
+    cache evicting the entry -- also waits for the work that stream has queued.  Inside a CUDA-graph capture it does nothing:
+    capture starts from a synchronised device, and the caches rebuild their entries in a captured stream anyway."""
+
+    __slots__ = ("tensors", "event", "streams")
+
+    def __init__(self, *tensors: torch.Tensor):
+        stream = torch.cuda.current_stream(tensors[0].device)
+        self.tensors = tensors
+        self.event = torch.cuda.Event()
+        self.event.record(stream)
+        self.streams = {stream.cuda_stream}
+
+    def ready(self) -> None:
+        stream = torch.cuda.current_stream(self.tensors[0].device)
+        # streams are told apart by their handle: torch's pooled streams live as long as the process, but a destroyed external
+        # stream whose handle the driver hands out again would be taken for the one that waited; and the capture check is that of
+        # the current device's stream, the one the library's launches go to
+        if stream.cuda_stream in self.streams or torch.cuda.is_current_stream_capturing():
+            return
+        stream.wait_event(self.event)
+        for t in self.tensors:
+            t.record_stream(stream)
+        self.streams.add(stream.cuda_stream)
+
+
 def _check_codebooks(cbs: Sequence[torch.Tensor], D: int) -> List[torch.Tensor]:
     out = [_f32c(c) for c in cbs]
     K = out[0].shape[0]
@@ -254,11 +284,12 @@ def split_operand_cached(t: torch.Tensor, transposed: bool = False) -> SplitOper
     key = (t.data_ptr(), t._version, tuple(t.shape), tuple(t.stride()), t.device.index, bool(transposed))
     hit = _SPLIT_CACHE.get(key)
     if hit is not None and hit[0]() is t:
+        hit[2].ready()
         return hit[1]
     if len(_SPLIT_CACHE) >= _SPLIT_CACHE_MAX:
         _SPLIT_CACHE.pop(next(iter(_SPLIT_CACHE)))
     op = SplitOperand(t, transposed)
-    _SPLIT_CACHE[key] = (weakref.ref(t), op)
+    _SPLIT_CACHE[key] = (weakref.ref(t), op, StreamBuild(op.buf))
     return op
 
 
@@ -429,12 +460,12 @@ class GumbelQuantizeFunction(torch.autograd.Function):
         B, D = x.shape
         K = cb.shape[0]
         dev = x.device
-        st = _stream()
         cc = torch.empty(K, dtype=torch.float32, device=dev)
         ids = torch.empty(B, dtype=torch.int64, device=dev)
         loss = torch.empty(B, dtype=torch.float32, device=dev)
         w = torch.empty((B, K), dtype=torch.float32, device=dev)
         with torch.cuda.device(dev):
+            st = _stream()
             _lib.check(lib.rqb200_row_sqnorm(_p(cb), K, D, _p(cc), st), "row_sqnorm")
             dist = linear_nt(x, cb)                                              # x @ C^T
             _lib.check(lib.rqb200_dist_finish(_p(dist), _p(x), x.stride(0), _p(cc), B, D, K, _p(ids), st), "dist")
@@ -455,7 +486,6 @@ class GumbelQuantizeFunction(torch.autograd.Function):
         B, D = x.shape
         K = cb.shape[0]
         dev = x.device
-        st = _stream()
         g_emb = None if g_emb is None else (g_emb if g_emb.dtype == torch.float32 else g_emb.float())
         g_loss = None if g_loss is None else (g_loss if g_loss.dtype == torch.float32 else g_loss.float())
         gl_s = g_loss.stride(0) if g_loss is not None else 0
@@ -463,6 +493,7 @@ class GumbelQuantizeFunction(torch.autograd.Function):
         rowsum = torch.empty(B, dtype=torch.float32, device=dev)
         colsum = torch.empty(K, dtype=torch.float32, device=dev)
         with torch.cuda.device(dev):
+            st = _stream()
             _lib.check(lib.rqb200_gumbel_bwd_ge(_p(g_emb), g_emb.stride(0) if g_emb is not None else 0,
                                                 g_emb.stride(1) if g_emb is not None else 0, _p(g_loss), gl_s,
                                                 _p(x), x.stride(0), _p(emb), _p(gE), B, D, st), "bwd_ge")
@@ -580,6 +611,12 @@ class SidPrefixIndex:
             _lib.check(lib.rqb200_sid_trie_build(_p(ids), self.N, self.C, self.K, _p(self.ws), nbytes, _p(scratch), scratch_bytes,
                                                  _stream()), "sid_trie_build")
         _count(1)                                             # one build call (the trie's sort and scans are several kernels)
+        self._build = StreamBuild(self.ws)
+
+    def ready(self) -> "SidPrefixIndex":
+        """This index, with the current stream ordered after its build and that of its cached levels (``StreamBuild``)."""
+        self._build.ready()
+        return self
 
     def check(self, prefix: torch.Tensor) -> torch.Tensor:
         """bool [P]: does some corpus row start with prefix[p] ([P, l], l <= C)."""
@@ -720,11 +757,14 @@ class SidPrefixIndex:
     def levels(self, n: Sequence[int]) -> "SidTrieLevels":
         """The level arrays of levels 1..C as device tensors, given the node counts n = ``counts()`` read on the host; one launch
         per level.  Built once and cached on the index."""
+        self.ready()
         if getattr(self, "_levels", None) is None:
             n = [int(v) for v in n]
             if len(n) != self.C + 1 or n[0] != 1:
                 raise ValueError(f"levels: n must be the {self.C + 1} node counts of counts(), got {n}")
-            code, parent, child = [None], [None], [torch.tensor([0, n[1]], dtype=torch.int32, device=self.device)]
+            child0 = torch.zeros(2, dtype=torch.int32, device=self.device)
+            child0[1:].fill_(n[1])                            # not torch.tensor(..., device=): that copy synchronises the stream
+            code, parent, child = [None], [None], [child0]
             lib = _lib.load()
             for l in range(1, self.C + 1):
                 c = torch.empty(n[l], dtype=torch.int32, device=self.device)
@@ -739,6 +779,7 @@ class SidPrefixIndex:
                 parent.append(p)
                 child.append(ch)
             self._levels = SidTrieLevels(n, code, parent, child)
+            self._build = StreamBuild(self.ws, *(t for t in code + parent + child if t is not None))
         return self._levels
 
 
@@ -777,6 +818,12 @@ class SidItemTable:
             _lib.check(lib.rqb200_sid_items_build(_p(ids), self.N, self.C, self.K, _p(self.ws), nbytes, _stream()),
                        "sid_items_build")
         _count(1)                                             # one build call (the sort and the scan are several kernels)
+        self._build = StreamBuild(self.ws)
+
+    def ready(self) -> "SidItemTable":
+        """This table, with the current stream ordered after its build and that of its cached positions (``StreamBuild``)."""
+        self._build.ready()
+        return self
 
     def lookup(self, ids: torch.Tensor, with_dedup: bool = False) -> torch.Tensor:
         """int64 [...]: the item of each tuple ids[..., :C] -- its first item, or with ``with_dedup`` the item of dedup rank
@@ -827,6 +874,7 @@ class SidItemTable:
     def arrays(self):
         """(row int32 [N], start int32 [N + 1]): views of the table's workspace.  Tuple u's items are row[start[u] .. start[u + 1])
         in dedup order; only the first U + 1 entries of start are written (U: the distinct retrievable tuples)."""
+        self.ready()
         row_off, start_off = ctypes.c_size_t(), ctypes.c_size_t()
         _lib.check(_lib.load().rqb200_sid_items_offsets(self.N, self.C, self.K, ctypes.byref(row_off), ctypes.byref(start_off)),
                    "sid_items_offsets")
@@ -842,6 +890,8 @@ class SidItemTable:
             inv = torch.empty(self.N, dtype=torch.int32, device=self.device)
             inv[row.long()] = torch.arange(self.N, dtype=torch.int32, device=self.device)
             self._positions = inv
+            self._build = StreamBuild(self.ws, inv)
+        self.ready()
         return self._positions
 
 
@@ -1808,7 +1858,7 @@ class TcState:
         with torch.cuda.device(self.device):
             _lib.check(lib.rqb200_tokenize_tc_prepare(_ptr_array(cbs), self.D, self.K, self.L, _p(self.buf), nbytes,
                                                       _stream()), "tokenize_tc_prepare")
-        _count(6 + self.L * (self.L - 1) // 2)
+        _count(7 + self.L * (self.L - 1) // 2)
         global TC_PREPARES
         TC_PREPARES += 1
 
@@ -1863,11 +1913,12 @@ def tc_state_for(codebooks: Sequence[torch.Tensor]) -> TcState:
     key = _tc_cache_key(codebooks)
     hit = _TC_CACHE.get(key)
     if hit is not None and all(r() is c for r, c in zip(hit[0], codebooks)):
+        hit[2].ready()
         return hit[1]
     if len(_TC_CACHE) >= _TC_CACHE_MAX:
         _TC_CACHE.pop(next(iter(_TC_CACHE)))
     st = TcState(codebooks)
-    _TC_CACHE[key] = ([weakref.ref(c) for c in codebooks], st)
+    _TC_CACHE[key] = ([weakref.ref(c) for c in codebooks], st, StreamBuild(st.buf))
     return st
 
 

@@ -39,12 +39,21 @@ class CorpusTokenizer:
         if use_tc is None:
             use_tc = bool(ops.tc_padded_dim(self.D, self.K, self.L))
         self.use_tc = bool(use_tc)
-        self.state = ops.TcState(self.codebooks) if self.use_tc else None
+        self._state = ops.TcState(self.codebooks) if self.use_tc else None
+        self._state_build = ops.StreamBuild(self._state.buf) if self.use_tc else None
         self.encoder = encoder
         self.chunk_rows = chunk_rows
         self._copy_stream = None
         self._host_out = None
         self._ring = None
+
+    @property
+    def state(self) -> Optional[ops.TcState]:
+        """The prepared codebooks of the tensor-core tokeniser (None without it), with the current stream ordered after their
+        preparation (``ops.StreamBuild``)."""
+        if self._state_build is not None:
+            self._state_build.ready()
+        return self._state
 
     # ---- device resident rows
     @torch.no_grad()

@@ -227,3 +227,28 @@ def test_forward_traces_with_projected_and_normalised_codebooks(kw, mode_name):
     names = {str(n.target) for n in gm.graph.nodes if n.op == "call_function" and "rqb200" in str(n.target)}
     assert "rqb200.mlp_fwd.default" in names and "rqb200.count_unique_id_tuples.default" in names
     assert ("rqb200.gumbel_level_fwd.default" if mode_name == "GUMBEL_SOFTMAX" else "rqb200.rq_chain_fwd.default") in names
+
+
+def test_every_kernel_stream_is_taken_inside_its_device_block():
+    """ops._stream() is the current stream of the CURRENT device: taken before ``with torch.cuda.device(dev)`` it is another
+    device's stream for inputs off the current device, and the launch runs unordered with the caller's stream there."""
+    import ast
+    path = os.path.join(ROOT, "rq_vae_recommender_b200", "ops.py")
+    tree = ast.parse(open(path).read(), path)
+
+    def is_device_block(node):
+        return isinstance(node, ast.With) and any(
+            isinstance(it.context_expr, ast.Call) and ast.unparse(it.context_expr.func) == "torch.cuda.device"
+            for it in node.items)
+
+    outside, inside = [], []
+
+    def walk(node, in_device):
+        if isinstance(node, ast.Call) and isinstance(node.func, ast.Name) and node.func.id == "_stream":
+            (inside if in_device else outside).append(node.lineno)
+        for child in ast.iter_child_nodes(node):
+            walk(child, in_device or is_device_block(node))
+
+    walk(tree, False)
+    assert len(inside) > 50
+    assert outside == [], f"ops.py calls _stream() outside a torch.cuda.device block at lines {outside}"
