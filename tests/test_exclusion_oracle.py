@@ -122,3 +122,22 @@ def test_rank_select():
     assert (items[3] == -1).all() and np.isneginf(s[3]).all() and rank[3] == -1
     t_dedup[1] = 3
     assert X.rank_select(t, excls, scores, t_leaf, t_dedup, 7)[2][1] == 1     # row 3 follows row 2 once rows 0, 1 are gone
+
+
+@pytest.mark.parametrize("K,H,accepted", [(2048, 6, False), (256, 8, False), (1024, 6, True), (2048, 5, True)])
+def test_filter_entry_points_take_keys_of_at_most_62_bits(K, H, accepted):
+    """rqb200_sid_exclusion_build and rqb200_sid_inclusion_build refuse H * bits(K - 1) > 62 (66 and 64 bits here) before
+    reading any pointer, and take 60 and 55 bits (B = 0: nothing to launch)."""
+    from rq_vae_recommender_b200 import _lib
+    lib = _lib.load()
+    calls = {"sid_exclusion_build": lambda B: lib.rqb200_sid_exclusion_build(0, B, 4, 10, 0, 0, 0, 5, H, K, 0, 0, 0, 0),
+             "sid_inclusion_build": lambda B: lib.rqb200_sid_inclusion_build(0, B, 4, 10, 0, 0, 0, 5, H, K, 0, 0, 0, 0, 0, 0, 0,
+                                                                             0, 0)}
+    for name, call in calls.items():
+        if accepted:
+            assert call(0) == 0
+            assert call(1) == 1 and b"null pointer" in lib.rqb200_last_error()
+        else:
+            assert call(1) == 3
+            msg = lib.rqb200_last_error().decode()
+            assert msg.startswith(name) and "H * bits(K - 1) <= 62" in msg and f"H = {H}, K = {K}" in msg

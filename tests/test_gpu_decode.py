@@ -152,16 +152,19 @@ def both_decoders(m, mask, ids, users, search, seed=5):
     return out
 
 
-SHAPES = {"small": (lambda M, corpus: small_model(M, corpus, 256, 3), 11, 48, 20), "decoder_amazon": (amazon_model, 12, 64, 20)}
+# name: (model of a corpus, seed, histories, items per history, K); K = 300 leaves a partial last word in the child masks
+SHAPES = {"small": (lambda M, corpus: small_model(M, corpus, 256, 3), 11, 48, 20, 256),
+          "decoder_amazon": (amazon_model, 12, 64, 20, 256),
+          "small_k300": (lambda M, corpus: small_model(M, corpus, 300, 3), 13, 48, 20, 300)}
 
 
 @pytest.mark.parametrize("shape", list(SHAPES))
 @pytest.mark.parametrize("search", ["sample", "beam"])
 def test_generate_fused_equals_hf_at_highest(shape, search):
     from rq_vae_recommender_b200.modules import model as M
-    make, seed, B, items = SHAPES[shape]
+    make, seed, B, items, K = SHAPES[shape]
     rs = np.random.RandomState(seed)
-    K, H = 256, 3
+    H = 3
     m = make(M, realistic_corpus(rs, 3000, H, K))
     mask, ids, users = history(rs, B, items, H, K)
     with highest():

@@ -167,9 +167,9 @@ def encoder_runs(m, mask, ids, users, search, decoder, seed=5):
 @pytest.mark.parametrize("decoder", ["hf", "fused"])
 def test_generate_fused_encoder_equals_hf_at_highest(shape, search, decoder):
     from rq_vae_recommender_b200.modules import model as M
-    make, seed, B, items = SHAPES[shape]
+    make, seed, B, items, K = SHAPES[shape]
     rs = np.random.RandomState(seed)
-    K, H = 256, 3
+    H = 3
     m = make(M, realistic_corpus(rs, 3000, H, K))
     mask, ids, users = history(rs, B, items, H, K)
     mask[-3:, : 12 * H] = 0                                                         # some shorter histories too

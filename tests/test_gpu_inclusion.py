@@ -53,7 +53,7 @@ def built(corpus, K, items, ex_items=None):
 
 @pytest.mark.parametrize("excluding", [False, True])
 @pytest.mark.parametrize("K,H", [(256, 3), (2048, 3), (256, 5), (2048, 5)])
-@pytest.mark.parametrize("M", [1, 511, 512, 513, 4096])
+@pytest.mark.parametrize("M", [1, 511, 512, 513, 1024, 1025, 2048, 2049, 4096])
 def test_build_matches_oracle(M, K, H, excluding):
     rs = np.random.RandomState(M + K + H)
     B, N = 5, 3000

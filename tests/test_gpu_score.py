@@ -14,8 +14,8 @@ from test_score_ref import candidate_trie, candidates_with_edges, score_decompos
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize("C", [1, 7, 101, 4096])
-@pytest.mark.parametrize("K", [256, 2048])
+@pytest.mark.parametrize("C", [1, 7, 101, 512, 513, 1024, 1025, 2048, 2049, 4096])
+@pytest.mark.parametrize("K", [256, 300, 2048])
 @pytest.mark.parametrize("H", [3, 5])
 def test_trie_build_matches_host_statement(C, K, H):
     from rq_vae_recommender_b200 import ops
