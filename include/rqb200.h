@@ -280,6 +280,55 @@ int rqb200_sid_trie_beam_topk_including(const float* logits, int64_t logits_stri
                                         const int* in_pos, const int64_t* in_keys, const int* in_count, int in_M, int in_H,
                                         void* stream);
 
+/* sid_trie_beam_topk_wide : one level of the same exhaustive search for up to 1024 beams per history, on one thread-block
+ *                    cluster per history.  Arguments, scores, order, `bad` and results as sid_trie_beam_topk, bit for bit
+ *                    wherever both run.
+ *   cluster          CTAs per history: 1, 2, 4 or 8, or 0 to let the call choose from B, kp, K and the SM count.  A size whose
+ *                    shared memory cannot hold the level or of which no cluster can be resident is RQB_ERR_UNSUPPORTED when
+ *                    asked for, skipped when choosing.  No result depends on the size.
+ *   limits           K <= 2048, k <= 1024, k <= K, kp <= 1024, h < C <= 8; RQB_ERR_UNSUPPORTED otherwise.  B = 0 is a no-op.
+ * _excluding / _including take the filter arguments of sid_trie_beam_topk_excluding / _including after `cluster`. */
+int rqb200_sid_trie_beam_topk_wide(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas,
+                                   int B, int kp, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
+                                   float* out_log_probas, int64_t* out_parent, int* bad, int cluster, void* stream);
+int rqb200_sid_trie_beam_topk_wide_excluding(const float* logits, int64_t logits_stride, const int64_t* generated,
+                                             const float* log_probas, int B, int kp, int h, int k, int C, int K,
+                                             const void* prefix_workspace, int64_t* out_generated, float* out_log_probas,
+                                             int64_t* out_parent, int* bad, int cluster, const int* ex_pos, const int64_t* ex_blocked,
+                                             const int* ex_count, int ex_M, int ex_H, void* stream);
+int rqb200_sid_trie_beam_topk_wide_including(const float* logits, int64_t logits_stride, const int64_t* generated,
+                                             const float* log_probas, int B, int kp, int h, int k, int C, int K,
+                                             const void* prefix_workspace, int64_t* out_generated, float* out_log_probas,
+                                             int64_t* out_parent, int* bad, int cluster, const int* in_pos, const int64_t* in_keys,
+                                             const int* in_count, int in_M, int in_H, void* stream);
+/* sid_trie_sample_select_wide : one level of the sampled search for up to 1024 beams per history, on one thread-block cluster
+ *                    per history.  Arguments, draws, scores, order, `reject` and results as sid_trie_sample_select, bit for bit
+ *                    wherever both run; when k > kp * nc the slots past kp * nc repeat candidate 0 with -inf.
+ *   workspace        device scratch of sid_trie_sample_select_wide_workspace_bytes(B, kp, nc) bytes (every draw's token and key)
+ *   cluster          as sid_trie_beam_topk_wide.
+ *   limits           1 <= nc <= 64, nc <= K <= 2048, kp <= 1024, k <= 1024, h < C <= 8; RQB_ERR_UNSUPPORTED otherwise.
+ * _excluding / _including take the filter arguments of sid_trie_sample_select_excluding / _including after `cluster`. */
+size_t rqb200_sid_trie_sample_select_wide_workspace_bytes(int B, int kp, int nc);
+int rqb200_sid_trie_sample_select_wide(const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride,
+                                       const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k, int C,
+                                       int K, const void* prefix_workspace, int64_t* out_generated, float* out_log_probas,
+                                       int64_t* out_parent, int64_t* samples, float* samp_log_p, int* reject, void* workspace,
+                                       size_t workspace_bytes, int cluster, void* stream);
+int rqb200_sid_trie_sample_select_wide_excluding(const float* probas, int64_t probas_stride, const float* noise,
+                                                 int64_t noise_stride, const int64_t* generated, const float* log_probas, int B,
+                                                 int kp, int nc, int h, int k, int C, int K, const void* prefix_workspace,
+                                                 int64_t* out_generated, float* out_log_probas, int64_t* out_parent,
+                                                 int64_t* samples, float* samp_log_p, int* reject, void* workspace,
+                                                 size_t workspace_bytes, int cluster, const int* ex_pos, const int64_t* ex_blocked,
+                                                 const int* ex_count, int ex_M, int ex_H, void* stream);
+int rqb200_sid_trie_sample_select_wide_including(const float* probas, int64_t probas_stride, const float* noise,
+                                                 int64_t noise_stride, const int64_t* generated, const float* log_probas, int B,
+                                                 int kp, int nc, int h, int k, int C, int K, const void* prefix_workspace,
+                                                 int64_t* out_generated, float* out_log_probas, int64_t* out_parent,
+                                                 int64_t* samples, float* samp_log_p, int* reject, void* workspace,
+                                                 size_t workspace_bytes, int cluster, const int* in_pos, const int64_t* in_keys,
+                                                 const int* in_count, int in_M, int in_H, void* stream);
+
 /* The trie's level arrays as plain device arrays (the exact ranking decodes one row per node).
  * sid_trie_counts : counts int32 [C + 1] = the node count of every level (counts[0] = 1, the root); one tiny launch.
  * sid_trie_level  : for level l (1..C) of n_l nodes below n_prev parents: code int32 [n_l] (each node's last id), parent int32
@@ -422,8 +471,9 @@ int rqb200_t5score_trie_build(const int64_t* ids, int B, int C, int H, int K, in
  *                         stride ldq; rows b * nq .. b * nq + nq - 1 belong to history b), k / v [B * S, inner] (row stride ldkv:
  *                         key s of history b is row b * S + s), mask [B, S] or null (a key whose mask is 0 gets -FLT_MAX added,
  *                         torch.finfo(float32).min as in HF's eager mask), out [B * nq, inner] (row stride ldo).  One CTA per
- *                         (head, history) reads the history's keys/values once for all its queries; any S >= 1.
- *                         Limits: nq <= 32, B <= 65535 (RQB_ERR_UNSUPPORTED).
+ *                         (head, history, group of 32 queries) reads the history's keys/values once for its queries; a query's
+ *                         result does not depend on nq; any S >= 1.
+ *                         Limits: nq <= 65535 * 32, B <= 65535 (RQB_ERR_UNSUPPORTED).
  * t5dec_self_attention  : the causal self-attention of query position h (< H <= 8) for R beam rows.  qkv [R, 3 inner] (q | k | v,
  *                         row stride ldqkv).  cache_k / cache_v hold slot j (position j) of row x at [j * slot_stride + x * inner];
  *                         the row's own k / v are written to slot h.  Earlier positions j < h of row r are read from row

@@ -85,6 +85,21 @@ _SIGNATURES = {
                                                         c_int, c_int, c_vp]),
     "rqb200_sid_trie_beam_topk_including": (c_int, [c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp,
                                                     c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
+    "rqb200_sid_trie_beam_topk_wide": (c_int, [c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp,
+                                               c_vp, c_vp, c_vp, c_int, c_vp]),
+    "rqb200_sid_trie_beam_topk_wide_excluding": (c_int, [c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp,
+                                                         c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
+    "rqb200_sid_trie_beam_topk_wide_including": (c_int, [c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp,
+                                                         c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
+    "rqb200_sid_trie_sample_select_wide_workspace_bytes": (c_size, [c_int, c_int, c_int]),
+    "rqb200_sid_trie_sample_select_wide": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int,
+                                                   c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_size, c_int, c_vp]),
+    "rqb200_sid_trie_sample_select_wide_excluding": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int,
+                                                             c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_size,
+                                                             c_int, c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
+    "rqb200_sid_trie_sample_select_wide_including": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int,
+                                                             c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_size,
+                                                             c_int, c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
     "rqb200_sid_items_workspace_bytes": (c_size, [c_i64, c_int, c_int]),
     "rqb200_sid_items_build": (c_int, [c_vp, c_i64, c_int, c_int, c_vp, c_size, c_vp]),
     "rqb200_sid_items_lookup": (c_int, [c_vp, c_vp, c_i64, c_i64, c_int, c_vp, c_vp]),

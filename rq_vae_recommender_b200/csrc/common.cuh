@@ -118,6 +118,20 @@ __device__ __forceinline__ uint32_t cluster_map(uint32_t smem_addr, uint32_t ran
 __device__ __forceinline__ void cluster_sync_all() {   // every thread of every CTA of the cluster
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
+// distributed shared memory: loads, stores and atomics at a shared::cluster address (cluster_map)
+__device__ __forceinline__ int ld_shared_cluster_s32(uint32_t cluster_addr) {
+  int v;
+  asm volatile("ld.shared::cluster.s32 %0, [%1];" : "=r"(v) : "r"(cluster_addr) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_shared_cluster_u64(uint32_t cluster_addr, unsigned long long v) {
+  asm volatile("st.shared::cluster.u64 [%0], %1;" ::"r"(cluster_addr), "l"(v) : "memory");
+}
+__device__ __forceinline__ uint32_t atom_add_shared_cluster_u32(uint32_t cluster_addr, uint32_t v) {
+  uint32_t old;
+  asm volatile("atom.shared::cluster.add.u32 %0, [%1], %2;" : "=r"(old) : "r"(cluster_addr), "r"(v) : "memory");
+  return old;
+}
 // arrive on an mbarrier anywhere in the cluster (own CTA included), release at cluster scope
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");

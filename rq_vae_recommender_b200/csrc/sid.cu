@@ -1742,3 +1742,586 @@ extern "C" int rqb200_sid_rank_hist(const int64_t* rank, int B, int64_t k, int64
   RQB_LAUNCH_CHECK();
   return RQB_OK;
 }
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Wide levels of both searches: up to 1024 beams per history, where sid_beam_topk_kernel (kp <= 32, k <= 32) and
+// sid_sample_select_kernel (kp * nc <= 1024, k <= 32) stop.  One thread-block cluster of 1, 2, 4 or 8 CTAs per history, one
+// launch per level.  CTA r of the cluster owns a contiguous range of the history's beams: it computes their log-sum-exps
+// (exhaustive) or their nc-sample draws (sampled, sid_warp_top_n), builds their child masks (sid_beam_mask<FILTER>) and forms
+// its candidates' keys
+//   v(e) = sid_topk_key(score) << 21 | (2^21 - 1 - e),   e = beam * K + code (exhaustive) or beam * nc + j (sampled),
+// distinct within a history (E <= 1024 * 2048 = 2^21), so "the k largest keys" is exactly the narrow kernels' order: descending
+// score (-0 folded into +0), equal scores by ascending e.  The scores are those of the narrow kernels, with the same explicit
+// roundings, so both give the same bits wherever both run.
+// Selection is a radix selection over the cluster (8-bit digits, stopping once the chosen bin holds exactly the entries still
+// wanted): each CTA histograms its own candidates, reads its peers' histograms through distributed shared memory after one
+// cluster barrier per pass and decides the same digit redundantly.  The histograms are double-buffered: the buffer a pass
+// clears was last read by the peers before they reached this pass's barrier.  The kept keys are then gathered into CTA 0,
+// sorted descending there (cub::BlockRadixSort, at most 1024 of them) and written out.  Histograms are integer counts and the
+// final sort orders distinct keys, so no result depends on the cluster size or on the order of atomics.
+// A CTA keeps its 32-bit score keys in shared memory while its slice holds at most SID_WIDE_SMEM_KEYS of them.  Above that
+// the exhaustive kernel recomputes them from the logits on every pass (bit-identical, as sid_beam_topk_kernel<false>), and the
+// sampled kernel re-reads them from its global workspace, where every draw is kept.
+#define SID_WIDE_MAX_BEAMS 1024
+#define SID_WIDE_MAX_NC 64
+#define SID_WIDE_MAX_SEL 1024                               // kept keys (k <= 1024)
+#define SID_WIDE_SMEM_KEYS (16 * 1024)                      // score keys per CTA held in shared memory
+#define SID_WIDE_E_BITS 21
+#define SID_WIDE_TOPK_THREADS 512
+#define SID_WIDE_SAMPLE_THREADS 256
+#define SID_WIDE_MAX_CLUSTER 8
+
+struct SidWideShared {
+  int hist[2][256];                                         // this CTA's histogram, double-buffered across passes
+  int ctl[3];                                               // chosen digit, entries above its bin, entries in its bin
+  unsigned int nsel;                                        // CTA 0: kept keys gathered so far
+  unsigned long long sel[SID_WIDE_MAX_SEL];                 // CTA 0: the kept keys
+};
+
+template <int NT>
+using SidWideSort = cub::BlockRadixSort<unsigned long long, NT, SID_WIDE_MAX_SEL / NT>;
+
+__device__ __forceinline__ unsigned long long sid_wide_key(unsigned int key, int e) {
+  return ((unsigned long long)key << SID_WIDE_E_BITS) | (unsigned int)((1 << SID_WIDE_E_BITS) - 1 - e);
+}
+
+__device__ __forceinline__ float sid_topk_key_inverse(unsigned int key) {
+  return __uint_as_float((key & 0x80000000u) ? key ^ 0x80000000u : ~key);
+}
+
+// Every CTA of the cluster (cs CTAs, one history): the `want` largest keys v(e) of the history, e over this CTA's candidates
+// [e0, e1) with key_at(e) their 32-bit score keys.  On return CTA 0 holds them in s.sel[0, want), in no particular order.
+// Starts and ends with cluster barriers between which no CTA touches a peer's shared memory before the peer has initialised it.
+template <typename KeyAt>
+__device__ void sid_wide_select(const KeyAt& key_at, int e0, int e1, int want, int cs, SidWideShared& s) {
+  const int nt = blockDim.x, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const unsigned int lt = (1u << lane) - 1u;
+  unsigned long long prefix = 0, pmask = 0;
+  int pass = 0;
+  for (int shift = 48; shift >= 0; shift -= 8, ++pass) {    // v has 21 + 32 = 53 bits
+    int* hist = s.hist[pass & 1];
+    for (int base = e0; base < e1; base += nt) {
+      const int e = base + threadIdx.x;
+      int d = 256;
+      if (e < e1) {
+        const unsigned long long v = sid_wide_key(key_at(e), e);
+        if ((v & pmask) == prefix) d = (int)((v >> shift) & 255u);
+      }
+      const unsigned int same = __match_any_sync(0xffffffffu, d);
+      if (d < 256 && (same & lt) == 0) atomicAdd(&hist[d], __popc(same));   // one add per distinct digit of the warp
+    }
+    cluster_sync_all();                                     // every CTA's histogram of this pass is complete
+    if (w == 0) {
+      int c[8], sum = 0;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) c[j] = 0;
+      for (int r = 0; r < cs; ++r) {                        // the cluster's bins lane * 8 .. lane * 8 + 7, peers in rank order
+        const uint32_t a = cluster_map(smem_u32(hist + lane * 8), (uint32_t)r);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) c[j] += ld_shared_cluster_s32(a + 4 * j);
+      }
+#pragma unroll
+      for (int j = 0; j < 8; ++j) sum += c[j];
+      int suf = sum;                                        // entries in bins >= lane * 8
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_down_sync(0xffffffffu, suf, o);
+        if (lane + o < 32) suf += t;
+      }
+      const int owner = 31 - __clz(__ballot_sync(0xffffffffu, suf >= want));
+      if (lane == owner) {
+        int acc = suf - sum;
+        for (int j = 7; j >= 0; --j) {
+          if (acc + c[j] >= want) {
+            s.ctl[0] = lane * 8 + j;
+            s.ctl[1] = acc;
+            s.ctl[2] = c[j];
+            break;
+          }
+          acc += c[j];
+        }
+      }
+    } else {                                                // the next pass's buffer: the peers read it before this barrier
+      int* next = s.hist[(pass + 1) & 1];
+      for (int i = threadIdx.x - 32; i < 256; i += nt - 32) next[i] = 0;
+    }
+    __syncthreads();
+    want -= s.ctl[1];
+    prefix |= (unsigned long long)s.ctl[0] << shift;
+    pmask |= 255ull << shift;
+    if (s.ctl[2] == want) break;                            // the whole bin is kept: the threshold is decided
+  }
+  // the kept set: keys whose decided digits are above the prefix or equal to it, appended to CTA 0's list
+  const uint32_t nsel0 = cluster_map(smem_u32(&s.nsel), 0), sel0 = cluster_map(smem_u32(s.sel), 0);
+  for (int base = e0; base < e1; base += nt) {
+    const int e = base + threadIdx.x;
+    unsigned long long v = 0;
+    bool keep = false;
+    if (e < e1) {
+      v = sid_wide_key(key_at(e), e);
+      keep = (v & pmask) >= prefix;
+    }
+    const unsigned int bk = __ballot_sync(0xffffffffu, keep);
+    if (bk == 0) continue;
+    uint32_t at = 0;
+    if (lane == 0) at = atom_add_shared_cluster_u32(nsel0, (uint32_t)__popc(bk));
+    at = __shfl_sync(0xffffffffu, at, 0);
+    if (keep) st_shared_cluster_u64(sel0 + 8u * (at + (uint32_t)__popc(bk & lt)), v);
+  }
+  cluster_sync_all();                                       // CTA 0 holds every kept key
+}
+
+// CTA 0 after sid_wide_select: keys[i] = the kept key of rank threadIdx.x * IPT + i (descending; 0 past the n kept)
+template <int NT>
+__device__ __forceinline__ void sid_wide_sort(SidWideShared& s, typename SidWideSort<NT>::TempStorage& tmp, int n,
+                                              unsigned long long (&keys)[SID_WIDE_MAX_SEL / NT]) {
+  constexpr int IPT = SID_WIDE_MAX_SEL / NT;
+#pragma unroll
+  for (int i = 0; i < IPT; ++i) {
+    const int r = threadIdx.x * IPT + i;
+    keys[i] = r < n ? s.sel[r] : 0ull;                      // every real key is above 0: sid_topk_key(-inf) > 0
+  }
+  SidWideSort<NT>(tmp).SortDescending(keys, 0, 32 + SID_WIDE_E_BITS);
+}
+
+__device__ __forceinline__ void sid_wide_init(SidWideShared& s) {
+  for (int i = threadIdx.x; i < 512; i += blockDim.x) (&s.hist[0][0])[i] = 0;
+  if (threadIdx.x == 0) s.nsel = 0;
+}
+
+// The exhaustive level (sid_beam_topk_kernel's scores) for history blockIdx.x / cs; this CTA owns beams
+// [rank * per_cta, rank * per_cta + per_cta) of the history.
+template <bool KEYS_IN_SMEM, int FILTER>
+__global__ void __launch_bounds__(SID_WIDE_TOPK_THREADS, 2) sid_beam_topk_wide_kernel(
+    const float* __restrict__ logits, int64_t ld, const int64_t* __restrict__ generated, const float* __restrict__ log_probas,
+    int kp, int h, int k, int K, int cs, int per_cta, SidTrie trie, int64_t* __restrict__ out_generated,
+    float* __restrict__ out_log_probas, int64_t* __restrict__ out_parent, int* __restrict__ bad, SidExcl ex) {
+  constexpr int NT = SID_WIDE_TOPK_THREADS, IPT = SID_WIDE_MAX_SEL / NT;
+  extern __shared__ __align__(16) unsigned char sid_smem[];
+  __shared__ SidWideShared s;
+  __shared__ typename SidWideSort<NT>::TempStorage sort_tmp;
+  const int W = NT >> 5, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int rank = (int)cluster_ctarank(), b = blockIdx.x / cs, KW = (K + 31) >> 5;
+  const int beam0 = min(kp, rank * per_cta), nb = min(kp, beam0 + per_cta) - beam0;
+  const int64_t row0 = (int64_t)b * kp;
+  float* s_lse = reinterpret_cast<float*>(sid_smem);                             // [per_cta]
+  float* s_plp = s_lse + per_cta;                                                // [per_cta]
+  unsigned int* s_mask = reinterpret_cast<unsigned int*>(s_plp + per_cta);       // [per_cta][KW]
+  unsigned int* s_key = s_mask + (size_t)per_cta * KW;                           // [per_cta * K] when KEYS_IN_SMEM
+  sid_wide_init(s);
+  for (int i = w; i < nb; i += W) {                         // warp per beam: row maximum, then log-sum-exp (as the narrow kernel)
+    const float* x = logits + (row0 + beam0 + i) * ld;
+    float m = -INFINITY;
+    bool odd = false;
+    for (int c = lane; c < K; c += 32) {
+      const float v = x[c];
+      m = fmaxf(m, v);
+      odd |= v != v || v == INFINITY;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    odd = __any_sync(0xffffffffu, odd);
+    float sum = 0.f;
+    for (int c = lane; c < K; c += 32) sum += expf(x[c] - m);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    if (lane == 0) {
+      s_lse[i] = m + logf(sum);
+      s_plp[i] = log_probas ? log_probas[row0 + beam0 + i] : 0.f;
+      if (bad && (odd || m == -INFINITY)) atomicAdd(bad, 1);
+    }
+    sid_beam_mask<FILTER>(trie, ex, b, generated + (row0 + beam0 + i) * h, h, K, s_mask + (size_t)i * KW, lane);
+  }
+  __syncthreads();
+  const int e0 = beam0 * K, e1 = (beam0 + nb) * K;
+  auto score_key = [=](int e) -> unsigned int {
+    const int beam = e / K, c = e - beam * K, i = beam - beam0;
+    const float lp = __fadd_rn(__fsub_rn(logits[(row0 + beam) * ld + c], s_lse[i]), s_plp[i]);
+    const float sc = sid_extension_score(sid_mask_has(s_mask + (size_t)i * KW, c), lp);
+    return sid_topk_key(sc == 0.f ? 0.f : sc);
+  };
+  if (KEYS_IN_SMEM) {
+    for (int e = e0 + threadIdx.x; e < e1; e += NT) s_key[e - e0] = score_key(e);
+    __syncthreads();
+    sid_wide_select([=](int e) { return s_key[e - e0]; }, e0, e1, k, cs, s);
+  } else {
+    sid_wide_select(score_key, e0, e1, k, cs, s);
+  }
+  if (rank != 0) return;
+  unsigned long long keys[IPT];
+  sid_wide_sort<NT>(s, sort_tmp, k, keys);
+#pragma unroll
+  for (int i = 0; i < IPT; ++i) {
+    const int r = threadIdx.x * IPT + i;
+    if (r >= k) continue;
+    const int e = (1 << SID_WIDE_E_BITS) - 1 - (int)(keys[i] & ((1u << SID_WIDE_E_BITS) - 1));
+    const int beam = e / K;
+    const int64_t o = (int64_t)b * k + r;
+    out_log_probas[o] = sid_topk_key_inverse((unsigned int)(keys[i] >> SID_WIDE_E_BITS));
+    out_parent[o] = row0 + beam;
+    int64_t* g = out_generated + o * (h + 1);
+    for (int j = 0; j < h; ++j) g[j] = generated[(row0 + beam) * h + j];
+    g[h] = e - beam * K;
+  }
+}
+
+// The sampled level (sid_sample_select_kernel's draws and scores) for history blockIdx.x / cs.  Each of the CTA's warps draws
+// one beam at a time into its own buffers; every draw's token goes to ws_tok [B][kp * nc] and its score key to shared memory
+// (KEYS_IN_SMEM) or ws_key [B][kp * nc].
+template <bool KEYS_IN_SMEM, int FILTER>
+__global__ void __launch_bounds__(SID_WIDE_SAMPLE_THREADS) sid_sample_select_wide_kernel(
+    const float* __restrict__ probas, int64_t p_stride, const float* __restrict__ noise, int64_t n_stride,
+    const int64_t* __restrict__ generated, const float* __restrict__ log_probas, int kp, int nc, int h, int k, int K, int cs,
+    int per_cta, SidTrie trie, int64_t* __restrict__ out_generated, float* __restrict__ out_log_probas,
+    int64_t* __restrict__ out_parent, int64_t* __restrict__ samples, float* __restrict__ samp_log_p, int* __restrict__ reject,
+    int* __restrict__ ws_tok, unsigned int* __restrict__ ws_key, SidExcl ex) {
+  constexpr int NT = SID_WIDE_SAMPLE_THREADS, IPT = SID_WIDE_MAX_SEL / NT, W = NT >> 5;
+  extern __shared__ __align__(16) unsigned char sid_smem[];
+  __shared__ SidWideShared s;
+  __shared__ typename SidWideSort<NT>::TempStorage sort_tmp;
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int rank = (int)cluster_ctarank(), b = blockIdx.x / cs, KW = (K + 31) >> 5, E = kp * nc;
+  const int beam0 = min(kp, rank * per_cta), nb = min(kp, beam0 + per_cta) - beam0;
+  int64_t* s_tok = reinterpret_cast<int64_t*>(sid_smem) + (size_t)w * nc;                                  // [W][nc]
+  unsigned int* s_rkey = reinterpret_cast<unsigned int*>(reinterpret_cast<int64_t*>(sid_smem) + (size_t)W * nc);   // [W][K]
+  int* s_hist = reinterpret_cast<int*>(s_rkey + (size_t)W * K) + w * 256;                                   // [W][256]
+  unsigned int* s_sk = reinterpret_cast<unsigned int*>(s_hist - w * 256 + W * 256) + w * nc;               // [W][nc]
+  int* s_si = reinterpret_cast<int*>(s_sk - w * nc + W * nc) + w * nc;                                     // [W][nc]
+  unsigned int* s_mask = reinterpret_cast<unsigned int*>(s_si - w * nc + W * nc) + w * KW;                 // [W][KW]
+  unsigned int* s_key = s_mask - w * KW + W * KW;                                                          // [per_cta * nc]
+  s_rkey += (size_t)w * K;
+  int* tok_b = ws_tok + (int64_t)b * E;
+  sid_wide_init(s);
+  for (int i = w; i < nb; i += W) {
+    const int beam = beam0 + i;
+    const int64_t row = (int64_t)b * kp + beam;
+    const float* p = probas + row * p_stride;
+    const float* q = noise + row * n_stride;
+    bool bad = false, nonzero = false;
+    for (int c = lane; c < K; c += 32) {
+      const float pv = p[c];
+      bad |= !(pv >= 0.f) || pv == INFINITY;
+      nonzero |= pv != 0.f;
+      s_rkey[c] = sid_topk_key(__fdiv_rn(pv, q[c]));
+    }
+    bad = __any_sync(0xffffffffu, bad);
+    nonzero = __any_sync(0xffffffffu, nonzero);
+    if (reject && lane == 0 && (bad || !nonzero)) atomicAdd(&reject[bad ? 0 : 1], 1);
+    __syncwarp();
+    sid_warp_top_n(s_rkey, K, nc, s_hist, s_sk, s_si, s_tok, lane);
+    sid_beam_mask<FILTER>(trie, ex, b, generated + row * h, h, K, s_mask, lane);
+    const float plp = log_probas ? log_probas[row] : 0.f;
+    for (int r = lane; r < nc; r += 32) {
+      const int64_t tok = s_tok[r];
+      const float lp = logf(p[tok]);
+      if (samples) samples[row * nc + r] = tok;
+      if (samp_log_p) samp_log_p[row * nc + r] = lp;
+      const float sc = sid_extension_score(sid_mask_has(s_mask, (int)tok), lp + plp);
+      const unsigned int key = sid_topk_key(sc == 0.f ? 0.f : sc);
+      const int e = beam * nc + r;
+      tok_b[e] = (int)tok;
+      if (KEYS_IN_SMEM) s_key[e - beam0 * nc] = key;
+      else ws_key[(int64_t)b * E + e] = key;
+    }
+    __syncwarp();
+  }
+  __syncthreads();
+  const int e0 = beam0 * nc, e1 = (beam0 + nb) * nc, n = min(k, E);
+  if (KEYS_IN_SMEM) sid_wide_select([=](int e) { return s_key[e - e0]; }, e0, e1, n, cs, s);
+  else sid_wide_select([=](int e) { return ws_key[(int64_t)b * E + e]; }, e0, e1, n, cs, s);
+  if (rank != 0) return;
+  unsigned long long keys[IPT];
+  sid_wide_sort<NT>(s, sort_tmp, n, keys);
+#pragma unroll
+  for (int i = 0; i < IPT; ++i) {
+    const int r = threadIdx.x * IPT + i;
+    if (r >= k) continue;
+    int e = 0;                                              // k > kp * nc: the remaining slots repeat entry 0 with -inf
+    float lp = -INFINITY;
+    if (r < n) {
+      e = (1 << SID_WIDE_E_BITS) - 1 - (int)(keys[i] & ((1u << SID_WIDE_E_BITS) - 1));
+      lp = sid_topk_key_inverse((unsigned int)(keys[i] >> SID_WIDE_E_BITS));
+    }
+    const int beam = e / nc;
+    const int64_t o = (int64_t)b * k + r, parent = (int64_t)b * kp + beam;
+    out_log_probas[o] = lp;
+    out_parent[o] = parent;
+    int64_t* g = out_generated + o * (h + 1);
+    for (int j = 0; j < h; ++j) g[j] = generated[parent * h + j];
+    g[h] = tok_b[e];
+  }
+}
+
+// A wide kernel instance for cluster size cs: the function, its dynamic shared memory and its beams per CTA
+struct SidWideLaunch {
+  const void* fn;
+  size_t smem;
+  int per_cta;
+};
+
+// Picks the cluster size (forced: 1, 2, 4 or 8; 0: choose) of a wide launch over B histories of kp beams, `work` elements read
+// per history, and sets up cfg (grid B * cs) for it.  pick(cs) gives the instance for cs.  The choice spreads small batches
+// over the GPU (B * cs up to the SM count, at least 16 K elements per CTA) and takes the nearest size whose shared memory fits
+// and of which a cluster can be resident (cudaOccupancyMaxActiveClusters).
+template <typename Pick>
+static int sid_wide_plan(int B, int kp, int64_t work, int forced, int nt, const Pick& pick, cudaStream_t st, const char* what,
+                         cudaLaunchConfig_t& cfg, cudaLaunchAttribute& attr, SidWideLaunch& L, int& cs) {
+  int dev = 0, nsm = 0, optin = 0;
+  RQB_CUDA(cudaGetDevice(&dev));
+  RQB_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
+  RQB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  if (forced != 0 && forced != 1 && forced != 2 && forced != 4 && forced != 8) {
+    rqb_set_error("%s: cluster = %d (0 to choose, or 1, 2, 4 or 8)", what, forced);
+    return RQB_ERR_INVALID;
+  }
+  int pref = 1;
+  while (pref < SID_WIDE_MAX_CLUSTER && 2 * pref <= kp && (int64_t)B * pref < nsm && work / (2 * pref) >= 16 * 1024) pref *= 2;
+  int order[SID_WIDE_MAX_CLUSTER], n = 0;
+  if (forced) {
+    order[n++] = forced;
+  } else {
+    for (int c = pref; c >= 1; c /= 2) order[n++] = c;
+    for (int c = 2 * pref; c <= SID_WIDE_MAX_CLUSTER; c *= 2) order[n++] = c;
+  }
+  attr.id = cudaLaunchAttributeClusterDimension;
+  cfg = cudaLaunchConfig_t{};
+  cfg.blockDim = dim3(nt);
+  cfg.stream = st;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
+  for (int i = 0; i < n; ++i) {
+    const int c = order[i];
+    const SidWideLaunch l = pick(c);
+    cudaFuncAttributes fa;
+    RQB_CUDA(cudaFuncGetAttributes(&fa, l.fn));
+    if (fa.sharedSizeBytes + l.smem > (size_t)optin) continue;
+    RQB_CUDA(cudaFuncSetAttribute(l.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l.smem));
+    attr.val.clusterDim.x = c;
+    attr.val.clusterDim.y = 1;
+    attr.val.clusterDim.z = 1;
+    cfg.gridDim = dim3((unsigned)(B * c));
+    cfg.dynamicSmemBytes = l.smem;
+    int active = 0;
+    if (cudaOccupancyMaxActiveClusters(&active, l.fn, &cfg) != cudaSuccess) {
+      cudaGetLastError();
+      active = 0;
+    }
+    if (active > 0) {
+      L = l;
+      cs = c;
+      return RQB_OK;
+    }
+  }
+  rqb_set_error("%s: no cluster size %s fits kp = %d beams of this level in shared memory", what,
+                forced ? "of the one asked for" : "of 1, 2, 4 or 8", kp);
+  return RQB_ERR_UNSUPPORTED;
+}
+
+template <int FILTER>
+static SidWideLaunch sid_beam_topk_wide_pick(int kp, int K, int cs) {
+  const int per_cta = (kp + cs - 1) / cs;
+  const bool keys = (int64_t)per_cta * K <= SID_WIDE_SMEM_KEYS;
+  const size_t smem = (size_t)per_cta * (2 * sizeof(float) + ((K + 31) / 32) * sizeof(unsigned int)) +
+                      (keys ? (size_t)per_cta * K * sizeof(unsigned int) : 0);
+  return {keys ? (const void*)sid_beam_topk_wide_kernel<true, FILTER> : (const void*)sid_beam_topk_wide_kernel<false, FILTER>,
+          smem, per_cta};
+}
+
+template <int FILTER>
+static int sid_beam_topk_wide_launch(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas,
+                                     int B, int kp, int h, int k, int K, const SidTrie& trie, int64_t* out_generated,
+                                     float* out_log_probas, int64_t* out_parent, int* bad, const SidExcl& ex, int cluster,
+                                     cudaStream_t st) {
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr;
+  SidWideLaunch L;
+  int cs = 0;
+  const int rc = sid_wide_plan(B, kp, (int64_t)kp * K, cluster, SID_WIDE_TOPK_THREADS,
+                               [&](int c) { return sid_beam_topk_wide_pick<FILTER>(kp, K, c); }, st, "sid_trie_beam_topk_wide",
+                               cfg, attr, L, cs);
+  if (rc != RQB_OK) return rc;
+  SidTrie tr = trie;
+  SidExcl fx = ex;
+  void* args[] = {&logits, &logits_stride, &generated, &log_probas, &kp, &h, &k, &K, &cs, &L.per_cta, &tr,
+                  &out_generated, &out_log_probas, &out_parent, &bad, &fx};
+  RQB_CUDA(cudaLaunchKernelExC(&cfg, L.fn, args));
+  return RQB_OK;
+}
+
+static int sid_beam_topk_wide(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas, int B,
+                              int kp, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
+                              float* out_log_probas, int64_t* out_parent, int* bad, const SidExcl& ex, int cluster, void* stream) {
+  RQB_CHECK_ARG(B >= 0 && kp > 0 && h >= 0 && h < C && C <= 8 && k > 0 && K > 0 && logits_stride >= K,
+                "sid_trie_beam_topk_wide: bad argument (B=%d kp=%d h=%d k=%d C=%d K=%d)", B, kp, h, k, C, K);
+  if (K > SID_TOPK_MAX_K || k > SID_WIDE_MAX_SEL || k > K || kp > SID_WIDE_MAX_BEAMS) {
+    rqb_set_error("sid_trie_beam_topk_wide: need K <= %d, k <= %d, k <= K, kp <= %d (K = %d, k = %d, kp = %d)", SID_TOPK_MAX_K,
+                  SID_WIDE_MAX_SEL, SID_WIDE_MAX_BEAMS, K, k, kp);
+    return RQB_ERR_UNSUPPORTED;
+  }
+  if (B == 0) return RQB_OK;
+  RQB_CHECK_ARG(logits && prefix_workspace && out_generated && out_log_probas && out_parent && (h == 0 || generated) &&
+                    (h == 0 || log_probas), "sid_trie_beam_topk_wide: null pointer");
+  const SidTrie trie{reinterpret_cast<const unsigned char*>(prefix_workspace), h + 1};
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  switch (sid_filter_mode(ex)) {
+    case SID_FILTER_INCLUDE:
+      return sid_beam_topk_wide_launch<SID_FILTER_INCLUDE>(logits, logits_stride, generated, log_probas, B, kp, h, k, K, trie,
+                                                           out_generated, out_log_probas, out_parent, bad, ex, cluster, st);
+    case SID_FILTER_EXCLUDE:
+      return sid_beam_topk_wide_launch<SID_FILTER_EXCLUDE>(logits, logits_stride, generated, log_probas, B, kp, h, k, K, trie,
+                                                           out_generated, out_log_probas, out_parent, bad, ex, cluster, st);
+    default:
+      return sid_beam_topk_wide_launch<SID_FILTER_NONE>(logits, logits_stride, generated, log_probas, B, kp, h, k, K, trie,
+                                                        out_generated, out_log_probas, out_parent, bad, ex, cluster, st);
+  }
+}
+
+extern "C" int rqb200_sid_trie_beam_topk_wide(const float* logits, int64_t logits_stride, const int64_t* generated,
+                                              const float* log_probas, int B, int kp, int h, int k, int C, int K,
+                                              const void* prefix_workspace, int64_t* out_generated, float* out_log_probas,
+                                              int64_t* out_parent, int* bad, int cluster, void* stream) {
+  return sid_beam_topk_wide(logits, logits_stride, generated, log_probas, B, kp, h, k, C, K, prefix_workspace, out_generated,
+                            out_log_probas, out_parent, bad, SidExcl{}, cluster, stream);
+}
+
+extern "C" int rqb200_sid_trie_beam_topk_wide_excluding(const float* logits, int64_t logits_stride, const int64_t* generated,
+                                                        const float* log_probas, int B, int kp, int h, int k, int C, int K,
+                                                        const void* prefix_workspace, int64_t* out_generated, float* out_log_probas,
+                                                        int64_t* out_parent, int* bad, int cluster, const int* ex_pos,
+                                                        const int64_t* ex_blocked, const int* ex_count, int ex_M, int ex_H,
+                                                        void* stream) {
+  SidExcl ex;
+  const int rc = sid_excl_of(ex_pos, ex_blocked, ex_count, ex_M, ex_H, h + 1, "sid_trie_beam_topk_wide_excluding", ex);
+  if (rc != RQB_OK) return rc;
+  return sid_beam_topk_wide(logits, logits_stride, generated, log_probas, B, kp, h, k, C, K, prefix_workspace, out_generated,
+                            out_log_probas, out_parent, bad, ex, cluster, stream);
+}
+
+extern "C" int rqb200_sid_trie_beam_topk_wide_including(const float* logits, int64_t logits_stride, const int64_t* generated,
+                                                        const float* log_probas, int B, int kp, int h, int k, int C, int K,
+                                                        const void* prefix_workspace, int64_t* out_generated, float* out_log_probas,
+                                                        int64_t* out_parent, int* bad, int cluster, const int* in_pos,
+                                                        const int64_t* in_keys, const int* in_count, int in_M, int in_H,
+                                                        void* stream) {
+  SidExcl in;
+  const int rc = sid_excl_of(in_pos, in_keys, in_count, in_M, in_H, h + 1, "sid_trie_beam_topk_wide_including", in, true);
+  if (rc != RQB_OK) return rc;
+  return sid_beam_topk_wide(logits, logits_stride, generated, log_probas, B, kp, h, k, C, K, prefix_workspace, out_generated,
+                            out_log_probas, out_parent, bad, in, cluster, stream);
+}
+
+extern "C" size_t rqb200_sid_trie_sample_select_wide_workspace_bytes(int B, int kp, int nc) {
+  return B < 0 || kp < 0 || nc < 0 ? 0 : (size_t)B * kp * nc * (sizeof(int) + sizeof(unsigned int));
+}
+
+template <int FILTER>
+static SidWideLaunch sid_sample_select_wide_pick(int kp, int nc, int K, int cs) {
+  constexpr int W = SID_WIDE_SAMPLE_THREADS / 32;
+  const int per_cta = (kp + cs - 1) / cs;
+  const bool keys = (int64_t)per_cta * nc <= SID_WIDE_SMEM_KEYS;
+  const size_t smem = (size_t)W * (nc * sizeof(int64_t) + (K + 256 + 2 * nc + (K + 31) / 32) * 4) +
+                      (keys ? (size_t)per_cta * nc * sizeof(unsigned int) : 0);
+  return {keys ? (const void*)sid_sample_select_wide_kernel<true, FILTER> : (const void*)sid_sample_select_wide_kernel<false, FILTER>,
+          smem, per_cta};
+}
+
+template <int FILTER>
+static int sid_sample_select_wide_launch(const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride,
+                                         const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k,
+                                         int K, const SidTrie& trie, int64_t* out_generated, float* out_log_probas,
+                                         int64_t* out_parent, int64_t* samples, float* samp_log_p, int* reject, int* ws_tok,
+                                         unsigned int* ws_key, const SidExcl& ex, int cluster, cudaStream_t st) {
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr;
+  SidWideLaunch L;
+  int cs = 0;
+  const int rc = sid_wide_plan(B, kp, (int64_t)kp * K, cluster, SID_WIDE_SAMPLE_THREADS,
+                               [&](int c) { return sid_sample_select_wide_pick<FILTER>(kp, nc, K, c); }, st,
+                               "sid_trie_sample_select_wide", cfg, attr, L, cs);
+  if (rc != RQB_OK) return rc;
+  SidTrie tr = trie;
+  SidExcl fx = ex;
+  void* args[] = {&probas, &probas_stride, &noise, &noise_stride, &generated, &log_probas, &kp, &nc, &h, &k, &K, &cs, &L.per_cta,
+                  &tr, &out_generated, &out_log_probas, &out_parent, &samples, &samp_log_p, &reject, &ws_tok, &ws_key, &fx};
+  RQB_CUDA(cudaLaunchKernelExC(&cfg, L.fn, args));
+  return RQB_OK;
+}
+
+static int sid_sample_select_wide(const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride,
+                                  const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k, int C, int K,
+                                  const void* prefix_workspace, int64_t* out_generated, float* out_log_probas, int64_t* out_parent,
+                                  int64_t* samples, float* samp_log_p, int* reject, void* workspace, size_t workspace_bytes,
+                                  int cluster, const SidExcl& ex, void* stream) {
+  RQB_CHECK_ARG(B >= 0 && kp > 0 && nc > 0 && h >= 0 && h < C && C <= 8 && k > 0 && K > 0 && probas_stride >= K &&
+                    noise_stride >= K, "sid_trie_sample_select_wide: bad argument (B=%d kp=%d nc=%d h=%d k=%d C=%d K=%d)", B, kp,
+                nc, h, k, C, K);
+  if (nc > K || K > SID_SAMPLE_MAX_K || nc > SID_WIDE_MAX_NC || kp > SID_WIDE_MAX_BEAMS || k > SID_WIDE_MAX_SEL) {
+    rqb_set_error("sid_trie_sample_select_wide: need nc <= K <= %d, nc <= %d, kp <= %d, k <= %d (nc = %d, K = %d, kp = %d, k = %d)",
+                  SID_SAMPLE_MAX_K, SID_WIDE_MAX_NC, SID_WIDE_MAX_BEAMS, SID_WIDE_MAX_SEL, nc, K, kp, k);
+    return RQB_ERR_UNSUPPORTED;
+  }
+  if (B == 0) return RQB_OK;
+  RQB_CHECK_ARG(probas && noise && prefix_workspace && out_generated && out_log_probas && out_parent && workspace &&
+                    (h == 0 || generated) && (h == 0 || log_probas), "sid_trie_sample_select_wide: null pointer");
+  if (workspace_bytes < rqb200_sid_trie_sample_select_wide_workspace_bytes(B, kp, nc)) {
+    rqb_set_error("sid_trie_sample_select_wide: workspace too small");
+    return RQB_ERR_WORKSPACE;
+  }
+  int* ws_tok = reinterpret_cast<int*>(workspace);
+  unsigned int* ws_key = reinterpret_cast<unsigned int*>(ws_tok + (size_t)B * kp * nc);
+  const SidTrie trie{reinterpret_cast<const unsigned char*>(prefix_workspace), h + 1};
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  switch (sid_filter_mode(ex)) {
+    case SID_FILTER_INCLUDE:
+      return sid_sample_select_wide_launch<SID_FILTER_INCLUDE>(probas, probas_stride, noise, noise_stride, generated, log_probas, B,
+                                                               kp, nc, h, k, K, trie, out_generated, out_log_probas, out_parent,
+                                                               samples, samp_log_p, reject, ws_tok, ws_key, ex, cluster, st);
+    case SID_FILTER_EXCLUDE:
+      return sid_sample_select_wide_launch<SID_FILTER_EXCLUDE>(probas, probas_stride, noise, noise_stride, generated, log_probas, B,
+                                                               kp, nc, h, k, K, trie, out_generated, out_log_probas, out_parent,
+                                                               samples, samp_log_p, reject, ws_tok, ws_key, ex, cluster, st);
+    default:
+      return sid_sample_select_wide_launch<SID_FILTER_NONE>(probas, probas_stride, noise, noise_stride, generated, log_probas, B,
+                                                            kp, nc, h, k, K, trie, out_generated, out_log_probas, out_parent,
+                                                            samples, samp_log_p, reject, ws_tok, ws_key, ex, cluster, st);
+  }
+}
+
+extern "C" int rqb200_sid_trie_sample_select_wide(const float* probas, int64_t probas_stride, const float* noise,
+                                                  int64_t noise_stride, const int64_t* generated, const float* log_probas, int B,
+                                                  int kp, int nc, int h, int k, int C, int K, const void* prefix_workspace,
+                                                  int64_t* out_generated, float* out_log_probas, int64_t* out_parent,
+                                                  int64_t* samples, float* samp_log_p, int* reject, void* workspace,
+                                                  size_t workspace_bytes, int cluster, void* stream) {
+  return sid_sample_select_wide(probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K,
+                                prefix_workspace, out_generated, out_log_probas, out_parent, samples, samp_log_p, reject, workspace,
+                                workspace_bytes, cluster, SidExcl{}, stream);
+}
+
+extern "C" int rqb200_sid_trie_sample_select_wide_excluding(
+    const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride, const int64_t* generated,
+    const float* log_probas, int B, int kp, int nc, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
+    float* out_log_probas, int64_t* out_parent, int64_t* samples, float* samp_log_p, int* reject, void* workspace,
+    size_t workspace_bytes, int cluster, const int* ex_pos, const int64_t* ex_blocked, const int* ex_count, int ex_M, int ex_H,
+    void* stream) {
+  SidExcl ex;
+  const int rc = sid_excl_of(ex_pos, ex_blocked, ex_count, ex_M, ex_H, h + 1, "sid_trie_sample_select_wide_excluding", ex);
+  if (rc != RQB_OK) return rc;
+  return sid_sample_select_wide(probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K,
+                                prefix_workspace, out_generated, out_log_probas, out_parent, samples, samp_log_p, reject, workspace,
+                                workspace_bytes, cluster, ex, stream);
+}
+
+extern "C" int rqb200_sid_trie_sample_select_wide_including(
+    const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride, const int64_t* generated,
+    const float* log_probas, int B, int kp, int nc, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
+    float* out_log_probas, int64_t* out_parent, int64_t* samples, float* samp_log_p, int* reject, void* workspace,
+    size_t workspace_bytes, int cluster, const int* in_pos, const int64_t* in_keys, const int* in_count, int in_M, int in_H,
+    void* stream) {
+  SidExcl in;
+  const int rc = sid_excl_of(in_pos, in_keys, in_count, in_M, in_H, h + 1, "sid_trie_sample_select_wide_including", in, true);
+  if (rc != RQB_OK) return rc;
+  return sid_sample_select_wide(probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K,
+                                prefix_workspace, out_generated, out_log_probas, out_parent, samples, samp_log_p, reject, workspace,
+                                workspace_bytes, cluster, in, stream);
+}

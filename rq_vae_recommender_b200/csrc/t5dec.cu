@@ -4,7 +4,7 @@
 //
 //   rqb200_t5dec_cross_attention  attention over the encoder output, one CTA per (history, head).  Every beam of a history has the
 //                                 same cross keys and values, so they are stored once per history ([B, S] rows) and the CTA reads
-//                                 them once for all of the history's nq queries (1 at level 0, top_k later).  Keys stream through
+//                                 them once for up to 32 of the history's nq queries (1 at level 0, the beam width later).  Keys stream through
 //                                 shared memory 32 at a time with an online softmax: the encoder length has no fixed limit.
 //   rqb200_t5dec_self_attention   the step's causal self-attention, one warp per (beam row, head).  The step's own key/value go to
 //                                 slot h of a cache of H positions; earlier positions are read through an int32 ancestor table
@@ -50,7 +50,8 @@ __device__ __forceinline__ float warp_max(float v) {
 }
 
 // ------------------------------------------------------------------------------------------------ cross-attention
-// grid (heads, B), XA_WARPS warps.  q row b * nq + i, head n: q[(b * nq + i) * ldq + n * 64 + d]; key s of history b:
+// grid (heads, B, ceil(nq / 32)), XA_WARPS warps: CTA z takes the history's queries 32 z .. 32 z + 31, so a query's arithmetic
+// does not depend on nq.  q row b * nq + i, head n: q[(b * nq + i) * ldq + n * 64 + d]; key s of history b:
 // k[(b * S + s) * ldkv + n * 64 + d] (v likewise); mask[b * S + s] == 0 masks the key (mask may be null); out like q.
 __global__ void __launch_bounds__(XA_WARPS * 32) t5dec_cross_attention_kernel(
     const float* __restrict__ q, int64_t ldq, const float* __restrict__ k, const float* __restrict__ v, int64_t ldkv,
@@ -62,8 +63,10 @@ __global__ void __launch_bounds__(XA_WARPS * 32) t5dec_cross_attention_kernel(
   const int n = blockIdx.x, b = blockIdx.y;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t col = (int64_t)n * T5_DKV;
-  for (int i = threadIdx.x; i < nq * T5_DKV; i += blockDim.x)
-    sq[i / T5_DKV][i % T5_DKV] = q[((int64_t)b * nq + i / T5_DKV) * ldq + col + i % T5_DKV];
+  const int64_t row0 = (int64_t)b * nq + (int64_t)blockIdx.z * XA_MAX_NQ;     // this CTA's first query row
+  const int ng = min(XA_MAX_NQ, nq - (int)blockIdx.z * XA_MAX_NQ);            // and its queries
+  for (int i = threadIdx.x; i < ng * T5_DKV; i += blockDim.x)
+    sq[i / T5_DKV][i % T5_DKV] = q[(row0 + i / T5_DKV) * ldq + col + i % T5_DKV];
 
   float m[XA_QPW], l[XA_QPW], acc0[XA_QPW], acc1[XA_QPW];
 #pragma unroll
@@ -86,7 +89,7 @@ __global__ void __launch_bounds__(XA_WARPS * 32) t5dec_cross_attention_kernel(
 #pragma unroll
     for (int t = 0; t < XA_QPW; ++t) {
       const int qi = warp + t * XA_WARPS;
-      if (qi >= nq) continue;
+      if (qi >= ng) continue;
       float dot = 0.f;
 #pragma unroll 16
       for (int d = 0; d < T5_DKV; ++d) dot = fmaf(sq[qi][d], sk[lane][d], dot);
@@ -111,8 +114,8 @@ __global__ void __launch_bounds__(XA_WARPS * 32) t5dec_cross_attention_kernel(
 #pragma unroll
   for (int t = 0; t < XA_QPW; ++t) {
     const int qi = warp + t * XA_WARPS;
-    if (qi >= nq) continue;
-    float* o = out + ((int64_t)b * nq + qi) * ldo + col;
+    if (qi >= ng) continue;
+    float* o = out + (row0 + qi) * ldo + col;
     o[lane] = acc0[t] / l[t];
     o[lane + 32] = acc1[t] / l[t];
   }
@@ -526,15 +529,17 @@ extern "C" int rqb200_t5dec_cross_attention(const float* q, int64_t ldq, const f
                                             void* stream) {
   RQB_CHECK_ARG(B >= 0 && nq > 0 && S > 0 && heads > 0, "t5dec_cross_attention: bad shape (B=%d nq=%d S=%d heads=%d)", B, nq,
                 S, heads);
-  if (nq > XA_MAX_NQ || B > 65535) {
-    rqb_set_error("t5dec_cross_attention: need nq <= %d queries per history and B <= 65535 (nq = %d, B = %d)", XA_MAX_NQ, nq, B);
+  const int groups = (nq + XA_MAX_NQ - 1) / XA_MAX_NQ;
+  if (groups > 65535 || B > 65535) {
+    rqb_set_error("t5dec_cross_attention: need nq <= %d queries per history and B <= 65535 (nq = %d, B = %d)", 65535 * XA_MAX_NQ,
+                  nq, B);
     return RQB_ERR_UNSUPPORTED;
   }
   const int64_t inner = (int64_t)heads * T5_DKV;
   RQB_CHECK_ARG(ldq >= inner && ldkv >= inner && ldo >= inner, "t5dec_cross_attention: a leading dimension is below heads * 64");
   if (B == 0) return RQB_OK;
   RQB_CHECK_ARG(q && k && v && out, "t5dec_cross_attention: null pointer");
-  t5dec_cross_attention_kernel<<<dim3(heads, B), XA_WARPS * 32, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+  t5dec_cross_attention_kernel<<<dim3(heads, B, groups), XA_WARPS * 32, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       q, ldq, k, v, ldkv, mask, nq, S, out, ldo);
   RQB_LAUNCH_CHECK();
   return RQB_OK;

@@ -56,6 +56,8 @@ from ..data.schemas import TokenizedSeqBatch
 torch.set_float32_matmul_precision("high")
 
 MAX_CANDIDATES = 64
+#: the widest beam generate(num_beams=...) takes (the cluster selection kernels keep at most 1024 beams per history)
+MAX_NUM_BEAMS = 1024
 #: the search generate() runs when it is not given one: "sample" (the reference's sampled beam search) or "beam" (exhaustive)
 DEFAULT_SEARCH = "sample"
 SEARCHES = ("sample", "beam")
@@ -903,15 +905,29 @@ class EncoderDecoderRetrievalModel(nn.Module):
 
     def _sample_and_select(self, index: ops.SidPrefixIndex, probas: Tensor, generated: Optional[Tensor],
                            log_probas: Optional[Tensor], k: int, n_cands: int, reject: Tensor,
-                           exclude: Optional[ops.SidExclusion] = None, include: Optional[ops.SidInclusion] = None):
-        """One level of the search after the softmax: n_cands samples per beam, prefix check, scores, the k best beams."""
+                           exclude: Optional[ops.SidExclusion] = None, include: Optional[ops.SidInclusion] = None,
+                           wide: bool = False):
+        """One level of the search after the softmax: n_cands samples per beam, prefix check, scores, the k best beams
+        (``wide``: on the cluster kernel, ``SidPrefixIndex.sample_select_wide``)."""
         filt = {} if exclude is None else {"exclude": exclude}
         if include is not None:
             filt["include"] = include
-        return index.sample_select(probas, draw_exponential(probas), generated, log_probas, k, n_cands, reject=reject, **filt)
+        select = index.sample_select_wide if wide else index.sample_select
+        return select(probas, draw_exponential(probas), generated, log_probas, k, n_cands, reject=reject, **filt)
 
-    def _check_search_limits(self, search: str, k: int, n_cands: int) -> None:
+    @staticmethod
+    def _narrow_search(search: str, k: int, n_cands: int) -> bool:
+        """A search of beam width k fits the one-CTA-per-history selection kernels (``beam_topk`` / ``sample_select``)."""
+        return k <= 32 and (search == "beam" or k * n_cands <= 1024)
+
+    def _check_search_limits(self, search: str, k: int, n_cands: int, num_beams: Optional[int] = None) -> None:
         K = self.num_embeddings_per_hierarchy
+        if num_beams is not None:
+            top = MAX_NUM_BEAMS if search == "sample" else min(MAX_NUM_BEAMS, K)
+            if not 1 <= num_beams <= top or K > 2048:
+                raise Rqb200Error(f"generate: num_beams = {num_beams} with {K} codes per level is outside the {search} search's "
+                                  f"limits (1 <= num_beams <= {top}, at most 2048 codes per level)")
+            return
         if search == "sample":
             if k > 32 or k * n_cands > 1024 or K > 2048:
                 raise Rqb200Error(f"generate: top_k_for_generation = {k} (at most 32, and top_k * {n_cands} candidates at most "
@@ -1001,7 +1017,7 @@ class EncoderDecoderRetrievalModel(nn.Module):
     @torch.no_grad()
     def generate(self, attention_mask, input_ids, user_id=None, search: Optional[str] = None, decoder: Optional[str] = None,
                  encoder: Optional[str] = None, encoder_attention: Optional[str] = None, exclude_items: Optional[Tensor] = None,
-                 include_items: Optional[Tensor] = None):
+                 include_items: Optional[Tensor] = None, num_beams: Optional[int] = None):
         """Top-k semantic ids by beam search restricted to id prefixes of the corpus.  ``search`` (default: the module's
         ``DEFAULT_SEARCH``, read at call time):
           "sample"  per level, n_cands = min(64, K) tokens sampled without replacement per beam, scored by cumulative
@@ -1025,11 +1041,19 @@ class EncoderDecoderRetrievalModel(nn.Module):
         item of its history -- one in its allow-list, retrievable and not excluded; an extension without one under it is
         invalid, like a prefix the corpus lacks.  None means no restriction; a row without an eligible item gets -inf fillers
         only.  It adds one launch and no host read; ids outside [-1, N) raise ``ValueError`` after the search.
-        Returns generated [B, top_k, num_hierarchies] and log_probas [B, top_k]."""
+        ``num_beams`` (default None: ``top_k_for_generation``, with its limits) is the beam width w of this call:
+        1 <= w <= min(1024, K) for "beam", 1 <= w <= 1024 for "sample" (still n_cands samples per beam), K <= 2048; outside
+        them ``Rqb200Error`` before any launch.  Widths the one-CTA-per-history selection kernels take (w <= 32, and
+        w * n_cands <= 1024 for "sample") run on them; wider ones select each level on one thread-block cluster per history
+        (``SidPrefixIndex.beam_topk_wide`` / ``sample_select_wide``), with the same rules.  The fused decoder's self-attention
+        cache is [layers, 2, H, B * w, inner] fp32; the HF decoder repeats the encoder output w times per history.
+        Returns generated [B, w, num_hierarchies] and log_probas [B, w]."""
         return self._generate(attention_mask, input_ids, user_id, search, decoder, encoder, encoder_attention,
-                              self._filters(exclude_items, include_items, attention_mask.shape[0], attention_mask.device))
+                              self._filters(exclude_items, include_items, attention_mask.shape[0], attention_mask.device),
+                              num_beams)
 
-    def _generate(self, attention_mask, input_ids, user_id, search, decoder, encoder, encoder_attention, filters: list):
+    def _generate(self, attention_mask, input_ids, user_id, search, decoder, encoder, encoder_attention, filters: list,
+                  num_beams: Optional[int] = None):
         decoder = _choice(decoder, DEFAULT_DECODER, DECODERS, "generate", "decoder")
         if decoder == "fused" and self.training:
             raise ValueError("generate: decoder=\"fused\" runs the decoder in eval mode only; call model.eval() first (in "
@@ -1040,10 +1064,12 @@ class EncoderDecoderRetrievalModel(nn.Module):
             raise ValueError("generate: encoder=\"fused\" runs the encoder in eval mode only; call model.eval() first (in "
                              "training mode HF's encoder applies dropout)")
         search = _choice(search, DEFAULT_SEARCH, SEARCHES, "generate", "search")
-        k = self.top_k_for_generation
+        num_beams = None if num_beams is None else int(num_beams)
+        k = self.top_k_for_generation if num_beams is None else num_beams
         n_cands = min(MAX_CANDIDATES, self.num_embeddings_per_hierarchy)
-        self._check_search_limits(search, k, n_cands)
+        self._check_search_limits(search, k, n_cands, num_beams)
         beam = search == "beam"
+        wide = not self._narrow_search(search, k, n_cands)
         if encoder == "fused":
             # "fp32" without an argument: a caller may have replaced _fused_encoder with a function of none
             fused_encoder = self._fused_encoder() if att == "fp32" else self._fused_encoder(att)
@@ -1068,7 +1094,11 @@ class EncoderDecoderRetrievalModel(nn.Module):
                     attention_mask_for_encoder=enc_mask if first else rep_mask, use_cache=True, past_key_values=past_kv)
                 logits = self.decoder_mlp[h](dec_out[:, -1, :])
             if beam:
-                generated, log_probas, parent_global = index.beam_topk(logits, generated, log_probas, k, bad=reject, **filt)
+                topk = index.beam_topk_wide if wide else index.beam_topk
+                generated, log_probas, parent_global = topk(logits, generated, log_probas, k, bad=reject, **filt)
+            elif wide:
+                generated, log_probas, parent_global = self._sample_and_select(index, F.softmax(logits, dim=-1), generated,
+                                                                               log_probas, k, n_cands, reject, wide=True, **filt)
             else:
                 generated, log_probas, parent_global = self._sample_and_select(index, F.softmax(logits, dim=-1), generated,
                                                                                log_probas, k, n_cands, reject, **filt)
@@ -1100,11 +1130,11 @@ class EncoderDecoderRetrievalModel(nn.Module):
                              batch.sem_ids.device)
 
     def _generate_batch(self, batch: TokenizedSeqBatch, search, decoder, encoder, encoder_attention,
-                        filters: list) -> GenerationOutput:
+                        filters: list, num_beams: Optional[int] = None) -> GenerationOutput:
         H = self.num_hierarchies
         generated, log_probas = self._generate(_strip_dedup_col(batch.seq_mask.long(), H + 1, H),
                                                _strip_dedup_col(batch.sem_ids, H + 1, H), batch.user_ids, search, decoder,
-                                               encoder, encoder_attention, filters)
+                                               encoder, encoder_attention, filters, num_beams)
         return GenerationOutput(sem_ids=generated, log_probas=log_probas)
 
     @torch.no_grad()
@@ -1112,27 +1142,31 @@ class EncoderDecoderRetrievalModel(nn.Module):
                              search: Optional[str] = None, decoder: Optional[str] = None,
                              encoder: Optional[str] = None, encoder_attention: Optional[str] = None,
                              exclude_items: Optional[Tensor] = None, exclude_history: Optional[bool] = None,
-                             include_items: Optional[Tensor] = None) -> GenerationOutput:
-        """``generate`` on the batch's histories.  ``exclude_items`` and ``include_items`` as in ``generate``;
+                             include_items: Optional[Tensor] = None, num_beams: Optional[int] = None) -> GenerationOutput:
+        """``generate`` on the batch's histories.  ``exclude_items``, ``include_items`` and ``num_beams`` as in ``generate``;
         ``exclude_history`` (default ``DEFAULT_EXCLUDE_HISTORY``, read at call time) also excludes each history's own items
         (``history_items``)."""
         return self._generate_batch(batch, search, decoder, encoder, encoder_attention,
-                                    self._batch_filters(batch, exclude_items, exclude_history, include_items))
+                                    self._batch_filters(batch, exclude_items, exclude_history, include_items), num_beams)
 
     @torch.no_grad()
     def generate_items(self, batch: TokenizedSeqBatch, n: Optional[int] = None, search: Optional[str] = None,
                        decoder: Optional[str] = None, encoder: Optional[str] = None,
                        encoder_attention: Optional[str] = None, exclude_items: Optional[Tensor] = None,
-                       exclude_history: Optional[bool] = None, include_items: Optional[Tensor] = None) -> ItemGenerationOutput:
+                       exclude_history: Optional[bool] = None, include_items: Optional[Tensor] = None,
+                       num_beams: Optional[int] = None) -> ItemGenerationOutput:
         """The top corpus items for each history: ``generate_next_sem_id``'s beams, unchanged, then one launch that takes the
         items of every finite beam whose ids are in the corpus, beam by beam in descending score order, each beam's items by
-        dedup rank, no item twice, at most n (default top_k_for_generation) per history.  ``exclude_items`` /
-        ``exclude_history`` as in ``generate_next_sem_id``: the search and the retrieval both leave the excluded items out.
-        ``include_items`` as in ``generate``: the search and the retrieval both return only each history's eligible items."""
+        dedup rank, no item twice, at most n (default: the call's beam width, ``num_beams`` or else top_k_for_generation; at
+        most ``ops.SidItemTable.MAX_N``) per history.  ``exclude_items`` / ``exclude_history`` as in
+        ``generate_next_sem_id``: the search and the retrieval both leave the excluded items out.  ``include_items`` as in
+        ``generate``: the search and the retrieval both return only each history's eligible items.  ``num_beams`` as in
+        ``generate``: a wider search yields more candidate items (``n`` up to 4096)."""
         filters = self._batch_filters(batch, exclude_items, exclude_history, include_items)
-        out = self._generate_batch(batch, search, decoder, encoder, encoder_attention, filters)
+        out = self._generate_batch(batch, search, decoder, encoder, encoder_attention, filters, num_beams)
         table = self._item_table(out.sem_ids.device)
-        items, beams, count = table.retrieve(out.sem_ids, out.log_probas, self.top_k_for_generation if n is None else n,
+        width = self.top_k_for_generation if num_beams is None else num_beams
+        items, beams, count = table.retrieve(out.sem_ids, out.log_probas, width if n is None else n,
                                              **self._filter_kwargs(filters))
         return ItemGenerationOutput(item_ids=items, beams=beams, count=count, sem_ids=out.sem_ids, log_probas=out.log_probas)
 

@@ -675,6 +675,22 @@ class SidPrefixIndex:
         exactly like prefixes the corpus lacks; the samples do not change.  ``include`` (``sid_inclusion_build``, one allow-list
         per history, any exclusion folded in; not with ``exclude``): extensions to a prefix without an eligible item of the
         history are invalid alike."""
+        return self._sample_select("sid_trie_sample_select", probas, noise, generated, log_probas, k, nc, want_samples, reject,
+                                   exclude, include)
+
+    def sample_select_wide(self, probas: torch.Tensor, noise: torch.Tensor, generated: Optional[torch.Tensor],
+                           log_probas: Optional[torch.Tensor], k: int, nc: int, want_samples: bool = False,
+                           reject: Optional[torch.Tensor] = None, exclude: Optional["SidExclusion"] = None,
+                           include: Optional["SidInclusion"] = None, cluster: int = 0):
+        """``sample_select`` for up to 1024 beams per history (rqb200_sid_trie_sample_select_wide): one thread-block cluster per
+        history, one launch.  Same arguments and results, bit for bit wherever both run; kp <= 1024, k <= 1024, nc <= 64.  When
+        k > kp * nc the slots past kp * nc repeat candidate 0 with -inf.  ``cluster``: CTAs per history (1, 2, 4 or 8; 0
+        chooses); no result depends on it."""
+        return self._sample_select("sid_trie_sample_select_wide", probas, noise, generated, log_probas, k, nc, want_samples,
+                                   reject, exclude, include, int(cluster))
+
+    def _sample_select(self, entry: str, probas, noise, generated, log_probas, k: int, nc: int, want_samples: bool, reject,
+                       exclude, include, cluster: Optional[int] = None):
         _need_cuda(probas, noise, reject)
         if generated is None:
             B, kp, h = probas.shape[0], 1, 0
@@ -697,11 +713,17 @@ class SidPrefixIndex:
         out_parent = torch.empty((B * k,), dtype=torch.int64, device=dev)
         samples = torch.empty((B * kp, nc), dtype=torch.int64, device=dev) if want_samples else None
         samp_log_p = torch.empty((B * kp, nc), dtype=torch.float32, device=dev) if want_samples else None
-        name, filt = _filter_entry("sid_trie_sample_select", exclude, include, B, h + 1, "sample_select")
+        name, filt = _filter_entry(entry, exclude, include, B, h + 1, entry[9:])
+        lib = _lib.load()
+        wide = ()
+        if cluster is not None:                               # the wide entry: its workspace and the cluster size
+            ws_bytes = lib.rqb200_sid_trie_sample_select_wide_workspace_bytes(B, kp, nc)
+            ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
+            wide = (_p(ws), ws_bytes, cluster)
         with torch.cuda.device(dev):
-            _lib.check(getattr(_lib.load(), "rqb200_" + name)(
+            _lib.check(getattr(lib, "rqb200_" + name)(
                 _p(probas), probas.stride(0), _p(noise), noise.stride(0), _p(generated), _p(log_probas), B, kp, nc, h, k, self.C,
-                self.K, _p(self.ws), _p(out_g), _p(out_p), _p(out_parent), _p(samples), _p(samp_log_p), _p(reject), *filt,
+                self.K, _p(self.ws), _p(out_g), _p(out_p), _p(out_parent), _p(samples), _p(samp_log_p), _p(reject), *wide, *filt,
                 _stream()), name)
         _count(1)
         if want_samples:
@@ -718,6 +740,18 @@ class SidPrefixIndex:
         best in descending order, equal scores by ascending beam * K + code.  Deterministic.  ``bad``, an int32 device tensor,
         is ADDED the number of beam rows whose logits hold a NaN or +inf or are all -inf.  ``exclude`` / ``include`` as in
         ``sample_select``: extensions to a prefix blocked for the history, or without an eligible item of it, score -inf."""
+        return self._beam_topk("sid_trie_beam_topk", logits, generated, log_probas, k, bad, exclude, include)
+
+    def beam_topk_wide(self, logits: torch.Tensor, generated: Optional[torch.Tensor], log_probas: Optional[torch.Tensor], k: int,
+                       bad: Optional[torch.Tensor] = None, exclude: Optional["SidExclusion"] = None,
+                       include: Optional["SidInclusion"] = None, cluster: int = 0):
+        """``beam_topk`` for up to 1024 beams per history (rqb200_sid_trie_beam_topk_wide): one thread-block cluster per history,
+        one launch.  Same arguments and results, bit for bit wherever both run; kp <= 1024, k <= min(1024, K).  ``cluster``:
+        CTAs per history (1, 2, 4 or 8; 0 chooses); no result depends on it."""
+        return self._beam_topk("sid_trie_beam_topk_wide", logits, generated, log_probas, k, bad, exclude, include, int(cluster))
+
+    def _beam_topk(self, entry: str, logits, generated, log_probas, k: int, bad, exclude, include,
+                   cluster: Optional[int] = None):
         _need_cuda(logits, bad)
         if generated is None:
             B, kp, h = logits.shape[0], 1, 0
@@ -738,11 +772,12 @@ class SidPrefixIndex:
         out_g = torch.empty((B, k, h + 1), dtype=torch.int64, device=dev)
         out_p = torch.empty((B, k), dtype=torch.float32, device=dev)
         out_parent = torch.empty((B * k,), dtype=torch.int64, device=dev)
-        name, filt = _filter_entry("sid_trie_beam_topk", exclude, include, B, h + 1, "beam_topk")
+        name, filt = _filter_entry(entry, exclude, include, B, h + 1, entry[9:])
+        wide = () if cluster is None else (cluster,)
         with torch.cuda.device(dev):
             _lib.check(getattr(_lib.load(), "rqb200_" + name)(
                 _p(logits), logits.stride(0), _p(generated), _p(log_probas), B, kp, h, k, self.C, self.K, _p(self.ws), _p(out_g),
-                _p(out_p), _p(out_parent), _p(bad), *filt, _stream()), name)
+                _p(out_p), _p(out_parent), _p(bad), *wide, *filt, _stream()), name)
         _count(1)
         return out_g, out_p, out_parent
 
