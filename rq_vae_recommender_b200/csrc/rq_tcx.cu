@@ -71,7 +71,6 @@ static_assert(TX_REG_LAUNCH * TX_THREADS <= 65536 && TX_REG_SCORER >= TX_REG_LAU
                   TX_REG_PRODUCER <= TX_REG_LAUNCH && TX_REG_SCORER + TX_REG_HELPER + TX_REG_PRODUCER <= 3 * TX_REG_LAUNCH,
               "setmaxnreg budgets must fit the registers the CTA is launched with");
 #define TX_SMEM_LIMIT 232448                      // 227 KB of opt-in shared memory per block
-#define TX_GC 4                                   // column groups per chunk of Gram-row loads in tx_score (8 spills)
 
 struct TxSmem {
   uint64_t full[TX_NB_MAX], empty[TX_NB_MAX];
@@ -273,8 +272,10 @@ __device__ __forceinline__ void tx_mma(float (&acc)[128], TxSmem* ms, uint32_t x
 }
 
 // score the block of codes [col, col + 256) of a level of K codes: h = T - S / 2^s in place; columns col + 8 jb + 2 q4 + {0, 1}
-// of rows r0 (acc[4 jb + 0..1]) and r1 (acc[4 jb + 2..3])
-template <class Id>
+// of rows r0 (acc[4 jb + 0..1]) and r1 (acc[4 jb + 2..3]).  GC = column groups per chunk of Gram-row loads: 16 (two chunks)
+// in the K = 256 kernel, 1.7 % shorter step on the H100 together with its early level constants; 4 in the blocked
+// kernel, which was 8-18 % slower at 16 (bench_large_k.py)
+template <int GC, class Id>
 __device__ __forceinline__ void tx_score(float (&acc)[128], const TxParams& p, const TcLevelConst& lc, int l, int col, int K,
                                          const Id* ids, int r0, int r1) {
   const int q4 = threadIdx.x & 3;
@@ -287,17 +288,17 @@ __device__ __forceinline__ void tx_score(float (&acc)[128], const TxParams& p, c
       acc[4 * jb + 2] = fmaf(acc[4 * jb + 2], ninv, t.x); acc[4 * jb + 3] = fmaf(acc[4 * jb + 3], ninv, t.y);
     }
   } else {
-    // Gram rows of the previous levels' ids, table (j, l) at gram + (l (l - 1) / 2 + j) K^2, summed in level order.  TX_GC
+    // Gram rows of the previous levels' ids, table (j, l) at gram + (l (l - 1) / 2 + j) K^2, summed in level order.  GC
     // column groups at a time: the loads of one table are independent, so a level costs l round trips to L2 per chunk rather
     // than one per column group and table
     const float* g0 = p.gram + (size_t)(l * (l - 1) / 2) * K * K + 2 * q4 + col;
     const float* a0 = g0 + (size_t)ids[r0] * K;
     const float* a1 = g0 + (size_t)ids[r1] * K;
 #pragma unroll
-    for (int jc = 0; jc < 32; jc += TX_GC) {
-      float2 t0[TX_GC], t1[TX_GC];
+    for (int jc = 0; jc < 32; jc += GC) {
+      float2 t0[GC], t1[GC];
 #pragma unroll
-      for (int i = 0; i < TX_GC; ++i) {
+      for (int i = 0; i < GC; ++i) {
         t0[i] = __ldg(reinterpret_cast<const float2*>(a0 + 8 * (jc + i)));
         t1[i] = __ldg(reinterpret_cast<const float2*>(a1 + 8 * (jc + i)));
       }
@@ -306,14 +307,14 @@ __device__ __forceinline__ void tx_score(float (&acc)[128], const TxParams& p, c
         const float* b0 = g0 + ((size_t)j * K + ids[j * TX_R + r0]) * K;
         const float* b1 = g0 + ((size_t)j * K + ids[j * TX_R + r1]) * K;
 #pragma unroll
-        for (int i = 0; i < TX_GC; ++i) {
+        for (int i = 0; i < GC; ++i) {
           const float2 u0 = __ldg(reinterpret_cast<const float2*>(b0 + 8 * (jc + i)));
           const float2 u1 = __ldg(reinterpret_cast<const float2*>(b1 + 8 * (jc + i)));
           t0[i].x += u0.x; t0[i].y += u0.y; t1[i].x += u1.x; t1[i].y += u1.y;
         }
       }
 #pragma unroll
-      for (int i = 0; i < TX_GC; ++i) {
+      for (int i = 0; i < GC; ++i) {
         const int jb = jc + i;
         acc[4 * jb + 0] = fmaf(acc[4 * jb + 0], ninv, t0[i].x); acc[4 * jb + 1] = fmaf(acc[4 * jb + 1], ninv, t0[i].y);
         acc[4 * jb + 2] = fmaf(acc[4 * jb + 2], ninv, t1[i].x); acc[4 * jb + 3] = fmaf(acc[4 * jb + 3], ninv, t1[i].y);
@@ -557,17 +558,20 @@ __global__ void __launch_bounds__(TX_THREADS, 1) rq_tcx_kernel(const __grid_cons
     mbar_wait_guarded(&sh.ms->img_full, n & 1, 5);
 #pragma unroll 1
     for (uint32_t l = 0; l < L; ++l) {
+      // the level's constants and the rows' candidate margins before the MMAs, whose wait hides the header's load (rowinfo
+      // holds this tile's statistics until the last level's Q_READY)
+      const TcLevelConst lc = p.hdr->lv[l];
+      const float mg0 = tx_margin(lc, sh.ms->rowinfo[r0]), mg1 = tx_margin(lc, sh.ms->rowinfo[r1]);
       float acc[128];
       tx_mma(acc, sh.ms, x_base, c_base, p.nkc, (uint32_t)p.nb, s);
       if (l + 1 == L) mbar_arrive(&sh.ms->img_free);       // the helper may convert the next tile
       // ids, candidate words and queue of the level before are drained by its re-rank
       if (n | l) mbar_wait_guarded(&sh.ms->rr_done, (n * L + l - 1) & 1, 6);
-      const TcLevelConst lc = p.hdr->lv[l];
-      tx_score(acc, p, lc, l, 0, TC_K, sh.ids, r0, r1);
+      tx_score<16>(acc, p, lc, l, 0, TC_K, sh.ids, r0, r1);
       // ---- candidates: the row minimum, then the 8 candidate words in registers; only a queued row stores its words
       float m0, m1;
       tx_quad_min(acc, m0, m1);
-      const float thr0 = m0 + tx_margin(lc, sh.ms->rowinfo[r0]), thr1 = m1 + tx_margin(lc, sh.ms->rowinfo[r1]);
+      const float thr0 = m0 + mg0, thr1 = m1 + mg1;
       uint32_t w0[8], w1[8];
       int cnt0 = 0, cnt1 = 0, first0 = TC_K, first1 = TC_K;
 #pragma unroll
@@ -617,7 +621,7 @@ __global__ void __launch_bounds__(TX_THREADS, 1) rq_tcx_blocked_kernel(const __g
         // ids, candidate words and queue of the level before are drained by its re-rank
         if (cb == 0 && (n | l)) mbar_wait_guarded(&sh.ms->rr_done, (n * L + l - 1) & 1, 6);
         const TcLevelConst lc = p.hdr->lv[l];
-        tx_score(acc, p, lc, l, cb * TC_K, K, sh.ids, r0, r1);
+        tx_score<4>(acc, p, lc, l, cb * TC_K, K, sh.ids, r0, r1);
         // ---- candidates: the block minimum, the running minimum, then the block's candidate words to shared memory
         float m0, m1;
         tx_quad_min(acc, m0, m1);
