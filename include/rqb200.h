@@ -464,6 +464,61 @@ int rqb200_t5rank_select_excluding(const float* scores, int B, int U, const int*
 int rqb200_t5score_trie_build(const int64_t* ids, int B, int C, int H, int K, int* counts, int* code, int* parent, int* child,
                               int* leaf, void* stream);
 
+/* ---- exact top-k search (modules/model.py generate(search="exact"), FusedT5Exact), csrc/t5rank.cu ----
+ * t5rank_cross_attention_ragged : t5rank_cross_attention over a ragged level: T query tiles, tile t = tiles[3 t ..] (int32:
+ *                          history b, first query row, query count <= 64), each over history b's keys; a query's arithmetic is
+ *                          that of the uniform fp32 kernel.  Limits: heads <= 65535.
+ * t5exact_frontier       : one CTA per history b of Bc over its scored children, nodes of trie level l (1 <= l < 8): entries
+ *                          coff[b] .. coff[b + 1] - 1 of sc / cnode / ccode / cpar (fp32 score, node id, last code, parent row), or
+ *                          with cnode null (l = 1, the root's children) entries b n_root .. of sc, child i being node i (code
+ *                          ccode[i], parent row b).  A child is kept when sc >= tau[b] (NaN never) and the filter does not block its
+ *                          prefix key pkey[parent] K + code (pkey int64 [rows], null at l = 1; needed with a filter).  Count pass
+ *                          (counts int32 [3, Bc], offs null): per history the kept rows, their children (lchild: the child ranges of
+ *                          level l, int32 [n_l + 1]) and their 64-query tiles.  Write pass (offs int32 [3, Bc + 1], the exclusive
+ *                          scans of counts, counts null): kept row r (trie order, history b's at offs[0][b] ..) gets row_code /
+ *                          row_par int64, row_score fp32, row_key int64 (with a filter), row_node int32; tiles int32 [T, 3] for
+ *                          t5rank_cross_attention_ragged; nrng int32 [R + 1] the rows' child ranges (global, for t5rank_children
+ *                          as one group), and per child g: nnode (node of level l + 1), ncode (lcode_next[node]), npar (row).
+ *                          b0: the chunk's first history in the filter.  Plain stores: the output is a function of the input.
+ * t5exact_select         : one CTA per history b over its leaf candidates (coff / cnode / n_root as t5exact_frontier's children,
+ *                          cnode the leaf ids; max_u the largest count): the w best by (score descending, leaf ascending), NaN and
+ *                          filter-blocked leaves (level H keys leaf_key[leaf], int64 [U]; needed with a filter) left out.  out_gen
+ *                          int64 [Bc, w, H] each chosen leaf's tuple along its path (codes / parents: host arrays of H + 1 device
+ *                          pointers, entry l = SidTrieLevels.code[l] / parent[l]), out_lp fp32 [Bc, w] its score; -1 / -inf past
+ *                          the valid candidates.  w <= 1024, H <= 8 (RQB_ERR_UNSUPPORTED).  No global atomics.
+ * _excluding / _including take an exclusion set (sid_exclusion_build) / an allow-list (sid_inclusion_build) of the whole batch
+ * (history b0 + b) after the other arguments, as the search kernels. */
+int rqb200_t5rank_cross_attention_ragged(const float* q, int64_t ldq, const float* k, const float* v, int64_t ldkv, const int* offsets,
+                                         const float* key_mask, const int* tiles, int T, int heads, float* out, int64_t ldo,
+                                         void* stream);
+int rqb200_t5exact_frontier(const float* sc, const int* coff, int n_root, const int* cnode, const int* ccode, const int* cpar,
+                            const int64_t* pkey, const float* tau, int Bc, int K, int l, const int* lchild, const int* lcode_next,
+                            int b0, int* counts, const int* offs, int64_t* row_code, int64_t* row_par, float* row_score,
+                            int64_t* row_key, int* row_node, int* tiles, int* nrng, int* nnode, int* ncode, int* npar, void* stream);
+int rqb200_t5exact_frontier_excluding(const float* sc, const int* coff, int n_root, const int* cnode, const int* ccode,
+                                      const int* cpar, const int64_t* pkey, const float* tau, int Bc, int K, int l, const int* lchild,
+                                      const int* lcode_next, int b0, int* counts, const int* offs, int64_t* row_code,
+                                      int64_t* row_par, float* row_score, int64_t* row_key, int* row_node, int* tiles, int* nrng,
+                                      int* nnode, int* ncode, int* npar, const int* ex_pos, const int64_t* ex_blocked,
+                                      const int* ex_count, int ex_M, int ex_H, void* stream);
+int rqb200_t5exact_frontier_including(const float* sc, const int* coff, int n_root, const int* cnode, const int* ccode,
+                                      const int* cpar, const int64_t* pkey, const float* tau, int Bc, int K, int l, const int* lchild,
+                                      const int* lcode_next, int b0, int* counts, const int* offs, int64_t* row_code,
+                                      int64_t* row_par, float* row_score, int64_t* row_key, int* row_node, int* tiles, int* nrng,
+                                      int* nnode, int* ncode, int* npar, const int* in_pos, const int64_t* in_keys,
+                                      const int* in_count, int in_M, int in_H, void* stream);
+int rqb200_t5exact_select(const float* sc, const int* coff, int n_root, const int* cnode, int max_u, const int64_t* leaf_key,
+                          const void* const* codes, const void* const* parents, int Bc, int H, int w, int b0, int64_t* out_gen,
+                          float* out_lp, void* stream);
+int rqb200_t5exact_select_excluding(const float* sc, const int* coff, int n_root, const int* cnode, int max_u,
+                                    const int64_t* leaf_key, const void* const* codes, const void* const* parents, int Bc, int H,
+                                    int w, int b0, int64_t* out_gen, float* out_lp, const int* ex_pos, const int64_t* ex_blocked,
+                                    const int* ex_count, int ex_M, int ex_H, void* stream);
+int rqb200_t5exact_select_including(const float* sc, const int* coff, int n_root, const int* cnode, int max_u,
+                                    const int64_t* leaf_key, const void* const* codes, const void* const* parents, int Bc, int H,
+                                    int w, int b0, int64_t* out_gen, float* out_lp, const int* in_pos, const int64_t* in_keys,
+                                    const int* in_count, int in_M, int in_H, void* stream);
+
 /* ---- one step of the generative-retrieval model's T5 decoder (modules/model.py, generate(decoder="fused")), csrc/t5dec.cu ----
  * HF T5 numerics in eval mode: attention without 1/sqrt(d) scaling, fp32 softmax, d_kv = 64 per head (inner = heads * 64).
  * The GEMMs around these calls are the caller's.  fp32 throughout; strides in elements.

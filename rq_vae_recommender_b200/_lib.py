@@ -126,6 +126,13 @@ _SIGNATURES = {
     "rqb200_t5rank_select_excluding": (c_int, [c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp,
                                                c_vp, c_int, c_int, c_vp]),
     "rqb200_t5score_trie_build": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "rqb200_t5rank_cross_attention_ragged": (c_int, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_i64, c_vp]),
+    "rqb200_t5exact_frontier": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "rqb200_t5exact_frontier_excluding": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
+    "rqb200_t5exact_frontier_including": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
+    "rqb200_t5exact_select": (c_int, [c_vp, c_vp, c_int, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
+    "rqb200_t5exact_select_excluding": (c_int, [c_vp, c_vp, c_int, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
+    "rqb200_t5exact_select_including": (c_int, [c_vp, c_vp, c_int, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
     "rqb200_t5dec_cross_attention": (c_int, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_int, c_int, c_int, c_int, c_vp, c_i64,
                                              c_vp]),
     "rqb200_t5dec_self_attention": (c_int, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int,

@@ -50,18 +50,37 @@ __global__ void __launch_bounds__(RK_WARPS * 32) t5rank_cross_attention_kernel(
     const float* __restrict__ q, int64_t ldq, const float* __restrict__ k, const float* __restrict__ v, int64_t ldkv,
     const int* __restrict__ offsets, const float* __restrict__ key_mask, int Q, float* __restrict__ out, int64_t ldo);
 
-template <>
-__global__ void __launch_bounds__(RK_WARPS * 32) t5rank_cross_attention_kernel<false>(
-    const float* __restrict__ q, int64_t ldq, const float* __restrict__ k, const float* __restrict__ v, int64_t ldkv,
-    const int* __restrict__ offsets, const float* __restrict__ key_mask, int Q, float* __restrict__ out, int64_t ldo) {
+// One fp32 query tile, head n = blockIdx.y, over history b's keys: queries qrow0 .. qrow0 + nq - 1 of q / out (nq <= 64).  The
+// uniform kernel (RAGGED false: tile blockIdx.x of history blockIdx.z) and the ragged one (t5rank_cross_attention_ragged_kernel:
+// tile blockIdx.x of the tile table) differ only in how a CTA finds (b, qrow0, nq), so a query's arithmetic does not depend on
+// the layout.
+template <bool RAGGED>
+__device__ __forceinline__ void rk_cross_attention_tile(const float* __restrict__ q, int64_t ldq, const float* __restrict__ k,
+                                                        const float* __restrict__ v, int64_t ldkv, const int* __restrict__ offsets,
+                                                        const float* __restrict__ key_mask, int Q, const int* __restrict__ tiles,
+                                                        float* __restrict__ out, int64_t ldo) {
   __shared__ float sq[RK_QTILE][RK_DKV];
   __shared__ float sk[RK_KTILE][RK_DKV + 1];   // +1: lane j reads row j, column d -> distinct banks
   __shared__ float sv[RK_KTILE][RK_DKV];
   __shared__ float sbias[RK_KTILE];
-  const int q0 = blockIdx.x * RK_QTILE, n = blockIdx.y, b = blockIdx.z;
-  const int nq = min(RK_QTILE, Q - q0);
+  int n, b, nq;
+  int64_t col, qrow0;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int64_t col = (int64_t)n * RK_DKV, qrow0 = (int64_t)b * Q + q0;
+  if (RAGGED) {
+    const int* tile = tiles + 3 * (int64_t)blockIdx.x;
+    n = blockIdx.y;
+    b = tile[0];
+    nq = tile[2];
+    col = (int64_t)n * RK_DKV;
+    qrow0 = tile[1];
+  } else {
+    const int q0 = blockIdx.x * RK_QTILE;
+    n = blockIdx.y;
+    b = blockIdx.z;
+    nq = min(RK_QTILE, Q - q0);
+    col = (int64_t)n * RK_DKV;
+    qrow0 = (int64_t)b * Q + q0;
+  }
   for (int i = threadIdx.x; i < RK_QTILE * RK_DKV; i += blockDim.x) {
     const int r = i / RK_DKV, d = i % RK_DKV;
     sq[r][d] = r < nq ? q[(qrow0 + r) * ldq + col + d] : 0.f;
@@ -119,6 +138,22 @@ __global__ void __launch_bounds__(RK_WARPS * 32) t5rank_cross_attention_kernel<f
     o[lane] = l[t] > 0.f ? acc0[t] / l[t] : 0.f;            // a history without keys gets zeros
     o[lane + 32] = l[t] > 0.f ? acc1[t] / l[t] : 0.f;
   }
+}
+
+template <>
+__global__ void __launch_bounds__(RK_WARPS * 32) t5rank_cross_attention_kernel<false>(
+    const float* __restrict__ q, int64_t ldq, const float* __restrict__ k, const float* __restrict__ v, int64_t ldkv,
+    const int* __restrict__ offsets, const float* __restrict__ key_mask, int Q, float* __restrict__ out, int64_t ldo) {
+  rk_cross_attention_tile<false>(q, ldq, k, v, ldkv, offsets, key_mask, Q, nullptr, out, ldo);
+}
+
+// grid (T, heads): a ragged level, history b's queries the rows roff[b] .. roff[b + 1] - 1 of q.  Tile t is tiles[3 t ..] =
+// (history, first query row, query count <= 64), as t5exact_frontier_kernel writes them.
+__global__ void __launch_bounds__(RK_WARPS * 32) t5rank_cross_attention_ragged_kernel(
+    const float* __restrict__ q, int64_t ldq, const float* __restrict__ k, const float* __restrict__ v, int64_t ldkv,
+    const int* __restrict__ offsets, const float* __restrict__ key_mask, const int* __restrict__ tiles, float* __restrict__ out,
+    int64_t ldo) {
+  rk_cross_attention_tile<true>(q, ldq, k, v, ldkv, offsets, key_mask, 0, tiles, out, ldo);
 }
 
 
@@ -276,6 +311,25 @@ extern "C" int rqb200_t5rank_cross_attention_tc(const float* q, int64_t ldq, con
                             stream);
 }
 
+extern "C" int rqb200_t5rank_cross_attention_ragged(const float* q, int64_t ldq, const float* k, const float* v, int64_t ldkv,
+                                                    const int* offsets, const float* key_mask, const int* tiles, int T, int heads,
+                                                    float* out, int64_t ldo, void* stream) {
+  RQB_CHECK_ARG(T >= 0 && heads > 0 && ldq >= (int64_t)heads * RK_DKV && ldkv >= (int64_t)heads * RK_DKV &&
+                    ldo >= (int64_t)heads * RK_DKV,
+                "t5rank_cross_attention_ragged: bad argument (T = %d, heads = %d)", T, heads);
+  if (heads > 65535) {
+    rqb_set_error("t5rank_cross_attention_ragged: need heads <= 65535 (heads = %d)", heads);
+    return RQB_ERR_UNSUPPORTED;
+  }
+  if (T == 0) return RQB_OK;
+  RQB_CHECK_ARG(q && k && v && offsets && tiles && out, "t5rank_cross_attention_ragged: null pointer");
+  t5rank_cross_attention_ragged_kernel<<<dim3((unsigned)T, (unsigned)heads), RK_WARPS * 32, 0,
+                                         reinterpret_cast<cudaStream_t>(stream)>>>(q, ldq, k, v, ldkv, offsets, key_mask, tiles,
+                                                                                   out, ldo);
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
+}
+
 // ------------------------------------------------------------------------------------------------ children scores
 // One warp per node row r = b * n_h + i of logits [R, K].  lse as sid_beam_topk_kernel: m = max, sum of expf(x - m) over c = lane,
 // lane + 32, ... then an xor butterfly (every lane ends with the same bits), lse = m + logf(sum).  Child j of node i (child[i] <=
@@ -355,75 +409,26 @@ struct RkBlockedCursor {
   }
 };
 
-template <bool KEYS_IN_SMEM, bool EXCL>
-__global__ void __launch_bounds__(RK_SEL_THREADS) t5rank_select_kernel(
-    const float* __restrict__ scores, int U, const int* __restrict__ row, const int* __restrict__ start,
-    const int64_t* __restrict__ t_leaf, const int64_t* __restrict__ t_dedup, int n, int64_t* __restrict__ out_items,
-    float* __restrict__ out_scores, int64_t* __restrict__ out_rank, SidExcl ex) {
-  using Scan = cub::BlockScan<int, RK_SEL_THREADS>;
-  using Reduce = cub::BlockReduce<long long, RK_SEL_THREADS>;
-  __shared__ union {
-    typename Scan::TempStorage scan;
-    typename Reduce::TempStorage reduce;
-  } tmp;
-  __shared__ int hist[256];
-  __shared__ int ctl[3];                                    // chosen digit, entries above its bin, entries in its bin
-  __shared__ int nsel_at, ties_base;
-  __shared__ unsigned long long sel[RK_SEL_MAX_N];
-  __shared__ int s_leaf[RK_SEL_MAX_N];
-  __shared__ int s_off[RK_SEL_MAX_N + 1];
-  __shared__ int x_leaf[EXCL ? SID_EXCL_MAX_M : 1];         // the leaf of each excluded position
-  __shared__ unsigned char x_full[EXCL ? SID_EXCL_MAX_M : 1];   // ... and whether that leaf's items are all excluded
-  __shared__ int n_blocked;
-  extern __shared__ __align__(16) unsigned int s_key[];     // [U] when KEYS_IN_SMEM
+// Radix selection of the nsel-th largest 32-bit key among entries u = 0 .. U - 1 (key_of(u); with SKIP, entries whose key is
+// RK_BLOCKED take no part): 8-bit digits from the top, stopping once the chosen bin is taken whole.  Leaves in prefix / pmask
+// the chosen key bits and in want how many entries at that prefix are taken (the caller takes the lowest-index ones).  Each pass
+// meets u in ascending order per thread, after key_of.restart().  hist [256] is zero on entry and on return; ctl holds 3 ints.
+template <bool SKIP, typename KeyOf>
+__device__ __forceinline__ void rk_radix_threshold(int U, int nsel, KeyOf& key_of, int* hist, int* ctl, unsigned int& prefix,
+                                                   unsigned int& pmask, int& want) {
   const int nt = RK_SEL_THREADS, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const unsigned int lt = (1u << lane) - 1u;
-  const int64_t b = blockIdx.x;
-  const float* sc = scores + b * U;
-  const int* xp = EXCL ? ex.pos_of(b) : nullptr;            // the history's excluded positions, ascending
-  const int nx = EXCL ? ex.npos(b) : 0;
-  for (int i = threadIdx.x; i < 256; i += nt) hist[i] = 0;
-  if (threadIdx.x == 0) {
-    nsel_at = 0;
-    ties_base = 0;
-    n_blocked = 0;
-  }
-  if (EXCL) {
-    __syncthreads();
-    for (int i = threadIdx.x; i < nx; i += nt) {
-      const int r = xp[i];
-      int lo = 0, hi = U;                                   // the leaf u with start[u] <= r < start[u + 1]
-      while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if (start[mid] <= r) lo = mid;
-        else hi = mid;
-      }
-      const int s = start[lo], e = start[lo + 1];
-      const bool full = sid_excluded_in(xp, nx, s, e) == e - s;
-      x_leaf[i] = lo;
-      x_full[i] = full ? 1 : 0;
-      if (full && (i == 0 || xp[i - 1] < s)) atomicAdd(&n_blocked, 1);   // an integer count: order does not matter
-    }
-    __syncthreads();
-  }
-  const int nsel = min(n, U - (EXCL ? n_blocked : 0));
-  if (KEYS_IN_SMEM) {
-    RkBlockedCursor cur;
-    for (int u = threadIdx.x; u < U; u += nt)
-      s_key[u] = (EXCL && cur.at(u, x_leaf, x_full, nx)) ? RK_BLOCKED : rk_score_key(sc[u]);
-  }
-  __syncthreads();
-  // radix selection of the nsel-th largest 32-bit score key (8-bit digits, stops once the chosen bin is taken whole)
-  unsigned int prefix = 0, pmask = 0;
-  int want = nsel;
+  prefix = 0;
+  pmask = 0;
+  want = nsel;
   for (int shift = 24; shift >= 0 && nsel > 0; shift -= 8) {
-    RkBlockedCursor cur;
+    key_of.restart();
     for (int base = 0; base < U; base += nt) {
       const int u = base + threadIdx.x;
       int d = 256;
       if (u < U) {
-        const unsigned int key = KEYS_IN_SMEM ? s_key[u] : (EXCL && cur.at(u, x_leaf, x_full, nx)) ? RK_BLOCKED : rk_score_key(sc[u]);
-        if ((key & pmask) == prefix && !(EXCL && key == RK_BLOCKED)) d = (int)((key >> shift) & 255u);
+        const unsigned int key = key_of(u);
+        if ((key & pmask) == prefix && !(SKIP && key == RK_BLOCKED)) d = (int)((key >> shift) & 255u);
       }
       const unsigned int same = __match_any_sync(0xffffffffu, d);
       if (d < 256 && (same & lt) == 0) atomicAdd(&hist[d], __popc(same));   // integer counts: order does not matter
@@ -465,6 +470,84 @@ __global__ void __launch_bounds__(RK_SEL_THREADS) t5rank_select_kernel(
     __syncthreads();                                        // ctl is read by every thread before the next pass writes it
     if (whole) break;
   }
+}
+
+// t5rank_select_kernel's leaf keys: from shared memory, or from the scores with the blocked-leaf cursor
+template <bool KEYS_IN_SMEM, bool EXCL>
+struct RkLeafKeys {
+  const unsigned int* s_key;
+  const float* sc;
+  const int* x_leaf;
+  const unsigned char* x_full;
+  int nx;
+  RkBlockedCursor cur;
+  __device__ __forceinline__ void restart() { cur = RkBlockedCursor(); }
+  __device__ __forceinline__ unsigned int operator()(int u) {
+    return KEYS_IN_SMEM ? s_key[u] : (EXCL && cur.at(u, x_leaf, x_full, nx)) ? RK_BLOCKED : rk_score_key(sc[u]);
+  }
+};
+
+template <bool KEYS_IN_SMEM, bool EXCL>
+__global__ void __launch_bounds__(RK_SEL_THREADS) t5rank_select_kernel(
+    const float* __restrict__ scores, int U, const int* __restrict__ row, const int* __restrict__ start,
+    const int64_t* __restrict__ t_leaf, const int64_t* __restrict__ t_dedup, int n, int64_t* __restrict__ out_items,
+    float* __restrict__ out_scores, int64_t* __restrict__ out_rank, SidExcl ex) {
+  using Scan = cub::BlockScan<int, RK_SEL_THREADS>;
+  using Reduce = cub::BlockReduce<long long, RK_SEL_THREADS>;
+  __shared__ union {
+    typename Scan::TempStorage scan;
+    typename Reduce::TempStorage reduce;
+  } tmp;
+  __shared__ int hist[256];
+  __shared__ int ctl[3];                                    // chosen digit, entries above its bin, entries in its bin
+  __shared__ int nsel_at, ties_base;
+  __shared__ unsigned long long sel[RK_SEL_MAX_N];
+  __shared__ int s_leaf[RK_SEL_MAX_N];
+  __shared__ int s_off[RK_SEL_MAX_N + 1];
+  __shared__ int x_leaf[EXCL ? SID_EXCL_MAX_M : 1];         // the leaf of each excluded position
+  __shared__ unsigned char x_full[EXCL ? SID_EXCL_MAX_M : 1];   // ... and whether that leaf's items are all excluded
+  __shared__ int n_blocked;
+  extern __shared__ __align__(16) unsigned int s_key[];     // [U] when KEYS_IN_SMEM
+  const int nt = RK_SEL_THREADS;
+  const int64_t b = blockIdx.x;
+  const float* sc = scores + b * U;
+  const int* xp = EXCL ? ex.pos_of(b) : nullptr;            // the history's excluded positions, ascending
+  const int nx = EXCL ? ex.npos(b) : 0;
+  for (int i = threadIdx.x; i < 256; i += nt) hist[i] = 0;
+  if (threadIdx.x == 0) {
+    nsel_at = 0;
+    ties_base = 0;
+    n_blocked = 0;
+  }
+  if (EXCL) {
+    __syncthreads();
+    for (int i = threadIdx.x; i < nx; i += nt) {
+      const int r = xp[i];
+      int lo = 0, hi = U;                                   // the leaf u with start[u] <= r < start[u + 1]
+      while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (start[mid] <= r) lo = mid;
+        else hi = mid;
+      }
+      const int s = start[lo], e = start[lo + 1];
+      const bool full = sid_excluded_in(xp, nx, s, e) == e - s;
+      x_leaf[i] = lo;
+      x_full[i] = full ? 1 : 0;
+      if (full && (i == 0 || xp[i - 1] < s)) atomicAdd(&n_blocked, 1);   // an integer count: order does not matter
+    }
+    __syncthreads();
+  }
+  const int nsel = min(n, U - (EXCL ? n_blocked : 0));
+  if (KEYS_IN_SMEM) {
+    RkBlockedCursor cur;
+    for (int u = threadIdx.x; u < U; u += nt)
+      s_key[u] = (EXCL && cur.at(u, x_leaf, x_full, nx)) ? RK_BLOCKED : rk_score_key(sc[u]);
+  }
+  __syncthreads();
+  unsigned int prefix, pmask;
+  int want;
+  RkLeafKeys<KEYS_IN_SMEM, EXCL> key_of{s_key, sc, x_leaf, x_full, nx};
+  rk_radix_threshold<EXCL>(U, nsel, key_of, hist, ctl, prefix, pmask, want);
   // keep every leaf above the threshold and the `want` lowest-index leaves at it (an ordered block scan over the ties), and count
   // the items of the leaves that sort before the target
   const int64_t tl = t_leaf[b];
@@ -722,3 +805,370 @@ extern "C" int rqb200_t5score_trie_build(const int64_t* ids, int B, int C, int H
   RQB_LAUNCH_CHECK();
   return RQB_OK;
 }
+
+// ------------------------------------------------------------------------------------------------ exact top-k search
+// The pruned exact decode of generate(search="exact") (modules/model.py FusedT5Exact).  A child never scores above its parent
+// (t5rank_children adds a log-probability <= 0), so with tau[b] the score of some b-th history's w-th best valid leaf already
+// known, a node scoring below tau[b] has no descendant in the exact top w.  Per level, after t5rank_children:
+//
+//   rqb200_t5exact_frontier[_excluding/_including]  one CTA per history over its scored children (nodes of trie level l): keeps
+//                                  each child with score >= tau[b] that the history's filter does not block (the binary searches of
+//                                  sid_excl.cuh in the level-l keys), block-scans the kept flags and the kept nodes' child counts,
+//                                  and writes the next decoder level's rows (ragged: history b's are roff[b] .. roff[b + 1] - 1, in
+//                                  trie order), their cross-attention query tiles, and the kept nodes' children (level l + 1) as one
+//                                  group of compact child ranges, codes, node ids and parent rows for t5rank_children.  Two phases
+//                                  from the same flags: a count pass (per history: kept rows, their children, query tiles), a scan
+//                                  and a host read of the totals by the caller, then a write pass at the scanned offsets.
+//   rqb200_t5exact_select[_excluding/_including]    one CTA per history over its leaf candidates (the children of the last
+//                                  decoded level): rk_radix_threshold selection of the w best keys rk_key64(score, candidate) --
+//                                  candidates are in leaf order, so (score descending, leaf ascending) -- with blocked and NaN leaves
+//                                  left out, then each chosen leaf's tuple (read along its trie path) and score, -1 / -inf past the
+//                                  valid candidates.
+// Plain stores only, no global atomics: each output is a function of the input.
+#define EX_THREADS 256
+
+// whether history b's level-l list of the filter holds key (ascending keys)
+__device__ __forceinline__ bool ex_listed(const SidExcl& f, int64_t b, int l, long long key) {
+  const long long* list = f.keys_of(b, l);
+  const int n = f.nkeys(b, l);
+  const int i = sid_lower_bound(list, n, key);
+  return i < n && __ldg(list + i) == key;
+}
+
+// whether the l-prefix key is invalid for history b under the consumer's filter mode
+template <int FILTER>
+__device__ __forceinline__ bool ex_blocked(const SidExcl& f, int64_t b, int l, long long key) {
+  if (FILTER == SID_FILTER_EXCLUDE) return ex_listed(f, b, l, key);
+  if (FILTER == SID_FILTER_INCLUDE) return !ex_listed(f, b, l, key);
+  return false;
+}
+
+// Children of history b: entries coff[b] .. coff[b + 1] - 1 of sc / cnode / ccode / cpar, or with cnode null (the root's children,
+// level 1) entries b n_root .. b n_root + n_root - 1 of sc, child i being node i of level 1 (code ccode[i], parent row b).
+// pkey [rows]: the prefix key of each parent row (null at level 1).  counts (count pass) int32 [3, Bc]; offs (write pass) int32
+// [3, Bc + 1], the exclusive scans of counts.
+template <int FILTER, bool WRITE>
+__global__ void __launch_bounds__(EX_THREADS) t5exact_frontier_kernel(
+    const float* __restrict__ sc, const int* __restrict__ coff, int n_root, const int* __restrict__ cnode,
+    const int* __restrict__ ccode, const int* __restrict__ cpar, const long long* __restrict__ pkey, const float* __restrict__ tau,
+    int Bc, int K, int l, const int* __restrict__ lchild, const int* __restrict__ lcode_next, SidExcl f, int b0,
+    int* __restrict__ counts, const int* __restrict__ offs, int64_t* __restrict__ row_code, int64_t* __restrict__ row_par,
+    float* __restrict__ row_score, long long* __restrict__ row_key, int* __restrict__ row_node, int* __restrict__ tiles,
+    int* __restrict__ nrng, int* __restrict__ nnode, int* __restrict__ ncode, int* __restrict__ npar) {
+  using Scan = cub::BlockScan<long long, EX_THREADS>;
+  __shared__ typename Scan::TempStorage tmp;
+  __shared__ long long carry;                               // (kept rows << 32) + their children, of the tiles before
+  const int b = blockIdx.x;
+  const int64_t bg = (int64_t)b0 + b;
+  const bool root = cnode == nullptr;
+  const int64_t cs = root ? (int64_t)b * n_root : coff[b], ce = root ? cs + n_root : coff[b + 1];
+  const float t = tau[b];
+  int roff = 0, cbase = 0, toff = 0;
+  if (WRITE) {
+    roff = offs[b];
+    cbase = offs[(Bc + 1) + b];
+    toff = offs[2 * (Bc + 1) + b];
+  }
+  if (threadIdx.x == 0) carry = 0;
+  __syncthreads();
+  for (int64_t base = cs; base < ce; base += EX_THREADS) {
+    const int64_t j = base + threadIdx.x;
+    long long flag = 0, key = 0;
+    int node = 0, code = 0, par = 0;
+    float s = 0.f;
+    if (j < ce) {
+      node = root ? (int)(j - cs) : cnode[j];
+      code = root ? ccode[node] : ccode[j];
+      par = root ? b : cpar[j];
+      s = sc[j];
+      bool keep = s >= t;                                   // NaN: never kept
+      if (FILTER != SID_FILTER_NONE) {
+        key = (root ? 0ll : pkey[par] * K) + code;
+        keep = keep && !ex_blocked<FILTER>(f, bg, l, key);
+      }
+      if (keep) flag = (1ll << 32) + (lchild[node + 1] - lchild[node]);
+    }
+    long long excl, total;
+    Scan(tmp).ExclusiveSum(flag, excl, total);
+    const long long at = carry + excl;
+    if (WRITE && flag) {
+      const int row = roff + (int)(at >> 32);
+      row_code[row] = code;
+      row_par[row] = par;
+      row_score[row] = s;
+      if (FILTER != SID_FILTER_NONE) row_key[row] = key;
+      row_node[row] = node;
+      nrng[row] = cbase + (int)(at & 0xffffffffll);
+    }
+    __syncthreads();                                        // carry read and scan storage used by every thread
+    if (threadIdx.x == 0) carry += total;
+    __syncthreads();
+  }
+  const int kept = (int)(carry >> 32), nch = (int)(carry & 0xffffffffll);
+  const int ntile = (kept + RK_QTILE - 1) / RK_QTILE;
+  if constexpr (!WRITE) {
+    if (threadIdx.x == 0) {
+      counts[b] = kept;
+      counts[Bc + b] = nch;
+      counts[2 * Bc + b] = ntile;
+    }
+  } else {
+    for (int i = threadIdx.x; i < ntile; i += EX_THREADS) {
+      int* tile = tiles + 3 * (int64_t)(toff + i);
+      tile[0] = b;
+      tile[1] = roff + i * RK_QTILE;
+      tile[2] = min(RK_QTILE, kept - i * RK_QTILE);
+    }
+    if (b == Bc - 1 && threadIdx.x == 0) nrng[roff + kept] = cbase + nch;   // the closing range entry
+    __syncthreads();                                          // this history's nrng / row_node entries are written
+    // child c of the history: in the range of the last kept row starting at or before it (ranges are ascending)
+    for (int c = threadIdx.x; c < nch; c += EX_THREADS) {
+      const int g = cbase + c;
+      int lo = 0, hi = kept;
+      while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (nrng[roff + mid] <= g) lo = mid;
+        else hi = mid;
+      }
+      const int row = roff + lo;
+      const int child = lchild[row_node[row]] + (g - nrng[row]);
+      nnode[g] = child;
+      ncode[g] = lcode_next[child];
+      npar[g] = row;
+    }
+  }
+}
+
+// t5exact_select_kernel's candidate keys: rk_score_key of the score, RK_BLOCKED for NaN and for leaves the filter blocks
+template <bool KEYS_IN_SMEM, int FILTER>
+struct ExLeafKeys {
+  const unsigned int* s_key;
+  const float* sc;
+  const int* cnode;
+  const long long* leaf_key;
+  SidExcl f;
+  int64_t b;
+  int H;
+  __device__ __forceinline__ void restart() {}
+  __device__ __forceinline__ unsigned int compute(int u) const {
+    const float s = sc[u];
+    if (s != s) return RK_BLOCKED;
+    if (FILTER != SID_FILTER_NONE && ex_blocked<FILTER>(f, b, H, leaf_key[cnode ? cnode[u] : u])) return RK_BLOCKED;
+    return rk_score_key(s);
+  }
+  __device__ __forceinline__ unsigned int operator()(int u) const { return KEYS_IN_SMEM ? s_key[u] : compute(u); }
+};
+
+// the trie's levels 1..H (SidTrieLevels): each node's last code and its node in the level above
+struct ExPath {
+  const int* code[RQB_MAX_LEVELS + 1];
+  const int* parent[RQB_MAX_LEVELS + 1];
+};
+
+template <bool KEYS_IN_SMEM, int FILTER>
+__global__ void __launch_bounds__(RK_SEL_THREADS) t5exact_select_kernel(
+    const float* __restrict__ sc, const int* __restrict__ coff, int n_root, const int* __restrict__ cnode,
+    const long long* __restrict__ leaf_key, ExPath path, int H, int w, SidExcl f, int b0, int64_t* __restrict__ out_gen,
+    float* __restrict__ out_lp) {
+  using Scan = cub::BlockScan<int, RK_SEL_THREADS>;
+  using Reduce = cub::BlockReduce<int, RK_SEL_THREADS>;
+  __shared__ union {
+    typename Scan::TempStorage scan;
+    typename Reduce::TempStorage reduce;
+  } tmp;
+  __shared__ int hist[256];
+  __shared__ int ctl[3];
+  __shared__ int nsel_at, ties_base, n_valid;
+  __shared__ unsigned long long sel[RK_SEL_MAX_N];
+  extern __shared__ __align__(16) unsigned int s_key[];     // [U] when KEYS_IN_SMEM
+  const int nt = RK_SEL_THREADS;
+  const int b = blockIdx.x;
+  const bool root = cnode == nullptr;
+  const int64_t cs = root ? (int64_t)b * n_root : coff[b];
+  const int U = root ? n_root : (int)(coff[b + 1] - cs);
+  for (int i = threadIdx.x; i < 256; i += nt) hist[i] = 0;
+  if (threadIdx.x == 0) {
+    nsel_at = 0;
+    ties_base = 0;
+  }
+  ExLeafKeys<KEYS_IN_SMEM, FILTER> key_of{s_key, sc + cs, root ? nullptr : cnode + cs, leaf_key, f, (int64_t)b0 + b, H};
+  int mine = 0;
+  for (int u = threadIdx.x; u < U; u += nt) {
+    const unsigned int key = key_of.compute(u);
+    if (KEYS_IN_SMEM) s_key[u] = key;
+    mine += key != RK_BLOCKED;
+  }
+  const int valid = Reduce(tmp.reduce).Sum(mine);
+  if (threadIdx.x == 0) n_valid = valid;
+  __syncthreads();
+  const int nsel = min(w, n_valid);
+  unsigned int prefix, pmask;
+  int want;
+  rk_radix_threshold<true>(U, nsel, key_of, hist, ctl, prefix, pmask, want);
+  // keep every candidate above the threshold and the `want` lowest-index ones at it (an ordered block scan over the ties)
+  for (int base = 0; base < U; base += nt) {
+    const int u = base + threadIdx.x;
+    const unsigned int key = u < U ? key_of(u) : RK_BLOCKED;
+    const bool in = nsel > 0 && key != RK_BLOCKED;
+    const bool above = in && (key & pmask) > prefix;
+    const int tie = (in && (key & pmask) == prefix) ? 1 : 0;
+    int excl, total;
+    Scan(tmp.scan).ExclusiveSum(tie, excl, total);
+    if (above || (tie && ties_base + excl < want)) sel[atomicAdd(&nsel_at, 1)] = rk_key64(key, u);   // a slot only
+    __syncthreads();                                        // scan storage and ties_base reused
+    if (threadIdx.x == 0) ties_base += total;
+    __syncthreads();
+  }
+  // each kept key's rank among the kept ones (distinct keys) is its output slot
+  for (int i = threadIdx.x; i < nsel; i += nt) {
+    const unsigned long long key = sel[i];
+    int r = 0;
+    for (int j = 0; j < nsel; ++j) r += sel[j] > key;
+    const int u = (int)(0xffffffffu - (unsigned int)(key & 0xffffffffull));
+    int node = root ? u : cnode[cs + u];                    // the leaf's tuple along its path
+    int64_t* g = out_gen + ((int64_t)b * w + r) * H;
+    for (int l = H; l >= 1; --l) {
+      g[l - 1] = path.code[l][node];
+      node = path.parent[l][node];
+    }
+    out_lp[(int64_t)b * w + r] = sc[cs + u];
+  }
+  for (int o = nsel + threadIdx.x; o < w; o += nt) {
+    for (int h = 0; h < H; ++h) out_gen[((int64_t)b * w + o) * H + h] = -1;
+    out_lp[(int64_t)b * w + o] = -INFINITY;
+  }
+}
+
+static int ex_filter_of(const int* pos, const int64_t* keys, const int* count, int M, int H, int levels, bool include,
+                        const char* what, SidExcl& f) {
+  f = SidExcl{pos, reinterpret_cast<const long long*>(keys), count, M, H, include};
+  RQB_CHECK_ARG(pos && keys && count && M > 0 && M <= SID_EXCL_MAX_M && H >= levels && H <= RQB_MAX_LEVELS,
+                "%s: bad %s (M = %d, H = %d, need M <= %d and H >= %d)", what, include ? "inclusion" : "exclusion", M, H,
+                SID_EXCL_MAX_M, levels);
+  return RQB_OK;
+}
+
+template <bool WRITE>
+static int ex_frontier_launch(int mode, dim3 grid, cudaStream_t st, const float* sc, const int* coff, int n_root, const int* cnode,
+                              const int* ccode, const int* cpar, const int64_t* pkey, const float* tau, int Bc, int K, int l,
+                              const int* lchild, const int* lcode_next, const SidExcl& f, int b0, int* counts, const int* offs,
+                              int64_t* row_code, int64_t* row_par, float* row_score, int64_t* row_key, int* row_node, int* tiles,
+                              int* nrng, int* nnode, int* ncode, int* npar) {
+  auto kernel = mode == SID_FILTER_INCLUDE   ? t5exact_frontier_kernel<SID_FILTER_INCLUDE, WRITE>
+                : mode == SID_FILTER_EXCLUDE ? t5exact_frontier_kernel<SID_FILTER_EXCLUDE, WRITE>
+                                             : t5exact_frontier_kernel<SID_FILTER_NONE, WRITE>;
+  kernel<<<grid, EX_THREADS, 0, st>>>(sc, coff, n_root, cnode, ccode, cpar, reinterpret_cast<const long long*>(pkey), tau, Bc, K, l,
+                                      lchild, lcode_next, f, b0, counts, offs, row_code, row_par, row_score,
+                                      reinterpret_cast<long long*>(row_key), row_node, tiles, nrng, nnode, ncode, npar);
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
+}
+
+static int ex_frontier(int mode, const float* sc, const int* coff, int n_root, const int* cnode, const int* ccode, const int* cpar,
+                       const int64_t* pkey, const float* tau, int Bc, int K, int l, const int* lchild, const int* lcode_next, int b0,
+                       int* counts, const int* offs, int64_t* row_code, int64_t* row_par, float* row_score, int64_t* row_key,
+                       int* row_node, int* tiles, int* nrng, int* nnode, int* ncode, int* npar, const SidExcl& f, void* stream) {
+  RQB_CHECK_ARG(Bc >= 0 && K > 0 && l >= 1 && l < RQB_MAX_LEVELS && b0 >= 0 && n_root >= 0 && (counts != nullptr) != (offs != nullptr),
+                "t5exact_frontier: bad argument (Bc = %d, K = %d, l = %d, b0 = %d; one of counts / offs)", Bc, K, l, b0);
+  if (Bc == 0) return RQB_OK;
+  RQB_CHECK_ARG(tau && lchild && ccode && (cnode ? coff && cpar && (mode == SID_FILTER_NONE || pkey) : l == 1),
+                "t5exact_frontier: null pointer");
+  RQB_CHECK_ARG(counts || (row_code && row_par && row_score && row_node && tiles && nrng && (mode == SID_FILTER_NONE || row_key)),
+                "t5exact_frontier: null output");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (counts)
+    return ex_frontier_launch<false>(mode, dim3(Bc), st, sc, coff, n_root, cnode, ccode, cpar, pkey, tau, Bc, K, l, lchild, lcode_next,
+                                     f, b0, counts, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                     nullptr, nullptr);
+  return ex_frontier_launch<true>(mode, dim3(Bc), st, sc, coff, n_root, cnode, ccode, cpar, pkey, tau, Bc, K, l, lchild, lcode_next,
+                                  f, b0, nullptr, offs, row_code, row_par, row_score, row_key, row_node, tiles, nrng, nnode, ncode,
+                                  npar);
+}
+
+extern "C" int rqb200_t5exact_frontier(const float* sc, const int* coff, int n_root, const int* cnode, const int* ccode,
+                                       const int* cpar, const int64_t* pkey, const float* tau, int Bc, int K, int l, const int* lchild,
+                                       const int* lcode_next, int b0, int* counts, const int* offs, int64_t* row_code,
+                                       int64_t* row_par, float* row_score, int64_t* row_key, int* row_node, int* tiles, int* nrng,
+                                       int* nnode, int* ncode, int* npar, void* stream) {
+  return ex_frontier(SID_FILTER_NONE, sc, coff, n_root, cnode, ccode, cpar, pkey, tau, Bc, K, l, lchild, lcode_next, b0, counts, offs,
+                     row_code, row_par, row_score, row_key, row_node, tiles, nrng, nnode, ncode, npar, SidExcl{}, stream);
+}
+
+#define EX_FRONTIER_FILTERED(NAME, MODE, INCLUDE)                                                                                    \
+  extern "C" int NAME(const float* sc, const int* coff, int n_root, const int* cnode, const int* ccode, const int* cpar,             \
+                      const int64_t* pkey, const float* tau, int Bc, int K, int l, const int* lchild, const int* lcode_next, int b0, \
+                      int* counts, const int* offs, int64_t* row_code, int64_t* row_par, float* row_score, int64_t* row_key,       \
+                      int* row_node, int* tiles, int* nrng, int* nnode, int* ncode, int* npar, const int* f_pos,                  \
+                      const int64_t* f_keys, const int* f_count, int f_M, int f_H, void* stream) {                                 \
+    SidExcl f;                                                                                                                      \
+    const int rc = ex_filter_of(f_pos, f_keys, f_count, f_M, f_H, l, INCLUDE, #NAME, f);                                            \
+    if (rc != RQB_OK) return rc;                                                                                                    \
+    return ex_frontier(MODE, sc, coff, n_root, cnode, ccode, cpar, pkey, tau, Bc, K, l, lchild, lcode_next, b0, counts, offs,       \
+                       row_code, row_par, row_score, row_key, row_node, tiles, nrng, nnode, ncode, npar, f, stream);                \
+  }
+EX_FRONTIER_FILTERED(rqb200_t5exact_frontier_excluding, SID_FILTER_EXCLUDE, false)
+EX_FRONTIER_FILTERED(rqb200_t5exact_frontier_including, SID_FILTER_INCLUDE, true)
+
+template <bool KEYS_IN_SMEM>
+static int ex_select_launch(int mode, int Bc, size_t smem, cudaStream_t st, const float* sc, const int* coff, int n_root,
+                            const int* cnode, const int64_t* leaf_key, const ExPath& path, int H, int w, const SidExcl& f, int b0,
+                            int64_t* out_gen, float* out_lp) {
+  auto kernel = mode == SID_FILTER_INCLUDE   ? t5exact_select_kernel<KEYS_IN_SMEM, SID_FILTER_INCLUDE>
+                : mode == SID_FILTER_EXCLUDE ? t5exact_select_kernel<KEYS_IN_SMEM, SID_FILTER_EXCLUDE>
+                                             : t5exact_select_kernel<KEYS_IN_SMEM, SID_FILTER_NONE>;
+  if (KEYS_IN_SMEM) {
+    static unsigned long long done[3] = {0, 0, 0};
+    const int rc = rk_set_smem_once(reinterpret_cast<const void*>(kernel), RK_SEL_SMEM_KEYS * (int)sizeof(unsigned int), &done[mode]);
+    if (rc != RQB_OK) return rc;
+  }
+  kernel<<<Bc, RK_SEL_THREADS, smem, st>>>(sc, coff, n_root, cnode, reinterpret_cast<const long long*>(leaf_key), path, H, w, f, b0,
+                                           out_gen, out_lp);
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
+}
+
+static int ex_select(int mode, const float* sc, const int* coff, int n_root, const int* cnode, int max_u, const int64_t* leaf_key,
+                     const void* const* codes, const void* const* parents, int Bc, int H, int w, int b0, int64_t* out_gen,
+                     float* out_lp, const SidExcl& f, void* stream) {
+  RQB_CHECK_ARG(Bc >= 0 && H > 0 && w > 0 && b0 >= 0 && n_root >= 0 && max_u >= 0,
+                "t5exact_select: bad argument (Bc = %d, H = %d, w = %d, b0 = %d)", Bc, H, w, b0);
+  if (w > RK_SEL_MAX_N || H > RQB_MAX_LEVELS) {
+    rqb_set_error("t5exact_select: need w <= %d and H <= %d (w = %d, H = %d)", RK_SEL_MAX_N, RQB_MAX_LEVELS, w, H);
+    return RQB_ERR_UNSUPPORTED;
+  }
+  if (Bc == 0) return RQB_OK;
+  RQB_CHECK_ARG((sc || max_u == 0) && (cnode ? coff != nullptr : true) && (leaf_key || mode == SID_FILTER_NONE) && codes &&
+                    parents && out_gen && out_lp,
+                "t5exact_select: null pointer");
+  ExPath path{};
+  for (int l = 1; l <= H; ++l) {
+    path.code[l] = static_cast<const int*>(codes[l]);
+    path.parent[l] = static_cast<const int*>(parents[l]);
+    RQB_CHECK_ARG(max_u == 0 || (path.code[l] && path.parent[l]), "t5exact_select: null level %d", l);
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (max_u <= RK_SEL_SMEM_KEYS)
+    return ex_select_launch<true>(mode, Bc, (size_t)max_u * sizeof(unsigned int), st, sc, coff, n_root, cnode, leaf_key, path, H,
+                                  w, f, b0, out_gen, out_lp);
+  return ex_select_launch<false>(mode, Bc, 0, st, sc, coff, n_root, cnode, leaf_key, path, H, w, f, b0, out_gen, out_lp);
+}
+
+extern "C" int rqb200_t5exact_select(const float* sc, const int* coff, int n_root, const int* cnode, int max_u,
+                                     const int64_t* leaf_key, const void* const* codes, const void* const* parents, int Bc, int H,
+                                     int w, int b0, int64_t* out_gen, float* out_lp, void* stream) {
+  return ex_select(SID_FILTER_NONE, sc, coff, n_root, cnode, max_u, leaf_key, codes, parents, Bc, H, w, b0, out_gen, out_lp,
+                   SidExcl{}, stream);
+}
+
+#define EX_SELECT_FILTERED(NAME, MODE, INCLUDE)                                                                                      \
+  extern "C" int NAME(const float* sc, const int* coff, int n_root, const int* cnode, int max_u, const int64_t* leaf_key,          \
+                      const void* const* codes, const void* const* parents, int Bc, int H, int w, int b0, int64_t* out_gen,      \
+                      float* out_lp, const int* f_pos, const int64_t* f_keys, const int* f_count, int f_M, int f_H,              \
+                      void* stream) {                                                                                               \
+    SidExcl f;                                                                                                                      \
+    const int rc = ex_filter_of(f_pos, f_keys, f_count, f_M, f_H, H, INCLUDE, #NAME, f);                                            \
+    if (rc != RQB_OK) return rc;                                                                                                    \
+    return ex_select(MODE, sc, coff, n_root, cnode, max_u, leaf_key, codes, parents, Bc, H, w, b0, out_gen, out_lp, f, stream);   \
+  }
+EX_SELECT_FILTERED(rqb200_t5exact_select_excluding, SID_FILTER_EXCLUDE, false)
+EX_SELECT_FILTERED(rqb200_t5exact_select_including, SID_FILTER_INCLUDE, true)

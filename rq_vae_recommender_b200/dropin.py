@@ -10,7 +10,8 @@ the replacement modules of this package; everything else (data/, evaluate/, the 
 tree untouched.  ``replace_model=True`` also aliases ``modules.model`` (train_decoder.py:14), whose
 ``EncoderDecoderRetrievalModel.generate`` then runs its beam search on the fused sampling and selection kernel;
 ``search="beam"`` (with ``replace_model=True``) makes the exhaustive, deterministic beam search over every code its default, so
-an unmodified ``train_decoder.py`` evaluates with it; ``decoder="fused"`` (with ``replace_model=True``) likewise makes generate's
+an unmodified ``train_decoder.py`` evaluates with it (``search="exact"``: the exact top-k search, the most probable corpus tuples
+with no search error); ``decoder="fused"`` (with ``replace_model=True``) likewise makes generate's
 decoder passes run on the fused decoder-step kernels (``FusedT5Decode``), and ``encoder="fused"`` its encoder pass over the
 unpadded positions only (``FusedT5Encode``); ``forward_encoder="fused"`` makes the training pass ``forward`` run its encoder on
 the trainable packed pass (``FusedT5EncodeTrain``), and ``forward_decoder="fused"`` its decoder on the fused training
@@ -43,8 +44,8 @@ _METRICS = ("evaluate.metrics", "rq_vae_recommender_b200.evaluate.metrics")
 def install(reference_root=None, replace_tokenizer=True, gin_shim=True, replace_model=False, search="sample",
             replace_metrics=False, decoder="hf", encoder="hf", forward_encoder="hf", forward_decoder="hf",
             encoder_attention="fp32", exclude_history=False):
-    if search not in ("sample", "beam"):
-        raise ValueError(f"search must be 'sample' or 'beam', got {search!r}")
+    if search not in ("sample", "beam", "exact"):
+        raise ValueError(f"search must be 'sample', 'beam' or 'exact', got {search!r}")
     if search != "sample" and not replace_model:
         raise ValueError(f"search={search!r} selects the replacement model's search: it needs replace_model=True")
     if decoder not in ("hf", "fused"):

@@ -15,6 +15,8 @@ The search (``generate``, ``generate_items``):
     reference's.  Nothing in the level loop waits for the device: rows ``torch.multinomial`` would reject are counted on the
     device and raise its error after the last level;
   * ``search="beam"``: an exhaustive, deterministic beam search over every code (``SidPrefixIndex.beam_topk``), no sampling;
+  * ``search="exact"``: the w valid corpus tuples of highest exact log-probability (``rank_sem_ids``' score, bit for bit): a beam
+    search of width w bounds the w-th best score, and ``FusedT5Exact`` decodes only the trie nodes that reach the bound;
   * ``generate_items`` resolves the beams to corpus items with one more launch (``ops.SidItemTable.retrieve``); ``item_of``
     resolves ``sem_ids_fut`` to the true next item;
   * ``exclude_items`` / ``exclude_history`` leave given items (or each history's own) out of the search, the retrieval and
@@ -58,9 +60,10 @@ torch.set_float32_matmul_precision("high")
 MAX_CANDIDATES = 64
 #: the widest beam generate(num_beams=...) takes (the cluster selection kernels keep at most 1024 beams per history)
 MAX_NUM_BEAMS = 1024
-#: the search generate() runs when it is not given one: "sample" (the reference's sampled beam search) or "beam" (exhaustive)
+#: the search generate() runs when it is not given one: "sample" (the reference's sampled beam search), "beam" (exhaustive) or
+#: "exact" (the w most probable corpus tuples, no search error)
 DEFAULT_SEARCH = "sample"
-SEARCHES = ("sample", "beam")
+SEARCHES = ("sample", "beam", "exact")
 #: the decoder passes generate() runs when it is not given a decoder: "hf" (transformers' T5Stack with its cache, as the
 #: reference) or "fused" (FusedT5Decode: cross keys/values once per history, the decoder-step kernels of csrc/t5dec.cu)
 DEFAULT_DECODER = "hf"
@@ -346,6 +349,79 @@ class FusedT5Rank(_T5DecoderLevels):
                                                                         tf32=self.tf32))
             ops.t5rank_children(ops.gemm_split(nrm, self.heads_w[h]), score, child[h], code[h], R // nxt[h].shape[0], nxt[h], bad)
             score = nxt[h]
+
+
+#: decoder rows the pruned decode of the last generate(search="exact") call ran, summed over its chunks (neither the bound's beam
+#: search and rescoring nor a level abandoned for a smaller chunk counts); observation only
+EXACT_DECODER_ROWS = 0
+
+
+def _read_frontier(offsets: Tensor, counts: Tensor) -> List[int]:
+    """The totals of the next level of one chunk of generate(search="exact"): its decoder rows, their children, their query tiles
+    and the most children of one history, read on the host to size the level: one read per level per chunk."""
+    return torch.cat([offsets[:, -1], counts[1].max().view(1)]).tolist()
+
+
+def _grow_rows(t: Tensor, dim: int, rows: int) -> Tensor:
+    """t with dimension ``dim`` enlarged to ``rows``, the existing entries copied."""
+    shape = list(t.shape)
+    shape[dim] = rows
+    out = t.new_empty(shape)
+    out.narrow(dim, 0, t.shape[dim]).copy_(t)
+    return out
+
+
+class FusedT5Exact(FusedT5Rank):
+    """The pruned exact decode of ``generate(search="exact")``: ``FusedT5Rank``'s maths over the corpus trie, decoding per history
+    only the nodes whose exact score is at least tau[b], a score some valid leaf of the history reaches.  A child never scores
+    above its parent (``t5rank_children`` adds a log-probability <= 0), so no pruned node has a descendant in the history's
+    exact top w, and the nodes kept get ``rank_sem_ids``' bits: every GEMM is row-wise, and the ragged cross-attention gives a
+    query the uniform kernel's arithmetic.  Per level, after the head and ``t5rank_children``:
+      * ``t5exact_frontier_count`` counts each history's kept children (score >= tau[b], allowed by the filter), a scan gives the
+        offsets, ``_read_frontier`` reads the totals on the host, and ``t5exact_frontier_write`` lays out the next level's rows --
+        ragged, history b's contiguous with no padding -- their query tiles, and their children as one group;
+      * the level's rows run ``_T5DecoderLevels.level`` with ``t5rank_cross_attention_ragged``; level 0 is each history's BOS row.
+    ``t5exact_select`` then takes each history's w best leaves among the last level's children."""
+
+    def run(self, b0: int, b1: int, levels: ops.SidTrieLevels, tau: Tensor, w: int, leaf_key: Tensor, filt: dict, max_rows: int,
+            gen: Tensor, lp: Tensor, bad: Tensor) -> Optional[int]:
+        """The w best leaves of histories b0 .. b1 - 1 into gen [b1 - b0, w, H] / lp [b1 - b0, w]; returns the decoder rows run,
+        or None (nothing written) when a level of two or more histories would exceed ``max_rows`` rows."""
+        H, Bc, dev = self.H, b1 - b0, self.cross_kv.device
+        K = self.model.num_embeddings_per_hierarchy
+        offsets, tau_c, heads = self.offsets[b0:b1 + 1], tau[b0:b1], self.t5.heads
+        cap = Bc                                             # cache and ancestor rows, grown with the levels
+        cache = torch.empty((len(self.w), 2, H, cap, self.t5.inner), dtype=torch.float32, device=dev)
+        anc = [torch.zeros((cap, H), dtype=torch.int32, device=dev), torch.empty((cap, H), dtype=torch.int32, device=dev)]
+        nrm = self.level(0, Bc, None, None, cache, anc,
+                         lambda q, k, v: ops.t5rank_cross_attention(q, k, v, offsets, self.key_mask, 1, heads))
+        first = torch.empty((Bc, levels.n[1]), dtype=torch.float32, device=dev)
+        ops.t5rank_children(ops.gemm_split(nrm, self.heads_w[0]), None, levels.child[0], levels.code[1], 1, first, bad)
+        children, max_u, rows = ops.ExactChildren(first.view(-1), levels.n[1]), levels.n[1], Bc
+        for l in range(1, H):
+            counts = ops.t5exact_frontier_count(children, levels.code[1], tau_c, K, l, levels.child[l], b0, **filt)
+            scan = torch.zeros((3, Bc + 1), dtype=torch.int32, device=dev)
+            scan[:, 1:] = counts.cumsum(1)
+            R, C, T, max_u = _read_frontier(scan, counts)
+            if R > max_rows and Bc > 1:
+                return None
+            if R == 0:                                       # every history's frontier is empty: no valid leaf reaches tau
+                gen.fill_(-1)
+                lp.fill_(float("-inf"))
+                return rows
+            nxt = ops.t5exact_frontier_write(children, levels.code[1], tau_c, K, l, levels.child[l], levels.code[l + 1], scan,
+                                             (R, C, T), b0, **filt)
+            if R > cap:
+                cap = min(max(R, 2 * cap), max(R, max_rows))
+                cache = _grow_rows(cache, 3, cap)
+                anc = [_grow_rows(anc[0], 0, cap), torch.empty((cap, H), dtype=torch.int32, device=dev)]
+            nrm = self.level(l, R, nxt.code, nxt.parent, cache, anc,
+                             lambda q, k, v: ops.t5rank_cross_attention_ragged(q, k, v, offsets, self.key_mask, nxt.tiles, heads))
+            ops.t5rank_children(ops.gemm_split(nrm, self.heads_w[l]), nxt.score, nxt.child, nxt.children.code, R,
+                                nxt.children.scores.view(1, -1), bad)
+            children, rows = nxt.children, rows + R
+        ops.t5exact_select(children, max_u, levels, H, leaf_key, w, gen, lp, b0, **filt)
+        return rows
 
 
 def _encoder_attention(encoder: str, encoder_attention: Optional[str], what: str) -> str:
@@ -1065,17 +1141,28 @@ class EncoderDecoderRetrievalModel(nn.Module):
                              "training mode HF's encoder applies dropout)")
         search = _choice(search, DEFAULT_SEARCH, SEARCHES, "generate", "search")
         num_beams = None if num_beams is None else int(num_beams)
+        if search == "exact":
+            return self._generate_exact(attention_mask, input_ids, user_id, decoder, encoder, encoder_attention, filters,
+                                        num_beams)
         k = self.top_k_for_generation if num_beams is None else num_beams
         n_cands = min(MAX_CANDIDATES, self.num_embeddings_per_hierarchy)
         self._check_search_limits(search, k, n_cands, num_beams)
-        beam = search == "beam"
-        wide = not self._narrow_search(search, k, n_cands)
         if encoder == "fused":
             # "fp32" without an argument: a caller may have replaced _fused_encoder with a function of none
             fused_encoder = self._fused_encoder() if att == "fp32" else self._fused_encoder(att)
             enc_out, enc_mask = fused_encoder(attention_mask, input_ids, user_id)
         else:
             enc_out, enc_mask = self.encoder_forward_pass(attention_mask=attention_mask, input_ids=input_ids, user_id=user_id)
+        generated, log_probas, reject = self._search_levels(enc_out, enc_mask, search, decoder, k, filters)
+        self._finish_search(search, reject, filters)
+        return generated, log_probas
+
+    def _search_levels(self, enc_out: Tensor, enc_mask: Tensor, search: str, decoder: str, k: int, filters: list):
+        """The level loop of a "sample" or "beam" search of width k over the encoder output: (generated [B, k, H], log_probas
+        [B, k], the device counters ``_finish_search`` reads)."""
+        n_cands = min(MAX_CANDIDATES, self.num_embeddings_per_hierarchy)
+        beam = search == "beam"
+        wide = not self._narrow_search(search, k, n_cands)
         index = self._prefix_index(enc_out.device)
         fused = self._fused_decoder(enc_out, enc_mask, k) if decoder == "fused" else None
         if fused is None:
@@ -1108,18 +1195,70 @@ class EncoderDecoderRetrievalModel(nn.Module):
                 past_kv = EncoderDecoderCache(DynamicCache(), DynamicCache())   # level 1 re-runs the decoder on B * k rows
             else:
                 past_kv.reorder_cache(parent_global)
-        if beam:
+        return generated, log_probas, reject
+
+    def _finish_search(self, search: str, reject: Tensor, filters: list) -> None:
+        """The one host read after a "sample" or "beam" search's levels: its counters, then the errors they report."""
+        if search == "beam":
             n_bad = int(reject[0]) if not filters else self._read_counters(reject, filters, "generate")[0]
             if n_bad:
                 raise RuntimeError(f"generate: {n_bad} beam row(s) of the decoder head's logits hold a NaN or +inf or are all "
                                    "-inf; the beam search cannot rank them")
-            return generated, log_probas
+            return
         bad, zero_sum = self._read_counters(reject, filters, "generate")
         if bad:
             raise RuntimeError(_MULTINOMIAL_ERRORS[0])
         if zero_sum:
             raise RuntimeError(_MULTINOMIAL_ERRORS[1])
-        return generated, log_probas
+
+    def _generate_exact(self, attention_mask, input_ids, user_id, decoder, encoder, encoder_attention, filters: list,
+                        num_beams: Optional[int]):
+        """generate(search="exact"): the bound (the beam search of width w with the call's filters and decoder, its leaves
+        rescored exactly; tau[b] the w-th largest exact score when all w are finite, else -inf), then ``FusedT5Exact`` in
+        chunks of histories sized by ``RANK_BYTE_BUDGET`` (a chunk whose level would not fit reruns with half its
+        histories)."""
+        global EXACT_DECODER_ROWS
+        what = "generate(search=\"exact\")"
+        encoder, att, _ = self._check_rank_call(encoder, encoder_attention, None, what)
+        H, K, B = self.num_hierarchies, self.num_embeddings_per_hierarchy, attention_mask.shape[0]
+        w = self.top_k_for_generation if num_beams is None else num_beams
+        if not 1 <= w <= min(MAX_NUM_BEAMS, K) or K > 2048:
+            raise Rqb200Error(f"{what}: num_beams = {w} with {K} codes per level is outside the exact search's limits "
+                              f"(1 <= num_beams <= min({MAX_NUM_BEAMS}, K), at most 2048 codes per level)")
+        _check_tuple_key(H, K, what, max_levels=8)
+        dev = attention_mask.device
+        levels, leaf_key, _ = self._rank_levels(dev)
+        if encoder == "fused":
+            packed = self._fused_encoder(att).packed(attention_mask, input_ids, user_id)
+            enc_out, enc_mask = ops.t5enc_scatter(packed.rows, packed.slot), packed.enc_mask
+        else:
+            enc_out, enc_mask = self.encoder_forward_pass(attention_mask=attention_mask, input_ids=input_ids, user_id=user_id)
+            packed = PackedEncoderOutput.of_padded(enc_out, enc_mask)
+        beams, beam_lp, reject = self._search_levels(enc_out, enc_mask, "beam", decoder, w, filters)
+        self._finish_search("beam", reject, filters)
+        gen = torch.full((B, w, H), -1, dtype=torch.int64, device=dev)
+        lp = torch.full((B, w), float("-inf"), dtype=torch.float32, device=dev)
+        EXACT_DECODER_ROWS = 0
+        if B == 0 or levels.n[H] == 0:
+            return gen, lp
+        ranker = FusedT5Exact(self, *packed.keys()[:3])
+        bad = torch.zeros(1, dtype=torch.int32, device=dev)
+        exact = self._score_candidates(lambda: ranker, beams, None, bad, what)
+        bounded = (torch.isfinite(beam_lp) & torch.isfinite(exact)).all(1)
+        tau = torch.where(bounded, exact.min(1).values, float("-inf")).contiguous()
+        max_rows = max(max(levels.n[:H]), RANK_BYTE_BUDGET // FusedT5Rank.row_bytes(self))
+        filt = self._filter_kwargs(filters)
+        rows, b0, chunk = 0, 0, min(B, max_rows)
+        while b0 < B:
+            b1 = min(B, b0 + chunk)
+            ran = ranker.run(b0, b1, levels, tau, w, leaf_key, filt, max_rows, gen[b0:b1], lp[b0:b1], bad)
+            if ran is None:
+                chunk = max(1, (b1 - b0) // 2)
+                continue
+            rows, b0 = rows + ran, b1
+        EXACT_DECODER_ROWS = rows
+        self._raise_bad(bad, what)
+        return gen, lp
 
     def _batch_exclusion(self, batch: TokenizedSeqBatch, exclude_items, exclude_history) -> Optional[ops.SidExclusion]:
         return self._exclusion(self._excluded_items(batch, exclude_items, exclude_history), batch.sem_ids.shape[0],
@@ -1326,6 +1465,15 @@ class EncoderDecoderRetrievalModel(nn.Module):
         C = sem_ids.shape[1]
         if not 1 <= C <= ops.SCORE_MAX_CANDIDATES:
             raise ValueError(f"{what}: C = {C} candidates per history must be in [1, {ops.SCORE_MAX_CANDIDATES}]")
+        return self._score_candidates(
+            lambda: FusedT5Rank(self, *self._rank_encoder(attention_mask, input_ids, user_id, encoder, att), attention), sem_ids,
+            max_rows, bad, what)
+
+    def _score_candidates(self, make_ranker, sem_ids: Tensor, max_rows, bad: Tensor, what: str) -> Tensor:
+        """fp32 [B, C]: the candidate tuples sem_ids [B, C, H] scored on the ranker ``make_ranker()`` returns (built once the
+        tries are, and only when there are histories)."""
+        H, K = self.num_hierarchies, self.num_embeddings_per_hierarchy
+        B, C = sem_ids.shape[0], sem_ids.shape[1]
         trie = ops.t5score_trie_build(sem_ids, K)
         need = [[1] + [max(1, c) for c in row] for row in _read_node_counts(trie.counts)]   # rows per level, n[0] = 1 (BOS)
         max_rows = self._row_budget(max_rows, max((sum(n[:H]) for n in need), default=0), what)
@@ -1342,7 +1490,7 @@ class EncoderDecoderRetrievalModel(nn.Module):
                 n, b1 = wider, b1 + 1
             chunks.append((b0, b1, n))
             b0 = b1
-        ranker = FusedT5Rank(self, *self._rank_encoder(attention_mask, input_ids, user_id, encoder, att), attention)
+        ranker = make_ranker()
         for b0, b1, n in chunks:
             ranker.run_candidates(b0, b1, n, trie, scores, bad)
         return scores

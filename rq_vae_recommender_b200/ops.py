@@ -2021,3 +2021,151 @@ def mlp_forward_bf16(x: torch.Tensor, weights: Sequence[torch.Tensor], normalize
             _count(1)
             a = nxt
     return l2norm_rows(out) if normalize else out
+
+
+# ---------------------------------------------------------------------------------------------- exact top-k search (csrc/t5rank.cu)
+def t5rank_cross_attention_ragged(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, offsets: torch.Tensor,
+                                  key_mask: Optional[torch.Tensor], tiles: torch.Tensor, heads: int) -> torch.Tensor:
+    """``t5rank_cross_attention`` (fp32) over a ragged level (rqb200_t5rank_cross_attention_ragged), one launch: q [R, heads * 64]
+    the level's query rows, tiles int32 [T, 3] (history b, first query row, query count <= 64; ``t5exact_frontier_write``), each
+    tile's queries over history b's keys (k, v, offsets, key_mask as ``t5rank_cross_attention``) -> [R, heads * 64].  Each row
+    gets the bits the uniform kernel gives it."""
+    _need_cuda(q, k, v, offsets, key_mask, tiles)
+    inner = heads * T5_DKV
+    q, k, v = _rows_of(q, inner, "q"), _rows_of(k, inner, "k"), _rows_of(v, inner, "v")
+    if tiles.dtype != torch.int32 or tiles.dim() != 2 or tiles.shape[1] != 3 or not tiles.is_contiguous():
+        raise ValueError(f"tiles must be a contiguous int32 [T, 3] tensor, got {tiles.dtype} {tuple(tiles.shape)}")
+    if offsets.dtype != torch.int32 or offsets.dim() != 1 or not offsets.is_contiguous():
+        raise ValueError("offsets must be a contiguous int32 vector")
+    if k.shape != v.shape:
+        raise ValueError(f"k {tuple(k.shape)} and v {tuple(v.shape)} must have one shape")
+    if k.stride(0) != v.stride(0):
+        k, v = k.contiguous(), v.contiguous()
+    if key_mask is not None:
+        key_mask = _f32c(key_mask)
+        if key_mask.dim() != 1 or key_mask.shape[0] != k.shape[0]:
+            raise ValueError(f"key_mask {tuple(key_mask.shape)} must be [{k.shape[0]}], one entry per key row")
+    out = torch.empty((q.shape[0], inner), dtype=torch.float32, device=q.device)
+    with torch.cuda.device(q.device):
+        _lib.check(_lib.load().rqb200_t5rank_cross_attention_ragged(_p(q), q.stride(0), _p(k), _p(v), k.stride(0), _p(offsets),
+                                                                    _p(key_mask), _p(tiles), tiles.shape[0], heads, _p(out),
+                                                                    out.stride(0), _stream()), "t5rank_cross_attention_ragged")
+    _count(1)
+    return out
+
+
+class ExactChildren(NamedTuple):
+    """The scored children of one decoder level of the exact search, history by history, as ``t5exact_frontier_*`` and
+    ``t5exact_select`` read them.  scores fp32 [C]; for the root's children (level 1) offsets, node, code and parent are None and
+    history b's children are the n_root entries from b * n_root, child i being node i of level 1.  Otherwise offsets int32
+    [Bc + 1] (history b's children are offsets[b] .. offsets[b + 1] - 1), node / code / parent int32 [C] (node id, last code,
+    parent row) and key int64 [rows] (each parent row's prefix key; None without a filter)."""
+    scores: torch.Tensor
+    n_root: int
+    offsets: Optional[torch.Tensor] = None
+    node: Optional[torch.Tensor] = None
+    code: Optional[torch.Tensor] = None
+    parent: Optional[torch.Tensor] = None
+    key: Optional[torch.Tensor] = None
+
+
+class ExactLevel(NamedTuple):
+    """The next decoder level of the exact search (``t5exact_frontier_write``): rows in trie order (history b's are offsets[0][b]
+    .. offsets[0][b + 1] - 1), their last codes and parent rows (int64 [R], ``_T5DecoderLevels.level``'s ids / parent), scores
+    fp32 [R], prefix keys int64 [R] (None without a filter), query tiles int32 [T, 3], and the rows' children: child ranges
+    int32 [R + 1] (one group) and ``children`` (scores not yet written)."""
+    code: torch.Tensor
+    parent: torch.Tensor
+    score: torch.Tensor
+    key: Optional[torch.Tensor]
+    tiles: torch.Tensor
+    child: torch.Tensor
+    children: ExactChildren
+
+
+def _exact_children_args(ch: ExactChildren):
+    return (_p(ch.scores), _p(ch.offsets), int(ch.n_root), _p(ch.node), _p(ch.code), _p(ch.parent), _p(ch.key))
+
+
+def t5exact_frontier_count(ch: ExactChildren, root_code: Optional[torch.Tensor], tau: torch.Tensor, K: int, l: int,
+                           lchild: torch.Tensor, b0: int = 0, exclude: Optional[SidExclusion] = None,
+                           include: Optional[SidInclusion] = None) -> torch.Tensor:
+    """The count pass of the exact search's frontier (rqb200_t5exact_frontier[_excluding/_including]), one launch: per history
+    of the chunk, its children (nodes of level l) with score >= tau[b] (fp32 [Bc]) that the filter (of the whole batch; the
+    chunk's first history is b0) does not block -> int32 [3, Bc]: kept rows, their children (lchild = SidTrieLevels.child[l]),
+    their 64-query tiles.  root_code: SidTrieLevels.code[1] for the root's children (``ch.node`` None)."""
+    Bc = tau.shape[0]
+    counts = torch.empty((3, Bc), dtype=torch.int32, device=tau.device)
+    _t5exact_frontier(ch, root_code, tau, K, l, lchild, None, b0, counts, None, (None,) * 10, exclude, include)
+    return counts
+
+
+def t5exact_frontier_write(ch: ExactChildren, root_code: Optional[torch.Tensor], tau: torch.Tensor, K: int, l: int,
+                           lchild: torch.Tensor, lcode_next: torch.Tensor, offsets: torch.Tensor, totals: Sequence[int],
+                           b0: int = 0, exclude: Optional[SidExclusion] = None,
+                           include: Optional[SidInclusion] = None) -> ExactLevel:
+    """The write pass (the same entry points), one launch: offsets int32 [3, Bc + 1] the exclusive scans of the count pass,
+    totals their last column (R rows, C children, T tiles, read on the host by the caller) -> the next level (``ExactLevel``);
+    lcode_next = SidTrieLevels.code[l + 1]."""
+    R, C, T = (int(t) for t in totals[:3])
+    Bc, dev = tau.shape[0], tau.device
+    filt = exclude is not None or include is not None
+    code, parent = (torch.empty(R, dtype=torch.int64, device=dev) for _ in range(2))
+    score = torch.empty(R, dtype=torch.float32, device=dev)
+    key = torch.empty(R, dtype=torch.int64, device=dev) if filt else None
+    node = torch.empty(max(R, 1), dtype=torch.int32, device=dev)
+    tiles = torch.empty((T, 3), dtype=torch.int32, device=dev)
+    child = torch.empty(R + 1, dtype=torch.int32, device=dev)
+    nnode, ncode, npar = (torch.empty(C, dtype=torch.int32, device=dev) for _ in range(3))
+    nxt = ExactChildren(torch.empty(C, dtype=torch.float32, device=dev), 0, offsets[1], nnode, ncode, npar, key)
+    _t5exact_frontier(ch, root_code, tau, K, l, lchild, lcode_next, b0, None, offsets,
+                      (code, parent, score, key, node, tiles, child, nnode, ncode, npar), exclude, include)
+    return ExactLevel(code, parent, score, key, tiles, child, nxt)
+
+
+def _t5exact_frontier(ch, root_code, tau, K, l, lchild, lcode_next, b0, counts, offsets, outs, exclude, include):
+    _need_cuda(ch.scores, tau, lchild)
+    if ch.node is None and root_code is None:
+        raise ValueError("t5exact_frontier: the root's children need root_code (SidTrieLevels.code[1])")
+    if offsets is not None and (offsets.dtype != torch.int32 or offsets.shape != (3, tau.shape[0] + 1) or not offsets.is_contiguous()):
+        raise ValueError(f"t5exact_frontier: offsets must be a contiguous int32 [3, {tau.shape[0] + 1}] tensor")
+    ch_args = list(_exact_children_args(ch))
+    if ch.node is None:
+        ch_args[4] = _p(root_code)
+    name, filt = _filter_entry("t5exact_frontier", exclude, include, _filter_rows(exclude, include), l, "t5exact_frontier")
+    with torch.cuda.device(tau.device):
+        _lib.check(getattr(_lib.load(), "rqb200_" + name)(*ch_args, _p(tau), tau.shape[0], int(K), int(l), _p(lchild),
+                                                          _p(lcode_next), int(b0), _p(counts), _p(offsets),
+                                                          *(_p(t) for t in outs), *filt, _stream()), name)
+    _count(1)
+
+
+def _filter_rows(exclude, include) -> int:
+    """The histories a filter holds (the whole batch; a chunk indexes it from its first history)."""
+    f = include if include is not None else exclude
+    return 0 if f is None else f.pos.shape[0]
+
+
+def t5exact_select(ch: ExactChildren, max_u: int, levels: SidTrieLevels, H: int, leaf_key: torch.Tensor, w: int,
+                   out_gen: torch.Tensor, out_lp: torch.Tensor, b0: int = 0, exclude: Optional[SidExclusion] = None,
+                   include: Optional[SidInclusion] = None) -> None:
+    """The exact search's selection (rqb200_t5exact_select[_excluding/_including]), one launch: per history of the chunk, the w
+    best of its leaf candidates ``ch`` (leaf ids in ``ch.node``; max_u the largest count of a history) by score descending,
+    then leaf ascending, NaN and blocked leaves left out -> out_gen int64 [Bc, w, H] (written: each leaf's tuple, from
+    ``levels``' codes and parents) and out_lp fp32 [Bc, w]; -1 / -inf past the valid candidates.  leaf_key int64 [U]: the
+    leaves' ``_tuple_key`` (read with a filter)."""
+    _need_cuda(ch.scores, out_gen, out_lp, leaf_key)
+    Bc = out_lp.shape[0]
+    if out_gen.dtype != torch.int64 or out_gen.shape != (Bc, w, H) or not out_gen.is_contiguous():
+        raise ValueError(f"out_gen must be a contiguous int64 [{Bc}, {w}, {H}] tensor")
+    if out_lp.dtype != torch.float32 or out_lp.shape != (Bc, w) or not out_lp.is_contiguous():
+        raise ValueError(f"out_lp must be a contiguous fp32 [{Bc}, {w}] tensor")
+    name, filt = _filter_entry("t5exact_select", exclude, include, _filter_rows(exclude, include), H, "t5exact_select")
+    args = _exact_children_args(ch)
+    codes = _ptr_array([None] + [levels.code[l] for l in range(1, H + 1)])
+    parents = _ptr_array([None] + [levels.parent[l] for l in range(1, H + 1)])
+    with torch.cuda.device(out_lp.device):
+        _lib.check(getattr(_lib.load(), "rqb200_" + name)(args[0], args[1], args[2], args[3], int(max_u), _p(leaf_key), codes,
+                                                          parents, Bc, int(H), int(w), int(b0), _p(out_gen), _p(out_lp), *filt,
+                                                          _stream()), name)
+    _count(1)
