@@ -562,6 +562,10 @@ int rqb200_t5dec_add_norm(float* x, const float* delta, int64_t ld_delta, const 
  *                  packed row x = the input row -- user_table[remainder(user_ids[b * user_stride], n_users)] (user_table and
  *                  user_ids both null: no user row), item_table[(ids[b, c] + (c % H) * K) * mask[b, c]] (an id outside
  *                  [0, n_items) gives a NaN row), or sep_row (null: sep = 0) -- and out = T5LayerNorm(x) * weight; x, out [N, D].
+ * t5enc_assemble_capacity: t5enc_assemble at a fixed capacity of B * S rows, for a caller that cannot read N (a CUDA-graph
+ *                  capture): x, out [B * S, D] and src [B * S]; rows 0 .. N - 1 as t5enc_assemble writes them, rows N .. B * S - 1
+ *                  x = out = 0 and src = -1.  No attention kernel reads or writes a row past N, and rqb200_t5dec_add_norm keeps a zero
+ *                  row zero, so those rows stay zero through the pass when the attention output's rows past N are zeros.
  * t5enc_attention: bidirectional self-attention among each history's packed rows.  qkv [N, 3 inner] (q | k | v, row stride
  *                  ldqkv, a multiple of 4, 16-byte aligned), rel [heads, 2S - 1]: the score of query position i and key position
  *                  j is q . k + (rel[n, j - i + S - 1] + key_mask[b]), no 1/sqrt(d) scaling, fp32 softmax.  out [N, inner] (row
@@ -572,6 +576,11 @@ int rqb200_t5enc_assemble(const float* mask, const int64_t* ids, int64_t ids_str
                           const float* item_table, int64_t n_items, const float* sep_row, const float* user_table, int64_t n_users,
                           int64_t K, int B, int n, int H, int D, const int* offsets, const float* weight, float eps, float* x,
                           float* out, int* src, int* slot, void* stream);
+int rqb200_t5enc_assemble_capacity(const float* mask, const int64_t* ids, int64_t ids_stride, const int64_t* user_ids,
+                                   int64_t user_stride, const float* item_table, int64_t n_items, const float* sep_row,
+                                   const float* user_table, int64_t n_users, int64_t K, int B, int n, int H, int D,
+                                   const int* offsets, const float* weight, float eps, float* x, float* out, int* src, int* slot,
+                                   void* stream);
 int rqb200_t5enc_attention(const float* qkv, int64_t ldqkv, const int* src, const int* offsets, const float* key_mask,
                            const float* rel, int B, int S, int heads, float* out, int64_t ldo, void* stream);
 int rqb200_t5enc_scatter(const float* rows, const int* slot, int64_t n_out, int D, float* out, void* stream);

@@ -141,6 +141,8 @@ _SIGNATURES = {
     "rqb200_t5enc_offsets": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
     "rqb200_t5enc_assemble": (c_int, [c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i64, c_i64, c_int, c_int, c_int,
                                       c_int, c_vp, c_vp, c_f32, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "rqb200_t5enc_assemble_capacity": (c_int, [c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i64, c_i64, c_int, c_int,
+                                               c_int, c_int, c_vp, c_vp, c_f32, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "rqb200_t5enc_attention": (c_int, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_i64, c_vp]),
     "rqb200_t5enc_scatter": (c_int, [c_vp, c_vp, c_i64, c_int, c_vp, c_vp]),
     "rqb200_t5enc_attention_train": (c_int, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_f32, c_vp, c_i64,

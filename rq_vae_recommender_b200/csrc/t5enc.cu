@@ -11,6 +11,8 @@
 //                           index src [N] = b * S + p and its inverse slot [B * S] (-1 for a dropped position), then one warp per
 //                           kept row gathers the input row (user embedding, level-offset item id, separator) into x and writes
 //                           out = T5LayerNorm(x) * weight.
+//   rqb200_t5enc_assemble_capacity  the same at a fixed capacity of B * S rows (a CUDA graph cannot read N): each CTA also
+//                           zeroes its share of the rows past N (x = out = 0, src = -1), which every later kernel leaves zero.
 //   rqb200_t5enc_attention  bidirectional self-attention over the packed rows, one CTA per (history, head, 128 queries), one
 //                           thread per query with its q and output row in registers.  Keys and values stream through shared memory
 //                           32 at a time with an online fp32 softmax, so the history length has no fixed limit.  Each score is
@@ -101,6 +103,9 @@ __global__ void __launch_bounds__(TE_SCAN) t5enc_offsets_kernel(const float* __r
 }
 
 // ------------------------------------------------------------------------------------------------ input assembly + first norm
+// CAPACITY: x, out and src hold B * S rows; history b also owns the S - cnt rows past offsets[B] that its dropped positions leave
+// (starting at offsets[B] + b * S - offsets[b], so the B ranges tile offsets[B] .. B * S - 1) and writes them x = out = 0, src = -1.
+template <bool CAPACITY>
 __global__ void __launch_bounds__(TE_ASM) t5enc_assemble_kernel(
     const float* __restrict__ mask, const int64_t* __restrict__ ids, int64_t ids_stride, const int64_t* __restrict__ user_ids,
     int64_t user_stride, const float* __restrict__ item_table, int64_t n_items, const float* __restrict__ sep_row,
@@ -162,6 +167,16 @@ __global__ void __launch_bounds__(TE_ASM) t5enc_assemble_kernel(
     const float inv = rsqrtf(warp_sum(ss) / (float)D + eps);
     float* orow = out + (int64_t)r * D;
     for (int d = lane; d < D; d += 32) orow[d] = weight[d] * (xr[d] * inv);
+  }
+  if (CAPACITY) {
+    const int r0 = offsets[gridDim.x] + b * S - off;
+    for (int r = r0 + warp; r < r0 + S - cnt; r += TE_ASM / 32) {
+      for (int d = lane; d < D; d += 32) {
+        x[(int64_t)r * D + d] = 0.f;
+        out[(int64_t)r * D + d] = 0.f;
+      }
+      if (lane == 0) src[r] = -1;
+    }
   }
 }
 
@@ -595,23 +610,42 @@ extern "C" int rqb200_t5enc_offsets(const float* mask, int B, int n, int H, int 
   return RQB_OK;
 }
 
+template <bool CAPACITY>
+static int t5enc_assemble_launch(const char* what, const float* mask, const int64_t* ids, int64_t ids_stride,
+                                 const int64_t* user_ids, int64_t user_stride, const float* item_table, int64_t n_items,
+                                 const float* sep_row, const float* user_table, int64_t n_users, int64_t K, int B, int n, int H, int D,
+                                 const int* offsets, const float* weight, float eps, float* x, float* out, int* src, int* slot,
+                                 void* stream) {
+  RQB_CHECK_ARG(B >= 0 && n >= 0 && H > 0 && n % H == 0 && D > 0 && n_items > 0 && K >= 0 && ids_stride >= n,
+                "%s: bad shape (B=%d n=%d H=%d D=%d)", what, B, n, H, D);
+  RQB_CHECK_ARG(!user_table == !user_ids && (!user_table || n_users > 0), "%s: user_ids and user_table go together", what);
+  const int64_t S = enc_len(n, H, sep_row != nullptr, user_table != nullptr);
+  RQB_CHECK_ARG(S > 0 && (int64_t)B * S <= INT32_MAX, "%s: bad encoder length (S=%lld, B=%d)", what, (long long)S, B);
+  if (B == 0) return RQB_OK;
+  RQB_CHECK_ARG(mask && ids && item_table && offsets && weight && x && out && src && slot, "%s: null pointer", what);
+  t5enc_assemble_kernel<CAPACITY><<<B, TE_ASM, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      mask, ids, ids_stride, user_ids, user_stride, item_table, n_items, sep_row, user_table, n_users, K, n, H, (int)S, D, offsets,
+      weight, eps, x, out, src, slot);
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
+}
+
 extern "C" int rqb200_t5enc_assemble(const float* mask, const int64_t* ids, int64_t ids_stride, const int64_t* user_ids,
                                      int64_t user_stride, const float* item_table, int64_t n_items, const float* sep_row,
                                      const float* user_table, int64_t n_users, int64_t K, int B, int n, int H, int D,
                                      const int* offsets, const float* weight, float eps, float* x, float* out, int* src, int* slot,
                                      void* stream) {
-  RQB_CHECK_ARG(B >= 0 && n >= 0 && H > 0 && n % H == 0 && D > 0 && n_items > 0 && K >= 0 && ids_stride >= n,
-                "t5enc_assemble: bad shape (B=%d n=%d H=%d D=%d)", B, n, H, D);
-  RQB_CHECK_ARG(!user_table == !user_ids && (!user_table || n_users > 0), "t5enc_assemble: user_ids and user_table go together");
-  const int64_t S = enc_len(n, H, sep_row != nullptr, user_table != nullptr);
-  RQB_CHECK_ARG(S > 0 && (int64_t)B * S <= INT32_MAX, "t5enc_assemble: bad encoder length (S=%lld, B=%d)", (long long)S, B);
-  if (B == 0) return RQB_OK;
-  RQB_CHECK_ARG(mask && ids && item_table && offsets && weight && x && out && src && slot, "t5enc_assemble: null pointer");
-  t5enc_assemble_kernel<<<B, TE_ASM, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      mask, ids, ids_stride, user_ids, user_stride, item_table, n_items, sep_row, user_table, n_users, K, n, H, (int)S, D, offsets,
-      weight, eps, x, out, src, slot);
-  RQB_LAUNCH_CHECK();
-  return RQB_OK;
+  return t5enc_assemble_launch<false>("t5enc_assemble", mask, ids, ids_stride, user_ids, user_stride, item_table, n_items,
+                                      sep_row, user_table, n_users, K, B, n, H, D, offsets, weight, eps, x, out, src, slot, stream);
+}
+
+extern "C" int rqb200_t5enc_assemble_capacity(const float* mask, const int64_t* ids, int64_t ids_stride, const int64_t* user_ids,
+                                              int64_t user_stride, const float* item_table, int64_t n_items, const float* sep_row,
+                                              const float* user_table, int64_t n_users, int64_t K, int B, int n, int H, int D,
+                                              const int* offsets, const float* weight, float eps, float* x, float* out, int* src,
+                                              int* slot, void* stream) {
+  return t5enc_assemble_launch<true>("t5enc_assemble_capacity", mask, ids, ids_stride, user_ids, user_stride, item_table, n_items,
+                                     sep_row, user_table, n_users, K, B, n, H, D, offsets, weight, eps, x, out, src, slot, stream);
 }
 
 extern "C" int rqb200_t5enc_attention(const float* qkv, int64_t ldqkv, const int* src, const int* offsets, const float* key_mask,

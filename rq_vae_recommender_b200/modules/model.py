@@ -504,14 +504,18 @@ class FusedT5Encode:
         set to 0, and enc_mask [B, S] with the same values.
     N is read on the host once per call (``_read_n_kept``) to size the GEMMs; it is the pass's only host synchronisation, and
     ``n_kept`` keeps the last call's.  ``attention`` picks the self-attention kernel: "fp32" (``ops.t5enc_attention``) or "tf32"
-    (``ops.t5enc_attention_tc``)."""
+    (``ops.t5enc_attention_tc``).
+    ``capacity=True`` reads nothing on the host, for a CUDA-graph capture: the packed rows are B * S, rows N .. B * S - 1 zero
+    (``ops.t5enc_assemble_capacity``, and one zero-filled attention output that the attention kernels never write past N), so
+    the GEMMs run B * S rows and rows 0 .. N - 1 differ from the eager pass only by the GEMMs' rounding at another row count."""
 
-    def __init__(self, model: "EncoderDecoderRetrievalModel", attention: str = "fp32"):
+    def __init__(self, model: "EncoderDecoderRetrievalModel", attention: str = "fp32", capacity: bool = False):
         self.model = model
         self.t5 = _T5Weights(model.encoder.encoder, "encoder=\"fused\"")
         tf32 = _choice(attention, None, ENCODER_ATTENTIONS, "FusedT5Encode", "attention") == "tf32"
         self.attention = ops.t5enc_attention_tc if tf32 else ops.t5enc_attention
         self.w = [self.t5.layer(l) for l in range(len(self.t5.blocks))]
+        self.capacity = capacity
         self.n_kept = None
 
     def __call__(self, attention_mask: Tensor, input_ids: Tensor, user_id: Optional[Tensor] = None):
@@ -526,14 +530,19 @@ class FusedT5Encode:
         user = user_id is not None and m.user_embedding is not None
         enc_mask = _encoder_mask(m, attention_mask, user)
         offsets, key_mask = ops.t5enc_offsets(attention_mask, H, sep, user)
-        self.n_kept = _read_n_kept(offsets)
-        x, nrm, src, slot = ops.t5enc_assemble(
-            attention_mask, input_ids, user_id if user else None, m.item_sid_embedding_table.weight, m.sep_token if sep else None,
-            m.user_embedding.weight if user else None, m.num_embeddings_per_hierarchy, H, offsets, self.n_kept, norms[0], eps)
+        inputs = (attention_mask, input_ids, user_id if user else None, m.item_sid_embedding_table.weight,
+                  m.sep_token if sep else None, m.user_embedding.weight if user else None, m.num_embeddings_per_hierarchy, H, offsets)
+        a_out = None
+        if self.capacity:
+            x, nrm, src, slot = ops.t5enc_assemble_capacity(*inputs, norms[0], eps)
+            a_out = x.new_zeros((x.shape[0], self.t5.inner))
+        else:
+            self.n_kept = _read_n_kept(offsets)
+            x, nrm, src, slot = ops.t5enc_assemble(*inputs, self.n_kept, norms[0], eps)
         S = slot.shape[1]
         rel = ops.t5enc_rel_bias(self.t5.blocks[0][0].SelfAttention.compute_bias(S, S)[0])
         for l, (w_qkv, w_o, w_i, w_fo) in enumerate(self.w):
-            a = self.attention(F.linear(nrm, w_qkv), src, offsets, key_mask, rel, S)
+            a = self.attention(F.linear(nrm, w_qkv), src, offsets, key_mask, rel, S, a_out)
             ops.t5dec_add_norm(x, F.linear(a, w_o), norms[2 * l + 1], nrm, eps)
             ops.t5dec_add_norm(x, F.linear(_linear(nrm, w_i, relu=True), w_fo), norms[2 * l + 2], nrm, eps)
         return PackedEncoderOutput(nrm, offsets, key_mask, src, slot, S, enc_mask)
@@ -1067,13 +1076,25 @@ class EncoderDecoderRetrievalModel(nn.Module):
         return {"include" if isinstance(filters[-1], ops.SidInclusion) else "exclude": filters[-1]}
 
     @staticmethod
+    def _counter_values(counters: Tensor, filters: list) -> Tensor:
+        """int32 on the device: the counters, then each filter's count of ids outside [-1, N) -- what ``_read_counters`` reads."""
+        if not filters:
+            return counters
+        return torch.cat([counters.int()] + [f.count[:, -1].sum(dtype=torch.int32).view(1) for f in filters])
+
+    @staticmethod
     def _read_counters(counters: Tensor, filters: list, what: str) -> List[int]:
         """The one host read at the end of a call: its counters, after which the excluded or allowed ids outside [-1, N) of
         the call's filters (``_filters``) raise."""
         if not filters:
             return counters.tolist()
-        values = torch.cat([counters.int()] + [f.count[:, -1].sum(dtype=torch.int32).view(1) for f in filters]).tolist()
-        values, n_ids = values[:counters.numel()], values[counters.numel():]
+        values = EncoderDecoderRetrievalModel._counter_values(counters, filters).tolist()
+        return EncoderDecoderRetrievalModel._check_filter_counts(values, counters.numel(), filters, what)
+
+    @staticmethod
+    def _check_filter_counts(values: List[int], n_counters: int, filters: list, what: str) -> List[int]:
+        """values as read from ``_counter_values``: the ``ValueError`` of a filter id outside [-1, N), else the counters."""
+        values, n_ids = values[:n_counters], values[n_counters:]
         for f, n in zip(filters, n_ids):
             if n:
                 kind = "allowed" if isinstance(f, ops.SidInclusion) else "excluded"
@@ -1199,13 +1220,22 @@ class EncoderDecoderRetrievalModel(nn.Module):
 
     def _finish_search(self, search: str, reject: Tensor, filters: list) -> None:
         """The one host read after a "sample" or "beam" search's levels: its counters, then the errors they report."""
+        if search == "beam" and not filters:
+            counters = [int(reject[0])]
+        else:
+            counters = self._read_counters(reject, filters, "generate")
+        self._raise_search_errors(search, counters)
+
+    @staticmethod
+    def _raise_search_errors(search: str, counters: List[int]) -> None:
+        """The errors of a "sample" or "beam" search's counters, as read on the host."""
         if search == "beam":
-            n_bad = int(reject[0]) if not filters else self._read_counters(reject, filters, "generate")[0]
+            n_bad = counters[0]
             if n_bad:
                 raise RuntimeError(f"generate: {n_bad} beam row(s) of the decoder head's logits hold a NaN or +inf or are all "
                                    "-inf; the beam search cannot rank them")
             return
-        bad, zero_sum = self._read_counters(reject, filters, "generate")
+        bad, zero_sum = counters
         if bad:
             raise RuntimeError(_MULTINOMIAL_ERRORS[0])
         if zero_sum:
@@ -1308,6 +1338,21 @@ class EncoderDecoderRetrievalModel(nn.Module):
         items, beams, count = table.retrieve(out.sem_ids, out.log_probas, width if n is None else n,
                                              **self._filter_kwargs(filters))
         return ItemGenerationOutput(item_ids=items, beams=beams, count=count, sem_ids=out.sem_ids, log_probas=out.log_probas)
+
+    def capture_generate_items(self, batch: TokenizedSeqBatch, n: Optional[int] = None, search: Optional[str] = None,
+                               num_beams: Optional[int] = None, encoder_attention: Optional[str] = None,
+                               exclude_items: Optional[Tensor] = None, exclude_history: Optional[bool] = None,
+                               include_items: Optional[Tensor] = None, encoder: str = "fused",
+                               decoder: str = "fused") -> "GenerateItemsGraph":
+        """``generate_items(batch, ..., encoder="fused", decoder="fused")`` captured as one CUDA graph, for serving: calling the
+        returned ``GenerateItemsGraph`` with a batch of the same shapes is one graph replay and one host read of the error
+        counters.  The example batch fixes every shape: B, the history width, whether ``user_ids`` is given, and the widths of
+        ``exclude_items`` / ``include_items`` (and whether each is given).  ``search`` is "sample" or "beam" at any width those
+        searches take; ``search``, ``n``, ``num_beams``, ``encoder_attention`` and ``exclude_history`` are read once, here, with
+        ``generate_items``' defaults.  Raises ``ValueError`` for search="exact" (one host read per level), an HF encoder or
+        decoder, training mode and an active autocast region.  See ``GenerateItemsGraph`` for what a replay follows."""
+        return GenerateItemsGraph(self, batch, n, search, num_beams, encoder_attention, exclude_items, exclude_history,
+                                  include_items, encoder, decoder)
 
     @torch.no_grad()
     def item_of(self, sem_ids_fut: Tensor) -> Tensor:
@@ -1561,3 +1606,137 @@ class EncoderDecoderRetrievalModel(nn.Module):
         rank = torch.where(match.any(1), before.sum(1), -1)
         self._raise_score_errors(counters, "score_items")
         return ItemScoreOutput(scores=scores, target_rank=rank)
+
+
+def _read_search_counters(values: Tensor) -> List[int]:
+    """The one host read of a ``GenerateItemsGraph`` call, after its replay: the search's counters, then each filter's count of
+    ids outside [-1, N) (``EncoderDecoderRetrievalModel._counter_values``)."""
+    return values.tolist()
+
+
+def _input_spec(t: Optional[Tensor]):
+    return None if t is None else (tuple(t.shape), t.dtype, t.device)
+
+
+class GenerateItemsGraph:
+    """One ``generate_items(..., encoder="fused", decoder="fused")`` call captured as a CUDA graph
+    (``EncoderDecoderRetrievalModel.capture_generate_items``).  ``graph(batch, exclude_items=None, include_items=None)`` copies
+    ``batch.sem_ids``, ``batch.seq_mask``, ``batch.user_ids`` and the item lists into the graph's static buffers, replays the
+    graph on the current stream, reads the counters once and returns an ``ItemGenerationOutput`` of new tensors (a later call
+    does not overwrite them).  Inputs must match the captured ones in shape, dtype, device and presence, else ``ValueError``
+    before any launch: pad histories with masked rows and shorter histories with mask zeros, as ``SeqData`` does.
+      * Results: the eager call's on the same inputs, with the decoder at the eager B * w rows.  The encoder runs at a fixed
+        capacity of B * S packed rows (``FusedT5Encode(capacity=True)``, no host read of N): with every position unmasked it is
+        the eager pass; with padding its GEMMs run B * S rows instead of N, which changes only their rounding.  "sample" draws
+        its noise from torch's CUDA generator through the graph-safe Philox offsets, so consecutive replays consume the generator
+        as consecutive eager calls do.  Capturing leaves the generator's state as it found it.
+      * Weights: a replay reads the live parameters (the q|k|v and cross k|v concatenations are copies inside the graph), so an
+        in-place update (``optimizer.step()``, ``load_state_dict``) is followed without recapture.  A parameter whose storage
+        moved (``model.to``, a replaced tensor) makes the next call recapture.
+      * Corpus: the graph bakes in the prefix index, the item table and the trie levels; when the ``codebooks`` buffer is
+        replaced, written to or moved, the next call recaptures before replaying.
+      * Errors: the eager ``RuntimeError``s (non-finite head rows, rows ``torch.multinomial`` rejects) and ``ValueError`` (filter
+        ids outside [-1, N)) with the same texts, from the one host read after the replay (``_read_search_counters``).
+      * Streams: capture and replay order with the caller's current stream (capture runs on torch's side stream when that is
+        the default stream, which cannot capture)."""
+
+    def __init__(self, model: EncoderDecoderRetrievalModel, batch: TokenizedSeqBatch, n: Optional[int], search: Optional[str],
+                 num_beams: Optional[int], encoder_attention: Optional[str], exclude_items: Optional[Tensor],
+                 exclude_history: Optional[bool], include_items: Optional[Tensor], encoder: str = "fused",
+                 decoder: str = "fused"):
+        what = "capture_generate_items"
+        if encoder != "fused" or decoder != "fused":
+            raise ValueError(f"{what}: a CUDA graph runs the fused encoder and decoder only (encoder={encoder!r}, "
+                             f"decoder={decoder!r}); HF's passes are host-driven")
+        self._check_mode(model, what)
+        self.search = _choice(search, DEFAULT_SEARCH, SEARCHES, what, "search")
+        if self.search == "exact":
+            raise ValueError(f"{what}: search=\"exact\" reads its frontier's size on the host once per level; it cannot be "
+                             "captured (use \"sample\" or \"beam\")")
+        self.attention = _encoder_attention("fused", encoder_attention, what)
+        self.k = model.top_k_for_generation if num_beams is None else int(num_beams)
+        model._check_search_limits(self.search, self.k, min(MAX_CANDIDATES, model.num_embeddings_per_hierarchy),
+                                   None if num_beams is None else self.k)
+        self.n = self.k if n is None else int(n)
+        self.exclude_history = DEFAULT_EXCLUDE_HISTORY if exclude_history is None else bool(exclude_history)
+        self.model = model
+        self.device = model.device
+        inputs = (batch.sem_ids, batch.seq_mask, batch.user_ids, exclude_items, include_items)
+        for t in inputs:
+            if t is not None and t.device != self.device:
+                raise ValueError(f"{what}: every input must be on the model's device {self.device}, got {t.device}")
+        self._spec = tuple(_input_spec(t) for t in inputs)
+        self._static = tuple(None if t is None else t.clone() for t in inputs)
+        self._graph = None
+        self._capture()
+
+    @staticmethod
+    def _check_mode(model: EncoderDecoderRetrievalModel, what: str) -> None:
+        if model.training:
+            raise ValueError(f"{what}: the fused passes run in eval mode only; call model.eval() first")
+        _check_no_autocast(what)
+
+    def _state_key(self):
+        """What the captured graph bakes in: the corpus (the prefix index's cache key) and every parameter's storage."""
+        cb = self.model.codebooks
+        return (id(cb), cb._version, cb.device), tuple(p.data_ptr() for p in self.model.parameters())
+
+    def _run(self):
+        """The captured work on the static inputs: (outputs, the device counters, the counter count, the filters)."""
+        m, H = self.model, self.model.num_hierarchies
+        sem, seq, users, exclude_items, include_items = self._static
+        batch = TokenizedSeqBatch(user_ids=users, sem_ids=sem, sem_ids_fut=None, seq_mask=seq, token_type_ids=None,
+                                  token_type_ids_fut=None)
+        filters = m._batch_filters(batch, exclude_items, self.exclude_history, include_items)
+        enc_out, enc_mask = FusedT5Encode(m, self.attention, capacity=True)(
+            _strip_dedup_col(seq.long(), H + 1, H), _strip_dedup_col(sem, H + 1, H), users)
+        generated, log_probas, reject = m._search_levels(enc_out, enc_mask, self.search, "fused", self.k, filters)
+        items, beams, count = m._item_table(sem.device).retrieve(generated, log_probas, self.n, **m._filter_kwargs(filters))
+        out = ItemGenerationOutput(item_ids=items, beams=beams, count=count, sem_ids=generated, log_probas=log_probas)
+        return out, m._counter_values(reject, filters), reject.numel(), filters
+
+    @torch.no_grad()
+    def _capture(self) -> None:
+        """Warm up on the capture stream (module loads, cuBLAS handles, the corpus caches and their host reads), restore the
+        generator, capture."""
+        self._graph = self._captured = self._key = None       # the previous graph's memory goes back before the new capture
+        dev = self.device
+        caller = torch.cuda.current_stream(dev)
+        stream = caller if caller != torch.cuda.default_stream(dev) else torch.cuda.Stream(dev)
+        stream.wait_stream(caller)
+        rng = torch.cuda.get_rng_state(dev)
+        with torch.cuda.stream(stream):
+            self._run()
+        torch.cuda.set_rng_state(rng, dev)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph, stream=stream):
+            captured = self._run()
+        caller.wait_stream(stream)
+        self._graph, self._captured, self._key = graph, captured, self._state_key()
+
+    def _check_inputs(self, batch: TokenizedSeqBatch, exclude_items: Optional[Tensor], include_items: Optional[Tensor]):
+        inputs = (batch.sem_ids, batch.seq_mask, batch.user_ids, exclude_items, include_items)
+        names = ("batch.sem_ids", "batch.seq_mask", "batch.user_ids", "exclude_items", "include_items")
+        for name, t, spec in zip(names, inputs, self._spec):
+            if _input_spec(t) != spec:
+                want = "None" if spec is None else f"{spec[1]} {list(spec[0])} on {spec[2]}"
+                got = "None" if t is None else f"{t.dtype} {list(t.shape)} on {t.device}"
+                raise ValueError(f"GenerateItemsGraph: {name} must match the captured call ({want}), got {got}")
+        return inputs
+
+    @torch.no_grad()
+    def __call__(self, batch: TokenizedSeqBatch, exclude_items: Optional[Tensor] = None,
+                 include_items: Optional[Tensor] = None) -> ItemGenerationOutput:
+        self._check_mode(self.model, "GenerateItemsGraph")
+        inputs = self._check_inputs(batch, exclude_items, include_items)
+        for dst, src in zip(self._static, inputs):
+            if dst is not None:
+                dst.copy_(src)
+        if self._state_key() != self._key:
+            self._capture()
+        self._graph.replay()
+        out, values, n_counters, filters = self._captured
+        counters = EncoderDecoderRetrievalModel._check_filter_counts(_read_search_counters(values), n_counters, filters,
+                                                                     "generate")
+        EncoderDecoderRetrievalModel._raise_search_errors(self.search, counters)
+        return ItemGenerationOutput(*(t.clone() for t in out))

@@ -1404,6 +1404,23 @@ def t5enc_assemble(mask: torch.Tensor, ids: torch.Tensor, user_ids: Optional[tor
     row stride), user_ids int64 [B, *] (column 0 is read) with user_table [U, D], or both None; item_table [V, D]; sep_row [D] or
     None; offsets from ``t5enc_offsets`` with n_kept = offsets[B].  Returns x, out [n_kept, D] (the input rows and
     T5LayerNorm(x) * weight), src int32 [n_kept] (b * S + p of each packed row) and slot int32 [B, S] (packed row or -1)."""
+    return _t5enc_assemble("t5enc_assemble", mask, ids, user_ids, item_table, sep_row, user_table, K, H, offsets, n_kept, weight,
+                           eps)
+
+
+def t5enc_assemble_capacity(mask: torch.Tensor, ids: torch.Tensor, user_ids: Optional[torch.Tensor], item_table: torch.Tensor,
+                            sep_row: Optional[torch.Tensor], user_table: Optional[torch.Tensor], K: int, H: int,
+                            offsets: torch.Tensor, weight: torch.Tensor, eps: float):
+    """``t5enc_assemble`` without N (rqb200_t5enc_assemble_capacity), one launch, for a pass that cannot read offsets[B] on the
+    host (a CUDA-graph capture): x, out and src hold B * S rows, rows offsets[B] .. B * S - 1 being x = out = 0 and src = -1.
+    The attention kernels neither read nor write those rows, and ``t5dec_add_norm`` keeps a zero row zero."""
+    B, n = mask.shape
+    rows = B * t5enc_len(n, H, sep_row is not None, user_table is not None)
+    return _t5enc_assemble("t5enc_assemble_capacity", mask, ids, user_ids, item_table, sep_row, user_table, K, H, offsets, rows,
+                           weight, eps)
+
+
+def _t5enc_assemble(name, mask, ids, user_ids, item_table, sep_row, user_table, K, H, offsets, n_kept, weight, eps):
     _need_cuda(mask, ids, user_ids, item_table, sep_row, user_table, offsets, weight)
     if (user_ids is None) != (user_table is None):
         raise ValueError("user_ids and user_table go together")
@@ -1438,10 +1455,10 @@ def t5enc_assemble(mask: torch.Tensor, ids: torch.Tensor, user_ids: Optional[tor
     src = torch.empty(n_kept, dtype=torch.int32, device=mask.device)
     slot = torch.empty((B, S), dtype=torch.int32, device=mask.device)
     with torch.cuda.device(mask.device):
-        _lib.check(_lib.load().rqb200_t5enc_assemble(
+        _lib.check(getattr(_lib.load(), "rqb200_" + name)(
             _p(mask), _p(ids), ids.stride(0), _p(user_ids), user_ids.stride(0) if user_ids is not None else 0, _p(item_table),
             item_table.shape[0], _p(sep_row), _p(user_table), user_table.shape[0] if user_table is not None else 0, int(K), B, n, H,
-            D, _p(offsets), _p(weight), float(eps), _p(x), _p(out), _p(src), _p(slot), _stream()), "t5enc_assemble")
+            D, _p(offsets), _p(weight), float(eps), _p(x), _p(out), _p(src), _p(slot), _stream()), name)
     _count(1)
     return x, out, src, slot
 
@@ -1453,17 +1470,18 @@ def t5enc_rel_bias(bias: torch.Tensor) -> torch.Tensor:
 
 
 def t5enc_attention(qkv: torch.Tensor, src: torch.Tensor, offsets: torch.Tensor, key_mask: torch.Tensor, rel: torch.Tensor,
-                    S: int) -> torch.Tensor:
+                    S: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Bidirectional T5 self-attention among each history's packed rows (rqb200_t5enc_attention), one launch.  qkv [N, 3 inner]
     (q | k | v), src / offsets / key_mask as ``t5enc_assemble`` / ``t5enc_offsets`` give them, rel [heads, 2S - 1] from
-    ``t5enc_rel_bias`` -> [N, inner]."""
-    return _t5enc_attention_eval("t5enc_attention", qkv, src, offsets, key_mask, rel, S)
+    ``t5enc_rel_bias`` -> [N, inner].  ``out``: a contiguous fp32 [N, inner] tensor to write instead of a new one; its rows past
+    offsets[B] (``t5enc_assemble_capacity``'s) are not written and keep their values."""
+    return _t5enc_attention_eval("t5enc_attention", qkv, src, offsets, key_mask, rel, S, out)
 
 
 def t5enc_attention_tc(qkv: torch.Tensor, src: torch.Tensor, offsets: torch.Tensor, key_mask: torch.Tensor, rel: torch.Tensor,
-                       S: int) -> torch.Tensor:
+                       S: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``t5enc_attention`` with its products on TF32 tensor cores (rqb200_t5enc_attention_tc, csrc/t5enc_tc.cu), one launch."""
-    return _t5enc_attention_eval("t5enc_attention_tc", qkv, src, offsets, key_mask, rel, S)
+    return _t5enc_attention_eval("t5enc_attention_tc", qkv, src, offsets, key_mask, rel, S, out)
 
 
 def _rows_of16(t: torch.Tensor, width: int, what: str) -> torch.Tensor:
@@ -1472,8 +1490,8 @@ def _rows_of16(t: torch.Tensor, width: int, what: str) -> torch.Tensor:
     return t.contiguous() if t.stride(0) % 4 or t.data_ptr() % 16 else t
 
 
-def _t5enc_attention_eval(name, qkv, src, offsets, key_mask, rel, S):
-    _need_cuda(qkv, src, offsets, key_mask, rel)
+def _t5enc_attention_eval(name, qkv, src, offsets, key_mask, rel, S, out=None):
+    _need_cuda(qkv, src, offsets, key_mask, rel, out)
     rel = _f32c(rel)
     heads = rel.shape[0]
     if rel.shape != (heads, 2 * S - 1):
@@ -1484,7 +1502,10 @@ def _t5enc_attention_eval(name, qkv, src, offsets, key_mask, rel, S):
     if offsets.dtype != torch.int32 or src.dtype != torch.int32 or src.shape != (qkv.shape[0],) or key_mask.shape != (B,):
         raise ValueError("src must be int32 [N] with N = qkv rows, offsets int32 [B + 1], key_mask [B]")
     key_mask = _f32c(key_mask)
-    out = torch.empty((qkv.shape[0], inner), dtype=torch.float32, device=qkv.device)
+    if out is None:
+        out = torch.empty((qkv.shape[0], inner), dtype=torch.float32, device=qkv.device)
+    elif out.dtype != torch.float32 or out.shape != (qkv.shape[0], inner) or not out.is_contiguous() or out.data_ptr() % 16:
+        raise ValueError(f"out must be a contiguous, 16-byte aligned fp32 [{qkv.shape[0]}, {inner}] tensor")
     with torch.cuda.device(qkv.device):
         _lib.check(getattr(_lib.load(), "rqb200_" + name)(_p(qkv), qkv.stride(0), _p(src), _p(offsets), _p(key_mask), _p(rel), B,
                                                          S, heads, _p(out), out.stride(0), _stream()), name)
