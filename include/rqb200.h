@@ -328,6 +328,57 @@ int rqb200_sid_trie_sample_select_wide_including(const float* probas, int64_t pr
                                                  int64_t* samples, float* samp_log_p, int* reject, void* workspace,
                                                  size_t workspace_bytes, int cluster, const int* in_pos, const int64_t* in_keys,
                                                  const int* in_count, int in_M, int in_H, void* stream);
+/* sid_trie_sample_select_warped : one level of the sampled search drawn from the head's logits at a temperature and within a
+ *                    top-p nucleus (the same kernel as sid_trie_sample_select, in its warped mode).  Per beam row x:
+ *                      p_T = expf((x - max x) / temperature) / S, S their fp32 sum; N = {c : p_T[c] >= t}, t the largest p_T
+ *                      whose codes at or above it hold at least top_p of the total mass (integer fixed-point sums, 2^-40 units;
+ *                      ties at t all in; top_p = 1: every code); the beam draws the min(nc, |N+|) largest p_T / noise over
+ *                      N+ = the codes of N with p_T > 0 (equal ratios by ascending code); the other slots are -inf fillers.
+ *                    A drawn code scores (x[c] - lse) + log_probas[beam], lse as sid_trie_beam_topk computes it, -inf off the
+ *                    trie or blocked by the filter; samp_log_p = x[c] - lse (-inf for a filler).  Selection as
+ *                    sid_trie_sample_select.
+ *   logits           [B * kp, K] fp32 rows (row stride logits_stride), in place of probas
+ *   bad              int32 device counter or null: ADDED the number of beam rows holding a NaN or +inf, or all -inf
+ *   temperature      finite, > 0;  top_p in (0, 1]; RQB_ERR_INVALID otherwise
+ * _excluding / _including take the filter arguments of sid_trie_sample_select_excluding / _including after top_p; the _wide
+ * variants are sid_trie_sample_select_wide's cluster kernel in the same mode (workspace and cluster before temperature). */
+int rqb200_sid_trie_sample_select_warped(const float* logits, int64_t logits_stride, const float* noise, int64_t noise_stride,
+                                         const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k,
+                                         int C, int K, const void* prefix_workspace, int64_t* out_generated, float* out_log_probas,
+                                         int64_t* out_parent, int64_t* samples, float* samp_log_p, int* bad, float temperature,
+                                         float top_p, void* stream);
+int rqb200_sid_trie_sample_select_warped_excluding(const float* logits, int64_t logits_stride, const float* noise,
+                                                   int64_t noise_stride, const int64_t* generated, const float* log_probas, int B,
+                                                   int kp, int nc, int h, int k, int C, int K, const void* prefix_workspace,
+                                                   int64_t* out_generated, float* out_log_probas, int64_t* out_parent,
+                                                   int64_t* samples, float* samp_log_p, int* bad, float temperature, float top_p,
+                                                   const int* ex_pos, const int64_t* ex_blocked, const int* ex_count, int ex_M,
+                                                   int ex_H, void* stream);
+int rqb200_sid_trie_sample_select_warped_including(const float* logits, int64_t logits_stride, const float* noise,
+                                                   int64_t noise_stride, const int64_t* generated, const float* log_probas, int B,
+                                                   int kp, int nc, int h, int k, int C, int K, const void* prefix_workspace,
+                                                   int64_t* out_generated, float* out_log_probas, int64_t* out_parent,
+                                                   int64_t* samples, float* samp_log_p, int* bad, float temperature, float top_p,
+                                                   const int* in_pos, const int64_t* in_keys, const int* in_count, int in_M,
+                                                   int in_H, void* stream);
+int rqb200_sid_trie_sample_select_warped_wide(const float* logits, int64_t logits_stride, const float* noise, int64_t noise_stride,
+                                              const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k,
+                                              int C, int K, const void* prefix_workspace, int64_t* out_generated,
+                                              float* out_log_probas, int64_t* out_parent, int64_t* samples, float* samp_log_p,
+                                              int* bad, void* workspace, size_t workspace_bytes, int cluster, float temperature,
+                                              float top_p, void* stream);
+int rqb200_sid_trie_sample_select_warped_wide_excluding(
+    const float* logits, int64_t logits_stride, const float* noise, int64_t noise_stride, const int64_t* generated,
+    const float* log_probas, int B, int kp, int nc, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
+    float* out_log_probas, int64_t* out_parent, int64_t* samples, float* samp_log_p, int* bad, void* workspace,
+    size_t workspace_bytes, int cluster, float temperature, float top_p, const int* ex_pos, const int64_t* ex_blocked,
+    const int* ex_count, int ex_M, int ex_H, void* stream);
+int rqb200_sid_trie_sample_select_warped_wide_including(
+    const float* logits, int64_t logits_stride, const float* noise, int64_t noise_stride, const int64_t* generated,
+    const float* log_probas, int B, int kp, int nc, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
+    float* out_log_probas, int64_t* out_parent, int64_t* samples, float* samp_log_p, int* bad, void* workspace,
+    size_t workspace_bytes, int cluster, float temperature, float top_p, const int* in_pos, const int64_t* in_keys,
+    const int* in_count, int in_M, int in_H, void* stream);
 
 /* The trie's level arrays as plain device arrays (the exact ranking decodes one row per node).
  * sid_trie_counts : counts int32 [C + 1] = the node count of every level (counts[0] = 1, the root); one tiny launch.

@@ -100,6 +100,25 @@ _SIGNATURES = {
     "rqb200_sid_trie_sample_select_wide_including": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int,
                                                              c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_size,
                                                              c_int, c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
+    "rqb200_sid_trie_sample_select_warped": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int,
+                                                     c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_f32, c_f32, c_vp]),
+    "rqb200_sid_trie_sample_select_warped_excluding": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int,
+                                                               c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_f32,
+                                                               c_f32, c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
+    "rqb200_sid_trie_sample_select_warped_including": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int,
+                                                               c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_f32,
+                                                               c_f32, c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
+    "rqb200_sid_trie_sample_select_warped_wide": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int,
+                                                          c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_size,
+                                                          c_int, c_f32, c_f32, c_vp]),
+    "rqb200_sid_trie_sample_select_warped_wide_excluding": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int,
+                                                                    c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                                                    c_vp, c_vp, c_size, c_int, c_f32, c_f32, c_vp, c_vp, c_vp,
+                                                                    c_int, c_int, c_vp]),
+    "rqb200_sid_trie_sample_select_warped_wide_including": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int,
+                                                                    c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                                                    c_vp, c_vp, c_size, c_int, c_f32, c_f32, c_vp, c_vp, c_vp,
+                                                                    c_int, c_int, c_vp]),
     "rqb200_sid_items_workspace_bytes": (c_size, [c_i64, c_int, c_int]),
     "rqb200_sid_items_build": (c_int, [c_vp, c_i64, c_int, c_int, c_vp, c_size, c_vp]),
     "rqb200_sid_items_lookup": (c_int, [c_vp, c_vp, c_i64, c_i64, c_int, c_vp, c_vp]),

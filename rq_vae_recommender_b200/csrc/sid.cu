@@ -802,25 +802,150 @@ __device__ void sid_warp_top_n(const unsigned int* key, int K, int n, int* hist,
   __syncwarp();
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// The warped draw: a sampling mode of sid_sample_select_kernel / sid_sample_select_wide_kernel that draws from the head's
+// logits at a temperature T and within a top-p nucleus.  Per beam row x[0, K), one warp:
+//   m = max x,  lse = m + logf(sum expf(x - m))             (sid_beam_topk_kernel's statement and order)
+//   p_T[c] = expf((x[c] - m) / T) / S,  S = sum_c expf((x[c] - m) / T)   (fp32, lane-strided sums, then a butterfly)
+//   N = {c : p_T[c] >= t}, t the largest p_T with mass(p_T >= t) >= top_p * mass(all)   (ties at t all in; top_p = 1: all)
+// where mass sums fx(p_T) = floor(p_T * 2^40) as 64-bit integers, so it is independent of any order.  The keys of the codes
+// of N with p_T > 0 (N+) are sid_topk_key(p_T / q), those of every other code 0 (below every ratio's key: sid_warp_top_n
+// draws them last, as -inf fillers).  A row with a NaN or +inf, or all -inf, has every key 0 and is reported bad.
+#define SID_FX_ONE 1099511627776.f                          // 2^40: fixed-point unit of the nucleus masses
+
+__device__ __forceinline__ unsigned long long sid_fx(float p) { return __float2ull_rz(p * SID_FX_ONE); }
+
+// One warp: the bits of t over the p_T bits key[0, K) (non-negative floats: their bits order as their values), given
+// 0 < target <= the total mass.  Radix selection on 7-bit digits (bits 31..4 in four passes, then 3..0) of integer mass
+// histograms hist[128]: each pass keeps the largest digit whose bin, with the larger bins and the mass above, reaches target.
+// The chosen bin always holds mass, so t is some code's p_T.
+__device__ __forceinline__ unsigned int sid_nucleus_threshold(const unsigned int* key, int K, unsigned long long target, unsigned long long* hist,
+                                              int lane) {
+  unsigned int prefix = 0, pmask = 0;
+  unsigned long long above = 0;                             // mass of the codes above the decided digits
+  for (int pass = 0; pass < 5; ++pass) {
+    const int shift = pass < 4 ? 25 - 7 * pass : 0;
+    const unsigned int dmask = pass < 4 ? 127u : 15u;
+    for (int i = lane; i < 128; i += 32) hist[i] = 0;
+    __syncwarp();
+    for (int c = lane; c < K; c += 32) {
+      const unsigned int v = key[c];
+      if ((v & pmask) != prefix) continue;
+      const unsigned long long f = sid_fx(__uint_as_float(v));
+      if (f) atomicAdd(&hist[(v >> shift) & dmask], f);
+    }
+    __syncwarp();
+    unsigned long long s = 0;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) s += hist[lane * 4 + j];
+    unsigned long long suf = s;                             // mass in bins >= lane * 4
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned long long t = __shfl_down_sync(0xffffffffu, suf, o);
+      if (lane + o < 32) suf += t;
+    }
+    const int owner = 31 - __clz(__ballot_sync(0xffffffffu, above + suf >= target));
+    int digit = 0;
+    unsigned long long acc = 0;
+    if (lane == owner) {
+      acc = above + suf - s;
+      for (int j = 3; j >= 0; --j) {
+        const unsigned long long c = hist[lane * 4 + j];
+        if (acc + c >= target) { digit = lane * 4 + j; break; }
+        acc += c;
+      }
+    }
+    digit = __shfl_sync(0xffffffffu, digit, owner);
+    above = __shfl_sync(0xffffffffu, acc, owner);
+    prefix |= (unsigned int)digit << shift;
+    pmask |= dmask << shift;
+    __syncwarp();
+  }
+  return prefix;
+}
+
+struct SidWarpedRow {
+  float lse;
+  bool bad;
+};
+
+// One warp, beam row x / noise q: key[0, K) = the warped draw's keys (above), hist = 128 64-bit bins of scratch (8-byte
+// aligned).  Returns the row's lse and whether it is bad.  The warp is synchronised on return.
+__device__ __forceinline__ SidWarpedRow sid_warped_keys(const float* __restrict__ x, const float* __restrict__ q, int K, float temp, double top_p,
+                                        unsigned int* key, unsigned long long* hist, int lane) {
+  float m = -INFINITY;
+  bool odd = false;
+  for (int c = lane; c < K; c += 32) {
+    const float v = x[c];
+    m = fmaxf(m, v);
+    odd |= v != v || v == INFINITY;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  odd = __any_sync(0xffffffffu, odd);
+  const bool bad = odd || m == -INFINITY;
+  float sum = 0.f, st = 0.f;
+  for (int c = lane; c < K; c += 32) {
+    const float v = x[c];
+    sum += expf(v - m);
+    const float e = expf(__fdiv_rn(__fsub_rn(v, m), temp));
+    st = __fadd_rn(st, e);
+    key[c] = bad ? 0u : __float_as_uint(e);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    sum += __shfl_xor_sync(0xffffffffu, sum, o);            // every lane ends with the same bits
+    st = __fadd_rn(st, __shfl_xor_sync(0xffffffffu, st, o));
+  }
+  const float lse = m + logf(sum);
+  __syncwarp();
+  if (bad) return {lse, true};
+  unsigned long long total = 0;                             // S >= 1: the maximum's term is expf(0) = 1
+  for (int c = lane; c < K; c += 32) {
+    const float p = __fdiv_rn(__uint_as_float(key[c]), st);
+    key[c] = __float_as_uint(p);
+    total += sid_fx(p);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
+  __syncwarp();
+  unsigned int t = 0;
+  if (top_p < 1.0) {
+    const unsigned long long target = (unsigned long long)ceil(top_p * (double)total);
+    t = sid_nucleus_threshold(key, K, target < 1 ? 1 : target, hist, lane);
+  }
+  for (int c = lane; c < K; c += 32) {
+    const unsigned int v = key[c];
+    key[c] = (v >= t && v != 0u) ? sid_topk_key(__fdiv_rn(__uint_as_float(v), q[c])) : 0u;
+  }
+  __syncwarp();
+  return {lse, false};
+}
+
+template <bool WARP>
 static size_t sid_sample_smem(int kp, int nc, int K) {
   const int W = kp < SID_SAMPLE_MAX_WARPS ? kp : SID_SAMPLE_MAX_WARPS;
   const size_t E = (size_t)kp * nc;
-  return E * (sizeof(int64_t) + sizeof(float) + 1) + (size_t)W * (K + 256 + 2 * nc + (K + 31) / 32) * 4;
+  return E * (sizeof(int64_t) + sizeof(float) + 1) + (size_t)W * (K + 256 + 2 * nc + (K + 31) / 32) * 4 + (WARP ? 4 : 0);
 }
 
-template <int FILTER>                                       // SidFilterMode: the filter's code is compiled only with one
-__global__ void __launch_bounds__(SID_SAMPLE_MAX_WARPS * 32) sid_sample_select_kernel(
+// WARP: the warped draw (above) from the head's logits (`probas` holds them), else the untempered draw from the softmax.
+template <int FILTER, bool WARP>                            // SidFilterMode: the filter's code is compiled only with one
+__global__ void __launch_bounds__(SID_SAMPLE_MAX_WARPS * 32, WARP ? 1 : 0) sid_sample_select_kernel(
     const float* __restrict__ probas, int64_t p_stride, const float* __restrict__ noise, int64_t n_stride,
     const int64_t* __restrict__ generated, const float* __restrict__ log_probas, int kp, int nc, int h, int k, int K, SidTrie trie,
     int64_t* __restrict__ out_generated, float* __restrict__ out_log_probas, int64_t* __restrict__ out_parent,
-    int64_t* __restrict__ samples, float* __restrict__ samp_log_p, int* __restrict__ reject, SidExcl ex) {
+    int64_t* __restrict__ samples, float* __restrict__ samp_log_p, int* __restrict__ reject, SidExcl ex, float temp,
+    double top_p) {
   extern __shared__ __align__(16) unsigned char sid_smem[];
   const int W = blockDim.x >> 5, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int b = blockIdx.x, E = kp * nc, KW = (K + 31) >> 5;
   int64_t* s_tok = reinterpret_cast<int64_t*>(sid_smem);                          // [E] candidate tokens
   float* s_score = reinterpret_cast<float*>(s_tok + E);                          // [E] candidate scores
   unsigned int* s_key = reinterpret_cast<unsigned int*>(s_score + E) + (size_t)w * K;                      // [W][K]
-  int* s_hist = reinterpret_cast<int*>(reinterpret_cast<unsigned int*>(s_score + E) + (size_t)W * K) + w * 256;   // [W][256]
+  unsigned int* s_key_end = reinterpret_cast<unsigned int*>(s_score + E) + (size_t)W * K;
+  if (WARP) s_key_end += ((E + W * K) & 1);                 // the warped mode's 64-bit histograms: 8-byte aligned
+  int* s_hist = reinterpret_cast<int*>(s_key_end) + w * 256;                                               // [W][256]
   unsigned int* s_sk = reinterpret_cast<unsigned int*>(s_hist - w * 256 + W * 256) + w * nc;               // [W][nc]
   int* s_si = reinterpret_cast<int*>(s_sk - w * nc + W * nc) + w * nc;                                     // [W][nc]
   unsigned int* s_mask = reinterpret_cast<unsigned int*>(s_si - w * nc + W * nc) + w * KW;                 // [W][KW]
@@ -829,26 +954,41 @@ __global__ void __launch_bounds__(SID_SAMPLE_MAX_WARPS * 32) sid_sample_select_k
     const int64_t row = (int64_t)b * kp + beam;
     const float* p = probas + row * p_stride;
     const float* q = noise + row * n_stride;
-    bool bad = false, nonzero = false;
-    for (int i = lane; i < K; i += 32) {
-      const float pv = p[i];
-      bad |= !(pv >= 0.f) || pv == INFINITY;               // what torch.multinomial rejects: NaN, +-inf, negative ...
-      nonzero |= pv != 0.f;                                 // ... or a zero sum
-      s_key[i] = sid_topk_key(__fdiv_rn(pv, q[i]));
+    float lse = 0.f;
+    if (WARP) {
+      const SidWarpedRow wr = sid_warped_keys(p, q, K, temp, top_p, s_key, reinterpret_cast<unsigned long long*>(s_hist), lane);
+      lse = wr.lse;
+      if (reject && lane == 0 && wr.bad) atomicAdd(reject, 1);
+    } else {
+      bool bad = false, nonzero = false;
+      for (int i = lane; i < K; i += 32) {
+        const float pv = p[i];
+        bad |= !(pv >= 0.f) || pv == INFINITY;             // what torch.multinomial rejects: NaN, +-inf, negative ...
+        nonzero |= pv != 0.f;                               // ... or a zero sum
+        s_key[i] = sid_topk_key(__fdiv_rn(pv, q[i]));
+      }
+      bad = __any_sync(0xffffffffu, bad);
+      nonzero = __any_sync(0xffffffffu, nonzero);
+      if (reject && lane == 0 && (bad || !nonzero)) atomicAdd(&reject[bad ? 0 : 1], 1);
     }
-    bad = __any_sync(0xffffffffu, bad);
-    nonzero = __any_sync(0xffffffffu, nonzero);
-    if (reject && lane == 0 && (bad || !nonzero)) atomicAdd(&reject[bad ? 0 : 1], 1);
     __syncwarp();
     sid_warp_top_n(s_key, K, nc, s_hist, s_sk, s_si, s_tok + beam * nc, lane);
     sid_beam_mask<FILTER>(trie, ex, b, generated + row * h, h, K, s_mask, lane);
     const float plp = log_probas ? log_probas[row] : 0.f;
     for (int r = lane; r < nc; r += 32) {
       const int64_t tok = s_tok[beam * nc + r];
-      const float lp = logf(p[tok]);
-      if (samples) samples[row * nc + r] = tok;
-      if (samp_log_p) samp_log_p[row * nc + r] = lp;
-      s_score[beam * nc + r] = sid_extension_score(sid_mask_has(s_mask, (int)tok), lp + plp);
+      if (WARP) {                                           // the model's log-probability; key 0: a filler outside N+
+        const bool drawn = s_key[tok] != 0u;
+        const float lp = drawn ? __fsub_rn(p[tok], lse) : -INFINITY;
+        if (samples) samples[row * nc + r] = tok;
+        if (samp_log_p) samp_log_p[row * nc + r] = lp;
+        s_score[beam * nc + r] = sid_extension_score(drawn && sid_mask_has(s_mask, (int)tok), __fadd_rn(lp, plp));
+      } else {
+        const float lp = logf(p[tok]);
+        if (samples) samples[row * nc + r] = tok;
+        if (samp_log_p) samp_log_p[row * nc + r] = lp;
+        s_score[beam * nc + r] = sid_extension_score(sid_mask_has(s_mask, (int)tok), lp + plp);
+      }
       s_taken[beam * nc + r] = 0;
     }
   }
@@ -869,13 +1009,24 @@ static int sid_excl_of(const int* pos, const int64_t* keys, const int* count, in
   return RQB_OK;
 }
 
+// The sampling temperature and nucleus mass of a warped draw: finite T > 0, 0 < top_p <= 1
+static int sid_check_warp(float temp, float top_p, const char* what) {
+  RQB_CHECK_ARG(temp > 0.f && temp < INFINITY && top_p > 0.f && top_p <= 1.f,
+                "%s: need a finite temperature > 0 and 0 < top_p <= 1 (temperature = %g, top_p = %g)", what, (double)temp,
+                (double)top_p);
+  return RQB_OK;
+}
+
+template <bool WARP>
 static int sid_sample_select(const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride,
                              const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k, int C, int K,
                              const void* prefix_workspace, int64_t* out_generated, float* out_log_probas, int64_t* out_parent,
-                             int64_t* samples, float* samp_log_p, int* reject, const SidExcl& ex, void* stream) {
+                             int64_t* samples, float* samp_log_p, int* reject, const SidExcl& ex, float temp, float top_p,
+                             void* stream) {
   RQB_CHECK_ARG(B >= 0 && kp > 0 && nc > 0 && h >= 0 && h < C && C <= 8 && k > 0 && K > 0 && probas_stride >= K &&
                     noise_stride >= K, "sid_trie_sample_select: bad argument (B=%d kp=%d nc=%d h=%d k=%d C=%d K=%d)", B, kp, nc, h,
                 k, C, K);
+  if (WARP && sid_check_warp(temp, top_p, "sid_trie_sample_select_warped") != RQB_OK) return RQB_ERR_INVALID;
   if (nc > K || K > SID_SAMPLE_MAX_K || kp * nc > SID_BEAM_MAX_E || k > 32) {
     rqb_set_error("sid_trie_sample_select: need nc <= K <= %d, kp * nc <= %d, k <= 32 (nc = %d, K = %d, kp * nc = %d, k = %d)",
                   SID_SAMPLE_MAX_K, SID_BEAM_MAX_E, nc, K, kp * nc, k);
@@ -885,16 +1036,16 @@ static int sid_sample_select(const float* probas, int64_t probas_stride, const f
   RQB_CHECK_ARG(probas && noise && prefix_workspace && out_generated && out_log_probas && out_parent && (h == 0 || generated) &&
                     (h == 0 || log_probas), "sid_trie_sample_select: null pointer");
   const int W = kp < SID_SAMPLE_MAX_WARPS ? kp : SID_SAMPLE_MAX_WARPS;
-  const size_t smem = sid_sample_smem(kp, nc, K);
+  const size_t smem = sid_sample_smem<WARP>(kp, nc, K);
   const int mode = sid_filter_mode(ex);
-  auto kernel = mode == SID_FILTER_INCLUDE ? sid_sample_select_kernel<SID_FILTER_INCLUDE>
-                : mode == SID_FILTER_EXCLUDE ? sid_sample_select_kernel<SID_FILTER_EXCLUDE>
-                                             : sid_sample_select_kernel<SID_FILTER_NONE>;
+  auto kernel = mode == SID_FILTER_INCLUDE ? sid_sample_select_kernel<SID_FILTER_INCLUDE, WARP>
+                : mode == SID_FILTER_EXCLUDE ? sid_sample_select_kernel<SID_FILTER_EXCLUDE, WARP>
+                                             : sid_sample_select_kernel<SID_FILTER_NONE, WARP>;
   RQB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kernel<<<B, W * 32, smem, reinterpret_cast<cudaStream_t>(stream)>>>(
       probas, probas_stride, noise, noise_stride, generated, log_probas, kp, nc, h, k, K,
       SidTrie{reinterpret_cast<const unsigned char*>(prefix_workspace), h + 1}, out_generated, out_log_probas, out_parent, samples,
-      samp_log_p, reject, ex);
+      samp_log_p, reject, ex, temp, top_p);
   RQB_LAUNCH_CHECK();
   return RQB_OK;
 }
@@ -904,8 +1055,9 @@ extern "C" int rqb200_sid_trie_sample_select(const float* probas, int64_t probas
                                              int C, int K, const void* prefix_workspace, int64_t* out_generated,
                                              float* out_log_probas, int64_t* out_parent, int64_t* samples, float* samp_log_p,
                                              int* reject, void* stream) {
-  return sid_sample_select(probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K, prefix_workspace,
-                           out_generated, out_log_probas, out_parent, samples, samp_log_p, reject, SidExcl{}, stream);
+  return sid_sample_select<false>(probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K,
+                                  prefix_workspace, out_generated, out_log_probas, out_parent, samples, samp_log_p, reject, SidExcl{},
+                                  1.f, 1.f, stream);
 }
 
 extern "C" int rqb200_sid_trie_sample_select_excluding(
@@ -916,8 +1068,9 @@ extern "C" int rqb200_sid_trie_sample_select_excluding(
   SidExcl ex;
   const int rc = sid_excl_of(ex_pos, ex_blocked, ex_count, ex_M, ex_H, h + 1, "sid_trie_sample_select_excluding", ex);
   if (rc != RQB_OK) return rc;
-  return sid_sample_select(probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K, prefix_workspace,
-                           out_generated, out_log_probas, out_parent, samples, samp_log_p, reject, ex, stream);
+  return sid_sample_select<false>(probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K,
+                                  prefix_workspace, out_generated, out_log_probas, out_parent, samples, samp_log_p, reject, ex, 1.f,
+                                  1.f, stream);
 }
 
 extern "C" int rqb200_sid_trie_sample_select_including(
@@ -928,8 +1081,46 @@ extern "C" int rqb200_sid_trie_sample_select_including(
   SidExcl in;
   const int rc = sid_excl_of(in_pos, in_keys, in_count, in_M, in_H, h + 1, "sid_trie_sample_select_including", in, true);
   if (rc != RQB_OK) return rc;
-  return sid_sample_select(probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K, prefix_workspace,
-                           out_generated, out_log_probas, out_parent, samples, samp_log_p, reject, in, stream);
+  return sid_sample_select<false>(probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K,
+                                  prefix_workspace, out_generated, out_log_probas, out_parent, samples, samp_log_p, reject, in, 1.f,
+                                  1.f, stream);
+}
+
+extern "C" int rqb200_sid_trie_sample_select_warped(const float* logits, int64_t logits_stride, const float* noise,
+                                                    int64_t noise_stride, const int64_t* generated, const float* log_probas, int B,
+                                                    int kp, int nc, int h, int k, int C, int K, const void* prefix_workspace,
+                                                    int64_t* out_generated, float* out_log_probas, int64_t* out_parent,
+                                                    int64_t* samples, float* samp_log_p, int* bad, float temperature, float top_p,
+                                                    void* stream) {
+  return sid_sample_select<true>(logits, logits_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K,
+                                 prefix_workspace, out_generated, out_log_probas, out_parent, samples, samp_log_p, bad, SidExcl{},
+                                 temperature, top_p, stream);
+}
+
+extern "C" int rqb200_sid_trie_sample_select_warped_excluding(
+    const float* logits, int64_t logits_stride, const float* noise, int64_t noise_stride, const int64_t* generated,
+    const float* log_probas, int B, int kp, int nc, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
+    float* out_log_probas, int64_t* out_parent, int64_t* samples, float* samp_log_p, int* bad, float temperature, float top_p,
+    const int* ex_pos, const int64_t* ex_blocked, const int* ex_count, int ex_M, int ex_H, void* stream) {
+  SidExcl ex;
+  const int rc = sid_excl_of(ex_pos, ex_blocked, ex_count, ex_M, ex_H, h + 1, "sid_trie_sample_select_warped_excluding", ex);
+  if (rc != RQB_OK) return rc;
+  return sid_sample_select<true>(logits, logits_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K,
+                                 prefix_workspace, out_generated, out_log_probas, out_parent, samples, samp_log_p, bad, ex,
+                                 temperature, top_p, stream);
+}
+
+extern "C" int rqb200_sid_trie_sample_select_warped_including(
+    const float* logits, int64_t logits_stride, const float* noise, int64_t noise_stride, const int64_t* generated,
+    const float* log_probas, int B, int kp, int nc, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
+    float* out_log_probas, int64_t* out_parent, int64_t* samples, float* samp_log_p, int* bad, float temperature, float top_p,
+    const int* in_pos, const int64_t* in_keys, const int* in_count, int in_M, int in_H, void* stream) {
+  SidExcl in;
+  const int rc = sid_excl_of(in_pos, in_keys, in_count, in_M, in_H, h + 1, "sid_trie_sample_select_warped_including", in, true);
+  if (rc != RQB_OK) return rc;
+  return sid_sample_select<true>(logits, logits_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K,
+                                 prefix_workspace, out_generated, out_log_probas, out_parent, samples, samp_log_p, bad, in,
+                                 temperature, top_p, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -1967,14 +2158,14 @@ __global__ void __launch_bounds__(SID_WIDE_TOPK_THREADS, 2) sid_beam_topk_wide_k
 
 // The sampled level (sid_sample_select_kernel's draws and scores) for history blockIdx.x / cs.  Each of the CTA's warps draws
 // one beam at a time into its own buffers; every draw's token goes to ws_tok [B][kp * nc] and its score key to shared memory
-// (KEYS_IN_SMEM) or ws_key [B][kp * nc].
-template <bool KEYS_IN_SMEM, int FILTER>
-__global__ void __launch_bounds__(SID_WIDE_SAMPLE_THREADS) sid_sample_select_wide_kernel(
+// (KEYS_IN_SMEM) or ws_key [B][kp * nc].  WARP: the warped draw from the head's logits, as sid_sample_select_kernel's.
+template <bool KEYS_IN_SMEM, int FILTER, bool WARP>
+__global__ void __launch_bounds__(SID_WIDE_SAMPLE_THREADS, WARP ? 1 : 0) sid_sample_select_wide_kernel(
     const float* __restrict__ probas, int64_t p_stride, const float* __restrict__ noise, int64_t n_stride,
     const int64_t* __restrict__ generated, const float* __restrict__ log_probas, int kp, int nc, int h, int k, int K, int cs,
     int per_cta, SidTrie trie, int64_t* __restrict__ out_generated, float* __restrict__ out_log_probas,
     int64_t* __restrict__ out_parent, int64_t* __restrict__ samples, float* __restrict__ samp_log_p, int* __restrict__ reject,
-    int* __restrict__ ws_tok, unsigned int* __restrict__ ws_key, SidExcl ex) {
+    int* __restrict__ ws_tok, unsigned int* __restrict__ ws_key, SidExcl ex, float temp, double top_p) {
   constexpr int NT = SID_WIDE_SAMPLE_THREADS, IPT = SID_WIDE_MAX_SEL / NT, W = NT >> 5;
   extern __shared__ __align__(16) unsigned char sid_smem[];
   __shared__ SidWideShared s;
@@ -1984,7 +2175,7 @@ __global__ void __launch_bounds__(SID_WIDE_SAMPLE_THREADS) sid_sample_select_wid
   const int beam0 = min(kp, rank * per_cta), nb = min(kp, beam0 + per_cta) - beam0;
   int64_t* s_tok = reinterpret_cast<int64_t*>(sid_smem) + (size_t)w * nc;                                  // [W][nc]
   unsigned int* s_rkey = reinterpret_cast<unsigned int*>(reinterpret_cast<int64_t*>(sid_smem) + (size_t)W * nc);   // [W][K]
-  int* s_hist = reinterpret_cast<int*>(s_rkey + (size_t)W * K) + w * 256;                                   // [W][256]
+  int* s_hist = reinterpret_cast<int*>(s_rkey + (size_t)W * K) + w * 256;   // [W][256], 8-byte aligned (W nc 8 + W K 4 bytes in)
   unsigned int* s_sk = reinterpret_cast<unsigned int*>(s_hist - w * 256 + W * 256) + w * nc;               // [W][nc]
   int* s_si = reinterpret_cast<int*>(s_sk - w * nc + W * nc) + w * nc;                                     // [W][nc]
   unsigned int* s_mask = reinterpret_cast<unsigned int*>(s_si - w * nc + W * nc) + w * KW;                 // [W][KW]
@@ -1997,26 +2188,42 @@ __global__ void __launch_bounds__(SID_WIDE_SAMPLE_THREADS) sid_sample_select_wid
     const int64_t row = (int64_t)b * kp + beam;
     const float* p = probas + row * p_stride;
     const float* q = noise + row * n_stride;
-    bool bad = false, nonzero = false;
-    for (int c = lane; c < K; c += 32) {
-      const float pv = p[c];
-      bad |= !(pv >= 0.f) || pv == INFINITY;
-      nonzero |= pv != 0.f;
-      s_rkey[c] = sid_topk_key(__fdiv_rn(pv, q[c]));
+    float lse = 0.f;
+    if (WARP) {
+      const SidWarpedRow wr = sid_warped_keys(p, q, K, temp, top_p, s_rkey, reinterpret_cast<unsigned long long*>(s_hist), lane);
+      lse = wr.lse;
+      if (reject && lane == 0 && wr.bad) atomicAdd(reject, 1);
+    } else {
+      bool bad = false, nonzero = false;
+      for (int c = lane; c < K; c += 32) {
+        const float pv = p[c];
+        bad |= !(pv >= 0.f) || pv == INFINITY;
+        nonzero |= pv != 0.f;
+        s_rkey[c] = sid_topk_key(__fdiv_rn(pv, q[c]));
+      }
+      bad = __any_sync(0xffffffffu, bad);
+      nonzero = __any_sync(0xffffffffu, nonzero);
+      if (reject && lane == 0 && (bad || !nonzero)) atomicAdd(&reject[bad ? 0 : 1], 1);
     }
-    bad = __any_sync(0xffffffffu, bad);
-    nonzero = __any_sync(0xffffffffu, nonzero);
-    if (reject && lane == 0 && (bad || !nonzero)) atomicAdd(&reject[bad ? 0 : 1], 1);
     __syncwarp();
     sid_warp_top_n(s_rkey, K, nc, s_hist, s_sk, s_si, s_tok, lane);
     sid_beam_mask<FILTER>(trie, ex, b, generated + row * h, h, K, s_mask, lane);
     const float plp = log_probas ? log_probas[row] : 0.f;
     for (int r = lane; r < nc; r += 32) {
       const int64_t tok = s_tok[r];
-      const float lp = logf(p[tok]);
-      if (samples) samples[row * nc + r] = tok;
-      if (samp_log_p) samp_log_p[row * nc + r] = lp;
-      const float sc = sid_extension_score(sid_mask_has(s_mask, (int)tok), lp + plp);
+      float lp, sc;
+      if (WARP) {
+        const bool drawn = s_rkey[tok] != 0u;
+        lp = drawn ? __fsub_rn(p[tok], lse) : -INFINITY;
+        if (samples) samples[row * nc + r] = tok;
+        if (samp_log_p) samp_log_p[row * nc + r] = lp;
+        sc = sid_extension_score(drawn && sid_mask_has(s_mask, (int)tok), __fadd_rn(lp, plp));
+      } else {
+        lp = logf(p[tok]);
+        if (samples) samples[row * nc + r] = tok;
+        if (samp_log_p) samp_log_p[row * nc + r] = lp;
+        sc = sid_extension_score(sid_mask_has(s_mask, (int)tok), lp + plp);
+      }
       const unsigned int key = sid_topk_key(sc == 0.f ? 0.f : sc);
       const int e = beam * nc + r;
       tok_b[e] = (int)tok;
@@ -2214,47 +2421,53 @@ extern "C" size_t rqb200_sid_trie_sample_select_wide_workspace_bytes(int B, int 
   return B < 0 || kp < 0 || nc < 0 ? 0 : (size_t)B * kp * nc * (sizeof(int) + sizeof(unsigned int));
 }
 
-template <int FILTER>
+template <int FILTER, bool WARP>
 static SidWideLaunch sid_sample_select_wide_pick(int kp, int nc, int K, int cs) {
   constexpr int W = SID_WIDE_SAMPLE_THREADS / 32;
   const int per_cta = (kp + cs - 1) / cs;
   const bool keys = (int64_t)per_cta * nc <= SID_WIDE_SMEM_KEYS;
   const size_t smem = (size_t)W * (nc * sizeof(int64_t) + (K + 256 + 2 * nc + (K + 31) / 32) * 4) +
                       (keys ? (size_t)per_cta * nc * sizeof(unsigned int) : 0);
-  return {keys ? (const void*)sid_sample_select_wide_kernel<true, FILTER> : (const void*)sid_sample_select_wide_kernel<false, FILTER>,
+  return {keys ? (const void*)sid_sample_select_wide_kernel<true, FILTER, WARP>
+               : (const void*)sid_sample_select_wide_kernel<false, FILTER, WARP>,
           smem, per_cta};
 }
 
-template <int FILTER>
+template <int FILTER, bool WARP>
 static int sid_sample_select_wide_launch(const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride,
                                          const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k,
                                          int K, const SidTrie& trie, int64_t* out_generated, float* out_log_probas,
                                          int64_t* out_parent, int64_t* samples, float* samp_log_p, int* reject, int* ws_tok,
-                                         unsigned int* ws_key, const SidExcl& ex, int cluster, cudaStream_t st) {
+                                         unsigned int* ws_key, const SidExcl& ex, int cluster, float temp, float top_p,
+                                         cudaStream_t st) {
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr;
   SidWideLaunch L;
   int cs = 0;
   const int rc = sid_wide_plan(B, kp, (int64_t)kp * K, cluster, SID_WIDE_SAMPLE_THREADS,
-                               [&](int c) { return sid_sample_select_wide_pick<FILTER>(kp, nc, K, c); }, st,
+                               [&](int c) { return sid_sample_select_wide_pick<FILTER, WARP>(kp, nc, K, c); }, st,
                                "sid_trie_sample_select_wide", cfg, attr, L, cs);
   if (rc != RQB_OK) return rc;
   SidTrie tr = trie;
   SidExcl fx = ex;
+  double mass = top_p;                                      // the kernel's nucleus mass parameter
   void* args[] = {&probas, &probas_stride, &noise, &noise_stride, &generated, &log_probas, &kp, &nc, &h, &k, &K, &cs, &L.per_cta,
-                  &tr, &out_generated, &out_log_probas, &out_parent, &samples, &samp_log_p, &reject, &ws_tok, &ws_key, &fx};
+                  &tr, &out_generated, &out_log_probas, &out_parent, &samples, &samp_log_p, &reject, &ws_tok, &ws_key, &fx,
+                  &temp, &mass};
   RQB_CUDA(cudaLaunchKernelExC(&cfg, L.fn, args));
   return RQB_OK;
 }
 
+template <bool WARP>
 static int sid_sample_select_wide(const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride,
                                   const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k, int C, int K,
                                   const void* prefix_workspace, int64_t* out_generated, float* out_log_probas, int64_t* out_parent,
                                   int64_t* samples, float* samp_log_p, int* reject, void* workspace, size_t workspace_bytes,
-                                  int cluster, const SidExcl& ex, void* stream) {
+                                  int cluster, const SidExcl& ex, float temp, float top_p, void* stream) {
   RQB_CHECK_ARG(B >= 0 && kp > 0 && nc > 0 && h >= 0 && h < C && C <= 8 && k > 0 && K > 0 && probas_stride >= K &&
                     noise_stride >= K, "sid_trie_sample_select_wide: bad argument (B=%d kp=%d nc=%d h=%d k=%d C=%d K=%d)", B, kp,
                 nc, h, k, C, K);
+  if (WARP && sid_check_warp(temp, top_p, "sid_trie_sample_select_warped_wide") != RQB_OK) return RQB_ERR_INVALID;
   if (nc > K || K > SID_SAMPLE_MAX_K || nc > SID_WIDE_MAX_NC || kp > SID_WIDE_MAX_BEAMS || k > SID_WIDE_MAX_SEL) {
     rqb_set_error("sid_trie_sample_select_wide: need nc <= K <= %d, nc <= %d, kp <= %d, k <= %d (nc = %d, K = %d, kp = %d, k = %d)",
                   SID_SAMPLE_MAX_K, SID_WIDE_MAX_NC, SID_WIDE_MAX_BEAMS, SID_WIDE_MAX_SEL, nc, K, kp, k);
@@ -2273,17 +2486,17 @@ static int sid_sample_select_wide(const float* probas, int64_t probas_stride, co
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   switch (sid_filter_mode(ex)) {
     case SID_FILTER_INCLUDE:
-      return sid_sample_select_wide_launch<SID_FILTER_INCLUDE>(probas, probas_stride, noise, noise_stride, generated, log_probas, B,
+      return sid_sample_select_wide_launch<SID_FILTER_INCLUDE, WARP>(probas, probas_stride, noise, noise_stride, generated, log_probas, B,
                                                                kp, nc, h, k, K, trie, out_generated, out_log_probas, out_parent,
-                                                               samples, samp_log_p, reject, ws_tok, ws_key, ex, cluster, st);
+                                                               samples, samp_log_p, reject, ws_tok, ws_key, ex, cluster, temp, top_p, st);
     case SID_FILTER_EXCLUDE:
-      return sid_sample_select_wide_launch<SID_FILTER_EXCLUDE>(probas, probas_stride, noise, noise_stride, generated, log_probas, B,
+      return sid_sample_select_wide_launch<SID_FILTER_EXCLUDE, WARP>(probas, probas_stride, noise, noise_stride, generated, log_probas, B,
                                                                kp, nc, h, k, K, trie, out_generated, out_log_probas, out_parent,
-                                                               samples, samp_log_p, reject, ws_tok, ws_key, ex, cluster, st);
+                                                               samples, samp_log_p, reject, ws_tok, ws_key, ex, cluster, temp, top_p, st);
     default:
-      return sid_sample_select_wide_launch<SID_FILTER_NONE>(probas, probas_stride, noise, noise_stride, generated, log_probas, B,
+      return sid_sample_select_wide_launch<SID_FILTER_NONE, WARP>(probas, probas_stride, noise, noise_stride, generated, log_probas, B,
                                                             kp, nc, h, k, K, trie, out_generated, out_log_probas, out_parent,
-                                                            samples, samp_log_p, reject, ws_tok, ws_key, ex, cluster, st);
+                                                            samples, samp_log_p, reject, ws_tok, ws_key, ex, cluster, temp, top_p, st);
   }
 }
 
@@ -2293,9 +2506,9 @@ extern "C" int rqb200_sid_trie_sample_select_wide(const float* probas, int64_t p
                                                   int64_t* out_generated, float* out_log_probas, int64_t* out_parent,
                                                   int64_t* samples, float* samp_log_p, int* reject, void* workspace,
                                                   size_t workspace_bytes, int cluster, void* stream) {
-  return sid_sample_select_wide(probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K,
-                                prefix_workspace, out_generated, out_log_probas, out_parent, samples, samp_log_p, reject, workspace,
-                                workspace_bytes, cluster, SidExcl{}, stream);
+  return sid_sample_select_wide<false>(probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K,
+                                       prefix_workspace, out_generated, out_log_probas, out_parent, samples, samp_log_p, reject,
+                                       workspace, workspace_bytes, cluster, SidExcl{}, 1.f, 1.f, stream);
 }
 
 extern "C" int rqb200_sid_trie_sample_select_wide_excluding(
@@ -2307,9 +2520,9 @@ extern "C" int rqb200_sid_trie_sample_select_wide_excluding(
   SidExcl ex;
   const int rc = sid_excl_of(ex_pos, ex_blocked, ex_count, ex_M, ex_H, h + 1, "sid_trie_sample_select_wide_excluding", ex);
   if (rc != RQB_OK) return rc;
-  return sid_sample_select_wide(probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K,
-                                prefix_workspace, out_generated, out_log_probas, out_parent, samples, samp_log_p, reject, workspace,
-                                workspace_bytes, cluster, ex, stream);
+  return sid_sample_select_wide<false>(probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K,
+                                       prefix_workspace, out_generated, out_log_probas, out_parent, samples, samp_log_p, reject,
+                                       workspace, workspace_bytes, cluster, ex, 1.f, 1.f, stream);
 }
 
 extern "C" int rqb200_sid_trie_sample_select_wide_including(
@@ -2321,7 +2534,48 @@ extern "C" int rqb200_sid_trie_sample_select_wide_including(
   SidExcl in;
   const int rc = sid_excl_of(in_pos, in_keys, in_count, in_M, in_H, h + 1, "sid_trie_sample_select_wide_including", in, true);
   if (rc != RQB_OK) return rc;
-  return sid_sample_select_wide(probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K,
-                                prefix_workspace, out_generated, out_log_probas, out_parent, samples, samp_log_p, reject, workspace,
-                                workspace_bytes, cluster, in, stream);
+  return sid_sample_select_wide<false>(probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K,
+                                       prefix_workspace, out_generated, out_log_probas, out_parent, samples, samp_log_p, reject,
+                                       workspace, workspace_bytes, cluster, in, 1.f, 1.f, stream);
+}
+
+extern "C" int rqb200_sid_trie_sample_select_warped_wide(const float* logits, int64_t logits_stride, const float* noise,
+                                                         int64_t noise_stride, const int64_t* generated, const float* log_probas,
+                                                         int B, int kp, int nc, int h, int k, int C, int K,
+                                                         const void* prefix_workspace, int64_t* out_generated,
+                                                         float* out_log_probas, int64_t* out_parent, int64_t* samples,
+                                                         float* samp_log_p, int* bad, void* workspace, size_t workspace_bytes,
+                                                         int cluster, float temperature, float top_p, void* stream) {
+  return sid_sample_select_wide<true>(logits, logits_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K,
+                                      prefix_workspace, out_generated, out_log_probas, out_parent, samples, samp_log_p, bad, workspace,
+                                      workspace_bytes, cluster, SidExcl{}, temperature, top_p, stream);
+}
+
+extern "C" int rqb200_sid_trie_sample_select_warped_wide_excluding(
+    const float* logits, int64_t logits_stride, const float* noise, int64_t noise_stride, const int64_t* generated,
+    const float* log_probas, int B, int kp, int nc, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
+    float* out_log_probas, int64_t* out_parent, int64_t* samples, float* samp_log_p, int* bad, void* workspace,
+    size_t workspace_bytes, int cluster, float temperature, float top_p, const int* ex_pos, const int64_t* ex_blocked,
+    const int* ex_count, int ex_M, int ex_H, void* stream) {
+  SidExcl ex;
+  const int rc = sid_excl_of(ex_pos, ex_blocked, ex_count, ex_M, ex_H, h + 1, "sid_trie_sample_select_warped_wide_excluding", ex);
+  if (rc != RQB_OK) return rc;
+  return sid_sample_select_wide<true>(logits, logits_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K,
+                                      prefix_workspace, out_generated, out_log_probas, out_parent, samples, samp_log_p, bad, workspace,
+                                      workspace_bytes, cluster, ex, temperature, top_p, stream);
+}
+
+extern "C" int rqb200_sid_trie_sample_select_warped_wide_including(
+    const float* logits, int64_t logits_stride, const float* noise, int64_t noise_stride, const int64_t* generated,
+    const float* log_probas, int B, int kp, int nc, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
+    float* out_log_probas, int64_t* out_parent, int64_t* samples, float* samp_log_p, int* bad, void* workspace,
+    size_t workspace_bytes, int cluster, float temperature, float top_p, const int* in_pos, const int64_t* in_keys,
+    const int* in_count, int in_M, int in_H, void* stream) {
+  SidExcl in;
+  const int rc = sid_excl_of(in_pos, in_keys, in_count, in_M, in_H, h + 1, "sid_trie_sample_select_warped_wide_including", in,
+                             true);
+  if (rc != RQB_OK) return rc;
+  return sid_sample_select_wide<true>(logits, logits_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K,
+                                      prefix_workspace, out_generated, out_log_probas, out_parent, samples, samp_log_p, bad, workspace,
+                                      workspace_bytes, cluster, in, temperature, top_p, stream);
 }

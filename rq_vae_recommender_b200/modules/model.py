@@ -13,7 +13,8 @@ The search (``generate``, ``generate_items``):
     scores and keeps the k best.  ``torch.multinomial(p, n)`` without replacement is ``topk(p / q, n)`` with
     ``q = draw_exponential(p)`` from the same generator, so under the same seed the samples, beams and log-probabilities are the
     reference's.  Nothing in the level loop waits for the device: rows ``torch.multinomial`` would reject are counted on the
-    device and raise its error after the last level;
+    device and raise its error after the last level.  ``temperature`` / ``top_p`` (per call, per level) draw instead from
+    softmax(logits / T) within a top-p nucleus, in the same kernel's warped mode (``SidPrefixIndex.sample_select_warped``);
   * ``search="beam"``: an exhaustive, deterministic beam search over every code (``SidPrefixIndex.beam_topk``), no sampling;
   * ``search="exact"``: the w valid corpus tuples of highest exact log-probability (``rank_sem_ids``' score, bit for bit): a beam
     search of width w bounds the w-th best score, and ``FusedT5Exact`` decodes only the trie nodes that reach the bound;
@@ -36,6 +37,7 @@ The fused T5 passes, each HF's maths as GEMMs between this project's kernels, de
 log-probability, one decoder row per corpus-trie node per history, and ranked.  ``score_items`` / ``score_sem_ids`` give the same
 exact log-probability for items the caller chooses, decoding per history the trie of its own candidates with the same kernels.
 """
+import math
 from typing import List
 from typing import NamedTuple
 from typing import Optional
@@ -814,6 +816,41 @@ def _check_tuple_key(H: int, K: int, what: str, max_levels: Optional[int] = None
                           + (f" (at most {max_levels} levels)" if max_levels is not None else ""))
 
 
+def _level_values(value, H: int, name: str, what: str) -> List[float]:
+    """A sampling control given as one float or as a sequence of H floats (one per level) -> H floats."""
+    if isinstance(value, (int, float)) and not isinstance(value, bool):
+        return [float(value)] * H
+    try:
+        values = [float(v) for v in value]
+    except (TypeError, ValueError):
+        raise ValueError(f"{what}: {name} must be a float or a sequence of {H} floats (one per level), got {value!r}") from None
+    if len(values) != H:
+        raise ValueError(f"{what}: {name} has {len(values)} values; it takes one float or one per level ({H})")
+    return values
+
+
+def _sampling_controls(search: str, temperature, top_p, H: int, what: str, ignore_temperature: bool = False):
+    """The per-level (temperature, top_p) of a search, checked before any launch: None for the untempered search (T = 1 and
+    top_p = 1 at every level, or a deterministic search).  T must be finite and > 0 and top_p in (0, 1], else ``ValueError``;
+    so must anything but the defaults with search "beam" or "exact", except a temperature ``ignore_temperature`` drops (the
+    reference's ``generate_next_sem_id`` argument, which those searches ignore)."""
+    deterministic = search != "sample"
+    temps = [1.0] * H if deterministic and ignore_temperature else _level_values(temperature, H, "temperature", what)
+    ps = _level_values(top_p, H, "top_p", what)
+    for t in temps:
+        if not (math.isfinite(t) and t > 0):
+            raise ValueError(f"{what}: temperature must be finite and > 0, got {t}")
+    for p in ps:
+        if not 0 < p <= 1:
+            raise ValueError(f"{what}: top_p must be in (0, 1], got {p}")
+    if all(t == 1 for t in temps) and all(p == 1 for p in ps):
+        return None
+    if deterministic:
+        raise ValueError(f"{what}: temperature and top_p shape the sampled search only; search={search!r} is deterministic "
+                         "(use search=\"sample\", or leave them at 1)")
+    return list(zip(temps, ps))
+
+
 def _non_finite_error(what: str, n_bad: int) -> RuntimeError:
     return RuntimeError(f"{what}: {n_bad} decoder row(s) of the head's logits "
                         "hold a NaN or +inf or are all -inf; the items below them score NaN")
@@ -1001,6 +1038,16 @@ class EncoderDecoderRetrievalModel(nn.Module):
         return select(probas, draw_exponential(probas), generated, log_probas, k, n_cands, reject=reject, **filt)
 
     @staticmethod
+    def _warped_sample_and_select(index: ops.SidPrefixIndex, logits: Tensor, generated: Optional[Tensor],
+                                  log_probas: Optional[Tensor], k: int, n_cands: int, bad: Tensor, control: tuple,
+                                  wide: bool, filt: dict):
+        """One level of the search from the head's logits at this level's (temperature, top_p): the noise is drawn as the
+        untempered level draws it (``draw_exponential`` of a [B * kp, K] tensor), then one launch of
+        ``SidPrefixIndex.sample_select_warped`` (``_wide`` on the cluster kernel)."""
+        select = index.sample_select_warped_wide if wide else index.sample_select_warped
+        return select(logits, draw_exponential(logits), generated, log_probas, k, n_cands, *control, bad=bad, **filt)
+
+    @staticmethod
     def _narrow_search(search: str, k: int, n_cands: int) -> bool:
         """A search of beam width k fits the one-CTA-per-history selection kernels (``beam_topk`` / ``sample_select``)."""
         return k <= 32 and (search == "beam" or k * n_cands <= 1024)
@@ -1114,7 +1161,7 @@ class EncoderDecoderRetrievalModel(nn.Module):
     @torch.no_grad()
     def generate(self, attention_mask, input_ids, user_id=None, search: Optional[str] = None, decoder: Optional[str] = None,
                  encoder: Optional[str] = None, encoder_attention: Optional[str] = None, exclude_items: Optional[Tensor] = None,
-                 include_items: Optional[Tensor] = None, num_beams: Optional[int] = None):
+                 include_items: Optional[Tensor] = None, num_beams: Optional[int] = None, temperature=1.0, top_p=1.0):
         """Top-k semantic ids by beam search restricted to id prefixes of the corpus.  ``search`` (default: the module's
         ``DEFAULT_SEARCH``, read at call time):
           "sample"  per level, n_cands = min(64, K) tokens sampled without replacement per beam, scored by cumulative
@@ -1144,13 +1191,24 @@ class EncoderDecoderRetrievalModel(nn.Module):
         w * n_cands <= 1024 for "sample") run on them; wider ones select each level on one thread-block cluster per history
         (``SidPrefixIndex.beam_topk_wide`` / ``sample_select_wide``), with the same rules.  The fused decoder's self-attention
         cache is [layers, 2, H, B * w, inner] fp32; the HF decoder repeats the encoder output w times per history.
+        ``temperature`` / ``top_p`` (default 1: the untempered search above, launch for launch) shape the "sample" search's
+        draw, each a float or one float per level: level h draws from softmax(logits / T_h) restricted to its top-p_h nucleus
+        (``SidPrefixIndex.sample_select_warped``); the beams still score and return the model's own log-probabilities.  T
+        finite and > 0, 0 < top_p <= 1; anything else, or anything but 1 with "beam" or "exact", raises ``ValueError``
+        before any launch.  Bad head rows then raise the "beam" search's ``RuntimeError``.
         Returns generated [B, w, num_hierarchies] and log_probas [B, w]."""
+        warp = self._sampling(search, temperature, top_p, "generate")
         return self._generate(attention_mask, input_ids, user_id, search, decoder, encoder, encoder_attention,
                               self._filters(exclude_items, include_items, attention_mask.shape[0], attention_mask.device),
-                              num_beams)
+                              num_beams, warp)
+
+    def _sampling(self, search: Optional[str], temperature, top_p, what: str, ignore_temperature: bool = False):
+        """``_sampling_controls`` of a call's search (default ``DEFAULT_SEARCH``, read at call time)."""
+        search = _choice(search, DEFAULT_SEARCH, SEARCHES, what, "search")
+        return _sampling_controls(search, temperature, top_p, self.num_hierarchies, what, ignore_temperature)
 
     def _generate(self, attention_mask, input_ids, user_id, search, decoder, encoder, encoder_attention, filters: list,
-                  num_beams: Optional[int] = None):
+                  num_beams: Optional[int] = None, warp: Optional[list] = None):
         decoder = _choice(decoder, DEFAULT_DECODER, DECODERS, "generate", "decoder")
         if decoder == "fused" and self.training:
             raise ValueError("generate: decoder=\"fused\" runs the decoder in eval mode only; call model.eval() first (in "
@@ -1174,13 +1232,15 @@ class EncoderDecoderRetrievalModel(nn.Module):
             enc_out, enc_mask = fused_encoder(attention_mask, input_ids, user_id)
         else:
             enc_out, enc_mask = self.encoder_forward_pass(attention_mask=attention_mask, input_ids=input_ids, user_id=user_id)
-        generated, log_probas, reject = self._search_levels(enc_out, enc_mask, search, decoder, k, filters)
-        self._finish_search(search, reject, filters)
+        generated, log_probas, reject = self._search_levels(enc_out, enc_mask, search, decoder, k, filters, warp)
+        self._finish_search(_counter_kind(search, warp), reject, filters)
         return generated, log_probas
 
-    def _search_levels(self, enc_out: Tensor, enc_mask: Tensor, search: str, decoder: str, k: int, filters: list):
+    def _search_levels(self, enc_out: Tensor, enc_mask: Tensor, search: str, decoder: str, k: int, filters: list,
+                       warp: Optional[list] = None):
         """The level loop of a "sample" or "beam" search of width k over the encoder output: (generated [B, k, H], log_probas
-        [B, k], the device counters ``_finish_search`` reads)."""
+        [B, k], the device counters ``_finish_search`` reads).  ``warp``: the per-level (temperature, top_p) of a warped
+        "sample" search (``_sampling_controls``), whose counter is the "beam" search's count of bad head rows."""
         n_cands = min(MAX_CANDIDATES, self.num_embeddings_per_hierarchy)
         beam = search == "beam"
         wide = not self._narrow_search(search, k, n_cands)
@@ -1189,7 +1249,7 @@ class EncoderDecoderRetrievalModel(nn.Module):
         if fused is None:
             rep_enc, rep_mask = enc_out.repeat_interleave(k, dim=0), enc_mask.repeat_interleave(k, dim=0)
             past_kv = EncoderDecoderCache(DynamicCache(), DynamicCache())
-        reject = torch.zeros(1 if beam else 2, dtype=torch.int32, device=enc_out.device)
+        reject = torch.zeros(1 if beam or warp is not None else 2, dtype=torch.int32, device=enc_out.device)
         filt = self._filter_kwargs(filters)
         generated, log_probas, parent_global = None, None, None
         for h in range(self.num_hierarchies):
@@ -1204,6 +1264,9 @@ class EncoderDecoderRetrievalModel(nn.Module):
             if beam:
                 topk = index.beam_topk_wide if wide else index.beam_topk
                 generated, log_probas, parent_global = topk(logits, generated, log_probas, k, bad=reject, **filt)
+            elif warp is not None:
+                generated, log_probas, parent_global = self._warped_sample_and_select(index, logits, generated, log_probas, k,
+                                                                                      n_cands, reject, warp[h], wide, filt)
             elif wide:
                 generated, log_probas, parent_global = self._sample_and_select(index, F.softmax(logits, dim=-1), generated,
                                                                                log_probas, k, n_cands, reject, wide=True, **filt)
@@ -1219,7 +1282,8 @@ class EncoderDecoderRetrievalModel(nn.Module):
         return generated, log_probas, reject
 
     def _finish_search(self, search: str, reject: Tensor, filters: list) -> None:
-        """The one host read after a "sample" or "beam" search's levels: its counters, then the errors they report."""
+        """The one host read after a "sample" or "beam" search's levels: its counters, then the errors they report (``search``:
+        whose counters, ``_counter_kind``)."""
         if search == "beam" and not filters:
             counters = [int(reject[0])]
         else:
@@ -1299,11 +1363,11 @@ class EncoderDecoderRetrievalModel(nn.Module):
                              batch.sem_ids.device)
 
     def _generate_batch(self, batch: TokenizedSeqBatch, search, decoder, encoder, encoder_attention,
-                        filters: list, num_beams: Optional[int] = None) -> GenerationOutput:
+                        filters: list, num_beams: Optional[int] = None, warp: Optional[list] = None) -> GenerationOutput:
         H = self.num_hierarchies
         generated, log_probas = self._generate(_strip_dedup_col(batch.seq_mask.long(), H + 1, H),
                                                _strip_dedup_col(batch.sem_ids, H + 1, H), batch.user_ids, search, decoder,
-                                               encoder, encoder_attention, filters, num_beams)
+                                               encoder, encoder_attention, filters, num_beams, warp)
         return GenerationOutput(sem_ids=generated, log_probas=log_probas)
 
     @torch.no_grad()
@@ -1311,28 +1375,34 @@ class EncoderDecoderRetrievalModel(nn.Module):
                              search: Optional[str] = None, decoder: Optional[str] = None,
                              encoder: Optional[str] = None, encoder_attention: Optional[str] = None,
                              exclude_items: Optional[Tensor] = None, exclude_history: Optional[bool] = None,
-                             include_items: Optional[Tensor] = None, num_beams: Optional[int] = None) -> GenerationOutput:
-        """``generate`` on the batch's histories.  ``exclude_items``, ``include_items`` and ``num_beams`` as in ``generate``;
-        ``exclude_history`` (default ``DEFAULT_EXCLUDE_HISTORY``, read at call time) also excludes each history's own items
-        (``history_items``)."""
+                             include_items: Optional[Tensor] = None, num_beams: Optional[int] = None,
+                             top_p=1.0) -> GenerationOutput:
+        """``generate`` on the batch's histories.  ``exclude_items``, ``include_items``, ``num_beams``, ``temperature`` and
+        ``top_p`` as in ``generate``, except that "beam" and "exact" ignore ``temperature`` (the reference ignores it for every
+        search; ``top_p`` < 1 still raises with them); ``exclude_history`` (default ``DEFAULT_EXCLUDE_HISTORY``, read at call
+        time) also excludes each history's own items (``history_items``).  ``top_k`` is accepted for the reference's
+        signature."""
+        warp = self._sampling(search, temperature, top_p, "generate_next_sem_id", ignore_temperature=True)
         return self._generate_batch(batch, search, decoder, encoder, encoder_attention,
-                                    self._batch_filters(batch, exclude_items, exclude_history, include_items), num_beams)
+                                    self._batch_filters(batch, exclude_items, exclude_history, include_items), num_beams, warp)
 
     @torch.no_grad()
     def generate_items(self, batch: TokenizedSeqBatch, n: Optional[int] = None, search: Optional[str] = None,
                        decoder: Optional[str] = None, encoder: Optional[str] = None,
                        encoder_attention: Optional[str] = None, exclude_items: Optional[Tensor] = None,
                        exclude_history: Optional[bool] = None, include_items: Optional[Tensor] = None,
-                       num_beams: Optional[int] = None) -> ItemGenerationOutput:
+                       num_beams: Optional[int] = None, temperature=1.0, top_p=1.0) -> ItemGenerationOutput:
         """The top corpus items for each history: ``generate_next_sem_id``'s beams, unchanged, then one launch that takes the
         items of every finite beam whose ids are in the corpus, beam by beam in descending score order, each beam's items by
         dedup rank, no item twice, at most n (default: the call's beam width, ``num_beams`` or else top_k_for_generation; at
         most ``ops.SidItemTable.MAX_N``) per history.  ``exclude_items`` / ``exclude_history`` as in
         ``generate_next_sem_id``: the search and the retrieval both leave the excluded items out.  ``include_items`` as in
         ``generate``: the search and the retrieval both return only each history's eligible items.  ``num_beams`` as in
-        ``generate``: a wider search yields more candidate items (``n`` up to 4096)."""
+        ``generate``: a wider search yields more candidate items (``n`` up to 4096).  ``temperature`` / ``top_p`` as in
+        ``generate``."""
+        warp = self._sampling(search, temperature, top_p, "generate_items")
         filters = self._batch_filters(batch, exclude_items, exclude_history, include_items)
-        out = self._generate_batch(batch, search, decoder, encoder, encoder_attention, filters, num_beams)
+        out = self._generate_batch(batch, search, decoder, encoder, encoder_attention, filters, num_beams, warp)
         table = self._item_table(out.sem_ids.device)
         width = self.top_k_for_generation if num_beams is None else num_beams
         items, beams, count = table.retrieve(out.sem_ids, out.log_probas, width if n is None else n,
@@ -1343,16 +1413,16 @@ class EncoderDecoderRetrievalModel(nn.Module):
                                num_beams: Optional[int] = None, encoder_attention: Optional[str] = None,
                                exclude_items: Optional[Tensor] = None, exclude_history: Optional[bool] = None,
                                include_items: Optional[Tensor] = None, encoder: str = "fused",
-                               decoder: str = "fused") -> "GenerateItemsGraph":
+                               decoder: str = "fused", temperature=1.0, top_p=1.0) -> "GenerateItemsGraph":
         """``generate_items(batch, ..., encoder="fused", decoder="fused")`` captured as one CUDA graph, for serving: calling the
         returned ``GenerateItemsGraph`` with a batch of the same shapes is one graph replay and one host read of the error
         counters.  The example batch fixes every shape: B, the history width, whether ``user_ids`` is given, and the widths of
         ``exclude_items`` / ``include_items`` (and whether each is given).  ``search`` is "sample" or "beam" at any width those
-        searches take; ``search``, ``n``, ``num_beams``, ``encoder_attention`` and ``exclude_history`` are read once, here, with
-        ``generate_items``' defaults.  Raises ``ValueError`` for search="exact" (one host read per level), an HF encoder or
+        searches take; ``search``, ``n``, ``num_beams``, ``encoder_attention``, ``exclude_history``, ``temperature`` and
+        ``top_p`` are read once, here, with ``generate_items``' defaults and checks.  Raises ``ValueError`` for search="exact" (one host read per level), an HF encoder or
         decoder, training mode and an active autocast region.  See ``GenerateItemsGraph`` for what a replay follows."""
         return GenerateItemsGraph(self, batch, n, search, num_beams, encoder_attention, exclude_items, exclude_history,
-                                  include_items, encoder, decoder)
+                                  include_items, encoder, decoder, temperature, top_p)
 
     @torch.no_grad()
     def item_of(self, sem_ids_fut: Tensor) -> Tensor:
@@ -1608,6 +1678,12 @@ class EncoderDecoderRetrievalModel(nn.Module):
         return ItemScoreOutput(scores=scores, target_rank=rank)
 
 
+def _counter_kind(search: str, warp: Optional[list]) -> str:
+    """Whose counters and errors a "sample" or "beam" search reports: a warped "sample" search counts bad head rows as "beam"
+    does (it reads the logits, not a softmax ``torch.multinomial`` would check)."""
+    return "beam" if warp is not None else search
+
+
 def _read_search_counters(values: Tensor) -> List[int]:
     """The one host read of a ``GenerateItemsGraph`` call, after its replay: the search's counters, then each filter's count of
     ids outside [-1, N) (``EncoderDecoderRetrievalModel._counter_values``)."""
@@ -1643,13 +1719,15 @@ class GenerateItemsGraph:
     def __init__(self, model: EncoderDecoderRetrievalModel, batch: TokenizedSeqBatch, n: Optional[int], search: Optional[str],
                  num_beams: Optional[int], encoder_attention: Optional[str], exclude_items: Optional[Tensor],
                  exclude_history: Optional[bool], include_items: Optional[Tensor], encoder: str = "fused",
-                 decoder: str = "fused"):
+                 decoder: str = "fused", temperature=1.0, top_p=1.0):
         what = "capture_generate_items"
         if encoder != "fused" or decoder != "fused":
             raise ValueError(f"{what}: a CUDA graph runs the fused encoder and decoder only (encoder={encoder!r}, "
                              f"decoder={decoder!r}); HF's passes are host-driven")
         self._check_mode(model, what)
         self.search = _choice(search, DEFAULT_SEARCH, SEARCHES, what, "search")
+        #: the per-level (temperature, top_p) of a warped "sample" search, fixed at capture (None: untempered)
+        self.warp = _sampling_controls(self.search, temperature, top_p, model.num_hierarchies, what)
         if self.search == "exact":
             raise ValueError(f"{what}: search=\"exact\" reads its frontier's size on the host once per level; it cannot be "
                              "captured (use \"sample\" or \"beam\")")
@@ -1690,7 +1768,7 @@ class GenerateItemsGraph:
         filters = m._batch_filters(batch, exclude_items, self.exclude_history, include_items)
         enc_out, enc_mask = FusedT5Encode(m, self.attention, capacity=True)(
             _strip_dedup_col(seq.long(), H + 1, H), _strip_dedup_col(sem, H + 1, H), users)
-        generated, log_probas, reject = m._search_levels(enc_out, enc_mask, self.search, "fused", self.k, filters)
+        generated, log_probas, reject = m._search_levels(enc_out, enc_mask, self.search, "fused", self.k, filters, self.warp)
         items, beams, count = m._item_table(sem.device).retrieve(generated, log_probas, self.n, **m._filter_kwargs(filters))
         out = ItemGenerationOutput(item_ids=items, beams=beams, count=count, sem_ids=generated, log_probas=log_probas)
         return out, m._counter_values(reject, filters), reject.numel(), filters
@@ -1738,5 +1816,5 @@ class GenerateItemsGraph:
         out, values, n_counters, filters = self._captured
         counters = EncoderDecoderRetrievalModel._check_filter_counts(_read_search_counters(values), n_counters, filters,
                                                                      "generate")
-        EncoderDecoderRetrievalModel._raise_search_errors(self.search, counters)
+        EncoderDecoderRetrievalModel._raise_search_errors(_counter_kind(self.search, self.warp), counters)
         return ItemGenerationOutput(*(t.clone() for t in out))

@@ -689,8 +689,35 @@ class SidPrefixIndex:
         return self._sample_select("sid_trie_sample_select_wide", probas, noise, generated, log_probas, k, nc, want_samples,
                                    reject, exclude, include, int(cluster))
 
+    def sample_select_warped(self, logits: torch.Tensor, noise: torch.Tensor, generated: Optional[torch.Tensor],
+                             log_probas: Optional[torch.Tensor], k: int, nc: int, temperature: float, top_p: float,
+                             want_samples: bool = False, bad: Optional[torch.Tensor] = None,
+                             exclude: Optional["SidExclusion"] = None, include: Optional["SidInclusion"] = None):
+        """``sample_select`` drawn from the head's logits at ``temperature`` and within a ``top_p`` nucleus
+        (rqb200_sid_trie_sample_select_warped), one launch.  logits / noise [B * kp, K].  Per beam row x:
+        p_T = softmax(x / T) in fp32; the nucleus N = the codes with p_T >= t, t the largest p_T whose codes at or above it
+        hold at least top_p of the mass (fixed-point sums; ties at t all in; top_p = 1: every code); the beam draws the
+        min(nc, |N+|) largest p_T / noise over N+ (the codes of N with p_T > 0), equal ratios by ascending code, and fills the
+        other slots with -inf.  A drawn code scores its model log-probability x[c] - lse (``beam_topk``'s lse, bit for bit)
+        plus the parent's, -inf off the trie or blocked by the filter; ``samp_log_p`` holds x[c] - lse (-inf for a filler).
+        ``bad``, an int32 device tensor, is ADDED the number of beam rows holding a NaN or +inf or all -inf (their slots are
+        fillers).  T finite and > 0, 0 < top_p <= 1, else ``Rqb200Error``.  ``exclude`` / ``include`` as in ``sample_select``."""
+        return self._sample_select("sid_trie_sample_select_warped", logits, noise, generated, log_probas, k, nc, want_samples,
+                                   bad, exclude, include, warp=(float(temperature), float(top_p)))
+
+    def sample_select_warped_wide(self, logits: torch.Tensor, noise: torch.Tensor, generated: Optional[torch.Tensor],
+                                  log_probas: Optional[torch.Tensor], k: int, nc: int, temperature: float, top_p: float,
+                                  want_samples: bool = False, bad: Optional[torch.Tensor] = None,
+                                  exclude: Optional["SidExclusion"] = None, include: Optional["SidInclusion"] = None,
+                                  cluster: int = 0):
+        """``sample_select_warped`` on the cluster kernel (rqb200_sid_trie_sample_select_warped_wide), with
+        ``sample_select_wide``'s limits and ``cluster``; bit for bit wherever both run, and no result depends on the cluster
+        size."""
+        return self._sample_select("sid_trie_sample_select_warped_wide", logits, noise, generated, log_probas, k, nc,
+                                   want_samples, bad, exclude, include, int(cluster), warp=(float(temperature), float(top_p)))
+
     def _sample_select(self, entry: str, probas, noise, generated, log_probas, k: int, nc: int, want_samples: bool, reject,
-                       exclude, include, cluster: Optional[int] = None):
+                       exclude, include, cluster: Optional[int] = None, warp: Optional[tuple] = None):
         _need_cuda(probas, noise, reject)
         if generated is None:
             B, kp, h = probas.shape[0], 1, 0
@@ -705,7 +732,10 @@ class SidPrefixIndex:
             raise ValueError(f"probas {tuple(probas.shape)} / noise {tuple(noise.shape)} must both be [B * kp = {B * kp}, K]")
         if probas.shape[1] != self.K:
             raise ValueError(f"probas has {probas.shape[1]} codes, the prefix index {self.K}")
-        if reject is not None and (reject.dtype != torch.int32 or reject.numel() < 2 or not reject.is_contiguous()):
+        if warp is not None:
+            if reject is not None and (reject.dtype != torch.int32 or reject.numel() < 1 or not reject.is_contiguous()):
+                raise ValueError("bad must be a contiguous int32 tensor")
+        elif reject is not None and (reject.dtype != torch.int32 or reject.numel() < 2 or not reject.is_contiguous()):
             raise ValueError("reject must be a contiguous int32 tensor of 2 elements")
         dev = probas.device
         out_g = torch.empty((B, k, h + 1), dtype=torch.int64, device=dev)
@@ -720,11 +750,12 @@ class SidPrefixIndex:
             ws_bytes = lib.rqb200_sid_trie_sample_select_wide_workspace_bytes(B, kp, nc)
             ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
             wide = (_p(ws), ws_bytes, cluster)
+        warp = () if warp is None else warp                   # the warped entries: temperature, top_p
         with torch.cuda.device(dev):
             _lib.check(getattr(lib, "rqb200_" + name)(
                 _p(probas), probas.stride(0), _p(noise), noise.stride(0), _p(generated), _p(log_probas), B, kp, nc, h, k, self.C,
-                self.K, _p(self.ws), _p(out_g), _p(out_p), _p(out_parent), _p(samples), _p(samp_log_p), _p(reject), *wide, *filt,
-                _stream()), name)
+                self.K, _p(self.ws), _p(out_g), _p(out_p), _p(out_parent), _p(samples), _p(samp_log_p), _p(reject), *wide, *warp,
+                *filt, _stream()), name)
         _count(1)
         if want_samples:
             return out_g, out_p, out_parent, samples, samp_log_p
