@@ -600,6 +600,57 @@ int rqb200_t5dec_self_attention(const float* qkv, int64_t ldqkv, float* cache_k,
 int rqb200_t5dec_add_norm(float* x, const float* delta, int64_t ld_delta, const float* emb, const int64_t* ids, int64_t ids_stride,
                           int64_t id_offset, int64_t n_emb, const float* weight, int R, int D, float eps, float* out, void* stream);
 
+/* ---- device-counted launches: the decoder level of a CUDA-graph replay whose row count exists only on the device
+ * (modules/model.py FusedT5Exact(capacity=True)) ----
+ * Each call takes the host-counted call's arguments, with its row (or tile) count as a CAPACITY that sizes the grid and the
+ * buffers, and a device count: rows (tiles) below min(*live, capacity) get the host-counted call's bits at that count, and the
+ * CTAs / warps past it exit without writing.  The host-counted entry points are unchanged.
+ *   f32_to_split_image_counted : row-major operands only; rows = capacity (the image layout), *live_rows the source rows.
+ *   gemm_split_counted         : M = capacity (of the A image), *live_m the rows written.
+ *   t5dec_self_attention_counted / t5dec_add_norm_counted : R = capacity, *live_r the rows (ancestor advance and embedding
+ *                                gather included).
+ *   t5rank_cross_attention_ragged_counted : T = capacity, *live_t the tiles.
+ *   t5rank_children_counted    : one group of R = capacity rows (n_h = R), live[0] the rows, live[1] the children (<= n_next, the
+ *                                capacity of out / code).
+ *   t5exact_frontier_capacity[_excluding/_including] : the write pass of t5exact_frontier with outputs of r_cap rows, c_cap children
+ *                                and t_cap tiles, the totals offs[., Bc] read on the device.  When they fit it writes the write
+ *                                pass's outputs, live int32 [3] = (R, C, T) and noff int32 [Bc + 1] = offs[1] (the children's
+ *                                offsets for the next level).  When a total exceeds its capacity it writes no row, sets live and
+ *                                noff to 0 and *overflow = 1 (never cleared here), so the next level's launches find no rows. */
+int rqb200_f32_to_split_image_counted(const float* x, int64_t ldx, int rows, int K, const int* live_rows, void* image, void* stream);
+int rqb200_gemm_split_counted(const void* a_image, const void* b_image, int M, int N, int K, int relu, const float* mask, int64_t ldm,
+                              const int* live_m, float* out, int64_t ldo, void* stream);
+int rqb200_t5dec_self_attention_counted(const float* qkv, int64_t ldqkv, float* cache_k, float* cache_v, int64_t slot_stride,
+                                        const float* bias, const int* anc_in, const int64_t* parent, int* anc_out, int R,
+                                        const int* live_r, int heads, int h, int H, float* out, int64_t ldo, void* stream);
+int rqb200_t5dec_add_norm_counted(float* x, const float* delta, int64_t ld_delta, const float* emb, const int64_t* ids,
+                                  int64_t ids_stride, int64_t id_offset, int64_t n_emb, const float* weight, int R, const int* live_r,
+                                  int D, float eps, float* out, void* stream);
+int rqb200_t5rank_cross_attention_ragged_counted(const float* q, int64_t ldq, const float* k, const float* v, int64_t ldkv,
+                                                 const int* offsets, const float* key_mask, const int* tiles, int T, const int* live_t,
+                                                 int heads, float* out, int64_t ldo, void* stream);
+int rqb200_t5rank_children_counted(const float* logits, int64_t ld, int R, int K, const float* parent, const int* child,
+                                   const int* code, int n_next, const int* live, float* out, int* bad, void* stream);
+int rqb200_t5exact_frontier_capacity(const float* sc, const int* coff, int n_root, const int* cnode, const int* ccode, const int* cpar,
+                                     const int64_t* pkey, const float* tau, int Bc, int K, int l, const int* lchild,
+                                     const int* lcode_next, int b0, const int* offs, int64_t* row_code, int64_t* row_par,
+                                     float* row_score, int64_t* row_key, int* row_node, int* tiles, int* nrng, int* nnode, int* ncode,
+                                     int* npar, int r_cap, int c_cap, int t_cap, int* live, int* overflow, int* noff, void* stream);
+int rqb200_t5exact_frontier_capacity_excluding(const float* sc, const int* coff, int n_root, const int* cnode, const int* ccode,
+                                               const int* cpar, const int64_t* pkey, const float* tau, int Bc, int K, int l,
+                                               const int* lchild, const int* lcode_next, int b0, const int* offs, int64_t* row_code,
+                                               int64_t* row_par, float* row_score, int64_t* row_key, int* row_node, int* tiles,
+                                               int* nrng, int* nnode, int* ncode, int* npar, int r_cap, int c_cap, int t_cap,
+                                               int* live, int* overflow, int* noff, const int* ex_pos, const int64_t* ex_blocked,
+                                               const int* ex_count, int ex_M, int ex_H, void* stream);
+int rqb200_t5exact_frontier_capacity_including(const float* sc, const int* coff, int n_root, const int* cnode, const int* ccode,
+                                               const int* cpar, const int64_t* pkey, const float* tau, int Bc, int K, int l,
+                                               const int* lchild, const int* lcode_next, int b0, const int* offs, int64_t* row_code,
+                                               int64_t* row_par, float* row_score, int64_t* row_key, int* row_node, int* tiles,
+                                               int* nrng, int* nnode, int* ncode, int* npar, int r_cap, int c_cap, int t_cap,
+                                               int* live, int* overflow, int* noff, const int* in_pos, const int64_t* in_keys,
+                                               const int* in_count, int in_M, int in_H, void* stream);
+
 /* ---- the generative-retrieval model's T5 encoder pass over kept tokens only (modules/model.py, generate(encoder="fused")),
  * csrc/t5enc.cu ----
  * The encoder input of a history of n = items * H ids (mask [B, n] fp32, ids [B, n] int64) has S = user + items * (H + sep)

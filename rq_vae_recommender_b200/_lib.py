@@ -194,6 +194,18 @@ _SIGNATURES = {
     "rqb200_f32_to_split_image": (c_int, [c_vp, c_i64, c_int, c_int, c_int, c_vp, c_vp]),
     "rqb200_gemm_split": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_i64, c_vp, c_i64, c_vp]),
     "rqb200_gemm_split_k_slices": (c_int, [c_int, c_int, c_int]),
+    "rqb200_f32_to_split_image_counted": (c_int, [c_vp, c_i64, c_int, c_int, c_vp, c_vp, c_vp]),
+    "rqb200_gemm_split_counted": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp]),
+    "rqb200_t5dec_self_attention_counted": (c_int, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_int, c_int,
+                                                    c_int, c_vp, c_i64, c_vp]),
+    "rqb200_t5dec_add_norm_counted": (c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_vp, c_int, c_vp, c_int, c_f32, c_vp,
+                                              c_vp]),
+    "rqb200_t5rank_cross_attention_ragged_counted": (c_int, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_int, c_vp, c_int, c_vp,
+                                                             c_i64, c_vp]),
+    "rqb200_t5rank_children_counted": (c_int, [c_vp, c_i64, c_int, c_int, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp]),
+    "rqb200_t5exact_frontier_capacity": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_int, c_vp] + [c_vp] * 10 + [c_int] * 3 + [c_vp] * 3 + [c_vp]),
+    "rqb200_t5exact_frontier_capacity_excluding": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_int, c_vp] + [c_vp] * 10 + [c_int] * 3 + [c_vp] * 3 + [c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
+    "rqb200_t5exact_frontier_capacity_including": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_int, c_vp] + [c_vp] * 10 + [c_int] * 3 + [c_vp] * 3 + [c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
     "rqb200_gemm_split_k": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_i64, c_vp]),
 }
 

@@ -274,10 +274,17 @@ __device__ __forceinline__ void gs_split8(const float (&v)[8], float s, uint4& h
 // stays in registers between the maximum and the split.  grid = row tiles, block = 256.  Few registers on purpose: the kernel
 // is a pure HBM stream (read 4 B, write 4 B per element) and needs many warps per SM in flight -- the first version (one
 // generic 12-chunk instantiation, 133 registers, one CTA per SM) ran at 0.8-2 TB/s.
-template <int NCH, int W>
-__global__ void __launch_bounds__(256) gs_split_rows_kernel(const float* __restrict__ x, int64_t ldx, int rows, int K, unsigned char* img) {
+// LIVE (rqb200_f32_to_split_image_counted): the grid and image are sized for `rows` (the capacity) and the source rows are the
+// first min(*live, rows): the CTAs of tiles past them exit, the rest write what a call with that row count writes.
+template <int NCH, int W, bool LIVE>
+__global__ void __launch_bounds__(256) gs_split_rows_kernel(const float* __restrict__ x, int64_t ldx, int rows, int K, unsigned char* img,
+                                                            const int* __restrict__ live) {
   const int nkc = (K + GT_KC - 1) / GT_KC, mtiles = gridDim.x;
   const int mt = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (LIVE) {
+    rows = min(rows, max(0, *live));
+    if (mt * 128 >= rows) return;
+  }
   unsigned char* hi_img = img;
   unsigned char* lo_img = img + (size_t)mtiles * nkc * GT_BLK_BYTES;
   float* scales = reinterpret_cast<float*>(img + 2 * (size_t)mtiles * nkc * GT_BLK_BYTES);
@@ -329,11 +336,16 @@ __global__ void __launch_bounds__(256) gs_split_rows_kernel(const float* __restr
 
 // Rows wider than the register-resident splitter takes (K > 32 * 8 * GS_MAX_CHUNKS): one warp per image row, two passes over
 // the row -- its maximum, then the split (the second read comes from L2: at most 8 rows of a CTA are in flight).  Same image
-// and scale as gs_split_rows_kernel.  grid = 16 per row tile (8 rows each), block = 256.
+// and scale as gs_split_rows_kernel.  grid = 16 per row tile (8 rows each), block = 256.  LIVE as gs_split_rows_kernel.
+template <bool LIVE>
 __global__ void __launch_bounds__(256) gs_split_rows_wide_kernel(const float* __restrict__ x, int64_t ldx, int rows, int K,
-                                                                 unsigned char* img) {
+                                                                 unsigned char* img, const int* __restrict__ live) {
   const int nkc = (K + GT_KC - 1) / GT_KC, mtiles = gridDim.x / 16;
   const int mt = blockIdx.x / 16, r = (blockIdx.x % 16) * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (LIVE) {
+    rows = min(rows, max(0, *live));
+    if (mt * 128 >= rows) return;
+  }
   const int row = mt * 128 + r;
   unsigned char* hi_img = img;
   unsigned char* lo_img = img + (size_t)mtiles * nkc * GT_BLK_BYTES;
@@ -427,6 +439,20 @@ __global__ void __launch_bounds__(256) gs_split_cols_kernel(const float* __restr
   }
 }
 
+// the row-major splitter for K: the register-resident kernel whose lanes cover a row, or the two-pass one past 32 * 8 * GS_MAX_CHUNKS
+template <bool LIVE>
+static void gs_split_rows(const float* x, int64_t ldx, int rows, int K, unsigned char* im, const int* live, cudaStream_t st) {
+  const int mtiles = (rows + 127) / 128, nchunks = ((K + GT_KC - 1) / GT_KC) * 8;
+  if (nchunks <= 8) gs_split_rows_kernel<1, 8, LIVE><<<mtiles, 256, 0, st>>>(x, ldx, rows, K, im, live);
+  else if (nchunks <= 16) gs_split_rows_kernel<1, 16, LIVE><<<mtiles, 256, 0, st>>>(x, ldx, rows, K, im, live);
+  else if (nchunks <= 32) gs_split_rows_kernel<1, 32, LIVE><<<mtiles, 256, 0, st>>>(x, ldx, rows, K, im, live);
+  else if (nchunks <= 64) gs_split_rows_kernel<2, 32, LIVE><<<mtiles, 256, 0, st>>>(x, ldx, rows, K, im, live);
+  else if (nchunks <= 96) gs_split_rows_kernel<3, 32, LIVE><<<mtiles, 256, 0, st>>>(x, ldx, rows, K, im, live);
+  else if (nchunks <= 128) gs_split_rows_kernel<4, 32, LIVE><<<mtiles, 256, 0, st>>>(x, ldx, rows, K, im, live);
+  else if (nchunks <= 32 * GS_MAX_CHUNKS) gs_split_rows_kernel<GS_MAX_CHUNKS, 32, LIVE><<<mtiles, 256, 0, st>>>(x, ldx, rows, K, im, live);
+  else gs_split_rows_wide_kernel<LIVE><<<mtiles * 16, 256, 0, st>>>(x, ldx, rows, K, im, live);
+}
+
 extern "C" int rqb200_f32_to_split_image(const float* x, int64_t ldx, int rows, int K, int transposed, void* image, void* stream) {
   RQB_CHECK_ARG(K > 0 && rows >= 0, "f32_to_split_image: bad shape (rows=%d K=%d)", rows, K);
   RQB_CHECK_ARG(transposed ? ldx >= rows : ldx >= K, "f32_to_split_image: ld too small");
@@ -450,17 +476,19 @@ extern "C" int rqb200_f32_to_split_image(const float* x, int64_t ldx, int rows, 
     RQB_LAUNCH_CHECK();
     gs_split_cols_kernel<<<dim3(mtiles, nkc), 256, 0, st>>>(x, ldx, rows, K, im);
   } else {
-    unsigned char* im = reinterpret_cast<unsigned char*>(image);
-    const int nchunks = ((K + GT_KC - 1) / GT_KC) * 8;
-    if (nchunks <= 8) gs_split_rows_kernel<1, 8><<<mtiles, 256, 0, st>>>(x, ldx, rows, K, im);
-    else if (nchunks <= 16) gs_split_rows_kernel<1, 16><<<mtiles, 256, 0, st>>>(x, ldx, rows, K, im);
-    else if (nchunks <= 32) gs_split_rows_kernel<1, 32><<<mtiles, 256, 0, st>>>(x, ldx, rows, K, im);
-    else if (nchunks <= 64) gs_split_rows_kernel<2, 32><<<mtiles, 256, 0, st>>>(x, ldx, rows, K, im);
-    else if (nchunks <= 96) gs_split_rows_kernel<3, 32><<<mtiles, 256, 0, st>>>(x, ldx, rows, K, im);
-    else if (nchunks <= 128) gs_split_rows_kernel<4, 32><<<mtiles, 256, 0, st>>>(x, ldx, rows, K, im);
-    else if (nchunks <= 32 * GS_MAX_CHUNKS) gs_split_rows_kernel<GS_MAX_CHUNKS, 32><<<mtiles, 256, 0, st>>>(x, ldx, rows, K, im);
-    else gs_split_rows_wide_kernel<<<mtiles * 16, 256, 0, st>>>(x, ldx, rows, K, im);
+    gs_split_rows<false>(x, ldx, rows, K, reinterpret_cast<unsigned char*>(image), nullptr, st);
   }
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
+}
+
+extern "C" int rqb200_f32_to_split_image_counted(const float* x, int64_t ldx, int rows, int K, const int* live_rows, void* image,
+                                                 void* stream) {
+  RQB_CHECK_ARG(K > 0 && rows >= 0 && ldx >= K, "f32_to_split_image_counted: bad shape (rows=%d K=%d)", rows, K);
+  if (rows == 0) return RQB_OK;
+  RQB_CHECK_ARG(x && image && live_rows, "f32_to_split_image_counted: null pointer");
+  RQB_CHECK_ARG((reinterpret_cast<uintptr_t>(image) & 15) == 0, "f32_to_split_image_counted: the image must be 16-byte aligned");
+  gs_split_rows<true>(x, ldx, rows, K, reinterpret_cast<unsigned char*>(image), live_rows, reinterpret_cast<cudaStream_t>(stream));
   RQB_LAUNCH_CHECK();
   return RQB_OK;
 }
@@ -477,7 +505,20 @@ struct GsParams {
   int64_t ldm;
 };
 
-__global__ void __launch_bounds__(GT_THREADS, 1) gs_gemm_kernel(GsParams p) {
+// LIVE (rqb200_gemm_split_counted): items are row-tile major, so the live rows' items are the first ones; the others are skipped
+// and each live item computes what it computes at the host row count.  The live count is re-read where it is used rather than
+// held in a register: the consumers have no register to spare (the host-counted instantiation must stay as it is).
+template <bool LIVE>
+__device__ __forceinline__ int gs_rows(const GsParams& p, const int* m_live) {
+  return LIVE ? min(p.M, max(0, __ldg(m_live))) : p.M;
+}
+template <bool LIVE>
+__device__ __forceinline__ int gs_items(const GsParams& p, const int* m_live) {
+  return LIVE ? (gs_rows<LIVE>(p, m_live) + 127) / 128 * p.nblocks * p.ksplit : p.nitems;
+}
+
+template <bool LIVE>
+__device__ __forceinline__ void gs_gemm(GsParams p, const int* __restrict__ m_live) {
   extern __shared__ __align__(1024) unsigned char gsm[];
   GtSmemMisc* ms = reinterpret_cast<GtSmemMisc*>(gsm + GS_STAGES * GS_STAGE_BYTES);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -493,7 +534,7 @@ __global__ void __launch_bounds__(GT_THREADS, 1) gs_gemm_kernel(GsParams p) {
     // ============================================================== producer: A hi, A lo, B hi, B lo per stage
     if (lane == 0) {
       uint32_t s = 0;
-      for (int item = blockIdx.x; item < p.nitems; item += gridDim.x) {
+      for (int item = blockIdx.x; item < gs_items<LIVE>(p, m_live); item += gridDim.x) {
         const int ks = item % p.ksplit, tile = item / p.ksplit;
         const int mt = tile / p.nblocks, nbk = tile % p.nblocks;
         const int kc_end = min(p.nkc, (ks + 1) * p.kc_per);
@@ -517,7 +558,7 @@ __global__ void __launch_bounds__(GT_THREADS, 1) gs_gemm_kernel(GsParams p) {
   const int ra = wg * 64 + (warp & 3) * 16 + (lane >> 2);
   const uint32_t base = smem_u32(gsm);
   uint32_t s = 0;
-  for (int item = blockIdx.x; item < p.nitems; item += gridDim.x) {
+  for (int item = blockIdx.x; item < gs_items<LIVE>(p, m_live); item += gridDim.x) {
     const int ks = item % p.ksplit, tile = item / p.ksplit;
     const int mt = tile / p.nblocks, nbk = tile % p.nblocks;
     const int kc_begin = ks * p.kc_per, kc_end = min(p.nkc, (ks + 1) * p.kc_per);
@@ -563,7 +604,7 @@ __global__ void __launch_bounds__(GT_THREADS, 1) gs_gemm_kernel(GsParams p) {
 #pragma unroll
       for (int jb = 0; jb < 16; ++jb) {
         const int col = col0 + 8 * jb + 2 * q4;
-        if (row >= p.M || col >= p.N) continue;
+        if (row >= gs_rows<LIVE>(p, m_live) || col >= p.N) continue;
         const float2 bs = __ldg(reinterpret_cast<const float2*>(p.b_scale + col));
         float v[2];
 #pragma unroll
@@ -582,6 +623,11 @@ __global__ void __launch_bounds__(GT_THREADS, 1) gs_gemm_kernel(GsParams p) {
   }
 }
 
+__global__ void __launch_bounds__(GT_THREADS, 1) gs_gemm_kernel(GsParams p) { gs_gemm<false>(p, nullptr); }
+__global__ void __launch_bounds__(GT_THREADS, 1) gs_gemm_counted_kernel(GsParams p, const int* __restrict__ m_live) {
+  gs_gemm<true>(p, m_live);
+}
+
 // out[i, j] = sum over the k slices of the partial sums (fixed order: deterministic)
 __global__ void gs_reduce_kernel(const float* __restrict__ part, int S, int M, int N, float* __restrict__ out, int64_t ldo) {
   const int64_t n = (int64_t)M * N;
@@ -592,8 +638,9 @@ __global__ void gs_reduce_kernel(const float* __restrict__ part, int S, int M, i
   }
 }
 
+template <bool LIVE = false>
 static int gs_run(const void* a_image, const void* b_image, int M, int N, int K, int relu, const float* mask, int64_t ldm,
-                  float* out, int64_t ldo, int ksplit, int kc_per, int64_t part_stride, cudaStream_t st) {
+                  float* out, int64_t ldo, int ksplit, int kc_per, int64_t part_stride, cudaStream_t st, const int* m_live = nullptr) {
   GsParams p{};
   p.M = M; p.N = N; p.nkc = (K + GT_KC - 1) / GT_KC;
   p.mtiles = (M + 127) / 128;
@@ -612,9 +659,14 @@ static int gs_run(const void* a_image, const void* b_image, int M, int N, int K,
   RQB_CUDA(cudaGetDevice(&dev));
   RQB_CUDA(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev));
   const size_t smem = (size_t)GS_STAGES * GS_STAGE_BYTES + sizeof(GtSmemMisc);
-  RQB_CUDA(cudaFuncSetAttribute(gs_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int grid = p.nitems < sm_count ? p.nitems : sm_count;
-  gs_gemm_kernel<<<grid, GT_THREADS, smem, st>>>(p);
+  if (LIVE) {
+    RQB_CUDA(cudaFuncSetAttribute(gs_gemm_counted_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    gs_gemm_counted_kernel<<<grid, GT_THREADS, smem, st>>>(p, m_live);
+  } else {
+    RQB_CUDA(cudaFuncSetAttribute(gs_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    gs_gemm_kernel<<<grid, GT_THREADS, smem, st>>>(p);
+  }
   RQB_LAUNCH_CHECK();
   return RQB_OK;
 }
@@ -627,6 +679,17 @@ extern "C" int rqb200_gemm_split(const void* a_image, const void* b_image, int M
   RQB_CHECK_ARG(!mask || ldm >= N, "gemm_split: ldm < N");
   return gs_run(a_image, b_image, M, N, K, relu, mask, ldm, out, ldo, 1, (K + GT_KC - 1) / GT_KC, 0,
                 reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int rqb200_gemm_split_counted(const void* a_image, const void* b_image, int M, int N, int K, int relu, const float* mask,
+                                         int64_t ldm, const int* live_m, float* out, int64_t ldo, void* stream) {
+  RQB_CHECK_ARG(M >= 0 && N > 0 && K > 0 && ldo >= N, "gemm_split_counted: bad shape (M=%d N=%d K=%d ldo=%lld)", M, N, K,
+                (long long)ldo);
+  if (M == 0) return RQB_OK;
+  RQB_CHECK_ARG(a_image && b_image && out && live_m, "gemm_split_counted: null pointer");
+  RQB_CHECK_ARG(!mask || ldm >= N, "gemm_split_counted: ldm < N");
+  return gs_run<true>(a_image, b_image, M, N, K, relu, mask, ldm, out, ldo, 1, (K + GT_KC - 1) / GT_KC, 0,
+                      reinterpret_cast<cudaStream_t>(stream), live_m);
 }
 
 // Split-K schedule for products with few output tiles and a long contraction (the weight gradients: M = out, N = in, K = batch):

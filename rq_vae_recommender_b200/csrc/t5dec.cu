@@ -124,12 +124,15 @@ __global__ void __launch_bounds__(XA_WARPS * 32) t5dec_cross_attention_kernel(
 // ------------------------------------------------------------------------------------------------ self-attention step
 // One warp per (row r, head n); lane holds dims lane and lane + 32.  qkv row r: q at n * 64, k at inner + n * 64, v at
 // 2 inner + n * 64.  cache slot j, row x, head n: cache[j * slot_stride + x * inner + n * 64 + d].  bias [heads, H, H]: the
-// relative-position bias table of decoder block 0 (HF's compute_bias(H, H)), query position h.
+// relative-position bias table of decoder block 0 (HF's compute_bias(H, H)), query position h.  LIVE: the grid is sized for R
+// rows (the capacity) and the rows are the first min(*live, R); the warps of the others exit.
+template <bool LIVE>
 __global__ void __launch_bounds__(256) t5dec_self_attention_kernel(
     const float* __restrict__ qkv, int64_t ldqkv, float* __restrict__ cache_k, float* __restrict__ cache_v, int64_t slot_stride,
     const float* __restrict__ bias, const int* __restrict__ anc_in, const int64_t* __restrict__ parent, int* __restrict__ anc_out,
-    int R, int heads, int h, int H, float* __restrict__ out, int64_t ldo) {
+    int R, int heads, int h, int H, float* __restrict__ out, int64_t ldo, const int* __restrict__ live) {
   const int gw = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (LIVE) R = min(R, max(0, *live));
   if (gw >= R * heads) return;
   const int r = gw / heads, n = gw % heads;
   const int inner = heads * T5_DKV;
@@ -185,12 +188,14 @@ __global__ void __launch_bounds__(256) t5dec_self_attention_kernel(
 
 // ------------------------------------------------------------------------------------------------ residual add + T5LayerNorm
 // One warp per row.  emb != null: x[r] = emb[(ids ? ids[r * ids_stride] + id_offset : 0)] (an id outside [0, n_emb) gives a NaN
-// row); else delta != null: x[r] += delta[r].  Then out[r] = weight * (x * rsqrt(mean(x^2) + eps)).
+// row); else delta != null: x[r] += delta[r].  Then out[r] = weight * (x * rsqrt(mean(x^2) + eps)).  LIVE as the self-attention.
+template <bool LIVE>
 __global__ void __launch_bounds__(256) t5dec_add_norm_kernel(
     float* __restrict__ x, const float* __restrict__ delta, int64_t ld_delta, const float* __restrict__ emb,
     const int64_t* __restrict__ ids, int64_t ids_stride, int64_t id_offset, int64_t n_emb, const float* __restrict__ weight,
-    int R, int D, float eps, float* __restrict__ out) {
+    int R, int D, float eps, float* __restrict__ out, const int* __restrict__ live) {
   const int r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (LIVE) R = min(R, max(0, *live));
   if (r >= R) return;
   float* xr = x + (int64_t)r * D;
   float ss = 0.f;
@@ -545,25 +550,53 @@ extern "C" int rqb200_t5dec_cross_attention(const float* q, int64_t ldq, const f
   return RQB_OK;
 }
 
-extern "C" int rqb200_t5dec_self_attention(const float* qkv, int64_t ldqkv, float* cache_k, float* cache_v, int64_t slot_stride,
-                                           const float* bias, const int* anc_in, const int64_t* parent, int* anc_out, int R,
-                                           int heads, int h, int H, float* out, int64_t ldo, void* stream) {
-  RQB_CHECK_ARG(R >= 0 && heads > 0 && h >= 0 && h < H, "t5dec_self_attention: bad shape (R=%d heads=%d h=%d H=%d)", R, heads,
-                h, H);
+template <bool LIVE>
+static int dec_self_attention(const char* what, const float* qkv, int64_t ldqkv, float* cache_k, float* cache_v, int64_t slot_stride,
+                              const float* bias, const int* anc_in, const int64_t* parent, int* anc_out, int R, int heads, int h,
+                              int H, float* out, int64_t ldo, const int* live, void* stream) {
+  RQB_CHECK_ARG(R >= 0 && heads > 0 && h >= 0 && h < H, "%s: bad shape (R=%d heads=%d h=%d H=%d)", what, R, heads, h, H);
   if (H > T5_MAX_H) {
-    rqb_set_error("t5dec_self_attention: at most %d positions (H = %d)", T5_MAX_H, H);
+    rqb_set_error("%s: at most %d positions (H = %d)", what, T5_MAX_H, H);
     return RQB_ERR_UNSUPPORTED;
   }
   const int64_t inner = (int64_t)heads * T5_DKV;
   RQB_CHECK_ARG(ldqkv >= 3 * inner && ldo >= inner && slot_stride >= (int64_t)R * inner,
-                "t5dec_self_attention: a leading dimension or the slot stride is too small");
+                "%s: a leading dimension or the slot stride is too small", what);
   if (R == 0) return RQB_OK;
-  RQB_CHECK_ARG(qkv && cache_k && cache_v && bias && out, "t5dec_self_attention: null pointer");
-  RQB_CHECK_ARG(h == 0 || (anc_in && (!parent || anc_out)), "t5dec_self_attention: h > 0 needs the ancestor table");
+  RQB_CHECK_ARG(qkv && cache_k && cache_v && bias && out && (live || !LIVE), "%s: null pointer", what);
+  RQB_CHECK_ARG(h == 0 || (anc_in && (!parent || anc_out)), "%s: h > 0 needs the ancestor table", what);
   const int64_t warps = (int64_t)R * heads;
-  RQB_CHECK_ARG(warps <= (int64_t)INT32_MAX - 7, "t5dec_self_attention: too many rows");
-  t5dec_self_attention_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      qkv, ldqkv, cache_k, cache_v, slot_stride, bias, anc_in, parent, anc_out, R, heads, h, H, out, ldo);
+  RQB_CHECK_ARG(warps <= (int64_t)INT32_MAX - 7, "%s: too many rows", what);
+  t5dec_self_attention_kernel<LIVE><<<(unsigned)((warps + 7) / 8), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      qkv, ldqkv, cache_k, cache_v, slot_stride, bias, anc_in, parent, anc_out, R, heads, h, H, out, ldo, live);
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
+}
+
+extern "C" int rqb200_t5dec_self_attention(const float* qkv, int64_t ldqkv, float* cache_k, float* cache_v, int64_t slot_stride,
+                                           const float* bias, const int* anc_in, const int64_t* parent, int* anc_out, int R,
+                                           int heads, int h, int H, float* out, int64_t ldo, void* stream) {
+  return dec_self_attention<false>("t5dec_self_attention", qkv, ldqkv, cache_k, cache_v, slot_stride, bias, anc_in, parent, anc_out,
+                                   R, heads, h, H, out, ldo, nullptr, stream);
+}
+
+extern "C" int rqb200_t5dec_self_attention_counted(const float* qkv, int64_t ldqkv, float* cache_k, float* cache_v,
+                                                   int64_t slot_stride, const float* bias, const int* anc_in, const int64_t* parent,
+                                                   int* anc_out, int R, const int* live_r, int heads, int h, int H, float* out,
+                                                   int64_t ldo, void* stream) {
+  return dec_self_attention<true>("t5dec_self_attention_counted", qkv, ldqkv, cache_k, cache_v, slot_stride, bias, anc_in, parent,
+                                  anc_out, R, heads, h, H, out, ldo, live_r, stream);
+}
+
+template <bool LIVE>
+static int dec_add_norm(const char* what, float* x, const float* delta, int64_t ld_delta, const float* emb, const int64_t* ids,
+                        int64_t ids_stride, int64_t id_offset, int64_t n_emb, const float* weight, int R, int D, float eps, float* out,
+                        const int* live, void* stream) {
+  RQB_CHECK_ARG(R >= 0 && D > 0 && (!delta || ld_delta >= D) && (!emb || n_emb > 0), "%s: bad shape (R=%d D=%d)", what, R, D);
+  if (R == 0) return RQB_OK;
+  RQB_CHECK_ARG(x && weight && out && (live || !LIVE), "%s: null pointer", what);
+  t5dec_add_norm_kernel<LIVE><<<(R + 7) / 8, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      x, delta, ld_delta, emb, ids, ids_stride, id_offset, n_emb, weight, R, D, eps, out, live);
   RQB_LAUNCH_CHECK();
   return RQB_OK;
 }
@@ -571,14 +604,15 @@ extern "C" int rqb200_t5dec_self_attention(const float* qkv, int64_t ldqkv, floa
 extern "C" int rqb200_t5dec_add_norm(float* x, const float* delta, int64_t ld_delta, const float* emb, const int64_t* ids,
                                      int64_t ids_stride, int64_t id_offset, int64_t n_emb, const float* weight, int R, int D,
                                      float eps, float* out, void* stream) {
-  RQB_CHECK_ARG(R >= 0 && D > 0 && (!delta || ld_delta >= D) && (!emb || n_emb > 0), "t5dec_add_norm: bad shape (R=%d D=%d)", R,
-                D);
-  if (R == 0) return RQB_OK;
-  RQB_CHECK_ARG(x && weight && out, "t5dec_add_norm: null pointer");
-  t5dec_add_norm_kernel<<<(R + 7) / 8, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      x, delta, ld_delta, emb, ids, ids_stride, id_offset, n_emb, weight, R, D, eps, out);
-  RQB_LAUNCH_CHECK();
-  return RQB_OK;
+  return dec_add_norm<false>("t5dec_add_norm", x, delta, ld_delta, emb, ids, ids_stride, id_offset, n_emb, weight, R, D, eps, out,
+                             nullptr, stream);
+}
+
+extern "C" int rqb200_t5dec_add_norm_counted(float* x, const float* delta, int64_t ld_delta, const float* emb, const int64_t* ids,
+                                             int64_t ids_stride, int64_t id_offset, int64_t n_emb, const float* weight, int R,
+                                             const int* live_r, int D, float eps, float* out, void* stream) {
+  return dec_add_norm<true>("t5dec_add_norm_counted", x, delta, ld_delta, emb, ids, ids_stride, id_offset, n_emb, weight, R, D, eps,
+                            out, live_r, stream);
 }
 
 static int dec_train_args(int B, int T, int heads, float p, const char* what) {

@@ -148,11 +148,14 @@ __global__ void __launch_bounds__(RK_WARPS * 32) t5rank_cross_attention_kernel<f
 }
 
 // grid (T, heads): a ragged level, history b's queries the rows roff[b] .. roff[b + 1] - 1 of q.  Tile t is tiles[3 t ..] =
-// (history, first query row, query count <= 64), as t5exact_frontier_kernel writes them.
+// (history, first query row, query count <= 64), as t5exact_frontier_kernel writes them.  LIVE: the grid is sized for T tiles (the
+// capacity) and the tiles are the first *live; the CTAs of the others exit.
+template <bool LIVE>
 __global__ void __launch_bounds__(RK_WARPS * 32) t5rank_cross_attention_ragged_kernel(
     const float* __restrict__ q, int64_t ldq, const float* __restrict__ k, const float* __restrict__ v, int64_t ldkv,
     const int* __restrict__ offsets, const float* __restrict__ key_mask, const int* __restrict__ tiles, float* __restrict__ out,
-    int64_t ldo) {
+    int64_t ldo, const int* __restrict__ live) {
+  if (LIVE && (int)blockIdx.x >= *live) return;
   rk_cross_attention_tile<true>(q, ldq, k, v, ldkv, offsets, key_mask, 0, tiles, out, ldo);
 }
 
@@ -311,35 +314,53 @@ extern "C" int rqb200_t5rank_cross_attention_tc(const float* q, int64_t ldq, con
                             stream);
 }
 
-extern "C" int rqb200_t5rank_cross_attention_ragged(const float* q, int64_t ldq, const float* k, const float* v, int64_t ldkv,
-                                                    const int* offsets, const float* key_mask, const int* tiles, int T, int heads,
-                                                    float* out, int64_t ldo, void* stream) {
+template <bool LIVE>
+static int rk_ragged(const char* what, const float* q, int64_t ldq, const float* k, const float* v, int64_t ldkv, const int* offsets,
+                     const float* key_mask, const int* tiles, int T, const int* live, int heads, float* out, int64_t ldo, void* stream) {
   RQB_CHECK_ARG(T >= 0 && heads > 0 && ldq >= (int64_t)heads * RK_DKV && ldkv >= (int64_t)heads * RK_DKV &&
                     ldo >= (int64_t)heads * RK_DKV,
-                "t5rank_cross_attention_ragged: bad argument (T = %d, heads = %d)", T, heads);
+                "%s: bad argument (T = %d, heads = %d)", what, T, heads);
   if (heads > 65535) {
-    rqb_set_error("t5rank_cross_attention_ragged: need heads <= 65535 (heads = %d)", heads);
+    rqb_set_error("%s: need heads <= 65535 (heads = %d)", what, heads);
     return RQB_ERR_UNSUPPORTED;
   }
   if (T == 0) return RQB_OK;
-  RQB_CHECK_ARG(q && k && v && offsets && tiles && out, "t5rank_cross_attention_ragged: null pointer");
-  t5rank_cross_attention_ragged_kernel<<<dim3((unsigned)T, (unsigned)heads), RK_WARPS * 32, 0,
-                                         reinterpret_cast<cudaStream_t>(stream)>>>(q, ldq, k, v, ldkv, offsets, key_mask, tiles,
-                                                                                   out, ldo);
+  RQB_CHECK_ARG(q && k && v && offsets && tiles && out && (live || !LIVE), "%s: null pointer", what);
+  t5rank_cross_attention_ragged_kernel<LIVE><<<dim3((unsigned)T, (unsigned)heads), RK_WARPS * 32, 0,
+                                               reinterpret_cast<cudaStream_t>(stream)>>>(q, ldq, k, v, ldkv, offsets, key_mask, tiles,
+                                                                                         out, ldo, live);
   RQB_LAUNCH_CHECK();
   return RQB_OK;
+}
+
+extern "C" int rqb200_t5rank_cross_attention_ragged(const float* q, int64_t ldq, const float* k, const float* v, int64_t ldkv,
+                                                    const int* offsets, const float* key_mask, const int* tiles, int T, int heads,
+                                                    float* out, int64_t ldo, void* stream) {
+  return rk_ragged<false>("t5rank_cross_attention_ragged", q, ldq, k, v, ldkv, offsets, key_mask, tiles, T, nullptr, heads, out, ldo,
+                          stream);
+}
+
+extern "C" int rqb200_t5rank_cross_attention_ragged_counted(const float* q, int64_t ldq, const float* k, const float* v, int64_t ldkv,
+                                                            const int* offsets, const float* key_mask, const int* tiles, int T,
+                                                            const int* live_t, int heads, float* out, int64_t ldo, void* stream) {
+  return rk_ragged<true>("t5rank_cross_attention_ragged_counted", q, ldq, k, v, ldkv, offsets, key_mask, tiles, T, live_t, heads, out,
+                         ldo, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ children scores
 // One warp per node row r = b * n_h + i of logits [R, K].  lse as sid_beam_topk_kernel: m = max, sum of expf(x - m) over c = lane,
 // lane + 32, ... then an xor butterfly (every lane ends with the same bits), lse = m + logf(sum).  Child j of node i (child[i] <=
 // j < child[i + 1], a node of level h + 1) gets out[b * n_next + j] = (x[code[j]] - lse) + parent[r] with explicit roundings.
+// LIVE: one group (n_h = R) whose rows are the first min(live[0], R) of the grid's R (the capacity); the warps of the others
+// exit.  live[1], the group's children, is what child[] ranges over: with one group it offsets nothing.
+template <bool LIVE>
 __global__ void __launch_bounds__(256) t5rank_children_kernel(const float* __restrict__ logits, int64_t ld, int R, int K, int n_h,
                                                               const float* __restrict__ parent, const int* __restrict__ child,
                                                               const int* __restrict__ code, int n_next, float* __restrict__ out,
-                                                              int* __restrict__ bad) {
+                                                              int* __restrict__ bad, const int* __restrict__ live) {
   const int64_t r = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
+  if (LIVE) R = min(R, max(0, live[0]));
   if (r >= R) return;
   const int64_t b = r / n_h;
   const int i = (int)(r - b * n_h);
@@ -373,8 +394,23 @@ extern "C" int rqb200_t5rank_children(const float* logits, int64_t ld, int R, in
   if (R == 0) return RQB_OK;
   RQB_CHECK_ARG(logits && child && code && out, "t5rank_children: null pointer");
   const int rows_per_block = 8;
-  t5rank_children_kernel<<<(R + rows_per_block - 1) / rows_per_block, rows_per_block * 32, 0,
-                           reinterpret_cast<cudaStream_t>(stream)>>>(logits, ld, R, K, n_h, parent, child, code, n_next, out, bad);
+  t5rank_children_kernel<false><<<(R + rows_per_block - 1) / rows_per_block, rows_per_block * 32, 0,
+                                  reinterpret_cast<cudaStream_t>(stream)>>>(logits, ld, R, K, n_h, parent, child, code, n_next, out,
+                                                                            bad, nullptr);
+  RQB_LAUNCH_CHECK();
+  return RQB_OK;
+}
+
+extern "C" int rqb200_t5rank_children_counted(const float* logits, int64_t ld, int R, int K, const float* parent, const int* child,
+                                              const int* code, int n_next, const int* live, float* out, int* bad, void* stream) {
+  RQB_CHECK_ARG(R >= 0 && K > 0 && n_next >= 0 && ld >= K, "t5rank_children_counted: bad argument (R = %d, K = %d, n_next = %d)", R,
+                K, n_next);
+  if (R == 0) return RQB_OK;
+  RQB_CHECK_ARG(logits && child && code && out && live, "t5rank_children_counted: null pointer");
+  const int rows_per_block = 8;
+  t5rank_children_kernel<true><<<(R + rows_per_block - 1) / rows_per_block, rows_per_block * 32, 0,
+                                 reinterpret_cast<cudaStream_t>(stream)>>>(logits, ld, R, K, R, parent, child, code, n_next, out, bad,
+                                                                           live);
   RQB_LAUNCH_CHECK();
   return RQB_OK;
 }
@@ -847,14 +883,26 @@ __device__ __forceinline__ bool ex_blocked(const SidExcl& f, int64_t b, int l, l
 // level 1) entries b n_root .. b n_root + n_root - 1 of sc, child i being node i of level 1 (code ccode[i], parent row b).
 // pkey [rows]: the prefix key of each parent row (null at level 1).  counts (count pass) int32 [3, Bc]; offs (write pass) int32
 // [3, Bc + 1], the exclusive scans of counts.
-template <int FILTER, bool WRITE>
+// CAP (the write pass of rqb200_t5exact_frontier_capacity*, for a caller that cannot read the totals on the host): the outputs
+// hold cap.r rows, cap.c children and cap.t tiles.  Every CTA reads the totals offs[., Bc]; when they fit, the pass writes what
+// the plain write pass writes, plus cap.live = the totals (R, C, T) and cap.noff [Bc + 1] = offs[1] (the children's offsets, which
+// the next level's passes read).  When a total exceeds its capacity it writes no row, sets cap.live and cap.noff to 0 -- the next
+// levels then see no rows -- and sets *cap.overflow = 1.
+struct ExCap {
+  int r, c, t;
+  int* live;
+  int* overflow;
+  int* noff;
+};
+
+template <int FILTER, bool WRITE, bool CAP>
 __global__ void __launch_bounds__(EX_THREADS) t5exact_frontier_kernel(
     const float* __restrict__ sc, const int* __restrict__ coff, int n_root, const int* __restrict__ cnode,
     const int* __restrict__ ccode, const int* __restrict__ cpar, const long long* __restrict__ pkey, const float* __restrict__ tau,
     int Bc, int K, int l, const int* __restrict__ lchild, const int* __restrict__ lcode_next, SidExcl f, int b0,
     int* __restrict__ counts, const int* __restrict__ offs, int64_t* __restrict__ row_code, int64_t* __restrict__ row_par,
     float* __restrict__ row_score, long long* __restrict__ row_key, int* __restrict__ row_node, int* __restrict__ tiles,
-    int* __restrict__ nrng, int* __restrict__ nnode, int* __restrict__ ncode, int* __restrict__ npar) {
+    int* __restrict__ nrng, int* __restrict__ nnode, int* __restrict__ ncode, int* __restrict__ npar, ExCap cap) {
   using Scan = cub::BlockScan<long long, EX_THREADS>;
   __shared__ typename Scan::TempStorage tmp;
   __shared__ long long carry;                               // (kept rows << 32) + their children, of the tiles before
@@ -868,6 +916,21 @@ __global__ void __launch_bounds__(EX_THREADS) t5exact_frontier_kernel(
     roff = offs[b];
     cbase = offs[(Bc + 1) + b];
     toff = offs[2 * (Bc + 1) + b];
+  }
+  if (CAP) {
+    const int R = offs[Bc], C = offs[2 * (Bc + 1) - 1], T = offs[3 * (Bc + 1) - 1];
+    const bool over = R > cap.r || C > cap.c || T > cap.t;
+    if (threadIdx.x == 0) {
+      cap.noff[b] = over ? 0 : cbase;
+      if (b == Bc - 1) cap.noff[Bc] = over ? 0 : C;
+      if (b == 0) {
+        cap.live[0] = over ? 0 : R;
+        cap.live[1] = over ? 0 : C;
+        cap.live[2] = over ? 0 : T;
+        if (over) *cap.overflow = 1;
+      }
+    }
+    if (over) return;
   }
   if (threadIdx.x == 0) carry = 0;
   __syncthreads();
@@ -1048,18 +1111,18 @@ static int ex_filter_of(const int* pos, const int64_t* keys, const int* count, i
   return RQB_OK;
 }
 
-template <bool WRITE>
+template <bool WRITE, bool CAP>
 static int ex_frontier_launch(int mode, dim3 grid, cudaStream_t st, const float* sc, const int* coff, int n_root, const int* cnode,
                               const int* ccode, const int* cpar, const int64_t* pkey, const float* tau, int Bc, int K, int l,
                               const int* lchild, const int* lcode_next, const SidExcl& f, int b0, int* counts, const int* offs,
                               int64_t* row_code, int64_t* row_par, float* row_score, int64_t* row_key, int* row_node, int* tiles,
-                              int* nrng, int* nnode, int* ncode, int* npar) {
-  auto kernel = mode == SID_FILTER_INCLUDE   ? t5exact_frontier_kernel<SID_FILTER_INCLUDE, WRITE>
-                : mode == SID_FILTER_EXCLUDE ? t5exact_frontier_kernel<SID_FILTER_EXCLUDE, WRITE>
-                                             : t5exact_frontier_kernel<SID_FILTER_NONE, WRITE>;
+                              int* nrng, int* nnode, int* ncode, int* npar, const ExCap& cap) {
+  auto kernel = mode == SID_FILTER_INCLUDE   ? t5exact_frontier_kernel<SID_FILTER_INCLUDE, WRITE, CAP>
+                : mode == SID_FILTER_EXCLUDE ? t5exact_frontier_kernel<SID_FILTER_EXCLUDE, WRITE, CAP>
+                                             : t5exact_frontier_kernel<SID_FILTER_NONE, WRITE, CAP>;
   kernel<<<grid, EX_THREADS, 0, st>>>(sc, coff, n_root, cnode, ccode, cpar, reinterpret_cast<const long long*>(pkey), tau, Bc, K, l,
                                       lchild, lcode_next, f, b0, counts, offs, row_code, row_par, row_score,
-                                      reinterpret_cast<long long*>(row_key), row_node, tiles, nrng, nnode, ncode, npar);
+                                      reinterpret_cast<long long*>(row_key), row_node, tiles, nrng, nnode, ncode, npar, cap);
   RQB_LAUNCH_CHECK();
   return RQB_OK;
 }
@@ -1067,7 +1130,8 @@ static int ex_frontier_launch(int mode, dim3 grid, cudaStream_t st, const float*
 static int ex_frontier(int mode, const float* sc, const int* coff, int n_root, const int* cnode, const int* ccode, const int* cpar,
                        const int64_t* pkey, const float* tau, int Bc, int K, int l, const int* lchild, const int* lcode_next, int b0,
                        int* counts, const int* offs, int64_t* row_code, int64_t* row_par, float* row_score, int64_t* row_key,
-                       int* row_node, int* tiles, int* nrng, int* nnode, int* ncode, int* npar, const SidExcl& f, void* stream) {
+                       int* row_node, int* tiles, int* nrng, int* nnode, int* ncode, int* npar, const SidExcl& f, void* stream,
+                       const ExCap* cap = nullptr) {
   RQB_CHECK_ARG(Bc >= 0 && K > 0 && l >= 1 && l < RQB_MAX_LEVELS && b0 >= 0 && n_root >= 0 && (counts != nullptr) != (offs != nullptr),
                 "t5exact_frontier: bad argument (Bc = %d, K = %d, l = %d, b0 = %d; one of counts / offs)", Bc, K, l, b0);
   if (Bc == 0) return RQB_OK;
@@ -1076,13 +1140,21 @@ static int ex_frontier(int mode, const float* sc, const int* coff, int n_root, c
   RQB_CHECK_ARG(counts || (row_code && row_par && row_score && row_node && tiles && nrng && (mode == SID_FILTER_NONE || row_key)),
                 "t5exact_frontier: null output");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (cap) {
+    RQB_CHECK_ARG(offs && cap->r > 0 && cap->c > 0 && cap->t > 0, "t5exact_frontier_capacity: bad capacity (R = %d, C = %d, T = %d)",
+                  cap->r, cap->c, cap->t);
+    RQB_CHECK_ARG(cap->live && cap->overflow && cap->noff && nnode && ncode && npar, "t5exact_frontier_capacity: null output");
+    return ex_frontier_launch<true, true>(mode, dim3(Bc), st, sc, coff, n_root, cnode, ccode, cpar, pkey, tau, Bc, K, l, lchild,
+                                          lcode_next, f, b0, nullptr, offs, row_code, row_par, row_score, row_key, row_node, tiles, nrng,
+                                          nnode, ncode, npar, *cap);
+  }
   if (counts)
-    return ex_frontier_launch<false>(mode, dim3(Bc), st, sc, coff, n_root, cnode, ccode, cpar, pkey, tau, Bc, K, l, lchild, lcode_next,
-                                     f, b0, counts, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
-                                     nullptr, nullptr);
-  return ex_frontier_launch<true>(mode, dim3(Bc), st, sc, coff, n_root, cnode, ccode, cpar, pkey, tau, Bc, K, l, lchild, lcode_next,
-                                  f, b0, nullptr, offs, row_code, row_par, row_score, row_key, row_node, tiles, nrng, nnode, ncode,
-                                  npar);
+    return ex_frontier_launch<false, false>(mode, dim3(Bc), st, sc, coff, n_root, cnode, ccode, cpar, pkey, tau, Bc, K, l, lchild,
+                                            lcode_next, f, b0, counts, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                            nullptr, nullptr, nullptr, nullptr, ExCap{});
+  return ex_frontier_launch<true, false>(mode, dim3(Bc), st, sc, coff, n_root, cnode, ccode, cpar, pkey, tau, Bc, K, l, lchild,
+                                         lcode_next, f, b0, nullptr, offs, row_code, row_par, row_score, row_key, row_node, tiles, nrng,
+                                         nnode, ncode, npar, ExCap{});
 }
 
 extern "C" int rqb200_t5exact_frontier(const float* sc, const int* coff, int n_root, const int* cnode, const int* ccode,
@@ -1108,6 +1180,35 @@ extern "C" int rqb200_t5exact_frontier(const float* sc, const int* coff, int n_r
   }
 EX_FRONTIER_FILTERED(rqb200_t5exact_frontier_excluding, SID_FILTER_EXCLUDE, false)
 EX_FRONTIER_FILTERED(rqb200_t5exact_frontier_including, SID_FILTER_INCLUDE, true)
+
+// the write pass at fixed capacities (ExCap): offs as the write pass's, the totals read on the device
+extern "C" int rqb200_t5exact_frontier_capacity(const float* sc, const int* coff, int n_root, const int* cnode, const int* ccode,
+                                                const int* cpar, const int64_t* pkey, const float* tau, int Bc, int K, int l,
+                                                const int* lchild, const int* lcode_next, int b0, const int* offs, int64_t* row_code,
+                                                int64_t* row_par, float* row_score, int64_t* row_key, int* row_node, int* tiles,
+                                                int* nrng, int* nnode, int* ncode, int* npar, int r_cap, int c_cap, int t_cap,
+                                                int* live, int* overflow, int* noff, void* stream) {
+  const ExCap cap{r_cap, c_cap, t_cap, live, overflow, noff};
+  return ex_frontier(SID_FILTER_NONE, sc, coff, n_root, cnode, ccode, cpar, pkey, tau, Bc, K, l, lchild, lcode_next, b0, nullptr, offs,
+                     row_code, row_par, row_score, row_key, row_node, tiles, nrng, nnode, ncode, npar, SidExcl{}, stream, &cap);
+}
+
+#define EX_FRONTIER_CAPACITY_FILTERED(NAME, MODE, INCLUDE)                                                                           \
+  extern "C" int NAME(const float* sc, const int* coff, int n_root, const int* cnode, const int* ccode, const int* cpar,             \
+                      const int64_t* pkey, const float* tau, int Bc, int K, int l, const int* lchild, const int* lcode_next, int b0, \
+                      const int* offs, int64_t* row_code, int64_t* row_par, float* row_score, int64_t* row_key, int* row_node,     \
+                      int* tiles, int* nrng, int* nnode, int* ncode, int* npar, int r_cap, int c_cap, int t_cap, int* live,        \
+                      int* overflow, int* noff, const int* f_pos, const int64_t* f_keys, const int* f_count, int f_M, int f_H,     \
+                      void* stream) {                                                                                               \
+    SidExcl f;                                                                                                                      \
+    const int rc = ex_filter_of(f_pos, f_keys, f_count, f_M, f_H, l, INCLUDE, #NAME, f);                                            \
+    if (rc != RQB_OK) return rc;                                                                                                    \
+    const ExCap cap{r_cap, c_cap, t_cap, live, overflow, noff};                                                                     \
+    return ex_frontier(MODE, sc, coff, n_root, cnode, ccode, cpar, pkey, tau, Bc, K, l, lchild, lcode_next, b0, nullptr, offs,      \
+                       row_code, row_par, row_score, row_key, row_node, tiles, nrng, nnode, ncode, npar, f, stream, &cap);          \
+  }
+EX_FRONTIER_CAPACITY_FILTERED(rqb200_t5exact_frontier_capacity_excluding, SID_FILTER_EXCLUDE, false)
+EX_FRONTIER_CAPACITY_FILTERED(rqb200_t5exact_frontier_capacity_including, SID_FILTER_INCLUDE, true)
 
 template <bool KEYS_IN_SMEM>
 static int ex_select_launch(int mode, int Bc, size_t smem, cudaStream_t st, const float* sc, const int* coff, int n_root,

@@ -37,6 +37,7 @@ The fused T5 passes, each HF's maths as GEMMs between this project's kernels, de
 log-probability, one decoder row per corpus-trie node per history, and ranked.  ``score_items`` / ``score_sem_ids`` give the same
 exact log-probability for items the caller chooses, decoding per history the trie of its own candidates with the same kernels.
 """
+import functools
 import math
 from typing import List
 from typing import NamedTuple
@@ -197,31 +198,34 @@ class _T5DecoderLevels:
         self.bias = t5.blocks[0][0].SelfAttention.compute_bias(self.H, self.H)[0].contiguous()
 
     def level(self, h: int, R: int, ids: Optional[Tensor], parent: Optional[Tensor], cache: Tensor, anc: List[Tensor],
-              cross) -> Tensor:
+              cross, live: Optional[Tensor] = None) -> Tensor:
         """The final-layer-normed hidden state [R, d_model] of query position h for R rows.  ids [R] are the rows' last codes
         (None at h = 0: BOS).  Self-attention keys/values of position j live in slot j of ``cache`` [layers, 2, H, >= R, inner];
         a row reads its past through the int32 ancestor table anc[0] [>= R, H], which this call advances from ``parent`` [R]
         (each row's row at level h - 1) into anc[1] and then swaps the pair, so no level copies the cache.
-        ``cross(q, k, v)`` is the cross-attention of the R queries over one layer's keys and values."""
+        ``cross(q, k, v)`` is the cross-attention of the R queries over one layer's keys and values.  ``live`` (int32 on the
+        device; ``ops.gemm_split`` levels only): R is a capacity and every launch runs the first live[0] rows."""
         m, linear, eps, norms, inner = self.model, self.linear, self.t5.eps, self.t5.norms, self.t5.inner
+        if live is not None:
+            linear = functools.partial(linear, live=live)
         x = torch.empty((R, m.bos_token.shape[1]), dtype=torch.float32, device=self.cross_kv.device)
         nrm = torch.empty_like(x)
         if ids is None:
-            ops.t5dec_add_norm(x, None, norms[0], nrm, eps, emb=m.bos_token)
+            ops.t5dec_add_norm(x, None, norms[0], nrm, eps, emb=m.bos_token, live=live)
         else:
             ops.t5dec_add_norm(x, None, norms[0], nrm, eps, emb=m.item_sid_embedding_table.weight, ids=ids,
-                               offset=(h - 1) * m.num_embeddings_per_hierarchy)
+                               offset=(h - 1) * m.num_embeddings_per_hierarchy, live=live)
         for l, (w_qkv, w_o, w_q, w_xo, w_i, w_fo) in enumerate(self.w):
             advance = h > 0 and l == 0
             a = ops.t5dec_self_attention(linear(nrm, w_qkv), cache[l, 0], cache[l, 1], self.bias, h, anc[0],
-                                         parent if advance else None, anc[1] if advance else None)
+                                         parent if advance else None, anc[1] if advance else None, live=live)
             if advance:
                 anc.reverse()
-            ops.t5dec_add_norm(x, linear(a, w_o), norms[3 * l + 1], nrm, eps)
+            ops.t5dec_add_norm(x, linear(a, w_o), norms[3 * l + 1], nrm, eps, live=live)
             kv = self.cross_kv[:, 2 * l * inner:(2 * l + 2) * inner]
             a = cross(linear(nrm, w_q), kv[:, :inner], kv[:, inner:])
-            ops.t5dec_add_norm(x, linear(a, w_xo), norms[3 * l + 2], nrm, eps)
-            ops.t5dec_add_norm(x, linear(linear(nrm, w_i, relu=True), w_fo), norms[3 * l + 3], nrm, eps)
+            ops.t5dec_add_norm(x, linear(a, w_xo), norms[3 * l + 2], nrm, eps, live=live)
+            ops.t5dec_add_norm(x, linear(linear(nrm, w_i, relu=True), w_fo), norms[3 * l + 3], nrm, eps, live=live)
         return nrm
 
 
@@ -423,6 +427,53 @@ class FusedT5Exact(FusedT5Rank):
                                 nxt.children.scores.view(1, -1), bad)
             children, rows = nxt.children, rows + R
         ops.t5exact_select(children, max_u, levels, H, leaf_key, w, gen, lp, b0, **filt)
+        return rows
+
+    @staticmethod
+    def capacities(n: List[int], B: int, K: int, max_rows: int) -> List[tuple]:
+        """(rows, children, tiles) capacities of pruned levels l = 1 .. H - 1 of a ``run_capacity`` of B histories over trie levels
+        of n[l] nodes: R_l = min(B n[l], max_rows), C_l = min(B n[l + 1], K R_l), T_l = ceil(R_l / 64) + B."""
+        caps = []
+        for l in range(1, len(n) - 1):
+            R = min(B * n[l], max_rows)
+            caps.append((R, min(B * n[l + 1], K * R), -(-R // 64) + B))
+        return caps
+
+    def run_capacity(self, levels: ops.SidTrieLevels, tau: Tensor, w: int, leaf_key: Tensor, filt: dict, max_rows: int,
+                     gen: Tensor, lp: Tensor, bad: Tensor, overflow: Tensor) -> Tensor:
+        """``run`` of the whole batch at fixed capacities (``capacities``), reading nothing on the host, for a CUDA-graph capture:
+        the cache, the ancestor tables and every level's buffers are sized once, and each pruned level's launches read its live
+        counts from the device (``ops.t5exact_frontier_capacity`` and the ``live`` launches).  The rows kept get ``run``'s bits.
+        A level whose frontier exceeds a capacity sets overflow[0] = 1 and leaves every later level empty, so gen / lp are then
+        not the search's result.  Returns the decoder rows run (int32 [1], on the device)."""
+        H, B, dev = self.H, tau.shape[0], self.cross_kv.device
+        K = self.model.num_embeddings_per_hierarchy
+        offsets, heads = self.offsets, self.t5.heads
+        caps = self.capacities(levels.n[:H + 1], B, K, max_rows)
+        cap = max([B] + [c[0] for c in caps])
+        cache = torch.empty((len(self.w), 2, H, cap, self.t5.inner), dtype=torch.float32, device=dev)
+        anc = [torch.zeros((cap, H), dtype=torch.int32, device=dev), torch.empty((cap, H), dtype=torch.int32, device=dev)]
+        nrm = self.level(0, B, None, None, cache, anc,
+                         lambda q, k, v: ops.t5rank_cross_attention(q, k, v, offsets, self.key_mask, 1, heads))
+        first = torch.empty((B, levels.n[1]), dtype=torch.float32, device=dev)
+        ops.t5rank_children(ops.gemm_split(nrm, self.heads_w[0]), None, levels.child[0], levels.code[1], 1, first, bad)
+        children, max_u = ops.ExactChildren(first.view(-1), levels.n[1]), levels.n[1]
+        rows = torch.full((1,), B, dtype=torch.int32, device=dev)
+        for l in range(1, H):
+            R, C, T = caps[l - 1]
+            counts = ops.t5exact_frontier_count(children, levels.code[1], tau, K, l, levels.child[l], 0, **filt)
+            scan = torch.zeros((3, B + 1), dtype=torch.int32, device=dev)
+            scan[:, 1:] = counts.cumsum(1)
+            nxt, live = ops.t5exact_frontier_capacity(children, levels.code[1], tau, K, l, levels.child[l], levels.code[l + 1], scan,
+                                                      (R, C, T), overflow, 0, **filt)
+            nrm = self.level(l, R, nxt.code, nxt.parent, cache, anc,
+                             lambda q, k, v: ops.t5rank_cross_attention_ragged(q, k, v, offsets, self.key_mask, nxt.tiles, heads,
+                                                                               live=live[2:]), live=live)
+            ops.t5rank_children(ops.gemm_split(nrm, self.heads_w[l], live=live), nxt.score, nxt.child, nxt.children.code, R,
+                                nxt.children.scores.view(1, -1), bad, live=live)
+            children, max_u = nxt.children, min(levels.n[H], C)
+            rows += live[:1]
+        ops.t5exact_select(children, max_u, levels, H, leaf_key, w, gen, lp, 0, **filt)
         return rows
 
 
@@ -1424,6 +1475,20 @@ class EncoderDecoderRetrievalModel(nn.Module):
         return GenerateItemsGraph(self, batch, n, search, num_beams, encoder_attention, exclude_items, exclude_history,
                                   include_items, encoder, decoder, temperature, top_p)
 
+    def capture_exact_items(self, batch: TokenizedSeqBatch, n: Optional[int] = None, num_beams: Optional[int] = None,
+                            max_rows: Optional[int] = None, encoder_attention: Optional[str] = None,
+                            exclude_items: Optional[Tensor] = None, exclude_history: Optional[bool] = None,
+                            include_items: Optional[Tensor] = None) -> "ExactItemsGraph":
+        """``generate_items(batch, ..., search="exact", encoder="fused", decoder="fused")`` captured as one CUDA graph, for serving
+        exact top-w results: calling the returned ``ExactItemsGraph`` with a batch of the same shapes is one graph replay and one
+        host read.  The example batch fixes every shape, as ``capture_generate_items``.  ``n``, ``num_beams``,
+        ``encoder_attention``, ``exclude_history`` are read once, here, with ``generate_items``' defaults, limits and errors.
+        ``max_rows`` bounds the decoder rows of one pruned level (default: ``RANK_BYTE_BUDGET`` bytes of decoder state, the eager
+        search's budget; the graph holds that memory while it lives).  A batch whose frontier exceeds it is answered by the eager
+        search (``ExactItemsGraph.fallbacks``).  Raises ``ValueError`` in training mode and in an active autocast region, before
+        any launch.  See ``ExactItemsGraph`` for what a replay follows."""
+        return ExactItemsGraph(self, batch, n, num_beams, max_rows, encoder_attention, exclude_items, exclude_history, include_items)
+
     @torch.no_grad()
     def item_of(self, sem_ids_fut: Tensor) -> Tensor:
         """int64 [B]: the corpus item of each row of ``TokenizedSeqBatch.sem_ids_fut`` (its H ids and the dedup column), -1
@@ -1678,6 +1743,9 @@ class EncoderDecoderRetrievalModel(nn.Module):
         return ItemScoreOutput(scores=scores, target_rank=rank)
 
 
+_EXACT = "generate(search=\"exact\")"
+
+
 def _counter_kind(search: str, warp: Optional[list]) -> str:
     """Whose counters and errors a "sample" or "beam" search reports: a warped "sample" search counts bad head rows as "beam"
     does (it reads the logits, not a softmax ``torch.multinomial`` would check)."""
@@ -1730,13 +1798,18 @@ class GenerateItemsGraph:
         self.warp = _sampling_controls(self.search, temperature, top_p, model.num_hierarchies, what)
         if self.search == "exact":
             raise ValueError(f"{what}: search=\"exact\" reads its frontier's size on the host once per level; it cannot be "
-                             "captured (use \"sample\" or \"beam\")")
+                             "captured here (use \"sample\" or \"beam\", or capture_exact_items for the exact search)")
         self.attention = _encoder_attention("fused", encoder_attention, what)
         self.k = model.top_k_for_generation if num_beams is None else int(num_beams)
         model._check_search_limits(self.search, self.k, min(MAX_CANDIDATES, model.num_embeddings_per_hierarchy),
                                    None if num_beams is None else self.k)
         self.n = self.k if n is None else int(n)
         self.exclude_history = DEFAULT_EXCLUDE_HISTORY if exclude_history is None else bool(exclude_history)
+        self._store(model, batch, exclude_items, include_items, what)
+
+    def _store(self, model: EncoderDecoderRetrievalModel, batch: TokenizedSeqBatch, exclude_items: Optional[Tensor],
+               include_items: Optional[Tensor], what: str) -> None:
+        """Keep the example inputs' specs and static copies, then capture."""
         self.model = model
         self.device = model.device
         inputs = (batch.sem_ids, batch.seq_mask, batch.user_ids, exclude_items, include_items)
@@ -1799,13 +1872,12 @@ class GenerateItemsGraph:
             if _input_spec(t) != spec:
                 want = "None" if spec is None else f"{spec[1]} {list(spec[0])} on {spec[2]}"
                 got = "None" if t is None else f"{t.dtype} {list(t.shape)} on {t.device}"
-                raise ValueError(f"GenerateItemsGraph: {name} must match the captured call ({want}), got {got}")
+                raise ValueError(f"{type(self).__name__}: {name} must match the captured call ({want}), got {got}")
         return inputs
 
-    @torch.no_grad()
-    def __call__(self, batch: TokenizedSeqBatch, exclude_items: Optional[Tensor] = None,
-                 include_items: Optional[Tensor] = None) -> ItemGenerationOutput:
-        self._check_mode(self.model, "GenerateItemsGraph")
+    def _replay(self, batch: TokenizedSeqBatch, exclude_items: Optional[Tensor], include_items: Optional[Tensor]) -> None:
+        """Check the inputs, copy them into the static buffers, recapture when the corpus or a parameter moved, replay."""
+        self._check_mode(self.model, type(self).__name__)
         inputs = self._check_inputs(batch, exclude_items, include_items)
         for dst, src in zip(self._static, inputs):
             if dst is not None:
@@ -1813,8 +1885,109 @@ class GenerateItemsGraph:
         if self._state_key() != self._key:
             self._capture()
         self._graph.replay()
+
+    @torch.no_grad()
+    def __call__(self, batch: TokenizedSeqBatch, exclude_items: Optional[Tensor] = None,
+                 include_items: Optional[Tensor] = None) -> ItemGenerationOutput:
+        self._replay(batch, exclude_items, include_items)
         out, values, n_counters, filters = self._captured
         counters = EncoderDecoderRetrievalModel._check_filter_counts(_read_search_counters(values), n_counters, filters,
                                                                      "generate")
         EncoderDecoderRetrievalModel._raise_search_errors(_counter_kind(self.search, self.warp), counters)
+        return ItemGenerationOutput(*(t.clone() for t in out))
+
+
+class ExactItemsGraph(GenerateItemsGraph):
+    """One ``generate_items(..., search="exact", encoder="fused", decoder="fused")`` call captured as a CUDA graph
+    (``EncoderDecoderRetrievalModel.capture_exact_items``).  Calls, input checks, static buffers, recapture rules, streams and
+    caller-owned results are ``GenerateItemsGraph``'s; what differs is what the graph runs and what its one read returns.
+      * The graph: the encoder at a fixed capacity (``FusedT5Encode(capacity=True)``), the width-w beam search of the bound, its
+        rescoring over each history's candidate trie at fixed level sizes [1, min(w, K), min(w, K^2), ...], and the pruned decode
+        of the whole batch as one chunk at fixed capacities (``FusedT5Exact.run_capacity``): pruned level l holds at most
+        R_l = min(B n_l, max_rows) decoder rows, n_l the corpus trie's nodes at level l.  No launch reads a count on the host.
+      * Results: the eager call's on the same inputs, bit for bit with unpadded histories; with padded histories the encoder's
+        GEMMs run B * S rows instead of N, which changes only their rounding (as ``GenerateItemsGraph``).
+      * Overflow: a replay whose frontier exceeds a level's capacity is not returned.  The call runs the eager exact search on
+        the same inputs instead, returns its result and counts the event in ``fallbacks``.
+      * The one read after the replay (``_read_search_counters``): the bound's beam counters and the filters' id counts (the
+        eager errors, with the eager texts), the non-finite head rows (the eager ``RuntimeError``), the overflow flag and the
+        decoder rows the replay ran, kept in ``rows`` (as ``EXACT_DECODER_ROWS``: the pruned decode's rows, level 0 included).
+      * What a replay follows: in-place weight updates, without recapture; a replaced, written or moved ``codebooks`` buffer
+        recaptures before the next replay.  The exact search draws no random numbers: the generator is never touched.
+      * Memory: the graph holds the decoder state of max_rows rows (default ``RANK_BYTE_BUDGET`` bytes of it, the eager search's
+        budget) plus each level's buffers at its capacity, for as long as it lives."""
+
+    def __init__(self, model: EncoderDecoderRetrievalModel, batch: TokenizedSeqBatch, n: Optional[int] = None,
+                 num_beams: Optional[int] = None, max_rows: Optional[int] = None, encoder_attention: Optional[str] = None,
+                 exclude_items: Optional[Tensor] = None, exclude_history: Optional[bool] = None,
+                 include_items: Optional[Tensor] = None):
+        what = "capture_exact_items"
+        self._check_mode(model, what)
+        self.search, self.warp = "exact", None
+        self.attention = _encoder_attention("fused", encoder_attention, what)
+        H, K = model.num_hierarchies, model.num_embeddings_per_hierarchy
+        self.k = model.top_k_for_generation if num_beams is None else int(num_beams)
+        if not 1 <= self.k <= min(MAX_NUM_BEAMS, K) or K > 2048:
+            raise Rqb200Error(f"{_EXACT}: num_beams = {self.k} with {K} codes per level is outside the exact search's limits "
+                              f"(1 <= num_beams <= min({MAX_NUM_BEAMS}, K), at most 2048 codes per level)")
+        _check_tuple_key(H, K, _EXACT, max_levels=8)
+        if max_rows is not None and (isinstance(max_rows, bool) or int(max_rows) != max_rows or max_rows < 1):
+            raise ValueError(f"{what}: max_rows = {max_rows!r} must be a positive integer")
+        #: most decoder rows of one pruned level (None: RANK_BYTE_BUDGET bytes of decoder state, at least the trie's widest level)
+        self.max_rows = None if max_rows is None else int(max_rows)
+        self.n = self.k if n is None else int(n)
+        self.exclude_history = DEFAULT_EXCLUDE_HISTORY if exclude_history is None else bool(exclude_history)
+        #: replays that overflowed a capacity and were answered by the eager search
+        self.fallbacks = 0
+        #: decoder rows the last replay ran (None before the first call)
+        self.rows = None
+        self._store(model, batch, exclude_items, include_items, what)
+
+    def _run(self):
+        m, H, K = self.model, self.model.num_hierarchies, self.model.num_embeddings_per_hierarchy
+        sem, seq, users, exclude_items, include_items = self._static
+        batch = TokenizedSeqBatch(user_ids=users, sem_ids=sem, sem_ids_fut=None, seq_mask=seq, token_type_ids=None,
+                                  token_type_ids_fut=None)
+        filters = m._batch_filters(batch, exclude_items, self.exclude_history, include_items)
+        filt = m._filter_kwargs(filters)
+        dev, B, w = sem.device, sem.shape[0], self.k
+        levels, leaf_key, _ = m._rank_levels(dev)
+        packed = FusedT5Encode(m, self.attention, capacity=True).packed(_strip_dedup_col(seq.long(), H + 1, H),
+                                                                        _strip_dedup_col(sem, H + 1, H), users)
+        beams, beam_lp, reject = m._search_levels(ops.t5enc_scatter(packed.rows, packed.slot), packed.enc_mask, "beam", "fused",
+                                                  w, filters)
+        gen = torch.full((B, w, H), -1, dtype=torch.int64, device=dev)
+        lp = torch.full((B, w), float("-inf"), dtype=torch.float32, device=dev)
+        bad, overflow, rows = (torch.zeros(1, dtype=torch.int32, device=dev) for _ in range(3))
+        if B and levels.n[H]:
+            # rows past N (src -1) belong to no history's key range: any history's mask does for them
+            key_mask = packed.key_mask.index_select(0, torch.div(packed.src.clamp(min=0), packed.S, rounding_mode="floor").long())
+            ranker = FusedT5Exact(m, packed.rows, packed.offsets, key_mask)
+            exact = torch.empty((B, w), dtype=torch.float32, device=dev)
+            ranker.run_candidates(0, B, [1] + [min(w, K ** h) for h in range(1, H + 1)], ops.t5score_trie_build(beams, K), exact,
+                                  bad)
+            bounded = (torch.isfinite(beam_lp) & torch.isfinite(exact)).all(1)
+            tau = torch.where(bounded, exact.min(1).values, float("-inf")).contiguous()
+            max_rows = self.max_rows or max(max(levels.n[:H]), RANK_BYTE_BUDGET // FusedT5Rank.row_bytes(m))
+            rows = ranker.run_capacity(levels, tau, w, leaf_key, filt, max_rows, gen, lp, bad, overflow)
+        items, item_beams, count = m._item_table(dev).retrieve(gen, lp, self.n, **filt)
+        out = ItemGenerationOutput(item_ids=items, beams=item_beams, count=count, sem_ids=gen, log_probas=lp)
+        return out, torch.cat([m._counter_values(reject, filters), bad, overflow, rows]), reject.numel(), filters
+
+    @torch.no_grad()
+    def __call__(self, batch: TokenizedSeqBatch, exclude_items: Optional[Tensor] = None,
+                 include_items: Optional[Tensor] = None) -> ItemGenerationOutput:
+        self._replay(batch, exclude_items, include_items)
+        out, values, n_counters, filters = self._captured
+        values = _read_search_counters(values)
+        counters = EncoderDecoderRetrievalModel._check_filter_counts(values[:-3], n_counters, filters, "generate")
+        EncoderDecoderRetrievalModel._raise_search_errors("beam", counters)
+        n_bad, overflow, self.rows = values[-3:]
+        if overflow:
+            self.fallbacks += 1
+            return self.model.generate_items(batch, n=self.n, search="exact", encoder="fused", decoder="fused",
+                                             encoder_attention=self.attention, exclude_items=exclude_items,
+                                             exclude_history=self.exclude_history, include_items=include_items, num_beams=self.k)
+        if n_bad:
+            raise _non_finite_error(_EXACT, n_bad)
         return ItemGenerationOutput(*(t.clone() for t in out))

@@ -35,6 +35,13 @@ def _stream() -> int:
     return torch.cuda.current_stream().cuda_stream
 
 
+def _live(live: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
+    """A device-counted launch's live count: an int32 CUDA tensor whose first entry the kernels read (None: host-counted)."""
+    if live is not None and (live.dtype != torch.int32 or not live.is_cuda or live.numel() < 1 or not live.is_contiguous()):
+        raise ValueError("live must be a contiguous int32 CUDA tensor")
+    return live
+
+
 def _need_cuda(*ts) -> None:
     for t in ts:
         if t is not None and not t.is_cuda:
@@ -237,9 +244,10 @@ SPLIT_CALLS = 0
 
 class SplitOperand:
     """One GEMM operand [rows, K] as hi + lo fp16 images with power-of-two row scales (rqb200_f32_to_split_image).
-    ``transposed=True`` builds the operand of t.T without materialising the transpose."""
+    ``transposed=True`` builds the operand of t.T without materialising the transpose.  ``live`` (int32 on the device; row-major
+    only, rqb200_f32_to_split_image_counted): t's rows are a capacity and only the first live[0] are converted."""
 
-    def __init__(self, t: torch.Tensor, transposed: bool = False):
+    def __init__(self, t: torch.Tensor, transposed: bool = False, live: Optional[torch.Tensor] = None):
         _need_cuda(t)
         lib = _lib.load()
         t = _rows(t.detach())
@@ -248,8 +256,14 @@ class SplitOperand:
         nbytes = lib.rqb200_split_image_bytes(self.rows, self.K)
         self.buf = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=t.device)
         with torch.cuda.device(t.device):
-            _lib.check(lib.rqb200_f32_to_split_image(_p(t), t.stride(0), self.rows, self.K, int(transposed), _p(self.buf),
-                                                     _stream()), "f32_to_split_image")
+            if live is None:
+                _lib.check(lib.rqb200_f32_to_split_image(_p(t), t.stride(0), self.rows, self.K, int(transposed), _p(self.buf),
+                                                         _stream()), "f32_to_split_image")
+            else:
+                if transposed:
+                    raise ValueError("SplitOperand: a device row count needs a row-major operand")
+                _lib.check(lib.rqb200_f32_to_split_image_counted(_p(t), t.stride(0), self.rows, self.K, _p(_live(live)),
+                                                                 _p(self.buf), _stream()), "f32_to_split_image_counted")
         _count(1)
 
 
@@ -294,12 +308,14 @@ def split_operand_cached(t: torch.Tensor, transposed: bool = False) -> SplitOper
 
 
 def gemm_split(a, b, *, relu: bool = False, mask: Optional[torch.Tensor] = None,
-               out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """out[M, N] = act(A[M, K] @ B[N, K]^T) on the fp16 tensor cores with fp32 accuracy; a, b: SplitOperand or fp32 tensor."""
+               out: Optional[torch.Tensor] = None, live: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out[M, N] = act(A[M, K] @ B[N, K]^T) on the fp16 tensor cores with fp32 accuracy; a, b: SplitOperand or fp32 tensor.
+    ``live`` (int32 on the device, rqb200_gemm_split_counted): M is a capacity and only rows below live[0] are computed and
+    written (a tensor ``a`` is converted with the same count)."""
     global SPLIT_CALLS
     lib = _lib.load()
     if not isinstance(a, SplitOperand):
-        a = SplitOperand(a)
+        a = SplitOperand(a, live=live)
     if not isinstance(b, SplitOperand):
         b = SplitOperand(b)
     if a.K != b.K:
@@ -310,9 +326,14 @@ def gemm_split(a, b, *, relu: bool = False, mask: Optional[torch.Tensor] = None,
     if mask is not None:
         mask = _rows(mask)
     with torch.cuda.device(a.device):
-        _lib.check(lib.rqb200_gemm_split(_p(a.buf), _p(b.buf), M, N, a.K, int(relu), _p(mask),
-                                         mask.stride(0) if mask is not None else 0, _p(out), out.stride(0), _stream()),
-                   "gemm_split")
+        if live is None:
+            _lib.check(lib.rqb200_gemm_split(_p(a.buf), _p(b.buf), M, N, a.K, int(relu), _p(mask),
+                                             mask.stride(0) if mask is not None else 0, _p(out), out.stride(0), _stream()),
+                       "gemm_split")
+        else:
+            _lib.check(lib.rqb200_gemm_split_counted(_p(a.buf), _p(b.buf), M, N, a.K, int(relu), _p(mask),
+                                                     mask.stride(0) if mask is not None else 0, _p(_live(live)), _p(out),
+                                                     out.stride(0), _stream()), "gemm_split_counted")
     _count(1)
     SPLIT_CALLS += 1
     return out
@@ -1190,12 +1211,13 @@ def t5dec_cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, mas
 
 def t5dec_self_attention(qkv: torch.Tensor, cache_k: torch.Tensor, cache_v: torch.Tensor, bias: torch.Tensor, h: int,
                          anc_in: Optional[torch.Tensor], parent: Optional[torch.Tensor] = None,
-                         anc_out: Optional[torch.Tensor] = None) -> torch.Tensor:
+                         anc_out: Optional[torch.Tensor] = None, live: Optional[torch.Tensor] = None) -> torch.Tensor:
     """The causal T5 self-attention of query position h for R beam rows (rqb200_t5dec_self_attention), one launch.
     qkv [R, 3 * heads * 64] (q | k | v); cache_k / cache_v [H, rows, heads * 64] contiguous, rows >= R: the rows' k / v are written
     to slot h, position j < h of row r is read from row anc[r, j] of slot j; bias [heads, H, H] (HF's compute_bias(H, H)[0]).
     anc = anc_in (int32 [*, H]) when parent is None; with parent (int64 [R]) anc[r] = anc_in[parent[r]] with position h - 1 set
-    to parent[r], written to anc_out (int32 [R', H], R' >= R, not anc_in).  Returns [R, heads * 64]."""
+    to parent[r], written to anc_out (int32 [R', H], R' >= R, not anc_in).  Returns [R, heads * 64].  ``live`` (int32 on the
+    device, rqb200_t5dec_self_attention_counted): R is a capacity and only rows below live[0] are computed and written."""
     _need_cuda(qkv, cache_k, cache_v, bias, anc_in, parent, anc_out)
     H, rows, inner = cache_k.shape
     heads = inner // T5_DKV
@@ -1219,18 +1241,25 @@ def t5dec_self_attention(qkv: torch.Tensor, cache_k: torch.Tensor, cache_v: torc
         raise ValueError(f"anc_in has {anc_in.shape[0]} rows, fewer than R = {R}")
     out = torch.empty((R, inner), dtype=torch.float32, device=qkv.device)
     with torch.cuda.device(qkv.device):
-        _lib.check(_lib.load().rqb200_t5dec_self_attention(_p(qkv), qkv.stride(0), _p(cache_k), _p(cache_v), rows * inner, _p(bias),
-                                                           _p(anc_in), _p(parent), _p(anc_out), R, heads, int(h), H, _p(out),
-                                                           out.stride(0), _stream()), "t5dec_self_attention")
+        if live is None:
+            _lib.check(_lib.load().rqb200_t5dec_self_attention(_p(qkv), qkv.stride(0), _p(cache_k), _p(cache_v), rows * inner,
+                                                               _p(bias), _p(anc_in), _p(parent), _p(anc_out), R, heads, int(h), H,
+                                                               _p(out), out.stride(0), _stream()), "t5dec_self_attention")
+        else:
+            _lib.check(_lib.load().rqb200_t5dec_self_attention_counted(
+                _p(qkv), qkv.stride(0), _p(cache_k), _p(cache_v), rows * inner, _p(bias), _p(anc_in), _p(parent), _p(anc_out), R,
+                _p(_live(live)), heads, int(h), H, _p(out), out.stride(0), _stream()), "t5dec_self_attention_counted")
     _count(1)
     return out
 
 
 def t5dec_add_norm(x: torch.Tensor, delta: Optional[torch.Tensor], weight: torch.Tensor, out: torch.Tensor, eps: float,
-                   emb: Optional[torch.Tensor] = None, ids: Optional[torch.Tensor] = None, offset: int = 0) -> torch.Tensor:
+                   emb: Optional[torch.Tensor] = None, ids: Optional[torch.Tensor] = None, offset: int = 0,
+                   live: Optional[torch.Tensor] = None) -> torch.Tensor:
     """A T5 sublayer boundary (rqb200_t5dec_add_norm), one launch: x += delta in place -- or, with emb [V, D], x = emb[ids + offset]
     (ids int64 [R], any stride; emb[0] for every row when ids is None) -- then out = T5LayerNorm(x) * weight.  x, out [R, D]
-    contiguous fp32.  Returns out."""
+    contiguous fp32.  Returns out.  ``live`` (int32 on the device, rqb200_t5dec_add_norm_counted): R is a capacity and only rows
+    below live[0] are read and written."""
     _need_cuda(x, delta, weight, out, emb, ids)
     R, D = x.shape
     for name, t in (("x", x), ("out", out)):
@@ -1250,11 +1279,14 @@ def t5dec_add_norm(x: torch.Tensor, delta: Optional[torch.Tensor], weight: torch
     if ids is not None:
         if ids.dtype != torch.int64 or ids.shape != (R,):
             raise ValueError(f"ids must be int64 [{R}]")
+    args = (_p(x), _p(delta), delta.stride(0) if delta is not None else 0, _p(emb), _p(ids), ids.stride(0) if ids is not None else 0,
+            int(offset), emb.shape[0] if emb is not None else 0, _p(weight), R)
     with torch.cuda.device(x.device):
-        _lib.check(_lib.load().rqb200_t5dec_add_norm(_p(x), _p(delta), delta.stride(0) if delta is not None else 0, _p(emb), _p(ids),
-                                                     ids.stride(0) if ids is not None else 0, int(offset),
-                                                     emb.shape[0] if emb is not None else 0, _p(weight), R, D, float(eps), _p(out),
-                                                     _stream()), "t5dec_add_norm")
+        if live is None:
+            _lib.check(_lib.load().rqb200_t5dec_add_norm(*args, D, float(eps), _p(out), _stream()), "t5dec_add_norm")
+        else:
+            _lib.check(_lib.load().rqb200_t5dec_add_norm_counted(*args, _p(_live(live)), D, float(eps), _p(out), _stream()),
+                       "t5dec_add_norm_counted")
     _count(1)
     return out
 
@@ -1299,11 +1331,13 @@ def t5rank_cross_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, of
 
 
 def t5rank_children(logits: torch.Tensor, parent: Optional[torch.Tensor], child: torch.Tensor, code: torch.Tensor, n_h: int,
-                    out: torch.Tensor, bad: Optional[torch.Tensor] = None) -> torch.Tensor:
+                    out: torch.Tensor, bad: Optional[torch.Tensor] = None, live: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Child scores of one trie level (rqb200_t5rank_children), one launch: logits [B * n_h, K] of the level's node rows, parent
     fp32 [B * n_h] (the nodes' scores; None: 0), child int32 [n_h + 1], code int32 [n_next] -> out fp32 [B, n_next] (written):
     out[b, j] = (logits[b * n_h + i, code[j]] - lse) + parent[b * n_h + i] for every child j of node i.  ``bad`` (int32, on the
-    device) is ADDED the rows holding a NaN or +inf logit or all -inf; their children score NaN."""
+    device) is ADDED the rows holding a NaN or +inf logit or all -inf; their children score NaN.  ``live`` (int32 [2] on the
+    device, rqb200_t5rank_children_counted): one group (n_h = R) of capacity R whose rows are the first live[0], with live[1] <=
+    n_next children."""
     _need_cuda(logits, parent, child, code, out, bad)
     logits = _rows(logits)
     R, K = logits.shape
@@ -1322,8 +1356,15 @@ def t5rank_children(logits: torch.Tensor, parent: Optional[torch.Tensor], child:
     if bad is not None and (bad.dtype != torch.int32 or bad.numel() < 1 or not bad.is_contiguous()):
         raise ValueError("bad must be a contiguous int32 tensor")
     with torch.cuda.device(logits.device):
-        _lib.check(_lib.load().rqb200_t5rank_children(_p(logits), logits.stride(0), R, K, n_h, _p(parent), _p(child), _p(code),
-                                                      n_next, _p(out), _p(bad), _stream()), "t5rank_children")
+        if live is None:
+            _lib.check(_lib.load().rqb200_t5rank_children(_p(logits), logits.stride(0), R, K, n_h, _p(parent), _p(child), _p(code),
+                                                          n_next, _p(out), _p(bad), _stream()), "t5rank_children")
+        else:
+            if n_h != R or _live(live).numel() < 2:
+                raise ValueError("t5rank_children: a device count takes one group (n_h = R) and live [rows, children]")
+            _lib.check(_lib.load().rqb200_t5rank_children_counted(_p(logits), logits.stride(0), R, K, _p(parent), _p(child), _p(code),
+                                                                  n_next, _p(live), _p(out), _p(bad), _stream()),
+                       "t5rank_children_counted")
     _count(1)
     return out
 
@@ -2077,11 +2118,13 @@ def mlp_forward_bf16(x: torch.Tensor, weights: Sequence[torch.Tensor], normalize
 
 # ---------------------------------------------------------------------------------------------- exact top-k search (csrc/t5rank.cu)
 def t5rank_cross_attention_ragged(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, offsets: torch.Tensor,
-                                  key_mask: Optional[torch.Tensor], tiles: torch.Tensor, heads: int) -> torch.Tensor:
+                                  key_mask: Optional[torch.Tensor], tiles: torch.Tensor, heads: int,
+                                  live: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``t5rank_cross_attention`` (fp32) over a ragged level (rqb200_t5rank_cross_attention_ragged), one launch: q [R, heads * 64]
     the level's query rows, tiles int32 [T, 3] (history b, first query row, query count <= 64; ``t5exact_frontier_write``), each
     tile's queries over history b's keys (k, v, offsets, key_mask as ``t5rank_cross_attention``) -> [R, heads * 64].  Each row
-    gets the bits the uniform kernel gives it."""
+    gets the bits the uniform kernel gives it.  ``live`` (int32 on the device, rqb200_t5rank_cross_attention_ragged_counted): T is
+    a capacity and only the first live[0] tiles run."""
     _need_cuda(q, k, v, offsets, key_mask, tiles)
     inner = heads * T5_DKV
     q, k, v = _rows_of(q, inner, "q"), _rows_of(k, inner, "k"), _rows_of(v, inner, "v")
@@ -2099,9 +2142,14 @@ def t5rank_cross_attention_ragged(q: torch.Tensor, k: torch.Tensor, v: torch.Ten
             raise ValueError(f"key_mask {tuple(key_mask.shape)} must be [{k.shape[0]}], one entry per key row")
     out = torch.empty((q.shape[0], inner), dtype=torch.float32, device=q.device)
     with torch.cuda.device(q.device):
-        _lib.check(_lib.load().rqb200_t5rank_cross_attention_ragged(_p(q), q.stride(0), _p(k), _p(v), k.stride(0), _p(offsets),
-                                                                    _p(key_mask), _p(tiles), tiles.shape[0], heads, _p(out),
-                                                                    out.stride(0), _stream()), "t5rank_cross_attention_ragged")
+        if live is None:
+            _lib.check(_lib.load().rqb200_t5rank_cross_attention_ragged(_p(q), q.stride(0), _p(k), _p(v), k.stride(0), _p(offsets),
+                                                                        _p(key_mask), _p(tiles), tiles.shape[0], heads, _p(out),
+                                                                        out.stride(0), _stream()), "t5rank_cross_attention_ragged")
+        else:
+            _lib.check(_lib.load().rqb200_t5rank_cross_attention_ragged_counted(
+                _p(q), q.stride(0), _p(k), _p(v), k.stride(0), _p(offsets), _p(key_mask), _p(tiles), tiles.shape[0], _p(_live(live)),
+                heads, _p(out), out.stride(0), _stream()), "t5rank_cross_attention_ragged_counted")
     _count(1)
     return out
 
@@ -2175,7 +2223,37 @@ def t5exact_frontier_write(ch: ExactChildren, root_code: Optional[torch.Tensor],
     return ExactLevel(code, parent, score, key, tiles, child, nxt)
 
 
-def _t5exact_frontier(ch, root_code, tau, K, l, lchild, lcode_next, b0, counts, offsets, outs, exclude, include):
+def t5exact_frontier_capacity(ch: ExactChildren, root_code: Optional[torch.Tensor], tau: torch.Tensor, K: int, l: int,
+                              lchild: torch.Tensor, lcode_next: torch.Tensor, offsets: torch.Tensor, caps: Sequence[int],
+                              overflow: torch.Tensor, b0: int = 0, exclude: Optional[SidExclusion] = None,
+                              include: Optional[SidInclusion] = None):
+    """The write pass at fixed capacities (rqb200_t5exact_frontier_capacity[_excluding/_including]), one launch, for a caller that
+    cannot read the totals on the host: caps = (R, C, T) size the outputs, and the kernel reads the totals offsets[:, Bc] itself.
+    -> (the next level, ``ExactLevel`` at those capacities with ``children.offsets`` the kernel's copy of offsets[1]; live int32
+    [3], the level's rows, children and tiles).  When a total exceeds its capacity nothing is written, live and the children's
+    offsets are 0 and overflow[0] (int32, on the device) is set to 1."""
+    R, C, T = (int(t) for t in caps)
+    if min(R, C, T) < 1:
+        raise ValueError(f"t5exact_frontier_capacity: capacities {(R, C, T)} must be >= 1")
+    Bc, dev = tau.shape[0], tau.device
+    filt = exclude is not None or include is not None
+    code, parent = (torch.empty(R, dtype=torch.int64, device=dev) for _ in range(2))
+    score = torch.empty(R, dtype=torch.float32, device=dev)
+    key = torch.empty(R, dtype=torch.int64, device=dev) if filt else None
+    node = torch.empty(R, dtype=torch.int32, device=dev)
+    tiles = torch.empty((T, 3), dtype=torch.int32, device=dev)
+    child = torch.empty(R + 1, dtype=torch.int32, device=dev)
+    nnode, ncode, npar = (torch.empty(C, dtype=torch.int32, device=dev) for _ in range(3))
+    live = torch.empty(3, dtype=torch.int32, device=dev)
+    noff = torch.empty(Bc + 1, dtype=torch.int32, device=dev)
+    nxt = ExactChildren(torch.empty(C, dtype=torch.float32, device=dev), 0, noff, nnode, ncode, npar, key)
+    _t5exact_frontier(ch, root_code, tau, K, l, lchild, lcode_next, b0, None, offsets,
+                      (code, parent, score, key, node, tiles, child, nnode, ncode, npar), exclude, include,
+                      (R, C, T, _p(live), _p(_live(overflow)), _p(noff)))
+    return ExactLevel(code, parent, score, key, tiles, child, nxt), live
+
+
+def _t5exact_frontier(ch, root_code, tau, K, l, lchild, lcode_next, b0, counts, offsets, outs, exclude, include, cap=None):
     _need_cuda(ch.scores, tau, lchild)
     if ch.node is None and root_code is None:
         raise ValueError("t5exact_frontier: the root's children need root_code (SidTrieLevels.code[1])")
@@ -2184,11 +2262,13 @@ def _t5exact_frontier(ch, root_code, tau, K, l, lchild, lcode_next, b0, counts, 
     ch_args = list(_exact_children_args(ch))
     if ch.node is None:
         ch_args[4] = _p(root_code)
-    name, filt = _filter_entry("t5exact_frontier", exclude, include, _filter_rows(exclude, include), l, "t5exact_frontier")
+    entry = "t5exact_frontier" if cap is None else "t5exact_frontier_capacity"
+    name, filt = _filter_entry(entry, exclude, include, _filter_rows(exclude, include), l, entry)
+    pass_args = (_p(counts), _p(offsets)) if cap is None else (_p(offsets),)
     with torch.cuda.device(tau.device):
         _lib.check(getattr(_lib.load(), "rqb200_" + name)(*ch_args, _p(tau), tau.shape[0], int(K), int(l), _p(lchild),
-                                                          _p(lcode_next), int(b0), _p(counts), _p(offsets),
-                                                          *(_p(t) for t in outs), *filt, _stream()), name)
+                                                          _p(lcode_next), int(b0), *pass_args, *(_p(t) for t in outs),
+                                                          *(cap or ()), *filt, _stream()), name)
     _count(1)
 
 
