@@ -279,6 +279,21 @@ int rqb200_sid_trie_beam_topk_including(const float* logits, int64_t logits_stri
                                         int64_t* out_generated, float* out_log_probas, int64_t* out_parent, int* bad,
                                         const int* in_pos, const int64_t* in_keys, const int* in_count, int in_M, int in_H,
                                         void* stream);
+/* sid_trie_beam_topk_capped : sid_trie_beam_topk with a cap on how many kept beams share a prefix.  A candidate's group is its
+ *                    parent's first prefix_len ids.  Walking down the uncapped order (score descending, lowest e first), a
+ *                    candidate is kept unless max_per_prefix candidates of its group were kept before it: each group keeps its
+ *                    max_per_prefix best, the others score -inf and rank among the -inf fillers by e.  So among a row's kept
+ *                    beams with a finite score at most max_per_prefix share a prefix; every kept score has the uncapped bits.
+ *   prefix_len       1 <= prefix_len <= h;  max_per_prefix >= 1; RQB_ERR_INVALID otherwise.  max_per_prefix >= k cannot bind
+ *                    and runs the uncapped kernel.
+ *   filter_mode      0 none, 1 an exclusion, 2 an allow-list: then f_pos .. f_H are the arguments of
+ *                    sid_trie_beam_topk_excluding / _including (null / 0 with mode 0).
+ *   limits           as sid_trie_beam_topk (no cluster variant). */
+int rqb200_sid_trie_beam_topk_capped(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas,
+                                     int B, int kp, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
+                                     float* out_log_probas, int64_t* out_parent, int* bad, int prefix_len, int max_per_prefix,
+                                     int filter_mode, const int* f_pos, const int64_t* f_keys, const int* f_count, int f_M, int f_H,
+                                     void* stream);
 
 /* sid_trie_beam_topk_wide : one level of the same exhaustive search for up to 1024 beams per history, on one thread-block
  *                    cluster per history.  Arguments, scores, order, `bad` and results as sid_trie_beam_topk, bit for bit
@@ -361,6 +376,24 @@ int rqb200_sid_trie_sample_select_warped_including(const float* logits, int64_t 
                                                    int64_t* samples, float* samp_log_p, int* bad, float temperature, float top_p,
                                                    const int* in_pos, const int64_t* in_keys, const int* in_count, int in_M,
                                                    int in_H, void* stream);
+/* sid_trie_sample_select_capped / sid_trie_sample_select_warped_capped : sid_trie_sample_select / _warped with the per-prefix cap
+ *                    of sid_trie_beam_topk_capped on the selection, in the candidates' order (score descending, lowest
+ *                    beam * nc + slot first).  The draws, samples and samp_log_p do not change.  prefix_len, max_per_prefix
+ *                    and the filter arguments as sid_trie_beam_topk_capped; limits as sid_trie_sample_select (no cluster
+ *                    variant). */
+int rqb200_sid_trie_sample_select_capped(const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride,
+                                         const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k,
+                                         int C, int K, const void* prefix_workspace, int64_t* out_generated, float* out_log_probas,
+                                         int64_t* out_parent, int64_t* samples, float* samp_log_p, int* reject, int prefix_len,
+                                         int max_per_prefix, int filter_mode, const int* f_pos, const int64_t* f_keys,
+                                         const int* f_count, int f_M, int f_H, void* stream);
+int rqb200_sid_trie_sample_select_warped_capped(const float* logits, int64_t logits_stride, const float* noise,
+                                                int64_t noise_stride, const int64_t* generated, const float* log_probas, int B, int kp,
+                                                int nc, int h, int k, int C, int K, const void* prefix_workspace,
+                                                int64_t* out_generated, float* out_log_probas, int64_t* out_parent, int64_t* samples,
+                                                float* samp_log_p, int* bad, float temperature, float top_p, int prefix_len,
+                                                int max_per_prefix, int filter_mode, const int* f_pos, const int64_t* f_keys,
+                                                const int* f_count, int f_M, int f_H, void* stream);
 int rqb200_sid_trie_sample_select_warped_wide(const float* logits, int64_t logits_stride, const float* noise, int64_t noise_stride,
                                               const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k,
                                               int C, int K, const void* prefix_workspace, int64_t* out_generated,

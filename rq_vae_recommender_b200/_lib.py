@@ -85,6 +85,14 @@ _SIGNATURES = {
                                                         c_int, c_int, c_vp]),
     "rqb200_sid_trie_beam_topk_including": (c_int, [c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp,
                                                     c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
+    "rqb200_sid_trie_beam_topk_capped": (c_int, [c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp,
+                                                 c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
+    "rqb200_sid_trie_sample_select_capped": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int,
+                                                     c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int,
+                                                     c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
+    "rqb200_sid_trie_sample_select_warped_capped": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int,
+                                                            c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_f32,
+                                                            c_f32, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
     "rqb200_sid_trie_beam_topk_wide": (c_int, [c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp,
                                                c_vp, c_vp, c_vp, c_int, c_vp]),
     "rqb200_sid_trie_beam_topk_wide_excluding": (c_int, [c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp,

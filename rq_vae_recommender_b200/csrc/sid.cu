@@ -929,14 +929,27 @@ static size_t sid_sample_smem(int kp, int nc, int K) {
   return E * (sizeof(int64_t) + sizeof(float) + 1) + (size_t)W * (K + 256 + 2 * nc + (K + 31) / 32) * 4 + (WARP ? 4 : 0);
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// The per-prefix cap (CAP mode of sid_beam_topk_kernel and sid_sample_select_kernel): at a level h >= len, at most m of a
+// history's kept beams with a finite score share their first len ids.  A candidate's group is its parent beam's len-prefix,
+// named by the lowest beam of the row with an equal prefix.  The kept set is the greedy walk down the uncapped order (score
+// descending, lowest flat index first) that skips a candidate whose group already holds m: it keeps each group's m best
+// candidates and drops the rest to -inf, where they rank among the -inf fillers by flat index as every filler does.  A group
+// holding fewer than m finite candidates loses none; -inf candidates are unchanged either way.
+struct SidCap {
+  int len;                                                  // prefix length, 1 <= len <= h
+  int m;                                                    // most kept beams per group, 1 <= m < k (m >= k cannot bind)
+};
+
 // WARP: the warped draw (above) from the head's logits (`probas` holds them), else the untempered draw from the softmax.
-template <int FILTER, bool WARP>                            // SidFilterMode: the filter's code is compiled only with one
+// CAP: the per-prefix cap (SidCap, defined with sid_beam_topk_kernel) on the selection; the draws do not change.
+template <int FILTER, bool WARP, bool CAP = false>          // SidFilterMode: the filter's code is compiled only with one
 __global__ void __launch_bounds__(SID_SAMPLE_MAX_WARPS * 32, WARP ? 1 : 0) sid_sample_select_kernel(
     const float* __restrict__ probas, int64_t p_stride, const float* __restrict__ noise, int64_t n_stride,
     const int64_t* __restrict__ generated, const float* __restrict__ log_probas, int kp, int nc, int h, int k, int K, SidTrie trie,
     int64_t* __restrict__ out_generated, float* __restrict__ out_log_probas, int64_t* __restrict__ out_parent,
     int64_t* __restrict__ samples, float* __restrict__ samp_log_p, int* __restrict__ reject, SidExcl ex, float temp,
-    double top_p) {
+    double top_p, SidCap cap) {
   extern __shared__ __align__(16) unsigned char sid_smem[];
   const int W = blockDim.x >> 5, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int b = blockIdx.x, E = kp * nc, KW = (K + 31) >> 5;
@@ -993,6 +1006,47 @@ __global__ void __launch_bounds__(SID_SAMPLE_MAX_WARPS * 32, WARP ? 1 : 0) sid_s
     }
   }
   __syncthreads();
+  if constexpr (CAP) {
+    // group of each beam (the lowest beam with the same len-prefix), then each candidate's rank in its group's order (score
+    // descending, lowest flat index first): past m it drops to -inf.  s_taken marks the dropped ones until every rank is taken.
+    int* s_grp = reinterpret_cast<int*>(s_taken + ((E + 3) & ~3));                                       // [kp]
+    const int nt = blockDim.x;
+    for (int t = threadIdx.x; t < kp; t += nt) {
+      const int64_t* ids = generated + ((int64_t)b * kp + t) * h;
+      int g = t;
+      for (int j = 0; j < t && g == t; ++j) {
+        const int64_t* jd = generated + ((int64_t)b * kp + j) * h;
+        bool eq = true;
+        for (int l = 0; l < cap.len; ++l) eq &= jd[l] == ids[l];
+        if (eq) g = j;
+      }
+      s_grp[t] = g;
+    }
+    __syncthreads();
+    for (int e = threadIdx.x; e < E; e += nt) {
+      const int g = s_grp[e / nc];
+      const float sc = s_score[e];
+      int above = 0;
+      for (int j = g; j < kp && above < cap.m; ++j) {
+        if (s_grp[j] != g) continue;
+#pragma unroll 1
+        for (int r = 0; r < nc; ++r) {
+          const int f = j * nc + r;
+          const float o = s_score[f];
+          above += o > sc || (o == sc && f < e);
+        }
+      }
+      s_taken[e] = above >= cap.m;
+    }
+    __syncthreads();
+    for (int e = threadIdx.x; e < E; e += nt) {
+      if (s_taken[e]) {
+        s_score[e] = -INFINITY;
+        s_taken[e] = 0;
+      }
+    }
+    __syncthreads();
+  }
   if (w == 0)
     sid_keep_best(s_score, s_taken, s_tok, E, nc, b, kp, h, k, generated, out_generated, out_log_probas, out_parent, lane);
 }
@@ -1017,16 +1071,38 @@ static int sid_check_warp(float temp, float top_p, const char* what) {
   return RQB_OK;
 }
 
+// The per-prefix cap of a level h: 1 <= len <= h and m >= 1 (RQB_ERR_INVALID otherwise)
+static int sid_check_cap(const SidCap& cap, int h, const char* what) {
+  RQB_CHECK_ARG(cap.len >= 1 && cap.len <= h && cap.m >= 1,
+                "%s: need 1 <= prefix_len <= h and max_per_prefix >= 1 (prefix_len = %d, h = %d, max_per_prefix = %d)", what,
+                cap.len, h, cap.m);
+  return RQB_OK;
+}
+
+// The filter of a *_capped entry point: mode (SidFilterMode), then the arrays of rqb200_sid_exclusion_build /
+// rqb200_sid_inclusion_build (null / 0 without a filter)
+static int sid_filter_of(int mode, const int* pos, const int64_t* keys, const int* count, int M, int H, int levels,
+                         const char* what, SidExcl& f) {
+  f = SidExcl{};
+  RQB_CHECK_ARG(mode == SID_FILTER_NONE || mode == SID_FILTER_EXCLUDE || mode == SID_FILTER_INCLUDE, "%s: bad filter mode %d",
+                what, mode);
+  if (mode == SID_FILTER_NONE) return RQB_OK;
+  RQB_CHECK_ARG(count, "%s: filter mode %d needs the filter's arrays", what, mode);
+  return sid_excl_of(pos, keys, count, M, H, levels, what, f, mode == SID_FILTER_INCLUDE);
+}
+
 template <bool WARP>
 static int sid_sample_select(const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride,
                              const int64_t* generated, const float* log_probas, int B, int kp, int nc, int h, int k, int C, int K,
                              const void* prefix_workspace, int64_t* out_generated, float* out_log_probas, int64_t* out_parent,
                              int64_t* samples, float* samp_log_p, int* reject, const SidExcl& ex, float temp, float top_p,
-                             void* stream) {
+                             void* stream, const SidCap* cap = nullptr) {
   RQB_CHECK_ARG(B >= 0 && kp > 0 && nc > 0 && h >= 0 && h < C && C <= 8 && k > 0 && K > 0 && probas_stride >= K &&
                     noise_stride >= K, "sid_trie_sample_select: bad argument (B=%d kp=%d nc=%d h=%d k=%d C=%d K=%d)", B, kp, nc, h,
                 k, C, K);
   if (WARP && sid_check_warp(temp, top_p, "sid_trie_sample_select_warped") != RQB_OK) return RQB_ERR_INVALID;
+  if (cap && sid_check_cap(*cap, h, WARP ? "sid_trie_sample_select_warped_capped" : "sid_trie_sample_select_capped") != RQB_OK)
+    return RQB_ERR_INVALID;
   if (nc > K || K > SID_SAMPLE_MAX_K || kp * nc > SID_BEAM_MAX_E || k > 32) {
     rqb_set_error("sid_trie_sample_select: need nc <= K <= %d, kp * nc <= %d, k <= 32 (nc = %d, K = %d, kp * nc = %d, k = %d)",
                   SID_SAMPLE_MAX_K, SID_BEAM_MAX_E, nc, K, kp * nc, k);
@@ -1036,16 +1112,21 @@ static int sid_sample_select(const float* probas, int64_t probas_stride, const f
   RQB_CHECK_ARG(probas && noise && prefix_workspace && out_generated && out_log_probas && out_parent && (h == 0 || generated) &&
                     (h == 0 || log_probas), "sid_trie_sample_select: null pointer");
   const int W = kp < SID_SAMPLE_MAX_WARPS ? kp : SID_SAMPLE_MAX_WARPS;
-  const size_t smem = sid_sample_smem<WARP>(kp, nc, K);
+  const bool capped = cap && cap->m < k;                    // a cap of k or more cannot bind: the uncapped kernel
+  size_t smem = sid_sample_smem<WARP>(kp, nc, K);
+  if (capped) smem = (smem + 3) / 4 * 4 + (size_t)kp * sizeof(int);   // the beams' groups after s_taken
   const int mode = sid_filter_mode(ex);
-  auto kernel = mode == SID_FILTER_INCLUDE ? sid_sample_select_kernel<SID_FILTER_INCLUDE, WARP>
+  auto kernel = capped ? (mode == SID_FILTER_INCLUDE ? sid_sample_select_kernel<SID_FILTER_INCLUDE, WARP, true>
+                          : mode == SID_FILTER_EXCLUDE ? sid_sample_select_kernel<SID_FILTER_EXCLUDE, WARP, true>
+                                                       : sid_sample_select_kernel<SID_FILTER_NONE, WARP, true>)
+                : mode == SID_FILTER_INCLUDE ? sid_sample_select_kernel<SID_FILTER_INCLUDE, WARP>
                 : mode == SID_FILTER_EXCLUDE ? sid_sample_select_kernel<SID_FILTER_EXCLUDE, WARP>
                                              : sid_sample_select_kernel<SID_FILTER_NONE, WARP>;
   RQB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kernel<<<B, W * 32, smem, reinterpret_cast<cudaStream_t>(stream)>>>(
       probas, probas_stride, noise, noise_stride, generated, log_probas, kp, nc, h, k, K,
       SidTrie{reinterpret_cast<const unsigned char*>(prefix_workspace), h + 1}, out_generated, out_log_probas, out_parent, samples,
-      samp_log_p, reject, ex, temp, top_p);
+      samp_log_p, reject, ex, temp, top_p, capped ? *cap : SidCap{0, 0});
   RQB_LAUNCH_CHECK();
   return RQB_OK;
 }
@@ -1123,6 +1204,35 @@ extern "C" int rqb200_sid_trie_sample_select_warped_including(
                                  temperature, top_p, stream);
 }
 
+extern "C" int rqb200_sid_trie_sample_select_capped(
+    const float* probas, int64_t probas_stride, const float* noise, int64_t noise_stride, const int64_t* generated,
+    const float* log_probas, int B, int kp, int nc, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
+    float* out_log_probas, int64_t* out_parent, int64_t* samples, float* samp_log_p, int* reject, int prefix_len, int max_per_prefix,
+    int filter_mode, const int* f_pos, const int64_t* f_keys, const int* f_count, int f_M, int f_H, void* stream) {
+  SidExcl f;
+  const int rc = sid_filter_of(filter_mode, f_pos, f_keys, f_count, f_M, f_H, h + 1, "sid_trie_sample_select_capped", f);
+  if (rc != RQB_OK) return rc;
+  const SidCap cap{prefix_len, max_per_prefix};
+  return sid_sample_select<false>(probas, probas_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K,
+                                  prefix_workspace, out_generated, out_log_probas, out_parent, samples, samp_log_p, reject, f, 1.f,
+                                  1.f, stream, &cap);
+}
+
+extern "C" int rqb200_sid_trie_sample_select_warped_capped(
+    const float* logits, int64_t logits_stride, const float* noise, int64_t noise_stride, const int64_t* generated,
+    const float* log_probas, int B, int kp, int nc, int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated,
+    float* out_log_probas, int64_t* out_parent, int64_t* samples, float* samp_log_p, int* bad, float temperature, float top_p,
+    int prefix_len, int max_per_prefix, int filter_mode, const int* f_pos, const int64_t* f_keys, const int* f_count, int f_M,
+    int f_H, void* stream) {
+  SidExcl f;
+  const int rc = sid_filter_of(filter_mode, f_pos, f_keys, f_count, f_M, f_H, h + 1, "sid_trie_sample_select_warped_capped", f);
+  if (rc != RQB_OK) return rc;
+  const SidCap cap{prefix_len, max_per_prefix};
+  return sid_sample_select<true>(logits, logits_stride, noise, noise_stride, generated, log_probas, B, kp, nc, h, k, C, K,
+                                 prefix_workspace, out_generated, out_log_probas, out_parent, samples, samp_log_p, bad, f,
+                                 temperature, top_p, stream, &cap);
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 // One level of the exhaustive constrained beam search, from the head's logits, in one launch: every code of every beam is a
 // candidate.  Per beam row lse = m + logf(sum expf(x - m)) in a fixed reduction order; candidate e = beam * K + c scores
@@ -1160,11 +1270,111 @@ __device__ __forceinline__ unsigned int sid_topk_candidate(const float* __restri
   return sid_topk_key(sc == 0.f ? 0.f : sc);
 }
 
-template <bool KEYS_IN_SMEM, int FILTER>                    // FILTER: SidFilterMode
+#define SID_FILLER_KEY 0x007fffffu                          // sid_topk_key(-inf): below every other candidate's key
+
+// byte offset of the CAP mode's per-beam arrays in sid_beam_topk_kernel's dynamic shared memory (after keys and masks), and
+// their size: 2 x 64-bit cut + 4 ints per beam
+__host__ __device__ __forceinline__ size_t sid_topk_cap_offset(int E, int kp, int K, bool keys_in_smem) {
+  return ((size_t)((keys_in_smem ? E : 0) + kp * ((K + 31) / 32)) * sizeof(unsigned int) + 7) / 8 * 8;
+}
+#define SID_TOPK_CAP_BYTES_PER_BEAM (2 * sizeof(unsigned long long) + 4 * sizeof(int))
+
+// Threads 0 .. kp - 1: grp[beam] = the lowest beam of the row whose first len ids equal beam's (ids [kp][h] in shared memory).
+// Then beams 0 .. kp - 1 again: order[pos] = the beams by (group, beam), start[g] / count[g] = a leader g's run in `order`.
+// Two __syncthreads; every thread must call.
+__device__ __forceinline__ void sid_cap_groups(const int64_t* ids, int h, int kp, int len, int* grp, int* order, int* start,
+                                               int* count) {
+  const int t = threadIdx.x;
+  if (t < kp) {
+    int g = t;
+    for (int j = 0; j < t && g == t; ++j) {
+      bool eq = true;
+      for (int l = 0; l < len; ++l) eq &= ids[j * h + l] == ids[t * h + l];
+      if (eq) g = j;
+    }
+    grp[t] = g;
+  }
+  __syncthreads();
+  if (t < kp) {
+    const int g = grp[t];
+    int pos = 0, n = 0, lead = 0;
+    for (int j = 0; j < kp; ++j) {
+      const int gj = grp[j];
+      pos += gj < g || (gj == g && j < t);
+      n += gj == g;
+      lead += gj < g;
+    }
+    order[pos] = t;
+    if (g == t) {
+      start[t] = lead;
+      count[t] = n;
+    }
+  }
+  __syncthreads();
+}
+
+// The whole block: the cut (prefix, digit mask) of the `want` largest of the n distinct 48-bit keys key_at(i), i < n -- a key
+// is among them iff (v & pmask) >= prefix -- by sid_beam_topk_kernel's radix selection.  s.hist is zero on entry and on return.
+template <typename KeyAt>
+__device__ __forceinline__ void sid_block_cut(const KeyAt& key_at, int n, int want, SidTopkShared& s, unsigned long long& prefix,
+                                              unsigned long long& pmask) {
+  const int nt = blockDim.x, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const unsigned int lt = (1u << lane) - 1u;
+  prefix = 0;
+  pmask = 0;
+  for (int shift = 40; shift >= 0; shift -= 8) {
+    for (int base = 0; base < n; base += nt) {
+      const int i = base + threadIdx.x;
+      int d = 256;
+      if (i < n) {
+        const unsigned long long v = key_at(i);
+        if ((v & pmask) == prefix) d = (int)((v >> shift) & 255u);
+      }
+      const unsigned int same = __match_any_sync(0xffffffffu, d);
+      if (d < 256 && (same & lt) == 0) atomicAdd(&s.hist[d], __popc(same));
+    }
+    __syncthreads();
+    if (w == 0) {
+      int c[8], sum = 0;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        c[j] = s.hist[lane * 8 + j];
+        s.hist[lane * 8 + j] = 0;
+        sum += c[j];
+      }
+      int suf = sum;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_down_sync(0xffffffffu, suf, o);
+        if (lane + o < 32) suf += t;
+      }
+      const int owner = 31 - __clz(__ballot_sync(0xffffffffu, suf >= want));
+      if (lane == owner) {
+        int acc = suf - sum;
+        for (int j = 7; j >= 0; --j) {
+          if (acc + c[j] >= want) {
+            s.ctl[0] = lane * 8 + j;
+            s.ctl[1] = acc;
+            s.ctl[2] = c[j];
+            break;
+          }
+          acc += c[j];
+        }
+      }
+    }
+    __syncthreads();
+    want -= s.ctl[1];
+    prefix |= (unsigned long long)s.ctl[0] << shift;
+    pmask |= 255ull << shift;
+    if (s.ctl[2] == want) break;
+  }
+}
+
+template <bool KEYS_IN_SMEM, int FILTER, bool CAP = false>  // FILTER: SidFilterMode; CAP: the per-prefix cap (SidCap)
 __global__ void __launch_bounds__(SID_TOPK_MAX_THREADS) sid_beam_topk_kernel(
     const float* __restrict__ logits, int64_t ld, const int64_t* __restrict__ generated, const float* __restrict__ log_probas,
     int kp, int h, int k, int K, SidTrie trie, int64_t* __restrict__ out_generated, float* __restrict__ out_log_probas,
-    int64_t* __restrict__ out_parent, int* __restrict__ bad, SidExcl ex) {
+    int64_t* __restrict__ out_parent, int* __restrict__ bad, SidExcl ex, SidCap cap) {
   extern __shared__ __align__(16) unsigned char sid_smem[];
   __shared__ SidTopkShared s;
   unsigned int* s_key = reinterpret_cast<unsigned int*>(sid_smem);                // [E] when KEYS_IN_SMEM
@@ -1173,6 +1383,12 @@ __global__ void __launch_bounds__(SID_TOPK_MAX_THREADS) sid_beam_topk_kernel(
   const int b = blockIdx.x, E = kp * K;
   const int64_t row0 = (int64_t)b * kp;
   unsigned int* s_mask = s_key + (KEYS_IN_SMEM ? E : 0);   // [kp][ceil(K / 32)]
+  // CAP: after the masks, per beam: the group's kept-key test (prefix, digit mask) at its leader, group, order, run start/count
+  unsigned long long* s_cut = reinterpret_cast<unsigned long long*>(sid_smem + sid_topk_cap_offset(E, kp, K, KEYS_IN_SMEM));
+  int* s_grp = reinterpret_cast<int*>(s_cut + 2 * kp);
+  int* s_order = s_grp + kp;
+  int* s_start = s_order + kp;
+  int* s_count = s_start + kp;
   for (int i = threadIdx.x; i < 256; i += nt) s.hist[i] = 0;
   for (int i = threadIdx.x; i < kp * h; i += nt) s.gen[i] = generated[row0 * h + i];
   if (threadIdx.x == 0) s.nsel = 0;
@@ -1202,6 +1418,40 @@ __global__ void __launch_bounds__(SID_TOPK_MAX_THREADS) sid_beam_topk_kernel(
   for (int beam = w; beam < kp; beam += W)
     sid_beam_mask<FILTER>(trie, ex, b, s.gen + beam * h, h, K, s_mask + beam * ((K + 31) >> 5), lane);
   __syncthreads();
+  // CAP: candidate e's key, or the filler's when its group's cut leaves it out
+  auto capped = [&](int e, unsigned int key) -> unsigned int {
+    const int g = s_grp[e / K];
+    const unsigned long long v = ((unsigned long long)key << 16) | (unsigned int)(0xffff - e);
+    return (v & s_cut[2 * g + 1]) >= s_cut[2 * g] ? key : SID_FILLER_KEY;
+  };
+  if constexpr (CAP) {                                      // each group's cut: the radix selection over its beams' candidates
+    sid_cap_groups(s.gen, h, kp, cap.len, s_grp, s_order, s_start, s_count);
+    if (KEYS_IN_SMEM) {
+      for (int e = threadIdx.x; e < E; e += nt) s_key[e] = sid_topk_candidate(logits, ld, row0, K, e, s, s_mask);
+      __syncthreads();
+    }
+    for (int g = 0; g < kp; ++g) {
+      if (s_grp[g] != g) continue;                          // uniform: every thread reads the same group table
+      const int* members = s_order + s_start[g];
+      auto key_at = [&](int i) -> unsigned long long {
+        const int j = i / K;
+        const int e = members[j] * K + (i - j * K);
+        const unsigned int key = KEYS_IN_SMEM ? s_key[e] : sid_topk_candidate(logits, ld, row0, K, e, s, s_mask);
+        return ((unsigned long long)key << 16) | (unsigned int)(0xffff - e);
+      };
+      unsigned long long cut, cut_mask;
+      sid_block_cut(key_at, s_count[g] * K, cap.m, s, cut, cut_mask);
+      if (threadIdx.x == 0) {
+        s_cut[2 * g] = cut;
+        s_cut[2 * g + 1] = cut_mask;
+      }
+    }
+    __syncthreads();
+    if (KEYS_IN_SMEM) {
+      for (int e = threadIdx.x; e < E; e += nt) s_key[e] = capped(e, s_key[e]);
+      __syncthreads();
+    }
+  }
   unsigned long long prefix = 0, pmask = 0;
   int want = k;                                             // entries still needed among those matching the decided digits
   for (int shift = 40; shift >= 0; shift -= 8) {
@@ -1211,10 +1461,11 @@ __global__ void __launch_bounds__(SID_TOPK_MAX_THREADS) sid_beam_topk_kernel(
       if (e < E) {
         unsigned int key;
         if (KEYS_IN_SMEM) {
-          if (shift == 40) s_key[e] = key = sid_topk_candidate(logits, ld, row0, K, e, s, s_mask);
+          if (shift == 40 && !CAP) s_key[e] = key = sid_topk_candidate(logits, ld, row0, K, e, s, s_mask);
           else key = s_key[e];
         } else {
           key = sid_topk_candidate(logits, ld, row0, K, e, s, s_mask);
+          if (CAP) key = capped(e, key);
         }
         const unsigned long long v = ((unsigned long long)key << 16) | (unsigned int)(0xffff - e);
         if ((v & pmask) == prefix) d = (int)((v >> shift) & 255u);
@@ -1259,7 +1510,8 @@ __global__ void __launch_bounds__(SID_TOPK_MAX_THREADS) sid_beam_topk_kernel(
   }
   // the kept set: keys whose decided digits are above the prefix (k - want of them) or equal to it (want of them)
   for (int e = threadIdx.x; e < E; e += nt) {
-    const unsigned int key = KEYS_IN_SMEM ? s_key[e] : sid_topk_candidate(logits, ld, row0, K, e, s, s_mask);
+    unsigned int key = KEYS_IN_SMEM ? s_key[e] : sid_topk_candidate(logits, ld, row0, K, e, s, s_mask);
+    if (CAP && !KEYS_IN_SMEM) key = capped(e, key);
     const unsigned long long v = ((unsigned long long)key << 16) | (unsigned int)(0xffff - e);
     if ((v & pmask) >= prefix) s.sel[atomicAdd(&s.nsel, 1)] = v;
   }
@@ -1280,21 +1532,24 @@ __global__ void __launch_bounds__(SID_TOPK_MAX_THREADS) sid_beam_topk_kernel(
   }
 }
 
-template <int FILTER>
+template <int FILTER, bool CAP>
 static int sid_beam_topk_launch(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas,
                                 int B, int kp, int h, int k, int K, const SidTrie& trie, int64_t* out_generated,
-                                float* out_log_probas, int64_t* out_parent, int* bad, const SidExcl& ex, cudaStream_t st) {
+                                float* out_log_probas, int64_t* out_parent, int* bad, const SidExcl& ex, const SidCap& cap,
+                                cudaStream_t st) {
   const int E = kp * K;
   const int nt = E >= 4096 ? SID_TOPK_MAX_THREADS : E >= 1024 ? 256 : 128;
   const size_t mask = (size_t)kp * ((K + 31) / 32) * sizeof(unsigned int);
   if (E <= SID_TOPK_SMEM_KEYS) {
-    const size_t smem = (size_t)E * sizeof(unsigned int) + mask;
-    RQB_CUDA(cudaFuncSetAttribute(sid_beam_topk_kernel<true, FILTER>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    sid_beam_topk_kernel<true, FILTER><<<B, nt, smem, st>>>(logits, logits_stride, generated, log_probas, kp, h, k, K, trie,
-                                                            out_generated, out_log_probas, out_parent, bad, ex);
+    const size_t smem = CAP ? sid_topk_cap_offset(E, kp, K, true) + kp * SID_TOPK_CAP_BYTES_PER_BEAM
+                            : (size_t)E * sizeof(unsigned int) + mask;
+    RQB_CUDA(cudaFuncSetAttribute(sid_beam_topk_kernel<true, FILTER, CAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    sid_beam_topk_kernel<true, FILTER, CAP><<<B, nt, smem, st>>>(logits, logits_stride, generated, log_probas, kp, h, k, K, trie,
+                                                                 out_generated, out_log_probas, out_parent, bad, ex, cap);
   } else {
-    sid_beam_topk_kernel<false, FILTER><<<B, nt, mask, st>>>(logits, logits_stride, generated, log_probas, kp, h, k, K, trie,
-                                                             out_generated, out_log_probas, out_parent, bad, ex);
+    const size_t smem = CAP ? sid_topk_cap_offset(E, kp, K, false) + kp * SID_TOPK_CAP_BYTES_PER_BEAM : mask;
+    sid_beam_topk_kernel<false, FILTER, CAP><<<B, nt, smem, st>>>(logits, logits_stride, generated, log_probas, kp, h, k, K, trie,
+                                                                  out_generated, out_log_probas, out_parent, bad, ex, cap);
   }
   RQB_LAUNCH_CHECK();
   return RQB_OK;
@@ -1302,9 +1557,10 @@ static int sid_beam_topk_launch(const float* logits, int64_t logits_stride, cons
 
 static int sid_beam_topk(const float* logits, int64_t logits_stride, const int64_t* generated, const float* log_probas, int B, int kp,
                          int h, int k, int C, int K, const void* prefix_workspace, int64_t* out_generated, float* out_log_probas,
-                         int64_t* out_parent, int* bad, const SidExcl& ex, void* stream) {
+                         int64_t* out_parent, int* bad, const SidExcl& ex, void* stream, const SidCap* cap = nullptr) {
   RQB_CHECK_ARG(B >= 0 && kp > 0 && h >= 0 && h < C && C <= 8 && k > 0 && K > 0 && logits_stride >= K,
                 "sid_trie_beam_topk: bad argument (B=%d kp=%d h=%d k=%d C=%d K=%d)", B, kp, h, k, C, K);
+  if (cap && sid_check_cap(*cap, h, "sid_trie_beam_topk_capped") != RQB_OK) return RQB_ERR_INVALID;
   if (K > SID_TOPK_MAX_K || k > 32 || k > K || kp > SID_TOPK_MAX_BEAMS) {
     rqb_set_error("sid_trie_beam_topk: need K <= %d, k <= 32, k <= K, kp <= %d (K = %d, k = %d, kp = %d)", SID_TOPK_MAX_K,
                   SID_TOPK_MAX_BEAMS, K, k, kp);
@@ -1315,16 +1571,30 @@ static int sid_beam_topk(const float* logits, int64_t logits_stride, const int64
                     (h == 0 || log_probas), "sid_trie_beam_topk: null pointer");
   const SidTrie trie{reinterpret_cast<const unsigned char*>(prefix_workspace), h + 1};
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const SidCap c = cap ? *cap : SidCap{0, 0};
+  if (cap && cap->m < k) {                                  // a cap of k or more cannot bind: the uncapped kernel
+    switch (sid_filter_mode(ex)) {
+      case SID_FILTER_INCLUDE:
+        return sid_beam_topk_launch<SID_FILTER_INCLUDE, true>(logits, logits_stride, generated, log_probas, B, kp, h, k, K, trie,
+                                                              out_generated, out_log_probas, out_parent, bad, ex, c, st);
+      case SID_FILTER_EXCLUDE:
+        return sid_beam_topk_launch<SID_FILTER_EXCLUDE, true>(logits, logits_stride, generated, log_probas, B, kp, h, k, K, trie,
+                                                              out_generated, out_log_probas, out_parent, bad, ex, c, st);
+      default:
+        return sid_beam_topk_launch<SID_FILTER_NONE, true>(logits, logits_stride, generated, log_probas, B, kp, h, k, K, trie,
+                                                           out_generated, out_log_probas, out_parent, bad, ex, c, st);
+    }
+  }
   switch (sid_filter_mode(ex)) {
     case SID_FILTER_INCLUDE:
-      return sid_beam_topk_launch<SID_FILTER_INCLUDE>(logits, logits_stride, generated, log_probas, B, kp, h, k, K, trie,
-                                                      out_generated, out_log_probas, out_parent, bad, ex, st);
+      return sid_beam_topk_launch<SID_FILTER_INCLUDE, false>(logits, logits_stride, generated, log_probas, B, kp, h, k, K, trie,
+                                                             out_generated, out_log_probas, out_parent, bad, ex, c, st);
     case SID_FILTER_EXCLUDE:
-      return sid_beam_topk_launch<SID_FILTER_EXCLUDE>(logits, logits_stride, generated, log_probas, B, kp, h, k, K, trie,
-                                                      out_generated, out_log_probas, out_parent, bad, ex, st);
+      return sid_beam_topk_launch<SID_FILTER_EXCLUDE, false>(logits, logits_stride, generated, log_probas, B, kp, h, k, K, trie,
+                                                             out_generated, out_log_probas, out_parent, bad, ex, c, st);
     default:
-      return sid_beam_topk_launch<SID_FILTER_NONE>(logits, logits_stride, generated, log_probas, B, kp, h, k, K, trie,
-                                                   out_generated, out_log_probas, out_parent, bad, ex, st);
+      return sid_beam_topk_launch<SID_FILTER_NONE, false>(logits, logits_stride, generated, log_probas, B, kp, h, k, K, trie,
+                                                          out_generated, out_log_probas, out_parent, bad, ex, c, st);
   }
 }
 
@@ -1357,6 +1627,20 @@ extern "C" int rqb200_sid_trie_beam_topk_including(const float* logits, int64_t 
   if (rc != RQB_OK) return rc;
   return sid_beam_topk(logits, logits_stride, generated, log_probas, B, kp, h, k, C, K, prefix_workspace, out_generated,
                        out_log_probas, out_parent, bad, in, stream);
+}
+
+extern "C" int rqb200_sid_trie_beam_topk_capped(const float* logits, int64_t logits_stride, const int64_t* generated,
+                                                const float* log_probas, int B, int kp, int h, int k, int C, int K,
+                                                const void* prefix_workspace, int64_t* out_generated, float* out_log_probas,
+                                                int64_t* out_parent, int* bad, int prefix_len, int max_per_prefix, int filter_mode,
+                                                const int* f_pos, const int64_t* f_keys, const int* f_count, int f_M, int f_H,
+                                                void* stream) {
+  SidExcl f;
+  const int rc = sid_filter_of(filter_mode, f_pos, f_keys, f_count, f_M, f_H, h + 1, "sid_trie_beam_topk_capped", f);
+  if (rc != RQB_OK) return rc;
+  const SidCap cap{prefix_len, max_per_prefix};
+  return sid_beam_topk(logits, logits_stride, generated, log_probas, B, kp, h, k, C, K, prefix_workspace, out_generated,
+                       out_log_probas, out_parent, bad, f, stream, &cap);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

@@ -902,6 +902,23 @@ def _sampling_controls(search: str, temperature, top_p, H: int, what: str, ignor
     return list(zip(temps, ps))
 
 
+def _prefix_cap_controls(search: str, max_per_prefix: Optional[int], prefix_len: int, H: int, what: str):
+    """The (prefix_len, max_per_prefix) of a capped search, checked before any launch: None without ``max_per_prefix``.
+    prefix_len must be in [1, H - 1] and max_per_prefix >= 1, else ``ValueError``; search="exact" raises ``ValueError``."""
+    if max_per_prefix is None:
+        return None
+    if isinstance(max_per_prefix, bool) or isinstance(prefix_len, bool):
+        raise ValueError(f"{what}: max_per_prefix and prefix_len must be integers")
+    if int(max_per_prefix) != max_per_prefix or max_per_prefix < 1:
+        raise ValueError(f"{what}: max_per_prefix must be an integer >= 1, got {max_per_prefix!r}")
+    if int(prefix_len) != prefix_len or not 1 <= prefix_len <= H - 1:
+        raise ValueError(f"{what}: prefix_len must be an integer in [1, {H - 1}] (the id tuple has {H} levels), got "
+                         f"{prefix_len!r}")
+    if search == "exact":
+        raise ValueError(f"{what}: max_per_prefix caps the \"beam\" and \"sample\" searches only; search=\"exact\" takes no cap")
+    return int(prefix_len), int(max_per_prefix)
+
+
 def _non_finite_error(what: str, n_bad: int) -> RuntimeError:
     return RuntimeError(f"{what}: {n_bad} decoder row(s) of the head's logits "
                         "hold a NaN or +inf or are all -inf; the items below them score NaN")
@@ -1079,29 +1096,44 @@ class EncoderDecoderRetrievalModel(nn.Module):
     def _sample_and_select(self, index: ops.SidPrefixIndex, probas: Tensor, generated: Optional[Tensor],
                            log_probas: Optional[Tensor], k: int, n_cands: int, reject: Tensor,
                            exclude: Optional[ops.SidExclusion] = None, include: Optional[ops.SidInclusion] = None,
-                           wide: bool = False):
+                           wide: bool = False, cap: Optional[tuple] = None):
         """One level of the search after the softmax: n_cands samples per beam, prefix check, scores, the k best beams
         (``wide``: on the cluster kernel, ``SidPrefixIndex.sample_select_wide``)."""
         filt = {} if exclude is None else {"exclude": exclude}
         if include is not None:
             filt["include"] = include
+        if cap is not None:
+            filt["cap"] = cap
         select = index.sample_select_wide if wide else index.sample_select
         return select(probas, draw_exponential(probas), generated, log_probas, k, n_cands, reject=reject, **filt)
 
     @staticmethod
     def _warped_sample_and_select(index: ops.SidPrefixIndex, logits: Tensor, generated: Optional[Tensor],
                                   log_probas: Optional[Tensor], k: int, n_cands: int, bad: Tensor, control: tuple,
-                                  wide: bool, filt: dict):
+                                  wide: bool, filt: dict, cap: Optional[tuple] = None):
         """One level of the search from the head's logits at this level's (temperature, top_p): the noise is drawn as the
         untempered level draws it (``draw_exponential`` of a [B * kp, K] tensor), then one launch of
         ``SidPrefixIndex.sample_select_warped`` (``_wide`` on the cluster kernel)."""
         select = index.sample_select_warped_wide if wide else index.sample_select_warped
+        if cap is not None:
+            filt = dict(filt, cap=cap)
         return select(logits, draw_exponential(logits), generated, log_probas, k, n_cands, *control, bad=bad, **filt)
 
     @staticmethod
     def _narrow_search(search: str, k: int, n_cands: int) -> bool:
         """A search of beam width k fits the one-CTA-per-history selection kernels (``beam_topk`` / ``sample_select``)."""
         return k <= 32 and (search == "beam" or k * n_cands <= 1024)
+
+    def _search_cap(self, cap: Optional[tuple], search: str, k: int, n_cands: int, what: str) -> Optional[tuple]:
+        """A checked cap (``_prefix_cap_controls``) at beam width k: None when max_per_prefix >= k (it cannot bind; the
+        uncapped path runs), else ``Rqb200Error`` when only the cluster kernels take the width (they have no capped mode)."""
+        if cap is None or cap[1] >= k:
+            return None
+        if not self._narrow_search(search, k, n_cands):
+            raise Rqb200Error(f"{what}: max_per_prefix = {cap[1]} caps the one-CTA selection kernels only; num_beams = {k} "
+                              f"(with {n_cands} candidates per beam for \"sample\") runs on the cluster kernels, which take no "
+                              "cap (need num_beams <= 32, and num_beams * candidates <= 1024 for \"sample\")")
+        return cap
 
     def _check_search_limits(self, search: str, k: int, n_cands: int, num_beams: Optional[int] = None) -> None:
         K = self.num_embeddings_per_hierarchy
@@ -1212,7 +1244,8 @@ class EncoderDecoderRetrievalModel(nn.Module):
     @torch.no_grad()
     def generate(self, attention_mask, input_ids, user_id=None, search: Optional[str] = None, decoder: Optional[str] = None,
                  encoder: Optional[str] = None, encoder_attention: Optional[str] = None, exclude_items: Optional[Tensor] = None,
-                 include_items: Optional[Tensor] = None, num_beams: Optional[int] = None, temperature=1.0, top_p=1.0):
+                 include_items: Optional[Tensor] = None, num_beams: Optional[int] = None, temperature=1.0, top_p=1.0,
+                 max_per_prefix: Optional[int] = None, prefix_len: int = 1):
         """Top-k semantic ids by beam search restricted to id prefixes of the corpus.  ``search`` (default: the module's
         ``DEFAULT_SEARCH``, read at call time):
           "sample"  per level, n_cands = min(64, K) tokens sampled without replacement per beam, scored by cumulative
@@ -1247,19 +1280,43 @@ class EncoderDecoderRetrievalModel(nn.Module):
         (``SidPrefixIndex.sample_select_warped``); the beams still score and return the model's own log-probabilities.  T
         finite and > 0, 0 < top_p <= 1; anything else, or anything but 1 with "beam" or "exact", raises ``ValueError``
         before any launch.  Bad head rows then raise the "beam" search's ``RuntimeError``.
+        ``max_per_prefix`` (default None: no cap) / ``prefix_len`` (default 1) cap how many beams share a prefix: among a
+        history's returned beams with a finite log-probability, at most max_per_prefix share their first prefix_len ids (the
+        -inf fillers are not beams and are exempt).  The cap binds at the levels h >= prefix_len (0-based; after level h a beam
+        holds h + 1 ids); earlier levels run unchanged.  There a candidate's group is its parent's first prefix_len ids, and the
+        level keeps what a walk down the search's own order (score descending, then lowest beam * K + code for "beam", the
+        sampled order for "sample") keeps when it skips a candidate whose group already holds max_per_prefix: each group's
+        max_per_prefix best, with the uncapped log-probability bits; the rest of the w slots are -inf fillers as before.  The
+        cap composes with the item filters (a blocked extension is invalid before the cap counts it) and, for "sample", with
+        temperature and top_p (the draws do not change).  "beam" stays deterministic.  prefix_len in [1, H - 1] and
+        max_per_prefix >= 1, else ``ValueError``; search="exact" raises ``ValueError``.  max_per_prefix >= w cannot bind and runs
+        the uncapped search, bit for bit; a cap that can bind on a width only the cluster kernels take (w > 32, or
+        w * n_cands > 1024 for "sample") raises ``Rqb200Error``.  All before any launch.
         Returns generated [B, w, num_hierarchies] and log_probas [B, w]."""
         warp = self._sampling(search, temperature, top_p, "generate")
+        cap = self._capping(search, max_per_prefix, prefix_len, num_beams, "generate")
         return self._generate(attention_mask, input_ids, user_id, search, decoder, encoder, encoder_attention,
                               self._filters(exclude_items, include_items, attention_mask.shape[0], attention_mask.device),
-                              num_beams, warp)
+                              num_beams, warp, cap)
 
     def _sampling(self, search: Optional[str], temperature, top_p, what: str, ignore_temperature: bool = False):
         """``_sampling_controls`` of a call's search (default ``DEFAULT_SEARCH``, read at call time)."""
         search = _choice(search, DEFAULT_SEARCH, SEARCHES, what, "search")
         return _sampling_controls(search, temperature, top_p, self.num_hierarchies, what, ignore_temperature)
 
+    def _capping(self, search: Optional[str], max_per_prefix: Optional[int], prefix_len: int, num_beams: Optional[int],
+                 what: str):
+        """The cap of a call (``_prefix_cap_controls``, then ``_search_cap`` at its beam width), checked on the host before any
+        launch; search defaults to ``DEFAULT_SEARCH``, read at call time."""
+        search = _choice(search, DEFAULT_SEARCH, SEARCHES, what, "search")
+        cap = _prefix_cap_controls(search, max_per_prefix, prefix_len, self.num_hierarchies, what)
+        if cap is None:
+            return None
+        k = self.top_k_for_generation if num_beams is None else int(num_beams)
+        return self._search_cap(cap, search, k, min(MAX_CANDIDATES, self.num_embeddings_per_hierarchy), what)
+
     def _generate(self, attention_mask, input_ids, user_id, search, decoder, encoder, encoder_attention, filters: list,
-                  num_beams: Optional[int] = None, warp: Optional[list] = None):
+                  num_beams: Optional[int] = None, warp: Optional[list] = None, cap: Optional[tuple] = None):
         decoder = _choice(decoder, DEFAULT_DECODER, DECODERS, "generate", "decoder")
         if decoder == "fused" and self.training:
             raise ValueError("generate: decoder=\"fused\" runs the decoder in eval mode only; call model.eval() first (in "
@@ -1283,15 +1340,16 @@ class EncoderDecoderRetrievalModel(nn.Module):
             enc_out, enc_mask = fused_encoder(attention_mask, input_ids, user_id)
         else:
             enc_out, enc_mask = self.encoder_forward_pass(attention_mask=attention_mask, input_ids=input_ids, user_id=user_id)
-        generated, log_probas, reject = self._search_levels(enc_out, enc_mask, search, decoder, k, filters, warp)
+        generated, log_probas, reject = self._search_levels(enc_out, enc_mask, search, decoder, k, filters, warp, cap)
         self._finish_search(_counter_kind(search, warp), reject, filters)
         return generated, log_probas
 
     def _search_levels(self, enc_out: Tensor, enc_mask: Tensor, search: str, decoder: str, k: int, filters: list,
-                       warp: Optional[list] = None):
+                       warp: Optional[list] = None, cap: Optional[tuple] = None):
         """The level loop of a "sample" or "beam" search of width k over the encoder output: (generated [B, k, H], log_probas
         [B, k], the device counters ``_finish_search`` reads).  ``warp``: the per-level (temperature, top_p) of a warped
-        "sample" search (``_sampling_controls``), whose counter is the "beam" search's count of bad head rows."""
+        "sample" search (``_sampling_controls``), whose counter is the "beam" search's count of bad head rows.  ``cap``: the
+        (prefix_len, max_per_prefix) of a capped search (``_search_cap``), applied at the levels h >= prefix_len."""
         n_cands = min(MAX_CANDIDATES, self.num_embeddings_per_hierarchy)
         beam = search == "beam"
         wide = not self._narrow_search(search, k, n_cands)
@@ -1312,7 +1370,18 @@ class EncoderDecoderRetrievalModel(nn.Module):
                     future_ids=None if first else generated.reshape(-1, h), encoder_output=enc_out if first else rep_enc,
                     attention_mask_for_encoder=enc_mask if first else rep_mask, use_cache=True, past_key_values=past_kv)
                 logits = self.decoder_mlp[h](dec_out[:, -1, :])
-            if beam:
+            level_cap = cap if cap is not None and h >= cap[0] else None
+            if level_cap is not None:                         # a cap binds on the one-CTA kernels only (_search_cap)
+                if beam:
+                    generated, log_probas, parent_global = index.beam_topk(logits, generated, log_probas, k, bad=reject,
+                                                                           cap=level_cap, **filt)
+                elif warp is not None:
+                    generated, log_probas, parent_global = self._warped_sample_and_select(
+                        index, logits, generated, log_probas, k, n_cands, reject, warp[h], False, filt, level_cap)
+                else:
+                    generated, log_probas, parent_global = self._sample_and_select(
+                        index, F.softmax(logits, dim=-1), generated, log_probas, k, n_cands, reject, cap=level_cap, **filt)
+            elif beam:
                 topk = index.beam_topk_wide if wide else index.beam_topk
                 generated, log_probas, parent_global = topk(logits, generated, log_probas, k, bad=reject, **filt)
             elif warp is not None:
@@ -1414,11 +1483,12 @@ class EncoderDecoderRetrievalModel(nn.Module):
                              batch.sem_ids.device)
 
     def _generate_batch(self, batch: TokenizedSeqBatch, search, decoder, encoder, encoder_attention,
-                        filters: list, num_beams: Optional[int] = None, warp: Optional[list] = None) -> GenerationOutput:
+                        filters: list, num_beams: Optional[int] = None, warp: Optional[list] = None,
+                        cap: Optional[tuple] = None) -> GenerationOutput:
         H = self.num_hierarchies
         generated, log_probas = self._generate(_strip_dedup_col(batch.seq_mask.long(), H + 1, H),
                                                _strip_dedup_col(batch.sem_ids, H + 1, H), batch.user_ids, search, decoder,
-                                               encoder, encoder_attention, filters, num_beams, warp)
+                                               encoder, encoder_attention, filters, num_beams, warp, cap)
         return GenerationOutput(sem_ids=generated, log_probas=log_probas)
 
     @torch.no_grad()
@@ -1427,33 +1497,37 @@ class EncoderDecoderRetrievalModel(nn.Module):
                              encoder: Optional[str] = None, encoder_attention: Optional[str] = None,
                              exclude_items: Optional[Tensor] = None, exclude_history: Optional[bool] = None,
                              include_items: Optional[Tensor] = None, num_beams: Optional[int] = None,
-                             top_p=1.0) -> GenerationOutput:
+                             top_p=1.0, max_per_prefix: Optional[int] = None, prefix_len: int = 1) -> GenerationOutput:
         """``generate`` on the batch's histories.  ``exclude_items``, ``include_items``, ``num_beams``, ``temperature`` and
         ``top_p`` as in ``generate``, except that "beam" and "exact" ignore ``temperature`` (the reference ignores it for every
         search; ``top_p`` < 1 still raises with them); ``exclude_history`` (default ``DEFAULT_EXCLUDE_HISTORY``, read at call
-        time) also excludes each history's own items (``history_items``).  ``top_k`` is accepted for the reference's
-        signature."""
+        time) also excludes each history's own items (``history_items``).  ``max_per_prefix`` / ``prefix_len`` as in
+        ``generate``.  ``top_k`` is accepted for the reference's signature."""
         warp = self._sampling(search, temperature, top_p, "generate_next_sem_id", ignore_temperature=True)
+        cap = self._capping(search, max_per_prefix, prefix_len, num_beams, "generate_next_sem_id")
         return self._generate_batch(batch, search, decoder, encoder, encoder_attention,
-                                    self._batch_filters(batch, exclude_items, exclude_history, include_items), num_beams, warp)
+                                    self._batch_filters(batch, exclude_items, exclude_history, include_items), num_beams, warp,
+                                    cap)
 
     @torch.no_grad()
     def generate_items(self, batch: TokenizedSeqBatch, n: Optional[int] = None, search: Optional[str] = None,
                        decoder: Optional[str] = None, encoder: Optional[str] = None,
                        encoder_attention: Optional[str] = None, exclude_items: Optional[Tensor] = None,
                        exclude_history: Optional[bool] = None, include_items: Optional[Tensor] = None,
-                       num_beams: Optional[int] = None, temperature=1.0, top_p=1.0) -> ItemGenerationOutput:
+                       num_beams: Optional[int] = None, temperature=1.0, top_p=1.0, max_per_prefix: Optional[int] = None,
+                       prefix_len: int = 1) -> ItemGenerationOutput:
         """The top corpus items for each history: ``generate_next_sem_id``'s beams, unchanged, then one launch that takes the
         items of every finite beam whose ids are in the corpus, beam by beam in descending score order, each beam's items by
         dedup rank, no item twice, at most n (default: the call's beam width, ``num_beams`` or else top_k_for_generation; at
         most ``ops.SidItemTable.MAX_N``) per history.  ``exclude_items`` / ``exclude_history`` as in
         ``generate_next_sem_id``: the search and the retrieval both leave the excluded items out.  ``include_items`` as in
         ``generate``: the search and the retrieval both return only each history's eligible items.  ``num_beams`` as in
-        ``generate``: a wider search yields more candidate items (``n`` up to 4096).  ``temperature`` / ``top_p`` as in
-        ``generate``."""
+        ``generate``: a wider search yields more candidate items (``n`` up to 4096).  ``temperature`` / ``top_p`` and
+        ``max_per_prefix`` / ``prefix_len`` as in ``generate``: with a cap, the items come from the capped beams only."""
         warp = self._sampling(search, temperature, top_p, "generate_items")
+        cap = self._capping(search, max_per_prefix, prefix_len, num_beams, "generate_items")
         filters = self._batch_filters(batch, exclude_items, exclude_history, include_items)
-        out = self._generate_batch(batch, search, decoder, encoder, encoder_attention, filters, num_beams, warp)
+        out = self._generate_batch(batch, search, decoder, encoder, encoder_attention, filters, num_beams, warp, cap)
         table = self._item_table(out.sem_ids.device)
         width = self.top_k_for_generation if num_beams is None else num_beams
         items, beams, count = table.retrieve(out.sem_ids, out.log_probas, width if n is None else n,
@@ -1464,16 +1538,17 @@ class EncoderDecoderRetrievalModel(nn.Module):
                                num_beams: Optional[int] = None, encoder_attention: Optional[str] = None,
                                exclude_items: Optional[Tensor] = None, exclude_history: Optional[bool] = None,
                                include_items: Optional[Tensor] = None, encoder: str = "fused",
-                               decoder: str = "fused", temperature=1.0, top_p=1.0) -> "GenerateItemsGraph":
+                               decoder: str = "fused", temperature=1.0, top_p=1.0, max_per_prefix: Optional[int] = None,
+                               prefix_len: int = 1) -> "GenerateItemsGraph":
         """``generate_items(batch, ..., encoder="fused", decoder="fused")`` captured as one CUDA graph, for serving: calling the
         returned ``GenerateItemsGraph`` with a batch of the same shapes is one graph replay and one host read of the error
         counters.  The example batch fixes every shape: B, the history width, whether ``user_ids`` is given, and the widths of
         ``exclude_items`` / ``include_items`` (and whether each is given).  ``search`` is "sample" or "beam" at any width those
-        searches take; ``search``, ``n``, ``num_beams``, ``encoder_attention``, ``exclude_history``, ``temperature`` and
-        ``top_p`` are read once, here, with ``generate_items``' defaults and checks.  Raises ``ValueError`` for search="exact" (one host read per level), an HF encoder or
+        searches take; ``search``, ``n``, ``num_beams``, ``encoder_attention``, ``exclude_history``, ``temperature``,
+        ``top_p``, ``max_per_prefix`` and ``prefix_len`` are read once, here, with ``generate_items``' defaults and checks.  Raises ``ValueError`` for search="exact" (one host read per level), an HF encoder or
         decoder, training mode and an active autocast region.  See ``GenerateItemsGraph`` for what a replay follows."""
         return GenerateItemsGraph(self, batch, n, search, num_beams, encoder_attention, exclude_items, exclude_history,
-                                  include_items, encoder, decoder, temperature, top_p)
+                                  include_items, encoder, decoder, temperature, top_p, max_per_prefix, prefix_len)
 
     def capture_exact_items(self, batch: TokenizedSeqBatch, n: Optional[int] = None, num_beams: Optional[int] = None,
                             max_rows: Optional[int] = None, encoder_attention: Optional[str] = None,
@@ -1787,7 +1862,8 @@ class GenerateItemsGraph:
     def __init__(self, model: EncoderDecoderRetrievalModel, batch: TokenizedSeqBatch, n: Optional[int], search: Optional[str],
                  num_beams: Optional[int], encoder_attention: Optional[str], exclude_items: Optional[Tensor],
                  exclude_history: Optional[bool], include_items: Optional[Tensor], encoder: str = "fused",
-                 decoder: str = "fused", temperature=1.0, top_p=1.0):
+                 decoder: str = "fused", temperature=1.0, top_p=1.0, max_per_prefix: Optional[int] = None,
+                 prefix_len: int = 1):
         what = "capture_generate_items"
         if encoder != "fused" or decoder != "fused":
             raise ValueError(f"{what}: a CUDA graph runs the fused encoder and decoder only (encoder={encoder!r}, "
@@ -1796,13 +1872,17 @@ class GenerateItemsGraph:
         self.search = _choice(search, DEFAULT_SEARCH, SEARCHES, what, "search")
         #: the per-level (temperature, top_p) of a warped "sample" search, fixed at capture (None: untempered)
         self.warp = _sampling_controls(self.search, temperature, top_p, model.num_hierarchies, what)
+        if self.search == "exact" and max_per_prefix is not None:
+            _prefix_cap_controls(self.search, max_per_prefix, prefix_len, model.num_hierarchies, what)
         if self.search == "exact":
             raise ValueError(f"{what}: search=\"exact\" reads its frontier's size on the host once per level; it cannot be "
                              "captured here (use \"sample\" or \"beam\", or capture_exact_items for the exact search)")
         self.attention = _encoder_attention("fused", encoder_attention, what)
         self.k = model.top_k_for_generation if num_beams is None else int(num_beams)
-        model._check_search_limits(self.search, self.k, min(MAX_CANDIDATES, model.num_embeddings_per_hierarchy),
-                                   None if num_beams is None else self.k)
+        n_cands = min(MAX_CANDIDATES, model.num_embeddings_per_hierarchy)
+        model._check_search_limits(self.search, self.k, n_cands, None if num_beams is None else self.k)
+        #: the (prefix_len, max_per_prefix) of a capped search, fixed at capture (None: uncapped, or a cap that cannot bind)
+        self.cap = model._capping(self.search, max_per_prefix, prefix_len, num_beams, what)
         self.n = self.k if n is None else int(n)
         self.exclude_history = DEFAULT_EXCLUDE_HISTORY if exclude_history is None else bool(exclude_history)
         self._store(model, batch, exclude_items, include_items, what)
@@ -1841,7 +1921,8 @@ class GenerateItemsGraph:
         filters = m._batch_filters(batch, exclude_items, self.exclude_history, include_items)
         enc_out, enc_mask = FusedT5Encode(m, self.attention, capacity=True)(
             _strip_dedup_col(seq.long(), H + 1, H), _strip_dedup_col(sem, H + 1, H), users)
-        generated, log_probas, reject = m._search_levels(enc_out, enc_mask, self.search, "fused", self.k, filters, self.warp)
+        generated, log_probas, reject = m._search_levels(enc_out, enc_mask, self.search, "fused", self.k, filters, self.warp,
+                                                         self.cap)
         items, beams, count = m._item_table(sem.device).retrieve(generated, log_probas, self.n, **m._filter_kwargs(filters))
         out = ItemGenerationOutput(item_ids=items, beams=beams, count=count, sem_ids=generated, log_probas=log_probas)
         return out, m._counter_values(reject, filters), reject.numel(), filters

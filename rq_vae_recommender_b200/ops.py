@@ -7,7 +7,7 @@ from __future__ import annotations
 
 import ctypes
 import weakref
-from typing import List, NamedTuple, Optional, Sequence
+from typing import List, NamedTuple, Optional, Sequence, Tuple
 
 import torch
 
@@ -685,7 +685,7 @@ class SidPrefixIndex:
     def sample_select(self, probas: torch.Tensor, noise: torch.Tensor, generated: Optional[torch.Tensor],
                       log_probas: Optional[torch.Tensor], k: int, nc: int, want_samples: bool = False,
                       reject: Optional[torch.Tensor] = None, exclude: Optional["SidExclusion"] = None,
-                      include: Optional["SidInclusion"] = None):
+                      include: Optional["SidInclusion"] = None, cap: Optional[Tuple[int, int]] = None):
         """The sampling step fused with ``beam_select`` (rqb200_sid_trie_sample_select), one launch.  probas / noise [B * kp, K]
         (kp = 1 on the first level; noise = the Exp(1) draw torch.multinomial makes, ``torch.empty_like(probas).exponential_(1)``),
         generated [B, kp, h] or None, log_probas [B, kp] or None -> (generated [B, k, h + 1], log_probas [B, k],
@@ -695,9 +695,10 @@ class SidPrefixIndex:
         ``exclude`` (``sid_exclusion_build``, one set per history): extensions to a prefix blocked for the history are invalid,
         exactly like prefixes the corpus lacks; the samples do not change.  ``include`` (``sid_inclusion_build``, one allow-list
         per history, any exclusion folded in; not with ``exclude``): extensions to a prefix without an eligible item of the
-        history are invalid alike."""
+        history are invalid alike.  ``cap`` = (prefix_len, max_per_prefix) caps the selection as ``beam_topk``'s ``cap``, in
+        the candidates' order (score descending, lowest beam * nc + slot first); the samples do not change."""
         return self._sample_select("sid_trie_sample_select", probas, noise, generated, log_probas, k, nc, want_samples, reject,
-                                   exclude, include)
+                                   exclude, include, cap=cap)
 
     def sample_select_wide(self, probas: torch.Tensor, noise: torch.Tensor, generated: Optional[torch.Tensor],
                            log_probas: Optional[torch.Tensor], k: int, nc: int, want_samples: bool = False,
@@ -713,7 +714,8 @@ class SidPrefixIndex:
     def sample_select_warped(self, logits: torch.Tensor, noise: torch.Tensor, generated: Optional[torch.Tensor],
                              log_probas: Optional[torch.Tensor], k: int, nc: int, temperature: float, top_p: float,
                              want_samples: bool = False, bad: Optional[torch.Tensor] = None,
-                             exclude: Optional["SidExclusion"] = None, include: Optional["SidInclusion"] = None):
+                             exclude: Optional["SidExclusion"] = None, include: Optional["SidInclusion"] = None,
+                             cap: Optional[Tuple[int, int]] = None):
         """``sample_select`` drawn from the head's logits at ``temperature`` and within a ``top_p`` nucleus
         (rqb200_sid_trie_sample_select_warped), one launch.  logits / noise [B * kp, K].  Per beam row x:
         p_T = softmax(x / T) in fp32; the nucleus N = the codes with p_T >= t, t the largest p_T whose codes at or above it
@@ -722,9 +724,10 @@ class SidPrefixIndex:
         other slots with -inf.  A drawn code scores its model log-probability x[c] - lse (``beam_topk``'s lse, bit for bit)
         plus the parent's, -inf off the trie or blocked by the filter; ``samp_log_p`` holds x[c] - lse (-inf for a filler).
         ``bad``, an int32 device tensor, is ADDED the number of beam rows holding a NaN or +inf or all -inf (their slots are
-        fillers).  T finite and > 0, 0 < top_p <= 1, else ``Rqb200Error``.  ``exclude`` / ``include`` as in ``sample_select``."""
+        fillers).  T finite and > 0, 0 < top_p <= 1, else ``Rqb200Error``.  ``exclude`` / ``include`` / ``cap`` as in
+        ``sample_select``."""
         return self._sample_select("sid_trie_sample_select_warped", logits, noise, generated, log_probas, k, nc, want_samples,
-                                   bad, exclude, include, warp=(float(temperature), float(top_p)))
+                                   bad, exclude, include, warp=(float(temperature), float(top_p)), cap=cap)
 
     def sample_select_warped_wide(self, logits: torch.Tensor, noise: torch.Tensor, generated: Optional[torch.Tensor],
                                   log_probas: Optional[torch.Tensor], k: int, nc: int, temperature: float, top_p: float,
@@ -738,7 +741,8 @@ class SidPrefixIndex:
                                    want_samples, bad, exclude, include, int(cluster), warp=(float(temperature), float(top_p)))
 
     def _sample_select(self, entry: str, probas, noise, generated, log_probas, k: int, nc: int, want_samples: bool, reject,
-                       exclude, include, cluster: Optional[int] = None, warp: Optional[tuple] = None):
+                       exclude, include, cluster: Optional[int] = None, warp: Optional[tuple] = None,
+                       cap: Optional[Tuple[int, int]] = None):
         _need_cuda(probas, noise, reject)
         if generated is None:
             B, kp, h = probas.shape[0], 1, 0
@@ -764,7 +768,7 @@ class SidPrefixIndex:
         out_parent = torch.empty((B * k,), dtype=torch.int64, device=dev)
         samples = torch.empty((B * kp, nc), dtype=torch.int64, device=dev) if want_samples else None
         samp_log_p = torch.empty((B * kp, nc), dtype=torch.float32, device=dev) if want_samples else None
-        name, filt = _filter_entry(entry, exclude, include, B, h + 1, entry[9:])
+        name, filt = _filter_entry(entry, exclude, include, B, h + 1, entry[9:], cap)
         lib = _lib.load()
         wide = ()
         if cluster is not None:                               # the wide entry: its workspace and the cluster size
@@ -784,15 +788,19 @@ class SidPrefixIndex:
 
     def beam_topk(self, logits: torch.Tensor, generated: Optional[torch.Tensor], log_probas: Optional[torch.Tensor], k: int,
                   bad: Optional[torch.Tensor] = None, exclude: Optional["SidExclusion"] = None,
-                  include: Optional["SidInclusion"] = None):
+                  include: Optional["SidInclusion"] = None, cap: Optional[Tuple[int, int]] = None):
         """One level of the exhaustive constrained beam search from the head's logits (rqb200_sid_trie_beam_topk), one launch.
         logits [B * kp, K] (kp = 1 on the first level), generated [B, kp, h] or None, log_probas [B, kp] or None ->
         (generated [B, k, h + 1], log_probas [B, k], parent_global [B * k]): of all kp * K extensions of each history, scored
         log_softmax(logits)[code] + the parent's log-probability (-inf when the extended prefix is not in the corpus), the k
         best in descending order, equal scores by ascending beam * K + code.  Deterministic.  ``bad``, an int32 device tensor,
         is ADDED the number of beam rows whose logits hold a NaN or +inf or are all -inf.  ``exclude`` / ``include`` as in
-        ``sample_select``: extensions to a prefix blocked for the history, or without an eligible item of it, score -inf."""
-        return self._beam_topk("sid_trie_beam_topk", logits, generated, log_probas, k, bad, exclude, include)
+        ``sample_select``: extensions to a prefix blocked for the history, or without an eligible item of it, score -inf.
+        ``cap`` = (prefix_len, max_per_prefix), 1 <= prefix_len <= h and max_per_prefix >= 1 (rqb200_sid_trie_beam_topk_capped):
+        walking down that order, a candidate is kept unless max_per_prefix candidates whose parents share its parent's first
+        prefix_len ids were kept before it; the dropped ones score -inf and rank among the -inf fillers by beam * K + code.
+        None (or max_per_prefix >= k, which cannot bind) gives the uncapped result."""
+        return self._beam_topk("sid_trie_beam_topk", logits, generated, log_probas, k, bad, exclude, include, cap=cap)
 
     def beam_topk_wide(self, logits: torch.Tensor, generated: Optional[torch.Tensor], log_probas: Optional[torch.Tensor], k: int,
                        bad: Optional[torch.Tensor] = None, exclude: Optional["SidExclusion"] = None,
@@ -803,7 +811,7 @@ class SidPrefixIndex:
         return self._beam_topk("sid_trie_beam_topk_wide", logits, generated, log_probas, k, bad, exclude, include, int(cluster))
 
     def _beam_topk(self, entry: str, logits, generated, log_probas, k: int, bad, exclude, include,
-                   cluster: Optional[int] = None):
+                   cluster: Optional[int] = None, cap: Optional[Tuple[int, int]] = None):
         _need_cuda(logits, bad)
         if generated is None:
             B, kp, h = logits.shape[0], 1, 0
@@ -824,7 +832,7 @@ class SidPrefixIndex:
         out_g = torch.empty((B, k, h + 1), dtype=torch.int64, device=dev)
         out_p = torch.empty((B, k), dtype=torch.float32, device=dev)
         out_parent = torch.empty((B * k,), dtype=torch.int64, device=dev)
-        name, filt = _filter_entry(entry, exclude, include, B, h + 1, entry[9:])
+        name, filt = _filter_entry(entry, exclude, include, B, h + 1, entry[9:], cap)
         wide = () if cluster is None else (cluster,)
         with torch.cuda.device(dev):
             _lib.check(getattr(_lib.load(), "rqb200_" + name)(
@@ -1000,12 +1008,20 @@ def _filter_args(f, kind: str, B: int, levels: int, what: str):
     return _p(f.pos), _p(f[1]), _p(f.count), f.pos.shape[1], H
 
 
-def _filter_entry(entry: str, exclude, include, B: int, levels: int, what: str):
+def _filter_entry(entry: str, exclude, include, B: int, levels: int, what: str, cap: Optional[Tuple[int, int]] = None):
     """(entry point name, filter arguments) of a consumer call: ``entry`` without a filter, ``entry``_excluding /
-    ``entry``_including with one.  An inclusion has the exclusion folded in, so a call takes at most one."""
+    ``entry``_including with one.  An inclusion has the exclusion folded in, so a call takes at most one.  With a ``cap``
+    (prefix_len, max_per_prefix): ``entry``_capped, whose arguments are the cap, the filter mode and the filter's arrays."""
     if exclude is not None and include is not None:
         raise ValueError(f"{what}: pass exclude or include, not both (sid_inclusion_build folds an exclusion into the "
                          "inclusion)")
+    if cap is not None:
+        prefix_len, max_per_prefix = (int(c) for c in cap)
+        if include is not None:
+            return entry + "_capped", (prefix_len, max_per_prefix, 2) + include.args(B, levels, what)
+        if exclude is not None:
+            return entry + "_capped", (prefix_len, max_per_prefix, 1) + exclude.args(B, levels, what)
+        return entry + "_capped", (prefix_len, max_per_prefix, 0, None, None, None, 0, 0)
     if include is not None:
         return entry + "_including", include.args(B, levels, what)
     if exclude is not None:
